@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """bench.py -- Mpix/s of dense DIS flow on synthetic 1024x436 pairs (op-point 2).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path (all pyramid levels: patch inverse search,
 densification, variational refinement == the reference's "O.Flow Run-Time"
 region, oflow.cpp:113-114,355-360) over B pairs per GPU (default 64 = the batch
-of BASELINE configs[3]; one pair alone leaves 147 of 148 SMs idle, see
+of BASELINE configs[3]; one pair alone leaves 131 of the H100's 132 SMs idle, see
 batch_sweep in the output).  Pixels are counted at the ORIGINAL image size, once
 per pair (SURVEY.md section 8d).
 
@@ -24,9 +24,12 @@ per pair (SURVEY.md section 8d).
   fast_mode : the opt-in red-black refinement (not bit-identical; throughput, delta to the exact flow, EPE of both)
   big_configs : BASELINE configs[2] and [4] (1920x1080 RGB, 2880x1988 stereo) on one GPU, per kernel class
   single_lane / batch_sweep : one lane, L2 flushed before every step (latency of 64, 8, 1 pairs)
-  roofline     : dominant kernel (lexicographic SOR), algorithmic bytes / CUDA-event time, plus the
-                 issue-slot utilisation of the whole overlapped step
-  cpu_baseline : the reference CPU build (oracle/_ref) or the C port on this box's cores
+  roofline     : dominant kernel (lexicographic SOR), algorithmic bytes / CUDA-event time
+  cpu_baseline : the reference CPU build (oracle/_ref) or the C port on this host's cores
+
+--dump-outputs DIR writes the flows of the last timed `value` step (level sc_l of every pair, what
+ofdis_get_flow_batch hands a caller) to DIR/flow.npy, float32 [pairs][h][w][nop]; the inputs are
+seeded, so two builds can be compared output for output.
 
 Under torchrun every rank owns B pairs (weak scaling, no data-path collective;
 frames are independent -- DESIGN.md section 6); time = max over ranks.
@@ -76,7 +79,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -253,7 +256,7 @@ def workload_config(args, world):
                         "single-pair and 8-pair latencies in batch_sweep)" % args.batch,
             "pairs_per_gpu": args.batch, "pairs_total": args.batch * world, "parallelism": "frames x%d" % world,
             "lanes": "%d contexts/streams per GPU, consecutive steps overlap" % max(1, args.lanes),
-            "l2": "two alternating working sets of ~2 MB per pair exceed the 126 MB L2 at the default batch; "
+            "l2": "two alternating working sets of ~2 MB per pair exceed the 50 MB L2 at the default batch; "
                   "single_lane and batch_sweep numbers are taken with L2 flushed (256 MiB write) before every step"}
 
 
@@ -308,7 +311,7 @@ def measure_sharded(args, prm, rank, world, local, stream, barrier, maxrank):
     return out
 
 
-def measure_big_configs():
+def measure_big_configs(steps):
     """BASELINE configs[2] and configs[4] on this GPU (tools/big_configs.py): step time, per kernel
     class and per level; the SOR of configs[4]'s level 1 at 8 pairs is the launch SURVEY 8(d) names."""
     sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -318,7 +321,7 @@ def measure_big_configs():
         rows = []
         for name, c in big_configs.CFGS.items():
             for b in (1, 8):
-                rows.append(big_configs.measure(name, c, b, {}))
+                rows.append(big_configs.measure(name, c, b, {}, steps))
         return rows
     except Exception as e:  # must not lose the headline numbers
         return {"error": str(e)}
@@ -340,6 +343,7 @@ def main():
                          "them (default: the region the reference arm times), finest = un-padded I0,I1 of the finest used "
                          "level, images = padded I0,I1 of every level, cli = 8-bit frames in / full-resolution flow out")
     ap.add_argument("--no-extras", action="store_true", help="skip the sharded and big_configs legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the flows of the last timed step to DIR/flow.npy")
     ap.add_argument("--opt", action="append", default=[], metavar="NAME=VALUE",
                     help="ofdis_set_option on every context (launch-geometry experiments; results are bit-identical)")
     args = ap.parse_args()
@@ -418,7 +422,7 @@ def main():
 
     # NL lanes (context + stream each): step i runs on lane i % NL, so consecutive steps overlap on the
     # device -- copies of one step under the kernels of the others, and the latency-bound refinement
-    # kernels of several batches side by side (one batch of 64 pairs occupies 64 of 148 SMs there).
+    # kernels of several batches side by side (one batch of 64 pairs occupies 64 of 132 SMs there).
     NL = max(1, args.lanes)
     lanes = [(ctx, stream, host_out)]  # + the cli leg's full-resolution host buffer, appended below
     for _ in range(NL - 1):
@@ -458,12 +462,16 @@ def main():
     t0 = time.time()
     ms_res = maxrank(pipelined(resident_step, args.steps))
     launches = (sum(l[0].launch_count for l in lanes) - l0) // args.steps
-    barrier()
-    # The K timed steps above last a few milliseconds.  The same loop over >= 0.5 s: clocks and thermals under a
-    # sustained load (the clock sampler runs through both), reported beside `value`, never instead of it.
-    n_sus = max(args.steps, int(0.5e3 / max(ms_res, 1e-3)))
-    ms_sus = maxrank(pipelined(resident_step, n_sus))
-    sustained = {"steps": n_sus, "ms_per_step": ms_sus, "value": None, "seconds": n_sus * ms_sus * 1e-3}
+    if args.dump_outputs and rank == 0:
+        # what the last timed step computed: the flows of its lane, read back outside the timed region
+        li0 = ctx.level_info(prm.sc_l)
+        flows = np.empty((B, li0["h"], li0["w"], prm.nop), np.float32)
+        last = lanes[(args.steps - 1) % NL][0]
+        last.get_flow_batch(0, B, flows)
+        last.sync()
+        keep = max(1, min(B, (64 << 20) // (flows[0].nbytes)))  # at most 64 MB: the first pairs of the batch
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "flow.npy"), flows[:keep])
     barrier()
     # one lane alone, L2 flushed before every step (latency of one batch)
     ms_res_single = maxrank(timed(lambda: ctx.run(B), args.steps))
@@ -532,7 +540,7 @@ def main():
             download(c, mode, ho, hfull)
 
         # Warm-up: W steps per lane, continued until 0.4 s of copies have run -- an idle PCIe link takes
-        # ~0.2 s of traffic to leave its low-power state (tools/e2e_probe.py: first pass 30 GB/s, then 54).
+        # a fraction of a second of traffic to leave its low-power state (tools/e2e_probe.py).
         n_warm, w_start = 0, time.perf_counter()
         while n_warm < NL * args.warmup or time.perf_counter() - w_start < 0.4:
             e2e_step(n_warm)
@@ -593,7 +601,7 @@ def main():
     ctx.set_graph_mode(False)
     roof = None
     try:
-        prof = ctx.profile_kernels(B, steps=max(3, min(args.steps, 10)))
+        prof = ctx.profile_kernels(B, steps=args.steps)
         peak, how = peaks()
         sor = prof["sor"]
         alg = 0
@@ -601,20 +609,6 @@ def main():
             g = ctx.level_info(lv)
             alg += prm.tv_innerit * (lv + 1) * 44 * g["w"] * g["h"] * B  # bytes, SURVEY 8(d)
         ach = alg / (sor["ms_per_step"] * 1e-3) / 1e9
-        traffic, issue = None, None
-        tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-        if os.path.exists(tp):
-            tj = json.load(open(tp))
-            traffic = tj.get("sor_dram_bytes_per_launch")
-            # what actually bounds the overlapped step: warp-instruction issue.  ncu counts the warp
-            # instructions of one step (profiles/r2_launches_step_b64.csv); an SM issues at most
-            # 4 per cycle.  Utilisation = instructions / (step time x SMs x 4 x SM clock).
-            wi = tj.get("warp_instructions_per_step")
-            if wi and B == 64 and clocks.get("sm_mhz"):
-                sms = torch.cuda.get_device_properties(local).multi_processor_count
-                issue = {"warp_instructions_per_step": wi, "sms": sms, "sm_mhz": clocks["sm_mhz"],
-                         "issue_slot_utilisation": wi / (ms_res * 1e-3 * sms * 4 * clocks["sm_mhz"] * 1e6),
-                         "ipc_per_sm": wi / (ms_res * 1e-3 * sms * clocks["sm_mhz"] * 1e6)}
         # the other exact SOR kernel (ofdis_set_option "sor_lane" 1: flag-synchronised warps, no CTA barrier) on the same
         # batch, one stream: the engine picks it by itself for launches of up to 16 frames (batch_sweep below)
         lane_alt = None
@@ -623,27 +617,24 @@ def main():
             cl.set_option("sor_lane", 1)
             cl.upload_packed(0, B, host_in.data_ptr())
             cl.run(B)
-            pl_ = cl.profile_kernels(B, steps=max(3, min(args.steps, 10)))
+            pl_ = cl.profile_kernels(B, steps=args.steps)
             cl.close()
             lane_alt = {"kernel": "sor_lane_kernel (same sweeps; warps of 32 rows x two-pixel blocks, shuffles + flag-synchronised "
                                   "shared-memory rings instead of a CTA barrier per super-step)",
                         "kernel_ms_per_step": pl_["sor"]["ms_per_step"], "achieved": alg / (pl_["sor"]["ms_per_step"] * 1e-3) / 1e9,
                         "frac": alg / (pl_["sor"]["ms_per_step"] * 1e-3) / 1e9 / peak,
-                        "note": "faster per launch, but 200 KB of shared memory per CTA at the 56-row level: with ten streams "
-                                "overlapping it costs 6 % of `value` (profiles/), so batches above 16 frames keep sor_wave_kernel"}
+                        "note": "faster per launch, but 200 KB of shared memory per CTA at the 56-row level (one CTA per SM), "
+                                "so batches above 16 frames keep sor_wave_kernel (ofdis_capi.cu, sor_lane)"}
         except Exception as e:
             lane_alt = {"error": str(e)}
         roof = {"bound": "hbm", "kernel": "sor_wave_kernel (lexicographic SOR wavefront, all sweeps fused, one CTA per frame at this level size)", "achieved": ach,
                 "sor_lane_kernel": lane_alt,
-                "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic, "traffic_note": "ncu dram bytes per SOR launch with caches flushed before every replay (1.04x the "
-                "algorithmic bytes); 0.32e6 with --cache-control none, i.e. behind assemble_kernel in the level loop "
-                "(profiles/roofline_traffic.json)", "issue": issue, "peak_source": how,
+                "peak": peak, "unit": "GB/s", "frac": ach / peak, "peak_source": how,
                 "algorithmic_bytes_per_step": alg, "kernel_ms_per_step": sor["ms_per_step"],
                 "launches_per_step": sor["launches_per_step"],
                 "share_of_step": {k: v["ms_per_step"] for k, v in prof.items()}}
     except Exception as e:  # profiling hook missing must not lose the headline numbers
-        roof = {"bound": "hbm", "achieved": None, "peak": peaks()[0], "unit": "GB/s", "frac": None, "traffic": None,
-                "error": str(e)}
+        roof = {"bound": "hbm", "achieved": None, "peak": peaks()[0], "unit": "GB/s", "frac": None, "error": str(e)}
 
     # ---- latency-bound small batches (configs[1] = one pair; configs[3]'s per-GPU shard = 8) ----
     sweep = {}
@@ -657,7 +648,7 @@ def main():
             c2.set_graph_mode(True)
             for _ in range(3):
                 c2.run(b)
-            ms = timed(lambda: c2.run(b), 10)
+            ms = timed(lambda: c2.run(b), args.steps)
 
             def e2e_b():
                 upload(c2, mode, b)
@@ -666,7 +657,7 @@ def main():
 
             for _ in range(3):  # the first upload allocates the context's staging buffer
                 e2e_b()
-            ms2 = timed(e2e_b, 10)
+            ms2 = timed(e2e_b, args.steps)
             sweep[str(b)] = {"ms_per_step": ms, "value": b * H_ORG * W_ORG / (ms * 1e-3) / 1e6,
                              "e2e_ms_per_step": ms2, "e2e_value": b * H_ORG * W_ORG / (ms2 * 1e-3) / 1e6,
                              "sor_kernel": "sor_lane_kernel (engine default for launches of up to 16 frames)"}
@@ -678,7 +669,7 @@ def main():
             c4.set_graph_mode(True)
             for _ in range(3):
                 c4.run(b)
-            sweep[str(b)]["sor_wave_kernel_ms_per_step"] = timed(lambda: c4.run(b), 10)
+            sweep[str(b)]["sor_wave_kernel_ms_per_step"] = timed(lambda: c4.run(b), args.steps)
             c4.close()
             if not args.no_extras:  # the same latency with the opt-in red-black refinement (see fast_mode)
                 c3 = api.Context(prm, pyrs[0].width, pyrs[0].height, pyrs[0].imgpadding, b, device=local,
@@ -688,7 +679,7 @@ def main():
                 c3.set_graph_mode(True)
                 for _ in range(3):
                     c3.run(b)
-                sweep[str(b)]["fast_mode_ms_per_step"] = timed(lambda: c3.run(b), 10)
+                sweep[str(b)]["fast_mode_ms_per_step"] = timed(lambda: c3.run(b), args.steps)
                 c3.close()
 
     # ---- opt-in red-black refinement (ofdis_set_option "sor_fast"; NOT the reference's iterate) ----
@@ -711,7 +702,7 @@ def main():
             # the red-black solver against the same HBM roofline as the exact one: algorithmic bytes of the SOR
             # (SURVEY 8d: 44 bytes per pixel and solve) / event time of its launches in an eager pass
             fl[0].set_graph_mode(False)
-            pf = fl[0].profile_kernels(B, steps=max(3, min(args.steps, 10)))
+            pf = fl[0].profile_kernels(B, steps=args.steps)
             fl[0].set_graph_mode(True)
             alg_f = sum(prm.tv_innerit * (lv + 1) * 44 * ctx.level_info(lv)["w"] * ctx.level_info(lv)["h"] * B
                         for lv in range(prm.sc_l, prm.sc_f + 1))
@@ -753,7 +744,7 @@ def main():
     cpu = cpu_reference(prm, pyrs, frames_u8, args.cpu_seconds, threads) if world == 1 else None
     big = None
     if world == 1 and not args.no_extras:
-        big = measure_big_configs()
+        big = measure_big_configs(args.steps)
     lead = dict(legs[mode])
     lead.update({"unit": "Mpix/s", "leg": mode, "host_numa_node": numa_node,
                  "flows_equal_resident_path": legs[mode]["result_checked_bitwise"],
@@ -765,8 +756,6 @@ def main():
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_res, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": workload_config(args, world),
-        "sustained": dict(sustained, value=pix / (sustained["ms_per_step"] * 1e-3) / 1e6, unit="Mpix/s",
-                          note="the `value` loop run for >= 0.5 s (clocks in `clocks` cover it)"),
         "single_lane": {"ms_per_step": ms_res_single, "value": pix / (ms_res_single * 1e-3) / 1e6,
                         "note": "one context, one stream, L2 flushed before every step"},
         "e2e": lead,

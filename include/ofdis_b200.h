@@ -1,4 +1,4 @@
-/* ofdis_b200.h -- C-ABI of the B200-native DIS optical-flow hot path.
+/* ofdis_b200.h -- C-ABI of the CUDA (sm_90a, H100) DIS optical-flow hot path.
  *
  * This is the drop-in boundary (DESIGN.md section 1): plain C, plain pointers
  * and sizes, no C++/torch types.  Everything the reference's three classes do

@@ -1,4 +1,4 @@
-"""Builds libofdis_b200.so (CUDA kernels + C-ABI) in-tree with nvcc for sm_100a.
+"""Builds libofdis_b200.so (CUDA kernels + C-ABI) in-tree with nvcc for sm_90a (H100).
 
     python -m of_dis_b200.build [--force] [--verbose]
 
@@ -18,7 +18,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libofdis_b200.so")
 SOURCES = ["ofdis_capi.cu", "patch_kernels.cu", "pyramid_kernels.cu", "varref_kernels.cu"]
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "static",
 ]
@@ -35,7 +35,9 @@ def needs_build() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "ofdis_b200.h")]
+    # build.py itself: a change of NVCC_FLAGS (e.g. the target architecture) must rebuild the library
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "ofdis_b200.h"),
+                                                              os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 

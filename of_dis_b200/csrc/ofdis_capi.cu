@@ -34,15 +34,15 @@ struct ofdis_ctx {
   int sor_single_max = 128, sor_max_cluster = 8, sor_dev_cluster = 8, sor_rt = 1;  // defaults set in ofdis_create
   // levels of few 32-row bands: pixel wavefront (sor_lane_kernel) instead of the block wavefront.  0 never, 1 always,
   // 2 (default) for launches of up to SOR_LANE_AUTO_FRAMES frames on levels of one or two bands (sor_lane_preferred):
-  // there the kernel is 10-20 % faster per launch, but it needs
-  // 200 KB of shared memory per CTA at 56-row levels (one CTA per SM), which costs 6 % of throughput when ten
-  // streams of 64 frames overlap (bench.py `value`)
+  // there it is faster per launch (H100, 700 W, one stream, operating point 2: 1 pair 0.344 vs 0.456 ms per step,
+  // 8 pairs 0.365 vs 0.470 ms), but it needs 200 KB of shared memory per CTA at 56-row levels (one CTA per SM), which
+  // costs 10-13 % of throughput when ten streams of 32 or 64 frames overlap (bench.py `value`)
   int sor_lane = 2;
   int last_vr_lane = 0;  // layout of the last refinement (ofdis_debug_get)
   // programmatic dependent launch of the level loop's kernels (pdl_wait, ofdis_internal.cuh): 0 never, 1 always,
-  // 2 (default) for launches of up to SOR_LANE_AUTO_FRAMES frames: one stream, graph replay, tools/pdl_ab.py:
-  // 1 pair 0.349 -> 0.342 ms, 8 pairs 0.373 -> 0.356 ms, 64 pairs 0.558 -> 0.598 ms (waiting CTAs of the next kernel
-  // take SM slots from the tail of the current one)
+  // 2 (default) for launches of up to SOR_LANE_AUTO_FRAMES frames: H100, one stream, graph replay: 1 pair
+  // 0.374 -> 0.344 ms, 8 pairs 0.390 -> 0.363 ms; 64 pairs 0.659 -> 0.690 ms, and 5-14 % less throughput when ten
+  // streams of 32 or 64 frames overlap (waiting CTAs of the next kernel take SM slots from the tail of the current one)
   int pdl = 2;
   int nlev = 0;                    // sc_f - sc_l + 1
   std::vector<LevelGeom> lev;      // index: level - sc_l
@@ -175,7 +175,7 @@ int run_levels(ofdis_ctx* ctx, int nframes, int use_initflow) {
 
 extern "C" {
 
-const char* ofdis_version(void) { return "ofdis_b200 0.1 (sm_100a)"; }
+const char* ofdis_version(void) { return "ofdis_b200 0.1 (sm_90a)"; }
 
 const char* ofdis_last_error(const ofdis_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 
@@ -224,9 +224,8 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
     ctx->own_stream = true;
   }
   if (prm->usetvref) {  // tallest refinement level: 256-row bands x the largest cluster the device grants
-    // Measured defaults (tools/big_configs.py, bench.py --opt): the largest cluster the device grants
-    // (16 CTAs: -10..20 % on levels of 272..1024 rows against 8); two rows per SOR thread for stereo
-    // (-23 % on configs[4]), one for flow (two rows: -3 % on configs[2], +4 % on the 56-row bench level).
+    // Defaults (compare with tools/big_configs.py, bench.py --opt): the largest cluster the device grants (an H100
+    // grants 16 CTAs), two rows per SOR thread for stereo, one for flow.
     ctx->sor_dev_cluster = sor_max_cluster_size();
     ctx->sor_max_cluster = ctx->sor_dev_cluster;
     ctx->sor_rt = (nop == 1) ? 2 : 1;

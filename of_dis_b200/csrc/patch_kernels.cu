@@ -1,4 +1,4 @@
-// Patch stage of the DIS hot path on sm_100a: K1 (template + Hessian), K2 (init
+// Patch stage of the DIS hot path on sm_90a: K1 (template + Hessian), K2 (init
 // from the coarser flow), K3 (inverse-compositional Gauss-Newton iterations)
 // fused in one kernel, and K4 (densification) as a deterministic gather.
 //
@@ -524,7 +524,7 @@ __global__ void __launch_bounds__(256) patch_p8c1_kernel(LevelGeom g, PatchParam
 //     around the patch's current integer position (M = 2 pixels of slack; stereo: P+1 rows, the row
 //     never moves) -- staged by the patch's own 8 lanes and re-staged only when the position leaves
 //     the slack.  The generic kernel issues 4 LDGs per element and iteration whose 32 lanes touch 4
-//     patches x 1..2 sectors each: the L1 tag stage, not the math, bounded it (profiles/).  From
+//     patches x 1..2 sectors each: the L1 tag stage, not the math, bounded it.  From
 //     shared memory the same taps are 4 LDS with at most a 2-way bank conflict between patches;
 //   * element offsets are walked incrementally (no offset table).
 // Arithmetic (operand order, reduction tree, stop tests) is that of patch_optimize_kernel.

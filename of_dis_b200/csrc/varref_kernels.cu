@@ -1,4 +1,4 @@
-// Variational refinement of the DIS hot path on sm_100a (K5..K12 of SURVEY.md):
+// Variational refinement of the DIS hot path on sm_90a (K5..K12 of SURVEY.md):
 // VarRefClass (refine_variational.cpp:25-336) and the FDF1.0.1 routines it calls
 // (opticalflow_aux.c:17-548, image.c:376-502, solver.c:77-466).
 //
@@ -645,9 +645,8 @@ extern "C" int ofdis_debug_sor_times(long long* dst) {
 #endif
 
 bool sor_lane_fits(int h, int K) { return sl_sweeps_per_launch((h + 31) / 32, K) >= 1; }
-// Where the lane kernel beats the block wavefront (tools/lane_ab.py, profiles/): one or two bands with all sweeps
-// in one launch.  Every further band adds 33 steps of start-up skew, and 1920x1080's 136- and 68-row levels
-// (5 and 3 bands) run 20-50 % slower with it.
+// Where the lane kernel beats the block wavefront (tools/lane_ab.py): one or two bands with all sweeps in one
+// launch.  Every further band adds 33 steps of start-up skew, which makes taller levels slower with it.
 bool sor_lane_preferred(int h, int K) { return (h + 31) / 32 <= 2 && sl_sweeps_per_launch((h + 31) / 32, K) >= (K < 1 ? 1 : K); }
 
 bool rb_smem_limit_exceeded(int nop, int K) { return K < 1 || rb_smem_bytes(nop, K) > 227 * 1024; }

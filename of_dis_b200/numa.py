@@ -2,7 +2,7 @@
 
 On a two-socket host a pinned buffer that lands on the socket remote from the GPU is
 read over the inter-socket link: the H2D copy of a batch then runs at about half the
-PCIe rate (measured on the B200 boxes: 27 GB/s remote vs 54 GB/s local, tools/upload_timing.py).
+PCIe rate (tools/upload_timing.py measures both).
 `bind_to_gpu_node(dev)` pins the calling thread to the CPUs of the GPU's NUMA node so that
 buffers allocated (first-touched) afterwards are local; `unbind(prev)` restores the mask.
 Pure sysfs + sched_setaffinity; does nothing when the topology cannot be read.

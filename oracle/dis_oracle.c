@@ -1,7 +1,7 @@
 /* oracle/dis_oracle.c -- CPU restatement of the DIS hot path (TEST INFRASTRUCTURE ONLY).
  *
  * See dis_oracle.h.  Every function cites the reference lines it follows
- * (paths relative to /root/reference).  All arithmetic is IEEE binary32, one
+ * (paths relative to the reference checkout).  All arithmetic is IEEE binary32, one
  * operation per rounding (build with -ffp-contract=off), in the expression
  * order of the reference, because the result must be bitwise equal to the
  * reference build (oracle/_ref) -- SURVEY.md finding 2.

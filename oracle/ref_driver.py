@@ -26,7 +26,7 @@ def _lib(flavour: str):
     if flavour not in _LIBS:
         path = os.path.join(_HERE, "_ref", "libofdis_ref_%s.so" % flavour)
         if not os.path.exists(path):
-            raise FileNotFoundError("%s missing: run `make -C oracle ref` where /root/reference exists" % path)
+            raise FileNotFoundError("%s missing: run `make -C oracle ref` where the reference sources are (oracle/Makefile REF)" % path)
         # RTLD_LOCAL: the four flavours export the same symbol names.
         _LIBS[flavour] = ctypes.CDLL(path, mode=ctypes.RTLD_LOCAL)
     return _LIBS[flavour]

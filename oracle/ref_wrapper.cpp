@@ -1,7 +1,7 @@
 // oracle/_ref wrapper -- TEST INFRASTRUCTURE ONLY.
 //
 // Thin extern "C" entry points around the UNMODIFIED reference classes
-// (compiled in place from /root/reference by oracle/Makefile against
+// (compiled in place from the reference checkout by oracle/Makefile against
 // oracle/eigen_shim).  Used by tests/, __graft_entry__.smoke() and bench.py's
 // cpu_baseline / --impl reference leg only; the product never links this.
 //

@@ -1,13 +1,20 @@
 """Generates tests/golden/*.npz from the REFERENCE build (oracle/_ref, i.e. the
-reference's own sources compiled in place by oracle/Makefile).  Run in the
-container that has /root/reference:
+reference's own sources compiled in place by oracle/Makefile).  Run where the
+reference sources are (oracle/Makefile's REF):
 
     make -C oracle ref && python tests/golden/make_golden.py
 
 Each fixture holds the uint8 input pair, the parameters (20 CLI numbers + noc +
 nop) and the reference flow at level sc_l, plus the patch-stage outputs of the
 finest level (p, conv, cnt) for a fixed seeded coarser flow.
+
+    python tests/golden/make_golden.py --digests
+
+writes reference_digests.json instead: SHA-256 of the reference's float32 output
+bits on the seeded inputs of tests/test_oracle.py (inputs the tests regenerate,
+outputs too large to store as arrays).
 """
+import json
 import os
 import sys
 
@@ -15,8 +22,30 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 from of_dis_b200 import params, preprocess, synth  # noqa: E402
 from oracle import ref_driver  # noqa: E402
+
+
+def write_digests(out_dir):
+    import test_oracle as t
+
+    out = {}
+    i0, i1, pyr, prm, fl = t.cfg1_inputs()
+    out["cfg1_input"] = t.input_digest(i0, i1)
+    out["cfg1_run"] = t.digest(ref_driver.ref_run(pyr, prm))
+    out["cfg1_varref"] = t.digest(ref_driver.ref_level_varref(pyr, prm, prm.sc_l, fl))
+    for seed in range(40):
+        i0, i1, pyr, prm = t.random_config_inputs(seed)
+        out["random_%d_input" % seed] = t.input_digest(i0, i1)
+        out["random_%d" % seed] = t.digest(ref_driver.ref_run(pyr, prm))
+    for name in t.BASELINE_CASES:
+        i0, i1, pyr, prm = t.baseline_inputs(name)
+        out["baseline_%s_input" % name] = t.input_digest(i0, i1)
+        out["baseline_" + name] = t.digest(ref_driver.ref_run(pyr, prm))
+    with open(os.path.join(out_dir, "reference_digests.json"), "w") as f:
+        json.dump(out, f, indent=1, sort_keys=True)
+        f.write("\n")
 
 CASES = {
     # name: (h, w, channels, cli numbers, nop, amp, stereo)
@@ -36,6 +65,9 @@ CASES = {
 
 def main():
     out_dir = os.path.dirname(os.path.abspath(__file__))
+    if sys.argv[1:] == ["--digests"]:
+        write_digests(out_dir)
+        return
     only = sys.argv[1:]  # optional: generate just these fixtures
     for name, (h, w, ch, cli, nop, amp, stereo) in CASES.items():
         if only and name not in only:

@@ -53,7 +53,7 @@ def test_missing_library_fails_loudly(monkeypatch):
 
 
 def test_reference_arm_prints_the_contract_line(tmp_path):
-    """bench.py --impl reference (the reference CPU build, or the oracle port when /root/reference is absent)
+    """bench.py --impl reference (the reference CPU build, or the oracle port when oracle/_ref is not built)
     prints one JSON line with the keys the driver reads."""
     import json
     import os

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Everything goes through
+"""GPU parity tests (run on an H100: pytest -m gpu).  Everything goes through
 the C-ABI (of_dis_b200/lib/libofdis_b200.so); the oracle (C restatement, pinned
 bitwise to the reference build) is only the checker.  Integer/bit-exact bar:
 all float outputs must be BITWISE equal, which is stronger than the 1e-3

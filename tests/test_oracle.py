@@ -1,7 +1,11 @@
 """CPU tests of the checker itself: the C restatement (oracle/dis_oracle.c) must
-equal (a) the committed golden fixtures produced by the reference build and
-(b), where oracle/_ref exists, the reference build itself -- bit for bit."""
+equal (a) the committed golden fixtures produced by the reference build -- whole
+arrays, or the SHA-256 of the reference's output bits (golden/reference_digests.json)
+where the output is too large to store -- and (b), where oracle/_ref exists, the
+reference build itself -- bit for bit."""
 import glob
+import hashlib
+import json
 import os
 
 import numpy as np
@@ -10,7 +14,26 @@ import pytest
 from of_dis_b200 import params, preprocess, synth
 from oracle import ref_driver
 
-GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "*.npz")))
+GOLDEN_DIR = os.path.join(os.path.dirname(__file__), "golden")
+GOLDEN = sorted(glob.glob(os.path.join(GOLDEN_DIR, "*.npz")))
+with open(os.path.join(GOLDEN_DIR, "reference_digests.json")) as _f:
+    REF_DIGESTS = json.load(_f)
+
+
+def digest(a, dtype=np.float32):
+    """Shape and SHA-256 of the bits of `a`: equal digests == bitwise equal arrays."""
+    a = np.ascontiguousarray(a, dtype)
+    return "%s:%s" % ("x".join(map(str, a.shape)), hashlib.sha256(a.tobytes()).hexdigest())
+
+
+def input_digest(i0, i1):
+    return digest(np.stack([i0, i1]), np.uint8)
+
+
+def check_inputs(key, i0, i1):
+    """The seeded 8-bit input pair must be the one the reference digest was taken on (synth.py goes through
+    numpy/scipy): a mismatch here means the inputs moved, not the port."""
+    assert input_digest(i0, i1) == REF_DIGESTS[key + "_input"], "%s: synthetic inputs differ from the recorded ones" % key
 
 
 def _load(path):
@@ -44,21 +67,25 @@ def test_reference_build_reproduces_golden(path):
     assert np.array_equal(bits(ref_driver.ref_run(pyr, prm)), bits(z["flow"]))
 
 
-@pytest.mark.skipif(not ref_driver.ref_available("m1c1"), reason="oracle/_ref not built")
-def test_port_vs_reference_cfg1_and_stages(oracle_port):
-    """BASELINE config 1 (640x480 gray, op-point 2) whole run, plus per-stage checks."""
+def cfg1_inputs():
+    """BASELINE config 1 (640x480 gray, op-point 2) and an arbitrary smooth-ish flow of its finest level."""
     i0, i1, _ = synth.synthetic_pair(480, 640, 1, seed=3)
     prm = params.operating_point(2, 640)
     pyr = preprocess.PairPyramids(i0, i1, prm.sc_f, prm.p_samp_s)
-    ref = ref_driver.ref_run(pyr, prm)
-    assert np.array_equal(bits(ref), bits(oracle_port.port_run(pyr, prm)))
-    # variational refinement alone, on an arbitrary smooth-ish flow
-    lv = prm.sc_l
-    h, w = pyr.level_shape(lv)
+    h, w = pyr.level_shape(prm.sc_l)
     rng = np.random.default_rng(0)
     fl = (rng.standard_normal((h, w, 2)) * 0.7).astype(np.float32)
-    assert np.array_equal(bits(ref_driver.ref_level_varref(pyr, prm, lv, fl)),
-                          bits(oracle_port.port_level_varref(pyr, prm, lv, fl)))
+    return i0, i1, pyr, prm, fl
+
+
+def test_port_vs_reference_cfg1_and_stages(oracle_port):
+    """BASELINE config 1 (640x480 gray, op-point 2) whole run, plus per-stage checks."""
+    i0, i1, pyr, prm, fl = cfg1_inputs()
+    check_inputs("cfg1", i0, i1)
+    assert digest(oracle_port.port_run(pyr, prm)) == REF_DIGESTS["cfg1_run"]
+    # variational refinement alone
+    lv = prm.sc_l
+    assert digest(oracle_port.port_level_varref(pyr, prm, lv, fl)) == REF_DIGESTS["cfg1_varref"]
     st = oracle_port.varref_stages(pyr, prm, lv, fl)
     out = np.stack([st["uu"], st["vv"]], -1)
     assert np.array_equal(bits(out), bits(oracle_port.port_level_varref(pyr, prm, lv, fl)))
@@ -107,21 +134,24 @@ def test_properties_zero_flow_and_translation(oracle_port):
 
 
 # ---- the port against the reference build on everything the GPU tests use it for ----------------
-@pytest.mark.skipif(not ref_driver.ref_available("m1c1"), reason="oracle/_ref not built")
-@pytest.mark.parametrize("seed", range(40))
-def test_port_vs_reference_on_the_random_configurations_of_the_gpu_suite(seed, oracle_port):
-    """The 40 seeded parameter sets of tests/test_gpu_parity.py::test_random_configurations_vs_oracle:
-    the port (the GPU tests' checker) must equal the reference build on each of them."""
+def random_config_inputs(seed):
+    """Inputs of tests/test_gpu_parity.py::test_random_configurations_vs_oracle[seed]."""
     from test_gpu_parity import _random_config
 
     rng = np.random.default_rng(1000 + seed)
     numbers, ch, nop, size, amp = _random_config(rng)
     prm = params.from_cli_numbers(numbers, noc=ch, nop=nop)
-    if not ref_driver.ref_available(prm.flavour()):
-        pytest.skip("flavour not built")
     i0, i1, _ = synth.synthetic_pair(size[0], size[1], ch, seed=200 + seed, stereo=(nop == 1), amp=amp)
-    pyr = preprocess.PairPyramids(i0, i1, prm.sc_f, prm.p_samp_s)
-    assert np.array_equal(bits(ref_driver.ref_run(pyr, prm)), bits(oracle_port.port_run(pyr, prm)))
+    return i0, i1, preprocess.PairPyramids(i0, i1, prm.sc_f, prm.p_samp_s), prm
+
+
+@pytest.mark.parametrize("seed", range(40))
+def test_port_vs_reference_on_the_random_configurations_of_the_gpu_suite(seed, oracle_port):
+    """The 40 seeded parameter sets of tests/test_gpu_parity.py::test_random_configurations_vs_oracle:
+    the port (the GPU tests' checker) must equal the reference build on each of them."""
+    i0, i1, pyr, prm = random_config_inputs(seed)
+    check_inputs("random_%d" % seed, i0, i1)
+    assert digest(oracle_port.port_run(pyr, prm)) == REF_DIGESTS["random_%d" % seed]
 
 
 BASELINE_CASES = {
@@ -133,17 +163,19 @@ BASELINE_CASES = {
 }
 
 
-@pytest.mark.skipif(not ref_driver.ref_available("m1c1"), reason="oracle/_ref not built")
+def baseline_inputs(name):
+    h, w, ch, mk, seed, stereo = BASELINE_CASES[name]
+    prm = mk()
+    i0, i1, _ = synth.synthetic_pair(h, w, ch, seed=seed, stereo=stereo, amp=6.0)
+    return i0, i1, preprocess.PairPyramids(i0, i1, prm.sc_f, prm.p_samp_s), prm
+
+
 @pytest.mark.parametrize("name", list(BASELINE_CASES))
 def test_port_vs_reference_at_baseline_sizes(name, oracle_port):
     """BASELINE configs[1], [2] and [4] at full size (the inputs of the GPU suite's full-size tests)."""
-    h, w, ch, mk, seed, stereo = BASELINE_CASES[name]
-    prm = mk()
-    if not ref_driver.ref_available(prm.flavour()):
-        pytest.skip("flavour not built")
-    i0, i1, _ = synth.synthetic_pair(h, w, ch, seed=seed, stereo=stereo, amp=6.0)
-    pyr = preprocess.PairPyramids(i0, i1, prm.sc_f, prm.p_samp_s)
-    assert np.array_equal(bits(ref_driver.ref_run(pyr, prm)), bits(oracle_port.port_run(pyr, prm)))
+    i0, i1, pyr, prm = baseline_inputs(name)
+    check_inputs("baseline_" + name, i0, i1)
+    assert digest(oracle_port.port_run(pyr, prm)) == REF_DIGESTS["baseline_" + name]
 
 
 @pytest.mark.skipif(not ref_driver.ref_available("m1c1"), reason="oracle/_ref not built")

@@ -3,7 +3,8 @@ one GPU: step time and, per kernel class, the achieved algorithmic GB/s (SURVEY 
 levels of these configs are the ones that stream from HBM.  Also the SOR time per pyramid level.
 python tools/big_configs.py [B ...] [--opt name=value ...] [--cfg substring]"""
 import sys, time, json
-sys.path.insert(0, '/root/repo')
+import os
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 from of_dis_b200 import api, params, preprocess, synth
@@ -15,7 +16,8 @@ CFGS = {
 }
 
 
-def measure(name, c, B, opts):
+def measure(name, c, B, opts, steps=5):
+    """Step time over `steps` graph replays; per-class and per-level times over `steps` eager profiled passes."""
     prm = c["prm"]()
     h, w = c["size"]
     st = torch.cuda.current_stream()
@@ -31,14 +33,14 @@ def measure(name, c, B, opts):
     for _ in range(2): ctx.run(B)
     torch.cuda.synchronize()
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    n = 5
+    n = steps
     a.record(st)
     for _ in range(n): ctx.run(B)
     b.record(st); torch.cuda.synchronize()
     ms = a.elapsed_time(b) / n
     ctx.set_graph_mode(False)
-    prof = ctx.profile_kernels(B, steps=2)
-    lev = ctx.profile_levels(B, steps=2)
+    prof = ctx.profile_kernels(B, steps=steps)
+    lev = ctx.profile_levels(B, steps=steps)
     # algorithmic bytes per step (SURVEY 8d)
     C, nop, P = prm.noc, prm.nop, prm.p_samp_s
     b_dis = b_sor = b_asm = b_setup = 0

@@ -4,7 +4,8 @@ one eager pass, and the graph-replayed step time.  python tools/lane_ab.py [B ..
 import json
 import sys
 
-sys.path.insert(0, '/root/repo')
+import os
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 from of_dis_b200 import api, params, synth

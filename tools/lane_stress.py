@@ -4,7 +4,8 @@ deterministic one).  python tools/lane_stress.py [replays]"""
 import json
 import sys
 
-sys.path.insert(0, '/root/repo')
+import os
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 from of_dis_b200 import api, params, preprocess, synth
 

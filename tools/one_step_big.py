@@ -2,8 +2,9 @@
 P = 12 patch kernel and the cluster SOR:
    ncu --set full -k regex:sor_wave -c 3 ... python tools/one_step_big.py cfg5 1"""
 import sys
-sys.path.insert(0, '/root/repo')
-sys.path.insert(0, '/root/repo/tools')
+import os
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 from of_dis_b200 import api, synth
 import big_configs

@@ -5,7 +5,8 @@ import json
 import sys
 import time
 
-sys.path.insert(0, '/root/repo')
+import os
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 from of_dis_b200 import api, params, synth
 

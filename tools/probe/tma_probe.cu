@@ -12,8 +12,9 @@
 #define H 72
 #define NF 2
 #ifndef XOFF
-#define XOFF 3
+#define XOFF 4  // box start along the inner dimension: must be a multiple of 4 floats (16 bytes), see DESIGN.md 5.2
 #endif
+static_assert(XOFF % 4 == 0, "an unaligned box start faults (illegal instruction)");
 #ifndef BW
 #define BW 20
 #endif

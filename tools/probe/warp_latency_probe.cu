@@ -1,5 +1,5 @@
 // Single-warp latency probes for sor_lane_kernel's design (a warp alone on its scheduler):
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/probe/warp_latency_probe tools/probe/warp_latency_probe.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/probe/warp_latency_probe tools/probe/warp_latency_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void probe(float* out, long long* cyc, int n) {

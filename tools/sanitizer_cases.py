@@ -26,7 +26,7 @@ CASES = [
     ("cluster_rows140_rt2", (140, 96), 1, 1, "1 0 6 6 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0",
      {"sor_lane": 0, "sor_single_max": 32, "sor_rows_per_thread": 2}),
 ]
-if os.environ.get("SANITIZER_LANE") is not None:  # racecheck: force one SOR kernel everywhere (see profiles/README.md)
+if os.environ.get("SANITIZER_LANE") is not None:  # racecheck: force one SOR kernel everywhere (DESIGN.md section 5.4)
     CASES = [(n, sz, ch, nop, num, dict(o, sor_lane=int(os.environ["SANITIZER_LANE"]))) for n, sz, ch, nop, num, o in CASES]
 for name, (h, w), ch, nop, numbers, opts in CASES:
     prm = params.from_cli_numbers(numbers.split(), noc=ch, nop=nop)

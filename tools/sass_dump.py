@@ -1,9 +1,9 @@
-"""SASS evidence for profiles/: per kernel family the instruction mix of the built library and the
-Blackwell/Hopper-specific mnemonics (UBLKCP = cp.async.bulk, UTMALDG = TMA tensor tile, SYNCS = mbarrier,
+"""SASS evidence: per kernel family the instruction mix of the built library and the
+Hopper-specific mnemonics (UBLKCP = cp.async.bulk, UTMALDG = TMA tensor tile, SYNCS = mbarrier,
 STAS = st.async to a peer CTA's shared memory, UCGABAR = cluster barrier, MUFU.RCP = the hoisted
 reciprocals of the stereo SOR).  No GPU needed:
-    python tools/sass_dump.py > profiles/r2_sass_summary.txt
-    python tools/sass_dump.py --full sor_wave_kernelILi2ELi64ELi1ELb0 > profiles/r2_sass_sor_flow.txt"""
+    python tools/sass_dump.py > sass_summary.txt
+    python tools/sass_dump.py --full sor_wave_kernelILi2ELi64ELi1ELb0 > sass_sor_flow.txt"""
 import collections
 import os
 import re

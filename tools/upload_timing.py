@@ -1,5 +1,6 @@
 import sys, time
-sys.path.insert(0, '/root/repo')
+import os
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, numpy as np
 from of_dis_b200 import api, params, preprocess, synth
 prm = params.operating_point(2, 1024)
