@@ -21,21 +21,6 @@ namespace ofdis {
 
 namespace {
 
-#ifdef OFDIS_SOR_TIMING
-// debug build only: per-warp cycle stamps of a few super-steps of frame 0 (tools/sor_timing.py)
-__device__ long long g_sor_times[64 * 8 * 16];  // sor_lane_kernel: [warp 16][chunk 32][4 stamps]
-#define SOR_STAMP(slot, dep1, dep2)                                                           \
-  do {                                                                                        \
-    if (fr == 0 && (tid & 31) == 0 && T >= 40 && T < 48) {                                    \
-      long long t__;                                                                          \
-      asm volatile("mov.u64 %0, %%clock64;" : "=l"(t__) : "f"(dep1), "f"(dep2) : "memory");   \
-      g_sor_times[((tid >> 5) * 8 + (T - 40)) * 16 + (slot)] = t__;                           \
-    }                                                                                         \
-  } while (0)
-#else
-#define SOR_STAMP(slot, dep1, dep2) do { } while (0)
-#endif
-
 #define DATANORM (0.1f * 0.1f)       /* opticalflow_aux.c:10 */
 #define EPS_COLOR (0.001f * 0.001f)  /* :11 */
 #define EPS_GRAD (0.001f * 0.001f)   /* :12 */
@@ -637,12 +622,6 @@ static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const 
   }
   return cudaGetLastError() == cudaSuccess ? launches : -1;
 }
-
-#ifdef OFDIS_SOR_TIMING
-extern "C" int ofdis_debug_sor_times(long long* dst) {
-  return cudaMemcpyFromSymbol(dst, g_sor_times, sizeof(g_sor_times)) == cudaSuccess ? 0 : -1;
-}
-#endif
 
 bool sor_lane_fits(int h, int K) { return sl_sweeps_per_launch((h + 31) / 32, K) >= 1; }
 // Where the lane kernel beats the block wavefront (tools/lane_ab.py): one or two bands with all sweeps in one
