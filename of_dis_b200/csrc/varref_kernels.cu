@@ -466,7 +466,7 @@ __global__ void __launch_bounds__(256) flow_update_kernel(LevelGeom g, VarRefPla
 // warp within the kernel's launch bound, stage ring + board within the 227 KB of an SM.
 static int sor_sweeps_per_launch(int nop, int hpad, int rt, int K) {
   int kl = K < 1 ? 1 : K;
-  while (kl > 1 && (kl * hpad + 32 > sor_max_threads(hpad) || sor_smem_bytes(nop, hpad, rt, kl) > 227 * 1024)) --kl;
+  while (kl > 1 && (kl * hpad + 32 > sor_max_threads(hpad) || sor_smem_bytes(nop, hpad, rt, kl, hpad) > 227 * 1024)) --kl;
   return kl;
 }
 
@@ -474,7 +474,8 @@ template <int NOP, int HPAD, int RT, bool CL>
 static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
                                 cudaStream_t st) {
   auto kern = sor_wave_kernel<NOP, HPAD, RT, CL>;
-  const size_t smem = sor_smem_bytes(NOP, HPAD, RT, kl);
+  const int ml = sor_stage_lanes(HPAD, RT, g.w, g.h, CL);
+  const size_t smem = sor_smem_bytes(NOP, HPAD, RT, kl, ml);
   if (smem > 227 * 1024) return cudaErrorInvalidConfiguration;
   // opt-in shared memory (and cluster size) once per device and instantiation
   static size_t smem_set[64] = {0};
@@ -507,7 +508,7 @@ static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, cons
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, kern, g, pl, vp, kl);
+  return cudaLaunchKernelEx(&cfg, kern, g, pl, vp, kl, ml);
 }
 
 template <int NOP, int RT>
@@ -631,7 +632,7 @@ bool sor_lane_preferred(int h, int K) { return (h + 31) / 32 <= 2 && sl_sweeps_p
 bool rb_smem_limit_exceeded(int nop, int K) { return K < 1 || rb_smem_bytes(nop, K) > 227 * 1024; }
 
 bool sor_fits(int nop, int hpad, int rt, int K) {
-  return K * hpad + 32 <= sor_max_threads(hpad) && sor_smem_bytes(nop, hpad, rt, K) <= 227 * 1024;
+  return K * hpad + 32 <= sor_max_threads(hpad) && sor_smem_bytes(nop, hpad, rt, K, hpad) <= 227 * 1024;
 }
 
 int sor_max_cluster_size() {
@@ -643,7 +644,7 @@ int sor_max_cluster_size() {
   if (cached[dev]) return cached[dev];
   int best = 8;
   auto kern = sor_wave_kernel<2, 128, 1, true>;
-  const size_t smem = sor_smem_bytes(2, 128, 1, 3);  // 128-row bands, 3 sweeps in flight: the largest common configuration
+  const size_t smem = sor_smem_bytes(2, 128, 1, 3, 128);  // 128-row bands, 3 sweeps in flight: the largest common configuration
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess &&
       cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
     cudaLaunchConfig_t cfg = {};
