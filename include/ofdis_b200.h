@@ -69,7 +69,7 @@ enum {
   OFDIS_OK = 0,
   OFDIS_ERR_ARG = -1,         /* bad argument / unsupported geometry */
   OFDIS_ERR_CUDA = -2,        /* a CUDA call failed; see ofdis_last_error */
-  OFDIS_ERR_UNSUPPORTED = -3, /* valid in the reference but not built here (refinement levels taller than ~256 rows x the largest thread-block cluster -- the SOR's shared-memory ring bounds the rows of one band --, i.e. 2048 rows, 4096 where the device grants 16-CTA clusters; ofdis_upload_packed with usefbcon) */
+  OFDIS_ERR_UNSUPPORTED = -3, /* valid in the reference but not built here (a finest refinement level of more than 16384 rows, refused by ofdis_create before it touches a device; ofdis_upload_packed with usefbcon) */
   OFDIS_ERR_NOMEM = -4
 };
 enum { OFDIS_MEM_HOST = 0, OFDIS_MEM_DEVICE = 1 };
@@ -210,7 +210,9 @@ int ofdis_set_direction(ofdis_ctx* ctx, int dir);
  *                     (a level needs W/4 + h/rows super-steps; sor_wave_kernel.cuh)
  *   "sor_single_max"  32 | 64 | 128 (default): refinement levels of up to this many SOR lanes (= rows / rows per
  *                     thread) run their SOR in one CTA, taller ones in a thread-block cluster of row bands
- *   "sor_max_cluster" 8 (portable) | 16 (default where the device grants it) */
+ *   "sor_max_cluster" 1 | 2 | 4 | 8 (portable) | 16 (default where the device grants it): at most this many SOR bands
+ *                     per thread-block cluster; levels with more bands run as a chain of bands, one sweep per launch.
+ *                     The workspace is sized at create for 8 and 16; 1, 2 or 4 reallocate it here when their chains need more */
 int ofdis_set_option(ofdis_ctx* ctx, const char* name, int value);
 /* CUDA-graph replay of ofdis_run (captured on first use per nframes). */
 int ofdis_set_graph_mode(ofdis_ctx* ctx, int enabled);

@@ -30,7 +30,8 @@ struct ofdis_ctx {
   int last_vr_fstep = 1;
   int sel_dir = -1;                // ofdis_set_direction: -1 = both directions / the forward grid
   // SOR band plan (sor_band_plan): levels of up to sor_single_max rows run in one CTA, taller ones in a
-  // cluster of up to sor_max_cluster CTAs (8 = portable limit; 16 where the device grants it)
+  // cluster of up to sor_max_cluster CTAs (8 = portable limit; 16 where the device grants it), levels with
+  // more bands than that in a chain of CTAs (one sweep per launch)
   int sor_single_max = 128, sor_max_cluster = 8, sor_dev_cluster = 8, sor_rt = 1;  // defaults set in ofdis_create
   // levels of few 32-row bands: pixel wavefront (sor_lane_kernel) instead of the block wavefront.  0 never, 1 always,
   // 2 (default) for launches of up to SOR_LANE_AUTO_FRAMES frames on levels of one or two bands (sor_lane_preferred):
@@ -61,6 +62,9 @@ struct ofdis_ctx {
   VarRefPlanes planes{};
   float* d_planes = nullptr;
   float* d_fast = nullptr;          // fast-mode records and (du,dv) ping-pong planes (ofdis_set_option "sor_fast")
+  int* d_chain = nullptr;           // SOR chain: ticket counter + progress words [frame][band], zero between launches
+  size_t rec_f4 = 0;                // float4 per frame of the SOR's lane rows in d_planes
+  int chain_nb = 0;                 // bands per frame d_chain holds
   int last_vr_fcur = 0;
   PatchParams pp{};
   long launches = 0;
@@ -171,6 +175,61 @@ int run_levels(ofdis_ctx* ctx, int nframes, int use_initflow) {
   return OFDIS_OK;
 }
 
+// Float4 per frame of the SOR's band-skewed lane rows (nb bands x (W4 + hpad + 2) diagonals x hpad lanes x lpitch)
+// and most bands of a chain, over every level, sor_single_max and sor_rows_per_thread with sor_max_cluster in
+// mc_lo .. mc_hi (powers of two), and the lane layout (sor_lane_kernel) of the levels it can take.
+void sor_workspace_need(const ofdis_ctx* c, int mc_lo, int mc_hi, size_t* recf4, int* chain_nb) {
+  *recf4 = 0;
+  *chain_nb = 0;
+  for (const LevelGeom& L : c->lev) {
+    for (int mc = mc_lo; mc <= mc_hi; mc *= 2)
+      for (int sm = 32; sm <= 128; sm *= 2)
+        for (int rt = 1; rt <= 4; rt *= 2) {
+          VarRefPlanes t{};
+          if (sor_band_plan(L.w, L.h, rt, sm, mc, c->nop, c->prm.tv_solverit, &t)) {
+            *recf4 = std::max(*recf4, (size_t)t.nb * t.ndiag * t.hpad * t.lpitch);
+            if (t.chain) *chain_nb = std::max(*chain_nb, t.nb);
+          }
+        }
+    if (sor_lane_fits(L.h, 1)) *recf4 = std::max(*recf4, lane_frame_f4(L.w, L.h));
+  }
+}
+
+// (Re)allocates the refinement planes of the finest level (mask, avg[C], 8 x deriv[C]) behind `recf4` float4 of SOR
+// lane rows per frame, and the chain's scratch for `chain_nb` bands per frame; all of it zeroed.  On failure the
+// previous buffers stay in place.
+bool alloc_refinement(ofdis_ctx* ctx, size_t recf4, int chain_nb) {
+  const LevelGeom& Lf = ctx->lev[0];
+  const size_t plane = (size_t)Lf.pitch * Lf.h, cap = (size_t)ctx->cap;
+  const int C = ctx->prm.noc;
+  const size_t per_frame = plane * (1 + C + 8 * C) + recf4 * 4, chain_ints = 1 + (size_t)chain_nb * cap;
+  float* planes = nullptr;
+  int* chain = nullptr;
+  if (cudaMalloc((void**)&planes, sizeof(float) * per_frame * cap) != cudaSuccess) return false;
+  if (cudaMalloc((void**)&chain, sizeof(int) * chain_ints) != cudaSuccess) {
+    cudaFree(planes);
+    return false;
+  }
+  if (ctx->d_planes || ctx->d_chain) cudaStreamSynchronize(ctx->stream);  // nothing in flight uses the old buffers
+  cudaFree(ctx->d_planes);
+  cudaFree(ctx->d_chain);
+  ctx->d_planes = planes;
+  ctx->d_chain = chain;
+  // never-written lane rows (wavefront ramps, padded lanes) are read by idle SOR lanes: keep them finite
+  cudaMemsetAsync(planes, 0, sizeof(float) * per_frame * cap, ctx->stream);
+  cudaMemsetAsync(chain, 0, sizeof(int) * chain_ints, ctx->stream);
+  float* q = planes;
+  VarRefPlanes& P = ctx->planes;
+  P.rec = reinterpret_cast<float4*>(q); q += recf4 * 4 * cap;   // first (alignment)
+  P.mask = q; q += plane * cap;
+  P.avg = q; q += plane * C * cap;
+  for (int k = 0; k < 8; ++k) { P.deriv[k] = q; q += plane * C * cap; }
+  P.plane = plane;
+  ctx->rec_f4 = recf4;
+  ctx->chain_nb = chain_nb;
+  return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -191,10 +250,8 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
   if (width <= 0 || height <= 0 || (width % (1 << prm->sc_f)) || (height % (1 << prm->sc_f))) return OFDIS_ERR_ARG;
   if (max_frames < 1 || prm->max_iter < 0) return OFDIS_ERR_ARG;
   if (prm->usetvref && ((height >> prm->sc_f) < 4 || (width >> prm->sc_f) < 2)) return OFDIS_ERR_ARG;  // image.c:401-434 needs >= 4 rows
-  if (prm->usetvref) {  // tallest refinement level: 256-row bands x a cluster of 16 CTAs at most (re-checked for the device below)
-    VarRefPlanes probe{};
-    if (!sor_band_plan(width >> prm->sc_l, height >> prm->sc_l, 4, 128, 16, nop, 1, &probe)) return OFDIS_ERR_UNSUPPORTED;
-  }
+  // tallest refinement level: SOR_MAX_ROWS (levels beyond the largest cluster run as a chain of bands)
+  if (prm->usetvref && (height >> prm->sc_l) > SOR_MAX_ROWS) return OFDIS_ERR_UNSUPPORTED;
 
   ofdis_ctx* ctx = new (std::nothrow) ofdis_ctx();
   if (!ctx) return OFDIS_ERR_NOMEM;
@@ -223,18 +280,12 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
     }
     ctx->own_stream = true;
   }
-  if (prm->usetvref) {  // tallest refinement level: 256-row bands x the largest cluster the device grants
+  if (prm->usetvref) {
     // Defaults (compare with tools/big_configs.py, bench.py --opt): the largest cluster the device grants (an H100
     // grants 16 CTAs), two rows per SOR thread for stereo, one for flow.
     ctx->sor_dev_cluster = sor_max_cluster_size();
     ctx->sor_max_cluster = ctx->sor_dev_cluster;
     ctx->sor_rt = (nop == 1) ? 2 : 1;
-    VarRefPlanes probe{};
-    const int fw = width >> prm->sc_l, fh = height >> prm->sc_l;
-    if (!sor_band_plan(fw, fh, ctx->sor_rt, 128, ctx->sor_max_cluster, nop, prm->tv_solverit, &probe)) {
-      ofdis_destroy(ctx);
-      return OFDIS_ERR_UNSUPPORTED;
-    }
   }
   ctx->pp.max_iter = prm->max_iter;
   ctx->pp.min_iter = prm->min_iter;
@@ -306,36 +357,12 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
     }
   }
   if (ok && prm->usetvref) {
-    // refinement planes sized for the finest level: mask, avg[C], 8 x deriv[C], and the SOR's lane rows
-    const LevelGeom& Lf = ctx->lev[0];
-    const size_t plane = (size_t)Lf.pitch * Lf.h;
-    const int C = prm->noc;
-    // band-skewed SOR array: nb bands x (W4 + hpad + 2) diagonals x hpad lanes x lpitch float4; sized for
-    // the largest level under every plan ofdis_set_option can select
+    // sized for the plans of the clusters the device grants (8 and 16 CTAs); a smaller sor_max_cluster, which only
+    // trades clusters for chains, grows the workspace in ofdis_set_option when its plans need more
     size_t recf4 = 0;
-    for (const LevelGeom& L : ctx->lev)
-      for (int mc = 8; mc <= ctx->sor_dev_cluster; mc += 8)
-        for (int sm = 32; sm <= 128; sm *= 2)
-          for (int rt = 1; rt <= 4; rt *= 2) {
-            VarRefPlanes t{};
-            if (sor_band_plan(L.w, L.h, rt, sm, mc, nop, prm->tv_solverit, &t))
-              recf4 = std::max(recf4, (size_t)t.nb * t.ndiag * t.hpad * t.lpitch);
-          }
-    for (const LevelGeom& L : ctx->lev)  // lane mode (sor_lane_kernel) of the levels it can take
-      if (sor_lane_fits(L.h, 1)) recf4 = std::max(recf4, lane_frame_f4(L.w, L.h));
-    const size_t per_frame = plane * (1 + C + 8 * C) + recf4 * 4;
-    ok = dalloc((void**)&ctx->d_planes, sizeof(float) * per_frame * cap);
-    if (ok) {
-      // never-written lane rows (wavefront ramps, padded lanes) are read by idle SOR lanes: keep them finite
-      cudaMemsetAsync(ctx->d_planes, 0, sizeof(float) * per_frame * cap, ctx->stream);
-      float* q = ctx->d_planes;
-      VarRefPlanes& P = ctx->planes;
-      P.rec = reinterpret_cast<float4*>(q); q += recf4 * 4 * cap;   // first (alignment)
-      P.mask = q; q += plane * cap;
-      P.avg = q; q += plane * C * cap;
-      for (int k = 0; k < 8; ++k) { P.deriv[k] = q; q += plane * C * cap; }
-      P.plane = plane;
-    }
+    int chain_nb = 0;
+    sor_workspace_need(ctx, 8, ctx->sor_dev_cluster, &recf4, &chain_nb);
+    ok = alloc_refinement(ctx, recf4, chain_nb);
   }
   if (!ok) {
     ofdis_destroy(ctx);
@@ -365,6 +392,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   }
   cudaFree(ctx->d_planes);
   cudaFree(ctx->d_fast);
+  cudaFree(ctx->d_chain);
   if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
   return OFDIS_OK;
@@ -663,8 +691,10 @@ static int varref_impl(ofdis_ctx* ctx, int level, int f0, int f1, int n_inner_ov
   VarRefPlanes pl = ctx->planes;
   pl.plane = (size_t)L->pitch * L->h;
   if (!sor_band_plan(L->w, L->h, ctx->sor_rt, ctx->sor_single_max, ctx->sor_max_cluster, ctx->nop, ctx->prm.tv_solverit, &pl))
-    return fail(ctx, OFDIS_ERR_UNSUPPORTED, "varref_refine: level too tall for the largest SOR cluster");
+    return fail(ctx, OFDIS_ERR_UNSUPPORTED, "varref_refine: no SOR band fits one CTA");
   pl.rec_stride = (size_t)pl.nb * pl.ndiag * pl.hpad * pl.lpitch;
+  if (pl.rec_stride > ctx->rec_f4 || (pl.chain && pl.nb > ctx->chain_nb))
+    return fail(ctx, OFDIS_ERR_UNSUPPORTED, "varref_refine: the SOR plan exceeds the refinement workspace");
   pl.lane = 0;
   const int nlaunch = (f1 - f0) * ctx->dirs;  // frames per launch
   L->pdl = (ctx->pdl == 1 || (ctx->pdl == 2 && nlaunch <= SOR_LANE_AUTO_FRAMES)) ? 1 : 0;
@@ -680,8 +710,8 @@ static int varref_impl(ofdis_ctx* ctx, int level, int f0, int f1, int n_inner_ov
   // usefbcon: both directions are refined except on the last level (oflow.cpp:285-294)
   const int D = ctx->dirs;
   const bool fwd_only = (D == 2 && level == ctx->prm.sc_l);
-  const int n = fwd_only ? launch_varref(stepped(*L, 2), pl, vp, f0 * 2, f0 * 2 + (f1 - f0), ctx->stream, ctx->prof)
-                         : launch_varref(*L, pl, vp, f0 * D, f1 * D, ctx->stream, ctx->prof);
+  const int n = fwd_only ? launch_varref(stepped(*L, 2), pl, vp, f0 * 2, f0 * 2 + (f1 - f0), ctx->stream, ctx->prof, ctx->d_chain)
+                         : launch_varref(*L, pl, vp, f0 * D, f1 * D, ctx->stream, ctx->prof, ctx->d_chain);
   if (n < 0) return fail(ctx, OFDIS_ERR_CUDA, "varref kernels launch", cudaGetLastError());
   ctx->launches += n;
   ctx->last_vr_level = level;
@@ -709,12 +739,19 @@ int ofdis_set_option(ofdis_ctx* ctx, const char* name, int value) {
   if (!strcmp(name, "sor_single_max")) {
     if (value != 32 && value != 64 && value != 128) return fail(ctx, OFDIS_ERR_ARG, "sor_single_max: 32, 64 or 128");
     ctx->sor_single_max = value;
-  } else if (!strcmp(name, "sor_max_cluster")) {
-    if (value != 8 && value != 16) return fail(ctx, OFDIS_ERR_ARG, "sor_max_cluster: 8 or 16");
+  } else if (!strcmp(name, "sor_max_cluster")) {  // at most this many bands per cluster; levels with more are chained
+    if (value != 1 && value != 2 && value != 4 && value != 8 && value != 16) return fail(ctx, OFDIS_ERR_ARG, "sor_max_cluster: 1, 2, 4, 8 or 16");
     if (value > ctx->sor_dev_cluster) return fail(ctx, OFDIS_ERR_UNSUPPORTED, "sor_max_cluster: the device does not grant clusters of 16 CTAs");
-    VarRefPlanes probe{};
-    if (ctx->prm.usetvref && !sor_band_plan(ctx->lev[0].w, ctx->lev[0].h, ctx->sor_rt, 128, value, ctx->nop, ctx->prm.tv_solverit, &probe))
-      return fail(ctx, OFDIS_ERR_UNSUPPORTED, "sor_max_cluster: the finest level needs the larger cluster");
+    if (ctx->d_planes) {  // the plans of a smaller cluster may need a larger workspace (chains of larger bands)
+      size_t recf4 = 0;
+      int chain_nb = 0;
+      sor_workspace_need(ctx, value, value, &recf4, &chain_nb);
+      if (recf4 > ctx->rec_f4 || chain_nb > ctx->chain_nb) {
+        CK(cudaSetDevice(ctx->device));
+        if (!alloc_refinement(ctx, std::max(recf4, ctx->rec_f4), std::max(chain_nb, ctx->chain_nb)))
+          return fail(ctx, OFDIS_ERR_NOMEM, "sor_max_cluster: refinement workspace");
+      }
+    }
     ctx->sor_max_cluster = value;
   } else if (!strcmp(name, "sor_lane")) {
     if (value < 0 || value > 2) return fail(ctx, OFDIS_ERR_ARG, "sor_lane: 0, 1 or 2");
@@ -739,9 +776,6 @@ int ofdis_set_option(ofdis_ctx* ctx, const char* name, int value) {
     ctx->planes.fast = value;
   } else if (!strcmp(name, "sor_rows_per_thread")) {
     if (value != 1 && value != 2 && value != 4) return fail(ctx, OFDIS_ERR_ARG, "sor_rows_per_thread: 1, 2 or 4");
-    VarRefPlanes probe{};
-    if (ctx->prm.usetvref && !sor_band_plan(ctx->lev[0].w, ctx->lev[0].h, value, 128, ctx->sor_max_cluster, ctx->nop, ctx->prm.tv_solverit, &probe))
-      return fail(ctx, OFDIS_ERR_UNSUPPORTED, "sor_rows_per_thread: the finest level needs more rows per thread or the larger cluster");
     ctx->sor_rt = value;
   } else {
     return fail(ctx, OFDIS_ERR_ARG, "set_option: unknown option");

@@ -470,11 +470,12 @@ static int sor_sweeps_per_launch(int nop, int hpad, int rt, int K) {
   return kl;
 }
 
-template <int NOP, int HPAD, int RT, bool CL>
+template <int NOP, int HPAD, int RT, int BM>
 static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
-                                cudaStream_t st) {
-  auto kern = sor_wave_kernel<NOP, HPAD, RT, CL>;
-  const int ml = sor_stage_lanes(HPAD, RT, g.w, g.h, CL);
+                                cudaStream_t st, int* sync) {
+  constexpr bool CL = (BM == SOR_CLUSTER);
+  auto kern = sor_wave_kernel<NOP, HPAD, RT, BM>;
+  const int ml = sor_stage_lanes(HPAD, RT, g.w, g.h, BM != SOR_SINGLE);
   const size_t smem = sor_smem_bytes(NOP, HPAD, RT, kl, ml);
   if (smem > 227 * 1024) return cudaErrorInvalidConfiguration;
   // opt-in shared memory (and cluster size) once per device and instantiation
@@ -488,7 +489,7 @@ static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, cons
     smem_set[dev] = smem;
   }
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(nf * (CL ? pl.nb : 1)));
+  cfg.gridDim = dim3((unsigned)(nf * (BM != SOR_SINGLE ? pl.nb : 1)));
   cfg.blockDim = dim3((unsigned)(kl * HPAD + 32));
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
@@ -508,34 +509,48 @@ static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, cons
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, kern, g, pl, vp, kl, ml);
+  return cudaLaunchKernelEx(&cfg, kern, g, pl, vp, kl, ml, sync);
+}
+
+// band of a chain plan: the largest that fits one sweep (sor_band_plan); the only chain instantiation per (NOP, RT)
+template <int NOP, int RT>
+constexpr int sor_chain_hpad() {
+  int p = 256;
+  while (p > 32 && !(p + 32 <= sor_max_threads(p) && sor_smem_bytes(NOP, p, RT, 1, p) <= 227 * 1024)) p /= 2;
+  return p;
 }
 
 template <int NOP, int RT>
 static cudaError_t launch_sor_rt(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
-                                 cudaStream_t st) {
+                                 cudaStream_t st, int* sync) {
+  if (pl.chain) {
+    constexpr int HC = sor_chain_hpad<NOP, RT>();
+    if (pl.hpad != HC || kl != 1 || !sync) return cudaErrorInvalidValue;
+    return launch_sor_t<NOP, HC, RT, SOR_CHAIN>(g, pl, vp, nf, kl, st, sync);
+  }
   const bool cl = pl.nb > 1;
+  constexpr int C1 = SOR_CLUSTER, S1 = SOR_SINGLE;
   switch (pl.hpad) {
-    case 32: return cl ? launch_sor_t<NOP, 32, RT, true>(g, pl, vp, nf, kl, st) : launch_sor_t<NOP, 32, RT, false>(g, pl, vp, nf, kl, st);
-    case 64: return cl ? launch_sor_t<NOP, 64, RT, true>(g, pl, vp, nf, kl, st) : launch_sor_t<NOP, 64, RT, false>(g, pl, vp, nf, kl, st);
-    case 128: return cl ? launch_sor_t<NOP, 128, RT, true>(g, pl, vp, nf, kl, st) : launch_sor_t<NOP, 128, RT, false>(g, pl, vp, nf, kl, st);
-    case 256: return cl ? launch_sor_t<NOP, 256, RT, true>(g, pl, vp, nf, kl, st) : launch_sor_t<NOP, 256, RT, false>(g, pl, vp, nf, kl, st);
+    case 32: return cl ? launch_sor_t<NOP, 32, RT, C1>(g, pl, vp, nf, kl, st, sync) : launch_sor_t<NOP, 32, RT, S1>(g, pl, vp, nf, kl, st, sync);
+    case 64: return cl ? launch_sor_t<NOP, 64, RT, C1>(g, pl, vp, nf, kl, st, sync) : launch_sor_t<NOP, 64, RT, S1>(g, pl, vp, nf, kl, st, sync);
+    case 128: return cl ? launch_sor_t<NOP, 128, RT, C1>(g, pl, vp, nf, kl, st, sync) : launch_sor_t<NOP, 128, RT, S1>(g, pl, vp, nf, kl, st, sync);
+    case 256: return cl ? launch_sor_t<NOP, 256, RT, C1>(g, pl, vp, nf, kl, st, sync) : launch_sor_t<NOP, 256, RT, S1>(g, pl, vp, nf, kl, st, sync);
   }
   return cudaErrorInvalidValue;
 }
 
 template <int NOP>
 static cudaError_t launch_sor(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
-                              cudaStream_t st) {
-  if (pl.rt == 1) return launch_sor_rt<NOP, 1>(g, pl, vp, nf, kl, st);
-  if (pl.rt == 2) return launch_sor_rt<NOP, 2>(g, pl, vp, nf, kl, st);
-  if (pl.rt == 4) return launch_sor_rt<NOP, 4>(g, pl, vp, nf, kl, st);
+                              cudaStream_t st, int* sync) {
+  if (pl.rt == 1) return launch_sor_rt<NOP, 1>(g, pl, vp, nf, kl, st, sync);
+  if (pl.rt == 2) return launch_sor_rt<NOP, 2>(g, pl, vp, nf, kl, st, sync);
+  if (pl.rt == 4) return launch_sor_rt<NOP, 4>(g, pl, vp, nf, kl, st, sync);
   return cudaErrorInvalidValue;
 }
 
 template <int C, int NOP>
 static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const VarRefParams& vp, int f0, int f1,
-                           cudaStream_t st, Profiler* prof) {
+                           cudaStream_t st, Profiler* prof, int* chain_sync) {
   VarRefPlanes pl = pl_in;  // fast mode toggles the (du,dv) ping-pong buffer
   const bool pdl = g.pdl != 0 && prof == nullptr;  // the profiler's events between launches would serialise them anyway
   pl.fcur = 0;
@@ -555,11 +570,11 @@ static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const 
     launch_k(pdl, deriv2_kernel<C>, gridc, block, 0, st, g, pl);
   }
   launches += 3;
-  // SOR: band plan of the level (pl.hpad rows per band, pl.nb bands == CTAs of a cluster) and as
+  // SOR: band plan of the level (pl.hpad rows per band, pl.nb bands == CTAs of a cluster or of a chain) and as
   // many sweeps per launch as the CTA's thread and shared-memory budgets hold (sweeps are sequential,
-  // so K sweeps in ceil(K / kl) launches give the same result)
+  // so K sweeps in ceil(K / kl) launches give the same result); a chain runs one sweep per launch
   const int K = vp.n_solver;
-  const int kl = sor_sweeps_per_launch(NOP, pl.hpad, pl.rt, K);
+  const int kl = pl.chain ? 1 : sor_sweeps_per_launch(NOP, pl.hpad, pl.rt, K);
   for (int it = 0; it < vp.n_inner; ++it) {
     {
       ProfScope scope(prof, KC_VR_ASSEMBLE);
@@ -612,7 +627,7 @@ static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const 
     }
     for (int s = 0; s < K; s += kl) {
       ProfScope scope(prof, KC_VR_SOR);
-      if (launch_sor<NOP>(g, pl, vp, nf, (K - s < kl) ? K - s : kl, st) != cudaSuccess) return -1;
+      if (launch_sor<NOP>(g, pl, vp, nf, (K - s < kl) ? K - s : kl, st, chain_sync) != cudaSuccess) return -1;
       ++launches;
     }
   }
@@ -643,7 +658,7 @@ int sor_max_cluster_size() {
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 8;
   if (cached[dev]) return cached[dev];
   int best = 8;
-  auto kern = sor_wave_kernel<2, 128, 1, true>;
+  auto kern = sor_wave_kernel<2, 128, 1, SOR_CLUSTER>;
   const size_t smem = sor_smem_bytes(2, 128, 1, 3, 128);  // 128-row bands, 3 sweeps in flight: the largest common configuration
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess &&
       cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
@@ -667,11 +682,11 @@ int sor_max_cluster_size() {
 }
 
 int launch_varref(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int f0, int f1,
-                  cudaStream_t st, Profiler* prof) {
-  if (g.noc == 1 && g.nop == 2) return launch_varref_t<1, 2>(g, pl, vp, f0, f1, st, prof);
-  if (g.noc == 3 && g.nop == 2) return launch_varref_t<3, 2>(g, pl, vp, f0, f1, st, prof);
-  if (g.noc == 1 && g.nop == 1) return launch_varref_t<1, 1>(g, pl, vp, f0, f1, st, prof);
-  if (g.noc == 3 && g.nop == 1) return launch_varref_t<3, 1>(g, pl, vp, f0, f1, st, prof);
+                  cudaStream_t st, Profiler* prof, int* chain_sync) {
+  if (g.noc == 1 && g.nop == 2) return launch_varref_t<1, 2>(g, pl, vp, f0, f1, st, prof, chain_sync);
+  if (g.noc == 3 && g.nop == 2) return launch_varref_t<3, 2>(g, pl, vp, f0, f1, st, prof, chain_sync);
+  if (g.noc == 1 && g.nop == 1) return launch_varref_t<1, 1>(g, pl, vp, f0, f1, st, prof, chain_sync);
+  if (g.noc == 3 && g.nop == 1) return launch_varref_t<3, 1>(g, pl, vp, f0, f1, st, prof, chain_sync);
   return -1;
 }
 

@@ -1,5 +1,5 @@
-"""BASELINE configs[2] (1920x1080 RGB, op-3 geometry, L1 cost) and configs[4] (2880x1988 stereo, op 4) on
-one GPU: step time and, per kernel class, the achieved algorithmic GB/s (SURVEY 8d formulas) -- the
+"""BASELINE configs[2] (1920x1080 RGB, op-3 geometry, L1 cost), configs[4] (2880x1988 stereo, op 4) and 4K UHD
+gray flow refined at level 0 (3840x2160) on one GPU: step time and, per kernel class, the achieved algorithmic GB/s (SURVEY 8d formulas) -- the
 levels of these configs are the ones that stream from HBM.  Also the SOR time per pyramid level.
 python tools/big_configs.py [B ...] [--opt name=value ...] [--cfg substring]"""
 import sys, time, json
@@ -13,6 +13,9 @@ CFGS = {
     "cfg3_1920x1080_rgb_l1": dict(size=(1080, 1920), ch=3, nop=2, prm=lambda: params.from_cli_numbers(
         "6 2 16 16 0.05 0.95 0 12 0.75 0 1 1 1 10 10 5 1 3 1.6 0".split(), noc=3)),
     "cfg5_2880x1988_stereo_op4": dict(size=(1988, 2880), ch=1, nop=1, prm=lambda: params.operating_point(4, 2880, noc=1, nop=1)),
+    # 4K UHD gray flow refined at level 0: 2176 rows after padding, more bands than a cluster holds (SOR chain)
+    "uhd_3840x2160_gray_flow_l0": dict(size=(2160, 3840), ch=1, nop=2, prm=lambda: params.from_cli_numbers(
+        "5 0 12 12 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=1)),
 }
 
 

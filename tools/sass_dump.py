@@ -3,7 +3,7 @@ Hopper-specific mnemonics (UBLKCP = cp.async.bulk, UTMALDG = TMA tensor tile, SY
 STAS = st.async to a peer CTA's shared memory, UCGABAR = cluster barrier, MUFU.RCP = the hoisted
 reciprocals of the stereo SOR).  No GPU needed:
     python tools/sass_dump.py > sass_summary.txt
-    python tools/sass_dump.py --full sor_wave_kernelILi2ELi64ELi1ELb0 > sass_sor_flow.txt"""
+    python tools/sass_dump.py --full sor_wave_kernelILi2ELi64ELi1ELi0 > sass_sor_flow.txt"""
 import collections
 import os
 import re
