@@ -176,6 +176,16 @@ int ofdis_get_patches(ofdis_ctx* ctx, int frame, int level, float* p, float* pwe
 long ofdis_debug_get(ofdis_ctx* ctx, const char* name, int frame, float* dst, size_t max_floats);
 /* Test hook: run only the first n_inner inner iterations of the refinement. */
 int ofdis_debug_varref_iters(ofdis_ctx* ctx, int level, int f0, int f1, int n_inner);
+/* Test hook: the stereo SOR's division b[i] / a[i] on the context's device and stream, for n host values.
+ * q_fast: the exact SOR kernels' written-out IEEE division; q_plain: the compiler's `/`; unsafe[i] = 1 where the
+ * kernels' exponent test sends the pair to the plain division (a or, if b != +-0, b outside 2^-60 <= |x| < 2^61).
+ * Where unsafe[i] == 0, q_fast[i] is the correctly rounded quotient. */
+int ofdis_debug_div(ofdis_ctx* ctx, const float* a, const float* b, long n, float* q_fast, float* q_plain,
+                    unsigned char* unsafe);
+/* Test hook: how often the stereo SOR took the plain division since create or the last reset -- tiles of
+ * sor_wave_kernel and pixel updates of a warp of sor_lane_kernel (0 on ordinary inputs: their operands stay in range).
+ * Synchronises the context's stream; reset != 0 zeroes the count after reading it. */
+int ofdis_debug_sor_div_fallbacks(ofdis_ctx* ctx, unsigned long long* count, int reset);
 
 /* Number of kernels this library has launched on the context since creation. */
 long ofdis_launch_count(const ofdis_ctx* ctx);

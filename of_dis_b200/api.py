@@ -31,6 +31,7 @@ EXPORTS = [
     "ofdis_set_camlr", "ofdis_set_dp_thresh_sq", "ofdis_packed_images_frame_floats", "ofdis_upload_packed_images",
     "ofdis_upload_frames_u8", "ofdis_finest_level_frame_floats", "ofdis_upload_finest_level", "ofdis_get_flow_fullres",
     "ofdis_get_level", "ofdis_upload_level_fb", "ofdis_set_option", "ofdis_profile_levels", "ofdis_set_direction",
+    "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks",
 ]
 
 
@@ -82,6 +83,8 @@ def lib():
         L.ofdis_patgrid_aggregate.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3
         L.ofdis_varref_refine.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3
         L.ofdis_debug_varref_iters.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 4
+        L.ofdis_debug_div.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_long] + [ctypes.c_void_p] * 3
+        L.ofdis_debug_sor_div_fallbacks.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_ulonglong), ctypes.c_int]
         L.ofdis_run.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
         L.ofdis_get_flow.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
         L.ofdis_set_flow.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
@@ -303,6 +306,23 @@ class Context:
         if name in ("dudv", "rec"):
             return buf.reshape(li["h"], pitch, per)[:, :li["w"]]
         return buf.reshape(per, li["h"], pitch)[:, :, :li["w"]]
+
+    def debug_div(self, a: np.ndarray, b: np.ndarray):
+        """The stereo SOR's division b / a on the device: (q_fast, q_plain, unsafe) -- the SOR kernels' written-out
+        IEEE division, the compiler's `/`, and where the kernels' range test sends the pair to the latter."""
+        a = np.ascontiguousarray(a, np.float32).reshape(-1)
+        b = np.ascontiguousarray(b, np.float32).reshape(-1)
+        assert a.shape == b.shape
+        q_fast, q_plain = np.empty_like(a), np.empty_like(a)
+        unsafe = np.empty(a.shape, np.uint8)
+        self._ck(lib().ofdis_debug_div(self._h, _ptr(a), _ptr(b), a.size, _ptr(q_fast), _ptr(q_plain), _ptr(unsafe)))
+        return q_fast, q_plain, unsafe.astype(bool)
+
+    def sor_div_fallbacks(self, reset: bool = False) -> int:
+        """How often the stereo SOR redid work with the plain division since create or the last reset."""
+        v = ctypes.c_ulonglong()
+        self._ck(lib().ofdis_debug_sor_div_fallbacks(self._h, ctypes.byref(v), 1 if reset else 0))
+        return v.value
 
 
 # ---------------------------------------------------------------------------

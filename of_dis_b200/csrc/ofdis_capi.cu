@@ -65,6 +65,7 @@ struct ofdis_ctx {
   int* d_chain = nullptr;           // SOR chain: ticket counter + progress words [frame][band], zero between launches
   size_t rec_f4 = 0;                // float4 per frame of the SOR's lane rows in d_planes
   int chain_nb = 0;                 // bands per frame d_chain holds
+  unsigned long long* d_div_fb = nullptr;  // stereo SOR work redone with the plain division (ofdis_debug_sor_div_fallbacks)
   int last_vr_fcur = 0;
   PatchParams pp{};
   long launches = 0;
@@ -107,6 +108,17 @@ int fail(ofdis_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess) 
     cudaError_t e__ = (call);                                           \
     if (e__ != cudaSuccess) return fail(ctx, OFDIS_ERR_CUDA, #call, e__); \
   } while (0)
+
+// ofdis_debug_div: the stereo SOR's division helpers (ofdis_internal.cuh), exactly as the SOR kernels call them
+__global__ void debug_div_kernel(const float* a, const float* b, long n, float* q_fast, float* q_plain,
+                                 unsigned char* unsafe) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float A = a[i], B = b[i];
+  q_fast[i] = fdiv_quot(A, B, fdiv_rcp(A));
+  q_plain[i] = B / A;
+  unsafe[i] = fdiv_unsafe(A, B) ? 1 : 0;
+}
 
 // camparam / optparam derivation (oflow.cpp:81-92,142-157; patchgrid.cpp:42-48)
 void make_level(LevelGeom& L, const ofdis_ctx* c, int sl) {
@@ -362,7 +374,8 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
     size_t recf4 = 0;
     int chain_nb = 0;
     sor_workspace_need(ctx, 8, ctx->sor_dev_cluster, &recf4, &chain_nb);
-    ok = alloc_refinement(ctx, recf4, chain_nb);
+    ok = alloc_refinement(ctx, recf4, chain_nb) && dalloc((void**)&ctx->d_div_fb, sizeof(unsigned long long));
+    if (ok) cudaMemsetAsync(ctx->d_div_fb, 0, sizeof(unsigned long long), ctx->stream);
   }
   if (!ok) {
     ofdis_destroy(ctx);
@@ -393,6 +406,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_planes);
   cudaFree(ctx->d_fast);
   cudaFree(ctx->d_chain);
+  cudaFree(ctx->d_div_fb);
   if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
   return OFDIS_OK;
@@ -710,8 +724,8 @@ static int varref_impl(ofdis_ctx* ctx, int level, int f0, int f1, int n_inner_ov
   // usefbcon: both directions are refined except on the last level (oflow.cpp:285-294)
   const int D = ctx->dirs;
   const bool fwd_only = (D == 2 && level == ctx->prm.sc_l);
-  const int n = fwd_only ? launch_varref(stepped(*L, 2), pl, vp, f0 * 2, f0 * 2 + (f1 - f0), ctx->stream, ctx->prof, ctx->d_chain)
-                         : launch_varref(*L, pl, vp, f0 * D, f1 * D, ctx->stream, ctx->prof, ctx->d_chain);
+  const int n = fwd_only ? launch_varref(stepped(*L, 2), pl, vp, f0 * 2, f0 * 2 + (f1 - f0), ctx->stream, ctx->prof, ctx->d_chain, ctx->d_div_fb)
+                         : launch_varref(*L, pl, vp, f0 * D, f1 * D, ctx->stream, ctx->prof, ctx->d_chain, ctx->d_div_fb);
   if (n < 0) return fail(ctx, OFDIS_ERR_CUDA, "varref kernels launch", cudaGetLastError());
   ctx->launches += n;
   ctx->last_vr_level = level;
@@ -948,6 +962,39 @@ long ofdis_debug_get(ofdis_ctx* ctx, const char* name, int frame, float* dst, si
   if (cudaMemcpyAsync(dst, src, sizeof(float) * n, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
   if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
   return (long)n;
+}
+
+int ofdis_debug_div(ofdis_ctx* ctx, const float* a, const float* b, long n, float* q_fast, float* q_plain,
+                    unsigned char* unsafe) {
+  if (!ctx || n < 0 || (n && (!a || !b || !q_fast || !q_plain || !unsafe))) return OFDIS_ERR_ARG;
+  if (!n) return OFDIS_OK;
+  CK(cudaSetDevice(ctx->device));
+  float* d = nullptr;  // a, b, q_fast, q_plain, then the flags
+  CK(cudaMalloc((void**)&d, (size_t)n * (4 * sizeof(float) + 1)));
+  cudaError_t e = cudaMemcpyAsync(d, a, sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d + n, b, sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) {
+    debug_div_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d, d + n, n, d + 2 * n, d + 3 * n,
+                                                                           reinterpret_cast<unsigned char*>(d + 4 * n));
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(q_fast, d + 2 * n, sizeof(float) * n, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(q_plain, d + 3 * n, sizeof(float) * n, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(unsafe, d + 4 * n, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  cudaFree(d);
+  if (e != cudaSuccess) return fail(ctx, OFDIS_ERR_CUDA, "debug_div", e);
+  return OFDIS_OK;
+}
+
+int ofdis_debug_sor_div_fallbacks(ofdis_ctx* ctx, unsigned long long* count, int reset) {
+  if (!ctx || !count) return OFDIS_ERR_ARG;
+  if (!ctx->d_div_fb) return fail(ctx, OFDIS_ERR_ARG, "debug_sor_div_fallbacks: context created with usetvref=0");
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaMemcpyAsync(count, ctx->d_div_fb, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+  if (reset) CK(cudaMemsetAsync(ctx->d_div_fb, 0, sizeof(unsigned long long), ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return OFDIS_OK;
 }
 
 long ofdis_launch_count(const ofdis_ctx* ctx) { return ctx ? ctx->launches : 0; }

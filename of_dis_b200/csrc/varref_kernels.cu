@@ -472,7 +472,7 @@ static int sor_sweeps_per_launch(int nop, int hpad, int rt, int K) {
 
 template <int NOP, int HPAD, int RT, int BM>
 static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
-                                cudaStream_t st, int* sync) {
+                                cudaStream_t st, int* sync, unsigned long long* div_fb) {
   constexpr bool CL = (BM == SOR_CLUSTER);
   auto kern = sor_wave_kernel<NOP, HPAD, RT, BM>;
   const int ml = sor_stage_lanes(HPAD, RT, g.w, g.h, BM != SOR_SINGLE);
@@ -509,7 +509,7 @@ static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, cons
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, kern, g, pl, vp, kl, ml, sync);
+  return cudaLaunchKernelEx(&cfg, kern, g, pl, vp, kl, ml, sync, div_fb);
 }
 
 // band of a chain plan: the largest that fits one sweep (sor_band_plan); the only chain instantiation per (NOP, RT)
@@ -522,35 +522,53 @@ constexpr int sor_chain_hpad() {
 
 template <int NOP, int RT>
 static cudaError_t launch_sor_rt(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
-                                 cudaStream_t st, int* sync) {
+                                 cudaStream_t st, int* sync, unsigned long long* div_fb) {
   if (pl.chain) {
     constexpr int HC = sor_chain_hpad<NOP, RT>();
     if (pl.hpad != HC || kl != 1 || !sync) return cudaErrorInvalidValue;
-    return launch_sor_t<NOP, HC, RT, SOR_CHAIN>(g, pl, vp, nf, kl, st, sync);
+    return launch_sor_t<NOP, HC, RT, SOR_CHAIN>(g, pl, vp, nf, kl, st, sync, div_fb);
   }
   const bool cl = pl.nb > 1;
   constexpr int C1 = SOR_CLUSTER, S1 = SOR_SINGLE;
   switch (pl.hpad) {
-    case 32: return cl ? launch_sor_t<NOP, 32, RT, C1>(g, pl, vp, nf, kl, st, sync) : launch_sor_t<NOP, 32, RT, S1>(g, pl, vp, nf, kl, st, sync);
-    case 64: return cl ? launch_sor_t<NOP, 64, RT, C1>(g, pl, vp, nf, kl, st, sync) : launch_sor_t<NOP, 64, RT, S1>(g, pl, vp, nf, kl, st, sync);
-    case 128: return cl ? launch_sor_t<NOP, 128, RT, C1>(g, pl, vp, nf, kl, st, sync) : launch_sor_t<NOP, 128, RT, S1>(g, pl, vp, nf, kl, st, sync);
-    case 256: return cl ? launch_sor_t<NOP, 256, RT, C1>(g, pl, vp, nf, kl, st, sync) : launch_sor_t<NOP, 256, RT, S1>(g, pl, vp, nf, kl, st, sync);
+    case 32: return cl ? launch_sor_t<NOP, 32, RT, C1>(g, pl, vp, nf, kl, st, sync, div_fb) : launch_sor_t<NOP, 32, RT, S1>(g, pl, vp, nf, kl, st, sync, div_fb);
+    case 64: return cl ? launch_sor_t<NOP, 64, RT, C1>(g, pl, vp, nf, kl, st, sync, div_fb) : launch_sor_t<NOP, 64, RT, S1>(g, pl, vp, nf, kl, st, sync, div_fb);
+    case 128: return cl ? launch_sor_t<NOP, 128, RT, C1>(g, pl, vp, nf, kl, st, sync, div_fb) : launch_sor_t<NOP, 128, RT, S1>(g, pl, vp, nf, kl, st, sync, div_fb);
+    case 256: return cl ? launch_sor_t<NOP, 256, RT, C1>(g, pl, vp, nf, kl, st, sync, div_fb) : launch_sor_t<NOP, 256, RT, S1>(g, pl, vp, nf, kl, st, sync, div_fb);
   }
   return cudaErrorInvalidValue;
 }
 
 template <int NOP>
 static cudaError_t launch_sor(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
-                              cudaStream_t st, int* sync) {
-  if (pl.rt == 1) return launch_sor_rt<NOP, 1>(g, pl, vp, nf, kl, st, sync);
-  if (pl.rt == 2) return launch_sor_rt<NOP, 2>(g, pl, vp, nf, kl, st, sync);
-  if (pl.rt == 4) return launch_sor_rt<NOP, 4>(g, pl, vp, nf, kl, st, sync);
+                              cudaStream_t st, int* sync, unsigned long long* div_fb) {
+  if (pl.rt == 1) return launch_sor_rt<NOP, 1>(g, pl, vp, nf, kl, st, sync, div_fb);
+  if (pl.rt == 2) return launch_sor_rt<NOP, 2>(g, pl, vp, nf, kl, st, sync, div_fb);
+  if (pl.rt == 4) return launch_sor_rt<NOP, 4>(g, pl, vp, nf, kl, st, sync, div_fb);
   return cudaErrorInvalidValue;
 }
 
+// Opt-in dynamic shared memory of a kernel that the launchers of gray and RGB levels share (sor_lane_kernel<NOP>,
+// sor_redblack_kernel<NOP>): the attribute belongs to the kernel, so its cache must too.  With one cache per
+// launch_varref_t<C, NOP> an RGB level that needed less shared memory lowered the attribute behind the gray
+// levels' cache, and their next larger launch failed (tests/test_sor_division_gpu.py after the RGB stereo tests).
+template <typename Tag, typename Kern>
+static bool smem_optin(Kern kern, size_t smem) {
+  static size_t smem_set[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev >= 0 && dev < 64 && smem_set[dev] < smem) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return false;
+    smem_set[dev] = smem;
+  }
+  return true;
+}
+template <int NOP> struct LaneKernTag {};
+template <int NOP> struct RbKernTag {};
+
 template <int C, int NOP>
 static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const VarRefParams& vp, int f0, int f1,
-                           cudaStream_t st, Profiler* prof, int* chain_sync) {
+                           cudaStream_t st, Profiler* prof, int* chain_sync, unsigned long long* div_fb) {
   VarRefPlanes pl = pl_in;  // fast mode toggles the (du,dv) ping-pong buffer
   const bool pdl = g.pdl != 0 && prof == nullptr;  // the profiler's events between launches would serialise them anyway
   pl.fcur = 0;
@@ -593,13 +611,7 @@ static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const 
       ProfScope scope(prof, KC_VR_SOR);
       const size_t smem = rb_smem_bytes(NOP, K);
       if (K < 1 || smem > 227 * 1024) return -1;
-      static size_t smem_set[64] = {0};
-      int dev = 0;
-      cudaGetDevice(&dev);
-      if (dev >= 0 && dev < 64 && smem_set[dev] < smem) {
-        if (cudaFuncSetAttribute(sor_redblack_kernel<NOP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
-        smem_set[dev] = smem;
-      }
+      if (!smem_optin<RbKernTag<NOP>>(sor_redblack_kernel<NOP>, smem)) return -1;
       const dim3 grid_rb((g.w + RB_TILE - 1) / RB_TILE, (g.h + RB_TILE - 1) / RB_TILE, nf);
       launch_k(pdl, sor_redblack_kernel<NOP>, grid_rb, dim3(256), smem, st, g, pl, vp);
       pl.fcur ^= 1;
@@ -613,21 +625,15 @@ static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const 
         ProfScope scope(prof, KC_VR_SOR);
         const int kk = (K - s < kll) ? K - s : kll;
         const size_t smem = sl_smem_bytes(pl.nb, kk);
-        static size_t smem_set[64] = {0};
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (dev >= 0 && dev < 64 && smem_set[dev] < smem) {
-          if (cudaFuncSetAttribute(sor_lane_kernel<NOP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
-          smem_set[dev] = smem;
-        }
-        launch_k(pdl, sor_lane_kernel<NOP>, dim3(nf), dim3(pl.nb * kk * 32), smem, st, g, pl, vp, kk);
+        if (!smem_optin<LaneKernTag<NOP>>(sor_lane_kernel<NOP>, smem)) return -1;
+        launch_k(pdl, sor_lane_kernel<NOP>, dim3(nf), dim3(pl.nb * kk * 32), smem, st, g, pl, vp, kk, div_fb);
         ++launches;
       }
       continue;
     }
     for (int s = 0; s < K; s += kl) {
       ProfScope scope(prof, KC_VR_SOR);
-      if (launch_sor<NOP>(g, pl, vp, nf, (K - s < kl) ? K - s : kl, st, chain_sync) != cudaSuccess) return -1;
+      if (launch_sor<NOP>(g, pl, vp, nf, (K - s < kl) ? K - s : kl, st, chain_sync, div_fb) != cudaSuccess) return -1;
       ++launches;
     }
   }
@@ -682,11 +688,11 @@ int sor_max_cluster_size() {
 }
 
 int launch_varref(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int f0, int f1,
-                  cudaStream_t st, Profiler* prof, int* chain_sync) {
-  if (g.noc == 1 && g.nop == 2) return launch_varref_t<1, 2>(g, pl, vp, f0, f1, st, prof, chain_sync);
-  if (g.noc == 3 && g.nop == 2) return launch_varref_t<3, 2>(g, pl, vp, f0, f1, st, prof, chain_sync);
-  if (g.noc == 1 && g.nop == 1) return launch_varref_t<1, 1>(g, pl, vp, f0, f1, st, prof, chain_sync);
-  if (g.noc == 3 && g.nop == 1) return launch_varref_t<3, 1>(g, pl, vp, f0, f1, st, prof, chain_sync);
+                  cudaStream_t st, Profiler* prof, int* chain_sync, unsigned long long* div_fb) {
+  if (g.noc == 1 && g.nop == 2) return launch_varref_t<1, 2>(g, pl, vp, f0, f1, st, prof, chain_sync, div_fb);
+  if (g.noc == 3 && g.nop == 2) return launch_varref_t<3, 2>(g, pl, vp, f0, f1, st, prof, chain_sync, div_fb);
+  if (g.noc == 1 && g.nop == 1) return launch_varref_t<1, 1>(g, pl, vp, f0, f1, st, prof, chain_sync, div_fb);
+  if (g.noc == 3 && g.nop == 1) return launch_varref_t<3, 1>(g, pl, vp, f0, f1, st, prof, chain_sync, div_fb);
   return -1;
 }
 

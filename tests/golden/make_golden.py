@@ -43,9 +43,28 @@ def write_digests(out_dir):
         i0, i1, pyr, prm = t.baseline_inputs(name)
         out["baseline_%s_input" % name] = t.input_digest(i0, i1)
         out["baseline_" + name] = t.digest(ref_driver.ref_run(pyr, prm))
+    out.update(sor_division_digests())
     with open(os.path.join(out_dir, "reference_digests.json"), "w") as f:
         json.dump(out, f, indent=1, sort_keys=True)
         f.write("\n")
+
+def sor_division_digests():
+    """The stereo SOR's division regimes (tests/test_sor_division_gpu.py: parameters that drive A11 and B1 out of the
+    range of the kernels' written-out division): whole run, and the refinement of level sc_l from the regime's
+    initial disparity."""
+    import test_oracle as t
+    from test_sor_division_gpu import DIV_CASES, REGIMES, division_inputs, initial_disparity
+
+    out = {}
+    for case in DIV_CASES:
+        for regime in REGIMES:
+            i0, i1, pyr, prm = division_inputs(case, regime)
+            key = "sor_div_%s_%s" % (case, regime)
+            out[key + "_input"] = t.input_digest(i0, i1)
+            out[key + "_run"] = t.digest(ref_driver.ref_run(pyr, prm))
+            out[key + "_varref"] = t.digest(ref_driver.ref_level_varref(pyr, prm, prm.sc_l, initial_disparity(regime, pyr, prm)))
+    return out
+
 
 CASES = {
     # name: (h, w, channels, cli numbers, nop, amp, stereo)

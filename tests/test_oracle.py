@@ -13,6 +13,7 @@ import pytest
 
 from of_dis_b200 import params, preprocess, synth
 from oracle import ref_driver
+from test_sor_division_gpu import DIV_CASES, REGIMES, division_inputs, initial_disparity
 
 GOLDEN_DIR = os.path.join(os.path.dirname(__file__), "golden")
 GOLDEN = sorted(glob.glob(os.path.join(GOLDEN_DIR, "*.npz")))
@@ -176,6 +177,20 @@ def test_port_vs_reference_at_baseline_sizes(name, oracle_port):
     i0, i1, pyr, prm = baseline_inputs(name)
     check_inputs("baseline_" + name, i0, i1)
     assert digest(oracle_port.port_run(pyr, prm)) == REF_DIGESTS["baseline_" + name]
+
+
+@pytest.mark.parametrize("regime", list(REGIMES))
+@pytest.mark.parametrize("case", DIV_CASES)
+def test_port_vs_reference_at_the_sor_division_regimes(case, regime, oracle_port):
+    """The stereo parameter regimes of tests/test_sor_division_gpu.py, which drive the SOR's A11 and B1 out of the
+    range of the GPU's written-out division (or make B1 exactly zero): whole run, and the refinement of level sc_l
+    from the regime's initial disparity, bit for bit as the reference build computes them."""
+    i0, i1, pyr, prm = division_inputs(case, regime)
+    key = "sor_div_%s_%s" % (case, regime)
+    check_inputs(key, i0, i1)
+    assert digest(oracle_port.port_run(pyr, prm)) == REF_DIGESTS[key + "_run"]
+    fl = initial_disparity(regime, pyr, prm)
+    assert digest(oracle_port.port_level_varref(pyr, prm, prm.sc_l, fl)) == REF_DIGESTS[key + "_varref"]
 
 
 @pytest.mark.skipif(not ref_driver.ref_available("m1c1"), reason="oracle/_ref not built")
