@@ -29,17 +29,15 @@ struct ofdis_ctx {
   int dirs = 1, cap = 0;
   int last_vr_fstep = 1;
   int sel_dir = -1;                // ofdis_set_direction: -1 = both directions / the forward grid
-  // SOR band plan (sor_band_plan): levels of up to sor_single_max rows run in one CTA, taller ones in a
-  // cluster of up to sor_max_cluster CTAs (8 = portable limit; 16 where the device grants it), levels with
-  // more bands than that in a chain of CTAs (one sweep per launch)
-  int sor_single_max = 128, sor_max_cluster = 8, sor_dev_cluster = 8, sor_rt = 1;  // defaults set in ofdis_create
-  // levels of few 32-row bands: pixel wavefront (sor_lane_kernel) instead of the block wavefront.  0 never, 1 always,
-  // 2 (default) for launches of up to SOR_LANE_AUTO_FRAMES frames on levels of one or two bands (sor_lane_preferred):
-  // there it is faster per launch (H100, 700 W, one stream, operating point 2: 1 pair 0.344 vs 0.456 ms per step,
-  // 8 pairs 0.365 vs 0.470 ms), but it needs 200 KB of shared memory per CTA at 56-row levels (one CTA per SM), which
-  // costs 10-13 % of throughput when ten streams of 32 or 64 frames overlap (bench.py `value`)
-  int sor_lane = 2;
-  int last_vr_lane = 0;  // layout of the last refinement (ofdis_debug_get)
+  // SOR options (sor_plan).  max_cluster: 8 = portable limit, 16 where the device grants it (sor_dev_cluster); rt:
+  // set in ofdis_create.  lane: pixel wavefront (sor_lane_kernel) instead of the block wavefront on levels of few
+  // 32-row bands, 0 never, 1 always, 2 (default) for launches of up to SOR_LANE_AUTO_FRAMES frames on levels of one
+  // or two bands: there it is faster per launch (H100, 700 W, one stream, operating point 2: 1 pair 0.344 vs 0.456 ms
+  // per step, 8 pairs 0.365 vs 0.470 ms), but it needs 200 KB of shared memory per CTA at 56-row levels (one CTA per
+  // SM), which costs 10-13 % of throughput when ten streams of 32 or 64 frames overlap (bench.py `value`)
+  SorOptions sor{/*lane*/ 2, /*fast*/ 0, /*rt*/ 1, /*single_max*/ 128, /*max_cluster*/ 8};
+  int sor_dev_cluster = 8;
+  SorPlan last_sor{};  // plan of the last refinement (ofdis_debug_get decodes its planes)
   // programmatic dependent launch of the level loop's kernels (pdl_wait, ofdis_internal.cuh): 0 never, 1 always,
   // 2 (default) for launches of up to SOR_LANE_AUTO_FRAMES frames: H100, one stream, graph replay: 1 pair
   // 0.374 -> 0.344 ms, 8 pairs 0.390 -> 0.363 ms; 64 pairs 0.659 -> 0.690 ms, and 5-14 % less throughput when ten
@@ -78,7 +76,6 @@ struct ofdis_ctx {
 };
 
 namespace {
-constexpr int SOR_LANE_AUTO_FRAMES = 16;
 
 // NVTX range per stage and level ("patch L3", "densify L3", "varref L3", "pyramid", "upsample"): free
 // when no profiler is attached, names the stages in Nsight Systems / ncu --nvtx timelines.
@@ -156,6 +153,9 @@ void make_level(LevelGeom& L, const ofdis_ctx* c, int sl) {
   L.fb_reach = nullptr;
 }
 
+// programmatic dependent launch for a launch of `frames` internal frames (ofdis_set_option "pdl")
+int pdl_for(const ofdis_ctx* c, int frames) { return c->pdl == 1 || (c->pdl == 2 && frames <= SOR_LANE_AUTO_FRAMES) ? 1 : 0; }
+
 LevelGeom* level_of(ofdis_ctx* c, int level) {
   if (level < c->prm.sc_l || level > c->prm.sc_f) return nullptr;
   return &c->lev[level - c->prm.sc_l];
@@ -187,24 +187,22 @@ int run_levels(ofdis_ctx* ctx, int nframes, int use_initflow) {
   return OFDIS_OK;
 }
 
-// Float4 per frame of the SOR's band-skewed lane rows (nb bands x (W4 + hpad + 2) diagonals x hpad lanes x lpitch)
-// and most bands of a chain, over every level, sor_single_max and sor_rows_per_thread with sor_max_cluster in
-// mc_lo .. mc_hi (powers of two), and the lane layout (sor_lane_kernel) of the levels it can take.
+// Float4 per frame of the SOR's lane rows and most bands of a chain that the plans (sor_plan) of every level need,
+// over sor_single_max, sor_rows_per_thread and sor_lane with sor_max_cluster in mc_lo .. mc_hi (powers of two).
 void sor_workspace_need(const ofdis_ctx* c, int mc_lo, int mc_hi, size_t* recf4, int* chain_nb) {
   *recf4 = 0;
   *chain_nb = 0;
-  for (const LevelGeom& L : c->lev) {
+  for (const LevelGeom& L : c->lev)
     for (int mc = mc_lo; mc <= mc_hi; mc *= 2)
       for (int sm = 32; sm <= 128; sm *= 2)
-        for (int rt = 1; rt <= 4; rt *= 2) {
-          VarRefPlanes t{};
-          if (sor_band_plan(L.w, L.h, rt, sm, mc, c->nop, c->prm.tv_solverit, &t)) {
-            *recf4 = std::max(*recf4, (size_t)t.nb * t.ndiag * t.hpad * t.lpitch);
-            if (t.chain) *chain_nb = std::max(*chain_nb, t.nb);
+        for (int rt = 1; rt <= 4; rt *= 2)
+          for (int lane = 0; lane <= 1; ++lane) {
+            SorPlan p;
+            if (sor_plan(L, c->prm.tv_solverit, SorOptions{lane, 0, rt, sm, mc}, 1, VarRefPlanes{}, &p)) {
+              *recf4 = std::max(*recf4, p.pl.rec_stride);
+              *chain_nb = std::max(*chain_nb, p.chain_nb);
+            }
           }
-        }
-    if (sor_lane_fits(L.h, 1)) *recf4 = std::max(*recf4, lane_frame_f4(L.w, L.h));
-  }
 }
 
 // (Re)allocates the refinement planes of the finest level (mask, avg[C], 8 x deriv[C]) behind `recf4` float4 of SOR
@@ -296,8 +294,8 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
     // Defaults (compare with tools/big_configs.py, bench.py --opt): the largest cluster the device grants (an H100
     // grants 16 CTAs), two rows per SOR thread for stereo, one for flow.
     ctx->sor_dev_cluster = sor_max_cluster_size();
-    ctx->sor_max_cluster = ctx->sor_dev_cluster;
-    ctx->sor_rt = (nop == 1) ? 2 : 1;
+    ctx->sor.max_cluster = ctx->sor_dev_cluster;
+    ctx->sor.rt = (nop == 1) ? 2 : 1;
   }
   ctx->pp.max_iter = prm->max_iter;
   ctx->pp.min_iter = prm->min_iter;
@@ -655,7 +653,7 @@ int ofdis_patgrid_optimize(ofdis_ctx* ctx, int level, int f0, int f1, int init_f
   NvtxRange nvtx("patch", level);
   const int q0 = ctx->sel_dir >= 0 ? f0 * ctx->dirs + ctx->sel_dir : f0 * ctx->dirs;
   const int q1 = ctx->sel_dir >= 0 ? q0 + 1 : f1 * ctx->dirs;
-  L->pdl = (ctx->pdl == 1 || (ctx->pdl == 2 && q1 - q0 <= SOR_LANE_AUTO_FRAMES)) ? 1 : 0;
+  L->pdl = pdl_for(ctx, q1 - q0);
   const int n = launch_patch_optimize(*L, ctx->pp, q0, q1, init_from_coarser != 0, ctx->stream, ctx->prof);
   if (n < 0) return fail(ctx, OFDIS_ERR_CUDA, "patch_optimize_kernel launch", cudaGetLastError());
   ctx->launches += n;
@@ -668,7 +666,7 @@ int ofdis_patgrid_aggregate(ofdis_ctx* ctx, int level, int f0, int f1) {
   if (!L || f0 < 0 || f1 > ctx->max_frames || f0 >= f1) return fail(ctx, OFDIS_ERR_ARG, "patgrid_aggregate: bad argument");
   CK(cudaSetDevice(ctx->device));
   NvtxRange nvtx("densify", level);
-  L->pdl = (ctx->pdl == 1 || (ctx->pdl == 2 && (f1 - f0) * ctx->dirs <= SOR_LANE_AUTO_FRAMES)) ? 1 : 0;
+  L->pdl = pdl_for(ctx, (f1 - f0) * ctx->dirs);
   int n;
   if (ctx->dirs == 2) {
     // both grids' patch positions first; the backward flow is not densified on the last level (oflow.cpp:269-270)
@@ -702,34 +700,22 @@ static int varref_impl(ofdis_ctx* ctx, int level, int f0, int f1, int n_inner_ov
   vp.quarter_alpha = 0.25f * ctx->prm.tv_alpha;
   vp.half_gamma_over3 = ctx->prm.tv_gamma * 0.5f / 3.0f;
   vp.half_delta_over3 = ctx->prm.tv_delta * 0.5f / 3.0f;
-  VarRefPlanes pl = ctx->planes;
-  pl.plane = (size_t)L->pitch * L->h;
-  if (!sor_band_plan(L->w, L->h, ctx->sor_rt, ctx->sor_single_max, ctx->sor_max_cluster, ctx->nop, ctx->prm.tv_solverit, &pl))
-    return fail(ctx, OFDIS_ERR_UNSUPPORTED, "varref_refine: no SOR band fits one CTA");
-  pl.rec_stride = (size_t)pl.nb * pl.ndiag * pl.hpad * pl.lpitch;
-  if (pl.rec_stride > ctx->rec_f4 || (pl.chain && pl.nb > ctx->chain_nb))
-    return fail(ctx, OFDIS_ERR_UNSUPPORTED, "varref_refine: the SOR plan exceeds the refinement workspace");
-  pl.lane = 0;
   const int nlaunch = (f1 - f0) * ctx->dirs;  // frames per launch
-  L->pdl = (ctx->pdl == 1 || (ctx->pdl == 2 && nlaunch <= SOR_LANE_AUTO_FRAMES)) ? 1 : 0;
-  if ((ctx->sor_lane == 1 || (ctx->sor_lane == 2 && nlaunch <= SOR_LANE_AUTO_FRAMES && sor_lane_preferred(L->h, ctx->prm.tv_solverit))) &&
-      !pl.fast && sor_lane_fits(L->h, 1)) {  // lane-skewed layout, bands of 32 rows
-    pl.lane = 1;
-    pl.nb = (L->h + 31) / 32;
-    pl.ndiag = lane_ndiag(L->w);
-    pl.rec_stride = lane_frame_f4(L->w, L->h);
-  }
-  pl.frec_stride = pl.plane * 8;   // fast mode: natural layout at this level's plane size
-  pl.fdu_stride = pl.plane * 4;
+  SorPlan plan;
+  if (!sor_plan(*L, ctx->prm.tv_solverit, ctx->sor, nlaunch, ctx->planes, &plan))
+    return fail(ctx, OFDIS_ERR_UNSUPPORTED, "varref_refine: no SOR band fits one CTA");
+  if (plan.pl.rec_stride > ctx->rec_f4 || plan.chain_nb > ctx->chain_nb)
+    return fail(ctx, OFDIS_ERR_UNSUPPORTED, "varref_refine: the SOR plan exceeds the refinement workspace");
+  L->pdl = pdl_for(ctx, nlaunch);
   // usefbcon: both directions are refined except on the last level (oflow.cpp:285-294)
   const int D = ctx->dirs;
   const bool fwd_only = (D == 2 && level == ctx->prm.sc_l);
-  const int n = fwd_only ? launch_varref(stepped(*L, 2), pl, vp, f0 * 2, f0 * 2 + (f1 - f0), ctx->stream, ctx->prof, ctx->d_chain, ctx->d_div_fb)
-                         : launch_varref(*L, pl, vp, f0 * D, f1 * D, ctx->stream, ctx->prof, ctx->d_chain, ctx->d_div_fb);
+  const int n = fwd_only ? launch_varref(stepped(*L, 2), plan, vp, f0 * 2, f0 * 2 + (f1 - f0), ctx->stream, ctx->prof, ctx->d_chain, ctx->d_div_fb)
+                         : launch_varref(*L, plan, vp, f0 * D, f1 * D, ctx->stream, ctx->prof, ctx->d_chain, ctx->d_div_fb);
   if (n < 0) return fail(ctx, OFDIS_ERR_CUDA, "varref kernels launch", cudaGetLastError());
   ctx->launches += n;
   ctx->last_vr_level = level;
-  ctx->last_vr_lane = pl.lane;
+  ctx->last_sor = plan;
   ctx->last_vr_fcur = vp.n_inner & 1;
   ctx->last_vr_f0 = f0;
   ctx->last_vr_fstep = fwd_only ? 1 : D;  // workspace slots per user frame
@@ -752,7 +738,7 @@ int ofdis_set_option(ofdis_ctx* ctx, const char* name, int value) {
   if (!ctx || !name) return OFDIS_ERR_ARG;
   if (!strcmp(name, "sor_single_max")) {
     if (value != 32 && value != 64 && value != 128) return fail(ctx, OFDIS_ERR_ARG, "sor_single_max: 32, 64 or 128");
-    ctx->sor_single_max = value;
+    ctx->sor.single_max = value;
   } else if (!strcmp(name, "sor_max_cluster")) {  // at most this many bands per cluster; levels with more are chained
     if (value != 1 && value != 2 && value != 4 && value != 8 && value != 16) return fail(ctx, OFDIS_ERR_ARG, "sor_max_cluster: 1, 2, 4, 8 or 16");
     if (value > ctx->sor_dev_cluster) return fail(ctx, OFDIS_ERR_UNSUPPORTED, "sor_max_cluster: the device does not grant clusters of 16 CTAs");
@@ -766,17 +752,20 @@ int ofdis_set_option(ofdis_ctx* ctx, const char* name, int value) {
           return fail(ctx, OFDIS_ERR_NOMEM, "sor_max_cluster: refinement workspace");
       }
     }
-    ctx->sor_max_cluster = value;
+    ctx->sor.max_cluster = value;
   } else if (!strcmp(name, "sor_lane")) {
     if (value < 0 || value > 2) return fail(ctx, OFDIS_ERR_ARG, "sor_lane: 0, 1 or 2");
-    ctx->sor_lane = value;
+    ctx->sor.lane = value;
   } else if (!strcmp(name, "pdl")) {
     if (value < 0 || value > 2) return fail(ctx, OFDIS_ERR_ARG, "pdl: 0, 1 or 2");
     ctx->pdl = value;
   } else if (!strcmp(name, "sor_fast")) {
     if (value != 0 && value != 1) return fail(ctx, OFDIS_ERR_ARG, "sor_fast: 0 or 1");
     if (!ctx->d_planes) return fail(ctx, OFDIS_ERR_ARG, "sor_fast: context created with usetvref=0");
-    if (value && rb_smem_limit_exceeded(ctx->nop, ctx->prm.tv_solverit))
+    SorOptions o = ctx->sor;
+    o.fast = 1;
+    SorPlan p;
+    if (value && !sor_plan(ctx->lev[0], ctx->prm.tv_solverit, o, 1, ctx->planes, &p))
       return fail(ctx, OFDIS_ERR_UNSUPPORTED, "sor_fast: too many sweeps for the tile's halo");
     if (value && !ctx->d_fast) {  // records 8 floats per pixel + 2 x 2 planes of (du,dv), finest level x frames
       const size_t plane = ctx->planes.plane;
@@ -787,10 +776,10 @@ int ofdis_set_option(ofdis_ctx* ctx, const char* name, int value) {
       ctx->planes.frec = ctx->d_fast;
       ctx->planes.fdu = ctx->d_fast + plane * 8 * ctx->cap;
     }
-    ctx->planes.fast = value;
+    ctx->sor.fast = value;
   } else if (!strcmp(name, "sor_rows_per_thread")) {
     if (value != 1 && value != 2 && value != 4) return fail(ctx, OFDIS_ERR_ARG, "sor_rows_per_thread: 1, 2 or 4");
-    ctx->sor_rt = value;
+    ctx->sor.rt = value;
   } else {
     return fail(ctx, OFDIS_ERR_ARG, "set_option: unknown option");
   }
@@ -909,52 +898,33 @@ long ofdis_debug_get(ofdis_ctx* ctx, const char* name, int frame, float* dst, si
     }
   if (!strcmp(name, "mask")) { src = ctx->planes.mask + (size_t)fr * plane; n = plane; }
   if (!strcmp(name, "dudv") || !strcmp(name, "rec")) {
-    // stored skewed (see VarRefPlanes); returned in natural (h, pitch, per-pixel) order
+    // stored in the layout of the last refinement's plan (see VarRefPlanes); returned in natural (h, pitch,
+    // per-pixel) order
     const bool is_rec = name[0] == 'r';
-    if (ctx->planes.fast) {  // natural layout: records 8 floats per pixel, (du,dv) two planes of the current buffer
-      const int per_f = is_rec ? (L->nop == 2 ? 8 : 5) : 2;
-      if (plane * per_f > max_floats) return OFDIS_ERR_ARG;
+    const VarRefPlanes& sp = ctx->last_sor.pl;  // its layout; the buffers are the context's current ones
+    const int per = is_rec ? sp.nq : 2;  // floats per pixel
+    if (plane * per > max_floats) return OFDIS_ERR_ARG;
+    if (sp.fast) {  // natural layout: records 8 floats per pixel, (du,dv) two planes of the current buffer
       std::vector<float> raw(is_rec ? plane * 8 : plane * 2);
-      const float* src_f = is_rec ? ctx->planes.frec + (size_t)fr * plane * 8
-                                  : ctx->planes.fdu + (size_t)fr * plane * 4 + (size_t)ctx->last_vr_fcur * 2 * plane;
+      const float* src_f = is_rec ? ctx->planes.frec + (size_t)fr * sp.frec_stride
+                                  : ctx->planes.fdu + (size_t)fr * sp.fdu_stride + (size_t)ctx->last_vr_fcur * 2 * plane;
       if (cudaMemcpyAsync(raw.data(), src_f, sizeof(float) * raw.size(), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
       if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
       for (size_t o = 0; o < plane; ++o)
-        for (int e = 0; e < per_f; ++e) dst[o * per_f + e] = is_rec ? raw[o * 8 + e] : raw[(size_t)e * plane + o];
-      return (long)(plane * per_f);
+        for (int e = 0; e < per; ++e) dst[o * per + e] = is_rec ? raw[o * 8 + e] : raw[(size_t)e * plane + o];
+      return (long)(plane * per);
     }
-    if (ctx->last_vr_lane) {  // lane-skewed layout (VarRefPlanes, lane mode)
-      VarRefPlanes lp{};
-      lp.nb = (L->h + 31) / 32;
-      lp.ndiag = lane_ndiag(L->w);
-      const int per_l = is_rec ? (L->nop == 2 ? 8 : 5) : 2;
-      const size_t stride_l = lane_frame_f4(L->w, L->h);
-      if (plane * per_l > max_floats) return OFDIS_ERR_ARG;
-      std::vector<float> raw(stride_l * 4);
-      if (cudaMemcpyAsync(raw.data(), ctx->planes.rec + (size_t)fr * stride_l, sizeof(float) * raw.size(), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
-      if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
-      for (int j = 0; j < L->h; ++j)
-        for (int i = 0; i < L->w; ++i)
-          for (int e = 0; e < per_l; ++e)
-            dst[((size_t)j * L->pitch + i) * per_l + e] =
-                is_rec ? raw[lane_rec_f4(lp, i, j, e >> 2) * 4 + (e & 3)] : raw[lane_dudv_f(lp, i, j) + e];
-      return (long)(plane * per_l);
-    }
-    VarRefPlanes bp{};
-    if (!sor_band_plan(L->w, L->h, ctx->sor_rt, ctx->sor_single_max, ctx->sor_max_cluster, ctx->nop, ctx->prm.tv_solverit, &bp)) return OFDIS_ERR_UNSUPPORTED;
-    const int per = is_rec ? bp.nq : 2;                              // floats per pixel
-    const size_t stride = (size_t)bp.nb * bp.ndiag * bp.hpad * bp.lpitch;  // float4 per frame
-    if (plane * per > max_floats) return OFDIS_ERR_ARG;
-    std::vector<float> raw(stride * 4);
-    const float4* base = ctx->planes.rec + (size_t)fr * stride;
-    if (cudaMemcpyAsync(raw.data(), base, sizeof(float) * raw.size(), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
+    std::vector<float> raw(sp.rec_stride * 4);
+    if (cudaMemcpyAsync(raw.data(), ctx->planes.rec + (size_t)fr * sp.rec_stride, sizeof(float) * raw.size(), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
     if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) return OFDIS_ERR_CUDA;
     for (int j = 0; j < L->h; ++j)
       for (int i = 0; i < L->w; ++i)
         for (int e = 0; e < per; ++e) {
-          // chunk e of the block's lane row holds field e of its 4 pixels; (du,dv) are chunks nq, nq+1
-          const size_t f4 = band_f4(bp, i >> 2, j, is_rec ? e : bp.nq + e);
-          dst[((size_t)j * L->pitch + i) * per + e] = raw[f4 * 4 + (i & 3)];
+          // lane layout: a record is two float4 (lane_rec_f4), (du,dv) consecutive floats (lane_dudv_f); band lane
+          // rows: chunk e of the block's lane row holds field e of its 4 pixels, (du,dv) are chunks nq, nq+1
+          const size_t k = sp.lane ? (is_rec ? lane_rec_f4(sp, i, j, e >> 2) * 4 + (e & 3) : lane_dudv_f(sp, i, j) + e)
+                                   : band_f4(sp, i >> 2, j, is_rec ? e : sp.nq + e) * 4 + (i & 3);
+          dst[((size_t)j * L->pitch + i) * per + e] = raw[k];
         }
     return (long)(plane * per);
   }

@@ -15,7 +15,10 @@
 // -fmad=false so nothing is contracted (bit-exactness, DESIGN.md section 4).
 #include "ofdis_internal.cuh"
 
+#include <map>
+#include <mutex>
 #include <type_traits>
+#include <utility>
 
 namespace ofdis {
 
@@ -462,42 +465,125 @@ __global__ void __launch_bounds__(256) flow_update_kernel(LevelGeom g, VarRefPla
 
 }  // namespace
 
-// Largest number of sweeps one launch can keep in flight: K*hpad compute threads + the producer
-// warp within the kernel's launch bound, stage ring + board within the 227 KB of an SM.
-static int sor_sweeps_per_launch(int nop, int hpad, int rt, int K) {
-  int kl = K < 1 ? 1 : K;
-  while (kl > 1 && (kl * hpad + 32 > sor_max_threads(hpad) || sor_smem_bytes(nop, hpad, rt, kl, hpad) > 227 * 1024)) --kl;
-  return kl;
+// Opt-in of `smem` bytes of dynamic shared memory for `kern` on the current device (and, with `nonportable`, of
+// clusters of more than 8 CTAs).  The attributes belong to the kernel, so the cache is keyed by device and kernel:
+// it only ever raises a kernel's setting, whichever of the launches that share the kernel (gray and RGB levels,
+// sor_max_cluster_size) comes first.  A cache per launcher once let an RGB level that needed less shared memory lower
+// the setting behind a gray level's cache, and the gray level's next larger launch failed.
+template <typename Kern>
+static cudaError_t smem_optin(Kern* kern, size_t smem, bool nonportable) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, std::pair<size_t, bool>> done;  // (device, kernel) -> (smem, nonportable)
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  std::lock_guard<std::mutex> lock(mu);
+  std::pair<size_t, bool>& d = done[{dev, (const void*)kern}];
+  if (d.first < smem) {
+    if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
+    d.first = smem;
+  }
+  if (nonportable && !d.second) {
+    if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1)) != cudaSuccess) return e;
+    d.second = true;
+  }
+  return cudaSuccess;
+}
+
+// Can a sor_wave_kernel CTA of `hpad` lanes keep K sweeps in flight: K * hpad compute threads + the producer warp
+// within the kernel's launch bound, stage ring + board within the shared memory of an SM?
+constexpr bool sor_wave_fits(int nop, int hpad, int rt, int K) {
+  return K * hpad + 32 <= sor_max_threads(hpad) && sor_smem_bytes(nop, hpad, rt, K, hpad) <= SMEM_OPTIN_MAX;
+}
+// band of a chain plan: the largest that fits one sweep; the only chain instantiation per (nop, rt)
+constexpr int sor_chain_hpad(int nop, int rt) {
+  int p = 256;
+  while (p > 32 && !sor_wave_fits(nop, p, rt, 1)) p /= 2;
+  return p;
+}
+
+bool sor_plan(const LevelGeom& L, int K, const SorOptions& o, int frames, const VarRefPlanes& buffers, SorPlan* plan) {
+  SorPlan p{};
+  VarRefPlanes& pl = p.pl;
+  pl = buffers;
+  const int nop = L.nop, rt = o.rt, k1 = K < 1 ? 1 : K;
+  const int lanes = (L.h + rt - 1) / rt;  // lanes the whole level needs
+  int hpad = 0;
+  // all K sweeps in flight if some band size allows it, else as many as the band found for one sweep holds
+  for (int kk = k1; !hpad; kk = 1) {
+    for (int q = 32; q <= 128 && !hpad; q *= 2)
+      if (lanes <= q && lanes <= o.single_max && sor_wave_fits(nop, q, rt, kk)) hpad = q;
+    for (int q = 32; q <= 256 && !hpad; q *= 2)
+      if (lanes > q && (lanes + q - 1) / q <= o.max_cluster && sor_wave_fits(nop, q, rt, kk)) hpad = q;
+    if (kk == 1) break;
+  }
+  pl.chain = !hpad;
+  if (pl.chain) hpad = sor_chain_hpad(nop, rt);
+  if (!sor_wave_fits(nop, hpad, rt, 1)) return false;
+  pl.hpad = hpad;
+  pl.rt = rt;
+  pl.rtshift = rt == 1 ? 0 : (rt == 2 ? 1 : 2);
+  pl.hbshift = (hpad == 32 ? 5 : (hpad == 64 ? 6 : (hpad == 128 ? 7 : 8))) + pl.rtshift;
+  pl.nb = (lanes + hpad - 1) / hpad;
+  pl.ndiag = (L.w + 3) / 4 + hpad + 2;
+  pl.nq = nop == 2 ? 8 : 5;
+  pl.lpitch = sor_lane_pitch(nop, rt);
+  pl.rec_stride = (size_t)pl.nb * pl.ndiag * pl.hpad * pl.lpitch;
+  pl.lane = 0;
+  pl.fast = o.fast;
+  pl.plane = (size_t)L.pitch * L.h;
+  pl.frec_stride = pl.plane * 8;  // fast mode: natural layout at this level's plane size
+  pl.fdu_stride = pl.plane * 4;
+  p.kind = pl.chain ? SOR_WAVE_CHAIN : (pl.nb > 1 ? SOR_WAVE_CLUSTER : SOR_WAVE_SINGLE);
+  p.sweeps = pl.chain ? 1 : k1;  // a chain runs one sweep per launch
+  while (p.sweeps > 1 && !sor_wave_fits(nop, hpad, rt, p.sweeps)) --p.sweeps;
+  p.ml = sor_stage_lanes(hpad, rt, L.w, L.h, p.kind != SOR_WAVE_SINGLE);
+  // sor_lane_kernel, bands of 32 rows.  By default where it beats the block wavefront (tools/lane_ab.py): one or two
+  // bands with all sweeps in one launch.  Every further band adds 33 steps of start-up skew, which makes taller
+  // levels slower with it.
+  const int nb32 = (L.h + 31) / 32, kl32 = sl_sweeps_per_launch(nb32, K);
+  if (!o.fast && kl32 >= 1 &&
+      (o.lane == 1 || (o.lane == 2 && frames <= SOR_LANE_AUTO_FRAMES && nb32 <= 2 && kl32 >= k1))) {
+    p.kind = SOR_LANE;
+    pl.lane = 1;
+    pl.nb = nb32;
+    pl.ndiag = lane_ndiag(L.w);
+    pl.rec_stride = lane_frame_f4(L.w, L.h);
+    p.sweeps = kl32;
+  }
+  if (o.fast) {  // sor_redblack_kernel: all K sweeps in one launch
+    p.kind = SOR_REDBLACK;
+    p.sweeps = k1;
+  }
+  auto smem = [&](int k) {
+    return p.kind == SOR_REDBLACK ? rb_smem_bytes(nop, k)
+                                  : (p.kind == SOR_LANE ? sl_smem_bytes(nb32, k) : sor_smem_bytes(nop, hpad, rt, k, p.ml));
+  };
+  p.smem = smem(p.sweeps);
+  p.tail_smem = K % p.sweeps > 0 ? smem(K % p.sweeps) : p.smem;
+  p.chain_nb = p.kind == SOR_WAVE_CHAIN ? pl.nb : 0;
+  if (p.kind == SOR_REDBLACK && (K < 1 || p.smem > SMEM_OPTIN_MAX)) return false;  // the tile's halo grows with K
+  *plan = p;
+  return true;
 }
 
 template <int NOP, int HPAD, int RT, int BM>
-static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
-                                cudaStream_t st, int* sync, unsigned long long* div_fb) {
+static cudaError_t launch_sor_t(const LevelGeom& g, const SorPlan& p, const VarRefParams& vp, int nf, int kk,
+                                size_t smem, cudaStream_t st, int* sync, unsigned long long* div_fb) {
   constexpr bool CL = (BM == SOR_CLUSTER);
   auto kern = sor_wave_kernel<NOP, HPAD, RT, BM>;
-  const int ml = sor_stage_lanes(HPAD, RT, g.w, g.h, BM != SOR_SINGLE);
-  const size_t smem = sor_smem_bytes(NOP, HPAD, RT, kl, ml);
-  if (smem > 227 * 1024) return cudaErrorInvalidConfiguration;
-  // opt-in shared memory (and cluster size) once per device and instantiation
-  static size_t smem_set[64] = {0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && smem_set[dev] < smem) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess && CL) e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    if (e != cudaSuccess) return e;
-    smem_set[dev] = smem;
-  }
+  const cudaError_t e = smem_optin(kern, smem, CL);
+  if (e != cudaSuccess) return e;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(nf * (BM != SOR_SINGLE ? pl.nb : 1)));
-  cfg.blockDim = dim3((unsigned)(kl * HPAD + 32));
+  cfg.gridDim = dim3((unsigned)(nf * (BM != SOR_SINGLE ? p.pl.nb : 1)));
+  cfg.blockDim = dim3((unsigned)(kk * HPAD + 32));
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[2];
   int na = 0;
   if (CL) {
     attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = (unsigned)pl.nb;
+    attr[na].val.clusterDim.x = (unsigned)p.pl.nb;
     attr[na].val.clusterDim.y = 1;
     attr[na].val.clusterDim.z = 1;
     ++na;
@@ -509,67 +595,41 @@ static cudaError_t launch_sor_t(const LevelGeom& g, const VarRefPlanes& pl, cons
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, kern, g, pl, vp, kl, ml, sync, div_fb);
-}
-
-// band of a chain plan: the largest that fits one sweep (sor_band_plan); the only chain instantiation per (NOP, RT)
-template <int NOP, int RT>
-constexpr int sor_chain_hpad() {
-  int p = 256;
-  while (p > 32 && !(p + 32 <= sor_max_threads(p) && sor_smem_bytes(NOP, p, RT, 1, p) <= 227 * 1024)) p /= 2;
-  return p;
+  return cudaLaunchKernelEx(&cfg, kern, g, p.pl, vp, kk, p.ml, sync, div_fb);
 }
 
 template <int NOP, int RT>
-static cudaError_t launch_sor_rt(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
-                                 cudaStream_t st, int* sync, unsigned long long* div_fb) {
-  if (pl.chain) {
-    constexpr int HC = sor_chain_hpad<NOP, RT>();
-    if (pl.hpad != HC || kl != 1 || !sync) return cudaErrorInvalidValue;
-    return launch_sor_t<NOP, HC, RT, SOR_CHAIN>(g, pl, vp, nf, kl, st, sync, div_fb);
+static cudaError_t launch_sor_rt(const LevelGeom& g, const SorPlan& p, const VarRefParams& vp, int nf, int kk,
+                                 size_t smem, cudaStream_t st, int* sync, unsigned long long* div_fb) {
+  if (p.kind == SOR_WAVE_CHAIN) {
+    constexpr int HC = sor_chain_hpad(NOP, RT);
+    if (p.pl.hpad != HC || kk != 1 || !sync) return cudaErrorInvalidValue;
+    return launch_sor_t<NOP, HC, RT, SOR_CHAIN>(g, p, vp, nf, kk, smem, st, sync, div_fb);
   }
-  const bool cl = pl.nb > 1;
+  const bool cl = p.kind == SOR_WAVE_CLUSTER;
   constexpr int C1 = SOR_CLUSTER, S1 = SOR_SINGLE;
-  switch (pl.hpad) {
-    case 32: return cl ? launch_sor_t<NOP, 32, RT, C1>(g, pl, vp, nf, kl, st, sync, div_fb) : launch_sor_t<NOP, 32, RT, S1>(g, pl, vp, nf, kl, st, sync, div_fb);
-    case 64: return cl ? launch_sor_t<NOP, 64, RT, C1>(g, pl, vp, nf, kl, st, sync, div_fb) : launch_sor_t<NOP, 64, RT, S1>(g, pl, vp, nf, kl, st, sync, div_fb);
-    case 128: return cl ? launch_sor_t<NOP, 128, RT, C1>(g, pl, vp, nf, kl, st, sync, div_fb) : launch_sor_t<NOP, 128, RT, S1>(g, pl, vp, nf, kl, st, sync, div_fb);
-    case 256: return cl ? launch_sor_t<NOP, 256, RT, C1>(g, pl, vp, nf, kl, st, sync, div_fb) : launch_sor_t<NOP, 256, RT, S1>(g, pl, vp, nf, kl, st, sync, div_fb);
+  switch (p.pl.hpad) {
+    case 32: return cl ? launch_sor_t<NOP, 32, RT, C1>(g, p, vp, nf, kk, smem, st, sync, div_fb) : launch_sor_t<NOP, 32, RT, S1>(g, p, vp, nf, kk, smem, st, sync, div_fb);
+    case 64: return cl ? launch_sor_t<NOP, 64, RT, C1>(g, p, vp, nf, kk, smem, st, sync, div_fb) : launch_sor_t<NOP, 64, RT, S1>(g, p, vp, nf, kk, smem, st, sync, div_fb);
+    case 128: return cl ? launch_sor_t<NOP, 128, RT, C1>(g, p, vp, nf, kk, smem, st, sync, div_fb) : launch_sor_t<NOP, 128, RT, S1>(g, p, vp, nf, kk, smem, st, sync, div_fb);
+    case 256: return cl ? launch_sor_t<NOP, 256, RT, C1>(g, p, vp, nf, kk, smem, st, sync, div_fb) : launch_sor_t<NOP, 256, RT, S1>(g, p, vp, nf, kk, smem, st, sync, div_fb);
   }
   return cudaErrorInvalidValue;
 }
 
 template <int NOP>
-static cudaError_t launch_sor(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int nf, int kl,
+static cudaError_t launch_sor(const LevelGeom& g, const SorPlan& p, const VarRefParams& vp, int nf, int kk, size_t smem,
                               cudaStream_t st, int* sync, unsigned long long* div_fb) {
-  if (pl.rt == 1) return launch_sor_rt<NOP, 1>(g, pl, vp, nf, kl, st, sync, div_fb);
-  if (pl.rt == 2) return launch_sor_rt<NOP, 2>(g, pl, vp, nf, kl, st, sync, div_fb);
-  if (pl.rt == 4) return launch_sor_rt<NOP, 4>(g, pl, vp, nf, kl, st, sync, div_fb);
+  if (p.pl.rt == 1) return launch_sor_rt<NOP, 1>(g, p, vp, nf, kk, smem, st, sync, div_fb);
+  if (p.pl.rt == 2) return launch_sor_rt<NOP, 2>(g, p, vp, nf, kk, smem, st, sync, div_fb);
+  if (p.pl.rt == 4) return launch_sor_rt<NOP, 4>(g, p, vp, nf, kk, smem, st, sync, div_fb);
   return cudaErrorInvalidValue;
 }
 
-// Opt-in dynamic shared memory of a kernel that the launchers of gray and RGB levels share (sor_lane_kernel<NOP>,
-// sor_redblack_kernel<NOP>): the attribute belongs to the kernel, so its cache must too.  With one cache per
-// launch_varref_t<C, NOP> an RGB level that needed less shared memory lowered the attribute behind the gray
-// levels' cache, and their next larger launch failed (tests/test_sor_division_gpu.py after the RGB stereo tests).
-template <typename Tag, typename Kern>
-static bool smem_optin(Kern kern, size_t smem) {
-  static size_t smem_set[64] = {0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && smem_set[dev] < smem) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return false;
-    smem_set[dev] = smem;
-  }
-  return true;
-}
-template <int NOP> struct LaneKernTag {};
-template <int NOP> struct RbKernTag {};
-
 template <int C, int NOP>
-static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const VarRefParams& vp, int f0, int f1,
+static int launch_varref_t(const LevelGeom& g, const SorPlan& plan, const VarRefParams& vp, int f0, int f1,
                            cudaStream_t st, Profiler* prof, int* chain_sync, unsigned long long* div_fb) {
-  VarRefPlanes pl = pl_in;  // fast mode toggles the (du,dv) ping-pong buffer
+  VarRefPlanes pl = plan.pl;  // fast mode toggles the (du,dv) ping-pong buffer
   const bool pdl = g.pdl != 0 && prof == nullptr;  // the profiler's events between launches would serialise them anyway
   pl.fcur = 0;
   int launches = 0;
@@ -588,11 +648,9 @@ static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const 
     launch_k(pdl, deriv2_kernel<C>, gridc, block, 0, st, g, pl);
   }
   launches += 3;
-  // SOR: band plan of the level (pl.hpad rows per band, pl.nb bands == CTAs of a cluster or of a chain) and as
-  // many sweeps per launch as the CTA's thread and shared-memory budgets hold (sweeps are sequential,
-  // so K sweeps in ceil(K / kl) launches give the same result); a chain runs one sweep per launch
+  // SOR: the launches of the level's plan (sor_plan); the sweeps are sequential, so K sweeps in ceil(K / sweeps)
+  // launches give the same result
   const int K = vp.n_solver;
-  const int kl = pl.chain ? 1 : sor_sweeps_per_launch(NOP, pl.hpad, pl.rt, K);
   for (int it = 0; it < vp.n_inner; ++it) {
     {
       ProfScope scope(prof, KC_VR_ASSEMBLE);
@@ -607,35 +665,25 @@ static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const 
       else launch_asm(std::integral_constant<int, 0>{});
     }
     ++launches;
-    if (pl.fast) {  // opt-in red-black solver: all K sweeps in one launch, (du,dv) ping-pong
+    for (int s = 0; s < K; s += plan.sweeps) {
       ProfScope scope(prof, KC_VR_SOR);
-      const size_t smem = rb_smem_bytes(NOP, K);
-      if (K < 1 || smem > 227 * 1024) return -1;
-      if (!smem_optin<RbKernTag<NOP>>(sor_redblack_kernel<NOP>, smem)) return -1;
-      const dim3 grid_rb((g.w + RB_TILE - 1) / RB_TILE, (g.h + RB_TILE - 1) / RB_TILE, nf);
-      launch_k(pdl, sor_redblack_kernel<NOP>, grid_rb, dim3(256), smem, st, g, pl, vp);
-      pl.fcur ^= 1;
-      ++launches;
-      continue;
-    }
-    if (pl.lane) {  // pixel wavefront, warps synchronised through shared-memory flags (levels of few 32-row bands)
-      const int kll = sl_sweeps_per_launch(pl.nb, K);
-      if (kll < 1) return -1;
-      for (int s = 0; s < K; s += kll) {
-        ProfScope scope(prof, KC_VR_SOR);
-        const int kk = (K - s < kll) ? K - s : kll;
-        const size_t smem = sl_smem_bytes(pl.nb, kk);
-        if (!smem_optin<LaneKernTag<NOP>>(sor_lane_kernel<NOP>, smem)) return -1;
-        launch_k(pdl, sor_lane_kernel<NOP>, dim3(nf), dim3(pl.nb * kk * 32), smem, st, g, pl, vp, kk, div_fb);
-        ++launches;
+      const int kk = (K - s < plan.sweeps) ? K - s : plan.sweeps;
+      const size_t smem = kk == plan.sweeps ? plan.smem : plan.tail_smem;
+      cudaError_t e;
+      if (plan.kind == SOR_REDBLACK) {  // opt-in red-black solver, (du,dv) ping-pong
+        const dim3 grid_rb((g.w + RB_TILE - 1) / RB_TILE, (g.h + RB_TILE - 1) / RB_TILE, nf);
+        if ((e = smem_optin(sor_redblack_kernel<NOP>, smem, false)) == cudaSuccess)
+          e = launch_k(pdl, sor_redblack_kernel<NOP>, grid_rb, dim3(256), smem, st, g, pl, vp);
+      } else if (plan.kind == SOR_LANE) {  // pixel wavefront, warps synchronised through shared-memory flags
+        if ((e = smem_optin(sor_lane_kernel<NOP>, smem, false)) == cudaSuccess)
+          e = launch_k(pdl, sor_lane_kernel<NOP>, dim3(nf), dim3(pl.nb * kk * 32), smem, st, g, pl, vp, kk, div_fb);
+      } else {
+        e = launch_sor<NOP>(g, plan, vp, nf, kk, smem, st, chain_sync, div_fb);
       }
-      continue;
-    }
-    for (int s = 0; s < K; s += kl) {
-      ProfScope scope(prof, KC_VR_SOR);
-      if (launch_sor<NOP>(g, pl, vp, nf, (K - s < kl) ? K - s : kl, st, chain_sync, div_fb) != cudaSuccess) return -1;
+      if (e != cudaSuccess) return -1;
       ++launches;
     }
+    pl.fcur ^= pl.fast;
   }
   if (vp.n_inner > 0) {
     ProfScope scope(prof, KC_VR_SETUP);
@@ -643,17 +691,6 @@ static int launch_varref_t(const LevelGeom& g, const VarRefPlanes& pl_in, const 
     ++launches;
   }
   return cudaGetLastError() == cudaSuccess ? launches : -1;
-}
-
-bool sor_lane_fits(int h, int K) { return sl_sweeps_per_launch((h + 31) / 32, K) >= 1; }
-// Where the lane kernel beats the block wavefront (tools/lane_ab.py): one or two bands with all sweeps in one
-// launch.  Every further band adds 33 steps of start-up skew, which makes taller levels slower with it.
-bool sor_lane_preferred(int h, int K) { return (h + 31) / 32 <= 2 && sl_sweeps_per_launch((h + 31) / 32, K) >= (K < 1 ? 1 : K); }
-
-bool rb_smem_limit_exceeded(int nop, int K) { return K < 1 || rb_smem_bytes(nop, K) > 227 * 1024; }
-
-bool sor_fits(int nop, int hpad, int rt, int K) {
-  return K * hpad + 32 <= sor_max_threads(hpad) && sor_smem_bytes(nop, hpad, rt, K, hpad) <= 227 * 1024;
 }
 
 int sor_max_cluster_size() {
@@ -666,8 +703,7 @@ int sor_max_cluster_size() {
   int best = 8;
   auto kern = sor_wave_kernel<2, 128, 1, SOR_CLUSTER>;
   const size_t smem = sor_smem_bytes(2, 128, 1, 3, 128);  // 128-row bands, 3 sweeps in flight: the largest common configuration
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess &&
-      cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
+  if (smem_optin(kern, smem, true) == cudaSuccess) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(16);
     cfg.blockDim = dim3(3 * 128 + 32);
@@ -687,12 +723,12 @@ int sor_max_cluster_size() {
   return best;
 }
 
-int launch_varref(const LevelGeom& g, const VarRefPlanes& pl, const VarRefParams& vp, int f0, int f1,
+int launch_varref(const LevelGeom& g, const SorPlan& plan, const VarRefParams& vp, int f0, int f1,
                   cudaStream_t st, Profiler* prof, int* chain_sync, unsigned long long* div_fb) {
-  if (g.noc == 1 && g.nop == 2) return launch_varref_t<1, 2>(g, pl, vp, f0, f1, st, prof, chain_sync, div_fb);
-  if (g.noc == 3 && g.nop == 2) return launch_varref_t<3, 2>(g, pl, vp, f0, f1, st, prof, chain_sync, div_fb);
-  if (g.noc == 1 && g.nop == 1) return launch_varref_t<1, 1>(g, pl, vp, f0, f1, st, prof, chain_sync, div_fb);
-  if (g.noc == 3 && g.nop == 1) return launch_varref_t<3, 1>(g, pl, vp, f0, f1, st, prof, chain_sync, div_fb);
+  if (g.noc == 1 && g.nop == 2) return launch_varref_t<1, 2>(g, plan, vp, f0, f1, st, prof, chain_sync, div_fb);
+  if (g.noc == 3 && g.nop == 2) return launch_varref_t<3, 2>(g, plan, vp, f0, f1, st, prof, chain_sync, div_fb);
+  if (g.noc == 1 && g.nop == 1) return launch_varref_t<1, 1>(g, plan, vp, f0, f1, st, prof, chain_sync, div_fb);
+  if (g.noc == 3 && g.nop == 1) return launch_varref_t<3, 1>(g, plan, vp, f0, f1, st, prof, chain_sync, div_fb);
   return -1;
 }
 

@@ -394,6 +394,41 @@ def test_lane_sor_and_block_sor_vs_oracle(name, lane, api, oracle_port):
     ctx.close()
 
 
+@pytest.mark.parametrize("lane", [0, 1])
+@pytest.mark.parametrize("name", ["cfg2_1024x436_gray_op2", "stereo_op4_small"])
+def test_debug_get_reads_the_layout_of_the_last_refinement(name, lane, api, oracle_port):
+    """ofdis_debug_get("rec" / "dudv") decodes the planes in the layout the last refinement used, whatever SOR options
+    are set after it: a refinement at one row per thread with the block wavefront (sor_lane 0) or the lane layout
+    (sor_lane 1), read and checked against the oracle, then read again after sor_rows_per_thread 2, sor_single_max 32
+    (and sor_lane 0), which would give the next refinement another layout.  Every later read equals the first."""
+    h, w, ch, mk, amp, stereo = CASES[name]
+    prm = mk()
+    i0, i1, _ = synth.synthetic_pair(h, w, ch, seed=17, amp=amp, stereo=stereo)
+    pyr = preprocess.PairPyramids(i0, i1, prm.sc_f, prm.p_samp_s)
+    ctx = api.Context(prm, pyr.width, pyr.height, pyr.imgpadding, 1)
+    ctx.set_option("sor_lane", lane)
+    ctx.set_option("sor_rows_per_thread", 1)
+    ctx.upload_pyramids(0, pyr)
+    lv = prm.sc_l
+    hh, ww = pyr.level_shape(lv)
+    dense = (np.random.default_rng(6).standard_normal((hh, ww, prm.nop)) * 1.5).astype(np.float32)
+    if stereo:
+        dense = -np.abs(dense)
+    it = oracle_port.varref_stages(pyr, prm, lv, dense, n_iters=2)["iters"][1]
+    ctx.set_flow(0, lv, dense)
+    ctx.varref_refine(lv, 0, 1, n_inner=2)
+    rec, dudv = ctx.debug_get("rec", 0, lv), ctx.debug_get("dudv", 0, lv)
+    assert_bits(rec[..., 1 if prm.nop == 1 else 3], it["b1"], "rec.b1")
+    assert_bits(dudv[..., 0], it["du"], "du")
+    if prm.nop == 2:
+        assert_bits(dudv[..., 1], it["dv"], "dv")
+    for k, v in [("sor_rows_per_thread", 2), ("sor_single_max", 32)] + [("sor_lane", 0)] * lane:
+        ctx.set_option(k, v)
+        assert_bits(ctx.debug_get("rec", 0, lv), rec, "rec after %s %d" % (k, v))
+        assert_bits(ctx.debug_get("dudv", 0, lv), dudv, "dudv after %s %d" % (k, v))
+    ctx.close()
+
+
 def test_cluster_of_sixteen_bands_where_the_device_grants_it(api, oracle_port):
     """Non-portable cluster size 16: 1100-row level as 9 bands of 64 lanes x 2 rows (all sweeps in flight)."""
     prm = params.from_cli_numbers("1 0 6 6 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=1, nop=2)
