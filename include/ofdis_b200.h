@@ -139,6 +139,15 @@ int ofdis_get_level(ofdis_ctx* ctx, int frame, int level, int which, float* dst,
  *   defines the run's input exactly. */
 int ofdis_upload_frames_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char* frames, int width_org, int height_org,
                            int memkind);
+/* Consecutive frames (extension): `frames` = [f1-f0+1][height_org][width_org][noc] 8-bit frames; pair slot
+ * f0+i gets (frames[i], frames[i+1]).  Same preprocessing as ofdis_upload_frames_u8 (divisibility padding,
+ * box-mean levels, Sobel/8, border paddings; usefbcon's swapped frames), each frame uploaded and each of its
+ * levels built once.  The following ofdis_run is bitwise what ofdis_upload_frames_u8 of the pairs gives.
+ * Same arguments and status codes as ofdis_upload_frames_u8; slots outside [f0, f1) are not touched.  The
+ * context keeps no frame between calls: to stream a clip in chunks, pass each chunk's last frame again as the
+ * next chunk's first. */
+int ofdis_upload_sequence_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char* frames, int width_org,
+                             int height_org, int memkind);
 size_t ofdis_finest_level_frame_floats(const ofdis_ctx* ctx);
 int ofdis_upload_finest_level(ofdis_ctx* ctx, int f0, int f1, const float* packed, int memkind);
 

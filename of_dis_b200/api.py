@@ -31,7 +31,7 @@ EXPORTS = [
     "ofdis_set_camlr", "ofdis_set_dp_thresh_sq", "ofdis_packed_images_frame_floats", "ofdis_upload_packed_images",
     "ofdis_upload_frames_u8", "ofdis_finest_level_frame_floats", "ofdis_upload_finest_level", "ofdis_get_flow_fullres",
     "ofdis_get_level", "ofdis_upload_level_fb", "ofdis_set_option", "ofdis_profile_levels", "ofdis_set_direction",
-    "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks",
+    "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8",
 ]
 
 
@@ -73,6 +73,8 @@ def lib():
         L.ofdis_upload_finest_level.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
         L.ofdis_upload_frames_u8.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_int]
+        L.ofdis_upload_sequence_u8.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                               ctypes.c_int, ctypes.c_int]
         L.ofdis_get_flow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_int]
         L.ofdis_upload_packed.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
@@ -208,6 +210,11 @@ class Context:
     def upload_frames_u8(self, f0, f1, frames, width_org, height_org, memkind=MEM_HOST):
         """[frame][2][height_org][width_org][noc] 8-bit pairs; whole pyramid built on the device."""
         self._ck(lib().ofdis_upload_frames_u8(self._h, f0, f1, _ptr(frames), width_org, height_org, memkind))
+
+    def upload_sequence_u8(self, f0, f1, frames, width_org, height_org, memkind=MEM_HOST):
+        """[f1-f0+1][height_org][width_org][noc] 8-bit consecutive frames; pair f0+i = (frames[i], frames[i+1]).
+        Bitwise the pyramids upload_frames_u8 builds from the duplicated pairs, each frame uploaded once."""
+        self._ck(lib().ofdis_upload_sequence_u8(self._h, f0, f1, _ptr(frames), width_org, height_org, memkind))
 
     def get_flow_fullres(self, f0, f1, dst, width_org, height_org, memkind=MEM_HOST):
         """Flow x 2^sc_l, upsampled to the original frame size and cropped (run_dense.cpp:407-414)."""

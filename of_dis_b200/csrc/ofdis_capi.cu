@@ -529,13 +529,14 @@ int ofdis_upload_packed_images(ofdis_ctx* ctx, int f0, int f1, const float* pack
   return finish_gradients(ctx, f0, f1);
 }
 
-// Coarser levels by 2x2 box means (forward frames), then finish_gradients.
-static int finish_pyramid(ofdis_ctx* ctx, int f0, int f1) {
+// Coarser levels by 2x2 box means (forward frames), then finish_gradients.  seq: the pairs hold consecutive
+// frames (ofdis_upload_sequence_u8), each frame's levels are built once.
+static int finish_pyramid(ofdis_ctx* ctx, int f0, int f1, bool seq = false) {
   NvtxRange nvtx("pyramid", -1);
   const int D = ctx->dirs, q0 = f0 * D, nq = f1 - f0;
   for (int sl = ctx->prm.sc_l + 1; sl <= ctx->prm.sc_f; ++sl) {
     const LevelGeom gs = stepped(ctx->lev[sl - 1 - ctx->prm.sc_l], D), gd = stepped(ctx->lev[sl - ctx->prm.sc_l], D);
-    if (launch_pyr_down(gs, gd, q0, q0 + nq, ctx->stream) < 0)
+    if ((seq ? launch_pyr_down_seq(gs, gd, q0, nq, ctx->stream) : launch_pyr_down(gs, gd, q0, q0 + nq, ctx->stream)) < 0)
       return fail(ctx, OFDIS_ERR_CUDA, "pyr_down_kernel launch", cudaGetLastError());
     ctx->launches += 1;
   }
@@ -588,6 +589,34 @@ int ofdis_upload_frames_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char* 
     return fail(ctx, OFDIS_ERR_CUDA, "pyr_from_u8_kernel launch", cudaGetLastError());
   ctx->launches += 1;
   return finish_pyramid(ctx, f0, f1);
+}
+
+int ofdis_upload_sequence_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char* frames, int width_org, int height_org,
+                             int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !frames) return fail(ctx, OFDIS_ERR_ARG, "upload_sequence_u8: bad argument");
+  if (ctx->prm.sc_l > 8) return fail(ctx, OFDIS_ERR_UNSUPPORTED, "upload_sequence_u8: box sums are exact in float32 up to level 8");
+  PyrSourceU8 src;
+  int rc = org_padding(ctx, width_org, height_org, &src.pad_left, &src.pad_top);
+  if (rc) return rc;
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0;
+  src.w_org = width_org;
+  src.h_org = height_org;
+  src.image_bytes = (size_t)width_org * height_org * ctx->prm.noc;
+  src.frames = frames;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    // the staging size of ofdis_upload_frames_u8 (2 x max_frames images; n + 1 <= max_frames + 1 frames fit), so
+    // that alternating the two uploads never reallocates
+    rc = ensure_stage(ctx, src.image_bytes * 2 * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(ctx->d_stage, frames, src.image_bytes * (size_t)(n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    src.frames = static_cast<const unsigned char*>(ctx->d_stage);
+  }
+  if (launch_pyr_from_u8_seq(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, n, src, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "pyr_from_u8_kernel launch", cudaGetLastError());
+  ctx->launches += 1;
+  return finish_pyramid(ctx, f0, f1, true);
 }
 
 size_t ofdis_finest_level_frame_floats(const ofdis_ctx* ctx) {

@@ -15,27 +15,42 @@ namespace {
 // is exact in int32 and (for l <= 8) in float32, so it equals l successive cv::resize(0.5) steps.
 // The divisibility padding (replicate, floor(pad/2) left/top) and the per-level border padding
 // (replicate, g.pad) are folded into the index clamps.  One thread per padded destination pixel.
-__global__ void __launch_bounds__(256) pyr_from_u8_kernel(LevelGeom g, int f0, PyrSourceU8 s) {
+// SEQ = false: s.frames = [pair][2][..], grid.z = 2 x pairs (pair, side).  SEQ = true: s.frames = [n + 1][..]
+// consecutive frames, grid.z = n + 1; frame t is computed once and stored as I0 of pair t (t < n) and as I1 of
+// pair t - 1 (t >= 1).
+template <bool SEQ>
+__global__ void __launch_bounds__(256) pyr_from_u8_kernel(LevelGeom g, int f0, PyrSourceU8 s, int n) {
   pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
   const int xp = blockIdx.x * blockDim.x + threadIdx.x, yp = blockIdx.y * blockDim.y + threadIdx.y;
   if (xp >= g.tmp_w || yp >= g.tmp_h) return;
-  const int fr = blockIdx.z >> 1, k = blockIdx.z & 1;  // k: 0 = I0, 1 = I1
-  const int C = g.noc, sh = g.level, n = 1 << sh;
-  const unsigned char* src = s.frames + ((size_t)fr * 2 + k) * s.image_bytes;
-  const int arr = k ? 3 : 0;
-  float* dst = const_cast<float*>(g.img[arr]) + (size_t)frame_of(g, f0, fr) * g.img_fs[arr] + ((size_t)yp * g.tmp_w + xp) * C;
+  const int fr = SEQ ? (int)blockIdx.z : (int)(blockIdx.z >> 1), k = blockIdx.z & 1;  // pairs: k 0 = I0, 1 = I1
+  const int C = g.noc, sh = g.level, nb = 1 << sh;
+  const unsigned char* src = s.frames + (SEQ ? (size_t)fr : (size_t)fr * 2 + k) * s.image_bytes;
+  const size_t o = ((size_t)yp * g.tmp_w + xp) * C;
   const int x = clampi(xp - g.pad, g.w), y = clampi(yp - g.pad, g.h);
   const float scale = __int_as_float((127 - 2 * sh) << 23);  // 4^-l
   int sum[3] = {0, 0, 0};
-  for (int dy = 0; dy < n; ++dy) {
+  for (int dy = 0; dy < nb; ++dy) {
     const int Y = clampi((y << sh) + dy - s.pad_top, s.h_org);
     const unsigned char* row = src + (size_t)Y * s.w_org * C;
-    for (int dx = 0; dx < n; ++dx) {
+    for (int dx = 0; dx < nb; ++dx) {
       const int X = clampi((x << sh) + dx - s.pad_left, s.w_org);
       for (int c = 0; c < C; ++c) sum[c] += (int)__ldg(row + X * C + c);
     }
   }
-  for (int c = 0; c < C; ++c) dst[c] = (float)sum[c] * scale;
+  if constexpr (SEQ) {
+    float* d0 = fr < n ? const_cast<float*>(g.img[0]) + (size_t)frame_of(g, f0, fr) * g.img_fs[0] + o : nullptr;
+    float* d1 = fr >= 1 ? const_cast<float*>(g.img[3]) + (size_t)frame_of(g, f0, fr - 1) * g.img_fs[3] + o : nullptr;
+    for (int c = 0; c < C; ++c) {
+      const float v = (float)sum[c] * scale;
+      if (d0) d0[c] = v;
+      if (d1) d1[c] = v;
+    }
+  } else {
+    const int arr = k ? 3 : 0;
+    float* dst = const_cast<float*>(g.img[arr]) + (size_t)frame_of(g, f0, fr) * g.img_fs[arr] + o;
+    for (int c = 0; c < C; ++c) dst[c] = (float)sum[c] * scale;
+  }
 }
 
 // Border padding of un-padded float images of level g.level ([frame][2][h][w][C], I0 then I1).
@@ -53,19 +68,37 @@ __global__ void __launch_bounds__(256) pyr_from_level_kernel(LevelGeom g, int f0
 
 // cv::resize(0.5, 0.5, INTER_LINEAR) of an even-sized image == 2x2 box mean (run_dense.cpp:150),
 // ((a+b)+(c+d))*0.25 with a,b the even row; reads the interior of the padded level gs, writes
-// level gd = gs+1 including its replicate border.
-__global__ void __launch_bounds__(256) pyr_down_kernel(LevelGeom gs, LevelGeom gd, int f0) {
+// level gd = gs+1 including its replicate border.  SEQ as in pyr_from_u8_kernel: frame t of the n + 1
+// consecutive frames reads its finer level from the pair that holds it (I0 of pair t, or I1 of pair n - 1 for
+// the last frame) and writes both pairs that hold it.
+template <bool SEQ>
+__global__ void __launch_bounds__(256) pyr_down_kernel(LevelGeom gs, LevelGeom gd, int f0, int n) {
   pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
   const int xp = blockIdx.x * blockDim.x + threadIdx.x, yp = blockIdx.y * blockDim.y + threadIdx.y;
   if (xp >= gd.tmp_w || yp >= gd.tmp_h) return;
-  const int fr = blockIdx.z >> 1, k = blockIdx.z & 1;
-  const int C = gd.noc, arr = k ? 3 : 0;
-  const float* src = gs.img[arr] + (size_t)frame_of(gd, f0, fr) * gs.img_fs[arr];
-  float* dst = const_cast<float*>(gd.img[arr]) + (size_t)frame_of(gd, f0, fr) * gd.img_fs[arr] + ((size_t)yp * gd.tmp_w + xp) * C;
+  const int C = gd.noc;
+  const size_t o = ((size_t)yp * gd.tmp_w + xp) * C;
   const int x = clampi(xp - gd.pad, gd.w), y = clampi(yp - gd.pad, gd.h);
-  const float* r0 = src + ((size_t)(2 * y + gs.pad) * gs.tmp_w + (2 * x + gs.pad)) * C;
-  const float* r1 = r0 + (size_t)gs.tmp_w * C;
-  for (int c = 0; c < C; ++c) dst[c] = ((r0[c] + r0[C + c]) + (r1[c] + r1[C + c])) * 0.25f;
+  const size_t so = ((size_t)(2 * y + gs.pad) * gs.tmp_w + (2 * x + gs.pad)) * C;
+  if constexpr (SEQ) {
+    const int t = blockIdx.z, sa = t < n ? 0 : 3, sf = t < n ? t : t - 1;
+    const float* r0 = gs.img[sa] + (size_t)frame_of(gd, f0, sf) * gs.img_fs[sa] + so;
+    const float* r1 = r0 + (size_t)gs.tmp_w * C;
+    float* d0 = t < n ? const_cast<float*>(gd.img[0]) + (size_t)frame_of(gd, f0, t) * gd.img_fs[0] + o : nullptr;
+    float* d1 = t >= 1 ? const_cast<float*>(gd.img[3]) + (size_t)frame_of(gd, f0, t - 1) * gd.img_fs[3] + o : nullptr;
+    for (int c = 0; c < C; ++c) {
+      const float v = ((r0[c] + r0[C + c]) + (r1[c] + r1[C + c])) * 0.25f;
+      if (d0) d0[c] = v;
+      if (d1) d1[c] = v;
+    }
+  } else {
+    const int fr = blockIdx.z >> 1, k = blockIdx.z & 1;
+    const int arr = k ? 3 : 0;
+    const float* r0 = gs.img[arr] + (size_t)frame_of(gd, f0, fr) * gs.img_fs[arr] + so;
+    const float* r1 = r0 + (size_t)gs.tmp_w * C;
+    float* dst = const_cast<float*>(gd.img[arr]) + (size_t)frame_of(gd, f0, fr) * gd.img_fs[arr] + o;
+    for (int c = 0; c < C; ++c) dst[c] = ((r0[c] + r0[C + c]) + (r1[c] + r1[C + c])) * 0.25f;
+  }
 }
 
 // Gradients of I0 on the device (the first "next" row of SURVEY 8f): cv::Sobel(CV_32F, 3x3,
@@ -155,7 +188,12 @@ int launch_sobel(const LevelGeom& g, int f0, int f1, cudaStream_t st) {
 }
 
 int launch_pyr_from_u8(const LevelGeom& g, int f0, int f1, const PyrSourceU8& s, cudaStream_t st) {
-  pyr_from_u8_kernel<<<padded_grid(g, 2 * (f1 - f0)), dim3(32, 8), 0, st>>>(g, f0, s);
+  pyr_from_u8_kernel<false><<<padded_grid(g, 2 * (f1 - f0)), dim3(32, 8), 0, st>>>(g, f0, s, 0);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_pyr_from_u8_seq(const LevelGeom& g, int f0, int n, const PyrSourceU8& s, cudaStream_t st) {
+  pyr_from_u8_kernel<true><<<padded_grid(g, n + 1), dim3(32, 8), 0, st>>>(g, f0, s, n);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -165,7 +203,12 @@ int launch_pyr_from_level(const LevelGeom& g, int f0, int f1, const float* stage
 }
 
 int launch_pyr_down(const LevelGeom& gs, const LevelGeom& gd, int f0, int f1, cudaStream_t st) {
-  pyr_down_kernel<<<padded_grid(gd, 2 * (f1 - f0)), dim3(32, 8), 0, st>>>(gs, gd, f0);
+  pyr_down_kernel<false><<<padded_grid(gd, 2 * (f1 - f0)), dim3(32, 8), 0, st>>>(gs, gd, f0, 0);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_pyr_down_seq(const LevelGeom& gs, const LevelGeom& gd, int f0, int n, cudaStream_t st) {
+  pyr_down_kernel<true><<<padded_grid(gd, n + 1), dim3(32, 8), 0, st>>>(gs, gd, f0, n);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -434,6 +434,12 @@ int main(int argc, char** argv) {
 // grouped into batches of up to N (default 64): 8-bit frames up, pyramid / hot path / upsampling
 // on the device, full-resolution flows back.  Every output is byte-identical to what the
 // single-pair binary writes for that pair.
+//
+// Video: pair k+1 continues pair k when its image1 path is pair k's image2 path (string equality).  A batch of two
+// or more pairs in which every pair continues the one before it is a clip of n+1 frames: each frame is decoded
+// once and the clip goes up with ofdis_upload_sequence_u8 (each frame uploaded and its levels built once).  A
+// batch that starts with the frame the previous one ended on takes that frame's decoded image over.  Every other
+// batch goes through ofdis_upload_frames_u8.
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr, "usage: %s listfile [--batch N] [oppoint | 20 parameters (README.md:66-88)]\n", argv[0]);
@@ -465,32 +471,60 @@ int main(int argc, char** argv) {
   const int nop = (SELECTMODE == 1) ? 2 : 1;
   timeval tv;
   gettimeofday(&tv, NULL);
-  size_t done = 0;
+  size_t done = 0, seq_pairs = 0, seq_decoded = 0;
   ofdis_ctx* ctx = nullptr;
   int ctx_w = -1, ctx_h = -1, verbosity = 0;
   vector<uint8_t> frames;
   vector<float> flows;
+  Image8 last;  // image2 of the previous batch's last pair
   size_t j0 = 0;
   while (j0 < jobs.size()) {
-    // load up to maxb pairs of one size
-    Image8 a8, b8;
-    int w = 0, h = 0, n = 0;
-    frames.clear();
+    // load up to maxb pairs of one size; a frame that continues the previous pair is not decoded again
+    vector<Image8> imgs;  // decoded frames of this batch
+    vector<int> ia, ib;   // per pair: indices of image1, image2 in imgs
+    int w = 0, h = 0, n = 0, decoded = 0;
     while (j0 + n < jobs.size() && n < maxb) {
       const Job& jb = jobs[j0 + n];
-      if (!load_image(jb.a.c_str(), nochannels, a8) || !load_image(jb.b.c_str(), nochannels, b8) || a8.w != b8.w ||
-          a8.h != b8.h) {
+      const bool in_batch = n > 0 && jb.a == jobs[j0 + n - 1].b;          // image1 = this batch's last frame
+      const bool from_last = n == 0 && j0 > 0 && jb.a == jobs[j0 - 1].b;  // image1 = the previous batch's last frame
+      Image8 a8, b8;
+      if (from_last) a8 = last;
+      const bool ok = in_batch || from_last || load_image(jb.a.c_str(), nochannels, a8);
+      const Image8& ra = in_batch ? imgs[ib.back()] : a8;
+      if (!ok || !load_image(jb.b.c_str(), nochannels, b8) || ra.w != b8.w || ra.h != b8.h) {
         fprintf(stderr, "error: cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)\n",
                 jb.a.c_str(), jb.b.c_str());
         if (ctx) ofdis_destroy(ctx);
         return 1;
       }
-      if (n == 0) { w = a8.w; h = a8.h; }
-      else if (a8.w != w || a8.h != h) break;  // next group
-      frames.insert(frames.end(), a8.px.begin(), a8.px.end());
-      frames.insert(frames.end(), b8.px.begin(), b8.px.end());
+      if (n == 0) { w = b8.w; h = b8.h; }
+      else if (b8.w != w || b8.h != h) break;  // next group
+      if (in_batch) ia.push_back(ib.back());
+      else {
+        decoded += from_last ? 0 : 1;
+        ia.push_back((int)imgs.size());
+        imgs.push_back(std::move(a8));
+      }
+      ib.push_back((int)imgs.size());
+      imgs.push_back(std::move(b8));
+      ++decoded;
       ++n;
     }
+    bool seq = n >= 2;
+    for (int k = 1; k < n && seq; ++k) seq = ia[k] == ib[k - 1];
+    frames.clear();
+    if (seq) {
+      frames.insert(frames.end(), imgs[ia[0]].px.begin(), imgs[ia[0]].px.end());
+      for (int k = 0; k < n; ++k) frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
+      seq_pairs += n;
+      seq_decoded += decoded;
+    } else {
+      for (int k = 0; k < n; ++k) {
+        frames.insert(frames.end(), imgs[ia[k]].px.begin(), imgs[ia[k]].px.end());
+        frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
+      }
+    }
+    last = std::move(imgs[ib.back()]);
     CliParams P;
     parse_cli_params(nnum, argv + first_num, w, P);
     verbosity = P.verbosity;
@@ -517,7 +551,8 @@ int main(int argc, char** argv) {
       ctx_h = h;
     }
     flows.resize((size_t)n * w * h * nop);
-    int rc = ofdis_upload_frames_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
+    int rc = seq ? ofdis_upload_sequence_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST)
+                 : ofdis_upload_frames_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
     if (rc == OFDIS_OK) rc = ofdis_run(ctx, n, 0);
     if (rc == OFDIS_OK) rc = ofdis_get_flow_fullres(ctx, 0, n, flows.data(), w, h, OFDIS_MEM_HOST);
     if (rc == OFDIS_OK) rc = ofdis_sync(ctx);
@@ -538,6 +573,7 @@ int main(int argc, char** argv) {
   }
   if (ctx) ofdis_destroy(ctx);
   if (verbosity > 0) printf("TIME (%zu pairs, load + flow + save) (ms): %3g\n", done, elapsed_ms(tv));
+  if (verbosity > 0 && seq_pairs) printf("SEQUENCE (%zu of %zu pairs from %zu decoded frames)\n", seq_pairs, done, seq_decoded);
   return 0;
 }
 #else

@@ -6,6 +6,7 @@ flow  : u = A sin(4x/W+.3) cos(3y/H),  v = .6A cos(2.5x/W) sin(5y/H+.7)
         (stereo: u = -(2 + A(.5+.5 sin(3.1x/W + 2y/H))), v = 0)
 I0    : centre crop of the canvas;  I1(x) = canvas(x - flow(x)) (cubic), so that
         I0(x) ~= I1(x + flow(x)) (the reference's convention, patch.cpp:217)
+clip  : frame t = canvas(x - t flow(x)) (synthetic_sequence; frames 0, 1 are the pair)
 Both are quantised to uint8 because the reference CLI reads 8-bit images.
 """
 from __future__ import annotations
@@ -24,8 +25,8 @@ def synthetic_flow(h: int, w: int, amp: float = 6.0, stereo: bool = False):
     return u, v
 
 
-def synthetic_pair(h: int, w: int, channels: int = 1, seed: int = 0, amp: float = 6.0, stereo: bool = False):
-    """Returns (img0_u8, img1_u8, flow_gt[h,w,2]); images are (h,w) or (h,w,3)."""
+def _canvas(h: int, w: int, channels: int, seed: int):
+    """The (h+2m)x(w+2m)xC float64 canvas in [0,255] and its margin m."""
     from scipy import ndimage
 
     rng = np.random.default_rng(seed)
@@ -38,16 +39,39 @@ def synthetic_pair(h: int, w: int, channels: int = 1, seed: int = 0, amp: float 
             acc += sigma * ndimage.gaussian_filter(rng.standard_normal((hc, wc)), sigma, mode="reflect")
         canv[..., c] = acc
     lo, hi = canv.min(), canv.max()
-    canv = (canv - lo) / (hi - lo) * 255.0
+    return (canv - lo) / (hi - lo) * 255.0, m
+
+
+def _frame(canv, m: int, h: int, w: int, u, v, t: int):
+    """Frame t of the canvas' clip, quantised to uint8: frame 0 is the centre crop, frame t >= 1 the canvas
+    sampled at x - t*flow(x) (cubic)."""
+    from scipy import ndimage
+
+    channels = canv.shape[2]
+    if t == 0:
+        img = canv[m:m + h, m:m + w]
+    else:
+        yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+        img = np.empty((h, w, channels))
+        for c in range(channels):
+            img[..., c] = ndimage.map_coordinates(canv[..., c], [yy + m - t * v, xx + m - t * u], order=3, mode="nearest")
+    q = np.clip(np.rint(img), 0, 255).astype(np.uint8)
+    return np.ascontiguousarray(q[..., 0] if channels == 1 else q)
+
+
+def synthetic_pair(h: int, w: int, channels: int = 1, seed: int = 0, amp: float = 6.0, stereo: bool = False):
+    """Returns (img0_u8, img1_u8, flow_gt[h,w,2]); images are (h,w) or (h,w,3)."""
+    canv, m = _canvas(h, w, channels, seed)
     u, v = synthetic_flow(h, w, amp, stereo)
-    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
-    img0 = canv[m:m + h, m:m + w]
     # I1(x + f(x)) = I0(x); first-order inverse: I1(x) = canvas(x - f(x))
-    img1 = np.empty_like(img0)
-    for c in range(channels):
-        img1[..., c] = ndimage.map_coordinates(canv[..., c], [yy + m - v, xx + m - u], order=3, mode="nearest")
-    q = lambda a: np.clip(np.rint(a), 0, 255).astype(np.uint8)
-    i0, i1 = q(img0), q(img1)
-    if channels == 1:
-        i0, i1 = i0[..., 0], i1[..., 0]
-    return np.ascontiguousarray(i0), np.ascontiguousarray(i1), np.stack([u, v], -1).astype(np.float32)
+    i0, i1 = _frame(canv, m, h, w, u, v, 0), _frame(canv, m, h, w, u, v, 1)
+    return i0, i1, np.stack([u, v], -1).astype(np.float32)
+
+
+def synthetic_sequence(n_frames: int, h: int, w: int, channels: int = 1, seed: int = 0, amp: float = 6.0,
+                       stereo: bool = False):
+    """A clip of n_frames uint8 frames, [n_frames][h][w] or [n_frames][h][w][3]: frame t is the canvas sampled at
+    x - t*flow(x), so frames 0 and 1 are synthetic_pair(h, w, channels, seed, amp, stereo)[:2] bit for bit."""
+    canv, m = _canvas(h, w, channels, seed)
+    u, v = synthetic_flow(h, w, amp, stereo)
+    return np.ascontiguousarray(np.stack([_frame(canv, m, h, w, u, v, t) for t in range(n_frames)]))
