@@ -153,8 +153,27 @@ int ofdis_upload_finest_level(ofdis_ctx* ctx, int f0, int f1, const float* packe
 
 /* Output stage on the device (extension, SURVEY 8f rank 2 == run_dense.cpp:407-414): flow of level
  * sc_l times 2^sc_l, bilinear upsampling by 2^sc_l (half-pixel centres, edge clamped), crop of the
- * divisibility padding.  `out` = [f1-f0][height_org][width_org][nop] floats. */
+ * divisibility padding.  `out` = [f1-f0][height_org][width_org][nop] floats.  Here and in the 8-bit uploads,
+ * width_org/height_org pad up to the context's size by multiples of 2^sc_f, or of 2^(sc_f+1) as a run with an init
+ * flow pads (run_dense.cpp:301); the crop is floor(pad/2) on the left/top either way. */
 int ofdis_get_flow_fullres(ofdis_ctx* ctx, int f0, int f1, float* out, int width_org, int height_org, int memkind);
+
+/* Init flow from a flow of the original frame size (extension; the reference's disabled file input,
+ * run_dense.cpp:292-301,355-378).  `flow` = [f1-f0][height_org][width_org][nop] floats.  Prepares the initflow of
+ * pairs [f0, f1) that the following ofdis_run(ctx, n, use_initflow = 1) reads: replicate padding to the context,
+ * x 2^-(sc_f+1), cv::resize(INTER_AREA) by 2^(sc_f+1) in OpenCV's summation order (DESIGN.md section 1), written to
+ * level sc_f+1 of the forward grid; with usefbcon the backward grid's level sc_f+1 is zeroed (the reference
+ * initialises only the forward grid, oflow.cpp:217-220).  The context's width and height must be multiples of
+ * 2^(sc_f+1) -- the padding of run_dense.cpp:301 -- else OFDIS_ERR_ARG; width_org/height_org must pad up to them.
+ * Host input goes through the context's staging buffer.  Slots outside [f0, f1) are not touched.  Otherwise the
+ * same arguments and status codes as ofdis_upload_frames_u8. */
+int ofdis_set_initflow_fullres(ofdis_ctx* ctx, int f0, int f1, const float* flow, int width_org, int height_org,
+                               int memkind);
+/* Warm start (extension): the init flow of pairs [f0, f1) from the last run's flow of pairs
+ * [src_f0, src_f0 + f1 - f0) -- bitwise ofdis_get_flow_fullres(DEVICE) of those pairs followed by
+ * ofdis_set_initflow_fullres(DEVICE), through the context's full-resolution scratch.  Source and destination slots
+ * may overlap (they are different buffers).  Same status codes as ofdis_set_initflow_fullres. */
+int ofdis_set_initflow_from_result(ofdis_ctx* ctx, int f0, int f1, int src_f0, int width_org, int height_org);
 
 /* Stage operators on frames [f0,f1) of one level. */
 int ofdis_patgrid_optimize(ofdis_ctx* ctx, int level, int f0, int f1, int init_from_coarser);
@@ -162,8 +181,9 @@ int ofdis_patgrid_aggregate(ofdis_ctx* ctx, int level, int f0, int f1);
 int ofdis_varref_refine(ofdis_ctx* ctx, int level, int f0, int f1);
 
 /* Whole coarse-to-fine run on frames [0,nframes): == OFClass ctor per frame.
- * use_initflow != 0 takes the flow stored at level sc_f+1 (ofdis_set_flow) as
- * the reference's `initflow` argument. */
+ * use_initflow != 0 takes the flow stored at level sc_f+1 (ofdis_set_flow,
+ * ofdis_set_initflow_fullres, ofdis_set_initflow_from_result) as the reference's
+ * `initflow` argument. */
 int ofdis_run(ofdis_ctx* ctx, int nframes, int use_initflow);
 int ofdis_sync(ofdis_ctx* ctx);
 

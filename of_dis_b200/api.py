@@ -31,7 +31,8 @@ EXPORTS = [
     "ofdis_set_camlr", "ofdis_set_dp_thresh_sq", "ofdis_packed_images_frame_floats", "ofdis_upload_packed_images",
     "ofdis_upload_frames_u8", "ofdis_finest_level_frame_floats", "ofdis_upload_finest_level", "ofdis_get_flow_fullres",
     "ofdis_get_level", "ofdis_upload_level_fb", "ofdis_set_option", "ofdis_profile_levels", "ofdis_set_direction",
-    "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8",
+    "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8", "ofdis_set_initflow_fullres",
+    "ofdis_set_initflow_from_result",
 ]
 
 
@@ -77,6 +78,9 @@ def lib():
                                                ctypes.c_int, ctypes.c_int]
         L.ofdis_get_flow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_int]
+        L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                 ctypes.c_int, ctypes.c_int, ctypes.c_int]
+        L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
         L.ofdis_upload_packed.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
         L.ofdis_upload_level.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int]
         L.ofdis_upload_level_fb.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 6 + [ctypes.c_int]
@@ -219,6 +223,19 @@ class Context:
     def get_flow_fullres(self, f0, f1, dst, width_org, height_org, memkind=MEM_HOST):
         """Flow x 2^sc_l, upsampled to the original frame size and cropped (run_dense.cpp:407-414)."""
         self._ck(lib().ofdis_get_flow_fullres(self._h, f0, f1, _ptr(dst), width_org, height_org, memkind))
+
+    def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
+        """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)
+        that run(n, use_initflow=True) starts from (preprocess.initflow_from_fullres on the device).  The context's
+        width and height must be multiples of 2^(sc_f+1)."""
+        if isinstance(flow, np.ndarray):
+            flow = np.ascontiguousarray(flow, np.float32)
+        self._ck(lib().ofdis_set_initflow_fullres(self._h, f0, f1, _ptr(flow), width_org, height_org, memkind))
+
+    def set_initflow_from_result(self, f0, f1, src_f0, width_org, height_org):
+        """Warm start: the init flow of pairs [f0, f1) from the last run's flows of pairs [src_f0, src_f0 + f1 - f0),
+        bitwise get_flow_fullres (device) followed by set_initflow_fullres (device)."""
+        self._ck(lib().ofdis_set_initflow_from_result(self._h, f0, f1, src_f0, width_org, height_org))
 
     def upload_packed(self, f0, f1, packed, memkind=MEM_HOST):
         self._ck(lib().ofdis_upload_packed(self._h, f0, f1, _ptr(packed), memkind))

@@ -178,6 +178,71 @@ __global__ void __launch_bounds__(256) flow_upsample_kernel(LevelGeom g, int f0,
   }
 }
 
+// Init flow of the reference's disabled file input (run_dense.cpp:355-378): the full-resolution flow
+// [frame][h_org][w_org][NOP], replicate-padded to the context (clamped reads, floor(pad/2) left/top), times
+// 2^-(sc_f+1), then cv::resize(INTER_AREA) by the integer factor s = 2^(sc_f+1).  That is OpenCV's area-fast path:
+// sum = 0, then for the s x s terms of the block in row-major order, groups of four add as
+// sum += ((t0 + t1) + t2) + t3, and the result is sum * (1/s^2); for s = 2 with one channel its SIMD body,
+// ((a + b) + (c + d)) * 0.25 (preprocess.initflow_from_fullres).  g: level sc_f, stepped by the context's directions;
+// writes level sc_f+1 (g.flow_prev) of the forward grid of every pair, and with usefbcon zeroes the backward grid's,
+// which the reference does not initialise (oflow.cpp:217-220).
+// TEAM == 1 (s <= 8): one thread per output pixel.  TEAM == 256: one CTA per output pixel; the threads form the
+// independent group partials of up to 1024 groups in shared memory, and thread c adds channel c's in order.
+template <int NOP, int TEAM>
+__global__ void __launch_bounds__(256) initflow_prepare_kernel(LevelGeom g, int f0, const float* src, int w_org,
+                                                               int h_org, int pad_left, int pad_top) {
+  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
+  const int W = g.w >> 1, H = g.h >> 1, sh = g.level + 1, s = 1 << sh;
+  const int pix = TEAM == 1 ? (int)(blockIdx.x * blockDim.x + threadIdx.x) : (int)blockIdx.x, fr = blockIdx.y;
+  if (pix >= W * H) return;
+  const int x0 = (pix % W) * s - pad_left, y0 = (pix / W) * s - pad_top;
+  const float* fl = src + (size_t)fr * h_org * w_org * NOP;
+  const float sc = __int_as_float((127 - sh) << 23), inv_area = __int_as_float((127 - 2 * sh) << 23);
+  auto term = [&](int k, int c) {  // term k (row-major in the block) of channel c, scaled
+    const int X = clampi(x0 + (k & (s - 1)), w_org), Y = clampi(y0 + (k >> sh), h_org);
+    return __ldg(fl + ((size_t)Y * w_org + X) * NOP + c) * sc;
+  };
+  auto group = [&](int gi, int c) {
+    const int k = 4 * gi;
+    return ((term(k, c) + term(k + 1, c)) + term(k + 2, c)) + term(k + 3, c);
+  };
+  const int ng = (s * s) >> 2;
+  float* dst = const_cast<float*>(g.flow_prev) + (size_t)frame_of(g, f0, fr) * g.flow_prev_frame_stride + (size_t)pix * NOP;
+  if constexpr (TEAM == 1) {
+    for (int c = 0; c < NOP; ++c) {
+      float v;
+      if (NOP == 1 && s == 2) {
+        v = ((term(0, c) + term(1, c)) + (term(2, c) + term(3, c))) * 0.25f;
+      } else {
+        float sum = 0.f;
+        for (int gi = 0; gi < ng; ++gi) sum += group(gi, c);
+        v = sum * inv_area;
+      }
+      dst[c] = v;
+      if (g.fstep == 2) dst[g.flow_prev_frame_stride + c] = 0.f;
+    }
+  } else {
+    __shared__ float part[NOP][1024 + 1];  // +1: the channels' rows start in different banks
+    float sum = 0.f;                       // thread c < NOP: channel c
+    for (int base = 0; base < ng; base += 1024) {
+      const int m = min(1024, ng - base);
+      for (int i = threadIdx.x; i < m; i += TEAM)
+        for (int c = 0; c < NOP; ++c) part[c][i] = group(base + i, c);
+      __syncthreads();
+      if (threadIdx.x < NOP) {
+        const float* p = part[threadIdx.x];
+#pragma unroll 8
+        for (int i = 0; i < m; ++i) sum += p[i];
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x < NOP) {
+      dst[threadIdx.x] = sum * inv_area;
+      if (g.fstep == 2) dst[g.flow_prev_frame_stride + threadIdx.x] = 0.f;
+    }
+  }
+}
+
 }  // namespace
 
 static dim3 padded_grid(const LevelGeom& g, int nz) { return dim3((g.tmp_w + 31) / 32, (g.tmp_h + 7) / 8, nz); }
@@ -217,6 +282,21 @@ int launch_flow_upsample(const LevelGeom& g, int f0, int f1, float* out, int w_o
   const dim3 block(32, 8), grid((w_org + 31) / 32, (h_org + 7) / 8, f1 - f0);
   if (g.nop == 2) flow_upsample_kernel<2><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
   else flow_upsample_kernel<1><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_initflow_prepare(const LevelGeom& g, int f0, int n, const float* flow, int w_org, int h_org, int pad_left,
+                            int pad_top, cudaStream_t st) {
+  const int npix = (g.w >> 1) * (g.h >> 1);
+  if ((2 << g.level) <= 8) {
+    const dim3 grid((npix + 255) / 256, n);
+    if (g.nop == 2) initflow_prepare_kernel<2, 1><<<grid, 256, 0, st>>>(g, f0, flow, w_org, h_org, pad_left, pad_top);
+    else initflow_prepare_kernel<1, 1><<<grid, 256, 0, st>>>(g, f0, flow, w_org, h_org, pad_left, pad_top);
+  } else {
+    const dim3 grid(npix, n);
+    if (g.nop == 2) initflow_prepare_kernel<2, 256><<<grid, 256, 0, st>>>(g, f0, flow, w_org, h_org, pad_left, pad_top);
+    else initflow_prepare_kernel<1, 256><<<grid, 256, 0, st>>>(g, f0, flow, w_org, h_org, pad_left, pad_top);
+  }
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
