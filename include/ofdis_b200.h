@@ -245,6 +245,11 @@ int ofdis_set_direction(ofdis_ctx* ctx, int dir);
  *   "pdl"             2 (default) | 1 | 0: programmatic dependent launch of the level loop's kernels (every kernel starts
  *                     with griddepcontrol.wait, so the next kernel's launch overlaps the tail of the current one):
  *                     1 always, 0 never, 2 for launches of up to 16 frames (2-5 % of the step there; larger batches lose)
+ *   "patch_lanes"     0 (default) | 8 | 4: lanes per patch of the P = 8 gray patch kernel (other patch sizes and RGB
+ *                     ignore it): 8 = one template column per lane, 4 patches per warp; 4 = two adjacent columns per
+ *                     lane, 8 patches per warp, so the per-patch work its lanes repeat (bilinear weights, reductions,
+ *                     Cholesky solve, stop tests) is paid once per 8 patches; 0 = 4 for launches of more than 16
+ *                     frames, 8 for smaller ones
  *   "sor_rows_per_thread" 1 (default for flow) | 2 (default for stereo) | 4: rows of the 4-column tile one SOR thread updates per super-step
  *                     (a level needs W/4 + h/rows super-steps; sor_wave_kernel.cuh)
  *   "sor_single_max"  32 | 64 | 128 (default): refinement levels of up to this many SOR lanes (= rows / rows per

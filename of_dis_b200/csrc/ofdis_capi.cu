@@ -43,7 +43,10 @@ struct ofdis_ctx {
   // 0.374 -> 0.344 ms, 8 pairs 0.390 -> 0.363 ms; 64 pairs 0.659 -> 0.690 ms, and 5-14 % less throughput when ten
   // streams of 32 or 64 frames overlap (waiting CTAs of the next kernel take SM slots from the tail of the current one)
   int pdl = 2;
-  int nlev = 0;                    // sc_f - sc_l + 1
+  // lanes per patch of the P = 8 gray patch kernel (patch_p8c1_kernel): 8 or 4, 0 (default) = 4 for launches of more
+  // than SOR_LANE_AUTO_FRAMES frames, 8 below (DESIGN.md section 5.9)
+  int patch_lanes = 0;
+  int nlev = 0;                   // sc_f - sc_l + 1
   std::vector<LevelGeom> lev;      // index: level - sc_l
   std::vector<size_t> img_off;     // [lev][4] offsets (floats) inside one packed frame
   size_t frame_floats = 0;
@@ -155,6 +158,12 @@ void make_level(LevelGeom& L, const ofdis_ctx* c, int sl) {
 
 // programmatic dependent launch for a launch of `frames` internal frames (ofdis_set_option "pdl")
 int pdl_for(const ofdis_ctx* c, int frames) { return c->pdl == 1 || (c->pdl == 2 && frames <= SOR_LANE_AUTO_FRAMES) ? 1 : 0; }
+
+// lanes per patch of patch_p8c1_kernel for a launch of `frames` internal frames (ofdis_set_option "patch_lanes")
+int patch_lanes_for(const ofdis_ctx* c, int frames) {
+  if (c->patch_lanes) return c->patch_lanes;
+  return frames > SOR_LANE_AUTO_FRAMES ? 4 : 8;
+}
 
 LevelGeom* level_of(ofdis_ctx* c, int level) {
   if (level < c->prm.sc_l || level > c->prm.sc_f) return nullptr;
@@ -757,7 +766,8 @@ int ofdis_patgrid_optimize(ofdis_ctx* ctx, int level, int f0, int f1, int init_f
   const int q0 = ctx->sel_dir >= 0 ? f0 * ctx->dirs + ctx->sel_dir : f0 * ctx->dirs;
   const int q1 = ctx->sel_dir >= 0 ? q0 + 1 : f1 * ctx->dirs;
   L->pdl = pdl_for(ctx, q1 - q0);
-  const int n = launch_patch_optimize(*L, ctx->pp, q0, q1, init_from_coarser != 0, ctx->stream, ctx->prof);
+  const int n = launch_patch_optimize(*L, ctx->pp, q0, q1, init_from_coarser != 0, patch_lanes_for(ctx, q1 - q0),
+                                      ctx->stream, ctx->prof);
   if (n < 0) return fail(ctx, OFDIS_ERR_CUDA, "patch_optimize_kernel launch", cudaGetLastError());
   ctx->launches += n;
   return OFDIS_OK;
@@ -862,6 +872,9 @@ int ofdis_set_option(ofdis_ctx* ctx, const char* name, int value) {
   } else if (!strcmp(name, "pdl")) {
     if (value < 0 || value > 2) return fail(ctx, OFDIS_ERR_ARG, "pdl: 0, 1 or 2");
     ctx->pdl = value;
+  } else if (!strcmp(name, "patch_lanes")) {
+    if (value != 0 && value != 4 && value != 8) return fail(ctx, OFDIS_ERR_ARG, "patch_lanes: 0, 4 or 8");
+    ctx->patch_lanes = value;
   } else if (!strcmp(name, "sor_fast")) {
     if (value != 0 && value != 1) return fail(ctx, OFDIS_ERR_ARG, "sor_fast: 0 or 1");
     if (!ctx->d_planes) return fail(ctx, OFDIS_ERR_ARG, "sor_fast: context created with usetvref=0");
