@@ -148,6 +148,32 @@ int ofdis_upload_frames_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char* 
  * next chunk's first. */
 int ofdis_upload_sequence_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char* frames, int width_org,
                              int height_org, int memkind);
+/* Two-way sequence (extension): `frames` = [n+1][height_org][width_org][noc] 8-bit frames.  Slot f0+t gets
+ * (frames[t], frames[t+1]), slot f0+n+t gets (frames[t+1], frames[t]); f0 + 2n <= max_frames.  Arguments, padding
+ * rules, staging and status codes as ofdis_upload_sequence_u8 (n < 1: OFDIS_ERR_ARG); each frame is uploaded and each
+ * of its levels built once.  Every slot's pyramid is bitwise what ofdis_upload_frames_u8 of the forward and the
+ * swapped pairs gives.  Marks slots [f0, f0+n) not swapped and [f0+n, f0+2n) swapped (see ofdis_set_swapped_slots);
+ * other uploads leave the marks alone. */
+int ofdis_upload_sequence_bidir_u8(ofdis_ctx* ctx, int f0, int n, const unsigned char* frames, int width_org,
+                                   int height_org, int memkind);
+/* Stereo (nop == 1): slots [f0, f1) hold swapped pairs (right image first) and run as the right camera -- every grid
+ * of such a slot has its camlr inverted (with usefbcon its forward grid clamps disparities to >= 0, its backward grid
+ * to <= 0).  Flow ignores the mark.  Default 0 for every slot; swapped is 0 or 1.  The marks are read when a run
+ * executes, so a captured graph follows later changes.  Enqueued on the context's stream. */
+int ofdis_set_swapped_slots(ofdis_ctx* ctx, int f0, int f1, int swapped);
+/* Forward-backward (flow) / left-right (stereo) consistency of the last run's slots [f0, f1) against partner slots
+ * [b0, b0 + f1 - f0), at the original frame size: mask = [f1-f0][height_org][width_org] bytes (0 consistent,
+ * 1 inconsistent, 2 leaves the frame), err = the same shape in float32 (may be NULL).  F is slot a's full-resolution
+ * flow and B its partner's, both exactly what ofdis_get_flow_fullres returns; per pixel, in float32 without
+ * contraction: (xs, ys) = (x, y) + F(x, y); outside [0, width_org-1] x [0, height_org-1] (or NaN): mask 2,
+ * err +inf; else b = B sampled bilinearly at (xs, ys) (corners floor and floor + 1 clamped to the frame, horizontal
+ * pass first), err = |F + b|^2 and mask = (err <= alpha (|F|^2 + |b|^2) + beta) ? 0 : 1.  Usual choices: flow
+ * alpha 0.01, beta 0.5 (Sundaram et al., ECCV 2010); stereo alpha 0, beta 1 (|d_L + d_R(x + d_L)| <= 1 px).
+ * alpha, beta finite and >= 0, a non-NULL mask and slots inside the context, else OFDIS_ERR_ARG; frame sizes as
+ * ofdis_get_flow_fullres checks them.  Computed from the level flows without a full-resolution copy of either;
+ * host output goes through the context's full-resolution scratch.  The flows are not changed. */
+int ofdis_consistency_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, unsigned char* mask, float* err, float alpha,
+                              float beta, int width_org, int height_org, int memkind);
 size_t ofdis_finest_level_frame_floats(const ofdis_ctx* ctx);
 int ofdis_upload_finest_level(ofdis_ctx* ctx, int f0, int f1, const float* packed, int memkind);
 

@@ -32,8 +32,12 @@ EXPORTS = [
     "ofdis_upload_frames_u8", "ofdis_finest_level_frame_floats", "ofdis_upload_finest_level", "ofdis_get_flow_fullres",
     "ofdis_get_level", "ofdis_upload_level_fb", "ofdis_set_option", "ofdis_profile_levels", "ofdis_set_direction",
     "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8", "ofdis_set_initflow_fullres",
-    "ofdis_set_initflow_from_result",
+    "ofdis_set_initflow_from_result", "ofdis_upload_sequence_bidir_u8", "ofdis_set_swapped_slots",
+    "ofdis_consistency_fullres",
 ]
+
+# default thresholds of consistency_fullres: flow (Sundaram, Brox, Keutzer, ECCV 2010) and stereo (|d_L + d_R| <= 1)
+CONSISTENCY_DEFAULTS = {2: (0.01, 0.5), 1: (0.0, 1.0)}
 
 
 class OfdisError(RuntimeError):
@@ -76,6 +80,11 @@ def lib():
                                              ctypes.c_int, ctypes.c_int]
         L.ofdis_upload_sequence_u8.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                                ctypes.c_int, ctypes.c_int]
+        L.ofdis_upload_sequence_bidir_u8.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                     ctypes.c_int, ctypes.c_int, ctypes.c_int]
+        L.ofdis_set_swapped_slots.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3
+        L.ofdis_consistency_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 2 + \
+            [ctypes.c_float] * 2 + [ctypes.c_int] * 3
         L.ofdis_get_flow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
@@ -219,6 +228,42 @@ class Context:
         """[f1-f0+1][height_org][width_org][noc] 8-bit consecutive frames; pair f0+i = (frames[i], frames[i+1]).
         Bitwise the pyramids upload_frames_u8 builds from the duplicated pairs, each frame uploaded once."""
         self._ck(lib().ofdis_upload_sequence_u8(self._h, f0, f1, _ptr(frames), width_org, height_org, memkind))
+
+    def upload_sequence_bidir_u8(self, f0, n, frames, width_org, height_org, memkind=MEM_HOST):
+        """[n+1][height_org][width_org][noc] 8-bit consecutive frames -> slot f0+t = (frames[t], frames[t+1]) and
+        slot f0+n+t = (frames[t+1], frames[t]), the latter marked swapped (set_swapped_slots).  Bitwise the pyramids
+        upload_frames_u8 builds from the forward and the swapped pairs, each frame uploaded once."""
+        self._ck(lib().ofdis_upload_sequence_bidir_u8(self._h, f0, n, _ptr(frames), width_org, height_org, memkind))
+
+    def set_swapped_slots(self, f0, f1, swapped):
+        """Stereo: slots [f0, f1) hold (right, left) pairs and run as the right camera (camlr inverted)."""
+        self._ck(lib().ofdis_set_swapped_slots(self._h, f0, f1, int(swapped)))
+
+    def consistency_fullres(self, f0, f1, b0, width_org, height_org, alpha=None, beta=None, with_err=False,
+                            memkind=MEM_HOST, mask=None, err=None):
+        """Forward-backward (flow) / left-right (stereo) check of the last run's slots [f0, f1) against slots
+        [b0, b0 + f1 - f0) at the original frame size (preprocess.consistency_check on the device).  Returns
+        (mask, err): [f1-f0][height_org][width_org] uint8 (0 consistent, 1 inconsistent, 2 leaves the frame) and
+        float32, err None unless with_err.  alpha/beta None: CONSISTENCY_DEFAULTS of the context's nop.  Host output
+        goes to new arrays, or to `mask` / `err` given as numpy arrays of exactly that shape and dtype.  With
+        memkind=MEM_DEVICE, mask (and err) are device addresses the caller owns."""
+        da, db = CONSISTENCY_DEFAULTS[self.prm.nop]
+        alpha = da if alpha is None else alpha
+        beta = db if beta is None else beta
+        shape = (f1 - f0, height_org, width_org)
+        if memkind == MEM_HOST:
+            mask = np.empty(shape, np.uint8) if mask is None else mask
+            err = (np.empty(shape, np.float32) if err is None else err) if with_err else None
+            for name, arr, dt in (("mask", mask, np.uint8), ("err", err, np.float32)):
+                if arr is not None and not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape == shape
+                                            and arr.flags["C_CONTIGUOUS"] and arr.flags["WRITEABLE"]):
+                    raise ValueError("consistency_fullres: %s must be a writeable C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shape))
+        self._ck(lib().ofdis_consistency_fullres(self._h, f0, f1, b0, _ptr(mask), _ptr(err), alpha, beta, width_org,
+                                                 height_org, memkind))
+        if memkind == MEM_HOST:
+            self.sync()
+        return mask, err
 
     def get_flow_fullres(self, f0, f1, dst, width_org, height_org, memkind=MEM_HOST):
         """Flow x 2^sc_l, upsampled to the original frame size and cropped (run_dense.cpp:407-414)."""

@@ -3,8 +3,10 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
 #include <cstdio>
+#include <climits>
 #include <cstring>
 #include <map>
 #include <new>
@@ -52,6 +54,9 @@ struct ofdis_ctx {
   size_t frame_floats = 0;
   size_t images_floats = 0;        // leading part of a packed frame that holds I0,I1 of all levels
   float* d_img = nullptr;          // [max_frames][frame_floats]
+  // swapped marks (ofdis_set_swapped_slots), one byte per internal frame, in the same allocation right in front of
+  // d_img (LevelGeom::swap_off); this is the pointer the allocation is freed by
+  unsigned char* d_swapped = nullptr;
   // lazily allocated staging of the pyramid / output stages (ofdis_upload_frames_u8,
   // ofdis_upload_finest_level, ofdis_get_flow_fullres)
   void* d_stage = nullptr;
@@ -142,6 +147,7 @@ void make_level(LevelGeom& L, const ofdis_ctx* c, int sl) {
   L.offh = (L.h - (L.noph - 1) * L.steps) / 2;
   L.level = sl;
   L.camlr = 0;
+  L.swap_off = 0;
   L.pitch = ((L.w + 3) / 4) * 4;
   L.lb = -(float)p.p_samp_s / 2;
   L.ubw = (float)(L.w + p.p_samp_s / 2 - 2);
@@ -338,7 +344,18 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
   auto dalloc = [&](void** p, size_t bytes) -> bool {
     return cudaMalloc(p, bytes ? bytes : 16) == cudaSuccess;
   };
-  bool ok = dalloc((void**)&ctx->d_img, sizeof(float) * ctx->frame_floats * cap);
+  // the swapped marks take the first 256 bytes per 256 internal frames of the image allocation (alignment kept)
+  const size_t marks = ((size_t)cap + 255) / 256 * 256;
+  // LevelGeom::swap_off counts 16-byte units back from a level's I0 (inside the image block): an int reaches 32 GB
+  if ((marks + sizeof(float) * ctx->images_floats) / 16 > (size_t)INT_MAX) {
+    ofdis_destroy(ctx);
+    return OFDIS_ERR_UNSUPPORTED;
+  }
+  bool ok = dalloc((void**)&ctx->d_swapped, marks + sizeof(float) * ctx->frame_floats * cap);
+  if (ok) {
+    ctx->d_img = reinterpret_cast<float*>(ctx->d_swapped + marks);
+    cudaMemsetAsync(ctx->d_swapped, 0, marks, ctx->stream);
+  }
   ctx->d_flow.assign(ctx->nlev + 1, nullptr);
   ctx->flow_floats.assign(ctx->nlev + 1, 0);
   for (int li = 0; li <= ctx->nlev && ok; ++li) {
@@ -356,6 +373,8 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
       L.img[k] = ctx->d_img + ctx->img_off[(size_t)li * 4 + k];
       L.img_fs[k] = ctx->frame_floats;
     }
+    // marks (a multiple of 256 bytes) and every array offset (a multiple of 4 floats) are 16-byte multiples
+    L.swap_off = ok ? -(int)((marks + sizeof(float) * ctx->img_off[(size_t)li * 4]) / 16) : 0;
     L.flow = ctx->d_flow[li];
     L.flow_frame_stride = ctx->flow_floats[li];
     L.flow_prev = ctx->d_flow[li + 1];
@@ -397,7 +416,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaSetDevice(ctx->device);
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
   for (auto& kv : ctx->graphs) cudaGraphExecDestroy(kv.second);
-  cudaFree(ctx->d_img);
+  cudaFree(ctx->d_swapped);  // d_img lies in the same allocation
   cudaFree(ctx->d_stage);
   cudaFree(ctx->d_full);
   for (float* p : ctx->d_flow) cudaFree(p);
@@ -538,15 +557,19 @@ int ofdis_upload_packed_images(ofdis_ctx* ctx, int f0, int f1, const float* pack
   return finish_gradients(ctx, f0, f1);
 }
 
-// Coarser levels by 2x2 box means (forward frames), then finish_gradients.  seq: the pairs hold consecutive
-// frames (ofdis_upload_sequence_u8), each frame's levels are built once.
-static int finish_pyramid(ofdis_ctx* ctx, int f0, int f1, bool seq = false) {
+// Coarser levels by 2x2 box means (forward frames), then finish_gradients.  SEQ: the pairs hold consecutive
+// frames (ofdis_upload_sequence_u8), BIDIR: the forward and the backward pairs of consecutive frames in two halves
+// (ofdis_upload_sequence_bidir_u8); each frame's levels are built once.
+enum PyramidSource { PAIRS, SEQ, BIDIR };
+static int finish_pyramid(ofdis_ctx* ctx, int f0, int f1, PyramidSource src = PAIRS) {
   NvtxRange nvtx("pyramid", -1);
   const int D = ctx->dirs, q0 = f0 * D, nq = f1 - f0;
   for (int sl = ctx->prm.sc_l + 1; sl <= ctx->prm.sc_f; ++sl) {
     const LevelGeom gs = stepped(ctx->lev[sl - 1 - ctx->prm.sc_l], D), gd = stepped(ctx->lev[sl - ctx->prm.sc_l], D);
-    if ((seq ? launch_pyr_down_seq(gs, gd, q0, nq, ctx->stream) : launch_pyr_down(gs, gd, q0, q0 + nq, ctx->stream)) < 0)
-      return fail(ctx, OFDIS_ERR_CUDA, "pyr_down_kernel launch", cudaGetLastError());
+    const int rc = src == SEQ     ? launch_pyr_down_seq(gs, gd, q0, nq, ctx->stream)
+                   : src == BIDIR ? launch_pyr_down_bidir(gs, gd, q0, nq / 2, ctx->stream)
+                                  : launch_pyr_down(gs, gd, q0, q0 + nq, ctx->stream);
+    if (rc < 0) return fail(ctx, OFDIS_ERR_CUDA, "pyr_down_kernel launch", cudaGetLastError());
     ctx->launches += 1;
   }
   return finish_gradients(ctx, f0, f1);
@@ -628,7 +651,51 @@ int ofdis_upload_sequence_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char
   if (launch_pyr_from_u8_seq(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, n, src, ctx->stream) < 0)
     return fail(ctx, OFDIS_ERR_CUDA, "pyr_from_u8_kernel launch", cudaGetLastError());
   ctx->launches += 1;
-  return finish_pyramid(ctx, f0, f1, true);
+  return finish_pyramid(ctx, f0, f1, SEQ);
+}
+
+int ofdis_upload_sequence_bidir_u8(ofdis_ctx* ctx, int f0, int n, const unsigned char* frames, int width_org,
+                                   int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || n < 1 || n > ctx->max_frames || f0 > ctx->max_frames - 2 * n || !frames)
+    return fail(ctx, OFDIS_ERR_ARG, "upload_sequence_bidir_u8: bad argument");
+  if (ctx->prm.sc_l > 8) return fail(ctx, OFDIS_ERR_UNSUPPORTED, "upload_sequence_bidir_u8: box sums are exact in float32 up to level 8");
+  PyrSourceU8 src;
+  int rc = org_padding(ctx, width_org, height_org, &src.pad_left, &src.pad_top);
+  if (rc) return rc;
+  CK(cudaSetDevice(ctx->device));
+  NvtxRange nvtx("upload", -1);
+  src.w_org = width_org;
+  src.h_org = height_org;
+  src.image_bytes = (size_t)width_org * height_org * ctx->prm.noc;
+  src.frames = frames;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    // the staging size of ofdis_upload_frames_u8; n + 1 <= max_frames / 2 + 1 frames fit
+    rc = ensure_stage(ctx, src.image_bytes * 2 * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(ctx->d_stage, frames, src.image_bytes * (size_t)(n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    src.frames = static_cast<const unsigned char*>(ctx->d_stage);
+  }
+  const int D = ctx->dirs;
+  if (launch_pyr_from_u8_bidir(stepped(ctx->lev[0], D), f0 * D, n, src, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "pyr_from_u8_kernel launch", cudaGetLastError());
+  ctx->launches += 1;
+  rc = finish_pyramid(ctx, f0, f0 + 2 * n, BIDIR);
+  if (rc) return rc;
+  // only once the pyramids are enqueued: the backward half runs as the right camera (stereo)
+  CK(cudaMemsetAsync(ctx->d_swapped + (size_t)f0 * D, 0, (size_t)n * D, ctx->stream));
+  CK(cudaMemsetAsync(ctx->d_swapped + (size_t)(f0 + n) * D, 1, (size_t)n * D, ctx->stream));
+  return OFDIS_OK;
+}
+
+int ofdis_set_swapped_slots(ofdis_ctx* ctx, int f0, int f1, int swapped) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || (swapped != 0 && swapped != 1))
+    return fail(ctx, OFDIS_ERR_ARG, "set_swapped_slots: bad argument");
+  CK(cudaSetDevice(ctx->device));
+  // stream-ordered: runs enqueued before keep the marks they were enqueued with; graphs read the marks at replay
+  CK(cudaMemsetAsync(ctx->d_swapped + (size_t)f0 * ctx->dirs, swapped, (size_t)(f1 - f0) * ctx->dirs, ctx->stream));
+  return OFDIS_OK;
 }
 
 size_t ofdis_finest_level_frame_floats(const ofdis_ctx* ctx) {
@@ -753,6 +820,41 @@ int ofdis_get_flow_fullres(ofdis_ctx* ctx, int f0, int f1, float* out, int width
   ctx->launches += 1;
   if (memkind != OFDIS_MEM_DEVICE)
     CK(cudaMemcpyAsync(out, dst, sizeof(float) * per * (size_t)(f1 - f0), cudaMemcpyDeviceToHost, ctx->stream));
+  return OFDIS_OK;
+}
+
+int ofdis_consistency_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, unsigned char* mask, float* err, float alpha,
+                              float beta, int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || b0 < 0 || b0 > ctx->max_frames - (f1 - f0) || !mask ||
+      !(alpha >= 0.f && alpha <= FLT_MAX) || !(beta >= 0.f && beta <= FLT_MAX))
+    return fail(ctx, OFDIS_ERR_ARG, "consistency_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("consistency", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0;
+  const size_t pix = (size_t)width_org * height_org;
+  unsigned char* dmask = mask;
+  float* derr = err;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    // the full-resolution scratch: err (if asked for) then the mask; sized for max_frames, and at least what
+    // ofdis_get_flow_fullres asks for, so that alternating the two never reallocates
+    rc = ensure_full(ctx, std::max(pix * ctx->nop, (pix * 5 + 3) / 4) * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    derr = err ? ctx->d_full : nullptr;
+    dmask = reinterpret_cast<unsigned char*>(ctx->d_full + (err ? pix * n : 0));
+  }
+  const int D = ctx->dirs;
+  if (launch_consistency(stepped(ctx->lev[0], D), f0 * D, b0 * D, n, dmask, derr, width_org, height_org, cx, cy, alpha,
+                         beta, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "consistency_kernel launch", cudaGetLastError());
+  ctx->launches += 1;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    CK(cudaMemcpyAsync(mask, dmask, pix * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (err) CK(cudaMemcpyAsync(err, derr, sizeof(float) * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
+  }
   return OFDIS_OK;
 }
 

@@ -15,11 +15,26 @@ namespace {
 // is exact in int32 and (for l <= 8) in float32, so it equals l successive cv::resize(0.5) steps.
 // The divisibility padding (replicate, floor(pad/2) left/top) and the per-level border padding
 // (replicate, g.pad) are folded into the index clamps.  One thread per padded destination pixel.
-// SEQ = false: s.frames = [pair][2][..], grid.z = 2 x pairs (pair, side).  SEQ = true: s.frames = [n + 1][..]
+// PYR_PAIRS: s.frames = [pair][2][..], grid.z = 2 x pairs (pair, side).  PYR_SEQ: s.frames = [n + 1][..]
 // consecutive frames, grid.z = n + 1; frame t is computed once and stored as I0 of pair t (t < n) and as I1 of
-// pair t - 1 (t >= 1).
-template <bool SEQ>
+// pair t - 1 (t >= 1).  PYR_BIDIR: as PYR_SEQ, and also as I0 of the backward pair n + t - 1 (t >= 1) and as I1 of
+// the backward pair n + t (t < n), pair n + t holding (frame t + 1, frame t).
+enum PyrMode { PYR_PAIRS, PYR_SEQ, PYR_BIDIR };
+
+// PYR_BIDIR: the element at offset o of frame t in the pairs that hold it, nullptr where a pair does not exist:
+// I0 of pair t, I1 of pair t - 1, I0 of backward pair n + t - 1, I1 of backward pair n + t
+__device__ __forceinline__ void bidir_dsts(const LevelGeom& g, int f0, int n, int t, size_t o, float* d[4]) {
+  float* i0 = const_cast<float*>(g.img[0]) + o;
+  float* i1 = const_cast<float*>(g.img[3]) + o;
+  d[0] = t < n ? i0 + (size_t)frame_of(g, f0, t) * g.img_fs[0] : nullptr;
+  d[1] = t >= 1 ? i1 + (size_t)frame_of(g, f0, t - 1) * g.img_fs[3] : nullptr;
+  d[2] = t >= 1 ? i0 + (size_t)frame_of(g, f0, n + t - 1) * g.img_fs[0] : nullptr;
+  d[3] = t < n ? i1 + (size_t)frame_of(g, f0, n + t) * g.img_fs[3] : nullptr;
+}
+
+template <int MODE>
 __global__ void __launch_bounds__(256) pyr_from_u8_kernel(LevelGeom g, int f0, PyrSourceU8 s, int n) {
+  constexpr bool SEQ = MODE != PYR_PAIRS;
   pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
   const int xp = blockIdx.x * blockDim.x + threadIdx.x, yp = blockIdx.y * blockDim.y + threadIdx.y;
   if (xp >= g.tmp_w || yp >= g.tmp_h) return;
@@ -38,13 +53,21 @@ __global__ void __launch_bounds__(256) pyr_from_u8_kernel(LevelGeom g, int f0, P
       for (int c = 0; c < C; ++c) sum[c] += (int)__ldg(row + X * C + c);
     }
   }
-  if constexpr (SEQ) {
+  if constexpr (MODE == PYR_SEQ) {
     float* d0 = fr < n ? const_cast<float*>(g.img[0]) + (size_t)frame_of(g, f0, fr) * g.img_fs[0] + o : nullptr;
     float* d1 = fr >= 1 ? const_cast<float*>(g.img[3]) + (size_t)frame_of(g, f0, fr - 1) * g.img_fs[3] + o : nullptr;
     for (int c = 0; c < C; ++c) {
       const float v = (float)sum[c] * scale;
       if (d0) d0[c] = v;
       if (d1) d1[c] = v;
+    }
+  } else if constexpr (MODE == PYR_BIDIR) {
+    float* d[4];
+    bidir_dsts(g, f0, n, fr, o, d);
+    for (int c = 0; c < C; ++c) {
+      const float v = (float)sum[c] * scale;
+      for (int j = 0; j < 4; ++j)
+        if (d[j]) d[j][c] = v;
     }
   } else {
     const int arr = k ? 3 : 0;
@@ -68,10 +91,10 @@ __global__ void __launch_bounds__(256) pyr_from_level_kernel(LevelGeom g, int f0
 
 // cv::resize(0.5, 0.5, INTER_LINEAR) of an even-sized image == 2x2 box mean (run_dense.cpp:150),
 // ((a+b)+(c+d))*0.25 with a,b the even row; reads the interior of the padded level gs, writes
-// level gd = gs+1 including its replicate border.  SEQ as in pyr_from_u8_kernel: frame t of the n + 1
+// level gd = gs+1 including its replicate border.  MODE as in pyr_from_u8_kernel: frame t of the n + 1
 // consecutive frames reads its finer level from the pair that holds it (I0 of pair t, or I1 of pair n - 1 for
-// the last frame) and writes both pairs that hold it.
-template <bool SEQ>
+// the last frame) and writes every pair that holds it.
+template <int MODE>
 __global__ void __launch_bounds__(256) pyr_down_kernel(LevelGeom gs, LevelGeom gd, int f0, int n) {
   pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
   const int xp = blockIdx.x * blockDim.x + threadIdx.x, yp = blockIdx.y * blockDim.y + threadIdx.y;
@@ -80,7 +103,18 @@ __global__ void __launch_bounds__(256) pyr_down_kernel(LevelGeom gs, LevelGeom g
   const size_t o = ((size_t)yp * gd.tmp_w + xp) * C;
   const int x = clampi(xp - gd.pad, gd.w), y = clampi(yp - gd.pad, gd.h);
   const size_t so = ((size_t)(2 * y + gs.pad) * gs.tmp_w + (2 * x + gs.pad)) * C;
-  if constexpr (SEQ) {
+  if constexpr (MODE == PYR_BIDIR) {
+    const int t = blockIdx.z, sa = t < n ? 0 : 3, sf = t < n ? t : t - 1;
+    const float* r0 = gs.img[sa] + (size_t)frame_of(gd, f0, sf) * gs.img_fs[sa] + so;
+    const float* r1 = r0 + (size_t)gs.tmp_w * C;
+    float* d[4];
+    bidir_dsts(gd, f0, n, t, o, d);
+    for (int c = 0; c < C; ++c) {
+      const float v = ((r0[c] + r0[C + c]) + (r1[c] + r1[C + c])) * 0.25f;
+      for (int j = 0; j < 4; ++j)
+        if (d[j]) d[j][c] = v;
+    }
+  } else if constexpr (MODE == PYR_SEQ) {
     const int t = blockIdx.z, sa = t < n ? 0 : 3, sf = t < n ? t : t - 1;
     const float* r0 = gs.img[sa] + (size_t)frame_of(gd, f0, sf) * gs.img_fs[sa] + so;
     const float* r1 = r0 + (size_t)gs.tmp_w * C;
@@ -140,20 +174,16 @@ __global__ void __launch_bounds__(256) sobel_kernel(LevelGeom g, int f0) {
 
 // Output stage of run_dense.cpp:407-414: flow * 2^lv_l, cv::resize(x 2^lv_l, INTER_LINEAR)
 // (src = (dst + .5)/s - .5, edge clamped, horizontal pass first), crop of the divisibility
-// padding.  One thread per full-resolution pixel; expression order of preprocess.upsample_linear.
-template <int NOP>
-__global__ void __launch_bounds__(256) flow_upsample_kernel(LevelGeom g, int f0, float* out, int w_org, int h_org,
-                                                            int crop_x, int crop_y) {
-  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
-  const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (X >= w_org || Y >= h_org) return;
-  const int fr = blockIdx.z;
-  const float* fl = g.flow + (size_t)frame_of(g, f0, fr) * g.flow_frame_stride;
-  float* o = out + ((size_t)fr * h_org * w_org + (size_t)Y * w_org + X) * NOP;
+// padding; expression order of preprocess.upsample_linear.  The value of every channel c of the
+// full-resolution pixel (X, Y) of level flow `fl`, cropped by (crop_x, crop_y), goes to emit(c, value), channel
+// after channel.
+template <int NOP, typename Emit>
+__device__ __forceinline__ void upsample_at(const LevelGeom& g, const float* fl, int X, int Y, int crop_x, int crop_y,
+                                            Emit emit) {
   const int s = 1 << g.level;
   if (s == 1) {
     const float* q = fl + ((size_t)(Y + crop_y) * g.w + (X + crop_x)) * NOP;
-    for (int c = 0; c < NOP; ++c) o[c] = q[c];
+    for (int c = 0; c < NOP; ++c) emit(c, q[c]);
     return;
   }
   const float fs = (float)s;
@@ -174,8 +204,69 @@ __global__ void __launch_bounds__(256) flow_upsample_kernel(LevelGeom g, int f0,
     const float a00 = fl[((size_t)ya * g.w + xa) * NOP + c] * fs, a01 = fl[((size_t)ya * g.w + xb) * NOP + c] * fs;
     const float a10 = fl[((size_t)yb * g.w + xa) * NOP + c] * fs, a11 = fl[((size_t)yb * g.w + xb) * NOP + c] * fs;
     const float r0 = a00 * gx + a01 * fx, r1 = a10 * gx + a11 * fx;
-    o[c] = r0 * gy + r1 * fy;
+    emit(c, r0 * gy + r1 * fy);
   }
+}
+
+// One thread per full-resolution pixel.
+template <int NOP>
+__global__ void __launch_bounds__(256) flow_upsample_kernel(LevelGeom g, int f0, float* out, int w_org, int h_org,
+                                                            int crop_x, int crop_y) {
+  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
+  const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (X >= w_org || Y >= h_org) return;
+  const int fr = blockIdx.z;
+  const float* fl = g.flow + (size_t)frame_of(g, f0, fr) * g.flow_frame_stride;
+  float* o = out + ((size_t)fr * h_org * w_org + (size_t)Y * w_org + X) * NOP;
+  upsample_at<NOP>(g, fl, X, Y, crop_x, crop_y, [o](int c, float v) { o[c] = v; });
+}
+
+// Forward-backward (flow) / left-right (stereo) consistency (Sundaram, Brox, Keutzer, ECCV 2010) of frame fa's
+// full-resolution flow F against frame fb's B, both exactly what flow_upsample_kernel writes, evaluated from the
+// level flows (upsample_at) where they are needed instead of through a full-resolution copy.  Per pixel, in
+// float32 without contraction (preprocess.consistency_check restates it):
+//   (xs, ys) = (x, y) + F(x, y); outside [0, w_org-1] x [0, h_org-1] (or NaN): mask 2, err +inf;
+//   b = B bilinear at (xs, ys) (corners x0 = floor(xs), x1 = min(x0 + 1, w_org - 1), horizontal pass first);
+//   err = |F + b|^2, mask = err <= alpha (|F|^2 + |b|^2) + beta ? 0 : 1.
+// One thread per full-resolution pixel; err may be nullptr.
+template <int NOP>
+__global__ void __launch_bounds__(256) consistency_kernel(LevelGeom g, int fa, int fb, unsigned char* mask, float* err,
+                                                          int w_org, int h_org, int crop_x, int crop_y, float alpha,
+                                                          float beta) {
+  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
+  const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (X >= w_org || Y >= h_org) return;
+  const int fr = blockIdx.z;
+  const float* F = g.flow + (size_t)frame_of(g, fa, fr) * g.flow_frame_stride;
+  const float* B = g.flow + (size_t)frame_of(g, fb, fr) * g.flow_frame_stride;
+  const size_t o = (size_t)fr * h_org * w_org + (size_t)Y * w_org + X;
+  float f[2] = {0.f, 0.f};
+  upsample_at<NOP>(g, F, X, Y, crop_x, crop_y, [&f](int c, float v) { f[c] = v; });
+  const float u = f[0], v = NOP == 2 ? f[1] : 0.f;
+  const float xs = (float)X + u, ys = (float)Y + v;
+  if (!(xs >= 0.f && xs <= (float)(w_org - 1) && ys >= 0.f && ys <= (float)(h_org - 1))) {
+    mask[o] = 2;
+    if (err) err[o] = __int_as_float(0x7f800000);
+    return;
+  }
+  const int x0 = (int)floorf(xs), y0 = (int)floorf(ys);
+  const int x1 = min(x0 + 1, w_org - 1), y1 = min(y0 + 1, h_org - 1);
+  const float fx = xs - (float)x0, fy = ys - (float)y0, gx = 1.0f - fx, gy = 1.0f - fy;
+  float c00[2], c10[2], c01[2], c11[2];
+  upsample_at<NOP>(g, B, x0, y0, crop_x, crop_y, [&c00](int c, float v) { c00[c] = v; });
+  upsample_at<NOP>(g, B, x1, y0, crop_x, crop_y, [&c10](int c, float v) { c10[c] = v; });
+  upsample_at<NOP>(g, B, x0, y1, crop_x, crop_y, [&c01](int c, float v) { c01[c] = v; });
+  upsample_at<NOP>(g, B, x1, y1, crop_x, crop_y, [&c11](int c, float v) { c11[c] = v; });
+  float b[2] = {0.f, 0.f};
+  for (int c = 0; c < NOP; ++c) {
+    const float r0 = c00[c] * gx + c10[c] * fx, r1 = c01[c] * gx + c11[c] * fx;
+    b[c] = r0 * gy + r1 * fy;
+  }
+  const float du = u + b[0], dv = NOP == 2 ? v + b[1] : 0.f;
+  const float e = du * du + dv * dv;
+  const float mag = (u * u + v * v) + (b[0] * b[0] + b[1] * b[1]);
+  mask[o] = e <= alpha * mag + beta ? 0 : 1;
+  if (err) err[o] = e;
 }
 
 // Init flow of the reference's disabled file input (run_dense.cpp:355-378): the full-resolution flow
@@ -253,12 +344,17 @@ int launch_sobel(const LevelGeom& g, int f0, int f1, cudaStream_t st) {
 }
 
 int launch_pyr_from_u8(const LevelGeom& g, int f0, int f1, const PyrSourceU8& s, cudaStream_t st) {
-  pyr_from_u8_kernel<false><<<padded_grid(g, 2 * (f1 - f0)), dim3(32, 8), 0, st>>>(g, f0, s, 0);
+  pyr_from_u8_kernel<PYR_PAIRS><<<padded_grid(g, 2 * (f1 - f0)), dim3(32, 8), 0, st>>>(g, f0, s, 0);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
 int launch_pyr_from_u8_seq(const LevelGeom& g, int f0, int n, const PyrSourceU8& s, cudaStream_t st) {
-  pyr_from_u8_kernel<true><<<padded_grid(g, n + 1), dim3(32, 8), 0, st>>>(g, f0, s, n);
+  pyr_from_u8_kernel<PYR_SEQ><<<padded_grid(g, n + 1), dim3(32, 8), 0, st>>>(g, f0, s, n);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_pyr_from_u8_bidir(const LevelGeom& g, int f0, int n, const PyrSourceU8& s, cudaStream_t st) {
+  pyr_from_u8_kernel<PYR_BIDIR><<<padded_grid(g, n + 1), dim3(32, 8), 0, st>>>(g, f0, s, n);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -268,12 +364,17 @@ int launch_pyr_from_level(const LevelGeom& g, int f0, int f1, const float* stage
 }
 
 int launch_pyr_down(const LevelGeom& gs, const LevelGeom& gd, int f0, int f1, cudaStream_t st) {
-  pyr_down_kernel<false><<<padded_grid(gd, 2 * (f1 - f0)), dim3(32, 8), 0, st>>>(gs, gd, f0, 0);
+  pyr_down_kernel<PYR_PAIRS><<<padded_grid(gd, 2 * (f1 - f0)), dim3(32, 8), 0, st>>>(gs, gd, f0, 0);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
 int launch_pyr_down_seq(const LevelGeom& gs, const LevelGeom& gd, int f0, int n, cudaStream_t st) {
-  pyr_down_kernel<true><<<padded_grid(gd, n + 1), dim3(32, 8), 0, st>>>(gs, gd, f0, n);
+  pyr_down_kernel<PYR_SEQ><<<padded_grid(gd, n + 1), dim3(32, 8), 0, st>>>(gs, gd, f0, n);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_pyr_down_bidir(const LevelGeom& gs, const LevelGeom& gd, int f0, int n, cudaStream_t st) {
+  pyr_down_kernel<PYR_BIDIR><<<padded_grid(gd, n + 1), dim3(32, 8), 0, st>>>(gs, gd, f0, n);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -282,6 +383,16 @@ int launch_flow_upsample(const LevelGeom& g, int f0, int f1, float* out, int w_o
   const dim3 block(32, 8), grid((w_org + 31) / 32, (h_org + 7) / 8, f1 - f0);
   if (g.nop == 2) flow_upsample_kernel<2><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
   else flow_upsample_kernel<1><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_consistency(const LevelGeom& g, int fa, int fb, int n, unsigned char* mask, float* err, int w_org,
+                       int h_org, int crop_x, int crop_y, float alpha, float beta, cudaStream_t st) {
+  const dim3 block(32, 8), grid((w_org + 31) / 32, (h_org + 7) / 8, n);
+  if (g.nop == 2)
+    consistency_kernel<2><<<grid, block, 0, st>>>(g, fa, fb, mask, err, w_org, h_org, crop_x, crop_y, alpha, beta);
+  else
+    consistency_kernel<1><<<grid, block, 0, st>>>(g, fa, fb, mask, err, w_org, h_org, crop_x, crop_y, alpha, beta);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

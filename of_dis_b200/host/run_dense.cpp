@@ -544,16 +544,49 @@ int main(int argc, char** argv) {
 // (ofdis_set_initflow_from_result); the first pair of a chain starts from zero.  Each output equals what the
 // single-pair binary writes given `1 <previous output>` (an all-zero flow for a chain's first pair).  Chaining makes
 // a clip serial, so this mode trades throughput for the warm start.
+//
+// --bidirectional: every pair also runs backward (image2 -> image1; stereo: the right view's disparity, as the
+// right camera), in the same launch.  A chained batch goes up with ofdis_upload_sequence_bidir_u8, any other batch
+// as its pairs followed by their swapped copies (marked with ofdis_set_swapped_slots).  For an output path
+// <stem><ext> it writes <stem><ext> (the forward flow, the same bytes as without the flag), <stem>_bw<ext> (the
+// backward flow / right disparity) and <stem>_occ.pgm, the forward slot's consistency mask
+// (ofdis_consistency_fullres with alpha 0.01, beta 0.5 for flow and 0, 1 for stereo) as binary PGM: 0 consistent,
+// 255 inconsistent, 128 the flow leaves the frame.
+
+// <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
+static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
+  const size_t slash = path.find_last_of('/'), dot = path.find_last_of('.');
+  const size_t cut = (dot != string::npos && (slash == string::npos || dot > slash)) ? dot : path.size();
+  return path.substr(0, cut) + suffix + (new_ext ? string(new_ext) : path.substr(cut));
+}
+
+static void save_mask_pgm(const uint8_t* mask, int w, int h, const char* filename) {
+  FILE* f = fopen(filename, "wb");
+  if (!f) {
+    cout << "WriteFile: could not open file" << endl;
+    return;
+  }
+  static const uint8_t level[3] = {0, 255, 128};
+  vector<uint8_t> px((size_t)w * h);
+  for (size_t i = 0; i < px.size(); ++i) px[i] = level[mask[i] < 3 ? mask[i] : 1];
+  fprintf(f, "P5\n%d %d\n255\n", w, h);
+  if (fwrite(px.data(), 1, px.size(), f) != px.size()) cout << "WriteFile: problem writing data" << endl;
+  fclose(f);
+}
+
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr,
-            "usage: %s listfile [--batch N | --warm-start] [oppoint | 20 parameters (README.md:66-88)]\n"
+            "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
-            "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n", argv[0]);
+            "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
+            "  --bidirectional: also the backward flow (stereo: the right view's disparity) of every pair, written to\n"
+            "  <stem>_bw<ext>, and the forward-backward consistency mask to <stem>_occ.pgm (0 consistent,\n"
+            "  255 inconsistent, 128 leaves the frame); not with --warm-start\n", argv[0]);
     return 2;
   }
   int maxb = 64, first_num = 2;
-  bool warm = false, batch_set = false;
+  bool warm = false, batch_set = false, bidir = false;
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -562,12 +595,19 @@ int main(int argc, char** argv) {
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--warm-start")) {
       warm = true;
       first_num += 1;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--bidirectional")) {
+      bidir = true;
+      first_num += 1;
     } else {
       break;
     }
   }
   if (warm && batch_set) {
     fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --batch\n");
+    return 2;
+  }
+  if (warm && bidir) {
+    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --bidirectional\n");
     return 2;
   }
   if (warm) maxb = 1;
@@ -597,6 +637,7 @@ int main(int argc, char** argv) {
   int ctx_w = -1, ctx_h = -1, verbosity = 0;
   vector<uint8_t> frames;
   vector<float> flows;
+  vector<uint8_t> masks;
   Image8 last;  // image2 of the previous batch's last pair
   size_t j0 = 0;
   while (j0 < jobs.size()) {
@@ -644,6 +685,10 @@ int main(int argc, char** argv) {
         frames.insert(frames.end(), imgs[ia[k]].px.begin(), imgs[ia[k]].px.end());
         frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
       }
+      for (int k = 0; k < n && bidir; ++k) {  // the swapped copies
+        frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
+        frames.insert(frames.end(), imgs[ia[k]].px.begin(), imgs[ia[k]].px.end());
+      }
     }
     last = std::move(imgs[ib.back()]);
     CliParams P;
@@ -662,7 +707,7 @@ int main(int argc, char** argv) {
       p.tv_innerit = P.tv_innerit; p.tv_solverit = P.tv_solverit; p.tv_sor = P.tv_sor; p.verbosity = P.verbosity;
       const int scf = 1 << (warm ? P.lv_f + 1 : P.lv_f);
       const int rc = ofdis_create(&ctx, 0, nullptr, &p, nop, (w + scf - 1) / scf * scf, (h + scf - 1) / scf * scf,
-                                  P.patchsz, maxb);
+                                  P.patchsz, bidir ? 2 * maxb : maxb);
       if (rc != OFDIS_OK) {
         fprintf(stderr, "error: ofdis_create failed with status %d for %dx%d frames\n", rc, w, h);
         return 1;
@@ -671,15 +716,30 @@ int main(int argc, char** argv) {
       ctx_w = w;
       ctx_h = h;
     }
-    flows.resize((size_t)n * w * h * nop);
-    int rc = seq ? ofdis_upload_sequence_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST)
-                 : ofdis_upload_frames_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
+    const int slots = bidir ? 2 * n : n;  // bidirectional: forward slots [0, n), backward slots [n, 2n)
+    flows.resize((size_t)slots * w * h * nop);
+    int rc;
+    if (bidir && seq) {
+      rc = ofdis_upload_sequence_bidir_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
+    } else if (bidir) {
+      rc = ofdis_upload_frames_u8(ctx, 0, 2 * n, frames.data(), w, h, OFDIS_MEM_HOST);
+      if (rc == OFDIS_OK) rc = ofdis_set_swapped_slots(ctx, 0, n, 0);
+      if (rc == OFDIS_OK) rc = ofdis_set_swapped_slots(ctx, n, 2 * n, 1);
+    } else {
+      rc = seq ? ofdis_upload_sequence_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST)
+               : ofdis_upload_frames_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
+    }
     // warm start: the context still holds the previous pair's flow (same size, so it was not recreated)
     const bool from_prev = warm && j0 > 0 && jobs[j0].a == jobs[j0 - 1].b;
     if (rc == OFDIS_OK && from_prev) rc = ofdis_set_initflow_from_result(ctx, 0, 1, 0, w, h);
     warm_pairs += from_prev ? 1 : 0;
-    if (rc == OFDIS_OK) rc = ofdis_run(ctx, n, from_prev ? 1 : 0);
-    if (rc == OFDIS_OK) rc = ofdis_get_flow_fullres(ctx, 0, n, flows.data(), w, h, OFDIS_MEM_HOST);
+    if (rc == OFDIS_OK) rc = ofdis_run(ctx, slots, from_prev ? 1 : 0);
+    if (rc == OFDIS_OK) rc = ofdis_get_flow_fullres(ctx, 0, slots, flows.data(), w, h, OFDIS_MEM_HOST);
+    if (rc == OFDIS_OK && bidir) {
+      masks.resize((size_t)n * w * h);
+      rc = ofdis_consistency_fullres(ctx, 0, n, n, masks.data(), nullptr, nop == 2 ? 0.01f : 0.0f,
+                                     nop == 2 ? 0.5f : 1.0f, w, h, OFDIS_MEM_HOST);
+    }
     if (rc == OFDIS_OK) rc = ofdis_sync(ctx);
     if (rc != OFDIS_OK) {
       fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
@@ -692,6 +752,12 @@ int main(int argc, char** argv) {
       out.px.assign(flows.begin() + (size_t)k * w * h * nop, flows.begin() + (size_t)(k + 1) * w * h * nop);
       if (SELECTMODE == 1) SaveFlowFile(out, jobs[j0 + k].out.c_str());
       else SavePFMFile(out, jobs[j0 + k].out.c_str());
+      if (!bidir) continue;
+      out.px.assign(flows.begin() + (size_t)(n + k) * w * h * nop, flows.begin() + (size_t)(n + k + 1) * w * h * nop);
+      const string bw = with_suffix(jobs[j0 + k].out, "_bw");
+      if (SELECTMODE == 1) SaveFlowFile(out, bw.c_str());
+      else SavePFMFile(out, bw.c_str());
+      save_mask_pgm(masks.data() + (size_t)k * w * h, w, h, with_suffix(jobs[j0 + k].out, "_occ", ".pgm").c_str());
     }
     j0 += n;
     done += n;

@@ -159,6 +159,68 @@ def postprocess(flow_level: np.ndarray, lv_l: int, padw: int, padh: int, width_o
     return np.ascontiguousarray(out[y0:y0 + height_org, x0:x0 + width_org])
 
 
+def consistency_check(fw: np.ndarray, bw: np.ndarray, alpha: float, beta: float):
+    """Forward-backward (flow) / left-right (stereo) consistency (Sundaram, Brox, Keutzer, ECCV 2010) of the
+    full-resolution flow `fw` against its partner `bw`, both (h, w, nop) or (h, w) float32; the restatement of
+    ofdis_consistency_fullres, float32 throughout, evaluated in this order without contraction:
+
+        (xs, ys) = (x, y) + F(x, y)                    (stereo: ys = y)
+        outside [0, w-1] x [0, h-1], or NaN:  mask 2, err +inf
+        x0 = floor(xs), x1 = min(x0 + 1, w - 1), fx = xs - x0 (and y); b = bilinear B at (xs, ys), rows first:
+            r0 = B(x0,y0) (1-fx) + B(x1,y0) fx,  r1 = B(x0,y1) (1-fx) + B(x1,y1) fx,  b = r0 (1-fy) + r1 fy
+        err = du^2 + dv^2 with (du, dv) = F + b;  mag = (u^2 + v^2) + (b0^2 + b1^2)
+        mask = 0 if err <= alpha mag + beta else 1
+
+    Returns (mask uint8 (h, w), err float32 (h, w))."""
+    f32 = np.float32
+    F = np.asarray(fw, f32)
+    B = np.asarray(bw, f32)
+    F = F.reshape(F.shape[:2] + (-1,))
+    B = B.reshape(B.shape[:2] + (-1,))
+    h, w, nop = F.shape
+    assert B.shape == F.shape
+    u = F[..., 0]
+    v = F[..., 1] if nop == 2 else np.zeros_like(u)
+    with np.errstate(invalid="ignore", over="ignore"):
+        xs = np.arange(w, dtype=f32)[None, :] + u
+        ys = np.arange(h, dtype=f32)[:, None] + v
+        inside = (xs >= 0) & (xs <= f32(w - 1)) & (ys >= 0) & (ys <= f32(h - 1))
+        xc = np.where(inside, xs, f32(0))
+        yc = np.where(inside, ys, f32(0))
+        x0 = np.floor(xc).astype(np.int64)
+        y0 = np.floor(yc).astype(np.int64)
+        x1 = np.minimum(x0 + 1, w - 1)
+        y1 = np.minimum(y0 + 1, h - 1)
+        fx = (xc - x0.astype(f32)).astype(f32)
+        fy = (yc - y0.astype(f32)).astype(f32)
+        gx, gy = f32(1) - fx, f32(1) - fy
+        b = []
+        for c in range(nop):
+            Bc = B[..., c]
+            r0 = Bc[y0, x0] * gx + Bc[y0, x1] * fx
+            r1 = Bc[y1, x0] * gx + Bc[y1, x1] * fx
+            b.append(r0 * gy + r1 * fy)
+        b0 = b[0]
+        b1 = b[1] if nop == 2 else np.zeros_like(u)
+        du = u + b0
+        dv = v + b1 if nop == 2 else np.zeros_like(u)
+        err = du * du + dv * dv
+        mag = (u * u + v * v) + (b0 * b0 + b1 * b1)
+        mask = np.where(err <= f32(alpha) * mag + f32(beta), 0, 1).astype(np.uint8)
+    mask[~inside] = 2
+    err = np.where(inside, err, f32(np.inf)).astype(f32)
+    return mask, err
+
+
+def write_pgm(path: str, img: np.ndarray) -> None:
+    """Binary PGM (P5), maxval 255: an (h, w) uint8 image, rows top-down."""
+    img = np.ascontiguousarray(img, np.uint8)
+    h, w = img.shape[:2]
+    with open(path, "wb") as f:
+        f.write(b"P5\n%d %d\n255\n" % (w, h))
+        f.write(img.reshape(h, w).tobytes())
+
+
 def write_flo(path: str, flow: np.ndarray) -> None:
     """SaveFlowFile (run_dense.cpp:16-57): 'PIEH', int32 w, int32 h, float32 row-major."""
     h, w = flow.shape[:2]
