@@ -174,6 +174,34 @@ int ofdis_set_swapped_slots(ofdis_ctx* ctx, int f0, int f1, int swapped);
  * host output goes through the context's full-resolution scratch.  The flows are not changed. */
 int ofdis_consistency_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, unsigned char* mask, float* err, float alpha,
                               float beta, int width_org, int height_org, int memkind);
+/* Error statistics of one (pair, class) of ofdis_flow_error_fullres (48 bytes). */
+typedef struct ofdis_error_stats {
+  long long n;          /* pixels counted */
+  long long n_over[3];  /* e > 1, e > 3, e > 5 */
+  long long n_outlier;  /* e > 3.0f && e > 0.05f * g   (KITTI Fl / D1, evaluated in float32 as written) */
+  double sum_err;       /* sum of e, in the fixed order below */
+} ofdis_error_stats;
+/* Evaluation against ground truth (extension) of the last run's slots [f0, f1) at the original frame size.  F is slot
+ * a's full-resolution flow, exactly what ofdis_get_flow_fullres returns (computed from the level flows, without a
+ * full-resolution copy); gt = G, [f1-f0][height_org][width_org][nop] float32 in this library's convention (stereo: the
+ * disparity sign ofdis_get_flow_fullres returns).  In float32 without contraction:
+ *   known ground truth: flow G_u, G_v not NaN and |G_u|, |G_v| <= 1e9 (Middlebury's UNKNOWN_FLOW_THRESH, so infinities
+ *     are unknown); stereo G not NaN and |G| <= 1e9;
+ *   flow: du = F_u - G_u, dv = F_v - G_v, e = sqrtf(du*du + dv*dv), g = sqrtf(G_u*G_u + G_v*G_v);
+ *   stereo: e = fabsf(F - G), g = fabsf(G);
+ *   err (optional, the same shape without nop): e where the ground truth is known, else the quiet NaN 0x7fc00000;
+ *   a pixel counts for (pair, class c) when its ground truth is known and c = classes[pixel] < nclasses (classes:
+ *     [f1-f0][height_org][width_org] bytes; NULL means class 0), so a byte of nclasses or more (e.g. 255) is ignored.
+ * stats = [f1-f0][nclasses], always host memory.  Counts are exact.  sum_err is summed in this fixed order: per row y a
+ * float64 sum starts at +0.0 and adds (double)e of the row's counted pixels of the class with x ascending; a float64
+ * total starts at +0.0 and adds the row sums with y ascending.  NaN flows are not special-cased: a NaN e counts, makes
+ * sum_err NaN and fails every > test.  gt, classes and err are in memkind (host ones go through the context's
+ * full-resolution scratch); classes and err may be NULL.  Slots inside the context, non-NULL gt and stats,
+ * 1 <= nclasses <= 16, classes non-NULL when nclasses > 1, else OFDIS_ERR_ARG; frame sizes as ofdis_get_flow_fullres
+ * checks them.  The flows are not changed.  Synchronises the context's stream before it returns. */
+int ofdis_flow_error_fullres(ofdis_ctx* ctx, int f0, int f1, const float* gt, const unsigned char* classes,
+                             int nclasses, ofdis_error_stats* stats, float* err, int width_org, int height_org,
+                             int memkind);
 size_t ofdis_finest_level_frame_floats(const ofdis_ctx* ctx);
 int ofdis_upload_finest_level(ofdis_ctx* ctx, int f0, int f1, const float* packed, int memkind);
 

@@ -33,11 +33,14 @@ EXPORTS = [
     "ofdis_get_level", "ofdis_upload_level_fb", "ofdis_set_option", "ofdis_profile_levels", "ofdis_set_direction",
     "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8", "ofdis_set_initflow_fullres",
     "ofdis_set_initflow_from_result", "ofdis_upload_sequence_bidir_u8", "ofdis_set_swapped_slots",
-    "ofdis_consistency_fullres",
+    "ofdis_consistency_fullres", "ofdis_flow_error_fullres",
 ]
 
 # default thresholds of consistency_fullres: flow (Sundaram, Brox, Keutzer, ECCV 2010) and stereo (|d_L + d_R| <= 1)
 CONSISTENCY_DEFAULTS = {2: (0.01, 0.5), 1: (0.0, 1.0)}
+
+# ofdis_error_stats (include/ofdis_b200.h), field for field: counts of one (pair, class) of flow_error_fullres
+ERROR_STATS_DTYPE = np.dtype([("n", "<i8"), ("n_over", "<i8", (3,)), ("n_outlier", "<i8"), ("sum_err", "<f8")])
 
 
 class OfdisError(RuntimeError):
@@ -85,6 +88,8 @@ def lib():
         L.ofdis_set_swapped_slots.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3
         L.ofdis_consistency_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 2 + \
             [ctypes.c_float] * 2 + [ctypes.c_int] * 3
+        L.ofdis_flow_error_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 2 + \
+            [ctypes.c_int] + [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
         L.ofdis_get_flow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
@@ -264,6 +269,38 @@ class Context:
         if memkind == MEM_HOST:
             self.sync()
         return mask, err
+
+    def flow_error_fullres(self, f0, f1, gt, width_org, height_org, classes=None, nclasses=None, with_err=False,
+                           memkind=MEM_HOST, err=None):
+        """Evaluation of the last run's slots [f0, f1) against ground truth at the original frame size
+        (preprocess.flow_error on the device, bitwise).  gt: [f1-f0][height_org][width_org][nop] float32 (stereo also
+        without the last axis); classes: [f1-f0][height_org][width_org] uint8, e.g. a consistency mask (then nclasses
+        is required; without classes it is 1).  Returns (stats, err): stats a (f1-f0, nclasses) array of
+        ERROR_STATS_DTYPE, err the float32 error map (NaN where the ground truth is unknown), None unless with_err
+        (host: a new array, or `err` given as a numpy array of exactly that shape).  With memkind=MEM_DEVICE, gt,
+        classes and err are device addresses the caller owns (err None: no map); stats are always returned on the
+        host.  The call synchronises the context's stream."""
+        if nclasses is None:
+            if classes is not None:
+                raise ValueError("flow_error_fullres: nclasses is required with classes")
+            nclasses = 1
+        shape = (f1 - f0, height_org, width_org)
+        if memkind == MEM_HOST:
+            nop = self.prm.nop
+            gt_shapes = (shape + (nop,),) + ((shape,) if nop == 1 else ())
+            err = (np.empty(shape, np.float32) if err is None else err) if with_err else None
+            for name, arr, dt, shapes, write in (("gt", gt, np.float32, gt_shapes, False),
+                                                 ("classes", classes, np.uint8, (shape,), False),
+                                                 ("err", err, np.float32, (shape,), True)):
+                if arr is not None and not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape in shapes
+                                            and arr.flags["C_CONTIGUOUS"] and (arr.flags["WRITEABLE"] or not write)):
+                    raise ValueError("flow_error_fullres: %s must be a %sC-contiguous %s array of shape %s"
+                                     % (name, "writeable " if write else "", np.dtype(dt).name,
+                                        " or ".join(map(str, shapes))))
+        stats = np.zeros((max(f1 - f0, 0), max(nclasses, 0)), ERROR_STATS_DTYPE)
+        self._ck(lib().ofdis_flow_error_fullres(self._h, f0, f1, _ptr(gt), _ptr(classes), nclasses, _ptr(stats),
+                                                _ptr(err), width_org, height_org, memkind))
+        return stats, err
 
     def get_flow_fullres(self, f0, f1, dst, width_org, height_org, memkind=MEM_HOST):
         """Flow x 2^sc_l, upsampled to the original frame size and cropped (run_dense.cpp:407-414)."""

@@ -63,6 +63,9 @@ struct ofdis_ctx {
   size_t stage_bytes = 0;
   float* d_full = nullptr;
   size_t full_floats = 0;
+  // lazily allocated workspace of ofdis_flow_error_fullres: the row partials [max_frames][16][height], then the
+  // device stats [max_frames][16]; never touched by ofdis_run
+  ErrRowPartial* d_eval = nullptr;
   std::vector<float*> d_flow;      // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -419,6 +422,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_swapped);  // d_img lies in the same allocation
   cudaFree(ctx->d_stage);
   cudaFree(ctx->d_full);
+  cudaFree(ctx->d_eval);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -855,6 +859,64 @@ int ofdis_consistency_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, unsigned c
     CK(cudaMemcpyAsync(mask, dmask, pix * n, cudaMemcpyDeviceToHost, ctx->stream));
     if (err) CK(cudaMemcpyAsync(err, derr, sizeof(float) * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
   }
+  return OFDIS_OK;
+}
+
+static constexpr int kEvalMaxClasses = 16;
+
+int ofdis_flow_error_fullres(ofdis_ctx* ctx, int f0, int f1, const float* gt, const unsigned char* classes,
+                             int nclasses, ofdis_error_stats* stats, float* err, int width_org, int height_org,
+                             int memkind) {
+  static_assert(sizeof(ofdis_error_stats) == 48, "ofdis_error_stats: 48 bytes, as api.ERROR_STATS_DTYPE");
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !gt || !stats || nclasses < 1 || nclasses > kEvalMaxClasses ||
+      (!classes && nclasses > 1))
+    return fail(ctx, OFDIS_ERR_ARG, "flow_error_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("evaluate", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0;
+  const size_t pix = (size_t)width_org * height_org, nop = (size_t)ctx->nop;
+  // the workspace: row partials for max_frames x 16 classes x the level-0 rows, then the device stats
+  const size_t part_count = (size_t)ctx->max_frames * kEvalMaxClasses * ctx->height;
+  if (!ctx->d_eval &&
+      cudaMalloc((void**)&ctx->d_eval, sizeof(ErrRowPartial) * part_count +
+                                           sizeof(ofdis_error_stats) * ctx->max_frames * kEvalMaxClasses) != cudaSuccess) {
+    ctx->d_eval = nullptr;
+    return fail(ctx, OFDIS_ERR_NOMEM, "flow_error_fullres workspace");
+  }
+  ofdis_error_stats* dstats = reinterpret_cast<ofdis_error_stats*>(ctx->d_eval + part_count);
+  const float* dgt = gt;
+  const unsigned char* dcls = classes;
+  float* derr = err;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    // the full-resolution scratch: gt, err (if asked for), then the classes (if given); sized for max_frames
+    rc = ensure_full(ctx, (pix * (nop + 1) + (pix + 3) / 4) * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    float* s = ctx->d_full;
+    CK(cudaMemcpyAsync(s, gt, sizeof(float) * pix * nop * n, cudaMemcpyHostToDevice, ctx->stream));
+    dgt = s;
+    s += pix * nop * n;
+    if (err) {
+      derr = s;
+      s += pix * n;
+    }
+    if (classes) {
+      CK(cudaMemcpyAsync(s, classes, pix * n, cudaMemcpyHostToDevice, ctx->stream));
+      dcls = reinterpret_cast<const unsigned char*>(s);
+    }
+  }
+  const int D = ctx->dirs;
+  if (launch_flow_error(stepped(ctx->lev[0], D), f0 * D, n, dgt, dcls, nclasses, derr, ctx->d_eval, dstats, width_org,
+                        height_org, cx, cy, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "flow_error_kernel launch", cudaGetLastError());
+  ctx->launches += 2;
+  if (memkind != OFDIS_MEM_DEVICE && err)
+    CK(cudaMemcpyAsync(err, derr, sizeof(float) * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(stats, dstats, sizeof(ofdis_error_stats) * n * nclasses, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
   return OFDIS_OK;
 }
 

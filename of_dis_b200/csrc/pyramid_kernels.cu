@@ -269,6 +269,111 @@ __global__ void __launch_bounds__(256) consistency_kernel(LevelGeom g, int fa, i
   if (err) err[o] = e;
 }
 
+// Evaluation of frame f0 + fr's full-resolution flow F (upsample_at, as flow_upsample_kernel writes it) against the
+// ground truth G of ofdis_flow_error_fullres (header, and preprocess.flow_error), float32 without contraction:
+//   known = G not NaN and |G| <= 1e9 per component; e = sqrtf(du*du + dv*dv) (stereo fabsf(F - G)), g = |G| likewise;
+//   err = known ? e : qNaN; the pixel counts for class classes[pixel] (0 without classes) if known and < nclasses.
+// One CTA of EV_THREADS per (row, pair).  The row goes through shared memory in chunks of EV_CHUNK pixels: every
+// thread computes EV_CHUNK / EV_THREADS of them (coalesced), then thread c < nclasses walks the chunk with x ascending
+// and adds class c's errors to its float64 row sum -- the fixed order of the contract -- and its counts.
+constexpr int EV_THREADS = 256, EV_CHUNK = 1024, EV_MAX_CLASSES = 16;
+constexpr unsigned char EV_SKIP = 0xff;  // the pixel counts for no class
+
+template <int NOP>
+__global__ void __launch_bounds__(EV_THREADS) flow_error_kernel(LevelGeom g, int f0, const float* gt,
+                                                                const unsigned char* classes, int nclasses, float* err,
+                                                                ErrRowPartial* part, int w_org, int h_org, int crop_x,
+                                                                int crop_y) {
+  __shared__ float se[EV_CHUNK];
+  __shared__ unsigned char sk[EV_CHUNK], sf[EV_CHUNK];  // class (EV_SKIP: none) and flags (bit k: test k true)
+  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
+  const int Y = blockIdx.x, fr = blockIdx.y, t = threadIdx.x;
+  const float* fl = g.flow + (size_t)frame_of(g, f0, fr) * g.flow_frame_stride;
+  const size_t row = ((size_t)fr * h_org + Y) * w_org;
+  const float unknown_thresh = 1e9f;
+  double sum = 0.0;
+  unsigned int cnt[5] = {0, 0, 0, 0, 0};
+  for (int x0 = 0; x0 < w_org; x0 += EV_CHUNK) {
+    const int m = min(EV_CHUNK, w_org - x0);
+    for (int i = t; i < m; i += EV_THREADS) {
+      const int X = x0 + i;
+      const size_t o = row + X;
+      float f[2] = {0.f, 0.f};
+      upsample_at<NOP>(g, fl, X, Y, crop_x, crop_y, [&f](int c, float v) { f[c] = v; });
+      float e, gm;
+      bool known;
+      if constexpr (NOP == 2) {
+        const float Gu = gt[2 * o], Gv = gt[2 * o + 1];  // a caller's device array may be only 4-byte aligned
+        known = fabsf(Gu) <= unknown_thresh && fabsf(Gv) <= unknown_thresh;  // NaN fails both
+        const float du = f[0] - Gu, dv = f[1] - Gv;
+        e = sqrtf(du * du + dv * dv);
+        gm = sqrtf(Gu * Gu + Gv * Gv);
+      } else {
+        const float G = gt[o];
+        known = fabsf(G) <= unknown_thresh;
+        e = fabsf(f[0] - G);
+        gm = fabsf(G);
+      }
+      if (err) err[o] = known ? e : __int_as_float(0x7fc00000);
+      const int k = classes ? classes[o] : 0;
+      se[i] = e;
+      sk[i] = known && k < nclasses ? (unsigned char)k : EV_SKIP;
+      sf[i] = (e > 1.0f ? 1 : 0) | (e > 3.0f ? 2 : 0) | (e > 5.0f ? 4 : 0) | (e > 3.0f && e > 0.05f * gm ? 8 : 0);
+    }
+    __syncthreads();
+    if (t < nclasses) {
+      for (int i = 0; i < m; ++i) {
+        const bool mine = sk[i] == t;
+        const unsigned int fl8 = sf[i];
+        sum += mine ? (double)se[i] : 0.0;  // + 0.0 leaves a sum of non-negative terms as it is
+        cnt[0] += mine ? 1u : 0u;
+        for (int b = 0; b < 4; ++b) cnt[b + 1] += mine ? (fl8 >> b) & 1u : 0u;
+      }
+    }
+    __syncthreads();
+  }
+  if (t < nclasses) {
+    ErrRowPartial& p = part[((size_t)fr * nclasses + t) * h_org + Y];
+    p.sum = sum;
+    for (int b = 0; b < 5; ++b) p.n[b] = cnt[b];
+  }
+}
+
+// Sums the row partials of one (pair, class) -- blockIdx.x = pair * nclasses + class -- with y ascending: the threads
+// stage EV_THREADS rows at a time in shared memory, thread 0 adds them in order.
+__global__ void __launch_bounds__(EV_THREADS) flow_error_reduce_kernel(const ErrRowPartial* part, int h_org,
+                                                                       ofdis_error_stats* stats) {
+  __shared__ double ss[EV_THREADS];
+  __shared__ unsigned int sn[5][EV_THREADS];
+  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
+  const ErrRowPartial* p = part + (size_t)blockIdx.x * h_org;
+  const int t = threadIdx.x;
+  double total = 0.0;
+  long long cnt[5] = {0, 0, 0, 0, 0};
+  for (int y0 = 0; y0 < h_org; y0 += EV_THREADS) {
+    const int m = min(EV_THREADS, h_org - y0);
+    if (t < m) {
+      ss[t] = p[y0 + t].sum;
+      for (int b = 0; b < 5; ++b) sn[b][t] = p[y0 + t].n[b];
+    }
+    __syncthreads();
+    if (t == 0) {
+      for (int i = 0; i < m; ++i) {
+        total += ss[i];
+        for (int b = 0; b < 5; ++b) cnt[b] += sn[b][i];
+      }
+    }
+    __syncthreads();
+  }
+  if (t == 0) {
+    ofdis_error_stats& s = stats[blockIdx.x];
+    s.n = cnt[0];
+    for (int b = 0; b < 3; ++b) s.n_over[b] = cnt[b + 1];
+    s.n_outlier = cnt[4];
+    s.sum_err = total;
+  }
+}
+
 // Init flow of the reference's disabled file input (run_dense.cpp:355-378): the full-resolution flow
 // [frame][h_org][w_org][NOP], replicate-padded to the context (clamped reads, floor(pad/2) left/top), times
 // 2^-(sc_f+1), then cv::resize(INTER_AREA) by the integer factor s = 2^(sc_f+1).  That is OpenCV's area-fast path:
@@ -393,6 +498,20 @@ int launch_consistency(const LevelGeom& g, int fa, int fb, int n, unsigned char*
     consistency_kernel<2><<<grid, block, 0, st>>>(g, fa, fb, mask, err, w_org, h_org, crop_x, crop_y, alpha, beta);
   else
     consistency_kernel<1><<<grid, block, 0, st>>>(g, fa, fb, mask, err, w_org, h_org, crop_x, crop_y, alpha, beta);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_flow_error(const LevelGeom& g, int f0, int n, const float* gt, const unsigned char* classes, int nclasses,
+                      float* err, ErrRowPartial* part, ofdis_error_stats* stats, int w_org, int h_org, int crop_x,
+                      int crop_y, cudaStream_t st) {
+  if (nclasses < 1 || nclasses > EV_MAX_CLASSES) return -1;
+  const dim3 grid(h_org, n);
+  if (g.nop == 2)
+    flow_error_kernel<2><<<grid, EV_THREADS, 0, st>>>(g, f0, gt, classes, nclasses, err, part, w_org, h_org, crop_x, crop_y);
+  else
+    flow_error_kernel<1><<<grid, EV_THREADS, 0, st>>>(g, f0, gt, classes, nclasses, err, part, w_org, h_org, crop_x, crop_y);
+  if (cudaGetLastError() != cudaSuccess) return -1;
+  flow_error_reduce_kernel<<<n * nclasses, EV_THREADS, 0, st>>>(part, h_org, stats);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

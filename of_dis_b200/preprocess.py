@@ -212,6 +212,74 @@ def consistency_check(fw: np.ndarray, bw: np.ndarray, alpha: float, beta: float)
     return mask, err
 
 
+UNKNOWN_FLOW_THRESH = 1e9  # Middlebury's flow-io: a ground-truth component above this (or NaN) is unknown
+_QNAN = np.uint32(0x7FC00000).view(np.float32)
+
+
+def flow_error(flow: np.ndarray, gt: np.ndarray, classes: np.ndarray | None = None, nclasses: int = 1):
+    """End-point error of full-resolution flows against ground truth, per pixel and per class; the restatement of
+    ofdis_flow_error_fullres, float32 without contraction:
+
+        known      flow: G_u, G_v not NaN and |G_u|, |G_v| <= 1e9;  stereo: G not NaN and |G| <= 1e9
+        e, g       flow: e = sqrt(du^2 + dv^2) with (du, dv) = F - G, g = sqrt(G_u^2 + G_v^2);  stereo: |F - G|, |G|
+        map        e where known, else the quiet NaN 0x7fc00000
+        counted    for class c: known and classes == c (classes None: every pixel is class 0), c < nclasses
+        counts     n, e > 1, e > 3, e > 5, outliers e > 3 and e > 0.05 g
+        sum_err    per row a float64 sum from +0.0 adds (double) e of the row's counted pixels with x ascending (+0.0
+                   for the others); the total from +0.0 adds the row sums with y ascending
+
+    flow and gt: one pair (h, w, nop) or (h, w) (stereo), or a batch (n, h, w, nop); classes uint8 of the same shape
+    without nop.  Returns (stats, err): stats of api.ERROR_STATS_DTYPE, (nclasses,) for one pair or (n, nclasses) for a
+    batch, and the float32 map (h, w) or (n, h, w)."""
+    from .api import ERROR_STATS_DTYPE
+
+    f32 = np.float32
+    F = np.asarray(flow, f32)
+    G = np.asarray(gt, f32)
+    assert F.shape == G.shape, (F.shape, G.shape)
+    single = F.ndim in (2, 3)
+    if F.ndim == 2:
+        F, G = F[..., None], G[..., None]
+    if single:
+        F, G = F[None], G[None]
+    n, h, w, nop = F.shape
+    assert nop in (1, 2) and 1 <= nclasses
+    cls = np.zeros((n, h, w), np.uint8) if classes is None else np.asarray(classes, np.uint8).reshape(n, h, w)
+    assert classes is not None or nclasses == 1
+    with np.errstate(invalid="ignore", over="ignore"):
+        lim = f32(UNKNOWN_FLOW_THRESH)
+        if nop == 2:
+            known = (np.abs(G[..., 0]) <= lim) & (np.abs(G[..., 1]) <= lim)
+            du, dv = F[..., 0] - G[..., 0], F[..., 1] - G[..., 1]
+            e = np.sqrt(du * du + dv * dv)
+            g = np.sqrt(G[..., 0] * G[..., 0] + G[..., 1] * G[..., 1])
+        else:
+            known = np.abs(G[..., 0]) <= lim
+            e = np.abs(F[..., 0] - G[..., 0])
+            g = np.abs(G[..., 0])
+        tests = (e > f32(1), e > f32(3), e > f32(5), (e > f32(3)) & (e > f32(0.05) * g))
+    err = np.where(known, e, _QNAN).astype(f32)
+    stats = np.zeros((n, nclasses), ERROR_STATS_DTYPE)
+    for p in range(n):
+        for c in range(nclasses):
+            counted = known[p] & (cls[p] == c)
+            st = stats[p, c]
+            st["n"] = int(counted.sum())
+            st["n_over"] = [int((counted & t[p]).sum()) for t in tests[:3]]
+            st["n_outlier"] = int((counted & tests[3][p]).sum())
+            terms = np.where(counted, e[p].astype(np.float64), 0.0)
+            rows = np.zeros(h, np.float64)
+            for x in range(w):  # x ascending, every row at once
+                rows = rows + terms[:, x]
+            total = 0.0
+            for y in range(h):
+                total += float(rows[y])
+            st["sum_err"] = total
+    if single:
+        return stats[0], err[0]
+    return stats, err
+
+
 def write_pgm(path: str, img: np.ndarray) -> None:
     """Binary PGM (P5), maxval 255: an (h, w) uint8 image, rows top-down."""
     img = np.ascontiguousarray(img, np.uint8)
