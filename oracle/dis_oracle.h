@@ -47,6 +47,19 @@ int dis_patches_level(const dis_level* L, const dis_params* prm, const float* i0
                       const float* i0y, const float* i1, const float* flow_prev, float* p_out,
                       float* pweight_out, int* conv_out, int* cnt_out);
 
+/* Data-dependent fallbacks of PatClass::ComputeHessian + Eigen LLT (patch.cpp:71-88), as bits:
+ * flow, det H == 0 with H00 == 0 / with H00 > 0 (both diagonals get +1e-10); flow, the Cholesky pivot
+ * H11 - L10^2 <= 0 (L11 keeps H11); stereo, H00 == 0. */
+#define DIS_HESS_SINGULAR_ZERO 1
+#define DIS_HESS_SINGULAR 2
+#define DIS_HESS_NOT_PD 4
+#define DIS_HESS_STEREO_ZERO 8
+
+/* Test query, no result of the run depends on it: for every patch of the level (ip order) the
+ * DIS_HESS_* bits its Hessian took into branch_out[np].  Returns np. */
+int dis_patches_level_branches(const dis_level* L, const dis_params* prm, const float* i0, const float* i0x,
+                               const float* i0y, int* branch_out);
+
 /* K4: densification (patchgrid.cpp:213-275,377-394). flow_out[h*w*nop] interleaved. */
 void dis_densify(const dis_level* L, const dis_params* prm, const float* p, const float* pweight,
                  float* flow_out);

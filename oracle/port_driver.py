@@ -71,6 +71,20 @@ def port_level_patches(pyr, prm, level: int, flow_prev=None, want_dense=True):
     return dict(p=p, pweight=pw, conv=conv, cnt=cnt, dense=dense, nopw=L.nopw, noph=L.noph)
 
 
+# bits of dis_patches_level_branches (oracle/dis_oracle.h): the Hessian fallbacks of the patch stage
+HESS_SINGULAR_ZERO, HESS_SINGULAR, HESS_NOT_PD, HESS_STEREO_ZERO = 1, 2, 4, 8
+
+
+def port_level_branches(pyr, prm, level: int) -> np.ndarray:
+    """Per patch of the level (ip order), the HESS_* bits of the Hessian fallbacks its template takes."""
+    L = make_level(pyr, prm, level)
+    cp = prm.to_c()
+    out = np.zeros(L.nopw * L.noph, np.int32)
+    lib().dis_patches_level_branches(ctypes.byref(L), ctypes.byref(cp), _fp(pyr.i0[level]), _fp(pyr.i0x[level]),
+                                     _fp(pyr.i0y[level]), out.ctypes.data_as(_IP))
+    return out
+
+
 def port_densify(pyr, prm, level: int, p, pweight):
     L = make_level(pyr, prm, level)
     cp = prm.to_c()

@@ -44,9 +44,27 @@ def write_digests(out_dir):
         out["baseline_%s_input" % name] = t.input_digest(i0, i1)
         out["baseline_" + name] = t.digest(ref_driver.ref_run(pyr, prm))
     out.update(sor_division_digests())
+    out.update(degenerate_digests())
     with open(os.path.join(out_dir, "reference_digests.json"), "w") as f:
         json.dump(out, f, indent=1, sort_keys=True)
         f.write("\n")
+
+
+def degenerate_digests():
+    """The degenerate image families of tests/test_degenerate_content_gpu.py on every parameter set there: input
+    pair, whole run, the patch stage at sc_l without and with the coarser flow, and the refinement of sc_l."""
+    import test_oracle as t
+    from test_degenerate_content_gpu import CASES, degenerate_inputs
+
+    out = {}
+    for family, route in CASES:
+        i0, i1, pyr, prm = degenerate_inputs(family, route)
+        key = "degen_%s_%s" % (family, route)
+        out[key + "_input"] = t.input_digest(i0, i1)
+        out[key + "_run"] = t.digest(ref_driver.ref_run(pyr, prm))
+        out[key + "_patches"], out[key + "_varref"] = t.degenerate_stage(ref_driver.ref_level_patches,
+                                                                         ref_driver.ref_level_varref, pyr, prm)
+    return out
 
 def sor_division_digests():
     """The stereo SOR's division regimes (tests/test_sor_division_gpu.py: parameters that drive A11 and B1 out of the

@@ -13,6 +13,8 @@ import pytest
 
 from of_dis_b200 import params, preprocess, synth
 from oracle import ref_driver
+from test_degenerate_content_gpu import CASE_IDS as DEGEN_IDS, CASES as DEGEN_CASES, ROUTES as DEGEN_ROUTES
+from test_degenerate_content_gpu import coarser_flow, degenerate_inputs, stage_params
 from test_sor_division_gpu import DIV_CASES, REGIMES, division_inputs, initial_disparity
 
 GOLDEN_DIR = os.path.join(os.path.dirname(__file__), "golden")
@@ -191,6 +193,79 @@ def test_port_vs_reference_at_the_sor_division_regimes(case, regime, oracle_port
     assert digest(oracle_port.port_run(pyr, prm)) == REF_DIGESTS[key + "_run"]
     fl = initial_disparity(regime, pyr, prm)
     assert digest(oracle_port.port_level_varref(pyr, prm, prm.sc_l, fl)) == REF_DIGESTS[key + "_varref"]
+
+
+# ---- degenerate content (tests/test_degenerate_content_gpu.py) ---------------------------------------------------
+def patches_digest(levels):
+    """SHA-256 of the bits of p, pweight, conv, cnt and dense of each patch-stage result in `levels`, in turn"""
+    h = hashlib.sha256()
+    for lvl in levels:
+        for k in ("p", "pweight", "conv", "cnt", "dense"):
+            h.update(np.ascontiguousarray(lvl[k]).tobytes())
+    return h.hexdigest()
+
+
+def degenerate_stage(drv_patches, drv_varref, pyr, prm):
+    """The per-stage checks of a degenerate case with one driver: the patch stage at sc_l without and with the
+    coarser flow, and the refinement of sc_l from the dense flow of the latter."""
+    sprm = stage_params(prm)
+    lv = [drv_patches(pyr, sprm, prm.sc_l, f) for f in (None, coarser_flow(pyr, prm))]
+    return patches_digest(lv), digest(drv_varref(pyr, sprm, prm.sc_l, lv[1]["dense"]))
+
+
+@pytest.mark.parametrize("family,route", DEGEN_CASES, ids=DEGEN_IDS)
+def test_port_vs_reference_on_degenerate_content(family, route, oracle_port):
+    """The inputs of tests/test_degenerate_content_gpu.py (flat, striped, checkerboard, noise, saturated and mixed
+    frames): the whole run, the patch stage at sc_l and the refinement of sc_l, bit for bit as the reference build
+    computes them; where oracle/_ref exists also the run against the reference build directly."""
+    i0, i1, pyr, prm = degenerate_inputs(family, route)
+    key = "degen_%s_%s" % (family, route)
+    check_inputs(key, i0, i1)
+    run = oracle_port.port_run(pyr, prm)
+    assert digest(run) == REF_DIGESTS[key + "_run"]
+    patches, varref = degenerate_stage(oracle_port.port_level_patches, oracle_port.port_level_varref, pyr, prm)
+    assert patches == REF_DIGESTS[key + "_patches"]
+    assert varref == REF_DIGESTS[key + "_varref"]
+    if ref_driver.ref_available(prm.flavour()):
+        assert np.array_equal(bits(ref_driver.ref_run(pyr, prm)), bits(run))
+
+
+# at least this many patches of every patch kernel's parameter sets take each fallback, and stop at cnt == 0
+BRANCH_FLOOR = 50
+
+
+def test_degenerate_content_reaches_the_hessian_fallbacks_on_every_patch_kernel(oracle_port):
+    """Without this the GPU tests of degenerate content could pass while testing nothing: per patch kernel (P = 8 gray
+    at 8 and 4 lanes per patch, P = 12, generic), the cases' patches at sc_l take each Hessian fallback (flow: A
+    det H == 0 with H00 == 0, B det H == 0 with H00 > 0, C Cholesky pivot <= 0; stereo: D H00 == 0) and stop at
+    cnt == 0 at least BRANCH_FLOOR times.  A patch without gradients (A, D) never moves (dp == 0), so where
+    min_iter < max_iter it stops at cnt == min_iter on the ratio test 0 / 0: that too, at least BRANCH_FLOOR times.
+    And the mixed frame holds, in one warp's aligned group of four patches, a fallback patch beside a regular one,
+    and a patch that stops at once beside one that iterates."""
+    pd = oracle_port
+    counts = {k[0]: dict(A=0, B=0, C=0, D=0, cnt0=0, ratio00=0) for k in DEGEN_ROUTES.values()}
+    for family, route in DEGEN_CASES:
+        _, _, pyr, prm = degenerate_inputs(family, route)
+        br = pd.port_level_branches(pyr, prm, prm.sc_l)
+        cnt = pd.port_level_patches(pyr, stage_params(prm), prm.sc_l, None, want_dense=False)["cnt"]
+        c = counts[DEGEN_ROUTES[route][0]]
+        c["A"] += int((br & pd.HESS_SINGULAR_ZERO != 0).sum())
+        c["B"] += int((br & pd.HESS_SINGULAR != 0).sum())
+        c["C"] += int((br & pd.HESS_NOT_PD != 0).sum())
+        c["D"] += int((br & pd.HESS_STEREO_ZERO != 0).sum())
+        c["cnt0"] += int((cnt == 0).sum())
+        if 0 < prm.min_iter < prm.max_iter:
+            still = (br & (pd.HESS_SINGULAR_ZERO | pd.HESS_STEREO_ZERO) != 0) & (cnt == prm.min_iter)
+            c["ratio00"] += int(still.sum())
+        if family == "mixed":
+            n4 = br.size // 4 * 4
+            g_br, g_cnt = br[:n4].reshape(-1, 4), cnt[:n4].reshape(-1, 4)
+            both = ((g_br != 0).any(1) & (g_br == 0).any(1)).sum()
+            stop = ((g_cnt == 0).any(1) & (g_cnt > 0).any(1)).sum()
+            assert both > 0 and stop > 0, (route, both, stop)
+    for kernel, c in counts.items():
+        for k, v in c.items():
+            assert v >= BRANCH_FLOOR, "%s: %s reached %d times only (%s)" % (kernel, k, v, c)
 
 
 @pytest.mark.skipif(not ref_driver.ref_available("m1c1"), reason="oracle/_ref not built")
