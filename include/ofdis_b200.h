@@ -69,9 +69,14 @@ enum {
   OFDIS_OK = 0,
   OFDIS_ERR_ARG = -1,         /* bad argument / unsupported geometry */
   OFDIS_ERR_CUDA = -2,        /* a CUDA call failed; see ofdis_last_error */
-  OFDIS_ERR_UNSUPPORTED = -3, /* valid in the reference but not built here (a finest refinement level of more than 16384 rows, refused by ofdis_create before it touches a device; ofdis_upload_packed with usefbcon) */
+  OFDIS_ERR_UNSUPPORTED = -3, /* valid in the reference but not built here (a finest refinement level of more than 16384 rows, or more frames than OFDIS_MAX_GRID_FRAMES allows, refused by ofdis_create before it touches a device; ofdis_upload_packed with usefbcon) */
   OFDIS_ERR_NOMEM = -4
 };
+/* Kernels put the frames of a launch in a grid dimension of at most 65535 blocks: ofdis_create refuses
+ * max_frames * max(2, dirs * noc) > OFDIS_MAX_GRID_FRAMES (dirs = 2 with usefbcon, else 1) with
+ * OFDIS_ERR_UNSUPPORTED.  The largest contexts are 32767 frames (gray, or usefbcon gray), 21845 (RGB) and
+ * 10922 (usefbcon RGB). */
+enum { OFDIS_MAX_GRID_FRAMES = 65535 };
 enum { OFDIS_MEM_HOST = 0, OFDIS_MEM_DEVICE = 1 };
 
 /* nop: 2 = optical flow (run_OF_*), 1 = stereo disparity (run_DE_*).
@@ -269,6 +274,15 @@ int ofdis_debug_div(ofdis_ctx* ctx, const float* a, const float* b, long n, floa
  * sor_wave_kernel and pixel updates of a warp of sor_lane_kernel (0 on ordinary inputs: their operands stay in range).
  * Synchronises the context's stream; reset != 0 zeroes the count after reading it. */
 int ofdis_debug_sor_div_fallbacks(ofdis_ctx* ctx, unsigned long long* count, int reset);
+/* Test hook, no context and no CUDA call: the launch plan ofdis_varref_refine takes for a w x h level of a nop / noc
+ * context with tv_solverit = solverit, `frames` internal frames per launch (pairs, x 2 with usefbcon) and the SOR
+ * options "sor_lane", "sor_fast", "sor_rows_per_thread", "sor_single_max", "sor_max_cluster" (ofdis_set_option).
+ * out[9]: kind (0 sor_wave_kernel one CTA per frame, 1 a cluster of bands, 2 a chain of bands, 3 sor_lane_kernel,
+ * 4 sor_redblack_kernel), lanes per band (sor_wave_kernel), rows per lane, lane-row slots of a stage, bands, sweeps
+ * per launch, sweeps of the shorter last launch (0: none), rows per thread of assemble_kernel, assemble_kernel's
+ * record layout (0 band lanes, 1 natural, 2 sor_lane_kernel's).  OFDIS_ERR_UNSUPPORTED where no plan exists. */
+int ofdis_debug_sor_plan(int w, int h, int nop, int noc, int solverit, int frames, int lane, int fast, int rt,
+                         int single_max, int max_cluster, int* out);
 
 /* Number of kernels this library has launched on the context since creation. */
 long ofdis_launch_count(const ofdis_ctx* ctx);

@@ -33,8 +33,12 @@ EXPORTS = [
     "ofdis_get_level", "ofdis_upload_level_fb", "ofdis_set_option", "ofdis_profile_levels", "ofdis_set_direction",
     "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8", "ofdis_set_initflow_fullres",
     "ofdis_set_initflow_from_result", "ofdis_upload_sequence_bidir_u8", "ofdis_set_swapped_slots",
-    "ofdis_consistency_fullres", "ofdis_flow_error_fullres",
+    "ofdis_consistency_fullres", "ofdis_flow_error_fullres", "ofdis_debug_sor_plan",
 ]
+
+# kind of ofdis_debug_sor_plan (SorKind)
+SOR_KINDS = ("wave_single", "wave_cluster", "wave_chain", "lane", "redblack")
+SOR_PLAN_FIELDS = ("kind", "hpad", "rt", "ml", "nb", "sweeps", "tail_sweeps", "assemble_rows", "assemble_mode")
 
 # default thresholds of consistency_fullres: flow (Sundaram, Brox, Keutzer, ECCV 2010) and stereo (|d_L + d_R| <= 1)
 CONSISTENCY_DEFAULTS = {2: (0.01, 0.5), 1: (0.0, 1.0)}
@@ -105,6 +109,7 @@ def lib():
         L.ofdis_debug_varref_iters.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 4
         L.ofdis_debug_div.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_long] + [ctypes.c_void_p] * 3
         L.ofdis_debug_sor_div_fallbacks.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_ulonglong), ctypes.c_int]
+        L.ofdis_debug_sor_plan.argtypes = [ctypes.c_int] * 11 + [_IP]
         L.ofdis_run.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
         L.ofdis_get_flow.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
         L.ofdis_set_flow.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
@@ -120,6 +125,20 @@ def lib():
         L.ofdis_profile_levels.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
         _lib = L
     return _lib
+
+
+def debug_sor_plan(w, h, nop, noc, solverit, frames, lane=2, fast=0, rt=1, single_max=128, max_cluster=8):
+    """The refinement's launch plan of a w x h level for `frames` internal frames per launch (ofdis_debug_sor_plan;
+    no device needed): a dict of SOR_PLAN_FIELDS, kind named by SOR_KINDS, or None where no plan exists."""
+    out = (ctypes.c_int * len(SOR_PLAN_FIELDS))()
+    rc = lib().ofdis_debug_sor_plan(w, h, nop, noc, solverit, frames, lane, fast, rt, single_max, max_cluster, out)
+    if rc == -3:
+        return None
+    if rc != 0:
+        raise OfdisError("debug_sor_plan: status %d" % rc)
+    d = dict(zip(SOR_PLAN_FIELDS, list(out)))
+    d["kind"] = SOR_KINDS[d["kind"]]
+    return d
 
 
 def _ptr(a):

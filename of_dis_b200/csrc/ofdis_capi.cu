@@ -280,6 +280,9 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
   if (prm->usetvref && ((height >> prm->sc_f) < 4 || (width >> prm->sc_f) < 2)) return OFDIS_ERR_ARG;  // image.c:401-434 needs >= 4 rows
   // tallest refinement level: SOR_MAX_ROWS (levels beyond the largest cluster run as a chain of bands)
   if (prm->usetvref && (height >> prm->sc_l) > SOR_MAX_ROWS) return OFDIS_ERR_UNSUPPORTED;
+  // launches that put the frames in gridDim.y / .z (at most 65535): the derivative kernels max_frames x dirs x noc,
+  // the pyramid kernels 2 x max_frames (both images of a pair), every other one max_frames x dirs or fewer
+  if ((long)max_frames * std::max(2, (prm->usefbcon ? 2 : 1) * prm->noc) > OFDIS_MAX_GRID_FRAMES) return OFDIS_ERR_UNSUPPORTED;
 
   ofdis_ctx* ctx = new (std::nothrow) ofdis_ctx();
   if (!ctx) return OFDIS_ERR_NOMEM;
@@ -1244,6 +1247,34 @@ int ofdis_debug_sor_div_fallbacks(ofdis_ctx* ctx, unsigned long long* count, int
   CK(cudaMemcpyAsync(count, ctx->d_div_fb, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
   if (reset) CK(cudaMemsetAsync(ctx->d_div_fb, 0, sizeof(unsigned long long), ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
+  return OFDIS_OK;
+}
+
+int ofdis_debug_sor_plan(int w, int h, int nop, int noc, int solverit, int frames, int lane, int fast, int rt,
+                         int single_max, int max_cluster, int* out) {
+  if (w < 2 || h < 4 || h > SOR_MAX_ROWS || (nop != 1 && nop != 2) || (noc != 1 && noc != 3) || solverit < 1 ||
+      frames < 1 || lane < 0 || lane > 2 || (fast != 0 && fast != 1) || (rt != 1 && rt != 2 && rt != 4) ||
+      (single_max != 32 && single_max != 64 && single_max != 128) ||
+      (max_cluster != 1 && max_cluster != 2 && max_cluster != 4 && max_cluster != 8 && max_cluster != 16) || !out)
+    return OFDIS_ERR_ARG;
+  LevelGeom L{};
+  L.w = w;
+  L.h = h;
+  L.nop = nop;
+  L.noc = noc;
+  L.pitch = ((w + 3) / 4) * 4;
+  SorPlan p;
+  if (!sor_plan(L, solverit, SorOptions{lane, fast, rt, single_max, max_cluster}, frames, VarRefPlanes{}, &p))
+    return OFDIS_ERR_UNSUPPORTED;
+  out[0] = p.kind;
+  out[1] = p.pl.hpad;
+  out[2] = p.pl.rt;
+  out[3] = p.ml;
+  out[4] = p.pl.nb;
+  out[5] = p.sweeps;
+  out[6] = solverit % p.sweeps;
+  out[7] = assemble_rows_per_thread(w, h, frames);
+  out[8] = p.kind == SOR_REDBLACK ? 1 : (p.kind == SOR_LANE ? 2 : 0);  // launch_varref_t's MODE
   return OFDIS_OK;
 }
 

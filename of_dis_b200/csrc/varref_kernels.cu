@@ -567,6 +567,14 @@ bool sor_plan(const LevelGeom& L, int K, const SorOptions& o, int frames, const 
   return true;
 }
 
+// assemble_kernel: as many rows per thread (less halo work) as still leave >= 256 CTAs
+int assemble_rows_per_thread(int w, int h, int frames) {
+  const long tiles_x = (w + TX - 1) / TX;
+  for (int r = 4; r > 1; r >>= 1)
+    if (tiles_x * ((h + TY * r - 1) / (TY * r)) * frames >= 256) return r;
+  return 1;
+}
+
 template <int NOP, int HPAD, int RT, int BM>
 static cudaError_t launch_sor_t(const LevelGeom& g, const SorPlan& p, const VarRefParams& vp, int nf, int kk,
                                 size_t smem, cudaStream_t st, int* sync, unsigned long long* div_fb) {
@@ -636,10 +644,7 @@ static int launch_varref_t(const LevelGeom& g, const SorPlan& plan, const VarRef
   const int nf = f1 - f0;
   const dim3 block(TX, TY), grid((g.w + TX - 1) / TX, (g.h + TY - 1) / TY, nf);
   const dim3 gridc(grid.x, grid.y, nf * C);
-  // assemble_kernel: as many rows per thread (less halo work) as still leave >= 256 CTAs
-  int rows_per_thread = 1;
-  for (int r = 4; r > 1; r >>= 1)
-    if ((long)grid.x * ((g.h + TY * r - 1) / (TY * r)) * nf >= 256) { rows_per_thread = r; break; }
+  const int rows_per_thread = assemble_rows_per_thread(g.w, g.h, nf);
   const dim3 grid_a(grid.x, (g.h + TY * rows_per_thread - 1) / (TY * rows_per_thread), nf);
   {
     ProfScope scope(prof, KC_VR_SETUP);

@@ -45,6 +45,7 @@ def write_digests(out_dir):
         out["baseline_" + name] = t.digest(ref_driver.ref_run(pyr, prm))
     out.update(sor_division_digests())
     out.update(degenerate_digests())
+    out.update(batched_digests())
     with open(os.path.join(out_dir, "reference_digests.json"), "w") as f:
         json.dump(out, f, indent=1, sort_keys=True)
         f.write("\n")
@@ -65,6 +66,18 @@ def degenerate_digests():
         out[key + "_patches"], out[key + "_varref"] = t.degenerate_stage(ref_driver.ref_level_patches,
                                                                          ref_driver.ref_level_varref, pyr, prm)
     return out
+
+def batched_digests():
+    """The distinct pairs of every configuration of tests/test_batched_configs_gpu.py and those of the largest context
+    of tests/test_cabi.py: input pairs, and one digest over the whole runs of the pairs."""
+    import test_oracle as t
+
+    out = {}
+    for name in t.BATCHED:
+        out["batched_%s_input" % name], out["batched_%s_runs" % name] = t.batched_digests(ref_driver.ref_run, name)
+    out["frame_limit_input"], out["frame_limit_runs"] = t.frame_limit_digests(ref_driver.ref_run)
+    return out
+
 
 def sor_division_digests():
     """The stereo SOR's division regimes (tests/test_sor_division_gpu.py: parameters that drive A11 and B1 out of the

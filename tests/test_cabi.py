@@ -71,3 +71,64 @@ def test_reference_arm_prints_the_contract_line(tmp_path):
     assert line["impl"] == "reference" and line["value"] > 0 and line["higher_is_better"] is True
     assert line["e2e"]["h2d_bytes_per_step"] == 0 and line["e2e"]["d2h_bytes_per_step"] == 0
     assert line["cpu_baseline"]["kind"] in ("reference", "port") and line["cpu_baseline"]["cores"] >= 1
+
+
+# Frames sit in gridDim.y / gridDim.z (at most 65535) of several launches: the derivative kernels take
+# max_frames x dirs x noc, the pyramid kernels 2 x max_frames.  Largest accepted max_frames per (noc, usefbcon):
+FRAME_BOUNDS = [(1, 0, 32767), (3, 0, 21845), (1, 1, 32767), (3, 1, 10922)]
+LIMIT_CLI = "2 0 8 8 0.05 0.95 0 4 0.4 %d 1 0 1 10 10 5 1 3 1.6 0"
+
+
+@pytest.mark.parametrize("noc,fb,bound", FRAME_BOUNDS)
+def test_create_refuses_more_frames_than_a_grid_dimension_holds(noc, fb, bound, built_lib):
+    from of_dis_b200 import params
+
+    cp = params.from_cli_numbers((LIMIT_CLI % fb).split(), noc=noc).to_c()
+    h = ctypes.c_void_p()
+    assert built_lib.ofdis_create(ctypes.byref(h), 0, None, ctypes.byref(cp), 2, 32, 16, 4, bound + 1) == -3
+    assert not h.value
+    rc = built_lib.ofdis_create(ctypes.byref(h), 0, None, ctypes.byref(cp), 2, 32, 16, 4, bound)
+    assert rc != -3  # created on a GPU; without one the first CUDA call fails
+    built_lib.ofdis_destroy(h)
+
+
+def limit_pairs():
+    """the 4 distinct 32 x 16 gray pairs of test_largest_frame_count_vs_oracle"""
+    from of_dis_b200 import synth
+
+    return [synth.synthetic_pair(16, 32, 1, seed=400 + d, amp=2.0)[:2] for d in range(4)]
+
+
+@pytest.mark.gpu
+def test_largest_frame_count_vs_oracle(oracle_port):
+    """The largest gray flow context without usefbcon (32767 pairs of 32 x 16, three levels): the 8-bit upload, the
+    run, the batch download and the full-resolution output all take it, and every slot equals the oracle's flow of
+    its pair (4 distinct pairs, cycled)."""
+    import numpy as np
+
+    from of_dis_b200 import api, params, preprocess
+
+    prm = params.from_cli_numbers((LIMIT_CLI % 0).split())
+    n = FRAME_BOUNDS[0][2]
+    pairs = limit_pairs()
+    pyrs = [preprocess.PairPyramids(a, b, prm.sc_f, prm.p_samp_s) for a, b in pairs]
+    exp = np.stack([oracle_port.port_run(p, prm) for p in pyrs])
+    full = np.stack([preprocess.postprocess(e, prm.sc_l, p.padw, p.padh, 32, 16) for e, p in zip(exp, pyrs)])
+    slots = np.arange(n) % len(pairs)
+    frames = np.ascontiguousarray(np.stack([np.stack(pairs[d]) for d in range(len(pairs))])[slots])
+    ctx = api.Context(prm, 32, 16, prm.p_samp_s, n)
+    try:
+        ctx.upload_frames_u8(0, n, frames, 32, 16)
+        ctx.run(n)
+        out = np.empty((n,) + exp.shape[1:], np.float32)
+        ctx.get_flow_batch(0, n, out)
+        ctx.sync()
+        bad = np.flatnonzero((out.view(np.uint32) != exp[slots].view(np.uint32)).reshape(n, -1).any(1))
+        assert bad.size == 0, "%d slots differ from the oracle, first %d" % (bad.size, bad[0])
+        fr = np.empty((n,) + full.shape[1:], np.float32)
+        ctx.get_flow_fullres(0, n, fr, 32, 16)
+        ctx.sync()
+        bad = np.flatnonzero((fr.view(np.uint32) != full[slots].view(np.uint32)).reshape(n, -1).any(1))
+        assert bad.size == 0, "%d full-resolution slots differ, first %d" % (bad.size, bad[0])
+    finally:
+        ctx.close()

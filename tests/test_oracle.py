@@ -13,6 +13,8 @@ import pytest
 
 from of_dis_b200 import params, preprocess, synth
 from oracle import ref_driver
+from test_batched_configs_gpu import CONFIGS as BATCHED, batched_inputs
+from test_cabi import LIMIT_CLI, limit_pairs
 from test_degenerate_content_gpu import CASE_IDS as DEGEN_IDS, CASES as DEGEN_CASES, ROUTES as DEGEN_ROUTES
 from test_degenerate_content_gpu import coarser_flow, degenerate_inputs, stage_params
 from test_sor_division_gpu import DIV_CASES, REGIMES, division_inputs, initial_disparity
@@ -284,3 +286,34 @@ def test_native_thread_pool_drivers_reproduce_single_runs():
         assert np.array_equal(bits(flows[q]), bits(one))
         exp = preprocess.postprocess(one, prm.sc_l, p.padw, p.padh, 203, 121)
         assert np.array_equal(bits(full[q]), bits(exp.reshape(full[q].shape)))
+
+
+# ---- batched launches (tests/test_batched_configs_gpu.py) and the largest context (tests/test_cabi.py) -------------
+def pairs_digests(run, prm, pairs, pyrs):
+    """digest of the 8-bit input pairs, and one digest over the flows `run` computes for them, in turn"""
+    return digest(np.stack([np.stack(p) for p in pairs]), np.uint8), digest(np.stack([run(p, prm) for p in pyrs]))
+
+
+def batched_digests(run, name):
+    prm, pairs, pyrs = batched_inputs(name)
+    return pairs_digests(run, prm, pairs, pyrs)
+
+
+def frame_limit_digests(run):
+    prm = params.from_cli_numbers((LIMIT_CLI % 0).split())
+    pairs = limit_pairs()
+    return pairs_digests(run, prm, pairs, [preprocess.PairPyramids(a, b, prm.sc_f, prm.p_samp_s) for a, b in pairs])
+
+
+@pytest.mark.parametrize("name", list(BATCHED))
+def test_port_vs_reference_on_the_batched_configurations(name, oracle_port):
+    """The distinct pairs of every configuration of the batched sweep: whole runs, bit for bit as the reference build
+    computes them."""
+    inp, runs = batched_digests(oracle_port.port_run, name)
+    assert inp == REF_DIGESTS["batched_%s_input" % name], "%s: synthetic inputs differ from the recorded ones" % name
+    assert runs == REF_DIGESTS["batched_%s_runs" % name]
+
+
+def test_port_vs_reference_on_the_pairs_of_the_largest_context(oracle_port):
+    inp, runs = frame_limit_digests(oracle_port.port_run)
+    assert inp == REF_DIGESTS["frame_limit_input"] and runs == REF_DIGESTS["frame_limit_runs"]
