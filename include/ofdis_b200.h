@@ -216,6 +216,29 @@ int ofdis_upload_finest_level(ofdis_ctx* ctx, int f0, int f1, const float* packe
  * width_org/height_org pad up to the context's size by multiples of 2^sc_f, or of 2^(sc_f+1) as a run with an init
  * flow pads (run_dense.cpp:301); the crop is floor(pad/2) on the left/top either way. */
 int ofdis_get_flow_fullres(ofdis_ctx* ctx, int f0, int f1, float* out, int width_org, int height_org, int memkind);
+/* Encoded full-resolution flow (extension): F is each slot's full-resolution flow, exactly what
+ * ofdis_get_flow_fullres returns, computed from the level-sc_l flows without a full-resolution float copy, and written
+ * in a compact encoding.  Everything is float32, evaluated without contraction; the uint16 values are in host byte
+ * order (a PNG writer stores them big-endian).
+ *   OFDIS_ENC_F16: out = [f1-f0][height_org][width_org][nop] uint16 holding IEEE binary16.  Each channel is rounded
+ *     to nearest even (__float2half_rn), so magnitudes of 65520 and more become +-inf.  Every NaN, whatever its sign
+ *     or payload, becomes 0x7e00 (numpy's astype(float16) of the quiet NaN 0x7fc00000).
+ *   OFDIS_ENC_KITTI, flow: out = [f1-f0][height_org][width_org][3] uint16, channels R, G, B of KITTI's 16-bit flow
+ *     PNG.  Valid when u and v are not NaN: R = (uint16)fminf(fmaxf(u * 64.0f + 32768.0f, 0.0f), 65535.0f), G the
+ *     same of v, B = 1.  Invalid: 0, 0, 0.
+ *   OFDIS_ENC_KITTI, stereo: out = [f1-f0][height_org][width_org] uint16, KITTI's 16-bit disparity PNG.  d is the
+ *     positive disparity: -F for an ordinary slot (the sign SavePFMFile writes), +F for a slot marked swapped
+ *     (ofdis_set_swapped_slots, ofdis_upload_sequence_bidir_u8), which holds the right view.  Valid when d >= 0 (NaN
+ *     fails, -0 passes): (uint16)fminf(fmaxf(d * 256.0f, 1.0f), 65535.0f); invalid: 0.  Disparities of 256 px and
+ *     more are clamped to 65535 here; KITTI's format itself does not say what happens to them.
+ * Arguments, slot and frame-size checks and status codes are those of ofdis_get_flow_fullres; an unknown encoding, a
+ * NULL out or a device out that is not 2-byte aligned is OFDIS_ERR_ARG.  Host output goes through the context's
+ * full-resolution scratch, sized as ofdis_get_flow_fullres sizes it (no encoding is larger than the float flow), so
+ * alternating the two calls never reallocates.  Enqueued on the context's stream; not part of ofdis_run's graph.
+ * The flows are not changed. */
+enum { OFDIS_ENC_F16 = 1, OFDIS_ENC_KITTI = 2 };
+int ofdis_get_flow_fullres_encoded(ofdis_ctx* ctx, int f0, int f1, int encoding, void* out, int width_org,
+                                   int height_org, int memkind);
 
 /* Init flow from a flow of the original frame size (extension; the reference's disabled file input,
  * run_dense.cpp:292-301,355-378).  `flow` = [f1-f0][height_org][width_org][nop] floats.  Prepares the initflow of

@@ -34,7 +34,11 @@ EXPORTS = [
     "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8", "ofdis_set_initflow_fullres",
     "ofdis_set_initflow_from_result", "ofdis_upload_sequence_bidir_u8", "ofdis_set_swapped_slots",
     "ofdis_consistency_fullres", "ofdis_flow_error_fullres", "ofdis_debug_sor_plan",
+    "ofdis_get_flow_fullres_encoded",
 ]
+
+# encodings of get_flow_fullres_encoded (OFDIS_ENC_F16, OFDIS_ENC_KITTI)
+ENCODINGS = {"f16": 1, "kitti": 2}
 
 # kind of ofdis_debug_sor_plan (SorKind)
 SOR_KINDS = ("wave_single", "wave_cluster", "wave_chain", "lane", "redblack")
@@ -96,6 +100,8 @@ def lib():
             [ctypes.c_int] + [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
         L.ofdis_get_flow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_int]
+        L.ofdis_get_flow_fullres_encoded.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] + \
+            [ctypes.c_int] * 3
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -324,6 +330,33 @@ class Context:
     def get_flow_fullres(self, f0, f1, dst, width_org, height_org, memkind=MEM_HOST):
         """Flow x 2^sc_l, upsampled to the original frame size and cropped (run_dense.cpp:407-414)."""
         self._ck(lib().ofdis_get_flow_fullres(self._h, f0, f1, _ptr(dst), width_org, height_org, memkind))
+
+    def get_flow_fullres_encoded(self, f0, f1, encoding, width_org, height_org, out=None, memkind=MEM_HOST):
+        """get_flow_fullres of slots [f0, f1), encoded on the device as `encoding` (a key of ENCODINGS; the format
+        contract is ofdis_get_flow_fullres_encoded's, restated by preprocess.encode_f16 / encode_kitti).  Host result:
+        "f16" a (f1-f0, height_org, width_org, nop) float16 array, "kitti" a (f1-f0, height_org, width_org, 3) uint16
+        array for flow and (f1-f0, height_org, width_org) for stereo -- a new array, or `out` given as a numpy array
+        of exactly that dtype and shape; the call then synchronises the stream.  With memkind=MEM_DEVICE, out is a
+        device address the caller owns (e.g. a torch.float16 tensor's data_ptr()) and is returned as given."""
+        if encoding not in ENCODINGS:
+            raise ValueError("get_flow_fullres_encoded: encoding must be one of %s" % ", ".join(ENCODINGS))
+        if memkind == MEM_HOST:
+            nop = self.prm.nop
+            shape = (max(f1 - f0, 0), height_org, width_org)
+            if encoding == "f16":
+                shape, dt = shape + (nop,), np.float16
+            else:
+                shape, dt = shape + ((3,) if nop == 2 else ()), np.uint16
+            out = np.empty(shape, dt) if out is None else out
+            if not (isinstance(out, np.ndarray) and out.dtype == dt and out.shape == shape
+                    and out.flags["C_CONTIGUOUS"] and out.flags["WRITEABLE"]):
+                raise ValueError("get_flow_fullres_encoded: out must be a writeable C-contiguous %s array of shape %s"
+                                 % (np.dtype(dt).name, shape))
+        self._ck(lib().ofdis_get_flow_fullres_encoded(self._h, f0, f1, ENCODINGS[encoding], _ptr(out), width_org,
+                                                      height_org, memkind))
+        if memkind == MEM_HOST:
+            self.sync()
+        return out
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstdio>
 #include <climits>
+#include <cstdint>
 #include <cstring>
 #include <map>
 #include <new>
@@ -827,6 +828,37 @@ int ofdis_get_flow_fullres(ofdis_ctx* ctx, int f0, int f1, float* out, int width
   ctx->launches += 1;
   if (memkind != OFDIS_MEM_DEVICE)
     CK(cudaMemcpyAsync(out, dst, sizeof(float) * per * (size_t)(f1 - f0), cudaMemcpyDeviceToHost, ctx->stream));
+  return OFDIS_OK;
+}
+
+int ofdis_get_flow_fullres_encoded(ofdis_ctx* ctx, int f0, int f1, int encoding, void* out, int width_org,
+                                   int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !out ||
+      (encoding != OFDIS_ENC_F16 && encoding != OFDIS_ENC_KITTI) ||
+      (memkind == OFDIS_MEM_DEVICE && reinterpret_cast<uintptr_t>(out) % 2))
+    return fail(ctx, OFDIS_ERR_ARG, "get_flow_fullres_encoded: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("encode", -1);
+  CK(cudaSetDevice(ctx->device));
+  const size_t pix = (size_t)width_org * height_org;
+  // uint16 values per slot: nop binary16, or KITTI's 3 (flow) / 1 (stereo)
+  const size_t per = encoding == OFDIS_ENC_F16 ? pix * ctx->nop : pix * (ctx->nop == 2 ? 3 : 1);
+  unsigned short* dst = static_cast<unsigned short*>(out);
+  if (memkind != OFDIS_MEM_DEVICE) {
+    // the size ofdis_get_flow_fullres asks for; every encoding fits in it
+    rc = ensure_full(ctx, pix * ctx->nop * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    dst = reinterpret_cast<unsigned short*>(ctx->d_full);
+  }
+  if (launch_flow_encode(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, f1 - f0, encoding, dst, width_org, height_org,
+                         cx, cy, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "flow_encode_kernel launch", cudaGetLastError());
+  ctx->launches += 1;
+  if (memkind != OFDIS_MEM_DEVICE)
+    CK(cudaMemcpyAsync(out, dst, sizeof(unsigned short) * per * (size_t)(f1 - f0), cudaMemcpyDeviceToHost, ctx->stream));
   return OFDIS_OK;
 }
 

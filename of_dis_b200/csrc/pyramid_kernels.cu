@@ -3,6 +3,7 @@
 // divisibility padding (run_dense.cpp:298-311) and the final resize/crop (run_dense.cpp:407-414).
 // Expression order follows of_dis_b200/preprocess.py, which for 8-bit input is bit-identical to
 // OpenCV (every intermediate is a dyadic rational that float32 holds exactly).
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include "ofdis_internal.cuh"
@@ -219,6 +220,38 @@ __global__ void __launch_bounds__(256) flow_upsample_kernel(LevelGeom g, int f0,
   const float* fl = g.flow + (size_t)frame_of(g, f0, fr) * g.flow_frame_stride;
   float* o = out + ((size_t)fr * h_org * w_org + (size_t)Y * w_org + X) * NOP;
   upsample_at<NOP>(g, fl, X, Y, crop_x, crop_y, [o](int c, float v) { o[c] = v; });
+}
+
+// The full-resolution flow F of flow_upsample_kernel, encoded per pixel (ofdis_get_flow_fullres_encoded; the header
+// states the format contract, preprocess.encode_f16 / encode_kitti restate it), float32 without contraction:
+//   OFDIS_ENC_F16:   every channel __float2half_rn(F), a NaN of any sign or payload 0x7e00;
+//   OFDIS_ENC_KITTI: flow (R, G, B) = (clamp(u * 64 + 32768), clamp(v * 64 + 32768), 1) when neither is NaN, else 0;
+//                    stereo d = -F (F where the slot is marked swapped), clamp(d * 256, 1, 65535) when d >= 0, else 0.
+// The float32 F itself is never stored.  One thread per full-resolution pixel.
+template <int NOP, int ENC>
+__global__ void __launch_bounds__(256) flow_encode_kernel(LevelGeom g, int f0, unsigned short* out, int w_org,
+                                                          int h_org, int crop_x, int crop_y) {
+  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
+  const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (X >= w_org || Y >= h_org) return;
+  const int fr = blockIdx.z, frame = frame_of(g, f0, fr);
+  const float* fl = g.flow + (size_t)frame * g.flow_frame_stride;
+  const size_t o = (size_t)fr * h_org * w_org + (size_t)Y * w_org + X;
+  float f[2] = {0.f, 0.f};
+  upsample_at<NOP>(g, fl, X, Y, crop_x, crop_y, [&f](int c, float v) { f[c] = v; });
+  if constexpr (ENC == OFDIS_ENC_F16) {
+    for (int c = 0; c < NOP; ++c)
+      out[o * NOP + c] = isnan(f[c]) ? (unsigned short)0x7e00 : __half_as_ushort(__float2half_rn(f[c]));
+  } else if constexpr (NOP == 2) {
+    const bool valid = !isnan(f[0]) && !isnan(f[1]);
+    auto q = [](float x) { return (unsigned short)fminf(fmaxf(x * 64.0f + 32768.0f, 0.0f), 65535.0f); };
+    out[o * 3] = valid ? q(f[0]) : (unsigned short)0;
+    out[o * 3 + 1] = valid ? q(f[1]) : (unsigned short)0;
+    out[o * 3 + 2] = valid ? (unsigned short)1 : (unsigned short)0;
+  } else {
+    const float d = swapped_of(g, frame) ? f[0] : -f[0];  // KITTI's positive disparity; NaN fails d >= 0, -0 passes
+    out[o] = d >= 0.0f ? (unsigned short)fminf(fmaxf(d * 256.0f, 1.0f), 65535.0f) : (unsigned short)0;
+  }
 }
 
 // Forward-backward (flow) / left-right (stereo) consistency (Sundaram, Brox, Keutzer, ECCV 2010) of frame fa's
@@ -488,6 +521,25 @@ int launch_flow_upsample(const LevelGeom& g, int f0, int f1, float* out, int w_o
   const dim3 block(32, 8), grid((w_org + 31) / 32, (h_org + 7) / 8, f1 - f0);
   if (g.nop == 2) flow_upsample_kernel<2><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
   else flow_upsample_kernel<1><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_flow_encode(const LevelGeom& g, int f0, int n, int enc, unsigned short* out, int w_org, int h_org,
+                       int crop_x, int crop_y, cudaStream_t st) {
+  const dim3 block(32, 8), grid((w_org + 31) / 32, (h_org + 7) / 8, n);
+  if (enc == OFDIS_ENC_F16) {
+    if (g.nop == 2)
+      flow_encode_kernel<2, OFDIS_ENC_F16><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
+    else
+      flow_encode_kernel<1, OFDIS_ENC_F16><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
+  } else if (enc == OFDIS_ENC_KITTI) {
+    if (g.nop == 2)
+      flow_encode_kernel<2, OFDIS_ENC_KITTI><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
+    else
+      flow_encode_kernel<1, OFDIS_ENC_KITTI><<<grid, block, 0, st>>>(g, f0, out, w_org, h_org, crop_x, crop_y);
+  } else {
+    return -1;
+  }
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -19,6 +19,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <iostream>
+#include <limits>
 #include <string>
 #include <vector>
 
@@ -566,7 +567,15 @@ int main(int argc, char** argv) {
 // and with --bidirectional one more per class, `EVAL consistent (...)`, `EVAL inconsistent (...)`, `EVAL leaves (...)`.
 // The totals add the per-pair stats in list order (sum_err in float64; the all-pixel line adds a pair's classes in
 // class order); epe = sum_err / n, percentages 100 * count / n, printed with %.6f; a line with n = 0 prints nan for
-// every value but n.  The output files keep their bytes.
+// every value but n.  The output files keep their bytes.  A ground-truth file that starts with the PNG signature is
+// read as KITTI's 16-bit ground truth: flow RGB16, (R - 32768) / 64 and (G - 32768) / 64 where B > 0; stereo gray16,
+// -(value / 256) (this library's sign) where the value is > 0; NaN (unknown) elsewhere.
+//
+// --kitti: every output (and with --bidirectional every _bw output) is written as KITTI's 16-bit PNG, whatever its
+// extension, encoded on the device (ofdis_get_flow_fullres_encoded, OFDIS_ENC_KITTI), so 6 (flow) or 2 (stereo)
+// bytes per pixel come back instead of 8 or 4.  Flow: RGB16 (u * 64 + 2^15, v * 64 + 2^15, 1), (0, 0, 0) where the
+// flow is NaN; stereo: gray16 d * 256 of the positive disparity d (the left view's -F, a _bw file's right-view +F),
+// clamped to [1, 65535], 0 where d is negative or NaN.  The _occ.pgm masks and the EVAL lines do not change.
 
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
@@ -612,6 +621,148 @@ static void add_stats(ofdis_error_stats& t, const ofdis_error_stats& s) {
   t.sum_err += s.sum_err;
 }
 
+static const uint8_t kPngSig[8] = {0x89, 'P', 'N', 'G', 0x0d, 0x0a, 0x1a, 0x0a};
+
+// KITTI ground truth: a 16-bit non-interlaced PNG of the image size, RGB16 for flow (nop 2), gray16 for stereo, every
+// row filter 0-4 undone with a byte distance of 2 * channels.  Returns [h][w][nop] floats in this library's
+// convention with NaN for the invalid pixels (kitti_to_flow of of_dis_b200/preprocess.py), or false with `err`.
+static bool read_kitti_png(const vector<uint8_t>& b, int w, int h, int nop, const string& what, vector<float>& flow,
+                           string& err) {
+  size_t pos = 8;
+  int iw = 0, ih = 0, depth = 0, ctype = -1, interlace = -1;
+  vector<uint8_t> idat;
+  while (pos + 12 <= b.size()) {
+    const uint32_t len = be32(&b[pos]);
+    const char* type = (const char*)&b[pos + 4];
+    const uint8_t* data = &b[pos + 8];
+    if (len > b.size() - pos - 12) break;
+    if (!memcmp(type, "IHDR", 4) && len >= 13) {
+      iw = (int)be32(data);
+      ih = (int)be32(data + 4);
+      depth = data[8];
+      ctype = data[9];
+      interlace = data[12];
+    } else if (!memcmp(type, "IDAT", 4)) idat.insert(idat.end(), data, data + len);
+    else if (!memcmp(type, "IEND", 4)) break;
+    pos += 12 + len;
+  }
+  const int ch = nop == 2 ? 3 : 1;
+  if (depth != 16 || ctype != (nop == 2 ? 2 : 0) || interlace != 0) {
+    err = "the " + what + " is not a 16-bit non-interlaced KITTI PNG (" + (nop == 2 ? "RGB16 flow)" : "gray16 disparity)");
+    return false;
+  }
+  if (iw != w || ih != h) {
+    err = "the " + what + "'s size differs from the images'";
+    return false;
+  }
+  const size_t stride = (size_t)w * ch * 2, bpp = 2 * ch;
+  vector<uint8_t> raw((stride + 1) * h);
+  uLongf rawlen = raw.size();
+  if (uncompress(raw.data(), &rawlen, idat.data(), idat.size()) != Z_OK || rawlen != raw.size()) {
+    err = "the " + what + "'s image data does not decompress to its size";
+    return false;
+  }
+  vector<uint8_t> img(stride * h), zero(stride, 0);
+  for (int y = 0; y < h; ++y) {
+    const uint8_t ft = raw[(stride + 1) * y];
+    const uint8_t* in = &raw[(stride + 1) * y + 1];
+    uint8_t* out = &img[stride * y];
+    const uint8_t* up = y ? &img[stride * (y - 1)] : zero.data();
+    for (size_t x = 0; x < stride; ++x) {
+      const int a = x >= bpp ? out[x - bpp] : 0, bb = up[x], c = x >= bpp ? up[x - bpp] : 0;
+      int pr = 0;
+      switch (ft) {
+        case 0: pr = 0; break;
+        case 1: pr = a; break;
+        case 2: pr = bb; break;
+        case 3: pr = (a + bb) >> 1; break;
+        case 4: {
+          const int p = a + bb - c, pa = abs(p - a), pb = abs(p - bb), pc = abs(p - c);
+          pr = (pa <= pb && pa <= pc) ? a : (pb <= pc ? bb : c);
+          break;
+        }
+        default:
+          err = "the " + what + " has an unknown PNG row filter";
+          return false;
+      }
+      out[x] = (uint8_t)(in[x] + pr);
+    }
+  }
+  const float nan = std::numeric_limits<float>::quiet_NaN();
+  flow.assign((size_t)w * h * nop, 0.f);
+  for (size_t i = 0; i < (size_t)w * h; ++i) {
+    const uint8_t* s = &img[i * bpp];
+    auto sample = [s](int k) { return (float)(((unsigned)s[2 * k] << 8) | s[2 * k + 1]); };
+    if (nop == 2) {
+      const bool valid = sample(2) > 0.0f;
+      flow[2 * i] = valid ? (sample(0) - 32768.0f) / 64.0f : nan;
+      flow[2 * i + 1] = valid ? (sample(1) - 32768.0f) / 64.0f : nan;
+    } else {
+      flow[i] = sample(0) > 0.0f ? -(sample(0) / 256.0f) : nan;
+    }
+  }
+  return true;
+}
+
+// a ground-truth file of --gt: KITTI's 16-bit PNG when it starts with the PNG signature, else read_flow_file's formats
+static bool read_gt_file(const char* path, int w, int h, int nop, vector<float>& flow, string& err) {
+  const string what = "ground-truth file";
+  vector<uint8_t> b;
+  if (read_file(path, b) && b.size() >= 8 && !memcmp(b.data(), kPngSig, 8)) {
+    try {
+      return read_kitti_png(b, w, h, nop, what, flow, err);
+    } catch (const std::exception&) {  // bad_alloc / length errors on malformed headers
+      err = "the " + what + " is not a readable KITTI PNG";
+      return false;
+    }
+  }
+  return read_flow_file(path, w, h, nop, what, flow, err);
+}
+
+// KITTI's 16-bit PNG of one encoded slot (`ch` = 3: RGB16, 1: gray16): IHDR, one IDAT of filter-0 rows with the
+// samples big-endian, IEND
+static void save_kitti_png(const uint16_t* enc, int w, int h, int ch, const char* filename) {
+  const size_t stride = (size_t)w * ch * 2;
+  vector<uint8_t> raw((stride + 1) * h);
+  for (int y = 0; y < h; ++y) {
+    uint8_t* r = &raw[(stride + 1) * y];
+    r[0] = 0;
+    const uint16_t* s = enc + (size_t)y * w * ch;
+    for (size_t k = 0; k < (size_t)w * ch; ++k) {
+      r[1 + 2 * k] = (uint8_t)(s[k] >> 8);
+      r[2 + 2 * k] = (uint8_t)(s[k] & 0xff);
+    }
+  }
+  vector<uint8_t> z(compressBound(raw.size()));
+  uLongf zlen = z.size();
+  if (compress2(z.data(), &zlen, raw.data(), raw.size(), 1) != Z_OK) {
+    cout << "WriteFile: problem compressing data" << endl;
+    return;
+  }
+  FILE* f = fopen(filename, "wb");
+  if (!f) {
+    cout << "WriteFile: could not open file" << endl;
+    return;
+  }
+  bool ok = fwrite(kPngSig, 1, 8, f) == 8;
+  auto chunk = [&](const char* type, const uint8_t* data, uint32_t len) {
+    uint8_t be[4] = {(uint8_t)(len >> 24), (uint8_t)(len >> 16), (uint8_t)(len >> 8), (uint8_t)len};
+    uLong crc = crc32(0L, (const Bytef*)type, 4);
+    if (len) crc = crc32(crc, data, len);
+    const uint8_t cb[4] = {(uint8_t)(crc >> 24), (uint8_t)(crc >> 16), (uint8_t)(crc >> 8), (uint8_t)crc};
+    ok = ok && fwrite(be, 1, 4, f) == 4 && fwrite(type, 1, 4, f) == 4 && (!len || fwrite(data, 1, len, f) == len) &&
+         fwrite(cb, 1, 4, f) == 4;
+  };
+  const uint8_t ihdr[13] = {(uint8_t)(w >> 24), (uint8_t)(w >> 16), (uint8_t)(w >> 8), (uint8_t)w,
+                            (uint8_t)(h >> 24), (uint8_t)(h >> 16), (uint8_t)(h >> 8), (uint8_t)h,
+                            16, (uint8_t)(ch == 3 ? 2 : 0), 0, 0, 0};
+  chunk("IHDR", ihdr, 13);
+  chunk("IDAT", z.data(), (uint32_t)zlen);
+  chunk("IEND", nullptr, 0);
+  if (!ok) cout << "WriteFile: problem writing data" << endl;
+  fclose(f);
+}
+
 static void save_mask_pgm(const uint8_t* mask, int w, int h, const char* filename) {
   FILE* f = fopen(filename, "wb");
   if (!f) {
@@ -629,20 +780,23 @@ static void save_mask_pgm(const uint8_t* mask, int w, int h, const char* filenam
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr,
-            "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist]\n"
+            "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
             "  --bidirectional: also the backward flow (stereo: the right view's disparity) of every pair, written to\n"
             "  <stem>_bw<ext>, and the forward-backward consistency mask to <stem>_occ.pgm (0 consistent,\n"
             "  255 inconsistent, 128 leaves the frame); not with --warm-start\n"
-            "  --gt gtlist: ground-truth files (.flo / .pfm), one per pair in list order; prints EVAL lines (end-point\n"
-            "  error, shares above 1, 3, 5 px, KITTI outliers; with --bidirectional also per consistency class)\n",
+            "  --gt gtlist: ground-truth files (.flo / .pfm, or KITTI's 16-bit PNG), one per pair in list order; prints\n"
+            "  EVAL lines (end-point error, shares above 1, 3, 5 px, KITTI outliers; with --bidirectional also per\n"
+            "  consistency class)\n"
+            "  --kitti: write every flow (and _bw) output as KITTI's 16-bit PNG (flow RGB16, stereo gray16 disparity),\n"
+            "  whatever its extension\n",
             argv[0]);
     return 2;
   }
   int maxb = 64, first_num = 2;
-  bool warm = false, batch_set = false, bidir = false;
+  bool warm = false, batch_set = false, bidir = false, kitti = false;
   const char* gtlist = nullptr;
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
@@ -654,6 +808,9 @@ int main(int argc, char** argv) {
       first_num += 1;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--bidirectional")) {
       bidir = true;
+      first_num += 1;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--kitti")) {
+      kitti = true;
       first_num += 1;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
@@ -718,7 +875,7 @@ int main(int argc, char** argv) {
                 jobs[k].a.c_str(), jobs[k].b.c_str());
         return 1;
       }
-      if (!read_flow_file(gts[k].c_str(), iw, ih, nop, "ground-truth file", gtf, err)) {
+      if (!read_gt_file(gts[k].c_str(), iw, ih, nop, gtf, err)) {
         fprintf(stderr, "error: %s: %s\n", gts[k].c_str(), err.c_str());
         return 1;
       }
@@ -735,6 +892,7 @@ int main(int argc, char** argv) {
   int ctx_w = -1, ctx_h = -1, verbosity = 0;
   vector<uint8_t> frames;
   vector<float> flows;
+  vector<uint16_t> kflows;  // --kitti: the encoded slots
   vector<uint8_t> masks;
   Image8 last;  // image2 of the previous batch's last pair
   size_t j0 = 0;
@@ -815,7 +973,9 @@ int main(int argc, char** argv) {
       ctx_h = h;
     }
     const int slots = bidir ? 2 * n : n;  // bidirectional: forward slots [0, n), backward slots [n, 2n)
-    flows.resize((size_t)slots * w * h * nop);
+    const int kch = nop == 2 ? 3 : 1;     // --kitti: uint16 values per pixel
+    if (kitti) kflows.resize((size_t)slots * w * h * kch);
+    else flows.resize((size_t)slots * w * h * nop);
     int rc;
     if (bidir && seq) {
       rc = ofdis_upload_sequence_bidir_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
@@ -832,7 +992,9 @@ int main(int argc, char** argv) {
     if (rc == OFDIS_OK && from_prev) rc = ofdis_set_initflow_from_result(ctx, 0, 1, 0, w, h);
     warm_pairs += from_prev ? 1 : 0;
     if (rc == OFDIS_OK) rc = ofdis_run(ctx, slots, from_prev ? 1 : 0);
-    if (rc == OFDIS_OK) rc = ofdis_get_flow_fullres(ctx, 0, slots, flows.data(), w, h, OFDIS_MEM_HOST);
+    if (rc == OFDIS_OK)
+      rc = kitti ? ofdis_get_flow_fullres_encoded(ctx, 0, slots, OFDIS_ENC_KITTI, kflows.data(), w, h, OFDIS_MEM_HOST)
+                 : ofdis_get_flow_fullres(ctx, 0, slots, flows.data(), w, h, OFDIS_MEM_HOST);
     if (rc == OFDIS_OK && bidir) {
       masks.resize((size_t)n * w * h);
       rc = ofdis_consistency_fullres(ctx, 0, n, n, masks.data(), nullptr, nop == 2 ? 0.01f : 0.0f,
@@ -843,7 +1005,7 @@ int main(int argc, char** argv) {
       gt_batch.resize((size_t)n * w * h * nop);
       for (int k = 0; k < n; ++k) {
         string err;
-        if (!read_flow_file(gts[j0 + k].c_str(), w, h, nop, "ground-truth file", gt_one, err)) {
+        if (!read_gt_file(gts[j0 + k].c_str(), w, h, nop, gt_one, err)) {
           fprintf(stderr, "error: %s: %s\n", gts[j0 + k].c_str(), err.c_str());
           ofdis_destroy(ctx);
           return 1;
@@ -864,9 +1026,17 @@ int main(int argc, char** argv) {
       ofdis_destroy(ctx);
       return 1;
     }
+    for (int k = 0; k < n && kitti; ++k) {
+      save_kitti_png(kflows.data() + (size_t)k * w * h * kch, w, h, kch, jobs[j0 + k].out.c_str());
+      if (bidir) {
+        save_kitti_png(kflows.data() + (size_t)(n + k) * w * h * kch, w, h, kch,
+                       with_suffix(jobs[j0 + k].out, "_bw").c_str());
+        save_mask_pgm(masks.data() + (size_t)k * w * h, w, h, with_suffix(jobs[j0 + k].out, "_occ", ".pgm").c_str());
+      }
+    }
     ImageF out;
     out.w = w; out.h = h; out.c = nop;
-    for (int k = 0; k < n; ++k) {
+    for (int k = 0; k < n && !kitti; ++k) {
       out.px.assign(flows.begin() + (size_t)k * w * h * nop, flows.begin() + (size_t)(k + 1) * w * h * nop);
       if (SELECTMODE == 1) SaveFlowFile(out, jobs[j0 + k].out.c_str());
       else SavePFMFile(out, jobs[j0 + k].out.c_str());

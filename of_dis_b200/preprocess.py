@@ -330,3 +330,150 @@ def read_pfm(path: str) -> np.ndarray:
     if body.size != w * h or len(parts[3]) != 4 * w * h:
         raise ValueError("truncated .pfm file")
     return np.ascontiguousarray(-body.reshape(h, w)[::-1]).astype(np.float32).reshape(h, w, 1)
+
+
+# ---- encoded flows (ofdis_get_flow_fullres_encoded) and KITTI's 16-bit PNGs ------------------------------------------
+F16_NAN = 0x7E00  # the one NaN of the binary16 encoding: numpy's astype(float16) of the quiet NaN 0x7fc00000
+
+
+def encode_f16(flow: np.ndarray) -> np.ndarray:
+    """OFDIS_ENC_F16: every value rounded to the nearest binary16, ties to even (magnitudes of 65520 and more become
+    +-inf); every NaN, whatever its sign and payload, becomes 0x7e00.  Returns float16 of the same shape."""
+    F = np.asarray(flow, np.float32)
+    with np.errstate(over="ignore"):
+        h = F.astype(np.float16).view(np.uint16)
+    return np.where(np.isnan(F), np.uint16(F16_NAN), h).astype(np.uint16).view(np.float16)
+
+
+def encode_kitti(flow: np.ndarray, swapped: bool = False) -> np.ndarray:
+    """OFDIS_ENC_KITTI in float32 without contraction.  flow: (..., 2) or stereo (..., 1), in this library's
+    convention (what get_flow_fullres returns).
+        flow    (..., 3) uint16 (R, G, B): where u and v are not NaN,
+                (clamp(u * 64 + 32768, 0, 65535), the same of v, 1) truncated to uint16, else (0, 0, 0)
+        stereo  (...) uint16: d = -F (F when `swapped`, the right view of a swapped slot); where d >= 0 (NaN fails,
+                -0 passes) clamp(d * 256, 1, 65535) truncated to uint16, else 0"""
+    f32 = np.float32
+    F = np.asarray(flow, f32)
+    assert F.shape[-1] in (1, 2), F.shape
+    if F.shape[-1] == 2:
+        u, v = F[..., 0], F[..., 1]
+        valid = ~np.isnan(u) & ~np.isnan(v)
+        out = np.zeros(F.shape[:-1] + (3,), np.uint16)
+        with np.errstate(over="ignore", invalid="ignore"):
+            for c, x in enumerate((u, v)):
+                q = np.fmin(np.fmax(np.where(valid, x, f32(0)) * f32(64) + f32(32768), f32(0)), f32(65535))
+                out[..., c] = np.where(valid, q, f32(0)).astype(np.uint16)
+        out[..., 2] = valid
+        return out
+    d = F[..., 0] if swapped else -F[..., 0]
+    with np.errstate(invalid="ignore"):
+        valid = d >= f32(0)
+    with np.errstate(over="ignore"):
+        q = np.fmin(np.fmax(np.where(valid, d, f32(0)) * f32(256), f32(1)), f32(65535))
+    return np.where(valid, q, f32(0)).astype(np.uint16)
+
+
+def kitti_to_flow(enc: np.ndarray, nop: int) -> np.ndarray:
+    """A KITTI 16-bit array in this library's convention, float32, NaN where it is invalid (flow_error treats NaN
+    ground truth as unknown).  Flow (nop 2): (..., 3) -> (..., 2), (R - 32768.0f) / 64.0f, valid where B > 0.
+    Stereo (nop 1): (...) -> (..., 1), -(val / 256.0f), the sign get_flow_fullres and .pfm use, valid where val > 0."""
+    f32 = np.float32
+    E = np.asarray(enc, np.uint16)
+    if nop == 2:
+        assert E.shape[-1] == 3, E.shape
+        F = (E[..., :2].astype(f32) - f32(32768)) / f32(64)
+        F[E[..., 2] == 0] = np.nan
+        return F
+    F = -(E.astype(f32) / f32(256))
+    F[E == 0] = np.nan
+    return F[..., None]
+
+
+_PNG_SIG = b"\x89PNG\r\n\x1a\n"
+
+
+def write_kitti_png(path: str, enc: np.ndarray) -> None:
+    """KITTI's 16-bit PNG: (h, w, 3) uint16 as colour type 2 (flow), (h, w) as colour type 0 (stereo); big-endian
+    samples, non-interlaced, every row filter 0."""
+    import struct
+    import zlib
+
+    E = np.asarray(enc)
+    assert E.dtype == np.uint16 and (E.ndim == 2 or (E.ndim == 3 and E.shape[2] == 3)), (E.dtype, E.shape)
+    h, w = E.shape[:2]
+    rows = np.ascontiguousarray(E, ">u2").reshape(h, -1).view(np.uint8)
+    raw = np.concatenate([np.zeros((h, 1), np.uint8), rows], axis=1).tobytes()
+
+    def chunk(t, d):
+        return struct.pack(">I", len(d)) + t + d + struct.pack(">I", zlib.crc32(t + d) & 0xFFFFFFFF)
+
+    with open(path, "wb") as f:
+        f.write(_PNG_SIG + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 16, 2 if E.ndim == 3 else 0, 0, 0, 0)))
+        f.write(chunk(b"IDAT", zlib.compress(raw, 1)) + chunk(b"IEND", b""))
+
+
+def _unfilter(ft: int, line: np.ndarray, up: np.ndarray, bpp: int) -> np.ndarray:
+    """One PNG row of filter type ft (0 None, 1 Sub, 2 Up, 3 Average, 4 Paeth), with `bpp` bytes per pixel."""
+    if ft == 0:
+        return line
+    if ft == 2:
+        return (line.astype(np.uint16) + up).astype(np.uint8)
+    if ft == 1:  # out[x] = in[x] + out[x - bpp]: running sums mod 256 per byte position of a pixel
+        return (np.cumsum(line.reshape(-1, bpp).astype(np.int64), axis=0) % 256).astype(np.uint8).reshape(-1)
+    out = bytearray(line.tobytes())
+    prior = up.tobytes()
+    for x in range(len(out)):
+        a = out[x - bpp] if x >= bpp else 0
+        b = prior[x]
+        if ft == 3:
+            pred = (a + b) >> 1
+        elif ft == 4:
+            c = prior[x - bpp] if x >= bpp else 0
+            p = a + b - c
+            pa, pb, pc = abs(p - a), abs(p - b), abs(p - c)
+            pred = a if (pa <= pb and pa <= pc) else (b if pb <= pc else c)
+        else:
+            raise ValueError("PNG filter type %d" % ft)
+        out[x] = (out[x] + pred) & 0xFF
+    return np.frombuffer(bytes(out), np.uint8)
+
+
+def read_kitti_png(path: str) -> np.ndarray:
+    """The 16-bit PNGs of write_kitti_png, from any writer: (h, w, 3) uint16 for colour type 2, (h, w) for colour type
+    0.  Bit depth 16 and no interlacing are required; every row may use any of the five filter types."""
+    import struct
+    import zlib
+
+    with open(path, "rb") as f:
+        b = f.read()
+    if b[:8] != _PNG_SIG:
+        raise ValueError("%s: not a PNG file" % path)
+    pos, idat, hdr = 8, [], None
+    while pos + 8 <= len(b):
+        n, t = struct.unpack(">I", b[pos:pos + 4])[0], b[pos + 4:pos + 8]
+        data = b[pos + 8:pos + 8 + n]
+        if t == b"IHDR":
+            hdr = struct.unpack(">IIBBBBB", data[:13])
+        elif t == b"IDAT":
+            idat.append(data)
+        elif t == b"IEND":
+            break
+        pos += 12 + n
+    if hdr is None:
+        raise ValueError("%s: no IHDR" % path)
+    w, h, depth, ctype, _, _, interlace = hdr
+    if depth != 16 or ctype not in (0, 2) or interlace != 0:
+        raise ValueError("%s: not a 16-bit non-interlaced gray or RGB PNG" % path)
+    ch = 3 if ctype == 2 else 1
+    stride = w * ch * 2
+    raw = np.frombuffer(zlib.decompress(b"".join(idat)), np.uint8)
+    if raw.size != h * (stride + 1):
+        raise ValueError("%s: image data of the wrong length" % path)
+    raw = raw.reshape(h, stride + 1)
+    img = np.zeros((h, stride), np.uint8)
+    up = np.zeros(stride, np.uint8)
+    for y in range(h):
+        img[y] = _unfilter(int(raw[y, 0]), raw[y, 1:], up, 2 * ch)
+        up = img[y]
+    out = img.view(">u2").astype(np.uint16)
+    return out.reshape(h, w, 3) if ch == 3 else out.reshape(h, w)
