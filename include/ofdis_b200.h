@@ -31,6 +31,23 @@
  * sits BELOW the reference API: one context processes frame pairs
  * [0, max_frames) per launch.
  *
+ * Threads and shared devices: one context is used by one host thread at a
+ * time (calls on the same context must not overlap; which thread makes them
+ * may change).  Different contexts may share a device and a stream, and
+ * each gives the same bits as it would alone.  Contexts on different streams
+ * may be used from different threads at once, in graph mode or not.  A
+ * context in graph mode captures its stream while ofdis_run records a graph
+ * (the first run of a frame count after ofdis_set_graph_mode(1) or after a
+ * call that discards its graphs, such as ofdis_set_option): whatever else is
+ * enqueued on that stream meanwhile, from any thread, is recorded into the
+ * graph or breaks the capture, and a synchronisation of the stream breaks
+ * it.  So contexts that share a stream, and the caller's own work on it,
+ * are used from one thread at a time once one of them is in graph mode.  A
+ * context on a caller's stream only enqueues its own work there, in call
+ * order, and leaves the stream's other work alone; ofdis_destroy waits for
+ * that stream.  Process-wide state is guarded inside the library (DESIGN.md
+ * section 5.13).
+ *
  * Arithmetic contract: IEEE binary32, no FMA contraction, expression order of
  * the reference, so results are bitwise equal to the reference CPU build on
  * the same inputs (tests/test_gpu_parity.py).

@@ -965,8 +965,10 @@ int ofdis_patgrid_optimize(ofdis_ctx* ctx, int level, int f0, int f1, int init_f
   const int q0 = ctx->sel_dir >= 0 ? f0 * ctx->dirs + ctx->sel_dir : f0 * ctx->dirs;
   const int q1 = ctx->sel_dir >= 0 ? q0 + 1 : f1 * ctx->dirs;
   L->pdl = pdl_for(ctx, q1 - q0);
+  cudaError_t optin = cudaSuccess;
   const int n = launch_patch_optimize(*L, ctx->pp, q0, q1, init_from_coarser != 0, patch_lanes_for(ctx, q1 - q0),
-                                      ctx->stream, ctx->prof);
+                                      ctx->stream, ctx->prof, &optin);
+  if (optin != cudaSuccess) return fail(ctx, OFDIS_ERR_CUDA, "patch kernel launch: shared-memory opt-in (smem_optin)", optin);
   if (n < 0) return fail(ctx, OFDIS_ERR_CUDA, "patch_optimize_kernel launch", cudaGetLastError());
   ctx->launches += n;
   return OFDIS_OK;

@@ -1068,8 +1068,15 @@ __global__ void __launch_bounds__(256) fb_prepare_kernel(LevelGeom g, int f0) {
 }  // namespace
 
 int launch_patch_optimize(const LevelGeom& g, const PatchParams& pp, int f0, int f1, bool init_from_coarser,
-                          int lanes, cudaStream_t st, Profiler* prof) {
+                          int lanes, cudaStream_t st, Profiler* prof, cudaError_t* optin_err) {
   ProfScope scope(prof, KC_PATCH);
+  // smem depends on P and C, and the kernels are shared by every context of the process: opt in through the
+  // raise-only cache, never to a launch's own size (which could lower the attribute under another context)
+  auto optin = [&](const void* kern, size_t smem) {
+    const cudaError_t e = smem > 48 * 1024 ? smem_optin(kern, smem, false) : cudaSuccess;
+    if (optin_err) *optin_err = e;
+    return e == cudaSuccess;
+  };
   if (g.P == 8 && g.noc == 1) {  // register-resident specialisation (operating points 1 and 2)
     constexpr int patches_per_cta = 32;
     const dim3 grid8((g.np + patches_per_cta - 1) / patches_per_cta, f1 - f0);
@@ -1094,8 +1101,7 @@ int launch_patch_optimize(const LevelGeom& g, const PatchParams& pp, int f0, int
   do {                                                                                                             \
     const size_t sm = sizeof(float) * ((size_t)(threads12 / 8) * PwCfg<NOPv, Cv>::WIN +                            \
                                        (Cv == 1 ? 0 : (size_t)2 * PwCfg<NOPv, Cv>::NK * threads12));               \
-    if (sm > 48 * 1024)                                                                                            \
-      cudaFuncSetAttribute(patch_p12_kernel<NOPv, Cv>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);      \
+    if (!optin((const void*)patch_p12_kernel<NOPv, Cv>, sm)) return -1;                                           \
     patch_p12_kernel<NOPv, Cv><<<grid12, threads12, sm, st>>>(g, pp, f0, init);                                    \
   } while (0)
     if (g.nop == 2 && g.noc == 1) OFDIS_P12(2, 1);
@@ -1111,15 +1117,9 @@ int launch_patch_optimize(const LevelGeom& g, const PatchParams& pp, int f0, int
   while (threads > 32 && (size_t)5 * NK * threads * sizeof(float) > 200 * 1024) threads >>= 1;
   const size_t smem = (size_t)5 * NK * threads * sizeof(float);
   const dim3 grid((g.np + threads / 8 - 1) / (threads / 8), f1 - f0);
-  if (g.nop == 2) {
-    if (smem > 48 * 1024)
-      cudaFuncSetAttribute(patch_optimize_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    patch_optimize_kernel<2><<<grid, threads, smem, st>>>(g, pp, f0, init_from_coarser ? 1 : 0);
-  } else {
-    if (smem > 48 * 1024)
-      cudaFuncSetAttribute(patch_optimize_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    patch_optimize_kernel<1><<<grid, threads, smem, st>>>(g, pp, f0, init_from_coarser ? 1 : 0);
-  }
+  if (!optin(g.nop == 2 ? (const void*)patch_optimize_kernel<2> : (const void*)patch_optimize_kernel<1>, smem)) return -1;
+  if (g.nop == 2) patch_optimize_kernel<2><<<grid, threads, smem, st>>>(g, pp, f0, init_from_coarser ? 1 : 0);
+  else patch_optimize_kernel<1><<<grid, threads, smem, st>>>(g, pp, f0, init_from_coarser ? 1 : 0);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -468,17 +468,19 @@ __global__ void __launch_bounds__(256) flow_update_kernel(LevelGeom g, VarRefPla
 // Opt-in of `smem` bytes of dynamic shared memory for `kern` on the current device (and, with `nonportable`, of
 // clusters of more than 8 CTAs).  The attributes belong to the kernel, so the cache is keyed by device and kernel:
 // it only ever raises a kernel's setting, whichever of the launches that share the kernel (gray and RGB levels,
-// sor_max_cluster_size) comes first.  A cache per launcher once let an RGB level that needed less shared memory lower
-// the setting behind a gray level's cache, and the gray level's next larger launch failed.
-template <typename Kern>
-static cudaError_t smem_optin(Kern* kern, size_t smem, bool nonportable) {
+// contexts of other patch sizes, sor_max_cluster_size) comes first.  A cache per launcher once let an RGB level that
+// needed less shared memory lower the setting behind a gray level's cache, and the gray level's next larger launch
+// failed.  Setting the attribute to each launch's own size would fail the same way across contexts: another thread's
+// smaller launch can lower it between this thread's set and launch, and a graph captured at the larger size can be
+// replayed after it.
+cudaError_t smem_optin(const void* kern, size_t smem, bool nonportable) {
   static std::mutex mu;
   static std::map<std::pair<int, const void*>, std::pair<size_t, bool>> done;  // (device, kernel) -> (smem, nonportable)
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   std::lock_guard<std::mutex> lock(mu);
-  std::pair<size_t, bool>& d = done[{dev, (const void*)kern}];
+  std::pair<size_t, bool>& d = done[{dev, kern}];
   if (d.first < smem) {
     if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
     d.first = smem;
@@ -580,7 +582,7 @@ static cudaError_t launch_sor_t(const LevelGeom& g, const SorPlan& p, const VarR
                                 size_t smem, cudaStream_t st, int* sync, unsigned long long* div_fb) {
   constexpr bool CL = (BM == SOR_CLUSTER);
   auto kern = sor_wave_kernel<NOP, HPAD, RT, BM>;
-  const cudaError_t e = smem_optin(kern, smem, CL);
+  const cudaError_t e = smem_optin((const void*)kern, smem, CL);
   if (e != cudaSuccess) return e;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(nf * (BM != SOR_SINGLE ? p.pl.nb : 1)));
@@ -677,10 +679,10 @@ static int launch_varref_t(const LevelGeom& g, const SorPlan& plan, const VarRef
       cudaError_t e;
       if (plan.kind == SOR_REDBLACK) {  // opt-in red-black solver, (du,dv) ping-pong
         const dim3 grid_rb((g.w + RB_TILE - 1) / RB_TILE, (g.h + RB_TILE - 1) / RB_TILE, nf);
-        if ((e = smem_optin(sor_redblack_kernel<NOP>, smem, false)) == cudaSuccess)
+        if ((e = smem_optin((const void*)sor_redblack_kernel<NOP>, smem, false)) == cudaSuccess)
           e = launch_k(pdl, sor_redblack_kernel<NOP>, grid_rb, dim3(256), smem, st, g, pl, vp);
       } else if (plan.kind == SOR_LANE) {  // pixel wavefront, warps synchronised through shared-memory flags
-        if ((e = smem_optin(sor_lane_kernel<NOP>, smem, false)) == cudaSuccess)
+        if ((e = smem_optin((const void*)sor_lane_kernel<NOP>, smem, false)) == cudaSuccess)
           e = launch_k(pdl, sor_lane_kernel<NOP>, dim3(nf), dim3(pl.nb * kk * 32), smem, st, g, pl, vp, kk, div_fb);
       } else {
         e = launch_sor<NOP>(g, plan, vp, nf, kk, smem, st, chain_sync, div_fb);
@@ -708,7 +710,7 @@ int sor_max_cluster_size() {
   int best = 8;
   auto kern = sor_wave_kernel<2, 128, 1, SOR_CLUSTER>;
   const size_t smem = sor_smem_bytes(2, 128, 1, 3, 128);  // 128-row bands, 3 sweeps in flight: the largest common configuration
-  if (smem_optin(kern, smem, true) == cudaSuccess) {
+  if (smem_optin((const void*)kern, smem, true) == cudaSuccess) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(16);
     cfg.blockDim = dim3(3 * 128 + 32);
