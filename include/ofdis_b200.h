@@ -256,6 +256,49 @@ int ofdis_get_flow_fullres(ofdis_ctx* ctx, int f0, int f1, float* out, int width
 enum { OFDIS_ENC_F16 = 1, OFDIS_ENC_KITTI = 2 };
 int ofdis_get_flow_fullres_encoded(ofdis_ctx* ctx, int f0, int f1, int encoding, void* out, int width_org,
                                    int height_org, int memkind);
+/* Color-coded full-resolution flow (extension): F is each slot's full-resolution flow, exactly what
+ * ofdis_get_flow_fullres returns, computed from the level-sc_l flows without a full-resolution float copy.
+ * rgb = [f1-f0][height_org][width_org][3] bytes, R, G, B; scale = NULL or [f1-f0] floats, the scale each slot was
+ * colored with.  Everything is float32 without contraction, with IEEE division and square root; PI_F = (float)M_PI;
+ * bytes are (uint8) of a float in [0, 256), by truncation.  preprocess.flow_to_color / disp_to_color restate it.
+ *   Flow (nop 2), Middlebury's MotionToColor / computeColor (Baker et al. 2011):
+ *     known pixel: u, v not NaN and |u|, |v| <= 1e9 (the rule of ofdis_flow_error_fullres, so +-inf is unknown);
+ *     scale: max_value if it is > 0, else m, the maximum of sqrtf(u*u + v*v) over the slot's known pixels starting
+ *       from 0, or 1 when m == 0 (an all-zero or all-unknown slot);
+ *     unknown pixel: (0, 0, 0);
+ *     known pixel: fx = u / scale, fy = v / scale, rad = sqrtf(fx*fx + fy*fy); a = atan2_f32(-v, -u) / PI_F of the
+ *       unscaled flow (fx, fy may overflow for a tiny max_value); fk = (a + 1) / 2 * 54, k0 = (int)fk,
+ *       k1 = (k0 + 1) % 55, f = fk - k0; per channel b
+ *       col = (1.0f - f) * (W[k0][b] / 255.0f) + f * (W[k1][b] / 255.0f),
+ *       col = rad <= 1 ? 1 - rad * (1 - col) : col * 0.75f, byte (uint8)(255.0f * col).  Zero flow is white.
+ *     W: 55 integer entries of Middlebury's makecolorwheel, integer division, segments RY 15 (255, 255*i/15, 0),
+ *       YG 6 (255 - 255*i/6, 255, 0), GC 4 (0, 255, 255*i/4), CB 11 (0, 255 - 255*i/11, 255),
+ *       BM 13 (255*i/13, 0, 255), MR 6 (255, 0, 255 - 255*i/6).
+ *     atan2_f32(y, x): the library's own float32 atan2, so the contract does not depend on a libm:
+ *       ax = |x|, ay = |y|, mx = max(ax, ay), mn = min(ax, ay), t = mx > 0 ? mn / mx : 0, s = t * t,
+ *       q = C7, then q = q * s + Ck for k = 6 .. 0, p = t * q with C0..C7 = 0.99999934f, -0.3332986f, 0.19946565f,
+ *       -0.13908629f, 0.09642195f, -0.055912293f, 0.021862935f, -0.0040545613f;
+ *       p = ay > ax ? PI_F * 0.5f - p : p; p = signbit(x) ? PI_F - p : p; result signbit(y) ? -p : p.
+ *       Within 1e-6 of float64 atan2, in [-PI_F, PI_F] for finite input; signed zeros and axes as C's atan2.
+ *   Stereo (nop 1), the color map of KITTI's stereo devkit (disp_to_color):
+ *     d = -F for an ordinary slot, +F for a slot marked swapped (as OFDIS_ENC_KITTI); valid when 0 <= d <= 1e9 (NaN
+ *       fails, -0 passes); scale: max_value if it is > 0, else fmaxf(m, 1), m the maximum valid d, starting from 0;
+ *     invalid pixel: (0, 0, 0);
+ *     M = {{0,0,0,114},{0,0,1,185},{1,0,0,114},{1,0,1,174},{0,1,0,114},{0,1,1,185},{1,1,0,114},{1,1,1,0}};
+ *       wt[i] = 1000.0f / M[i][3]; cum[0] = 0, cum[i+1] = cum[i] + M[i][3] / 1000.0f for i = 0..6 in order;
+ *     valid pixel: val = fminf(fmaxf(d / scale, 0), 1); i = the first of 0..6 with val < cum[i+1], else 6 (cum[7] is
+ *       1.0f, so val = 1 takes the last bin); w = 1 - (val - cum[i]) * wt[i]; channel c
+ *       (uint8)fminf(fmaxf((w * M[i][c] + (1 - w) * M[i+1][c]) * 255.0f, 0), 255).  In float32, w at val = 1 is
+ *       3.6e-7 rather than 0, so d >= scale gives (255, 255, 254).
+ *     These formulas follow the devkit's description; they have not been compared with the devkit's own output.
+ * rgb NULL, max_value NaN, negative or infinite, slots outside the context, or a device scale that is not 4-byte
+ * aligned is OFDIS_ERR_ARG; frame-size checks and status codes are those of ofdis_get_flow_fullres.  rgb and scale are
+ * in memkind; host output goes through the context's full-resolution scratch at the size ofdis_get_flow_fullres asks
+ * for, so alternating the two calls never reallocates.  The automatic scale launches two kernels (a per-slot
+ * maximum into a workspace allocated on the first call, then the colors), a fixed scale one.  Enqueued on the context's
+ * stream; not part of ofdis_run's graph.  The flows are not changed. */
+int ofdis_flow_color_fullres(ofdis_ctx* ctx, int f0, int f1, unsigned char* rgb, float* scale, float max_value,
+                             int width_org, int height_org, int memkind);
 
 /* Init flow from a flow of the original frame size (extension; the reference's disabled file input,
  * run_dense.cpp:292-301,355-378).  `flow` = [f1-f0][height_org][width_org][nop] floats.  Prepares the initflow of

@@ -34,7 +34,7 @@ EXPORTS = [
     "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8", "ofdis_set_initflow_fullres",
     "ofdis_set_initflow_from_result", "ofdis_upload_sequence_bidir_u8", "ofdis_set_swapped_slots",
     "ofdis_consistency_fullres", "ofdis_flow_error_fullres", "ofdis_debug_sor_plan",
-    "ofdis_get_flow_fullres_encoded",
+    "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres",
 ]
 
 # encodings of get_flow_fullres_encoded (OFDIS_ENC_F16, OFDIS_ENC_KITTI)
@@ -102,6 +102,8 @@ def lib():
                                              ctypes.c_int, ctypes.c_int]
         L.ofdis_get_flow_fullres_encoded.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] + \
             [ctypes.c_int] * 3
+        L.ofdis_flow_color_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 2 + \
+            [ctypes.c_float] + [ctypes.c_int] * 3
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -357,6 +359,31 @@ class Context:
         if memkind == MEM_HOST:
             self.sync()
         return out
+
+    def flow_color_fullres(self, f0, f1, width_org, height_org, max_value=0.0, out=None, with_scale=False,
+                           memkind=MEM_HOST, scale=None):
+        """The color images of slots [f0, f1) computed on the device: Middlebury's color wheel for flow, KITTI's
+        disparity map for stereo (the contract is ofdis_flow_color_fullres's, restated by preprocess.flow_to_color /
+        disp_to_color).  max_value > 0 fixes the scale; 0 takes each slot's own maximum.  Returns (rgb, scale).  Host:
+        rgb a (f1-f0, height_org, width_org, 3) uint8 array and scale a (f1-f0,) float32 array (None unless
+        with_scale), each new or given as a numpy array of exactly that dtype and shape; the call then synchronises
+        the stream.  With memkind=MEM_DEVICE, out and scale are device addresses the caller owns (scale may be None)
+        and are returned as given."""
+        if memkind == MEM_HOST:
+            n = max(f1 - f0, 0)
+            out = np.empty((n, height_org, width_org, 3), np.uint8) if out is None else out
+            scale = (np.empty(n, np.float32) if scale is None else scale) if with_scale else None
+            for name, arr, dt, shape in (("out", out, np.uint8, (n, height_org, width_org, 3)),
+                                         ("scale", scale, np.float32, (n,))):
+                if arr is not None and not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape == shape
+                                            and arr.flags["C_CONTIGUOUS"] and arr.flags["WRITEABLE"]):
+                    raise ValueError("flow_color_fullres: %s must be a writeable C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shape))
+        self._ck(lib().ofdis_flow_color_fullres(self._h, f0, f1, _ptr(out), _ptr(scale), max_value, width_org,
+                                                height_org, memkind))
+        if memkind == MEM_HOST:
+            self.sync()
+        return out, scale
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

@@ -67,6 +67,9 @@ struct ofdis_ctx {
   // lazily allocated workspace of ofdis_flow_error_fullres: the row partials [max_frames][16][height], then the
   // device stats [max_frames][16]; never touched by ofdis_run
   ErrRowPartial* d_eval = nullptr;
+  // lazily allocated workspace of ofdis_flow_color_fullres: the automatic scales' maxima [max_frames] as float bit
+  // patterns; never touched by ofdis_run
+  unsigned int* d_color = nullptr;
   std::vector<float*> d_flow;      // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -427,6 +430,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_stage);
   cudaFree(ctx->d_full);
   cudaFree(ctx->d_eval);
+  cudaFree(ctx->d_color);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -859,6 +863,44 @@ int ofdis_get_flow_fullres_encoded(ofdis_ctx* ctx, int f0, int f1, int encoding,
   ctx->launches += 1;
   if (memkind != OFDIS_MEM_DEVICE)
     CK(cudaMemcpyAsync(out, dst, sizeof(unsigned short) * per * (size_t)(f1 - f0), cudaMemcpyDeviceToHost, ctx->stream));
+  return OFDIS_OK;
+}
+
+int ofdis_flow_color_fullres(ofdis_ctx* ctx, int f0, int f1, unsigned char* rgb, float* scale, float max_value,
+                             int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !rgb || !(max_value >= 0.f && max_value <= FLT_MAX) ||
+      (memkind == OFDIS_MEM_DEVICE && reinterpret_cast<uintptr_t>(scale) % sizeof(float)))
+    return fail(ctx, OFDIS_ERR_ARG, "flow_color_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("color", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0;
+  const size_t pix = (size_t)width_org * height_org;
+  if (!ctx->d_color && cudaMalloc((void**)&ctx->d_color, sizeof(unsigned int) * ctx->max_frames) != cudaSuccess) {
+    ctx->d_color = nullptr;
+    return fail(ctx, OFDIS_ERR_NOMEM, "flow_color_fullres workspace");
+  }
+  unsigned char* drgb = rgb;
+  float* dscale = scale;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    // the full-resolution scratch: the images, then the scales at the next float; the size ofdis_get_flow_fullres
+    // asks for holds both unless a frame has fewer than 8 pixels
+    rc = ensure_full(ctx, std::max(pix * ctx->nop, (3 * pix + 7) / 4 + 1) * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    drgb = reinterpret_cast<unsigned char*>(ctx->d_full);
+    dscale = scale ? ctx->d_full + (3 * pix * n + 3) / 4 : nullptr;
+  }
+  const int k = launch_flow_color(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, n, ctx->d_color, max_value, drgb,
+                                  dscale, width_org, height_org, cx, cy, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "flow_color_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    CK(cudaMemcpyAsync(rgb, drgb, 3 * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (scale) CK(cudaMemcpyAsync(scale, dscale, sizeof(float) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  }
   return OFDIS_OK;
 }
 

@@ -254,6 +254,159 @@ __global__ void __launch_bounds__(256) flow_encode_kernel(LevelGeom g, int f0, u
   }
 }
 
+// Color coding of the full-resolution flow F (ofdis_flow_color_fullres; the header states the contract,
+// preprocess.atan2_f32 / flow_to_color / disp_to_color restate it bit for bit).  The tables, built once at compile
+// time in float32: Middlebury's color wheel (makecolorwheel, integer division) divided by 255, and the eight-entry
+// map of KITTI's stereo devkit (disp_to_color) with its bin weights and cumulative bin edges.
+constexpr float PI_F = 3.14159265358979323846f;
+constexpr int WHEEL = 55;
+struct ColorTables {
+  float wheel[WHEEL][3];  // W[k][b] / 255.0f
+  float disp_map[8][3];   // M[i][0..2]
+  float disp_wt[7];       // 1000.0f / M[i][3]
+  float disp_cum[8];      // cum[0] = 0, cum[i + 1] = cum[i] + M[i][3] / 1000.0f
+  float atan_c[8];        // the polynomial of atan2_f32
+};
+constexpr ColorTables make_color_tables() {
+  ColorTables t{};
+  constexpr int seg[6] = {15, 6, 4, 11, 13, 6};  // RY, YG, GC, CB, BM, MR
+  int k = 0;
+  for (int s = 0; s < 6; ++s)
+    for (int i = 0; i < seg[s]; ++i, ++k) {
+      const int up = 255 * i / seg[s], down = 255 - 255 * i / seg[s];
+      const int w[6][3] = {{255, up, 0}, {down, 255, 0}, {0, 255, up}, {0, down, 255}, {up, 0, 255}, {255, 0, down}};
+      for (int b = 0; b < 3; ++b) t.wheel[k][b] = (float)w[s][b] / 255.0f;
+    }
+  constexpr int M[8][4] = {{0, 0, 0, 114}, {0, 0, 1, 185}, {1, 0, 0, 114}, {1, 0, 1, 174},
+                           {0, 1, 0, 114}, {0, 1, 1, 185}, {1, 1, 0, 114}, {1, 1, 1, 0}};
+  for (int i = 0; i < 8; ++i)
+    for (int c = 0; c < 3; ++c) t.disp_map[i][c] = (float)M[i][c];
+  t.disp_cum[0] = 0.0f;
+  for (int i = 0; i < 7; ++i) {
+    t.disp_wt[i] = 1000.0f / (float)M[i][3];
+    t.disp_cum[i + 1] = t.disp_cum[i] + (float)M[i][3] / 1000.0f;
+  }
+  // atan(t) ~ t * (C0 + s * (C1 + ... + s * C7)), s = t * t, fitted on [0, 1] (|error| < 4e-8 before rounding)
+  constexpr float C[8] = {0.99999934f, -0.3332986f, 0.19946565f, -0.13908629f,
+                          0.09642195f, -0.055912293f, 0.021862935f, -0.0040545613f};
+  for (int k = 0; k < 8; ++k) t.atan_c[k] = C[k];
+  return t;
+}
+__constant__ ColorTables kColor = make_color_tables();
+
+// The library's float32 atan2: octant reduction to t = min / max in [0, 1] (0 where both are 0), the odd degree-15
+// polynomial kColor.atan_c (Horner in s = t * t), then pi/2 - p, pi - p and the sign, all on the sign bits,
+// so the signed zeros and the axes follow C.  |error| <= 1e-6 against float64 atan2; every finite input gives a value
+// in [-PI_F, PI_F].
+__device__ __forceinline__ float atan2_f32(float y, float x) {
+  const float ax = fabsf(x), ay = fabsf(y), mx = fmaxf(ax, ay), mn = fminf(ax, ay);
+  const float t = mx > 0.0f ? mn / mx : 0.0f, s = t * t;
+  float q = kColor.atan_c[7];
+#pragma unroll
+  for (int k = 6; k >= 0; --k) q = q * s + kColor.atan_c[k];
+  float p = t * q;
+  p = ay > ax ? PI_F * 0.5f - p : p;
+  p = signbit(x) ? PI_F - p : p;
+  return signbit(y) ? -p : p;
+}
+
+// What the automatic scale is the maximum of: flow the radius of a known pixel (|u|, |v| <= 1e9, so NaN and the
+// infinities are unknown), stereo the valid disparity d (0 <= d <= 1e9; d = -F, +F in a slot marked swapped).  +0
+// elsewhere, never -0, so the bit patterns order as the values do.
+template <int NOP>
+__device__ __forceinline__ float color_magnitude(const LevelGeom& g, int frame, const float f[2]) {
+  if constexpr (NOP == 2) {
+    const bool known = fabsf(f[0]) <= 1e9f && fabsf(f[1]) <= 1e9f;
+    return known ? sqrtf(f[0] * f[0] + f[1] * f[1]) : 0.0f;
+  } else {
+    const float d = swapped_of(g, frame) ? f[0] : -f[0];
+    return d > 0.0f && d <= 1e9f ? d : 0.0f;
+  }
+}
+
+// The automatic scale's maximum of slot fr: a block max of color_magnitude over the slot's full-resolution pixels,
+// then an atomicMax of its bit pattern (non-negative floats order as their patterns) into words[fr], which the
+// launcher zeroes first.  One thread per full-resolution pixel, blocks of 32 x 8.
+template <int NOP>
+__global__ void __launch_bounds__(256) flow_color_scale_kernel(LevelGeom g, int f0, unsigned int* words, int w_org,
+                                                               int h_org, int crop_x, int crop_y) {
+  __shared__ float warp_max[8];
+  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
+  const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y * blockDim.y + threadIdx.y;
+  const int fr = blockIdx.z, frame = frame_of(g, f0, fr);
+  float m = 0.0f;
+  if (X < w_org && Y < h_org) {
+    float f[2] = {0.f, 0.f};
+    upsample_at<NOP>(g, g.flow + (size_t)frame * g.flow_frame_stride, X, Y, crop_x, crop_y,
+                     [&f](int c, float v) { f[c] = v; });
+    m = color_magnitude<NOP>(g, frame, f);
+  }
+  for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (threadIdx.x == 0) warp_max[threadIdx.y] = m;
+  __syncthreads();
+  if (threadIdx.x == 0 && threadIdx.y == 0) {
+    for (int k = 1; k < 8; ++k) m = fmaxf(m, warp_max[k]);
+    if (m > 0.0f) atomicMax(words + fr, __float_as_uint(m));
+  }
+}
+
+// The color image of slot fr, 3 bytes (R, G, B) per full-resolution pixel, from F (upsample_at) without storing it:
+//   flow (Middlebury's computeColor): unknown black; else fx = u / scale, fy = v / scale, rad = |(fx, fy)|,
+//     a = atan2_f32(-v, -u) / PI_F of the unscaled flow, fk = (a + 1) / 2 * 54, the wheel entries k0 = (int)fk and
+//     (k0 + 1) % 55 mixed by f = fk - k0, whitened towards the centre (rad <= 1) or darkened by 0.75 beyond it;
+//   stereo (KITTI's disp_to_color): invalid black; else val = clamp(d / scale, 0, 1) in the first bin i with
+//     val < cum[i + 1] (else 6), mixed between map entries i and i + 1.
+// scale = max_value when it is > 0, else the slot's maximum (words[fr]): flow 1 where it is 0, stereo at least 1;
+// where scale_out is given, pixel (0, 0) writes it to scale_out[fr].  One thread per full-resolution pixel.
+template <int NOP>
+__global__ void __launch_bounds__(256) flow_color_kernel(LevelGeom g, int f0, const unsigned int* words,
+                                                         float max_value, unsigned char* rgb, float* scale_out,
+                                                         int w_org, int h_org, int crop_x, int crop_y) {
+  pdl_wait();  // programmatic dependent launch: nothing of the previous kernel is touched before this
+  const int X = blockIdx.x * blockDim.x + threadIdx.x, Y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (X >= w_org || Y >= h_org) return;
+  const int fr = blockIdx.z, frame = frame_of(g, f0, fr);
+  float scale = max_value;
+  if (!(max_value > 0.0f)) {
+    const float m = __uint_as_float(words[fr]);
+    scale = NOP == 2 ? (m == 0.0f ? 1.0f : m) : fmaxf(m, 1.0f);
+  }
+  if (scale_out && X == 0 && Y == 0) scale_out[fr] = scale;
+  float f[2] = {0.f, 0.f};
+  upsample_at<NOP>(g, g.flow + (size_t)frame * g.flow_frame_stride, X, Y, crop_x, crop_y,
+                   [&f](int c, float v) { f[c] = v; });
+  unsigned char col[3] = {0, 0, 0};
+  if constexpr (NOP == 2) {
+    const float u = f[0], v = f[1];
+    if (fabsf(u) <= 1e9f && fabsf(v) <= 1e9f) {
+      const float fx = u / scale, fy = v / scale, rad = sqrtf(fx * fx + fy * fy);
+      const float a = atan2_f32(-v, -u) / PI_F;
+      const float fk = (a + 1.0f) / 2.0f * (float)(WHEEL - 1);
+      const int k0 = (int)fk, k1 = (k0 + 1) % WHEEL;
+      const float fr_k = fk - (float)k0;
+      for (int b = 0; b < 3; ++b) {
+        float c = (1.0f - fr_k) * kColor.wheel[k0][b] + fr_k * kColor.wheel[k1][b];
+        c = rad <= 1.0f ? 1.0f - rad * (1.0f - c) : c * 0.75f;
+        col[b] = (unsigned char)(255.0f * c);
+      }
+    }
+  } else {
+    const float d = swapped_of(g, frame) ? f[0] : -f[0];
+    if (d >= 0.0f && d <= 1e9f) {  // NaN fails, -0 passes
+      const float val = fminf(fmaxf(d / scale, 0.0f), 1.0f);
+      int i = 6;
+#pragma unroll
+      for (int k = 6; k >= 0; --k) i = val < kColor.disp_cum[k + 1] ? k : i;  // the first bin that holds val
+      const float w = 1.0f - (val - kColor.disp_cum[i]) * kColor.disp_wt[i];
+      for (int c = 0; c < 3; ++c)
+        col[c] = (unsigned char)fminf(
+            fmaxf((w * kColor.disp_map[i][c] + (1.0f - w) * kColor.disp_map[i + 1][c]) * 255.0f, 0.0f), 255.0f);
+    }
+  }
+  unsigned char* o = rgb + ((size_t)fr * h_org * w_org + (size_t)Y * w_org + X) * 3;
+  for (int b = 0; b < 3; ++b) o[b] = col[b];
+}
+
 // Forward-backward (flow) / left-right (stereo) consistency (Sundaram, Brox, Keutzer, ECCV 2010) of frame fa's
 // full-resolution flow F against frame fb's B, both exactly what flow_upsample_kernel writes, evaluated from the
 // level flows (upsample_at) where they are needed instead of through a full-resolution copy.  Per pixel, in
@@ -541,6 +694,24 @@ int launch_flow_encode(const LevelGeom& g, int f0, int n, int enc, unsigned shor
     return -1;
   }
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_flow_color(const LevelGeom& g, int f0, int n, unsigned int* words, float max_value, unsigned char* rgb,
+                      float* scale, int w_org, int h_org, int crop_x, int crop_y, cudaStream_t st) {
+  const dim3 block(32, 8), grid((w_org + 31) / 32, (h_org + 7) / 8, n);
+  const bool automatic = !(max_value > 0.0f);
+  if (automatic) {
+    if (cudaMemsetAsync(words, 0, sizeof(unsigned int) * n, st) != cudaSuccess) return -1;
+    if (g.nop == 2) flow_color_scale_kernel<2><<<grid, block, 0, st>>>(g, f0, words, w_org, h_org, crop_x, crop_y);
+    else flow_color_scale_kernel<1><<<grid, block, 0, st>>>(g, f0, words, w_org, h_org, crop_x, crop_y);
+    if (cudaGetLastError() != cudaSuccess) return -1;
+  }
+  if (g.nop == 2)
+    flow_color_kernel<2><<<grid, block, 0, st>>>(g, f0, words, max_value, rgb, scale, w_org, h_org, crop_x, crop_y);
+  else
+    flow_color_kernel<1><<<grid, block, 0, st>>>(g, f0, words, max_value, rgb, scale, w_org, h_org, crop_x, crop_y);
+  if (cudaGetLastError() != cudaSuccess) return -1;
+  return automatic ? 2 : 1;
 }
 
 int launch_consistency(const LevelGeom& g, int fa, int fb, int n, unsigned char* mask, float* err, int w_org,

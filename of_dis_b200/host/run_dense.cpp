@@ -13,6 +13,7 @@
 #include <sys/time.h>
 #include <zlib.h>
 
+#include <cfloat>
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
@@ -576,6 +577,13 @@ int main(int argc, char** argv) {
 // bytes per pixel come back instead of 8 or 4.  Flow: RGB16 (u * 64 + 2^15, v * 64 + 2^15, 1), (0, 0, 0) where the
 // flow is NaN; stereo: gray16 d * 256 of the positive disparity d (the left view's -F, a _bw file's right-view +F),
 // clamped to [1, 65535], 0 where d is negative or NaN.  The _occ.pgm masks and the EVAL lines do not change.
+//
+// --color: every output also gets <stem>_color.png (with --bidirectional also <stem>_bw_color.png), an 8-bit RGB PNG
+// of the flow colored on the device (ofdis_flow_color_fullres): Middlebury's color wheel for flow, the color map of
+// KITTI's stereo devkit for the positive disparity (a _bw file's right-view +F).  Each pair is colored with its own
+// maximum, as Middlebury's tool does; --color-max M (a positive finite number; it needs --color) colors every pair
+// with the scale M, so that the frames of a clip compare.  3 bytes per pixel come back for it.  The other output files
+// keep their bytes.
 
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
@@ -719,15 +727,21 @@ static bool read_gt_file(const char* path, int w, int h, int nop, vector<float>&
   return read_flow_file(path, w, h, nop, what, flow, err);
 }
 
-// KITTI's 16-bit PNG of one encoded slot (`ch` = 3: RGB16, 1: gray16): IHDR, one IDAT of filter-0 rows with the
-// samples big-endian, IEND
-static void save_kitti_png(const uint16_t* enc, int w, int h, int ch, const char* filename) {
-  const size_t stride = (size_t)w * ch * 2;
+// A PNG of one slot with `depth` 16 (uint16 samples in host order; KITTI's flow RGB16 for `ch` = 3, disparity gray16
+// for 1) or 8 (bytes; the RGB color images of --color): IHDR, one IDAT of filter-0 rows with the samples big-endian,
+// IEND
+static void save_png(const void* samples, int w, int h, int ch, int depth, const char* filename) {
+  const int bytes = depth / 8;
+  const size_t stride = (size_t)w * ch * bytes;
   vector<uint8_t> raw((stride + 1) * h);
   for (int y = 0; y < h; ++y) {
     uint8_t* r = &raw[(stride + 1) * y];
     r[0] = 0;
-    const uint16_t* s = enc + (size_t)y * w * ch;
+    if (bytes == 1) {
+      memcpy(r + 1, static_cast<const uint8_t*>(samples) + (size_t)y * stride, stride);
+      continue;
+    }
+    const uint16_t* s = static_cast<const uint16_t*>(samples) + (size_t)y * w * ch;
     for (size_t k = 0; k < (size_t)w * ch; ++k) {
       r[1 + 2 * k] = (uint8_t)(s[k] >> 8);
       r[2 + 2 * k] = (uint8_t)(s[k] & 0xff);
@@ -755,7 +769,7 @@ static void save_kitti_png(const uint16_t* enc, int w, int h, int ch, const char
   };
   const uint8_t ihdr[13] = {(uint8_t)(w >> 24), (uint8_t)(w >> 16), (uint8_t)(w >> 8), (uint8_t)w,
                             (uint8_t)(h >> 24), (uint8_t)(h >> 16), (uint8_t)(h >> 8), (uint8_t)h,
-                            16, (uint8_t)(ch == 3 ? 2 : 0), 0, 0, 0};
+                            (uint8_t)depth, (uint8_t)(ch == 3 ? 2 : 0), 0, 0, 0};
   chunk("IHDR", ihdr, 13);
   chunk("IDAT", z.data(), (uint32_t)zlen);
   chunk("IEND", nullptr, 0);
@@ -781,6 +795,7 @@ int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr,
             "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
+            "       [--color [--color-max M]]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -791,12 +806,17 @@ int main(int argc, char** argv) {
             "  EVAL lines (end-point error, shares above 1, 3, 5 px, KITTI outliers; with --bidirectional also per\n"
             "  consistency class)\n"
             "  --kitti: write every flow (and _bw) output as KITTI's 16-bit PNG (flow RGB16, stereo gray16 disparity),\n"
-            "  whatever its extension\n",
+            "  whatever its extension\n"
+            "  --color: also write <stem>_color.png (and <stem>_bw_color.png), the 8-bit RGB color coding of every\n"
+            "  output (flow: Middlebury's color wheel, stereo: KITTI's disparity colors), colored on the device\n"
+            "  --color-max M: color every pair with the scale M (a positive finite number) instead of its own maximum\n",
             argv[0]);
     return 2;
   }
   int maxb = 64, first_num = 2;
-  bool warm = false, batch_set = false, bidir = false, kitti = false;
+  bool warm = false, batch_set = false, bidir = false, kitti = false, color = false;
+  float color_max = 0.0f;  // --color-max; 0: every pair's own maximum
+  const char* color_max_arg = nullptr;
   const char* gtlist = nullptr;
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
@@ -812,6 +832,16 @@ int main(int argc, char** argv) {
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--kitti")) {
       kitti = true;
       first_num += 1;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--color")) {
+      color = true;
+      first_num += 1;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--color-max")) {
+      if (argc < first_num + 2 || color_max_arg) {
+        fprintf(stderr, "error: --color-max takes one positive number\n");
+        return 2;
+      }
+      color_max_arg = argv[first_num + 1];
+      first_num += 2;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
         fprintf(stderr, "error: --gt takes one ground-truth list file\n");
@@ -830,6 +860,18 @@ int main(int argc, char** argv) {
   if (warm && bidir) {
     fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --bidirectional\n");
     return 2;
+  }
+  if (color_max_arg) {
+    char* end = nullptr;
+    color_max = strtof(color_max_arg, &end);
+    if (!color) {
+      fprintf(stderr, "error: --color-max needs --color\n");
+      return 2;
+    }
+    if (end == color_max_arg || *end || !(color_max > 0.0f && color_max <= FLT_MAX)) {
+      fprintf(stderr, "error: --color-max takes a positive finite number, got %s\n", color_max_arg);
+      return 2;
+    }
   }
   if (warm) maxb = 1;
   const int nnum = argc - first_num;
@@ -894,6 +936,7 @@ int main(int argc, char** argv) {
   vector<float> flows;
   vector<uint16_t> kflows;  // --kitti: the encoded slots
   vector<uint8_t> masks;
+  vector<uint8_t> colors;  // --color: the color images of the slots
   Image8 last;  // image2 of the previous batch's last pair
   size_t j0 = 0;
   while (j0 < jobs.size()) {
@@ -995,6 +1038,10 @@ int main(int argc, char** argv) {
     if (rc == OFDIS_OK)
       rc = kitti ? ofdis_get_flow_fullres_encoded(ctx, 0, slots, OFDIS_ENC_KITTI, kflows.data(), w, h, OFDIS_MEM_HOST)
                  : ofdis_get_flow_fullres(ctx, 0, slots, flows.data(), w, h, OFDIS_MEM_HOST);
+    if (rc == OFDIS_OK && color) {
+      colors.resize((size_t)slots * w * h * 3);
+      rc = ofdis_flow_color_fullres(ctx, 0, slots, colors.data(), nullptr, color_max, w, h, OFDIS_MEM_HOST);
+    }
     if (rc == OFDIS_OK && bidir) {
       masks.resize((size_t)n * w * h);
       rc = ofdis_consistency_fullres(ctx, 0, n, n, masks.data(), nullptr, nop == 2 ? 0.01f : 0.0f,
@@ -1027,12 +1074,18 @@ int main(int argc, char** argv) {
       return 1;
     }
     for (int k = 0; k < n && kitti; ++k) {
-      save_kitti_png(kflows.data() + (size_t)k * w * h * kch, w, h, kch, jobs[j0 + k].out.c_str());
+      save_png(kflows.data() + (size_t)k * w * h * kch, w, h, kch, 16, jobs[j0 + k].out.c_str());
       if (bidir) {
-        save_kitti_png(kflows.data() + (size_t)(n + k) * w * h * kch, w, h, kch,
-                       with_suffix(jobs[j0 + k].out, "_bw").c_str());
+        save_png(kflows.data() + (size_t)(n + k) * w * h * kch, w, h, kch, 16,
+                 with_suffix(jobs[j0 + k].out, "_bw").c_str());
         save_mask_pgm(masks.data() + (size_t)k * w * h, w, h, with_suffix(jobs[j0 + k].out, "_occ", ".pgm").c_str());
       }
+    }
+    for (int k = 0; k < n && color; ++k) {
+      save_png(colors.data() + (size_t)k * w * h * 3, w, h, 3, 8, with_suffix(jobs[j0 + k].out, "_color", ".png").c_str());
+      if (bidir)
+        save_png(colors.data() + (size_t)(n + k) * w * h * 3, w, h, 3, 8,
+                 with_suffix(jobs[j0 + k].out, "_bw_color", ".png").c_str());
     }
     ImageF out;
     out.w = w; out.h = h; out.c = nop;

@@ -477,3 +477,142 @@ def read_kitti_png(path: str) -> np.ndarray:
         up = img[y]
     out = img.view(">u2").astype(np.uint16)
     return out.reshape(h, w, 3) if ch == 3 else out.reshape(h, w)
+
+
+# ---- color-coded flows (ofdis_flow_color_fullres) -------------------------------------------------------------------
+PI_F = np.float32(np.pi)
+# the odd polynomial of atan2_f32: atan(t) ~ t * (C0 + s * (C1 + ... + s * C7)), s = t * t, fitted on [0, 1]
+ATAN_C = np.array([0.99999934, -0.3332986, 0.19946565, -0.13908629, 0.09642195, -0.055912293, 0.021862935,
+                   -0.0040545613], np.float32)
+COLOR_UNKNOWN_THRESH = np.float32(1e9)  # |u|, |v| (flow) or d (stereo) above this, or NaN, is not colored
+
+
+def make_color_wheel() -> np.ndarray:
+    """Middlebury's makecolorwheel: 55 (R, G, B) int entries, integer division; segments RY 15, YG 6, GC 4, CB 11,
+    BM 13, MR 6."""
+    w = []
+    for i in range(15):
+        w.append((255, 255 * i // 15, 0))
+    for i in range(6):
+        w.append((255 - 255 * i // 6, 255, 0))
+    for i in range(4):
+        w.append((0, 255, 255 * i // 4))
+    for i in range(11):
+        w.append((0, 255 - 255 * i // 11, 255))
+    for i in range(13):
+        w.append((255 * i // 13, 0, 255))
+    for i in range(6):
+        w.append((255, 0, 255 - 255 * i // 6))
+    return np.array(w, np.int32)
+
+
+COLOR_WHEEL = make_color_wheel()
+# KITTI's stereo devkit (disp_to_color): (R, G, B, bin width in 1/1000 of the scale)
+DISP_COLOR_MAP = np.array([[0, 0, 0, 114], [0, 0, 1, 185], [1, 0, 0, 114], [1, 0, 1, 174], [0, 1, 0, 114],
+                           [0, 1, 1, 185], [1, 1, 0, 114], [1, 1, 1, 0]], np.int32)
+
+
+def disp_color_bins():
+    """(wt[0..6], cum[0..7]) in float32: wt[i] = 1000.0f / M[i][3], cum[i+1] = cum[i] + M[i][3] / 1000.0f in order."""
+    f32 = np.float32
+    wt = np.array([f32(1000) / f32(DISP_COLOR_MAP[i, 3]) for i in range(7)], f32)
+    cum = [f32(0)]
+    for i in range(7):
+        cum.append(f32(cum[i] + f32(DISP_COLOR_MAP[i, 3]) / f32(1000)))
+    return wt, np.array(cum, f32)
+
+
+def atan2_f32(y, x) -> np.ndarray:
+    """The library's float32 atan2, the same expressions as the device's: t = min(|x|, |y|) / max(|x|, |y|) (0 where
+    both are 0), p = t * poly(t * t) by Horner with ATAN_C, then pi/2 - p where |y| > |x|, pi - p where x's sign bit
+    is set, and y's sign.  Within 1e-6 of float64 arctan2, in [-PI_F, PI_F] for finite input; C's signed zeros."""
+    f32 = np.float32
+    y, x = np.asarray(y, f32), np.asarray(x, f32)
+    ax, ay = np.abs(x), np.abs(y)
+    mx, mn = np.maximum(ax, ay), np.minimum(ax, ay)
+    with np.errstate(invalid="ignore", divide="ignore", over="ignore", under="ignore"):
+        t = np.where(mx > 0, mn / np.where(mx > 0, mx, f32(1)), f32(0)).astype(f32)
+        s = t * t
+        q = np.full_like(s, ATAN_C[7])
+        for k in range(6, -1, -1):
+            q = q * s + ATAN_C[k]
+        p = t * q
+        p = np.where(ay > ax, PI_F * f32(0.5) - p, p)
+        p = np.where(np.signbit(x), PI_F - p, p)
+        return np.where(np.signbit(y), -p, p).astype(f32)
+
+
+def _slots(flow: np.ndarray, nop: int) -> np.ndarray:
+    F = np.asarray(flow, np.float32)
+    assert F.ndim in (3, 4) and F.shape[-1] == nop, (F.shape, nop)
+    return F
+
+
+def flow_to_color(flow: np.ndarray, max_value: float = 0.0):
+    """ofdis_flow_color_fullres for flow, bit for bit: Middlebury's MotionToColor / computeColor in float32 without
+    contraction.  flow: one slot (h, w, 2) or a batch (n, h, w, 2).  Returns (rgb, scale): (..., 3) uint8 and the
+    scale of every slot (float32 scalar for one slot, (n,) for a batch)."""
+    f32 = np.float32
+    F = _slots(flow, 2)
+    one = F.ndim == 3
+    F = F[None] if one else F
+    u, v = F[..., 0], F[..., 1]
+    known = (np.abs(u) <= COLOR_UNKNOWN_THRESH) & (np.abs(v) <= COLOR_UNKNOWN_THRESH)  # NaN fails both
+    uk, vk = np.where(known, u, f32(0)), np.where(known, v, f32(0))
+    with np.errstate(over="ignore", under="ignore", invalid="ignore"):  # inf * 0 only in the branch not taken
+        rad0 = np.sqrt(uk * uk + vk * vk).astype(f32)
+        if max_value > 0:
+            scale = np.full(F.shape[0], max_value, f32)
+        else:
+            m = rad0.reshape(F.shape[0], -1).max(axis=1, initial=f32(0)).astype(f32)
+            scale = np.where(m == 0, f32(1), m).astype(f32)
+        sc = scale[:, None, None]
+        fx, fy = uk / sc, vk / sc
+        rad = np.sqrt(fx * fx + fy * fy).astype(f32)
+        a = atan2_f32(-vk, -uk) / PI_F
+        fk = (a + f32(1)) / f32(2) * f32(54)
+        k0 = fk.astype(np.int32)
+        k1 = (k0 + 1) % 55
+        fr = fk - k0.astype(f32)
+        rgb = np.zeros(F.shape[:-1] + (3,), np.uint8)
+        for b in range(3):
+            w0 = COLOR_WHEEL[k0, b].astype(f32) / f32(255)
+            w1 = COLOR_WHEEL[k1, b].astype(f32) / f32(255)
+            col = (f32(1) - fr) * w0 + fr * w1
+            col = np.where(rad <= f32(1), f32(1) - rad * (f32(1) - col), col * f32(0.75))
+            rgb[..., b] = np.where(known, (f32(255) * col).astype(np.uint8), np.uint8(0))
+    return (rgb[0], scale[0]) if one else (rgb, scale)
+
+
+def disp_to_color(flow: np.ndarray, max_value: float = 0.0, swapped=False):
+    """ofdis_flow_color_fullres for stereo, bit for bit: KITTI's disp_to_color in float32 without contraction.
+    flow: one slot (h, w, 1) or a batch (n, h, w, 1) in this library's sign; d = -F, or +F where `swapped` (a bool, or
+    one per slot of a batch).  Returns (rgb, scale) as flow_to_color does."""
+    f32 = np.float32
+    F = _slots(flow, 1)
+    one = F.ndim == 3
+    F = F[None] if one else F
+    sw = np.broadcast_to(np.asarray(swapped, bool), (F.shape[0],))
+    d = np.where(sw[:, None, None], F[..., 0], -F[..., 0])
+    with np.errstate(invalid="ignore"):
+        valid = (d >= 0) & (d <= COLOR_UNKNOWN_THRESH)
+    dv = np.where(valid, d, f32(0))
+    if max_value > 0:
+        scale = np.full(F.shape[0], max_value, f32)
+    else:
+        m = dv.reshape(F.shape[0], -1).max(axis=1, initial=f32(0)).astype(f32)
+        scale = np.fmax(m, f32(1)).astype(f32)
+    wt, cum = disp_color_bins()
+    with np.errstate(over="ignore", under="ignore"):
+        val = np.fmin(np.fmax(dv / scale[:, None, None], f32(0)), f32(1))
+        i = np.full(val.shape, 6, np.int32)
+        for k in range(6, -1, -1):
+            i = np.where(val < cum[k + 1], k, i)
+        w = f32(1) - (val - cum[i]) * np.concatenate([wt, [f32(0)]])[i]
+        rgb = np.zeros(F.shape[:-1] + (3,), np.uint8)
+        for c in range(3):
+            m0 = DISP_COLOR_MAP[i, c].astype(f32)
+            m1 = DISP_COLOR_MAP[i + 1, c].astype(f32)
+            x = np.fmin(np.fmax((w * m0 + (f32(1) - w) * m1) * f32(255), f32(0)), f32(255))
+            rgb[..., c] = np.where(valid, x.astype(np.uint8), np.uint8(0))
+    return (rgb[0], scale[0]) if one else (rgb, scale)
