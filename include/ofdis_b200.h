@@ -299,6 +299,53 @@ int ofdis_get_flow_fullres_encoded(ofdis_ctx* ctx, int f0, int f1, int encoding,
  * stream; not part of ofdis_run's graph.  The flows are not changed. */
 int ofdis_flow_color_fullres(ofdis_ctx* ctx, int f0, int f1, unsigned char* rgb, float* scale, float max_value,
                              int width_org, int height_org, int memkind);
+/* Frame interpolation from bidirectional flows (extension): the frame at time t between I0 and I1 of every pair
+ * k < f1-f0.  Slot a = f0+k holds the forward flow F (I0 -> I1) of the last run and slot b0+k its backward partner B
+ * (I1 -> I0): the layout of ofdis_upload_sequence_bidir_u8 (b0 = n), or of pairs followed by their swapped copies.
+ * F and B are exactly what ofdis_get_flow_fullres returns, computed from the level flows without a full-resolution
+ * copy; stereo (nop 1) uses F as a horizontal flow with v = 0, which gives the view at fraction t between the two
+ * cameras (swapped marks need no special case).  i0, i1: the 8-bit frames [height_org][width_org][noc] in the
+ * context's channel count, frame k at i0 + k*frame_stride and i1 + k*frame_stride, frame_stride >= height_org *
+ * width_org * noc (a clip: i1 = i0 + hwc, stride hwc; the pairs of ofdis_upload_frames_u8: stride 2hwc).
+ * out = [f1-f0][height_org][width_org][noc] bytes; flow_t = NULL or [f1-f0][height_org][width_org][nop] float32, the
+ * filled flow u_t at time t.  The algorithm follows the description of the interpolation in Baker et al.'s
+ * evaluation (IJCV 2011); it has not been compared with their implementation.  Everything is float32 without
+ * contraction, with IEEE division; preprocess.interpolate_frames restates it.  W = width_org, H = height_org;
+ * bil(I, xs, ys) is the bilinear rule of ofdis_consistency_fullres on the (float) byte values: x0 = floor(xs),
+ * x1 = min(x0 + 1, W - 1), fx = xs - x0 (the same in y), per channel r0 = I(x0,y0)*(1-fx) + I(x1,y0)*fx,
+ * r1 = I(x0,y1)*(1-fx) + I(x1,y1)*fx, bil = r0*(1-fy) + r1*fy.  "In the frame" is 0 <= x <= W-1 and 0 <= y <= H-1.
+ * Per pair:
+ *   1. m0 = the mask ofdis_consistency_fullres(alpha, beta) gives F against B (every pixel of I0), m1 the mask of B
+ *      against F (every pixel of I1), bitwise; a pixel whose mask is not 0 (1, or 2: it leaves the frame) is
+ *      occluded in the other frame.
+ *   2. Cost of source pixel (X, Y) of I0: xs = X + u, ys = Y + v with (u, v) = F(X, Y); c = +inf when (xs, ys) is
+ *      not in the frame (or NaN), else c = 0, then c += fabsf(I0(X,Y)[ch] - bil(I1, xs, ys)[ch]) in channel order.
+ *   3. Forward splat: a source with |u| <= 1e9 and |v| <= 1e9 (NaN fails) has the target p = (X + t*u, Y + t*v) and
+ *      reaches every pixel of the frame with a non-zero bilinear weight at p: x = floor(px), and floor(px) + 1 when
+ *      px > floor(px), the same in y.  Every target keeps the source with the smallest 64-bit key
+ *      (bits(c) << 32) | (Y*W + X): the lowest cost, on a tie the lowest source index.  u_t = F of that source.
+ *   4. Hole filling: pixels no source reached are holes.  In rounds r = 1, 2, ...: a hole with at least one neighbour
+ *      (left, right, up, down) filled before round r takes, per component, s = 0, s += each such neighbour's u_t in
+ *      that order, u_t = s / k with k their count; rounds repeat until no hole is left.  A pair that no source
+ *      reached has u_t = 0 everywhere.
+ *   5. Color: x0 = X - t*u_t, x1 = X + (1.0f - t)*u_t (the same in y); in0, in1 = (x0, y0), (x1, y1) in the frame;
+ *      s0 = bil(I0, clamp(x0, y0)), s1 = bil(I1, clamp(x1, y1)) with the coordinates clamped to the frame;
+ *      o0 = in0 && m0(rnd(x0), rnd(y0)) != 0, o1 = in1 && m1(rnd(x1), rnd(y1)) != 0, rnd(x) = (int)floorf(x + 0.5f);
+ *      value s0 when (in0 && !in1) || (o0 && !o1), s1 when (in1 && !in0) || (o1 && !o0), else
+ *      (1.0f - t)*s0 + t*s1; each byte (unsigned char)(fminf(fmaxf(value, 0), 255) + 0.5f).
+ * Slots outside the context, NULL i0, i1 or out, t not in (0, 1) (or NaN), frame_stride below one frame, alpha or
+ * beta not finite and >= 0, or a device flow_t that is not 4-byte aligned is OFDIS_ERR_ARG; frame-size checks and
+ * status codes are those of ofdis_get_flow_fullres.  i0, i1, out and flow_t are in memkind: host frames go through
+ * the context's staging buffer (two 2-D copies), host output through its full-resolution scratch at the size
+ * ofdis_get_flow_fullres asks for.  The workspace -- per pixel and pair 30 bytes for flow, 26 for stereo (the 64-bit
+ * keys, u_t, fill stamps, two hole lists, two masks), for max_frames pairs of the context's size -- is allocated on
+ * the first call and freed by ofdis_destroy; a context of more than 2^32 such pixels is OFDIS_ERR_UNSUPPORTED.  Not
+ * part of ofdis_run's graph; the flows are not changed.  The hole filling reads a count of the holes left on the host
+ * after rounds 8, 24, 56, ... (batches double up to 256 rounds), so the call synchronises the context's stream, once
+ * when the holes are at most 8 pixels from a splatted one. */
+int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* i0, const unsigned char* i1,
+                              size_t frame_stride, float t, float alpha, float beta, unsigned char* out, float* flow_t,
+                              int width_org, int height_org, int memkind);
 
 /* Init flow from a flow of the original frame size (extension; the reference's disabled file input,
  * run_dense.cpp:292-301,355-378).  `flow` = [f1-f0][height_org][width_org][nop] floats.  Prepares the initflow of

@@ -34,7 +34,7 @@ EXPORTS = [
     "ofdis_debug_div", "ofdis_debug_sor_div_fallbacks", "ofdis_upload_sequence_u8", "ofdis_set_initflow_fullres",
     "ofdis_set_initflow_from_result", "ofdis_upload_sequence_bidir_u8", "ofdis_set_swapped_slots",
     "ofdis_consistency_fullres", "ofdis_flow_error_fullres", "ofdis_debug_sor_plan",
-    "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres",
+    "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres", "ofdis_interpolate_fullres",
 ]
 
 # encodings of get_flow_fullres_encoded (OFDIS_ENC_F16, OFDIS_ENC_KITTI)
@@ -104,6 +104,8 @@ def lib():
             [ctypes.c_int] * 3
         L.ofdis_flow_color_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 2 + \
             [ctypes.c_float] + [ctypes.c_int] * 3
+        L.ofdis_interpolate_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 2 + \
+            [ctypes.c_size_t] + [ctypes.c_float] * 3 + [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -384,6 +386,58 @@ class Context:
         if memkind == MEM_HOST:
             self.sync()
         return out, scale
+
+    def interpolate_fullres(self, f0, f1, b0, frames0, frames1, t, width_org, height_org, alpha=None, beta=None,
+                            out=None, with_flow=False, memkind=MEM_HOST, flow_t=None, frame_stride=None):
+        """The frame at time t (0 < t < 1) between frames0[k] and frames1[k], from the last run's forward flow in slot
+        f0 + k and its backward partner in slot b0 + k (ofdis_interpolate_fullres; preprocess.interpolate_frames
+        restates it).  alpha/beta None: CONSISTENCY_DEFAULTS of the context's nop.  Returns (out, flow_t).  Host:
+        frames0, frames1 uint8 arrays (f1-f0, height_org, width_org[, noc]) whose frames are C-contiguous and whose
+        strides[0] agree -- frames[:-1] / frames[1:] of a clip and pairs[:, 0] / pairs[:, 1] both qualify; out a
+        (f1-f0, height_org, width_org[, noc]) uint8 array (no channel axis for gray) and flow_t a (f1-f0, height_org,
+        width_org, nop) float32 array (None unless with_flow), each new or given as a numpy array of exactly that
+        dtype and shape; the call then synchronises the stream.  With memkind=MEM_DEVICE, frames0, frames1, out and
+        flow_t are device addresses the caller owns (flow_t may be None) and frame_stride the bytes between frames
+        (default: one frame); out and flow_t are returned as given and are ready when the context's stream is.  The
+        hole filling synchronises the stream on the way."""
+        da, db = CONSISTENCY_DEFAULTS[self.prm.nop]
+        alpha = da if alpha is None else alpha
+        beta = db if beta is None else beta
+        noc, nop = self.prm.noc, self.prm.nop
+        n = max(f1 - f0, 0)
+        hwc = height_org * width_org * noc
+        frame = (height_org, width_org) + ((noc,) if noc > 1 else ())
+        if memkind == MEM_HOST:
+            strides = []
+            for name, arr in (("frames0", frames0), ("frames1", frames1)):
+                ok = isinstance(arr, np.ndarray) and arr.dtype == np.uint8 and arr.ndim >= 3 and arr.shape[0] == n \
+                    and arr.shape[1:] in (frame, (height_org, width_org, noc)) \
+                    and (n == 0 or arr[0].flags["C_CONTIGUOUS"]) and (n < 2 or arr.strides[0] >= hwc)
+                if not ok:
+                    raise ValueError("interpolate_fullres: %s must be a uint8 array of shape %s whose frames are "
+                                     "C-contiguous" % (name, (n,) + frame))
+                strides.append(arr.strides[0] if n > 1 else hwc)
+            if strides[0] != strides[1]:
+                raise ValueError("interpolate_fullres: frames0 and frames1 must have the same strides[0]")
+            frame_stride = strides[0]
+            out = np.empty((n,) + frame, np.uint8) if out is None else out
+            flow_t = (np.empty((n, height_org, width_org, nop), np.float32) if flow_t is None else flow_t) \
+                if with_flow else None
+            for name, arr, dt, shape in (("out", out, np.uint8, (n,) + frame),
+                                         ("flow_t", flow_t, np.float32, (n, height_org, width_org, nop))):
+                if arr is not None and not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape == shape
+                                            and arr.flags["C_CONTIGUOUS"] and arr.flags["WRITEABLE"]):
+                    raise ValueError("interpolate_fullres: %s must be a writeable C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shape))
+            p0, p1 = frames0.ctypes.data, frames1.ctypes.data
+        else:
+            frame_stride = hwc if frame_stride is None else frame_stride
+            p0, p1 = frames0, frames1
+        self._ck(lib().ofdis_interpolate_fullres(self._h, f0, f1, b0, _ptr(p0), _ptr(p1), frame_stride, t, alpha,
+                                                 beta, _ptr(out), _ptr(flow_t), width_org, height_org, memkind))
+        if memkind == MEM_HOST:
+            self.sync()
+        return out, flow_t
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

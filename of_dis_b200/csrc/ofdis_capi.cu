@@ -70,7 +70,11 @@ struct ofdis_ctx {
   // lazily allocated workspace of ofdis_flow_color_fullres: the automatic scales' maxima [max_frames] as float bit
   // patterns; never touched by ofdis_run
   unsigned int* d_color = nullptr;
-  std::vector<float*> d_flow;      // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
+  // lazily allocated workspace of ofdis_interpolate_fullres (InterpWork for max_frames pairs of width x height
+  // pixels); never touched by ofdis_run
+  void* d_interp = nullptr;
+  InterpWork interp{};
+  std::vector<float*> d_flow;     // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
   float* d_planes = nullptr;
@@ -431,6 +435,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_full);
   cudaFree(ctx->d_eval);
   cudaFree(ctx->d_color);
+  cudaFree(ctx->d_interp);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -936,6 +941,112 @@ int ofdis_consistency_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, unsigned c
     CK(cudaMemcpyAsync(mask, dmask, pix * n, cudaMemcpyDeviceToHost, ctx->stream));
     if (err) CK(cudaMemcpyAsync(err, derr, sizeof(float) * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
   }
+  return OFDIS_OK;
+}
+
+// The workspace of ofdis_interpolate_fullres for max_frames pairs of the context's size (InterpWork), allocated on
+// the first call: per pixel and pair the keys (8 bytes), u_t (4 nop), the fill stamps (4), two hole lists (4 + 4) and
+// the two consistency masks (1 + 1); then one word per pair and width + height round counts.
+static int ensure_interp(ofdis_ctx* ctx) {
+  if (ctx->d_interp) return OFDIS_OK;
+  const size_t P = (size_t)ctx->max_frames * ctx->width * ctx->height;
+  if (P > UINT_MAX) return fail(ctx, OFDIS_ERR_UNSUPPORTED, "interpolate_fullres: more than 2^32 pixels per call");
+  const size_t bytes = P * (22 + 4 * (size_t)ctx->nop) + sizeof(int) * ctx->max_frames +
+                       sizeof(unsigned int) * (ctx->width + ctx->height);
+  void* p = nullptr;
+  if (cudaMalloc(&p, bytes) != cudaSuccess) return fail(ctx, OFDIS_ERR_NOMEM, "interpolate_fullres workspace");
+  char* b = static_cast<char*>(p);
+  InterpWork& ws = ctx->interp;
+  ws.keys = reinterpret_cast<unsigned long long*>(b);
+  b += 8 * P;
+  ws.ut = reinterpret_cast<float*>(b);
+  b += 4 * ctx->nop * P;
+  ws.stamp = reinterpret_cast<int*>(b);
+  b += 4 * P;
+  ws.list[0] = reinterpret_cast<unsigned int*>(b);
+  b += 4 * P;
+  ws.list[1] = reinterpret_cast<unsigned int*>(b);
+  b += 4 * P;
+  ws.any = reinterpret_cast<int*>(b);
+  b += sizeof(int) * ctx->max_frames;
+  ws.count = reinterpret_cast<unsigned int*>(b);
+  b += sizeof(unsigned int) * (ctx->width + ctx->height);
+  ws.m0 = reinterpret_cast<unsigned char*>(b);
+  ws.m1 = ws.m0 + P;
+  ctx->d_interp = p;
+  return OFDIS_OK;
+}
+
+int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* i0, const unsigned char* i1,
+                              size_t frame_stride, float t, float alpha, float beta, unsigned char* out, float* flow_t,
+                              int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || b0 < 0 || b0 > ctx->max_frames - (f1 - f0) || !i0 || !i1 ||
+      !out || !(t > 0.f && t < 1.f) || !(alpha >= 0.f && alpha <= FLT_MAX) || !(beta >= 0.f && beta <= FLT_MAX) ||
+      (memkind == OFDIS_MEM_DEVICE && reinterpret_cast<uintptr_t>(flow_t) % sizeof(float)))
+    return fail(ctx, OFDIS_ERR_ARG, "interpolate_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  const size_t pix = (size_t)width_org * height_org, hwc = pix * ctx->prm.noc;
+  if (frame_stride < hwc) return fail(ctx, OFDIS_ERR_ARG, "interpolate_fullres: frame_stride below one frame");
+  NvtxRange nvtx("interpolate", -1);
+  CK(cudaSetDevice(ctx->device));
+  rc = ensure_interp(ctx);
+  if (rc) return rc;
+  const int n = f1 - f0, D = ctx->dirs, nop = ctx->nop;
+  const InterpWork& ws = ctx->interp;
+  InterpSrc s{i0, i1, frame_stride, width_org, height_org, cx, cy, t};
+  unsigned char* dout = out;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    // both frames of every pair into the staging buffer (2 x max_frames images), output through the full-resolution
+    // scratch at the size ofdis_get_flow_fullres asks for (an 8-bit frame is never larger than the float flow)
+    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    rc = ensure_full(ctx, pix * nop * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    unsigned char* st = static_cast<unsigned char*>(ctx->d_stage);
+    CK(cudaMemcpy2DAsync(st, hwc, i0, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(st + hwc * n, hwc, i1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    s = InterpSrc{st, st + hwc * n, hwc, width_org, height_org, cx, cy, t};
+    dout = reinterpret_cast<unsigned char*>(ctx->d_full);
+  }
+  const LevelGeom g = stepped(ctx->lev[0], D);
+  CK(cudaMemsetAsync(ws.keys, 0xff, sizeof(unsigned long long) * pix * n, ctx->stream));
+  CK(cudaMemsetAsync(ws.any, 0, sizeof(int) * n, ctx->stream));
+  CK(cudaMemsetAsync(ws.count, 0, sizeof(unsigned int) * (ctx->width + ctx->height), ctx->stream));
+  if (launch_consistency(g, f0 * D, b0 * D, n, ws.m0, nullptr, width_org, height_org, cx, cy, alpha, beta,
+                         ctx->stream) < 0 ||
+      launch_consistency(g, b0 * D, f0 * D, n, ws.m1, nullptr, width_org, height_org, cx, cy, alpha, beta,
+                         ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "consistency_kernel launch", cudaGetLastError());
+  if (launch_interp_splat(g, f0 * D, n, s, ws, ctx->stream) < 0 || launch_interp_resolve(g, f0 * D, n, s, ws, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "interp_splat_kernel launch", cudaGetLastError());
+  ctx->launches += 4;
+  // Hole filling: round r fills the holes 4-neighbour distance r from the nearest splatted pixel, so every hole is
+  // filled after width + height - 2 rounds.  The rounds go out in batches of 8, 16, ... 256 launches; the count of
+  // holes left is read after each batch, so that holes a few pixels wide cost one read, and a frame filled from one
+  // pixel one read per 256 rounds once the batches have grown.  Rounds after the last hole do nothing.
+  const int max_rounds = width_org + height_org - 2;
+  unsigned int bound = (unsigned int)(pix * n), left = 0;
+  for (int r = 0, batch = 8; r < max_rounds; batch = std::min(2 * batch, 256)) {
+    const int rounds = std::min(batch, max_rounds - r);
+    if (launch_interp_fill(nop, ws, width_org, height_org, r + 1, rounds, bound, ctx->stream) < 0)
+      return fail(ctx, OFDIS_ERR_CUDA, "interp_fill_kernel launch", cudaGetLastError());
+    ctx->launches += rounds;
+    r += rounds;
+    CK(cudaMemcpyAsync(&left, ws.count + r, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (!left) break;
+    bound = left;
+  }
+  if (left) return fail(ctx, OFDIS_ERR_CUDA, "interpolate_fullres: holes left after the last fill round");
+  if (launch_interp_blend(nop, ctx->prm.noc, n, s, ws, dout, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "interp_blend_kernel launch", cudaGetLastError());
+  ctx->launches += 1;
+  if (memkind != OFDIS_MEM_DEVICE) CK(cudaMemcpyAsync(out, dout, hwc * n, cudaMemcpyDeviceToHost, ctx->stream));
+  if (flow_t)
+    CK(cudaMemcpyAsync(flow_t, ws.ut, sizeof(float) * pix * nop * n, kind_out(memkind), ctx->stream));
   return OFDIS_OK;
 }
 

@@ -584,6 +584,13 @@ int main(int argc, char** argv) {
 // maximum, as Middlebury's tool does; --color-max M (a positive finite number; it needs --color) colors every pair
 // with the scale M, so that the frames of a clip compare.  3 bytes per pixel come back for it.  The other output files
 // keep their bytes.
+//
+// --interpolate T (0 < T < 1): every pair also gets <stem>_interp.png, the frame at time T between image1 and image2
+// synthesised on the device from the pair's forward and backward flows (ofdis_interpolate_fullres, with the
+// consistency thresholds of --bidirectional): 8-bit gray from the *_INT binaries, 8-bit RGB from the *_RGB binaries
+// (computed on the decoder's BGR order, written as RGB).  The backward slots run in the same launch, as with
+// --bidirectional, but the _bw and _occ files are only written when --bidirectional is given too; every other output
+// keeps its bytes.  Not with --warm-start.
 
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
@@ -795,7 +802,7 @@ int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr,
             "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
-            "       [--color [--color-max M]]\n"
+            "       [--color [--color-max M]] [--interpolate T]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -809,7 +816,9 @@ int main(int argc, char** argv) {
             "  whatever its extension\n"
             "  --color: also write <stem>_color.png (and <stem>_bw_color.png), the 8-bit RGB color coding of every\n"
             "  output (flow: Middlebury's color wheel, stereo: KITTI's disparity colors), colored on the device\n"
-            "  --color-max M: color every pair with the scale M (a positive finite number) instead of its own maximum\n",
+            "  --color-max M: color every pair with the scale M (a positive finite number) instead of its own maximum\n"
+            "  --interpolate T: also write <stem>_interp.png, the frame at time T (0 < T < 1) between image1 and image2,\n"
+            "  synthesised on the device from the forward and backward flows; not with --warm-start\n",
             argv[0]);
     return 2;
   }
@@ -817,6 +826,8 @@ int main(int argc, char** argv) {
   bool warm = false, batch_set = false, bidir = false, kitti = false, color = false;
   float color_max = 0.0f;  // --color-max; 0: every pair's own maximum
   const char* color_max_arg = nullptr;
+  const char* interp_arg = nullptr;  // --interpolate T
+  float interp_t = 0.0f;
   const char* gtlist = nullptr;
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
@@ -842,6 +853,13 @@ int main(int argc, char** argv) {
       }
       color_max_arg = argv[first_num + 1];
       first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--interpolate")) {
+      if (argc < first_num + 2 || interp_arg) {
+        fprintf(stderr, "error: --interpolate takes one time between 0 and 1\n");
+        return 2;
+      }
+      interp_arg = argv[first_num + 1];
+      first_num += 2;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
         fprintf(stderr, "error: --gt takes one ground-truth list file\n");
@@ -861,6 +879,20 @@ int main(int argc, char** argv) {
     fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --bidirectional\n");
     return 2;
   }
+  if (warm && interp_arg) {
+    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --interpolate\n");
+    return 2;
+  }
+  if (interp_arg) {
+    char* end = nullptr;
+    interp_t = strtof(interp_arg, &end);
+    if (end == interp_arg || *end || !(interp_t > 0.0f && interp_t < 1.0f)) {
+      fprintf(stderr, "error: --interpolate takes a time T with 0 < T < 1, got %s\n", interp_arg);
+      return 2;
+    }
+  }
+  // --interpolate needs the backward flows: the backward slots run whenever either option is given
+  const bool two_way = bidir || interp_arg;
   if (color_max_arg) {
     char* end = nullptr;
     color_max = strtof(color_max_arg, &end);
@@ -937,6 +969,7 @@ int main(int argc, char** argv) {
   vector<uint16_t> kflows;  // --kitti: the encoded slots
   vector<uint8_t> masks;
   vector<uint8_t> colors;  // --color: the color images of the slots
+  vector<uint8_t> interp, interp_png;  // --interpolate: the frames at time T, one written as RGB
   Image8 last;  // image2 of the previous batch's last pair
   size_t j0 = 0;
   while (j0 < jobs.size()) {
@@ -984,7 +1017,7 @@ int main(int argc, char** argv) {
         frames.insert(frames.end(), imgs[ia[k]].px.begin(), imgs[ia[k]].px.end());
         frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
       }
-      for (int k = 0; k < n && bidir; ++k) {  // the swapped copies
+      for (int k = 0; k < n && two_way; ++k) {  // the swapped copies
         frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
         frames.insert(frames.end(), imgs[ia[k]].px.begin(), imgs[ia[k]].px.end());
       }
@@ -1006,7 +1039,7 @@ int main(int argc, char** argv) {
       p.tv_innerit = P.tv_innerit; p.tv_solverit = P.tv_solverit; p.tv_sor = P.tv_sor; p.verbosity = P.verbosity;
       const int scf = 1 << (warm ? P.lv_f + 1 : P.lv_f);
       const int rc = ofdis_create(&ctx, 0, nullptr, &p, nop, (w + scf - 1) / scf * scf, (h + scf - 1) / scf * scf,
-                                  P.patchsz, bidir ? 2 * maxb : maxb);
+                                  P.patchsz, two_way ? 2 * maxb : maxb);
       if (rc != OFDIS_OK) {
         fprintf(stderr, "error: ofdis_create failed with status %d for %dx%d frames\n", rc, w, h);
         return 1;
@@ -1015,14 +1048,14 @@ int main(int argc, char** argv) {
       ctx_w = w;
       ctx_h = h;
     }
-    const int slots = bidir ? 2 * n : n;  // bidirectional: forward slots [0, n), backward slots [n, 2n)
+    const int slots = two_way ? 2 * n : n;  // two-way: forward slots [0, n), backward slots [n, 2n)
     const int kch = nop == 2 ? 3 : 1;     // --kitti: uint16 values per pixel
     if (kitti) kflows.resize((size_t)slots * w * h * kch);
     else flows.resize((size_t)slots * w * h * nop);
     int rc;
-    if (bidir && seq) {
+    if (two_way && seq) {
       rc = ofdis_upload_sequence_bidir_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
-    } else if (bidir) {
+    } else if (two_way) {
       rc = ofdis_upload_frames_u8(ctx, 0, 2 * n, frames.data(), w, h, OFDIS_MEM_HOST);
       if (rc == OFDIS_OK) rc = ofdis_set_swapped_slots(ctx, 0, n, 0);
       if (rc == OFDIS_OK) rc = ofdis_set_swapped_slots(ctx, n, 2 * n, 1);
@@ -1046,6 +1079,14 @@ int main(int argc, char** argv) {
       masks.resize((size_t)n * w * h);
       rc = ofdis_consistency_fullres(ctx, 0, n, n, masks.data(), nullptr, nop == 2 ? 0.01f : 0.0f,
                                      nop == 2 ? 0.5f : 1.0f, w, h, OFDIS_MEM_HOST);
+    }
+    const size_t hwc = (size_t)w * h * nochannels;
+    if (rc == OFDIS_OK && interp_arg) {
+      // image1 / image2 of pair k: frames k and k + 1 of a clip, or the k-th pair of the pairs layout
+      interp.resize((size_t)n * hwc);
+      rc = ofdis_interpolate_fullres(ctx, 0, n, n, frames.data(), frames.data() + hwc, seq ? hwc : 2 * hwc, interp_t,
+                                     nop == 2 ? 0.01f : 0.0f, nop == 2 ? 0.5f : 1.0f, interp.data(), nullptr, w, h,
+                                     OFDIS_MEM_HOST);
     }
     if (rc == OFDIS_OK) rc = ofdis_sync(ctx);
     if (rc == OFDIS_OK && gtlist) {
@@ -1086,6 +1127,19 @@ int main(int argc, char** argv) {
       if (bidir)
         save_png(colors.data() + (size_t)(n + k) * w * h * 3, w, h, 3, 8,
                  with_suffix(jobs[j0 + k].out, "_bw_color", ".png").c_str());
+    }
+    for (int k = 0; k < n && interp_arg; ++k) {
+      const uint8_t* im = interp.data() + (size_t)k * hwc;
+      if (nochannels == 3) {  // the decoder's BGR -> RGB
+        interp_png.resize(hwc);
+        for (size_t p = 0; p < hwc; p += 3) {
+          interp_png[p] = im[p + 2];
+          interp_png[p + 1] = im[p + 1];
+          interp_png[p + 2] = im[p];
+        }
+        im = interp_png.data();
+      }
+      save_png(im, w, h, nochannels, 8, with_suffix(jobs[j0 + k].out, "_interp", ".png").c_str());
     }
     ImageF out;
     out.w = w; out.h = h; out.c = nop;

@@ -616,3 +616,145 @@ def disp_to_color(flow: np.ndarray, max_value: float = 0.0, swapped=False):
             x = np.fmin(np.fmax((w * m0 + (f32(1) - w) * m1) * f32(255), f32(0)), f32(255))
             rgb[..., c] = np.where(valid, x.astype(np.uint8), np.uint8(0))
     return (rgb[0], scale[0]) if one else (rgb, scale)
+
+
+def _bilinear_frame(img: np.ndarray, xs: np.ndarray, ys: np.ndarray) -> np.ndarray:
+    """bil(I, xs, ys) of ofdis_interpolate_fullres: img (h, w, C) float32 of the bytes, (xs, ys) float32 positions in
+    the frame; corners floor and min(floor + 1, size - 1), horizontal pass first.  Returns (..., C) float32."""
+    f32 = np.float32
+    h, w = img.shape[:2]
+    x0 = np.floor(xs).astype(np.int64)
+    y0 = np.floor(ys).astype(np.int64)
+    x1 = np.minimum(x0 + 1, w - 1)
+    y1 = np.minimum(y0 + 1, h - 1)
+    fx = (xs - x0.astype(f32)).astype(f32)[..., None]
+    fy = (ys - y0.astype(f32)).astype(f32)[..., None]
+    gx, gy = f32(1) - fx, f32(1) - fy
+    r0 = img[y0, x0] * gx + img[y0, x1] * fx
+    r1 = img[y1, x0] * gx + img[y1, x1] * fx
+    return r0 * gy + r1 * fy
+
+
+def _fill_holes(ut: np.ndarray, filled: np.ndarray):
+    """Step 4 of ofdis_interpolate_fullres in place: Jacobi rounds in which a hole with a neighbour (left, right, up,
+    down) filled before the round takes s / k, s = 0 plus those neighbours in that order.  Returns the rounds run."""
+    f32 = np.float32
+    h, w, nop = ut.shape
+    rounds = 0
+    while not filled.all():
+        rounds += 1
+        s = np.zeros_like(ut)
+        k = np.zeros((h, w), np.int32)
+        for dy, dx in ((0, -1), (0, 1), (-1, 0), (1, 0)):  # left, right, up, down
+            nf = np.zeros((h, w), bool)
+            nv = np.zeros_like(ut)
+            ys, yd = (slice(0, h - 1), slice(1, h)) if dy < 0 else (slice(1, h), slice(0, h - 1)) if dy > 0 else \
+                (slice(0, h), slice(0, h))
+            xs, xd = (slice(0, w - 1), slice(1, w)) if dx < 0 else (slice(1, w), slice(0, w - 1)) if dx > 0 else \
+                (slice(0, w), slice(0, w))
+            nf[yd, xd] = filled[ys, xs]
+            nv[yd, xd] = ut[ys, xs]
+            s = s + np.where(nf[..., None], nv, f32(0))
+            k += nf
+        new = ~filled & (k > 0)
+        ut[new] = s[new] / k[new].astype(f32)[:, None]
+        filled |= new
+    return rounds
+
+
+def _interpolate_pair(i0: np.ndarray, i1: np.ndarray, F: np.ndarray, B: np.ndarray, t: float, alpha: float,
+                      beta: float):
+    f32 = np.float32
+    h, w, nop = F.shape
+    I0 = i0.reshape(h, w, -1).astype(f32)
+    I1 = i1.reshape(h, w, -1).astype(f32)
+    tt = f32(t)
+    m0, _ = consistency_check(F, B, alpha, beta)
+    m1, _ = consistency_check(B, F, alpha, beta)
+    X = np.arange(w, dtype=f32)[None, :]
+    Y = np.arange(h, dtype=f32)[:, None]
+    u = F[..., 0]
+    v = F[..., 1] if nop == 2 else np.zeros_like(u)
+    with np.errstate(invalid="ignore", over="ignore"):
+        # 2. match cost
+        xs, ys = X + u, Y + v
+        inside = (xs >= 0) & (xs <= f32(w - 1)) & (ys >= 0) & (ys <= f32(h - 1))
+        b = _bilinear_frame(I1, np.where(inside, xs, f32(0)), np.where(inside, ys, f32(0)))
+        c = np.zeros((h, w), f32)
+        for ch in range(I0.shape[2]):
+            c = c + np.abs(I0[..., ch] - b[..., ch])
+        c = np.where(inside, c, f32(np.inf)).astype(f32)
+        # 3. forward splat: the smallest key (cost bits, source index) per target
+        known = (np.abs(u) <= f32(INTERP_UNKNOWN_THRESH)) & (np.abs(v) <= f32(INTERP_UNKNOWN_THRESH))
+        px, py = X + tt * u, Y + tt * v
+        ok = known & (px > f32(-1)) & (px < f32(w)) & (py > f32(-1)) & (py < f32(h))
+    src = np.flatnonzero(ok)
+    pxs, pys = px.reshape(-1)[src], py.reshape(-1)[src]
+    flx, fly = np.floor(pxs), np.floor(pys)
+    tx, ty = flx.astype(np.int64), fly.astype(np.int64)
+    key = (c.reshape(-1)[src].view(np.uint32).astype(np.uint64) << np.uint64(32)) | src.astype(np.uint64)
+    keys = np.full(h * w, _NO_SOURCE, np.uint64)
+    for dy in (0, 1):
+        for dx in (0, 1):
+            xx, yy = tx + dx, ty + dy
+            sel = ((dx == 0) | (pxs > flx)) & ((dy == 0) | (pys > fly)) & (xx >= 0) & (xx < w) & (yy >= 0) & (yy < h)
+            np.minimum.at(keys, yy[sel] * w + xx[sel], key[sel])
+    filled = keys != _NO_SOURCE
+    ut = np.zeros((h * w, nop), f32)
+    ut[filled] = F.reshape(-1, nop)[(keys[filled] & np.uint64(0xFFFFFFFF)).astype(np.int64)]
+    ut = ut.reshape(h, w, nop)
+    # 4. hole filling (a pair that no source reached keeps u_t = 0)
+    rounds = _fill_holes(ut, filled.reshape(h, w)) if filled.any() else 0
+    # 5. color
+    uu = ut[..., 0]
+    vv = ut[..., 1] if nop == 2 else np.zeros_like(uu)
+    x0, y0 = X - tt * uu, Y - tt * vv
+    x1, y1 = X + (f32(1) - tt) * uu, Y + (f32(1) - tt) * vv
+    in0 = (x0 >= 0) & (x0 <= f32(w - 1)) & (y0 >= 0) & (y0 <= f32(h - 1))
+    in1 = (x1 >= 0) & (x1 <= f32(w - 1)) & (y1 >= 0) & (y1 <= f32(h - 1))
+    clampx = lambda a: np.fmin(np.fmax(a, f32(0)), f32(w - 1))  # noqa: E731
+    clampy = lambda a: np.fmin(np.fmax(a, f32(0)), f32(h - 1))  # noqa: E731
+    s0 = _bilinear_frame(I0, clampx(x0), clampy(y0))
+    s1 = _bilinear_frame(I1, clampx(x1), clampy(y1))
+    rnd = lambda a, ins: np.floor(np.where(ins, a, f32(0)) + f32(0.5)).astype(np.int64)  # noqa: E731
+    o0 = in0 & (m0[rnd(y0, in0), rnd(x0, in0)] != 0)
+    o1 = in1 & (m1[rnd(y1, in1), rnd(x1, in1)] != 0)
+    only0 = ((in0 & ~in1) | (o0 & ~o1))[..., None]
+    only1 = ((in1 & ~in0) | (o1 & ~o0))[..., None]
+    val = np.where(only0, s0, np.where(only1, s1, (f32(1) - tt) * s0 + tt * s1))
+    out = (np.fmin(np.fmax(val, f32(0)), f32(255)) + f32(0.5)).astype(np.uint8)
+    return out, ut, rounds
+
+
+INTERP_UNKNOWN_THRESH = 1e9  # a source splats only when |u|, |v| <= this (NaN fails), the rule of flow_error
+_NO_SOURCE = np.uint64(0xFFFFFFFFFFFFFFFF)
+
+
+def interpolate_frames(frames0: np.ndarray, frames1: np.ndarray, fw: np.ndarray, bw: np.ndarray, t: float,
+                       alpha: float, beta: float, with_rounds: bool = False):
+    """ofdis_interpolate_fullres bit for bit: the frame at time t between frames0 and frames1 from the forward flow
+    fw (frames0 -> frames1) and its backward partner bw, float32 without contraction.  One pair: frames (h, w[, noc])
+    uint8 and flows (h, w, nop); a batch: a leading axis on all four.  The masks are consistency_check's, the splat is
+    np.minimum.at on the 64-bit keys, the hole filling restates the Jacobi rounds.  Returns (out, flow_t): out uint8
+    of the frames' shape, flow_t float32 of the flows' shape (u_t); with_rounds also the most hole-filling rounds any
+    pair needed."""
+    F = np.asarray(fw, np.float32)
+    B = np.asarray(bw, np.float32)
+    a0 = np.asarray(frames0, np.uint8)
+    a1 = np.asarray(frames1, np.uint8)
+    one = F.ndim == 3
+    if one:
+        F, B, a0, a1 = F[None], B[None], a0[None], a1[None]
+    assert F.ndim == 4 and B.shape == F.shape and a0.shape == a1.shape and a0.shape[:3] == F.shape[:3], \
+        (F.shape, B.shape, a0.shape, a1.shape)
+    out = np.empty(a0.shape, np.uint8)
+    flow_t = np.empty(F.shape, np.float32)
+    rounds = 0
+    for k in range(F.shape[0]):
+        o, ut, r = _interpolate_pair(a0[k], a1[k], F[k], B[k], t, alpha, beta)
+        out[k] = o.reshape(a0.shape[1:])
+        flow_t[k] = ut
+        rounds = max(rounds, r)
+    if one:
+        out, flow_t = out[0], flow_t[0]
+    return (out, flow_t, rounds) if with_rounds else (out, flow_t)

@@ -4,7 +4,8 @@ the smoke configuration (P=8 gray flow) with both exact SOR kernels (sor_lane_ke
 sor_wave_kernel: single CTA), a forward-backward case, a P=12 RGB and a P=12 stereo case (window-staged patch
 kernel, stereo SOR), a 70-row level as three bands of the lane kernel and forced into a cluster of bands of the
 wave kernel with 1 and 2 rows per thread (st.async halo exchange), and the 8-bit frame path (pyramid and
-upsampling kernels).  Results are checked against the oracle so that a clean log means a correct run."""
+upsampling kernels), and a frame interpolation checked against its restatement.  Results are checked against the
+oracle so that a clean log means a correct run."""
 import os
 import sys
 
@@ -50,4 +51,20 @@ for name, (h, w), ch, nop, numbers, opts in CASES:
     print("%-22s %s" % (name, "bitwise equal to the oracle" if ok else "MISMATCH"), flush=True)
     if not ok:
         sys.exit(1)
+# frame interpolation (consistency masks, splat, resolve, fill rounds, blend) on a two-way clip, RGB flow
+h, w, n = 61, 90, 2
+prm = params.from_cli_numbers("3 1 8 8 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=3, nop=2)
+clip = synth.synthetic_sequence(n + 1, h, w, 3, seed=5, amp=3.0)
+ctx = api.Context(prm, 96, 64, prm.p_samp_s, 2 * n)
+ctx.upload_sequence_bidir_u8(0, n, clip, w, h)
+ctx.run(2 * n)
+full = np.empty((2 * n, h, w, 2), np.float32)
+ctx.get_flow_fullres(0, 2 * n, full, w, h)
+out, ut = ctx.interpolate_fullres(0, n, n, clip[:-1], clip[1:], 0.5, w, h, with_flow=True)
+ctx.close()
+exp, exp_ut = preprocess.interpolate_frames(clip[:-1], clip[1:], full[:n], full[n:], 0.5, 0.01, 0.5)
+ok = np.array_equal(out, exp) and np.array_equal(ut.view(np.uint32), exp_ut.view(np.uint32))
+print("%-22s %s" % ("interpolate_rgb", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
 print("all cases ok")
