@@ -291,6 +291,11 @@ int ofdis_create(ofdis_ctx** out, int device, void* stream, const ofdis_params* 
   // launches that put the frames in gridDim.y / .z (at most 65535): the derivative kernels max_frames x dirs x noc,
   // the pyramid kernels 2 x max_frames (both images of a pair), every other one max_frames x dirs or fewer
   if ((long)max_frames * std::max(2, (prm->usefbcon ? 2 : 1) * prm->noc) > OFDIS_MAX_GRID_FRAMES) return OFDIS_ERR_UNSUPPORTED;
+  // patches too large for the generic patch kernel's smallest CTA: the library builds for sm_90a only, so its
+  // opt-in ceiling is a constant and the refusal needs no device (RGB P >= 32, gray P >= 54)
+  size_t patch_smem;
+  patch_generic_threads(prm->noc * prm->p_samp_s * prm->p_samp_s, &patch_smem);
+  if (patch_smem > SMEM_OPTIN_MAX) return OFDIS_ERR_UNSUPPORTED;
 
   ofdis_ctx* ctx = new (std::nothrow) ofdis_ctx();
   if (!ctx) return OFDIS_ERR_NOMEM;

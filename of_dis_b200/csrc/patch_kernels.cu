@@ -1111,11 +1111,8 @@ int launch_patch_optimize(const LevelGeom& g, const PatchParams& pp, int f0, int
 #undef OFDIS_P12
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
   }
-  const int n = g.novals;
-  const int NK = (n / 8) + (((n % 8) >= 4) ? 1 : 0);
-  int threads = 256;
-  while (threads > 32 && (size_t)5 * NK * threads * sizeof(float) > 200 * 1024) threads >>= 1;
-  const size_t smem = (size_t)5 * NK * threads * sizeof(float);
+  size_t smem;
+  const int threads = patch_generic_threads(g.novals, &smem);
   const dim3 grid((g.np + threads / 8 - 1) / (threads / 8), f1 - f0);
   if (!optin(g.nop == 2 ? (const void*)patch_optimize_kernel<2> : (const void*)patch_optimize_kernel<1>, smem)) return -1;
   if (g.nop == 2) patch_optimize_kernel<2><<<grid, threads, smem, st>>>(g, pp, f0, init_from_coarser ? 1 : 0);

@@ -46,6 +46,7 @@ def write_digests(out_dir):
     out.update(sor_division_digests())
     out.update(degenerate_digests())
     out.update(batched_digests())
+    out.update(geometry_digests())
     with open(os.path.join(out_dir, "reference_digests.json"), "w") as f:
         json.dump(out, f, indent=1, sort_keys=True)
         f.write("\n")
@@ -76,6 +77,34 @@ def batched_digests():
     for name in t.BATCHED:
         out["batched_%s_input" % name], out["batched_%s_runs" % name] = t.batched_digests(ref_driver.ref_run, name)
     out["frame_limit_input"], out["frame_limit_runs"] = t.frame_limit_digests(ref_driver.ref_run)
+    return out
+
+
+def geometry_digests():
+    """The cases of tests/test_patch_geometry_gpu.py: paddings wider than the patch on every patch kernel (input pair,
+    whole run, patch stage at sc_l, refinement of sc_l), patch sizes 2 to 52 (input pair, whole run, patch stage), the
+    clips of the upload paths and the pairs of the batch of more than 16 frames (inputs, one digest over the runs)."""
+    import test_oracle as t
+    import test_patch_geometry as g
+    from test_patch_geometry_gpu import PAD_CASES, SIZE_CASES, UPLOAD_CASES, pad_inputs, size_inputs
+
+    out = {}
+    for route, pad in PAD_CASES:
+        i0, i1, pyr, _, prm = pad_inputs(route, pad)
+        key = "geometry_pad_%s_%s" % (route, pad)
+        run, lvl, vr = g.pad_stage(ref_driver.ref_run, ref_driver.ref_level_patches, ref_driver.ref_level_varref, pyr,
+                                   prm)
+        out[key + "_input"], out[key + "_run"] = t.input_digest(i0, i1), t.digest(run)
+        out[key + "_patches"], out[key + "_varref"] = t.patches_digest([lvl]), t.digest(vr)
+    for name in SIZE_CASES:
+        i0, i1, pyr, prm = size_inputs(name)
+        key = "geometry_size_%s" % name
+        run, lvl = g.size_stage(ref_driver.ref_run, ref_driver.ref_level_patches, pyr, prm)
+        out[key + "_input"], out[key + "_run"], out[key + "_patches"] = t.input_digest(i0, i1), t.digest(run), \
+            t.patches_digest([lvl])
+    for name in UPLOAD_CASES:
+        out["geometry_upload_%s_input" % name], out["geometry_upload_%s_runs" % name] = g.upload_digests(ref_driver.ref_run, name)
+    out["geometry_batch_input"], out["geometry_batch_runs"] = g.batch_digests(ref_driver.ref_run)
     return out
 
 

@@ -40,6 +40,18 @@ def test_create_rejects_bad_arguments_without_touching_the_gpu(built_lib):
     assert built_lib.ofdis_create(ctypes.byref(h), 0, None, ctypes.byref(cp), 2, 1024, 131104, 8, 1) == -3
     cp.noc = 2
     assert built_lib.ofdis_create(ctypes.byref(h), 0, None, ctypes.byref(cp), 2, 1024, 448, 8, 1) == -1
+    # patches whose generic patch kernel needs more shared memory than a CTA can opt in to (RGB P = 32: 245,760
+    # bytes, gray P = 54: 233,600): valid in the reference, not built.  The largest sizes that fit (RGB P = 30, gray
+    # P = 52: 216,320 bytes) are accepted: created on a GPU; without one the first CUDA call fails
+    for noc, P, refused in ((3, 32, True), (1, 54, True), (3, 30, False), (1, 52, False)):
+        cp = params.from_cli_numbers(("2 0 4 4 0.05 0.95 0 %d 0.4 0 1 0 1 10 10 5 1 3 1.6 0" % P).split(), noc=noc).to_c()
+        for nop in (1, 2):
+            rc = built_lib.ofdis_create(ctypes.byref(h), 0, None, ctypes.byref(cp), nop, 64, 32, P, 1)
+            if refused:
+                assert rc == -3 and not h.value, (noc, P, nop, rc)
+            else:
+                assert rc not in (-1, -3), (noc, P, nop, rc)
+                built_lib.ofdis_destroy(h)
     assert built_lib.ofdis_destroy(None) == 0
 
 
