@@ -1396,9 +1396,9 @@ long ofdis_debug_get(ofdis_ctx* ctx, const char* name, int frame, float* dst, si
       for (int i = 0; i < L->w; ++i)
         for (int e = 0; e < per; ++e) {
           // lane layout: a record is two float4 (lane_rec_f4), (du,dv) consecutive floats (lane_dudv_f); band lane
-          // rows: chunk e of the block's lane row holds field e of its 4 pixels, (du,dv) are chunks nq, nq+1
+          // rows: records as band_rec_f places them, (du,dv) are chunks nq, nq+1
           const size_t k = sp.lane ? (is_rec ? lane_rec_f4(sp, i, j, e >> 2) * 4 + (e & 3) : lane_dudv_f(sp, i, j) + e)
-                                   : band_f4(sp, i >> 2, j, is_rec ? e : sp.nq + e) * 4 + (i & 3);
+                                   : (is_rec ? band_rec_f(sp, i, j, e) : band_f4(sp, i >> 2, j, sp.nq + e) * 4 + (i & 3));
           dst[((size_t)j * L->pitch + i) * per + e] = raw[k];
         }
     return (long)(plane * per);

@@ -148,8 +148,9 @@ __global__ void __launch_bounds__(TX * TY) assemble_kernel(LevelGeom g, VarRefPl
   const int tid = threadIdx.y * TX + threadIdx.x;
   const int w = g.w, h = g.h, pitch = g.pitch;
   const float* const flow = g.flow + (size_t)frame * g.flow_frame_stride;
-  // Records and (du,dv) of pixel (x,y).  Exact mode: the band-skewed lane rows (band_f4): chunk f of a
-  // block holds field f of its 4 pixels, du is chunk nq, dv chunk nq+1.  Fast mode (red-black SOR):
+  // Records and (du,dv) of pixel (x,y).  Exact mode: the band-skewed lane rows (band_f4): flow records are two
+  // float4 per pixel, stereo records one float4 per field of the block's 4 pixels (band_rec_f); du is chunk nq of
+  // the block, dv chunk nq+1.  Fast mode (red-black SOR):
   // natural layout, 8 floats per pixel, (du,dv) in the current ping-pong planes.
   // Lane mode (sor_lane_kernel): lane-skewed layout, the record is two float4 (lane_rec_f4), (du,dv) one float2.
   constexpr bool fast = (MODE == 1), lane = (MODE == 2);
@@ -158,7 +159,7 @@ __global__ void __launch_bounds__(TX * TY) assemble_kernel(LevelGeom g, VarRefPl
   const int fs = fast ? 1 : 4;                       // floats between consecutive record fields of a pixel
   const int dv_off = lane ? 1 : (fast ? (int)pl.plane : 4);  // from du to dv
   auto rec_idx = [&pl, pitch](int x, int y) {
-    return lane ? (int)lane_rec_f4(pl, x, y, 0) * 4 : (fast ? (y * pitch + x) * 8 : (int)band_f4(pl, x >> 2, y, 0) * 4 + (x & 3));
+    return lane ? (int)lane_rec_f4(pl, x, y, 0) * 4 : (fast ? (y * pitch + x) * 8 : (int)band_rec_f(pl, x, y, 0));
   };
   auto du_idx = [&pl, pitch](int x, int y) {
     return lane ? (int)lane_dudv_f(pl, x, y) : (fast ? y * pitch + x : (int)band_f4(pl, x >> 2, y, pl.nq) * 4 + (x & 3));
@@ -364,12 +365,12 @@ __global__ void __launch_bounds__(TX * TY) assemble_kernel(LevelGeom g, VarRefPl
     else dps = hl + hh + vt + vv;
     const float iA11 = A22 + dps, iA22 = A11 + dps;
     const float det = iA11 * iA22 - A12 * A12;
-    // record of the 4-pixel block, SoA: float4 f of the block holds field f of its 4 pixels;
-    // fields: a11^-1, a12^-1, a22^-1, b1, b2, sh, sv, sv(row above)
-    if (lane) {
+    // record fields: a11^-1, a12^-1, a22^-1, b1, b2, sh, sv, sv(row above); two float4 per pixel in the lane and
+    // the band layouts, one float per field in the fast mode's natural layout
+    if (!fast) {
       float4* const r4 = reinterpret_cast<float4*>(rec + b0);
       r4[0] = make_float4(iA11 / det, A12 / -det, iA22 / det, B1);
-      r4[32] = make_float4(B2, hh, vv, vt);
+      r4[lane ? 32 : 1] = make_float4(B2, hh, vv, vt);
     } else {
     rec[b0] = iA11 / det;
     rec[b0 + fs] = A12 / -det;
