@@ -348,6 +348,71 @@ int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsi
                               size_t frame_stride, float t, float alpha, float beta, unsigned char* out, float* flow_t,
                               int width_org, int height_org, int memkind);
 
+/* Dense point trajectories (extension): the tracker of Sundaram, Brox and Keutzer ("Dense point trajectories by
+ * GPU-accelerated large displacement optical flow", ECCV 2010) through consecutive pairs of bidirectional flows.
+ * The context owns one tracker: the list of live tracks (sorted by id), the next id and the counters.  It persists
+ * across calls and across ofdis_run; ofdis_track_begin resets it and ofdis_destroy frees it.  Everything is float32
+ * without contraction, with IEEE division and square root; preprocess.track_points restates it.  W = width_org,
+ * H = height_org, s = spacing.
+ *   Seeding a frame (ofdis_track_begin: its frame; ofdis_track_advance: every target frame).  The cells (i, j) are
+ *   ceil(W/s) x ceil(H/s), in row-major order (j outer); cell (i, j) has the seed pixel cx = min(i*s + s/2, W-1),
+ *   cy = min(j*s + s/2, H-1).  A cell is occupied when a live track has ((int)x / s, (int)y / s) == (i, j) after the
+ *   frame's advance.  Brightness g: the byte for gray, ((float)c0 + (float)c1 + (float)c2) / 3.0f for 3 channels in
+ *   memory order.  Ix = (g(min(x+1, W-1), y) - g(max(x-1, 0), y)) * 0.5f, Iy the same in y.  Over the 5 x 5 window
+ *   around the seed pixel (coordinates clamped to the frame; dy outer, dx inner, both ascending; sums from +0.0f):
+ *   a = sum Ix*Ix, b = sum Ix*Iy, c = sum Iy*Iy; d = a - c, lambda = (a + c)*0.5f - sqrtf(d*d*0.25f + b*b).  An
+ *   unoccupied cell with lambda >= min_eig is a candidate.  Candidates take the ids next_id, next_id + 1, ... in cell
+ *   order and are appended after the surviving tracks at (cx, cy), as long as there are fewer than `capacity` live
+ *   tracks and next_id stays at most 2^31-1 (ids below 2^31-1); the lowest cells are kept, the others are counted in
+ *   `dropped`.
+ *   Advancing a track at (x, y) through pair k.  F is slot f0+k's full-resolution flow and B slot b0+k's, both
+ *   exactly what ofdis_get_flow_fullres returns, computed from the level flows without a full-resolution copy;
+ *   stereo (nop 1) uses v = 0.  bil(F, x, y) is the bilinear rule of ofdis_consistency_fullres (corners floor and
+ *   floor + 1 clamped to the frame, horizontal pass first).
+ *     (u, v) = bil(F, x, y); (x', y') = (x + u, y + v); outside [0, W-1] x [0, H-1] (or NaN): ends as *leaves*.
+ *     b = bil(B, x', y'); err = du*du + dv*dv with (du, dv) = (u + b0, v + b1); mag = (u*u + v*v) + (b0*b0 + b1*b1)
+ *     (stereo dv = b1 = 0); ends as *inconsistent* unless err <= alpha*mag + beta.
+ *     (xr, yr) = ((int)floorf(x + 0.5f), (int)floorf(y + 0.5f)); ux = (F(min(xr+1, W-1), yr) - F(max(xr-1, 0), yr))
+ *     * 0.5f and uy = (F(xr, min(yr+1, H-1)) - F(xr, max(yr-1, 0))) * 0.5f of the u component, vx, vy the same of v;
+ *     g2 = (ux*ux + uy*uy) + (vx*vx + vy*vy) (stereo ux*ux + uy*uy); ends as *boundary* if
+ *     g2 > mb_alpha*(u*u + v*v) + mb_beta.
+ *     Otherwise the track moves to (x', y') and keeps its id; survivors keep their order.
+ *   Sundaram et al. use alpha 0.01, beta 0.5 (as ofdis_consistency_fullres) and mb_alpha 0.01, mb_beta 0.002. */
+typedef struct ofdis_track_params {
+  int capacity;             /* live tracks the tracker holds, 1 .. 1<<24 */
+  int spacing;              /* seed grid step s in pixels, >= 1 */
+  float alpha, beta;        /* forward-backward test, as ofdis_consistency_fullres; finite and >= 0 */
+  float mb_alpha, mb_beta;  /* motion-boundary test; finite and >= 0 */
+  float min_eig;            /* seed where the structure tensor's smaller eigenvalue >= min_eig; not NaN */
+} ofdis_track_params;
+typedef struct ofdis_track_point { int id; float x, y; } ofdis_track_point;  /* 12 bytes */
+typedef struct ofdis_track_stats {
+  long long seeded, ended_leaves, ended_inconsistent, ended_boundary, dropped;  /* since ofdis_track_begin */
+  int alive, next_id;
+} ofdis_track_stats;
+/* Resets the tracker and seeds `frame` ([height_org][width_org][noc] bytes in memkind); its list goes to points
+ * ([capacity] records in memkind) and its length to *count (host).  Allocates the workspace -- the state, two track
+ * lists and the output records of max_frames pairs (12 bytes per track), the cell flags -- which grows with capacity
+ * and the cell count, never shrinks, and is freed by ofdis_destroy.  A NULL params, frame, points or count, a
+ * parameter out of range, or a device `points` that is not 4-byte aligned is OFDIS_ERR_ARG; frame sizes are checked
+ * as in ofdis_get_flow_fullres. */
+int ofdis_track_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const unsigned char* frame,
+                      ofdis_track_point* points, int* count, int width_org, int height_org, int memkind);
+/* Pairs k = 0 .. f1-f0-1 in order: advance every live track through slot f0+k (F) and slot b0+k (B) of the last run
+ * (the layout of ofdis_upload_sequence_bidir_u8 with b0 = f0 + n, or pairs followed by their swapped copies), then
+ * seed target frame k at frames + k*frame_stride (a clip: frames + hwc with stride hwc; the pairs of
+ * ofdis_upload_frames_u8: image2 at stride 2hwc).  The list after pair k goes to points + k*capacity and its length
+ * to counts[k] (host).  frames and points are in memkind; host frames go through the staging buffer, host records
+ * through the workspace.  The pairs are enqueued without a host round trip; the call synchronises the context's
+ * stream once, at the end, for the counts.  Slots outside the context, NULL frames, points or counts, frame_stride
+ * below one frame, a device `points` that is not 4-byte aligned, or a call before ofdis_track_begin or with another
+ * frame size than its is OFDIS_ERR_ARG.  Not part of ofdis_run's graph; the flows are not changed. */
+int ofdis_track_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames, size_t frame_stride,
+                        ofdis_track_point* points, int* counts, int width_org, int height_org, int memkind);
+/* The tracker's counters since ofdis_track_begin (synchronises the context's stream); OFDIS_ERR_ARG before the
+ * first ofdis_track_begin or with a NULL out. */
+int ofdis_track_stats_get(const ofdis_ctx* ctx, ofdis_track_stats* out);
+
 /* Init flow from a flow of the original frame size (extension; the reference's disabled file input,
  * run_dense.cpp:292-301,355-378).  `flow` = [f1-f0][height_org][width_org][nop] floats.  Prepares the initflow of
  * pairs [f0, f1) that the following ofdis_run(ctx, n, use_initflow = 1) reads: replicate padding to the context,

@@ -14,6 +14,7 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
+from .preprocess import TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE, TRACK_STATS_FIELDS
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("OFDIS_LIB") or os.path.join(_HERE, "lib", "libofdis_b200.so")  # OFDIS_LIB: experiments only
@@ -35,6 +36,7 @@ EXPORTS = [
     "ofdis_set_initflow_from_result", "ofdis_upload_sequence_bidir_u8", "ofdis_set_swapped_slots",
     "ofdis_consistency_fullres", "ofdis_flow_error_fullres", "ofdis_debug_sor_plan",
     "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres", "ofdis_interpolate_fullres",
+    "ofdis_track_begin", "ofdis_track_advance", "ofdis_track_stats_get",
 ]
 
 # encodings of get_flow_fullres_encoded (OFDIS_ENC_F16, OFDIS_ENC_KITTI)
@@ -49,6 +51,18 @@ CONSISTENCY_DEFAULTS = {2: (0.01, 0.5), 1: (0.0, 1.0)}
 
 # ofdis_error_stats (include/ofdis_b200.h), field for field: counts of one (pair, class) of flow_error_fullres
 ERROR_STATS_DTYPE = np.dtype([("n", "<i8"), ("n_over", "<i8", (3,)), ("n_outlier", "<i8"), ("sum_err", "<f8")])
+
+
+class TrackParams(ctypes.Structure):
+    """ofdis_track_params (include/ofdis_b200.h)."""
+    _fields_ = [("capacity", ctypes.c_int), ("spacing", ctypes.c_int)] + \
+        [(k, ctypes.c_float) for k in TRACK_PARAM_FIELDS[2:]]
+
+
+class TrackStats(ctypes.Structure):
+    """ofdis_track_stats (include/ofdis_b200.h)."""
+    _fields_ = [(k, ctypes.c_longlong) for k in TRACK_STATS_FIELDS[:5]] + \
+        [(k, ctypes.c_int) for k in TRACK_STATS_FIELDS[5:]]
 
 
 class OfdisError(RuntimeError):
@@ -106,6 +120,11 @@ def lib():
             [ctypes.c_float] + [ctypes.c_int] * 3
         L.ofdis_interpolate_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 2 + \
             [ctypes.c_size_t] + [ctypes.c_float] * 3 + [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
+        L.ofdis_track_begin.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackParams)] + [ctypes.c_void_p] * 3 + \
+            [ctypes.c_int] * 3
+        L.ofdis_track_advance.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p, ctypes.c_size_t] + \
+            [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
+        L.ofdis_track_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackStats)]
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -438,6 +457,69 @@ class Context:
         if memkind == MEM_HOST:
             self.sync()
         return out, flow_t
+
+    def _frames_u8(self, name, frames, n, width_org, height_org):
+        """Checks a host array of n 8-bit frames of the context's channel count whose frames are C-contiguous and
+        returns its frame stride in bytes."""
+        noc = self.prm.noc
+        hwc = height_org * width_org * noc
+        frame = (height_org, width_org) + ((noc,) if noc > 1 else ())
+        ok = isinstance(frames, np.ndarray) and frames.dtype == np.uint8 and frames.ndim >= 3 and \
+            frames.shape[0] == n and frames.shape[1:] in (frame, (height_org, width_org, noc)) and \
+            (n == 0 or frames[0].flags["C_CONTIGUOUS"]) and (n < 2 or frames.strides[0] >= hwc)
+        if not ok:
+            raise ValueError("%s must be a uint8 array of shape %s whose frames are C-contiguous" % (name, (n,) + frame))
+        return frames.strides[0] if n > 1 else hwc
+
+    def track_begin(self, params, frame, width_org, height_org, memkind=MEM_HOST, points=None):
+        """Resets the context's tracker and seeds `frame` (ofdis_track_begin; preprocess.track_points restates it).
+        params: a mapping with the keys of preprocess.TRACK_PARAM_FIELDS (or a TrackParams).  Host: frame a uint8
+        (height_org, width_org[, noc]) array; returns frame 0's tracks as an array of TRACK_POINT_DTYPE.  With
+        memkind=MEM_DEVICE, frame and points are device addresses the caller owns (points: `capacity` records) and
+        the count of records written is returned."""
+        if not isinstance(params, TrackParams):
+            params = TrackParams(*[params[k] for k in TRACK_PARAM_FIELDS])
+        self._track_capacity = params.capacity
+        count = ctypes.c_int(0)
+        if memkind == MEM_HOST:
+            self._frames_u8("track_begin: frame", np.asarray(frame)[None], 1, width_org, height_org)
+            frame = np.ascontiguousarray(frame)
+            points = np.empty(max(params.capacity, 0), TRACK_POINT_DTYPE)
+        self._ck(lib().ofdis_track_begin(self._h, ctypes.byref(params), _ptr(frame), _ptr(points), ctypes.byref(count),
+                                         width_org, height_org, memkind))
+        return points[:count.value].copy() if memkind == MEM_HOST else count.value
+
+    def track_advance(self, f0, f1, b0, frames, width_org, height_org, frame_stride=None, memkind=MEM_HOST,
+                      points=None):
+        """Advances the tracker through the last run's slots f0 + k (forward) and b0 + k (backward), seeding frames[k]
+        after pair k (ofdis_track_advance).  Host: frames a uint8 (f1-f0, height_org, width_org[, noc]) array whose
+        frames are C-contiguous -- clip[1:] of a clip, or pairs[:, 1] of a pair array; returns the f1-f0 lists of
+        TRACK_POINT_DTYPE.  With memkind=MEM_DEVICE, frames and points are device addresses the caller owns (points:
+        (f1-f0) x capacity records, list k at record k*capacity), frame_stride the bytes between frames (default one
+        frame), and the int32 counts of the lists are returned."""
+        n = max(f1 - f0, 0)
+        cap = getattr(self, "_track_capacity", 0)
+        counts = np.zeros(n, np.int32)
+        if memkind == MEM_HOST:
+            frame_stride = self._frames_u8("track_advance: frames", frames, n, width_org, height_org)
+            points = np.empty(n * cap, TRACK_POINT_DTYPE)
+            pf = frames.ctypes.data
+        else:
+            frame_stride = height_org * width_org * self.prm.noc if frame_stride is None else frame_stride
+            pf = frames
+        self._ck(lib().ofdis_track_advance(self._h, f0, f1, b0, _ptr(pf), frame_stride, _ptr(points), _ptr(counts),
+                                           width_org, height_org, memkind))
+        if memkind != MEM_HOST:
+            return counts
+        return [points[k * cap:k * cap + counts[k]].copy() for k in range(n)]
+
+    def track_stats(self):
+        """The tracker's counters since track_begin (ofdis_track_stats_get): a dict of preprocess.TRACK_STATS_FIELDS."""
+        st = TrackStats()
+        rc = lib().ofdis_track_stats_get(self._h, ctypes.byref(st))
+        if rc != 0:
+            raise OfdisError("track_stats: status %d" % rc)
+        return {k: int(getattr(st, k)) for k in TRACK_STATS_FIELDS}
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

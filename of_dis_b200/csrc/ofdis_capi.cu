@@ -74,7 +74,17 @@ struct ofdis_ctx {
   // pixels); never touched by ofdis_run
   void* d_interp = nullptr;
   InterpWork interp{};
-  std::vector<float*> d_flow;     // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
+  // the tracker of ofdis_track_begin / ofdis_track_advance: its workspace (TrackWork, then the host-output records of
+  // max_frames pairs), the geometry of the last begin and the list that holds the live tracks; never touched by
+  // ofdis_run
+  void* d_track = nullptr;
+  size_t track_bytes = 0;
+  TrackWork track{};
+  ofdis_track_point* track_out = nullptr;
+  TrackGeom tgeom{};
+  int track_cur = 0;
+  bool track_on = false;
+  std::vector<float*> d_flow;    // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
   float* d_planes = nullptr;
@@ -441,6 +451,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_eval);
   cudaFree(ctx->d_color);
   cudaFree(ctx->d_interp);
+  cudaFree(ctx->d_track);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -1052,6 +1063,183 @@ int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsi
   if (memkind != OFDIS_MEM_DEVICE) CK(cudaMemcpyAsync(out, dout, hwc * n, cudaMemcpyDeviceToHost, ctx->stream));
   if (flow_t)
     CK(cudaMemcpyAsync(flow_t, ws.ut, sizeof(float) * pix * nop * n, kind_out(memkind), ctx->stream));
+  return OFDIS_OK;
+}
+
+static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// The tracker's workspace for geometry t: the state, two track lists, the flags, the occupancy, the scan blocks'
+// sums, the counts of max_frames pairs, then the host-output records of max_frames pairs.  Grows, never shrinks.
+static int ensure_track(ofdis_ctx* ctx, const TrackGeom& t) {
+  const size_t list = align16(sizeof(ofdis_track_point) * t.capacity);
+  const size_t nflags = (size_t)t.cap_pad + t.cells_pad;
+  const size_t part[7] = {align16(sizeof(TrackState)), list, list, nflags, align16(t.cells),
+                          align16(sizeof(unsigned int) * (nflags / TRACK_BLOCK)), align16(sizeof(int) * ctx->max_frames)};
+  size_t bytes = sizeof(ofdis_track_point) * t.capacity * (size_t)ctx->max_frames;
+  for (size_t p : part) bytes += p;
+  if (bytes > ctx->track_bytes) {
+    CK(cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_track);
+    ctx->d_track = nullptr;
+    ctx->track_bytes = 0;
+    if (cudaMalloc(&ctx->d_track, bytes) != cudaSuccess) {
+      ctx->d_track = nullptr;
+      return fail(ctx, OFDIS_ERR_NOMEM, "track workspace");
+    }
+    ctx->track_bytes = bytes;
+  }
+  char* b = static_cast<char*>(ctx->d_track);
+  TrackWork& ws = ctx->track;
+  ws.state = reinterpret_cast<TrackState*>(b);
+  b += part[0];
+  ws.list[0] = reinterpret_cast<ofdis_track_point*>(b);
+  b += part[1];
+  ws.list[1] = reinterpret_cast<ofdis_track_point*>(b);
+  b += part[2];
+  ws.flags = reinterpret_cast<unsigned char*>(b);
+  b += part[3];
+  ws.occ = reinterpret_cast<unsigned char*>(b);
+  b += part[4];
+  ws.bsum = reinterpret_cast<unsigned int*>(b);
+  b += part[5];
+  ws.counts = reinterpret_cast<int*>(b);
+  b += part[6];
+  ctx->track_out = reinterpret_cast<ofdis_track_point*>(b);
+  return OFDIS_OK;
+}
+
+int ofdis_track_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const unsigned char* frame,
+                      ofdis_track_point* points, int* count, int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  auto finite_nonneg = [](float v) { return v >= 0.f && v <= FLT_MAX; };
+  if (!params || params->capacity < 1 || params->capacity > (1 << 24) || params->spacing < 1 ||
+      !finite_nonneg(params->alpha) || !finite_nonneg(params->beta) || !finite_nonneg(params->mb_alpha) ||
+      !finite_nonneg(params->mb_beta) || std::isnan(params->min_eig) || !frame || !points || !count ||
+      (memkind == OFDIS_MEM_DEVICE && reinterpret_cast<uintptr_t>(points) % 4))
+    return fail(ctx, OFDIS_ERR_ARG, "track_begin: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("track", -1);
+  CK(cudaSetDevice(ctx->device));
+  ctx->track_on = false;
+  TrackGeom t{};
+  t.w = width_org;
+  t.h = height_org;
+  t.s = params->spacing;
+  t.ncx = (width_org - 1) / t.s + 1;
+  const long long cells = (long long)t.ncx * ((height_org - 1) / t.s + 1);
+  if (cells > INT_MAX - TRACK_BLOCK) return fail(ctx, OFDIS_ERR_UNSUPPORTED, "track_begin: too many cells");
+  t.cells = (int)cells;
+  t.cells_pad = (t.cells + TRACK_BLOCK - 1) / TRACK_BLOCK * TRACK_BLOCK;
+  t.capacity = params->capacity;
+  t.cap_pad = (t.capacity + TRACK_BLOCK - 1) / TRACK_BLOCK * TRACK_BLOCK;
+  t.alpha = params->alpha;
+  t.beta = params->beta;
+  t.mb_alpha = params->mb_alpha;
+  t.mb_beta = params->mb_beta;
+  t.min_eig = params->min_eig;
+  rc = ensure_track(ctx, t);
+  if (rc) return rc;
+  ctx->tgeom = t;
+  const TrackWork& ws = ctx->track;
+  const size_t hwc = (size_t)width_org * height_org * ctx->prm.noc;
+  const unsigned char* I = frame;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(ctx->d_stage, frame, hwc, cudaMemcpyHostToDevice, ctx->stream));
+    I = static_cast<const unsigned char*>(ctx->d_stage);
+  }
+  // no track yet: every keep flag and every cell's occupancy is 0
+  CK(cudaMemsetAsync(ws.state, 0, sizeof(TrackState), ctx->stream));
+  CK(cudaMemsetAsync(ws.flags, 0, t.cap_pad, ctx->stream));
+  CK(cudaMemsetAsync(ws.occ, 0, t.cells, ctx->stream));
+  ofdis_track_point* out = memkind == OFDIS_MEM_DEVICE ? points : ctx->track_out;
+  const int k = launch_track_seed_compact(t, ws, ctx->prm.noc, I, 0, out, 0, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "track_seed_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  ctx->track_cur = 1;
+  CK(cudaMemcpyAsync(count, ws.counts, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (memkind != OFDIS_MEM_DEVICE && *count > 0) {
+    CK(cudaMemcpyAsync(points, out, sizeof(ofdis_track_point) * *count, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  ctx->track_on = true;
+  return OFDIS_OK;
+}
+
+int ofdis_track_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames, size_t frame_stride,
+                        ofdis_track_point* points, int* counts, int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || b0 < 0 || b0 > ctx->max_frames - (f1 - f0) || !frames ||
+      !points || !counts || (memkind == OFDIS_MEM_DEVICE && reinterpret_cast<uintptr_t>(points) % 4))
+    return fail(ctx, OFDIS_ERR_ARG, "track_advance: bad argument");
+  if (!ctx->track_on) return fail(ctx, OFDIS_ERR_ARG, "track_advance: no ofdis_track_begin");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  const TrackGeom& t = ctx->tgeom;
+  if (width_org != t.w || height_org != t.h)
+    return fail(ctx, OFDIS_ERR_ARG, "track_advance: frame size differs from ofdis_track_begin's");
+  const size_t hwc = (size_t)width_org * height_org * ctx->prm.noc;
+  if (frame_stride < hwc) return fail(ctx, OFDIS_ERR_ARG, "track_advance: frame_stride below one frame");
+  NvtxRange nvtx("track", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0, D = ctx->dirs;
+  const TrackWork& ws = ctx->track;
+  const unsigned char* src = frames;
+  size_t stride = frame_stride;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    CK(cudaMemcpy2DAsync(ctx->d_stage, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    src = static_cast<const unsigned char*>(ctx->d_stage);
+    stride = hwc;
+  }
+  ofdis_track_point* out = memkind == OFDIS_MEM_DEVICE ? points : ctx->track_out;
+  const LevelGeom g = stepped(ctx->lev[0], D);
+  // a call that fails on the way leaves the tracker to a new ofdis_track_begin
+  ctx->track_on = false;
+  int cur = ctx->track_cur;
+  for (int k = 0; k < n; ++k) {
+    if (launch_track_advance(g, (f0 + k) * D, (b0 + k) * D, t, ws, cur, cx, cy, ctx->stream) < 0)
+      return fail(ctx, OFDIS_ERR_CUDA, "track_advance_kernel launch", cudaGetLastError());
+    const int l = launch_track_seed_compact(t, ws, ctx->prm.noc, src + k * stride, cur, out + (size_t)k * t.capacity,
+                                            k, ctx->stream);
+    if (l < 0) return fail(ctx, OFDIS_ERR_CUDA, "track_seed_kernel launch", cudaGetLastError());
+    ctx->launches += 1 + l;
+    cur ^= 1;
+  }
+  ctx->track_cur = cur;
+  CK(cudaMemcpyAsync(counts, ws.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (memkind != OFDIS_MEM_DEVICE) {
+    for (int k = 0; k < n; ++k)
+      if (counts[k] > 0)
+        CK(cudaMemcpyAsync(points + (size_t)k * t.capacity, out + (size_t)k * t.capacity,
+                           sizeof(ofdis_track_point) * counts[k], cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  ctx->track_on = true;
+  return OFDIS_OK;
+}
+
+int ofdis_track_stats_get(const ofdis_ctx* ctx, ofdis_track_stats* out) {
+  if (!ctx || !out || !ctx->track_on) return OFDIS_ERR_ARG;
+  TrackState s;
+  if (cudaSetDevice(ctx->device) != cudaSuccess ||
+      cudaMemcpyAsync(&s, ctx->track.state, sizeof(s), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+      cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+    return OFDIS_ERR_CUDA;
+  out->seeded = (long long)s.seeded;
+  out->ended_leaves = (long long)s.ended[0];
+  out->ended_inconsistent = (long long)s.ended[1];
+  out->ended_boundary = (long long)s.ended[2];
+  out->dropped = (long long)s.dropped;
+  out->alive = s.alive;
+  out->next_id = s.next_id;
   return OFDIS_OK;
 }
 

@@ -399,19 +399,8 @@ __global__ void __launch_bounds__(256) consistency_kernel(LevelGeom g, int fa, i
     if (err) err[o] = __int_as_float(0x7f800000);
     return;
   }
-  const int x0 = (int)floorf(xs), y0 = (int)floorf(ys);
-  const int x1 = min(x0 + 1, w_org - 1), y1 = min(y0 + 1, h_org - 1);
-  const float fx = xs - (float)x0, fy = ys - (float)y0, gx = 1.0f - fx, gy = 1.0f - fy;
-  float c00[2], c10[2], c01[2], c11[2];
-  upsample_at<NOP>(g, B, x0, y0, crop_x, crop_y, [&c00](int c, float v) { c00[c] = v; });
-  upsample_at<NOP>(g, B, x1, y0, crop_x, crop_y, [&c10](int c, float v) { c10[c] = v; });
-  upsample_at<NOP>(g, B, x0, y1, crop_x, crop_y, [&c01](int c, float v) { c01[c] = v; });
-  upsample_at<NOP>(g, B, x1, y1, crop_x, crop_y, [&c11](int c, float v) { c11[c] = v; });
   float b[2] = {0.f, 0.f};
-  for (int c = 0; c < NOP; ++c) {
-    const float r0 = c00[c] * gx + c10[c] * fx, r1 = c01[c] * gx + c11[c] * fx;
-    b[c] = r0 * gy + r1 * fy;
-  }
+  flow_bilinear_at<NOP>(g, B, xs, ys, w_org, h_org, crop_x, crop_y, b);
   const float du = u + b[0], dv = NOP == 2 ? v + b[1] : 0.f;
   const float e = du * du + dv * dv;
   const float mag = (u * u + v * v) + (b[0] * b[0] + b[1] * b[1]);

@@ -591,6 +591,16 @@ int main(int argc, char** argv) {
 // (computed on the decoder's BGR order, written as RGB).  The backward slots run in the same launch, as with
 // --bidirectional, but the _bw and _occ files are only written when --bidirectional is given too; every other output
 // keeps its bytes.  Not with --warm-start.
+//
+// --tracks PATH: dense point trajectories through the pairs (ofdis_track_begin / ofdis_track_advance).  A pair that
+// does not continue the previous one starts a new clip with ofdis_track_begin on its image1; the pairs of a clip
+// continue the same tracker, across batches.  Settings: spacing 8, capacity 4 x the cells, alpha/beta of
+// --bidirectional, mb_alpha 0.01, mb_beta 0.002 (Sundaram et al.'s motion-boundary test), min_eig 25 (about 1 grey
+// level^2 per pixel over the 5 x 5 window).  PATH gets the header `# clip frame id x y`, then one line per live track
+// and frame, clips and frames counted from 0, x and y printed with %.9g (which round-trips float32).  The backward
+// slots run in the same launch, as with --interpolate; every other output keeps its bytes.  With verbosity > 0 a
+// line `TRACKS clips C frames N seeded S leaves L inconsistent I boundary B dropped D` follows the TIME line.  Not
+// with --warm-start.
 
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
@@ -802,7 +812,7 @@ int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr,
             "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
-            "       [--color [--color-max M]] [--interpolate T]\n"
+            "       [--color [--color-max M]] [--interpolate T] [--tracks PATH]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -818,7 +828,9 @@ int main(int argc, char** argv) {
             "  output (flow: Middlebury's color wheel, stereo: KITTI's disparity colors), colored on the device\n"
             "  --color-max M: color every pair with the scale M (a positive finite number) instead of its own maximum\n"
             "  --interpolate T: also write <stem>_interp.png, the frame at time T (0 < T < 1) between image1 and image2,\n"
-            "  synthesised on the device from the forward and backward flows; not with --warm-start\n",
+            "  synthesised on the device from the forward and backward flows; not with --warm-start\n"
+            "  --tracks PATH: dense point trajectories through every clip of the list, written to PATH as lines\n"
+            "  `clip frame id x y`; not with --warm-start\n",
             argv[0]);
     return 2;
   }
@@ -829,6 +841,7 @@ int main(int argc, char** argv) {
   const char* interp_arg = nullptr;  // --interpolate T
   float interp_t = 0.0f;
   const char* gtlist = nullptr;
+  const char* tracks_path = nullptr;  // --tracks PATH
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -860,6 +873,13 @@ int main(int argc, char** argv) {
       }
       interp_arg = argv[first_num + 1];
       first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--tracks")) {
+      if (argc < first_num + 2 || tracks_path) {
+        fprintf(stderr, "error: --tracks takes one output path\n");
+        return 2;
+      }
+      tracks_path = argv[first_num + 1];
+      first_num += 2;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
         fprintf(stderr, "error: --gt takes one ground-truth list file\n");
@@ -883,6 +903,10 @@ int main(int argc, char** argv) {
     fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --interpolate\n");
     return 2;
   }
+  if (warm && tracks_path) {
+    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --tracks\n");
+    return 2;
+  }
   if (interp_arg) {
     char* end = nullptr;
     interp_t = strtof(interp_arg, &end);
@@ -891,8 +915,8 @@ int main(int argc, char** argv) {
       return 2;
     }
   }
-  // --interpolate needs the backward flows: the backward slots run whenever either option is given
-  const bool two_way = bidir || interp_arg;
+  // --interpolate and --tracks need the backward flows: the backward slots run whenever one of them is given
+  const bool two_way = bidir || interp_arg || tracks_path;
   if (color_max_arg) {
     char* end = nullptr;
     color_max = strtof(color_max_arg, &end);
@@ -955,6 +979,15 @@ int main(int argc, char** argv) {
       }
     }
   }
+  FILE* tracks_file = nullptr;
+  if (tracks_path) {
+    tracks_file = fopen(tracks_path, "w");
+    if (!tracks_file) {
+      fprintf(stderr, "error: cannot write %s\n", tracks_path);
+      return 1;
+    }
+    fprintf(tracks_file, "# clip frame id x y\n");
+  }
   const int nclasses = bidir ? 3 : 1;  // with --bidirectional the forward consistency mask's classes
   vector<ofdis_error_stats> eval_total(nclasses + 1), eval_pairs;  // [0]: all pixels, [1 + c]: class c
   memset(eval_total.data(), 0, sizeof(ofdis_error_stats) * eval_total.size());
@@ -971,6 +1004,29 @@ int main(int argc, char** argv) {
   vector<uint8_t> colors;  // --color: the color images of the slots
   vector<uint8_t> interp, interp_png;  // --interpolate: the frames at time T, one written as RGB
   Image8 last;  // image2 of the previous batch's last pair
+  // --tracks: the tracker's points and counts, the clip being tracked (-1 none) and its next frame, the totals of the
+  // finished clips
+  vector<ofdis_track_point> tpoints;
+  vector<int> tcounts;
+  int tclip = -1, tframe = 0;
+  size_t tframes = 0;
+  ofdis_track_stats ttotal;
+  memset(&ttotal, 0, sizeof(ttotal));
+  auto end_clip = [&]() {  // adds the tracked clip's counters to the totals
+    ofdis_track_stats st;
+    if (tclip < 0 || ofdis_track_stats_get(ctx, &st) != OFDIS_OK) return;
+    ttotal.seeded += st.seeded;
+    ttotal.ended_leaves += st.ended_leaves;
+    ttotal.ended_inconsistent += st.ended_inconsistent;
+    ttotal.ended_boundary += st.ended_boundary;
+    ttotal.dropped += st.dropped;
+  };
+  auto write_tracks = [&](const ofdis_track_point* p, int count) {
+    for (int i = 0; i < count; ++i)
+      fprintf(tracks_file, "%d %d %d %.9g %.9g\n", tclip, tframe, p[i].id, (double)p[i].x, (double)p[i].y);
+    ++tframe;
+    ++tframes;
+  };
   size_t j0 = 0;
   while (j0 < jobs.size()) {
     // load up to maxb pairs of one size; a frame that continues the previous pair is not decoded again
@@ -1027,6 +1083,7 @@ int main(int argc, char** argv) {
     parse_cli_params(nnum, argv + first_num, w, P);
     verbosity = P.verbosity;
     if (w != ctx_w || h != ctx_h) {
+      end_clip();  // a pair of another size never continues the previous one
       if (ctx) ofdis_destroy(ctx);
       ctx = nullptr;
       ofdis_params p;
@@ -1087,6 +1144,33 @@ int main(int argc, char** argv) {
       rc = ofdis_interpolate_fullres(ctx, 0, n, n, frames.data(), frames.data() + hwc, seq ? hwc : 2 * hwc, interp_t,
                                      nop == 2 ? 0.01f : 0.0f, nop == 2 ? 0.5f : 1.0f, interp.data(), nullptr, w, h,
                                      OFDIS_MEM_HOST);
+    }
+    // --tracks: runs of pairs that continue each other; a run that does not continue the previous pair begins a clip
+    for (int k0 = 0, k1; k0 < n && tracks_file && rc == OFDIS_OK; k0 = k1) {
+      for (k1 = k0 + 1; k1 < n && jobs[j0 + k1].a == jobs[j0 + k1 - 1].b;) ++k1;
+      const size_t fs = seq ? hwc : 2 * hwc;  // image1 of pair k at k * fs, its image2 one frame later
+      const uint8_t* im1 = frames.data() + (size_t)k0 * fs;
+      const uint8_t* im2 = im1 + hwc;
+      ofdis_track_params tp;
+      tp.spacing = 8;
+      tp.capacity = 4 * ((w + 7) / 8) * ((h + 7) / 8);
+      tp.alpha = nop == 2 ? 0.01f : 0.0f;
+      tp.beta = nop == 2 ? 0.5f : 1.0f;
+      tp.mb_alpha = 0.01f;
+      tp.mb_beta = 0.002f;
+      tp.min_eig = 25.0f;
+      tpoints.resize((size_t)n * tp.capacity);
+      tcounts.resize(n);
+      if (j0 + k0 == 0 || jobs[j0 + k0].a != jobs[j0 + k0 - 1].b) {
+        end_clip();
+        ++tclip;
+        tframe = 0;
+        rc = ofdis_track_begin(ctx, &tp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
+        if (rc == OFDIS_OK) write_tracks(tpoints.data(), tcounts[0]);
+      }
+      if (rc == OFDIS_OK)
+        rc = ofdis_track_advance(ctx, k0, k1, n + k0, im2, fs, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
+      for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k) write_tracks(tpoints.data() + (size_t)k * tp.capacity, tcounts[k]);
     }
     if (rc == OFDIS_OK) rc = ofdis_sync(ctx);
     if (rc == OFDIS_OK && gtlist) {
@@ -1157,10 +1241,18 @@ int main(int argc, char** argv) {
     j0 += n;
     done += n;
   }
+  end_clip();
   if (ctx) ofdis_destroy(ctx);
+  if (tracks_file && fclose(tracks_file) != 0) {
+    fprintf(stderr, "error: cannot write %s\n", tracks_path);
+    return 1;
+  }
   if (verbosity > 0) printf("TIME (%zu pairs, load + flow + save) (ms): %3g\n", done, elapsed_ms(tv));
   if (verbosity > 0 && seq_pairs) printf("SEQUENCE (%zu of %zu pairs from %zu decoded frames)\n", seq_pairs, done, seq_decoded);
   if (verbosity > 0 && warm) printf("WARM START (%zu of %zu pairs from the previous pair's flow)\n", warm_pairs, done);
+  if (verbosity > 0 && tracks_path)
+    printf("TRACKS clips %d frames %zu seeded %lld leaves %lld inconsistent %lld boundary %lld dropped %lld\n", tclip + 1,
+           tframes, ttotal.seeded, ttotal.ended_leaves, ttotal.ended_inconsistent, ttotal.ended_boundary, ttotal.dropped);
   if (verbosity > 0 && gtlist) {
     static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
     print_eval("", done, eval_total[0]);

@@ -758,3 +758,149 @@ def interpolate_frames(frames0: np.ndarray, frames1: np.ndarray, fw: np.ndarray,
     if one:
         out, flow_t = out[0], flow_t[0]
     return (out, flow_t, rounds) if with_rounds else (out, flow_t)
+
+
+# ofdis_track_point (include/ofdis_b200.h), field for field
+TRACK_POINT_DTYPE = np.dtype([("id", "<i4"), ("x", "<f4"), ("y", "<f4")])
+# ofdis_track_params, field for field
+TRACK_PARAM_FIELDS = ("capacity", "spacing", "alpha", "beta", "mb_alpha", "mb_beta", "min_eig")
+TRACK_STATS_FIELDS = ("seeded", "ended_leaves", "ended_inconsistent", "ended_boundary", "dropped", "alive", "next_id")
+_TRACK_ID_END = 2 ** 31 - 1  # next_id never exceeds this
+
+
+def _flow_bilinear(F: np.ndarray, xs: np.ndarray, ys: np.ndarray):
+    """Channels of the full-resolution flow F (h, w, nop) at in-frame positions: the rule of consistency_check."""
+    f32 = np.float32
+    h, w, nop = F.shape
+    x0 = np.floor(xs).astype(np.int64)
+    y0 = np.floor(ys).astype(np.int64)
+    x1 = np.minimum(x0 + 1, w - 1)
+    y1 = np.minimum(y0 + 1, h - 1)
+    fx = (xs - x0.astype(f32)).astype(f32)
+    fy = (ys - y0.astype(f32)).astype(f32)
+    gx, gy = f32(1) - fx, f32(1) - fy
+    out = []
+    for c in range(nop):
+        Fc = F[..., c]
+        r0 = Fc[y0, x0] * gx + Fc[y0, x1] * fx
+        r1 = Fc[y1, x0] * gx + Fc[y1, x1] * fx
+        out.append(r0 * gy + r1 * fy)
+    return out
+
+
+def track_seed_eigen(frame: np.ndarray, spacing: int):
+    """The seed pixels (cx, cy) of every cell, row-major, and the smaller eigenvalue of the structure tensor over the
+    5 x 5 window around each (ofdis_track_begin's header), float32."""
+    f32 = np.float32
+    I = np.asarray(frame, np.uint8)
+    h, w = I.shape[:2]
+    if I.ndim == 3 and I.shape[2] == 3:
+        g = (I[..., 0].astype(f32) + I[..., 1].astype(f32) + I[..., 2].astype(f32)) / f32(3)
+    else:
+        g = I.reshape(h, w).astype(f32)
+    xs = np.arange(w)
+    ys = np.arange(h)
+    Ix = (g[:, np.minimum(xs + 1, w - 1)] - g[:, np.maximum(xs - 1, 0)]) * f32(0.5)
+    Iy = (g[np.minimum(ys + 1, h - 1), :] - g[np.maximum(ys - 1, 0), :]) * f32(0.5)
+    s = int(spacing)
+    ncx, ncy = (w - 1) // s + 1, (h - 1) // s + 1
+    c = np.arange(ncx * ncy)
+    cx = np.minimum((c % ncx) * s + s // 2, w - 1)
+    cy = np.minimum((c // ncx) * s + s // 2, h - 1)
+    a = np.zeros(c.size, f32)
+    b = np.zeros(c.size, f32)
+    d2 = np.zeros(c.size, f32)
+    for dy in range(-2, 3):
+        py = np.clip(cy + dy, 0, h - 1)
+        for dx in range(-2, 3):
+            px = np.clip(cx + dx, 0, w - 1)
+            ix, iy = Ix[py, px], Iy[py, px]
+            a = a + ix * ix
+            b = b + ix * iy
+            d2 = d2 + iy * iy
+    d = a - d2
+    lam = (a + d2) * f32(0.5) - np.sqrt(d * d * f32(0.25) + b * b)
+    return cx, cy, lam
+
+
+def _track_seed(frame, tracks, next_id, stats, p):
+    s = int(p["spacing"])
+    h, w = frame.shape[:2]
+    cx, cy, lam = track_seed_eigen(frame, s)
+    ncx = (w - 1) // s + 1
+    occ = np.zeros(cx.size, bool)
+    occ[(tracks["y"].astype(np.int64) // s) * ncx + tracks["x"].astype(np.int64) // s] = True
+    cells = np.flatnonzero(~occ & (lam >= np.float32(p["min_eig"])))
+    adm = max(min(cells.size, int(p["capacity"]) - tracks.size, _TRACK_ID_END - next_id), 0)
+    new = np.empty(adm, TRACK_POINT_DTYPE)
+    new["id"] = next_id + np.arange(adm)
+    new["x"] = cx[cells[:adm]]
+    new["y"] = cy[cells[:adm]]
+    stats["seeded"] += adm
+    stats["dropped"] += cells.size - adm
+    return np.concatenate([tracks, new]), next_id + adm
+
+
+def _track_advance(tracks, F, B, stats, p):
+    f32 = np.float32
+    h, w, nop = F.shape
+    x, y = tracks["x"], tracks["y"]
+    with np.errstate(invalid="ignore", over="ignore"):
+        f = _flow_bilinear(F, x, y)
+        u = f[0]
+        v = f[1] if nop == 2 else np.zeros_like(u)
+        xn, yn = x + u, y + v
+        inside = (xn >= 0) & (xn <= f32(w - 1)) & (yn >= 0) & (yn <= f32(h - 1))
+        b = _flow_bilinear(B, np.where(inside, xn, f32(0)), np.where(inside, yn, f32(0)))
+        b0 = b[0]
+        b1 = b[1] if nop == 2 else np.zeros_like(u)
+        du = u + b0
+        dv = v + b1 if nop == 2 else np.zeros_like(u)
+        err = du * du + dv * dv
+        mag = (u * u + v * v) + (b0 * b0 + b1 * b1)
+        consistent = inside & (err <= f32(p["alpha"]) * mag + f32(p["beta"]))
+        xr = np.floor(x + f32(0.5)).astype(np.int64)
+        yr = np.floor(y + f32(0.5)).astype(np.int64)
+        l, r = F[yr, np.maximum(xr - 1, 0)], F[yr, np.minimum(xr + 1, w - 1)]
+        up, dn = F[np.maximum(yr - 1, 0), xr], F[np.minimum(yr + 1, h - 1), xr]
+        ux = (r[:, 0] - l[:, 0]) * f32(0.5)
+        uy = (dn[:, 0] - up[:, 0]) * f32(0.5)
+        g2 = ux * ux + uy * uy
+        if nop == 2:
+            vx = (r[:, 1] - l[:, 1]) * f32(0.5)
+            vy = (dn[:, 1] - up[:, 1]) * f32(0.5)
+            g2 = g2 + (vx * vx + vy * vy)
+        boundary = consistent & (g2 > f32(p["mb_alpha"]) * (u * u + v * v) + f32(p["mb_beta"]))
+    keep = consistent & ~boundary
+    stats["ended_leaves"] += int((~inside).sum())
+    stats["ended_inconsistent"] += int((inside & ~consistent).sum())
+    stats["ended_boundary"] += int(boundary.sum())
+    out = tracks[keep].copy()
+    out["x"] = xn[keep]
+    out["y"] = yn[keep]
+    return out
+
+
+def track_points(frames: np.ndarray, fw: np.ndarray, bw: np.ndarray, params):
+    """ofdis_track_begin on frames[0] followed by ofdis_track_advance through the n pairs, bit for bit, float32
+    without contraction.  frames: the clip, (n + 1, h, w[, noc]) uint8; fw, bw: the full-resolution forward flows
+    (frame k -> k + 1) and their backward partners, (n, h, w, nop) float32 (stereo also without the last axis);
+    params: a mapping with the keys of TRACK_PARAM_FIELDS.  Returns (lists, stats): n + 1 arrays of
+    TRACK_POINT_DTYPE, the live tracks after each frame sorted by id, and a dict of TRACK_STATS_FIELDS."""
+    p = {k: params[k] for k in TRACK_PARAM_FIELDS}
+    clip = np.asarray(frames, np.uint8)
+    F = np.asarray(fw, np.float32)
+    B = np.asarray(bw, np.float32)
+    n = clip.shape[0] - 1
+    F = F.reshape(F.shape[:3] + (-1,))
+    B = B.reshape(B.shape[:3] + (-1,))
+    assert F.shape[0] == n and B.shape == F.shape and F.shape[1:3] == clip.shape[1:3], (clip.shape, F.shape, B.shape)
+    stats = dict.fromkeys(TRACK_STATS_FIELDS, 0)
+    tracks, next_id = _track_seed(clip[0], np.empty(0, TRACK_POINT_DTYPE), 0, stats, p)
+    lists = [tracks]
+    for k in range(n):
+        tracks = _track_advance(tracks, F[k], B[k], stats, p)
+        tracks, next_id = _track_seed(clip[k + 1], tracks, next_id, stats, p)
+        lists.append(tracks)
+    stats["alive"], stats["next_id"] = int(tracks.size), int(next_id)
+    return lists, stats

@@ -4,8 +4,8 @@ the smoke configuration (P=8 gray flow) with both exact SOR kernels (sor_lane_ke
 sor_wave_kernel: single CTA), a forward-backward case, a P=12 RGB and a P=12 stereo case (window-staged patch
 kernel, stereo SOR), a 70-row level as three bands of the lane kernel and forced into a cluster of bands of the
 wave kernel with 1 and 2 rows per thread (st.async halo exchange), and the 8-bit frame path (pyramid and
-upsampling kernels), and a frame interpolation checked against its restatement.  Results are checked against the
-oracle so that a clean log means a correct run."""
+upsampling kernels), and a frame interpolation and a point tracking (advance, seed, block scan, scatter) checked
+against their restatements.  Results are checked against the oracle so that a clean log means a correct run."""
 import os
 import sys
 
@@ -65,6 +65,20 @@ ctx.close()
 exp, exp_ut = preprocess.interpolate_frames(clip[:-1], clip[1:], full[:n], full[n:], 0.5, 0.01, 0.5)
 ok = np.array_equal(out, exp) and np.array_equal(ut.view(np.uint32), exp_ut.view(np.uint32))
 print("%-22s %s" % ("interpolate_rgb", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# point tracking through the same two-way clip, with a capacity that drops seeds (every tracker kernel, the
+# single-CTA scan over several blocks of flags)
+tp = dict(capacity=1000, spacing=2, alpha=0.01, beta=0.5, mb_alpha=0.01, mb_beta=0.002, min_eig=4.0)
+ctx = api.Context(prm, 96, 64, prm.p_samp_s, 2 * n)
+ctx.upload_sequence_bidir_u8(0, n, clip, w, h)
+ctx.run(2 * n)
+lists = [ctx.track_begin(tp, clip[0], w, h)] + ctx.track_advance(0, n, n, clip[1:], w, h)
+st = ctx.track_stats()
+ctx.close()
+exp, est = preprocess.track_points(clip, full[:n], full[n:], tp)
+ok = st == est and all(np.array_equal(g.view(np.uint8), e.view(np.uint8)) for g, e in zip(lists, exp))
+print("%-22s %s" % ("track_rgb", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
