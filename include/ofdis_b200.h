@@ -348,6 +348,57 @@ int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsi
                               size_t frame_stride, float t, float alpha, float beta, unsigned char* out, float* flow_t,
                               int width_org, int height_org, int memkind);
 
+/* Filtered disparity, depth and point cloud from stereo flows (extension, stereo contexts only).  Everything is
+ * float32 without contraction, with IEEE division; preprocess.disparity_filter restates it.  W = width_org,
+ * H = height_org, qNaN = the quiet NaN 0x7fc00000; "the smaller of a and b" is (b < a) ? b : a, so of two equal values
+ * (+0 and -0 among them) the first one is taken.  For every pair k < f1-f0, in this order:
+ *   1. Disparity.  F is slot a = f0+k's full-resolution flow, exactly what ofdis_get_flow_fullres returns (computed from
+ *      the level flows without a full-resolution copy); d = -F for an ordinary slot, +F for a slot marked swapped (the
+ *      rule of OFDIS_ENC_KITTI and of the stereo color map).
+ *   2. Status.  3 when d is not in [0, 1e9] (NaN fails, -0 passes); else, with lr_check, the mask of
+ *      ofdis_consistency_fullres(alpha, beta) of slot a against slot b0+k, bitwise (1 inconsistent, 2 leaves the
+ *      frame); else 0, valid.
+ *   3. Speckles (speckle_size > 0).  Two 4-neighbours of status 0 are joined when fabsf(d_p - d_q) <= speckle_diff
+ *      (diagonal neighbours are not); every pixel of a connected component of at most speckle_size pixels gets status 4.
+ *   4. Fill (fill = 1).  At first only the pixels of status 0 have a value, d.  Row pass: each maximal run [x1, x2] of
+ *      pixels without a value with x1 > 0 and x2 < W-1 takes the smaller of the values at x1-1 and x2+1; pixels left of
+ *      the row's first value take that value, pixels right of its last value that one.  Then the same rule along the
+ *      columns over what the row pass left.  After the row pass a row is either full or empty, so the column pass
+ *      fills the empty rows: bridging empty rows between two full ones is this library's choice (KITTI's devkit is
+ *      described as extrapolating up and down only).  A frame without a status-0 pixel stays empty.  These rules
+ *      follow the description of the devkit's interpolateBackground; they have not been compared with its output.
+ *   5. Outputs, each [n][H][W] in memkind and each may be NULL, but not all four:
+ *      disp: d where the status is 0, the filled value where one exists, else qNaN;
+ *      status: bytes 0..4; filling does not change it, so status != 0 with a finite disp marks a filled pixel;
+ *      depth: with D = disp, Z = (fx * baseline) / (D + doffs) where D + doffs > 0 (NaN fails), else qNaN; the product
+ *        fx * baseline is rounded once;
+ *      xyz: [n][H][W][3], (((float)x - cx) * Z) / fx, (((float)y - cy) * Z) / fy, Z.
+ *      Every NaN written to depth or xyz is qNaN.
+ * cam is required for depth and xyz, one camera per call (the right view's depth takes the right camera, e.g.
+ * Middlebury's cam1, in a call of its own): fx, fy, baseline finite and > 0, cx, cy, doffs finite.  filt: lr_check and
+ * fill 0 or 1, alpha, beta and speckle_diff finite and >= 0, speckle_size >= 0.  b0 is read only with lr_check.
+ * OFDIS_ERR_ARG: a flow context (nop 2), slots outside the context, a NULL or bad filt, a missing or bad cam when depth
+ * or xyz is asked for, all four outputs NULL, or a device output that is not aligned to its element; frame sizes as
+ * ofdis_get_flow_fullres checks them; W * H >= 2^31 is OFDIS_ERR_UNSUPPORTED (the labels are int32 per frame).
+ * The workspace -- per pixel and pair 13 bytes (d, the parent, the component size, the status) and per row and pair
+ * 12 (the row pass's flag and the nearest full rows), for max_frames pairs of the context's size -- is allocated on
+ * the first call, never shrinks, and is freed by ofdis_destroy.  Host outputs go through the context's
+ * full-resolution scratch, grown to max_frames x 21 bytes per pixel of the call's size (disp, depth and xyz floats, then
+ * the status bytes) and at least what ofdis_get_flow_fullres asks for.  Enqueued on the context's stream with a fixed
+ * number of kernels per call whatever the number of pairs (2, + 3 with speckles, + 2 with fill); host outputs
+ * synchronise it.  Not part of ofdis_run's graph; the flows are not changed. */
+typedef struct ofdis_disp_filter {
+  int lr_check;        /* 0 | 1: test slot f0+k against partner slot b0+k */
+  float alpha, beta;   /* the rule of ofdis_consistency_fullres (usual: 0, 1) */
+  int speckle_size;    /* 0: off; else components of at most this many pixels are removed */
+  float speckle_diff;  /* 4-neighbours join a component when |d_p - d_q| <= speckle_diff */
+  int fill;            /* 0 | 1: background fill */
+} ofdis_disp_filter;
+typedef struct ofdis_stereo_camera { float fx, fy, cx, cy, baseline, doffs; } ofdis_stereo_camera;
+int ofdis_disparity_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_disp_filter* filt,
+                            const ofdis_stereo_camera* cam, float* disp, unsigned char* status, float* depth,
+                            float* xyz, int width_org, int height_org, int memkind);
+
 /* Dense point trajectories (extension): the tracker of Sundaram, Brox and Keutzer ("Dense point trajectories by
  * GPU-accelerated large displacement optical flow", ECCV 2010) through consecutive pairs of bidirectional flows.
  * The context owns one tracker: the list of live tracks (sorted by id), the next id and the counters.  It persists

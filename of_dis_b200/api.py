@@ -14,7 +14,8 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE, TRACK_STATS_FIELDS
+from .preprocess import (DISP_FILTER_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE,
+                         TRACK_STATS_FIELDS)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("OFDIS_LIB") or os.path.join(_HERE, "lib", "libofdis_b200.so")  # OFDIS_LIB: experiments only
@@ -36,8 +37,11 @@ EXPORTS = [
     "ofdis_set_initflow_from_result", "ofdis_upload_sequence_bidir_u8", "ofdis_set_swapped_slots",
     "ofdis_consistency_fullres", "ofdis_flow_error_fullres", "ofdis_debug_sor_plan",
     "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres", "ofdis_interpolate_fullres",
-    "ofdis_track_begin", "ofdis_track_advance", "ofdis_track_stats_get",
+    "ofdis_track_begin", "ofdis_track_advance", "ofdis_track_stats_get", "ofdis_disparity_fullres",
 ]
+
+# outputs of disparity_fullres, in the C-ABI's argument order
+DISP_OUTPUTS = ("disp", "status", "depth", "xyz")
 
 # encodings of get_flow_fullres_encoded (OFDIS_ENC_F16, OFDIS_ENC_KITTI)
 ENCODINGS = {"f16": 1, "kitti": 2}
@@ -63,6 +67,20 @@ class TrackStats(ctypes.Structure):
     """ofdis_track_stats (include/ofdis_b200.h)."""
     _fields_ = [(k, ctypes.c_longlong) for k in TRACK_STATS_FIELDS[:5]] + \
         [(k, ctypes.c_int) for k in TRACK_STATS_FIELDS[5:]]
+
+
+class DispFilter(ctypes.Structure):
+    """ofdis_disp_filter (include/ofdis_b200.h)."""
+    _fields_ = [("lr_check", ctypes.c_int), ("alpha", ctypes.c_float), ("beta", ctypes.c_float),
+                ("speckle_size", ctypes.c_int), ("speckle_diff", ctypes.c_float), ("fill", ctypes.c_int)]
+
+
+class StereoCamera(ctypes.Structure):
+    """ofdis_stereo_camera (include/ofdis_b200.h)."""
+    _fields_ = [(k, ctypes.c_float) for k in STEREO_CAMERA_FIELDS]
+
+
+assert tuple(k for k, _ in DispFilter._fields_) == DISP_FILTER_FIELDS
 
 
 class OfdisError(RuntimeError):
@@ -124,6 +142,8 @@ def lib():
             [ctypes.c_int] * 3
         L.ofdis_track_advance.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p, ctypes.c_size_t] + \
             [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
+        L.ofdis_disparity_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
+            [ctypes.POINTER(DispFilter), ctypes.POINTER(StereoCamera)] + [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3
         L.ofdis_track_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackStats)]
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -317,6 +337,42 @@ class Context:
         if memkind == MEM_HOST:
             self.sync()
         return mask, err
+
+    def disparity_fullres(self, f0, f1, b0, width_org, height_org, lr_check=0, alpha=0.0, beta=1.0, speckle_size=0,
+                          speckle_diff=1.0, fill=0, camera=None, outputs=("disp", "status"), memkind=MEM_HOST,
+                          out=None):
+        """Filtered disparities of the last run's stereo slots [f0, f1), left-right checked against slots
+        [b0, b0 + f1 - f0) with lr_check, and from them depth and xyz with a camera (ofdis_disparity_fullres;
+        preprocess.disparity_filter restates it).  camera: None or a mapping with STEREO_CAMERA_FIELDS (required for
+        "depth" and "xyz").  Returns a dict of the requested DISP_OUTPUTS.  Host: "disp" and "depth" (f1-f0,
+        height_org, width_org) float32, "status" the same in uint8, "xyz" (f1-f0, height_org, width_org, 3) float32,
+        new or given in `out` as numpy arrays of exactly that dtype and shape; the call synchronises the stream.
+        With memkind=MEM_DEVICE, `out` maps the requested outputs to device addresses the caller owns, and the
+        call is enqueued on the context's stream."""
+        unknown = set(outputs) - set(DISP_OUTPUTS)
+        if unknown:
+            raise ValueError("disparity_fullres: unknown outputs %s" % sorted(unknown))
+        out = dict(out or {})
+        if memkind == MEM_HOST:
+            n = max(f1 - f0, 0)
+            for name in outputs:
+                shape = (n, height_org, width_org) + ((3,) if name == "xyz" else ())
+                dt = np.uint8 if name == "status" else np.float32
+                arr = out.setdefault(name, np.empty(shape, dt))
+                if not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape == shape
+                        and arr.flags["C_CONTIGUOUS"] and arr.flags["WRITEABLE"]):
+                    raise ValueError("disparity_fullres: %s must be a writeable C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shape))
+        else:
+            missing = [name for name in outputs if out.get(name) is None]
+            if missing:
+                raise ValueError("disparity_fullres: no device address for the requested outputs %s" % missing)
+        filt = DispFilter(int(lr_check), alpha, beta, int(speckle_size), speckle_diff, int(fill))
+        cam = None if camera is None else ctypes.byref(StereoCamera(*[camera[k] for k in STEREO_CAMERA_FIELDS]))
+        ptrs = [_ptr(out.get(k)) if k in outputs else None for k in DISP_OUTPUTS]
+        self._ck(lib().ofdis_disparity_fullres(self._h, f0, f1, b0, ctypes.byref(filt), cam, *ptrs, width_org,
+                                               height_org, memkind))
+        return {k: out.get(k) for k in outputs}
 
     def flow_error_fullres(self, f0, f1, gt, width_org, height_org, classes=None, nclasses=None, with_err=False,
                            memkind=MEM_HOST, err=None):

@@ -84,6 +84,9 @@ struct ofdis_ctx {
   TrackGeom tgeom{};
   int track_cur = 0;
   bool track_on = false;
+  // lazily allocated workspace of ofdis_disparity_fullres (DispWork for max_frames pairs of width x height pixels);
+  // never touched by ofdis_run
+  void* d_disp = nullptr;
   std::vector<float*> d_flow;    // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -452,6 +455,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_color);
   cudaFree(ctx->d_interp);
   cudaFree(ctx->d_track);
+  cudaFree(ctx->d_disp);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -1063,6 +1067,88 @@ int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsi
   if (memkind != OFDIS_MEM_DEVICE) CK(cudaMemcpyAsync(out, dout, hwc * n, cudaMemcpyDeviceToHost, ctx->stream));
   if (flow_t)
     CK(cudaMemcpyAsync(flow_t, ws.ut, sizeof(float) * pix * nop * n, kind_out(memkind), ctx->stream));
+  return OFDIS_OK;
+}
+
+// The workspace of ofdis_disparity_fullres for max_frames pairs of the context's size, allocated on the first call:
+// per pixel and pair d, the parent and the component size (4 bytes each) and the status (1); per row and pair the
+// row pass's flag and the nearest full rows above and below (4 bytes each).  A call of a smaller frame size packs its
+// pairs densely at the front of each array.
+static int ensure_disp(ofdis_ctx* ctx, DispWork* ws) {
+  const size_t P = (size_t)ctx->max_frames * ctx->width * ctx->height, R = (size_t)ctx->max_frames * ctx->height;
+  if (!ctx->d_disp && cudaMalloc(&ctx->d_disp, P * 13 + R * 12) != cudaSuccess) {
+    ctx->d_disp = nullptr;
+    return fail(ctx, OFDIS_ERR_NOMEM, "disparity_fullres workspace");
+  }
+  char* b = static_cast<char*>(ctx->d_disp);
+  ws->val = reinterpret_cast<float*>(b);
+  ws->parent = reinterpret_cast<int*>(b + 4 * P);
+  ws->size = reinterpret_cast<int*>(b + 8 * P);
+  ws->rowfull = reinterpret_cast<int*>(b + 12 * P);
+  ws->up = ws->rowfull + R;
+  ws->down = ws->up + R;
+  ws->status = reinterpret_cast<unsigned char*>(b + 12 * P + 12 * R);
+  return OFDIS_OK;
+}
+
+static bool finite_ge0(float v) { return v >= 0.f && v <= FLT_MAX; }
+static bool finite_gt0(float v) { return v > 0.f && v <= FLT_MAX; }
+static bool finite_f32(float v) { return v >= -FLT_MAX && v <= FLT_MAX; }
+
+int ofdis_disparity_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_disp_filter* filt,
+                            const ofdis_stereo_camera* cam, float* disp, unsigned char* status, float* depth,
+                            float* xyz, int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  auto misaligned = [dev](const float* p) { return dev && reinterpret_cast<uintptr_t>(p) % sizeof(float); };
+  const bool need_cam = depth || xyz;
+  if (ctx->nop != 1 || f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !filt ||
+      (filt->lr_check && (b0 < 0 || b0 > ctx->max_frames - (f1 - f0))) ||
+      (filt->lr_check != 0 && filt->lr_check != 1) || (filt->fill != 0 && filt->fill != 1) ||
+      !finite_ge0(filt->alpha) || !finite_ge0(filt->beta) || filt->speckle_size < 0 ||
+      !finite_ge0(filt->speckle_diff) || (!disp && !status && !depth && !xyz) ||
+      (need_cam && (!cam || !finite_gt0(cam->fx) || !finite_gt0(cam->fy) || !finite_gt0(cam->baseline) ||
+                    !finite_f32(cam->cx) || !finite_f32(cam->cy) || !finite_f32(cam->doffs))) ||
+      misaligned(disp) || misaligned(depth) || misaligned(xyz))
+    return fail(ctx, OFDIS_ERR_ARG, "disparity_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  const size_t pix = (size_t)width_org * height_org;
+  if (pix > (size_t)INT_MAX) return fail(ctx, OFDIS_ERR_UNSUPPORTED, "disparity_fullres: 2^31 pixels or more per frame");
+  NvtxRange nvtx("disparity", -1);
+  CK(cudaSetDevice(ctx->device));
+  DispWork ws;
+  rc = ensure_disp(ctx, &ws);
+  if (rc) return rc;
+  const int n = f1 - f0, D = ctx->dirs;
+  const size_t np = pix * n;
+  DispOutputs out{disp, status, depth, xyz};
+  if (!dev) {
+    // the full-resolution scratch: disp, depth and xyz floats (those asked for), then the status bytes; sized for
+    // max_frames, and at least what ofdis_get_flow_fullres asks for
+    rc = ensure_full(ctx, std::max(pix * ctx->nop, pix * 5 + (pix + 3) / 4) * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    float* q = ctx->d_full;
+    if (disp) out.disp = q, q += np;
+    if (depth) out.depth = q, q += np;
+    if (xyz) out.xyz = q, q += 3 * np;
+    out.status = status ? reinterpret_cast<unsigned char*>(q) : nullptr;
+  }
+  const DispFilter f{filt->lr_check, filt->alpha, filt->beta, filt->speckle_size, filt->speckle_diff, filt->fill};
+  DispCamera c{};
+  if (need_cam) c = DispCamera{cam->fx * cam->baseline, cam->fx, cam->fy, cam->cx, cam->cy, cam->doffs};
+  const int k = launch_disparity(stepped(ctx->lev[0], D), f0 * D, (filt->lr_check ? b0 : f0) * D, n, f, c, ws, out,
+                                 width_org, height_org, cx, cy, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "disp_classify_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  if (!dev) {
+    if (disp) CK(cudaMemcpyAsync(disp, out.disp, sizeof(float) * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (depth) CK(cudaMemcpyAsync(depth, out.depth, sizeof(float) * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (xyz) CK(cudaMemcpyAsync(xyz, out.xyz, sizeof(float) * 3 * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (status) CK(cudaMemcpyAsync(status, out.status, np, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
   return OFDIS_OK;
 }
 

@@ -392,20 +392,10 @@ __global__ void __launch_bounds__(256) consistency_kernel(LevelGeom g, int fa, i
   const size_t o = (size_t)fr * h_org * w_org + (size_t)Y * w_org + X;
   float f[2] = {0.f, 0.f};
   upsample_at<NOP>(g, F, X, Y, crop_x, crop_y, [&f](int c, float v) { f[c] = v; });
-  const float u = f[0], v = NOP == 2 ? f[1] : 0.f;
-  const float xs = (float)X + u, ys = (float)Y + v;
-  if (!(xs >= 0.f && xs <= (float)(w_org - 1) && ys >= 0.f && ys <= (float)(h_org - 1))) {
-    mask[o] = 2;
-    if (err) err[o] = __int_as_float(0x7f800000);
-    return;
-  }
-  float b[2] = {0.f, 0.f};
-  flow_bilinear_at<NOP>(g, B, xs, ys, w_org, h_org, crop_x, crop_y, b);
-  const float du = u + b[0], dv = NOP == 2 ? v + b[1] : 0.f;
-  const float e = du * du + dv * dv;
-  const float mag = (u * u + v * v) + (b[0] * b[0] + b[1] * b[1]);
-  mask[o] = e <= alpha * mag + beta ? 0 : 1;
-  if (err) err[o] = e;
+  consistency_at<NOP>(g, B, f, X, Y, w_org, h_org, crop_x, crop_y, alpha, beta, [&](unsigned char m, float e) {
+    mask[o] = m;
+    if (err) err[o] = e;
+  });
 }
 
 // Evaluation of frame f0 + fr's full-resolution flow F (upsample_at, as flow_upsample_kernel writes it) against the

@@ -14,6 +14,7 @@
 #include <zlib.h>
 
 #include <cfloat>
+#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
@@ -601,6 +602,19 @@ int main(int argc, char** argv) {
 // slots run in the same launch, as with --interpolate; every other output keeps its bytes.  With verbosity > 0 a
 // line `TRACKS clips C frames N seeded S leaves L inconsistent I boundary B dropped D` follows the TIME line.  Not
 // with --warm-start.
+//
+// Stereo binaries only (the flow binaries refuse these flags, and so does --warm-start): filtered disparities
+// (ofdis_disparity_fullres) of every pair's left view.  --lr-check invalidates the pixels that fail the left-right
+// check of --bidirectional (alpha 0, beta 1; the backward slots run in the same launch, the _bw and _occ files are only
+// written when --bidirectional is given too); --speckle N R removes the components of at most N pixels whose
+// 4-neighbours differ by at most R px; --fill fills the holes with the background disparity; --camera
+// fx,fy,cx,cy,baseline,doffs gives depth and points.  With any of them every pair also gets <stem>_filtered<ext>, the
+// filtered disparity in the format and sign of <stem><ext> (PFM of the positive disparity, NaN where invalid; with
+// --kitti KITTI's 16-bit PNG with NaN as 0).  With --camera also <stem>_depth.pfm (Z as is, NaN where invalid) and
+// <stem>.ply, a binary little-endian point cloud of the pixels with a finite Z in row-major order: float x, y, z, then
+// uchar red, green, blue from image1 (gray replicated).  With verbosity > 0 every batch prints a line
+// `DISP pairs N valid V inconsistent I leaves L range R speckle S filled F` (the status counts, and the pixels of
+// another status that got a value).  Every other output keeps its bytes.
 
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
@@ -813,6 +827,7 @@ int main(int argc, char** argv) {
     fprintf(stderr,
             "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
             "       [--color [--color-max M]] [--interpolate T] [--tracks PATH]\n"
+            "       [--lr-check] [--speckle N R] [--fill] [--camera fx,fy,cx,cy,baseline,doffs]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -830,7 +845,11 @@ int main(int argc, char** argv) {
             "  --interpolate T: also write <stem>_interp.png, the frame at time T (0 < T < 1) between image1 and image2,\n"
             "  synthesised on the device from the forward and backward flows; not with --warm-start\n"
             "  --tracks PATH: dense point trajectories through every clip of the list, written to PATH as lines\n"
-            "  `clip frame id x y`; not with --warm-start\n",
+            "  `clip frame id x y`; not with --warm-start\n"
+            "  --lr-check, --speckle N R, --fill, --camera ...: stereo only; also write <stem>_filtered<ext>, the\n"
+            "  disparity without the pixels that fail the left-right check and the speckles of at most N pixels (R px),\n"
+            "  holes filled with the background disparity, and with --camera <stem>_depth.pfm and <stem>.ply;\n"
+            "  not with --warm-start\n",
             argv[0]);
     return 2;
   }
@@ -842,6 +861,9 @@ int main(int argc, char** argv) {
   float interp_t = 0.0f;
   const char* gtlist = nullptr;
   const char* tracks_path = nullptr;  // --tracks PATH
+  bool lr_check = false, disp_fill = false;  // --lr-check, --fill
+  const char* speckle_arg[2] = {nullptr, nullptr};  // --speckle N R
+  const char* camera_arg = nullptr;  // --camera fx,fy,cx,cy,baseline,doffs
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -880,6 +902,27 @@ int main(int argc, char** argv) {
       }
       tracks_path = argv[first_num + 1];
       first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--lr-check")) {
+      lr_check = true;
+      first_num += 1;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--fill")) {
+      disp_fill = true;
+      first_num += 1;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--speckle")) {
+      if (argc < first_num + 3 || speckle_arg[0]) {
+        fprintf(stderr, "error: --speckle takes a size N and a difference R\n");
+        return 2;
+      }
+      speckle_arg[0] = argv[first_num + 1];
+      speckle_arg[1] = argv[first_num + 2];
+      first_num += 3;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--camera")) {
+      if (argc < first_num + 2 || camera_arg) {
+        fprintf(stderr, "error: --camera takes fx,fy,cx,cy,baseline,doffs\n");
+        return 2;
+      }
+      camera_arg = argv[first_num + 1];
+      first_num += 2;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
         fprintf(stderr, "error: --gt takes one ground-truth list file\n");
@@ -907,6 +950,55 @@ int main(int argc, char** argv) {
     fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --tracks\n");
     return 2;
   }
+  const bool disp_on = lr_check || disp_fill || speckle_arg[0] || camera_arg;
+  if (disp_on && SELECTMODE == 1) {
+    fprintf(stderr, "error: --lr-check, --speckle, --fill and --camera filter stereo disparities; the flow binaries "
+                    "take none of them\n");
+    return 2;
+  }
+  if (warm && disp_on) {
+    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --lr-check, --speckle, --fill or --camera\n");
+    return 2;
+  }
+  ofdis_disp_filter dfilt;
+  memset(&dfilt, 0, sizeof(dfilt));
+  dfilt.lr_check = lr_check ? 1 : 0;
+  dfilt.alpha = 0.0f;
+  dfilt.beta = 1.0f;
+  dfilt.speckle_diff = 1.0f;
+  dfilt.fill = disp_fill ? 1 : 0;
+  if (speckle_arg[0]) {
+    char *e0 = nullptr, *e1 = nullptr;
+    const long sz = strtol(speckle_arg[0], &e0, 10);
+    const float diff = strtof(speckle_arg[1], &e1);
+    if (e0 == speckle_arg[0] || *e0 || sz < 1 || sz > INT_MAX || e1 == speckle_arg[1] || *e1 ||
+        !(diff >= 0.0f && diff <= FLT_MAX)) {
+      fprintf(stderr, "error: --speckle takes a size N >= 1 and a finite difference R >= 0, got %s %s\n", speckle_arg[0],
+              speckle_arg[1]);
+      return 2;
+    }
+    dfilt.speckle_size = (int)sz;
+    dfilt.speckle_diff = diff;
+  }
+  ofdis_stereo_camera dcam;
+  memset(&dcam, 0, sizeof(dcam));
+  if (camera_arg) {
+    float v[6];
+    const char* q = camera_arg;
+    bool ok = true;
+    for (int i = 0; i < 6 && ok; ++i) {
+      char* end = nullptr;
+      v[i] = strtof(q, &end);
+      ok = end != q && (i < 5 ? *end == ',' : *end == 0) && v[i] >= -FLT_MAX && v[i] <= FLT_MAX;
+      q = end + (i < 5 ? 1 : 0);
+    }
+    if (!ok || !(v[0] > 0.0f) || !(v[1] > 0.0f) || !(v[4] > 0.0f)) {
+      fprintf(stderr, "error: --camera takes six finite numbers fx,fy,cx,cy,baseline,doffs with fx, fy and baseline "
+                      "> 0, got %s\n", camera_arg);
+      return 2;
+    }
+    dcam = ofdis_stereo_camera{v[0], v[1], v[2], v[3], v[4], v[5]};
+  }
   if (interp_arg) {
     char* end = nullptr;
     interp_t = strtof(interp_arg, &end);
@@ -916,7 +1008,7 @@ int main(int argc, char** argv) {
     }
   }
   // --interpolate and --tracks need the backward flows: the backward slots run whenever one of them is given
-  const bool two_way = bidir || interp_arg || tracks_path;
+  const bool two_way = bidir || interp_arg || tracks_path || lr_check;
   if (color_max_arg) {
     char* end = nullptr;
     color_max = strtof(color_max_arg, &end);
@@ -1003,6 +1095,8 @@ int main(int argc, char** argv) {
   vector<uint8_t> masks;
   vector<uint8_t> colors;  // --color: the color images of the slots
   vector<uint8_t> interp, interp_png;  // --interpolate: the frames at time T, one written as RGB
+  vector<float> ddisp, ddepth, dxyz;  // --lr-check / --speckle / --fill / --camera: the filtered outputs
+  vector<uint8_t> dstatus, dply;
   Image8 last;  // image2 of the previous batch's last pair
   // --tracks: the tracker's points and counts, the clip being tracked (-1 none) and its next frame, the totals of the
   // finished clips
@@ -1145,6 +1239,21 @@ int main(int argc, char** argv) {
                                      nop == 2 ? 0.01f : 0.0f, nop == 2 ? 0.5f : 1.0f, interp.data(), nullptr, w, h,
                                      OFDIS_MEM_HOST);
     }
+    size_t dcount[6] = {0, 0, 0, 0, 0, 0};  // statuses 0..4, filled
+    if (rc == OFDIS_OK && disp_on) {
+      const size_t np = (size_t)n * w * h;
+      ddisp.resize(np);
+      dstatus.resize(np);
+      ddepth.resize(camera_arg ? np : 0);
+      dxyz.resize(camera_arg ? 3 * np : 0);
+      rc = ofdis_disparity_fullres(ctx, 0, n, n, &dfilt, camera_arg ? &dcam : nullptr, ddisp.data(), dstatus.data(),
+                                   camera_arg ? ddepth.data() : nullptr, camera_arg ? dxyz.data() : nullptr, w, h,
+                                   OFDIS_MEM_HOST);
+      for (size_t i = 0; i < np && rc == OFDIS_OK; ++i) {
+        dcount[dstatus[i] < 5 ? dstatus[i] : 0] += 1;
+        dcount[5] += dstatus[i] != 0 && !std::isnan(ddisp[i]);
+      }
+    }
     // --tracks: runs of pairs that continue each other; a run that does not continue the previous pair begins a clip
     for (int k0 = 0, k1; k0 < n && tracks_file && rc == OFDIS_OK; k0 = k1) {
       for (k1 = k0 + 1; k1 < n && jobs[j0 + k1].a == jobs[j0 + k1 - 1].b;) ++k1;
@@ -1225,6 +1334,56 @@ int main(int argc, char** argv) {
       }
       save_png(im, w, h, nochannels, 8, with_suffix(jobs[j0 + k].out, "_interp", ".png").c_str());
     }
+    for (int k = 0; k < n && disp_on; ++k) {
+      const size_t o = (size_t)k * w * h;
+      if (kitti) {
+        vector<uint16_t> enc((size_t)w * h);
+        for (size_t i = 0; i < enc.size(); ++i) {
+          const float d = ddisp[o + i];  // NaN fails d >= 0 and is written as 0
+          enc[i] = d >= 0.0f ? (uint16_t)fminf(fmaxf(d * 256.0f, 1.0f), 65535.0f) : (uint16_t)0;
+        }
+        save_png(enc.data(), w, h, 1, 16, with_suffix(jobs[j0 + k].out, "_filtered").c_str());
+      } else {
+        ImageF f;  // SavePFMFile writes -value: the positive disparity goes in as -d, the sign of <stem><ext>
+        f.w = w; f.h = h; f.c = 1;
+        f.px.resize((size_t)w * h);
+        for (size_t i = 0; i < f.px.size(); ++i) f.px[i] = -ddisp[o + i];
+        SavePFMFile(f, with_suffix(jobs[j0 + k].out, "_filtered").c_str());
+      }
+      if (!camera_arg) continue;
+      ImageF z;
+      z.w = w; z.h = h; z.c = 1;
+      z.px.resize((size_t)w * h);
+      for (size_t i = 0; i < z.px.size(); ++i) z.px[i] = -ddepth[o + i];
+      SavePFMFile(z, with_suffix(jobs[j0 + k].out, "_depth", ".pfm").c_str());
+      // image1 of pair k: frame k of a clip, or the first image of the k-th pair
+      const uint8_t* im1 = frames.data() + (size_t)k * (seq ? hwc : 2 * hwc);
+      size_t npts = 0;
+      dply.clear();
+      for (size_t i = 0; i < (size_t)w * h; ++i) {
+        if (!std::isfinite(ddepth[o + i])) continue;
+        const float* q = dxyz.data() + (o + i) * 3;
+        const uint8_t* c = im1 + i * nochannels;
+        const uint8_t rgb[3] = {nochannels == 3 ? c[2] : c[0], c[nochannels == 3 ? 1 : 0], c[0]};  // the decoder's BGR
+        const uint8_t* qb = reinterpret_cast<const uint8_t*>(q);
+        dply.insert(dply.end(), qb, qb + 12);
+        dply.insert(dply.end(), rgb, rgb + 3);
+        ++npts;
+      }
+      const string ply = with_suffix(jobs[j0 + k].out, "", ".ply");
+      FILE* pf = fopen(ply.c_str(), "wb");
+      if (!pf) {
+        cout << "WriteFile: could not open file" << endl;
+        continue;
+      }
+      fprintf(pf, "ply\nformat binary_little_endian 1.0\nelement vertex %zu\nproperty float x\nproperty float y\n"
+                  "property float z\nproperty uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n", npts);
+      if (fwrite(dply.data(), 1, dply.size(), pf) != dply.size()) cout << "WriteFile: problem writing data" << endl;
+      fclose(pf);
+    }
+    if (verbosity > 0 && disp_on)
+      printf("DISP pairs %d valid %zu inconsistent %zu leaves %zu range %zu speckle %zu filled %zu\n", n, dcount[0],
+             dcount[1], dcount[2], dcount[3], dcount[4], dcount[5]);
     ImageF out;
     out.w = w; out.h = h; out.c = nop;
     for (int k = 0; k < n && !kitti; ++k) {

@@ -904,3 +904,104 @@ def track_points(frames: np.ndarray, fw: np.ndarray, bw: np.ndarray, params):
         lists.append(tracks)
     stats["alive"], stats["next_id"] = int(tracks.size), int(next_id)
     return lists, stats
+
+
+DISP_FILTER_FIELDS = ("lr_check", "alpha", "beta", "speckle_size", "speckle_diff", "fill")
+STEREO_CAMERA_FIELDS = ("fx", "fy", "cx", "cy", "baseline", "doffs")
+
+
+def _smaller(a: np.ndarray, b: np.ndarray) -> np.ndarray:
+    """(b < a) ? b : a elementwise: of two equal values (+0 and -0 among them) the first one."""
+    return np.where(b < a, b, a)
+
+
+def _fill_lines(v: np.ndarray, has: np.ndarray) -> np.ndarray:
+    """The fill rule along axis 1 of v (lines x positions) where `has` marks the values: a run without a value between
+    two values takes the smaller of them (the earlier one where equal), runs at either end the one value next to them;
+    a line without a value stays qNaN."""
+    n = v.shape[1]
+    pos = np.arange(n)[None, :]
+    left = np.maximum.accumulate(np.where(has, pos, -1), axis=1)
+    right = np.minimum.accumulate(np.where(has, pos, n)[:, ::-1], axis=1)[:, ::-1]
+    rows = np.arange(v.shape[0])[:, None]
+    vl = np.where(left >= 0, v[rows, np.clip(left, 0, n - 1)], _QNAN)
+    vr = np.where(right < n, v[rows, np.clip(right, 0, n - 1)], _QNAN)
+    out = np.where(left < 0, vr, np.where(right >= n, vl, _smaller(vl, vr)))
+    return np.where(has, v, out).astype(np.float32)
+
+
+def speckle_components(d: np.ndarray, valid: np.ndarray, diff: float):
+    """Connected components of the `valid` pixels of one frame, 4-neighbours joined when fabsf(d_p - d_q) <= diff in
+    float32 (scipy.sparse.csgraph.connected_components over the joined edges).  Returns (labels, sizes): a label per
+    pixel and each pixel's component size (0 where not valid)."""
+    from scipy.sparse import coo_matrix
+    from scipy.sparse.csgraph import connected_components
+
+    h, w = d.shape
+    f32 = np.float32
+    idx = np.arange(h * w).reshape(h, w)
+    edges = []
+    with np.errstate(invalid="ignore", over="ignore"):
+        for a, b, da, db in ((idx[:, :-1], idx[:, 1:], d[:, :-1], d[:, 1:]), (idx[:-1], idx[1:], d[:-1], d[1:])):
+            va = valid.reshape(-1)[a]
+            vb = valid.reshape(-1)[b]
+            ok = va & vb & (np.abs((da - db).astype(f32)) <= f32(diff))
+            edges.append((a[ok], b[ok]))
+    r = np.concatenate([e[0] for e in edges])
+    c = np.concatenate([e[1] for e in edges])
+    g = coo_matrix((np.ones(r.size, np.int8), (r, c)), shape=(h * w, h * w))
+    _, labels = connected_components(g, directed=False)
+    counts = np.bincount(labels[valid.reshape(-1)], minlength=labels.max() + 1 if labels.size else 0)
+    sizes = np.where(valid.reshape(-1), counts[labels], 0).reshape(h, w)
+    return labels.reshape(h, w), sizes
+
+
+def disparity_filter(F: np.ndarray, B: np.ndarray | None = None, swapped: bool = False, lr_check: int = 0,
+                     alpha: float = 0.0, beta: float = 1.0, speckle_size: int = 0, speckle_diff: float = 1.0,
+                     fill: int = 0, camera=None):
+    """One pair of ofdis_disparity_fullres, bit for bit, float32 without contraction.  F: slot a's full-resolution
+    stereo flow, (h, w) or (h, w, 1) float32, exactly what ofdis_get_flow_fullres returns; B: its partner slot's (read
+    only with lr_check); swapped: slot a is marked swapped.  camera: None or a mapping with STEREO_CAMERA_FIELDS.
+    Returns (disp, status, depth, xyz): (h, w) float32, (h, w) uint8, and with a camera (h, w) and (h, w, 3) float32
+    (else None).
+
+        d = -F (+F when swapped); status 3 where d is not in [0, 1e9], else with lr_check consistency_check's mask of F
+        against B, else 0.
+        speckle_size > 0: components of status-0 pixels (4-neighbours, fabsf(d_p - d_q) <= speckle_diff) of at most
+        speckle_size pixels get status 4.
+        fill: the row pass (_fill_lines on the rows, values where the status is 0), then the same along the columns.
+        disp: d where the status is 0, the filled value, else qNaN.
+        depth: Z = (fx * baseline) / (D + doffs) where D + doffs > 0, else qNaN; xyz: ((x - cx) Z / fx,
+        (y - cy) Z / fy, Z); every NaN of depth and xyz is qNaN."""
+    f32 = np.float32
+    Fa = np.asarray(F, f32)
+    Fa = Fa.reshape(Fa.shape[:2] + (-1,))
+    h, w = Fa.shape[:2]
+    d = Fa[..., 0] if swapped else -Fa[..., 0]
+    status = np.where((d >= 0) & (d <= f32(1e9)), 0, 3).astype(np.uint8)
+    if lr_check:
+        mask, _ = consistency_check(Fa, B, alpha, beta)
+        status = np.where(status == 0, mask, status).astype(np.uint8)
+    if speckle_size > 0:
+        _, sizes = speckle_components(d, status == 0, speckle_diff)
+        status[(status == 0) & (sizes <= speckle_size)] = 4
+    valid = status == 0
+    disp = np.where(valid, d, _QNAN).astype(f32)
+    if fill:
+        rows = _fill_lines(disp, valid)
+        full = valid.any(axis=1)
+        disp = _fill_lines(rows.T, np.broadcast_to(full[None, :], (w, h))).T.copy()
+    depth = xyz = None
+    if camera is not None:
+        cam = {k: f32(camera[k]) for k in STEREO_CAMERA_FIELDS}
+        fb = f32(cam["fx"] * cam["baseline"])
+        with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+            s = (disp + cam["doffs"]).astype(f32)
+            Z = np.where(s > 0, fb / np.where(s > 0, s, f32(1)), _QNAN).astype(f32)
+            Z = np.where(np.isnan(Z), _QNAN, Z).astype(f32)
+            X = ((np.arange(w, dtype=f32)[None, :] - cam["cx"]) * Z / cam["fx"]).astype(f32)
+            Y = ((np.arange(h, dtype=f32)[:, None] - cam["cy"]) * Z / cam["fy"]).astype(f32)
+        canon = lambda a: np.where(np.isnan(a), _QNAN, a).astype(f32)  # noqa: E731
+        depth = Z
+        xyz = np.stack([canon(X), canon(Y), Z], axis=-1)
+    return disp, status, depth, xyz

@@ -75,3 +75,36 @@ def synthetic_sequence(n_frames: int, h: int, w: int, channels: int = 1, seed: i
     canv, m = _canvas(h, w, channels, seed)
     u, v = synthetic_flow(h, w, amp, stereo)
     return np.ascontiguousarray(np.stack([_frame(canv, m, h, w, u, v, t) for t in range(n_frames)]))
+
+
+def layered_stereo(h: int, w: int, channels: int = 1, seed: int = 0, d_bg: int = 8, d_fg: int = 24,
+                   block=(0.3, 0.25, 0.7, 0.75)):
+    """A two-layer stereo pair with real occlusions: a textured background at the integer disparity d_bg and, in front
+    of it, a textured rectangle at the larger integer disparity d_fg covering the fractions `block` = (x0, y0, x1, y1)
+    of the left view.  The right view shows at column xr the foreground point xr + d_fg where that lies in the
+    rectangle, else the background point xr + d_bg (the library's convention I0(x) = I1(x - d(x)), stereo F = -d).
+    Both layers are crops of independent canvases (_canvas), sampled at integer positions, so every visible point has
+    exactly the same bytes in both views.  Returns (left_u8, right_u8, gt, occluded): gt the left view's positive
+    disparity (h, w) float32, occluded (h, w) bool where the left pixel's match in the right view is hidden by the
+    foreground or falls outside the frame."""
+    assert 0 <= d_bg < d_fg
+    bg, m = _canvas(h, w + d_fg, channels, seed)
+    fg, _ = _canvas(h, w + d_fg, channels, seed + 1)
+    X0, Y0, X1, Y1 = int(block[0] * w), int(block[1] * h), int(block[2] * w), int(block[3] * h)
+    y, x = np.mgrid[0:h, 0:w]
+    in_rows = (y >= Y0) & (y < Y1)
+    in_fg = in_rows & (x >= X0) & (x < X1)
+    left = np.where(in_fg[..., None], fg[m + y, m + x], bg[m + y, m + x])
+    xf, xb = x + d_fg, x + d_bg  # the left-view columns that the right view's column x shows
+    right_fg = in_rows & (xf >= X0) & (xf < X1)
+    right = np.where(right_fg[..., None], fg[m + y, m + xf], bg[m + y, m + xb])
+    gt = np.where(in_fg, d_fg, d_bg).astype(np.float32)
+    xr = x - gt.astype(np.int64)
+    hidden = ~in_fg & in_rows & (xr + d_fg >= X0) & (xr + d_fg < X1)
+    occluded = (xr < 0) | hidden
+
+    def q(img):
+        img = np.clip(np.rint(img), 0, 255).astype(np.uint8)
+        return np.ascontiguousarray(img[..., 0] if channels == 1 else img)
+
+    return q(left), q(right), gt, occluded

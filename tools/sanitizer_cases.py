@@ -4,8 +4,9 @@ the smoke configuration (P=8 gray flow) with both exact SOR kernels (sor_lane_ke
 sor_wave_kernel: single CTA), a forward-backward case, a P=12 RGB and a P=12 stereo case (window-staged patch
 kernel, stereo SOR), a 70-row level as three bands of the lane kernel and forced into a cluster of bands of the
 wave kernel with 1 and 2 rows per thread (st.async halo exchange), and the 8-bit frame path (pyramid and
-upsampling kernels), and a frame interpolation and a point tracking (advance, seed, block scan, scatter) checked
-against their restatements.  Results are checked against the oracle so that a clean log means a correct run."""
+upsampling kernels), and a frame interpolation, a point tracking (advance, seed, block scan, scatter) and a filtered
+disparity (union-find speckles, fill, depth and xyz) checked against their restatements.  Results are checked against
+the oracle so that a clean log means a correct run."""
 import os
 import sys
 
@@ -79,6 +80,28 @@ ctx.close()
 exp, est = preprocess.track_points(clip, full[:n], full[n:], tp)
 ok = st == est and all(np.array_equal(g.view(np.uint8), e.view(np.uint8)) for g, e in zip(lists, exp))
 print("%-22s %s" % ("track_rgb", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# filtered disparities on a two-way stereo clip with a non-divisible size (classify, tile and border union-find,
+# count, row and column fill, outputs), every stage on and every output asked for
+prm = params.from_cli_numbers("3 1 8 8 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=1, nop=1)
+clip = synth.synthetic_sequence(n + 1, h, w, 1, seed=5, amp=3.0, stereo=True)
+ctx = api.Context(prm, 96, 64, prm.p_samp_s, 2 * n)
+ctx.upload_sequence_bidir_u8(0, n, clip, w, h)
+ctx.run(2 * n)
+full = np.empty((2 * n, h, w, 1), np.float32)
+ctx.get_flow_fullres(0, 2 * n, full, w, h)
+ctx.sync()
+filt = dict(lr_check=1, alpha=0.0, beta=1.0, speckle_size=20, speckle_diff=0.05, fill=1)
+cam = dict(fx=100.0, fy=100.0, cx=45.0, cy=30.0, baseline=0.5, doffs=0.0)
+got = ctx.disparity_fullres(n, 2 * n, 0, w, h, camera=cam, outputs=("disp", "status", "depth", "xyz"), **filt)
+ctx.close()
+ok = True
+for k in range(n):
+    exp = preprocess.disparity_filter(full[n + k], full[k], True, camera=cam, **filt)
+    ok &= all(np.array_equal(np.asarray(g[k]).view(np.uint8), np.asarray(e).view(np.uint8))
+              for g, e in zip((got["disp"], got["status"], got["depth"], got["xyz"]), exp))
+print("%-22s %s" % ("disparity_stereo", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
