@@ -399,6 +399,90 @@ int ofdis_disparity_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
                             const ofdis_stereo_camera* cam, float* disp, unsigned char* status, float* depth,
                             float* xyz, int width_org, int height_org, int memkind);
 
+/* Global camera motion from dense flows (extension, flow contexts only): a RANSAC fit of one similarity, affine map
+ * or homography per pair, its least-squares refits on the inliers, and from the model per pixel the residual flow, a
+ * moving-pixel mask and I1 registered onto I0.  preprocess.global_motion restates it bit for bit.  float32 where
+ * marked, float64 in the solver, everything without contraction and with IEEE division.  W = width_org,
+ * H = height_org, s = step, qNaN = the quiet NaN 0x7fc00000.  For every pair k < f1-f0, slot a = f0+k:
+ *   1. Correspondences.  The cells (i, j) are ceil(W/s) x ceil(H/s) in row-major order (j outer), cell (i, j) has the
+ *      pixel cx = min(i*s + s/2, W-1), cy = min(j*s + s/2, H-1) (the seed grid of ofdis_track_begin).  F = (u, v) is
+ *      slot a's full-resolution flow at (cx, cy), exactly what ofdis_get_flow_fullres returns.  A cell is valid when
+ *      |u| <= 1e9 and |v| <= 1e9 (NaN fails), (xs, ys) = ((float)cx + u, (float)cy + v) lies in [0, W-1] x [0, H-1],
+ *      and, with fb_check, the mask of ofdis_consistency_fullres(alpha, beta) of slot a against slot b0+k is 0 there.
+ *      The valid cells, in cell order, are the m correspondences (x, y, p, q) in float32 normalized coordinates:
+ *      c_x = 0.5f * (float)(W-1), c_y = 0.5f * (float)(H-1), sigma = 2.0f / (float)max(W, H), x = ((float)cx - c_x)
+ *      * sigma, y = ((float)cy - c_y) * sigma, p = (xs - c_x) * sigma, q = (ys - c_y) * sigma.  m < n_min: status 1.
+ *   2. Hypotheses h = 0 .. hypotheses-1.  Draw d < n_min takes z = mix(seed + (uint64)(8h + d + 1) * G) with
+ *      G = 0x9E3779B97F4A7C15 and SplitMix64's finalizer mix(z): z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9,
+ *      z = (z ^ (z >> 27)) * 0x94D049BB133111EB, z ^ (z >> 31) (all mod 2^64; this is the (8h+d+1)-th output of the
+ *      SplitMix64 generator seeded with `seed`), and the correspondence index (uint32)(((z >> 32) * m) >> 32).  The
+ *      draws depend on h, d, m and seed only, so a pair's whole result depends only on its own flows and the params.
+ *      The draws give 2 n_min rows, point by point, row x then row y, of (double) of the float32 values:
+ *        similarity (k = 4):  [x, -y, 1, 0 | p], [y, x, 0, 1 | q];           H^ = [a, -b, tx; b, a, ty; 0, 0, 1]
+ *        affine     (k = 6):  [x, y, 1, 0, 0, 0 | p], [0, 0, 0, x, y, 1 | q]; H^ = [h0, h1, h2; h3, h4, h5; 0, 0, 1]
+ *        homography (k = 8):  [x, y, 1, 0, 0, 0, -(x*p), -(y*p) | p], [0, 0, 0, x, y, 1, -(x*q), -(y*q) | q];
+ *                             H^ = [h0, h1, h2; h3, h4, h5; h6, h7, 1]
+ *      solved by THE elimination of this call: for column j: the pivot row is the first i >= j of the largest
+ *      |a_ij|; a pivot that is not > 0 in magnitude fails; swap rows; for each i > j: f = a_ij / a_jj, a_ic = a_ic - f
+ *      * a_jc for c > j, b_i = b_i - f * b_j.  Back substitution for i = k-1 .. 0: x_i = b_i, x_i = x_i - a_ic * x_c for
+ *      c = i+1 .. k-1, x_i = x_i / a_ii.  A failed pivot or a non-finite x_i makes the hypothesis unsolvable (a repeated
+ *      index gives a zero pivot).
+ *   3. Scoring.  g0..g8 = H^ rounded to float32, t = threshold * sigma (float32).  Correspondence (x, y, p, q) is an
+ *      inlier iff W' > 0 and ex*ex + ey*ey <= (t*W')*(t*W') with X' = (g0*x + g1*y) + g2, Y' = (g3*x + g4*y) + g5,
+ *      W' = (g6*x + g7*y) + g8, ex = X' - p*W', ey = Y' - q*W' (reprojection error <= t, without a division).  The best
+ *      solvable hypothesis has the most inliers, the lowest h on a tie (the largest (count << 32) | (0xFFFFFFFF - h)).
+ *      No solvable hypothesis: status 2.
+ *   4. Refits, rounds 1 .. refine: the inliers of the current model (the test above); fewer than n_min: stop.  Normal
+ *      equations from each inlier's two rows r1 | b1, r2 | b2: N_ij = (r1_i*r1_j) + (r2_i*r2_j) for i <= j, the
+ *      right-hand side (r1_i*b1) + (r2_i*b2), other correspondences +0.0.  Each sum runs over chunks of 32 consecutive
+ *      correspondences, each chunk from +0.0 in order, then a pairwise tree over the chunk sums padded with +0.0 to a
+ *      power of two (level by level, v_i = v_2i + v_2i+1).  N is mirrored and solved by the elimination; a failure
+ *      stops and keeps the model, else the solution replaces it.
+ *   5. model (row-major 3 x 3, float64) = T^-1 H^ T in pixel coordinates, mapping an I0 pixel to its I1 position:
+ *      with h = H^, S = (double)sigma, Cx = (double)c_x, Cy = (double)c_y, per row r: A_r0 = h_r0*S, A_r1 = h_r1*S,
+ *      A_r2 = h_r2 - (A_r0*Cx + A_r1*Cy); M_0c = A_0c/S + Cx*A_2c, M_1c = A_1c/S + Cy*A_2c, M_2c = A_2c; a homography
+ *      is then divided entry by entry by the M_22 of before.  Every NaN of the model is the float64 qNaN
+ *      0x7ff8000000000000; status != 0: nine of them.
+ *   6. Per pixel (X, Y) of the frame, m0..m8 = model rounded to float32: mx = (m0*X + m1*Y) + m2, my = (m3*X + m4*Y)
+ *      + m5, w = (m6*X + m7*Y) + m8, the model flow (mx/w - X, my/w - Y).  residual = F - the model flow, per
+ *      component, every NaN written as qNaN.  mask: 2 where F is unknown, (X + u, Y + v) leaves the frame or, with
+ *      fb_check, the consistency mask is not 0; else 0 where rx*rx + ry*ry <= threshold*threshold (float32), else 1 (moves independently).
+ *      registered: with w > 0 and (mx/w, my/w) in the frame, I1 there by the bilinear byte rule and rounding of
+ *      ofdis_interpolate_fullres, else 0.  A pair of status != 0 writes residual qNaN, mask 2 and registered 0.
+ * stats per pair: status, n_corr = m, best_hypothesis (-1 unless status 0), ransac_inliers (its count), refits (the
+ * refits that replaced the model), n_inliers (the final model's count).  model = [n][9] doubles and stats = [n] are
+ * host memory.  mask [n][H][W] bytes, residual [n][H][W][2] float32 and registered [n][H][W][noc] bytes are optional
+ * (NULL skips them) and in memkind; registered needs i1: the 8-bit frame I1 of pair k at i1 + k*frame_stride, the
+ * convention of ofdis_interpolate_fullres (host frames go through the staging buffer, host outputs through the
+ * full-resolution scratch).  OFDIS_ERR_ARG: a stereo context, slots outside the context (b0 only with fb_check), a NULL
+ * p or one out of range (model 1..3, step >= 1, fb_check 0|1, alpha and beta finite and >= 0, hypotheses 1..65536,
+ * threshold finite and > 0, refine 0..16), a NULL model or stats, registered without i1, frame_stride below one frame,
+ * a device residual not 4-byte aligned, or more than 2^24 cells per pair; frame sizes as ofdis_get_flow_fullres checks
+ * them.  The workspace -- per cell and pair 28 bytes (the correspondence, its flag, the refit's chunk sums), per
+ * hypothesis and pair 112 (its float64 parameters and float32 H^) and 128 per pair -- is allocated on the first call,
+ * grows, never shrinks and is freed by ofdis_destroy.  Enqueued on the context's stream as 5 kernels, plus one when a
+ * per-pixel output is asked for, whatever the number of pairs; the call synchronises the stream once, at the end, for
+ * model and stats.  Not part of ofdis_run's graph; the flows are not changed. */
+enum { OFDIS_MOTION_SIMILARITY = 1, OFDIS_MOTION_AFFINE = 2, OFDIS_MOTION_HOMOGRAPHY = 3 };
+typedef struct ofdis_motion_params {
+  int model;                 /* OFDIS_MOTION_*: n_min = 2, 3, 4 points, k = 4, 6, 8 unknowns */
+  int step;                  /* correspondence grid step s >= 1 */
+  int fb_check;              /* 0 | 1: only correspondences whose consistency mask against slot b0+k is 0 */
+  float alpha, beta;         /* the rule of ofdis_consistency_fullres; finite, >= 0 */
+  int hypotheses;            /* 1 .. 65536 */
+  float threshold;           /* inlier reprojection error in pixels; finite, > 0 */
+  int refine;                /* 0 .. 16 least-squares refits on the inliers */
+  unsigned long long seed;
+} ofdis_motion_params;
+typedef struct ofdis_motion_stats {
+  int status;                /* 0 fitted, 1 fewer than n_min correspondences, 2 no solvable hypothesis */
+  int n_corr, best_hypothesis, ransac_inliers, refits, n_inliers;
+} ofdis_motion_stats;
+int ofdis_global_motion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_motion_params* p,
+                                const unsigned char* i1, size_t frame_stride, double* model,
+                                ofdis_motion_stats* stats, unsigned char* mask, float* residual,
+                                unsigned char* registered, int width_org, int height_org, int memkind);
+
 /* Dense point trajectories (extension): the tracker of Sundaram, Brox and Keutzer ("Dense point trajectories by
  * GPU-accelerated large displacement optical flow", ECCV 2010) through consecutive pairs of bidirectional flows.
  * The context owns one tracker: the list of live tracks (sorted by id), the next id and the counters.  It persists

@@ -14,8 +14,8 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import (DISP_FILTER_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE,
-                         TRACK_STATS_FIELDS)
+from .preprocess import (DISP_FILTER_FIELDS, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, STEREO_CAMERA_FIELDS,
+                         TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, motion_params)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("OFDIS_LIB") or os.path.join(_HERE, "lib", "libofdis_b200.so")  # OFDIS_LIB: experiments only
@@ -38,6 +38,7 @@ EXPORTS = [
     "ofdis_consistency_fullres", "ofdis_flow_error_fullres", "ofdis_debug_sor_plan",
     "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres", "ofdis_interpolate_fullres",
     "ofdis_track_begin", "ofdis_track_advance", "ofdis_track_stats_get", "ofdis_disparity_fullres",
+    "ofdis_global_motion_fullres",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -81,6 +82,22 @@ class StereoCamera(ctypes.Structure):
 
 
 assert tuple(k for k, _ in DispFilter._fields_) == DISP_FILTER_FIELDS
+
+
+class MotionParams(ctypes.Structure):
+    """ofdis_motion_params (include/ofdis_b200.h)."""
+    _fields_ = [("model", ctypes.c_int), ("step", ctypes.c_int), ("fb_check", ctypes.c_int), ("alpha", ctypes.c_float),
+                ("beta", ctypes.c_float), ("hypotheses", ctypes.c_int), ("threshold", ctypes.c_float),
+                ("refine", ctypes.c_int), ("seed", ctypes.c_ulonglong)]
+
+
+class MotionStats(ctypes.Structure):
+    """ofdis_motion_stats (include/ofdis_b200.h); MOTION_STATS_DTYPE is the same record as numpy sees it."""
+    _fields_ = [(k, ctypes.c_int) for k in MOTION_STATS_DTYPE.names]
+
+
+assert tuple(k for k, _ in MotionParams._fields_) == MOTION_PARAM_FIELDS
+assert ctypes.sizeof(MotionStats) == MOTION_STATS_DTYPE.itemsize
 
 
 class OfdisError(RuntimeError):
@@ -144,6 +161,8 @@ def lib():
             [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
         L.ofdis_disparity_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
             [ctypes.POINTER(DispFilter), ctypes.POINTER(StereoCamera)] + [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3
+        L.ofdis_global_motion_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
+            [ctypes.POINTER(MotionParams), ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 5 + [ctypes.c_int] * 3
         L.ofdis_track_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackStats)]
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -373,6 +392,45 @@ class Context:
         self._ck(lib().ofdis_disparity_fullres(self._h, f0, f1, b0, ctypes.byref(filt), cam, *ptrs, width_org,
                                                height_org, memkind))
         return {k: out.get(k) for k in outputs}
+
+    def global_motion_fullres(self, f0, f1, params, *, width_org, height_org, b0=None, i1=None, frame_stride=None,
+                              mask=None, residual=None, registered=None, memkind=MEM_HOST):
+        """The camera motion of the last run's slots [f0, f1): one RANSAC model per pair, refitted on its inliers, and
+        optionally the per-pixel residual flows, moving-pixel masks and registered I1 (ofdis_global_motion_fullres;
+        preprocess.global_motion restates it).  params: a mapping with preprocess.MOTION_PARAM_FIELDS (the model as a
+        number or a name of preprocess.MOTION_MODELS) or a MotionParams; b0: the partner slots of fb_check.  Returns
+        (models, stats): (f1-f0, 3, 3) float64 and (f1-f0,) of MOTION_STATS_DTYPE, always on the host; the call
+        synchronises the stream.  Host: mask (f1-f0, height_org, width_org) uint8, residual (..., 2) float32 and
+        registered (f1-f0, height_org, width_org[, noc]) uint8 are writeable C-contiguous numpy arrays to fill (None
+        skips them); i1 the pairs' I1, a uint8 (f1-f0, height_org, width_org[, noc]) array whose frames are
+        C-contiguous -- clip[1:] or pairs[:, 1] qualify.  With memkind=MEM_DEVICE they are device addresses the
+        caller owns and frame_stride the bytes between the frames of i1 (default one frame)."""
+        if not isinstance(params, MotionParams):
+            p = motion_params(params)
+            params = MotionParams(*[p[k] for k in MOTION_PARAM_FIELDS])
+        n = max(f1 - f0, 0)
+        noc = self.prm.noc
+        frame = (height_org, width_org) + ((noc,) if noc > 1 else ())
+        if memkind == MEM_HOST:
+            for name, arr, dt, shapes in (("mask", mask, np.uint8, ((n, height_org, width_org),)),
+                                          ("residual", residual, np.float32, ((n, height_org, width_org, 2),)),
+                                          ("registered", registered, np.uint8,
+                                           ((n,) + frame, (n, height_org, width_org, noc)))):
+                if arr is not None and not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape in shapes
+                                            and arr.flags["C_CONTIGUOUS"] and arr.flags["WRITEABLE"]):
+                    raise ValueError("global_motion_fullres: %s must be a writeable C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shapes[0]))
+            if i1 is not None:
+                frame_stride = self._frames_u8("global_motion_fullres: i1", i1, n, width_org, height_org)
+                i1 = i1.ctypes.data
+        if frame_stride is None:
+            frame_stride = height_org * width_org * noc
+        models = np.empty((n, 3, 3), np.float64)
+        stats = np.zeros(n, MOTION_STATS_DTYPE)
+        self._ck(lib().ofdis_global_motion_fullres(self._h, f0, f1, -1 if b0 is None else b0, ctypes.byref(params),
+                                                   _ptr(i1), frame_stride, _ptr(models), _ptr(stats), _ptr(mask),
+                                                   _ptr(residual), _ptr(registered), width_org, height_org, memkind))
+        return models, stats
 
     def flow_error_fullres(self, f0, f1, gt, width_org, height_org, classes=None, nclasses=None, with_err=False,
                            memkind=MEM_HOST, err=None):

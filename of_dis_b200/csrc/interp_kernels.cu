@@ -23,23 +23,6 @@ namespace {
 
 constexpr unsigned long long kNoSource = ~0ull;
 
-// bil(I, xs, ys) of an 8-bit frame [h][w][NOC] at an in-frame position: the bilinear rule of consistency_kernel
-// (corners floor and min(floor + 1, size - 1), horizontal pass first) on the (float) byte values
-template <int NOC>
-__device__ __forceinline__ void bil_u8(const unsigned char* I, int w, int h, float xs, float ys, float* out) {
-  const int x0 = (int)floorf(xs), y0 = (int)floorf(ys);
-  const int x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
-  const float fx = xs - (float)x0, fy = ys - (float)y0, gx = 1.0f - fx, gy = 1.0f - fy;
-  const unsigned char* p00 = I + ((size_t)y0 * w + x0) * NOC;
-  const unsigned char* p10 = I + ((size_t)y0 * w + x1) * NOC;
-  const unsigned char* p01 = I + ((size_t)y1 * w + x0) * NOC;
-  const unsigned char* p11 = I + ((size_t)y1 * w + x1) * NOC;
-  for (int c = 0; c < NOC; ++c) {
-    const float r0 = (float)p00[c] * gx + (float)p10[c] * fx, r1 = (float)p01[c] * gx + (float)p11[c] * fx;
-    out[c] = r0 * gy + r1 * fy;
-  }
-}
-
 __device__ __forceinline__ bool in_frame(float x, float y, int w, int h) {
   return x >= 0.f && x <= (float)(w - 1) && y >= 0.f && y <= (float)(h - 1);
 }

@@ -87,7 +87,12 @@ struct ofdis_ctx {
   // lazily allocated workspace of ofdis_disparity_fullres (DispWork for max_frames pairs of width x height pixels);
   // never touched by ofdis_run
   void* d_disp = nullptr;
-  std::vector<float*> d_flow;    // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
+  // lazily allocated workspace of ofdis_global_motion_fullres (MotionWork for max_frames pairs of motion_cells cells
+  // and motion_hyps hypotheses); grows, never shrinks; never touched by ofdis_run
+  void* d_motion = nullptr;
+  size_t motion_cells = 0, motion_hyps = 0;
+  MotionWork motion{};
+  std::vector<float*> d_flow;   // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
   float* d_planes = nullptr;
@@ -456,6 +461,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_interp);
   cudaFree(ctx->d_track);
   cudaFree(ctx->d_disp);
+  cudaFree(ctx->d_motion);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -1153,6 +1159,124 @@ int ofdis_disparity_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
 }
 
 static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// The workspace of ofdis_global_motion_fullres for max_frames pairs of at least `cells` cells and `hyps` hypotheses:
+// per cell the correspondence (16 bytes), its flag (1) and the refit's chunk sums (44 doubles per 32 cells, 11); per
+// hypothesis its float64 parameters (64) and MotionHyp (48); per pair MotionOut, the key and the count.  Grows, never
+// shrinks.
+static int ensure_motion(ofdis_ctx* ctx, size_t cells, size_t hyps) {
+  cells = (cells + 31) / 32 * 32;
+  const size_t n = (size_t)ctx->max_frames;
+  if (ctx->d_motion && cells <= ctx->motion_cells && hyps <= ctx->motion_hyps) return OFDIS_OK;
+  cells = std::max(cells, ctx->motion_cells);
+  hyps = std::max(hyps, ctx->motion_hyps);
+  const size_t b_corr = n * cells * sizeof(float4), b_chunk = n * (cells / 32) * MOTION_NE * sizeof(double);
+  const size_t b_hp = n * hyps * 8 * sizeof(double), b_hg = n * hyps * sizeof(MotionHyp);
+  const size_t b_out = align16(n * sizeof(MotionOut)), b_key = align16(n * 8), b_m = align16(n * 4);
+  CK(cudaStreamSynchronize(ctx->stream));
+  cudaFree(ctx->d_motion);
+  ctx->d_motion = nullptr;
+  ctx->motion_cells = ctx->motion_hyps = 0;
+  if (cudaMalloc(&ctx->d_motion, b_corr + b_chunk + b_hp + b_hg + b_out + b_key + b_m + n * cells) != cudaSuccess) {
+    ctx->d_motion = nullptr;
+    return fail(ctx, OFDIS_ERR_NOMEM, "global_motion_fullres workspace");
+  }
+  char* b = static_cast<char*>(ctx->d_motion);
+  MotionWork& ws = ctx->motion;
+  ws.corr = reinterpret_cast<float4*>(b);
+  b += b_corr;
+  ws.chunk = reinterpret_cast<double*>(b);
+  b += b_chunk;
+  ws.hp = reinterpret_cast<double*>(b);
+  b += b_hp;
+  ws.hg = reinterpret_cast<MotionHyp*>(b);
+  b += b_hg;
+  ws.out = reinterpret_cast<MotionOut*>(b);
+  b += b_out;
+  ws.key = reinterpret_cast<unsigned long long*>(b);
+  b += b_key;
+  ws.m = reinterpret_cast<int*>(b);
+  b += b_m;
+  ws.flag = reinterpret_cast<unsigned char*>(b);
+  ctx->motion_cells = cells;
+  ctx->motion_hyps = hyps;
+  return OFDIS_OK;
+}
+
+int ofdis_global_motion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_motion_params* p,
+                                const unsigned char* i1, size_t frame_stride, double* model,
+                                ofdis_motion_stats* stats, unsigned char* mask, float* residual,
+                                unsigned char* registered, int width_org, int height_org, int memkind) {
+  static_assert(sizeof(ofdis_motion_stats) == 24, "ofdis_motion_stats: 24 bytes, as api.MotionStats");
+  if (!ctx) return OFDIS_ERR_ARG;
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  if (ctx->nop != 2 || f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !p ||
+      (p->fb_check && (b0 < 0 || b0 > ctx->max_frames - (f1 - f0))) ||
+      p->model < OFDIS_MOTION_SIMILARITY || p->model > OFDIS_MOTION_HOMOGRAPHY || p->step < 1 ||
+      (p->fb_check != 0 && p->fb_check != 1) || !finite_ge0(p->alpha) || !finite_ge0(p->beta) ||
+      p->hypotheses < 1 || p->hypotheses > 65536 || !finite_gt0(p->threshold) || p->refine < 0 || p->refine > 16 ||
+      !model || !stats || (registered && !i1) || (dev && reinterpret_cast<uintptr_t>(residual) % sizeof(float)))
+    return fail(ctx, OFDIS_ERR_ARG, "global_motion_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  const size_t pix = (size_t)width_org * height_org, noc = (size_t)ctx->prm.noc, hwc = pix * noc;
+  if (registered && frame_stride < hwc) return fail(ctx, OFDIS_ERR_ARG, "global_motion_fullres: frame_stride below one frame");
+  const int s = p->step, ncx = (width_org - 1) / s + 1, ncy = (height_org - 1) / s + 1;
+  if ((long long)ncx * ncy > (1ll << 24)) return fail(ctx, OFDIS_ERR_ARG, "global_motion_fullres: more than 2^24 cells");
+  NvtxRange nvtx("global_motion", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0, D = ctx->dirs;
+  rc = ensure_motion(ctx, (size_t)ncx * ncy, (size_t)p->hypotheses);
+  if (rc) return rc;
+  MotionGeom mg{};
+  mg.w = width_org, mg.h = height_org, mg.s = s, mg.ncx = ncx, mg.cells = ncx * ncy, mg.model = p->model;
+  mg.n_min = p->model + 1, mg.nh = p->hypotheses, mg.fb_check = p->fb_check, mg.refine = p->refine;
+  mg.crop_x = cx, mg.crop_y = cy, mg.noc = ctx->prm.noc, mg.alpha = p->alpha, mg.beta = p->beta;
+  mg.cx = 0.5f * (float)(width_org - 1);
+  mg.cy = 0.5f * (float)(height_org - 1);
+  mg.sigma = 2.0f / (float)std::max(width_org, height_org);
+  mg.t = p->threshold * mg.sigma;
+  mg.thr = p->threshold;
+  mg.seed = p->seed;
+  mg.cell_cap = ctx->motion_cells, mg.chunk_cap = ctx->motion_cells / 32, mg.hyp_cap = ctx->motion_hyps;
+  MotionOutputs o{mask, residual, registered, i1, frame_stride};
+  if (!dev && (mask || residual || registered)) {
+    // the full-resolution scratch: residual floats, then the mask and registered bytes (those asked for); sized for
+    // max_frames, and at least what ofdis_get_flow_fullres asks for.  I1 goes through the staging buffer.
+    rc = ensure_full(ctx, std::max(pix * ctx->nop, 2 * pix + (pix * (1 + noc) + 3) / 4) * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    float* q = ctx->d_full;
+    if (residual) o.residual = q, q += 2 * pix * n;
+    unsigned char* qb = reinterpret_cast<unsigned char*>(q);
+    if (mask) o.mask = qb, qb += pix * n;
+    if (registered) {
+      o.registered = qb;
+      rc = ensure_stage(ctx, hwc * (size_t)ctx->max_frames);
+      if (rc) return rc;
+      CK(cudaMemcpy2DAsync(ctx->d_stage, hwc, i1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+      o.i1 = static_cast<const unsigned char*>(ctx->d_stage);
+      o.stride = hwc;
+    }
+  }
+  const int k = launch_global_motion(stepped(ctx->lev[0], D), f0 * D, (p->fb_check ? b0 : f0) * D, n, mg, ctx->motion,
+                                     o, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "motion kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  if (!dev) {
+    if (residual) CK(cudaMemcpyAsync(residual, o.residual, sizeof(float) * 2 * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (mask) CK(cudaMemcpyAsync(mask, o.mask, pix * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (registered) CK(cudaMemcpyAsync(registered, o.registered, hwc * n, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  std::vector<MotionOut> res(n);
+  CK(cudaMemcpyAsync(res.data(), ctx->motion.out, sizeof(MotionOut) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (int q = 0; q < n; ++q) {
+    std::memcpy(model + 9 * (size_t)q, res[q].M, sizeof(res[q].M));
+    stats[q] = res[q].st;
+  }
+  return OFDIS_OK;
+}
 
 // The tracker's workspace for geometry t: the state, two track lists, the flags, the occupancy, the scan blocks'
 // sums, the counts of max_frames pairs, then the host-output records of max_frames pairs.  Grows, never shrinks.

@@ -615,6 +615,17 @@ int main(int argc, char** argv) {
 // uchar red, green, blue from image1 (gray replicated).  With verbosity > 0 every batch prints a line
 // `DISP pairs N valid V inconsistent I leaves L range R speckle S filled F` (the status counts, and the pixels of
 // another status that got a value).  Every other output keeps its bytes.
+//
+// --global-motion MODEL PATH (flow binaries only; MODEL similarity, affine or homography): the camera motion of every
+// pair (ofdis_global_motion_fullres) with step 8, 1024 hypotheses, a 1 px threshold, 3 refits and seed 0; with
+// --bidirectional only the correspondences whose consistency mask of --bidirectional (alpha 0.01, beta 0.5) is 0.
+// PATH gets one line per pair, `stem m00 m01 m02 m10 m11 m12 m20 m21 m22 status n_corr n_inliers`, stem the output
+// path without its extension and the model (mapping an image1 pixel to its image2 position) printed with %.17g
+// (which round-trips float64).  Every pair also gets <stem>_residual<ext>, the flow minus the model's flow, in the
+// format of <stem><ext> (KITTI's 16-bit PNG with --kitti); <stem>_moving.pgm, 0 where a pixel moves with the camera,
+// 255 where it moves on its own and 128 where its flow is unknown, leaves the frame or (with --bidirectional) is
+// inconsistent, the code of _occ.pgm; and <stem>_registered.png, image2 sampled at the model's position of every
+// pixel of image1 (0 outside image2).  Every other output keeps its bytes.  Not with --warm-start.
 
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
@@ -828,6 +839,7 @@ int main(int argc, char** argv) {
             "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
             "       [--color [--color-max M]] [--interpolate T] [--tracks PATH]\n"
             "       [--lr-check] [--speckle N R] [--fill] [--camera fx,fy,cx,cy,baseline,doffs]\n"
+            "       [--global-motion similarity|affine|homography PATH]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -849,7 +861,9 @@ int main(int argc, char** argv) {
             "  --lr-check, --speckle N R, --fill, --camera ...: stereo only; also write <stem>_filtered<ext>, the\n"
             "  disparity without the pixels that fail the left-right check and the speckles of at most N pixels (R px),\n"
             "  holes filled with the background disparity, and with --camera <stem>_depth.pfm and <stem>.ply;\n"
-            "  not with --warm-start\n",
+            "  not with --warm-start\n"
+            "  --global-motion MODEL PATH: flow only; the camera motion of every pair, one line per pair in PATH, and\n"
+            "  <stem>_residual<ext>, <stem>_moving.pgm and <stem>_registered.png; not with --warm-start\n",
             argv[0]);
     return 2;
   }
@@ -864,6 +878,7 @@ int main(int argc, char** argv) {
   bool lr_check = false, disp_fill = false;  // --lr-check, --fill
   const char* speckle_arg[2] = {nullptr, nullptr};  // --speckle N R
   const char* camera_arg = nullptr;  // --camera fx,fy,cx,cy,baseline,doffs
+  const char* gm_arg[2] = {nullptr, nullptr};  // --global-motion MODEL PATH
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -923,6 +938,14 @@ int main(int argc, char** argv) {
       }
       camera_arg = argv[first_num + 1];
       first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--global-motion")) {
+      if (argc < first_num + 3 || gm_arg[0]) {
+        fprintf(stderr, "error: --global-motion takes a model (similarity, affine or homography) and an output path\n");
+        return 2;
+      }
+      gm_arg[0] = argv[first_num + 1];
+      gm_arg[1] = argv[first_num + 2];
+      first_num += 3;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
         fprintf(stderr, "error: --gt takes one ground-truth list file\n");
@@ -959,6 +982,25 @@ int main(int argc, char** argv) {
   if (warm && disp_on) {
     fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --lr-check, --speckle, --fill or --camera\n");
     return 2;
+  }
+  int gm_model = 0;  // --global-motion: OFDIS_MOTION_*
+  if (gm_arg[0]) {
+    if (SELECTMODE != 1) {
+      fprintf(stderr, "error: --global-motion fits the camera motion of flows; the stereo binaries take no "
+                      "--global-motion\n");
+      return 2;
+    }
+    if (warm) {
+      fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --global-motion\n");
+      return 2;
+    }
+    gm_model = !strcmp(gm_arg[0], "similarity") ? OFDIS_MOTION_SIMILARITY
+               : !strcmp(gm_arg[0], "affine")   ? OFDIS_MOTION_AFFINE
+               : !strcmp(gm_arg[0], "homography") ? OFDIS_MOTION_HOMOGRAPHY : 0;
+    if (!gm_model) {
+      fprintf(stderr, "error: --global-motion takes the model similarity, affine or homography, got %s\n", gm_arg[0]);
+      return 2;
+    }
   }
   ofdis_disp_filter dfilt;
   memset(&dfilt, 0, sizeof(dfilt));
@@ -1080,6 +1122,15 @@ int main(int argc, char** argv) {
     }
     fprintf(tracks_file, "# clip frame id x y\n");
   }
+  FILE* gm_file = nullptr;
+  if (gm_model) {
+    gm_file = fopen(gm_arg[1], "w");
+    if (!gm_file) {
+      fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
+      if (tracks_file) fclose(tracks_file);
+      return 1;
+    }
+  }
   const int nclasses = bidir ? 3 : 1;  // with --bidirectional the forward consistency mask's classes
   vector<ofdis_error_stats> eval_total(nclasses + 1), eval_pairs;  // [0]: all pixels, [1 + c]: class c
   memset(eval_total.data(), 0, sizeof(ofdis_error_stats) * eval_total.size());
@@ -1097,6 +1148,10 @@ int main(int argc, char** argv) {
   vector<uint8_t> interp, interp_png;  // --interpolate: the frames at time T, one written as RGB
   vector<float> ddisp, ddepth, dxyz;  // --lr-check / --speckle / --fill / --camera: the filtered outputs
   vector<uint8_t> dstatus, dply;
+  vector<double> gm_models;  // --global-motion: the models, stats and per-pixel outputs of the batch
+  vector<ofdis_motion_stats> gm_stats;
+  vector<uint8_t> gm_mask, gm_reg, gm_png;
+  vector<float> gm_res;
   Image8 last;  // image2 of the previous batch's last pair
   // --tracks: the tracker's points and counts, the clip being tracked (-1 none) and its next frame, the totals of the
   // finished clips
@@ -1239,6 +1294,29 @@ int main(int argc, char** argv) {
                                      nop == 2 ? 0.01f : 0.0f, nop == 2 ? 0.5f : 1.0f, interp.data(), nullptr, w, h,
                                      OFDIS_MEM_HOST);
     }
+    if (rc == OFDIS_OK && gm_model) {
+      // image2 of pair k: frame k + 1 of a clip, or the second image of the k-th pair
+      const size_t np = (size_t)n * w * h;
+      gm_models.resize((size_t)9 * n);
+      gm_stats.resize(n);
+      gm_mask.resize(np);
+      gm_res.resize(2 * np);
+      gm_reg.resize((size_t)n * hwc);
+      ofdis_motion_params mp;
+      memset(&mp, 0, sizeof(mp));
+      mp.model = gm_model;
+      mp.step = 8;
+      mp.fb_check = bidir ? 1 : 0;
+      mp.alpha = 0.01f;
+      mp.beta = 0.5f;
+      mp.hypotheses = 1024;
+      mp.threshold = 1.0f;
+      mp.refine = 3;
+      mp.seed = 0;
+      rc = ofdis_global_motion_fullres(ctx, 0, n, n, &mp, frames.data() + hwc, seq ? hwc : 2 * hwc, gm_models.data(),
+                                       gm_stats.data(), gm_mask.data(), gm_res.data(), gm_reg.data(), w, h,
+                                       OFDIS_MEM_HOST);
+    }
     size_t dcount[6] = {0, 0, 0, 0, 0, 0};  // statuses 0..4, filled
     if (rc == OFDIS_OK && disp_on) {
       const size_t np = (size_t)n * w * h;
@@ -1334,6 +1412,41 @@ int main(int argc, char** argv) {
       }
       save_png(im, w, h, nochannels, 8, with_suffix(jobs[j0 + k].out, "_interp", ".png").c_str());
     }
+    for (int k = 0; k < n && gm_model; ++k) {
+      const string& o = jobs[j0 + k].out;
+      fprintf(gm_file, "%s", with_suffix(o, "", "").c_str());
+      for (int i = 0; i < 9; ++i) fprintf(gm_file, " %.17g", gm_models[(size_t)9 * k + i]);
+      fprintf(gm_file, " %d %d %d\n", gm_stats[k].status, gm_stats[k].n_corr, gm_stats[k].n_inliers);
+      const float* r = gm_res.data() + (size_t)2 * k * w * h;
+      if (kitti) {  // the encoding of OFDIS_ENC_KITTI (flow)
+        vector<uint16_t> enc((size_t)3 * w * h);
+        for (size_t i = 0; i < (size_t)w * h; ++i) {
+          const float u = r[2 * i], v = r[2 * i + 1];
+          const bool valid = !std::isnan(u) && !std::isnan(v);
+          enc[3 * i] = valid ? (uint16_t)fminf(fmaxf(u * 64.0f + 32768.0f, 0.0f), 65535.0f) : (uint16_t)0;
+          enc[3 * i + 1] = valid ? (uint16_t)fminf(fmaxf(v * 64.0f + 32768.0f, 0.0f), 65535.0f) : (uint16_t)0;
+          enc[3 * i + 2] = valid ? 1 : 0;
+        }
+        save_png(enc.data(), w, h, 3, 16, with_suffix(o, "_residual").c_str());
+      } else {
+        ImageF f;
+        f.w = w; f.h = h; f.c = 2;
+        f.px.assign(r, r + (size_t)2 * w * h);
+        SaveFlowFile(f, with_suffix(o, "_residual").c_str());
+      }
+      save_mask_pgm(gm_mask.data() + (size_t)k * w * h, w, h, with_suffix(o, "_moving", ".pgm").c_str());
+      const uint8_t* im = gm_reg.data() + (size_t)k * hwc;
+      if (nochannels == 3) {  // the decoder's BGR -> RGB
+        gm_png.resize(hwc);
+        for (size_t q = 0; q < hwc; q += 3) {
+          gm_png[q] = im[q + 2];
+          gm_png[q + 1] = im[q + 1];
+          gm_png[q + 2] = im[q];
+        }
+        im = gm_png.data();
+      }
+      save_png(im, w, h, nochannels, 8, with_suffix(o, "_registered", ".png").c_str());
+    }
     for (int k = 0; k < n && disp_on; ++k) {
       const size_t o = (size_t)k * w * h;
       if (kitti) {
@@ -1404,6 +1517,10 @@ int main(int argc, char** argv) {
   if (ctx) ofdis_destroy(ctx);
   if (tracks_file && fclose(tracks_file) != 0) {
     fprintf(stderr, "error: cannot write %s\n", tracks_path);
+    return 1;
+  }
+  if (gm_file && fclose(gm_file) != 0) {
+    fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
     return 1;
   }
   if (verbosity > 0) printf("TIME (%zu pairs, load + flow + save) (ms): %3g\n", done, elapsed_ms(tv));

@@ -1005,3 +1005,288 @@ def disparity_filter(F: np.ndarray, B: np.ndarray | None = None, swapped: bool =
         depth = Z
         xyz = np.stack([canon(X), canon(Y), Z], axis=-1)
     return disp, status, depth, xyz
+
+
+# ofdis_motion_params / ofdis_motion_stats (include/ofdis_b200.h), field for field
+MOTION_MODELS = {"similarity": 1, "affine": 2, "homography": 3}
+MOTION_PARAM_FIELDS = ("model", "step", "fb_check", "alpha", "beta", "hypotheses", "threshold", "refine", "seed")
+MOTION_STATS_DTYPE = np.dtype([("status", "<i4"), ("n_corr", "<i4"), ("best_hypothesis", "<i4"),
+                               ("ransac_inliers", "<i4"), ("refits", "<i4"), ("n_inliers", "<i4")])
+MOTION_UNKNOWN_THRESH = 1e9  # a flow component above this (or NaN) is unknown, the rule of flow_error
+_SPLITMIX_GAMMA = 0x9E3779B97F4A7C15
+_QNAN64 = np.uint64(0x7FF8000000000000).view(np.float64)
+
+
+def splitmix64(z) -> np.ndarray:
+    """SplitMix64's finalizer on uint64 values (mod 2^64): the n-th output of the generator seeded with s is
+    splitmix64(s + n * 0x9E3779B97F4A7C15)."""
+    z = np.array(z, dtype=np.uint64, ndmin=1)
+    with np.errstate(over="ignore"):
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return z ^ (z >> np.uint64(31))
+
+
+def motion_draws(seed: int, hypotheses: int, n_min: int, m: int) -> np.ndarray:
+    """The correspondence indices (hypotheses, n_min) of ofdis_global_motion_fullres's draws."""
+    n = (8 * np.arange(hypotheses, dtype=np.uint64)[:, None] + np.arange(n_min, dtype=np.uint64)[None, :]
+         + np.uint64(1))
+    with np.errstate(over="ignore"):
+        z = splitmix64(np.uint64(seed % 2 ** 64) + n * np.uint64(_SPLITMIX_GAMMA)).reshape(n.shape)
+    return (((z >> np.uint64(32)) * np.uint64(m)) >> np.uint64(32)).astype(np.int64)
+
+
+def motion_rows(model: int, c: np.ndarray):
+    """The two rows of every correspondence c = (x, y, p, q) float32 (..., 4): (r1, r2, b1, b2), float64, r1 and r2
+    (..., k)."""
+    x, y, p, q = (c[..., i].astype(np.float64) for i in range(4))
+    one, zero = np.ones_like(x), np.zeros_like(x)
+    if model == 1:
+        r1 = [x, -y, one, zero]
+        r2 = [y, x, zero, one]
+    else:
+        r1 = [x, y, one, zero, zero, zero]
+        r2 = [zero, zero, zero, x, y, one]
+        if model == 3:
+            r1 += [-(x * p), -(y * p)]
+            r2 += [-(x * q), -(y * q)]
+    return np.stack(r1, -1), np.stack(r2, -1), p, q
+
+
+def motion_solve(A: np.ndarray, b: np.ndarray):
+    """The elimination of ofdis_global_motion_fullres on a batch of systems A (s, k, k), b (s, k) float64: partial
+    pivoting on the first row of the largest |a_ij|, then back substitution.  Returns (x (s, k), ok (s,))."""
+    A = np.array(A, np.float64)
+    b = np.array(b, np.float64)
+    s, k = b.shape
+    ar = np.arange(s)
+    ok = np.ones(s, bool)
+    with np.errstate(all="ignore"):
+        for j in range(k):
+            best = np.abs(A[:, j, j])
+            piv = np.full(s, j)
+            for i in range(j + 1, k):
+                a = np.abs(A[:, i, j])
+                upd = a > best
+                best = np.where(upd, a, best)
+                piv = np.where(upd, i, piv)
+            ok &= best > 0
+            rj, rp = A[ar, j].copy(), A[ar, piv].copy()
+            A[ar, piv], A[ar, j] = rj, rp
+            bj, bp = b[ar, j].copy(), b[ar, piv].copy()
+            b[ar, piv], b[ar, j] = bj, bp
+            for i in range(j + 1, k):
+                f = A[:, i, j] / A[:, j, j]
+                A[:, i, j + 1:] = A[:, i, j + 1:] - f[:, None] * A[:, j, j + 1:]
+                b[:, i] = b[:, i] - f * b[:, j]
+        x = np.zeros((s, k))
+        for i in range(k - 1, -1, -1):
+            xi = b[:, i]
+            for c in range(i + 1, k):
+                xi = xi - A[:, i, c] * x[:, c]
+            x[:, i] = xi / A[:, i, i]
+    return x, ok & np.isfinite(x).all(axis=1)
+
+
+def motion_hmat(model: int, x: np.ndarray) -> np.ndarray:
+    """H^ (..., 9) float64, row-major, of the parameters x (..., k)."""
+    z, o = np.zeros(x.shape[:-1]), np.ones(x.shape[:-1])
+    if model == 1:
+        h = [x[..., 0], -x[..., 1], x[..., 2], x[..., 1], x[..., 0], x[..., 3], z, z, o]
+    else:
+        h = [x[..., i] for i in range(6)] + ([x[..., 6], x[..., 7]] if model == 3 else [z, z]) + [o]
+    return np.stack(h, -1)
+
+
+def motion_inliers(g: np.ndarray, c: np.ndarray, t) -> np.ndarray:
+    """The inlier test of ofdis_global_motion_fullres, float32: g (..., 9) against the correspondences c (m, 4);
+    returns (..., m) bool."""
+    f32 = np.float32
+    g = np.asarray(g, f32)[..., None, :]
+    x, y, p, q = c[:, 0], c[:, 1], c[:, 2], c[:, 3]
+    with np.errstate(all="ignore"):
+        X = (g[..., 0] * x + g[..., 1] * y) + g[..., 2]
+        Y = (g[..., 3] * x + g[..., 4] * y) + g[..., 5]
+        W = (g[..., 6] * x + g[..., 7] * y) + g[..., 8]
+        ex, ey = X - p * W, Y - q * W
+        tw = f32(t) * W
+        return (W > 0) & (ex * ex + ey * ey <= tw * tw)
+
+
+def motion_normal_sums(model: int, c: np.ndarray, inl: np.ndarray):
+    """The refit's normal equations (A (k, k), b (k,)) from the inliers `inl` of c (m, 4), summed in chunks of 32 from
+    +0.0 and a pairwise tree over the chunk sums padded with +0.0 to a power of two."""
+    r1, r2, b1, b2 = motion_rows(model, c)
+    k = r1.shape[1]
+    terms = [(r1[:, a] * r1[:, b]) + (r2[:, a] * r2[:, b]) for a in range(k) for b in range(a, k)]
+    terms += [(r1[:, a] * b1) + (r2[:, a] * b2) for a in range(k)]
+    T = np.where(inl[:, None], np.stack(terms, -1), 0.0)
+    m, ne = T.shape
+    nc = (m + 31) // 32
+    T = np.concatenate([T, np.zeros((nc * 32 - m, ne))]).reshape(nc, 32, ne)
+    v = np.zeros((nc, ne))
+    for e in range(32):
+        v = v + T[:, e]
+    P = 1
+    while P < nc:
+        P *= 2
+    v = np.concatenate([v, np.zeros((P - nc, ne))])
+    while v.shape[0] > 1:
+        v = v[0::2] + v[1::2]
+    A = np.zeros((k, k))
+    e = 0
+    for a in range(k):
+        for b in range(a, k):
+            A[a, b] = A[b, a] = v[0, e]
+            e += 1
+    return A, v[0, e:]
+
+
+def motion_to_pixels(model: int, H: np.ndarray, cx, cy, sigma) -> np.ndarray:
+    """M = T^-1 H^ T (9,) float64 in the expression order of the header."""
+    S, Cx, Cy = float(sigma), float(cx), float(cy)
+    A = [0.0] * 9
+    for r in range(3):
+        A[3 * r] = float(H[3 * r]) * S
+        A[3 * r + 1] = float(H[3 * r + 1]) * S
+        A[3 * r + 2] = float(H[3 * r + 2]) - (A[3 * r] * Cx + A[3 * r + 1] * Cy)
+    M = [0.0] * 9
+    for c in range(3):
+        M[c] = A[c] / S + Cx * A[6 + c]
+        M[3 + c] = A[3 + c] / S + Cy * A[6 + c]
+        M[6 + c] = A[6 + c]
+    M = np.array(M)
+    if model == 3:
+        with np.errstate(all="ignore"):
+            M = M / M[8]
+    return np.where(np.isnan(M), _QNAN64, M)
+
+
+def motion_params(params) -> dict:
+    """The params mapping with the model as its number (names of MOTION_MODELS are accepted)."""
+    p = {k: params[k] for k in MOTION_PARAM_FIELDS}
+    p["model"] = MOTION_MODELS.get(p["model"], p["model"])
+    return p
+
+
+def _motion_pair(F, B, I1, p):
+    f32 = np.float32
+    h, w = F.shape[:2]
+    model, s = int(p["model"]), int(p["step"])
+    n_min, k = model + 1, 2 * (model + 1)
+    u, v = F[..., 0], F[..., 1]
+    X = np.arange(w, dtype=f32)[None, :]
+    Y = np.arange(h, dtype=f32)[:, None]
+    with np.errstate(invalid="ignore", over="ignore"):
+        xs, ys = X + u, Y + v
+        lim = f32(MOTION_UNKNOWN_THRESH)
+        valid = (np.abs(u) <= lim) & (np.abs(v) <= lim) & (xs >= 0) & (xs <= f32(w - 1)) & (ys >= 0) & \
+            (ys <= f32(h - 1))
+    if p["fb_check"]:
+        valid &= consistency_check(F, B, p["alpha"], p["beta"])[0] == 0
+    # 1. correspondences
+    ncx, ncy = (w - 1) // s + 1, (h - 1) // s + 1
+    cell = np.arange(ncx * ncy)
+    cxs = np.minimum((cell % ncx) * s + s // 2, w - 1)
+    cys = np.minimum((cell // ncx) * s + s // 2, h - 1)
+    sel = valid[cys, cxs]
+    cxs, cys = cxs[sel], cys[sel]
+    c_x, c_y = f32(0.5) * f32(w - 1), f32(0.5) * f32(h - 1)
+    sigma = f32(2.0) / f32(max(w, h))
+    corr = np.stack([(cxs.astype(f32) - c_x) * sigma, (cys.astype(f32) - c_y) * sigma,
+                     (xs[cys, cxs] - c_x) * sigma, (ys[cys, cxs] - c_y) * sigma], -1).astype(f32)
+    m = corr.shape[0]
+    t = f32(p["threshold"]) * sigma
+    st = np.zeros((), MOTION_STATS_DTYPE)
+    st["n_corr"], st["best_hypothesis"] = m, -1
+    status = 1 if m < n_min else 0
+    if not status:
+        # 2. hypotheses
+        idx = motion_draws(int(p["seed"]), int(p["hypotheses"]), n_min, m)
+        r1, r2, b1, b2 = motion_rows(model, corr[idx])  # (nh, n_min, k)
+        A = np.stack([r1, r2], 2).reshape(idx.shape[0], k, k)
+        b = np.stack([b1, b2], 2).reshape(idx.shape[0], k)
+        x, ok = motion_solve(A, b)
+        # 3. scoring
+        g = motion_hmat(model, x).astype(f32)
+        counts = np.zeros(idx.shape[0], np.int64)
+        for h0 in range(0, idx.shape[0], 256):
+            counts[h0:h0 + 256] = motion_inliers(g[h0:h0 + 256], corr, t).sum(axis=1)
+        if not ok.any():
+            status = 2
+    if status:
+        M = np.full(9, _QNAN64)
+    else:
+        keys = np.where(ok, (counts << 32) | (0xFFFFFFFF - np.arange(idx.shape[0])), -1)
+        best = int(np.argmax(keys))
+        st["best_hypothesis"], st["ransac_inliers"] = best, counts[best]
+        xm = x[best]
+        refits = 0
+        # 4. refits
+        for r in range(int(p["refine"]) + 1):
+            inl = motion_inliers(motion_hmat(model, xm).astype(f32), corr, t)
+            cnt = int(inl.sum())
+            if r == int(p["refine"]) or cnt < n_min:
+                break
+            An, bn = motion_normal_sums(model, corr, inl)
+            xn, okn = motion_solve(An[None], bn[None])
+            if not okn[0]:
+                break
+            xm, refits = xn[0], refits + 1
+        st["refits"], st["n_inliers"] = refits, cnt
+        # 5. the model in pixel coordinates
+        M = motion_to_pixels(model, motion_hmat(model, xm), c_x, c_y, sigma)
+    st["status"] = status
+    # 6. per pixel
+    if status:
+        residual = np.full((h, w, 2), _QNAN, f32)
+        mask = np.full((h, w), 2, np.uint8)
+        reg = None if I1 is None else np.zeros(I1.shape, np.uint8)
+        return M, st, mask, residual, reg
+    mm = M.astype(f32)
+    with np.errstate(all="ignore"):
+        mx = (mm[0] * X + mm[1] * Y) + mm[2]
+        my = (mm[3] * X + mm[4] * Y) + mm[5]
+        wq = (mm[6] * X + mm[7] * Y) + mm[8]
+        xw, yw = mx / wq, my / wq
+        rx, ry = u - (xw - X), v - (yw - Y)
+        close = rx * rx + ry * ry <= f32(p["threshold"]) * f32(p["threshold"])
+    residual = np.stack([rx, ry], -1).astype(f32)
+    residual = np.where(np.isnan(residual), _QNAN, residual).astype(f32)
+    mask = np.where(valid, np.where(close, 0, 1), 2).astype(np.uint8)
+    reg = None
+    if I1 is not None:
+        img = I1.reshape(h, w, -1).astype(f32)
+        with np.errstate(invalid="ignore"):
+            ins = (wq > 0) & (xw >= 0) & (xw <= f32(w - 1)) & (yw >= 0) & (yw <= f32(h - 1))
+        val = _bilinear_frame(img, np.where(ins, xw, f32(0)), np.where(ins, yw, f32(0)))
+        out = (np.fmin(np.fmax(val, f32(0)), f32(255)) + f32(0.5)).astype(np.uint8)
+        reg = np.where(ins[..., None], out, np.uint8(0)).reshape(I1.shape)
+    return M, st, mask, residual, reg
+
+
+def global_motion(F: np.ndarray, B: np.ndarray | None, frames1: np.ndarray | None, params):
+    """ofdis_global_motion_fullres, bit for bit: float32 as the header marks it, float64 in the solver, without
+    contraction.  F: the full-resolution flows of the pairs, (n, h, w, 2) or one pair (h, w, 2) float32, exactly what
+    ofdis_get_flow_fullres returns; B: their partners' (read with fb_check only); frames1: the 8-bit I1 of every pair,
+    (n, h, w[, noc]) (None: no registered frames); params: a mapping with MOTION_PARAM_FIELDS (the model as a number or
+    a name of MOTION_MODELS).  Returns (models (n, 3, 3) float64, stats (n,) MOTION_STATS_DTYPE, mask (n, h, w) uint8,
+    residual (n, h, w, 2) float32, registered (n, h, w[, noc]) uint8 or None), without the leading axis for one pair."""
+    p = motion_params(params)
+    Fa = np.asarray(F, np.float32)
+    one = Fa.ndim == 3
+    Fa = Fa[None] if one else Fa
+    Ba = None if B is None else np.asarray(B, np.float32).reshape(Fa.shape)
+    I1 = None if frames1 is None else np.asarray(frames1, np.uint8)
+    if I1 is not None and one:
+        I1 = I1[None]
+    res = [_motion_pair(Fa[i], None if Ba is None else Ba[i], None if I1 is None else I1[i], p)
+           for i in range(Fa.shape[0])]
+    models = np.stack([r[0] for r in res]).reshape(-1, 3, 3)
+    stats = np.stack([r[1] for r in res])
+    mask = np.stack([r[2] for r in res])
+    residual = np.stack([r[3] for r in res])
+    reg = None if I1 is None else np.stack([r[4] for r in res])
+    if one:
+        return models[0], stats[0], mask[0], residual[0], None if reg is None else reg[0]
+    return models, stats, mask, residual, reg

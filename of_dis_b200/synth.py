@@ -108,3 +108,47 @@ def layered_stereo(h: int, w: int, channels: int = 1, seed: int = 0, d_bg: int =
         return np.ascontiguousarray(img[..., 0] if channels == 1 else img)
 
     return q(left), q(right), gt, occluded
+
+
+def similarity_about_centre(h: int, w: int, angle_deg: float = 0.0, zoom: float = 1.0, shift=(0.0, 0.0)):
+    """The 3 x 3 float64 map of pixel positions that rotates by angle_deg and scales by zoom about the frame's centre
+    ((w-1)/2, (h-1)/2), then shifts by (dx, dy)."""
+    c, s = zoom * np.cos(np.deg2rad(angle_deg)), zoom * np.sin(np.deg2rad(angle_deg))
+    ox, oy = 0.5 * (w - 1), 0.5 * (h - 1)
+    return np.array([[c, -s, ox - c * ox + s * oy + shift[0]], [s, c, oy - s * ox - c * oy + shift[1]], [0, 0, 1.0]])
+
+
+def global_motion_clip(n: int, h: int, w: int, channels: int = 1, seed: int = 0, H=None,
+                       block=(0.55, 0.3, 0.85, 0.8), block_motion=(-4.0, 2.5)):
+    """A clip of n + 1 uint8 frames under one camera motion: frame t + 1 maps the pixel x of frame t to H x (H a 3 x 3
+    map of pixel positions, default the identity), i.e. frame t is the canvas of _canvas sampled at H^-t x (cubic).  In
+    front of it a textured rectangle of an independent canvas covers the fractions `block` = (x0, y0, x1, y1) of frame
+    0 and moves on its own by the translation block_motion = (dx, dy) per frame.  Returns (frames, models, masks):
+    frames (n + 1, h, w[, 3]), models (n, 3, 3) float64 (H for every pair) and masks (n, h, w) bool, the rectangle's
+    pixels in frame t of pair t."""
+    from scipy import ndimage
+
+    H = np.eye(3) if H is None else np.asarray(H, np.float64)
+    bg, m = _canvas(h, w, channels, seed)
+    fg, _ = _canvas(h, w, channels, seed + 1)
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    X0, Y0, X1, Y1 = block[0] * w, block[1] * h, block[2] * w, block[3] * h
+    frames, masks = [], []
+    Hinv = np.eye(3)
+    Hi = np.linalg.inv(H)
+    for t in range(n + 1):
+        sx = Hinv[0, 0] * xx + Hinv[0, 1] * yy + Hinv[0, 2]
+        sy = Hinv[1, 0] * xx + Hinv[1, 1] * yy + Hinv[1, 2]
+        sw = Hinv[2, 0] * xx + Hinv[2, 1] * yy + Hinv[2, 2]
+        bx, by = xx - t * block_motion[0], yy - t * block_motion[1]
+        inside = (bx >= X0) & (bx < X1) & (by >= Y0) & (by < Y1)
+        img = np.empty((h, w, channels))
+        for c in range(channels):
+            back = ndimage.map_coordinates(bg[..., c], [sy / sw + m, sx / sw + m], order=3, mode="nearest")
+            front = ndimage.map_coordinates(fg[..., c], [by + m, bx + m], order=3, mode="nearest")
+            img[..., c] = np.where(inside, front, back)
+        q = np.clip(np.rint(img), 0, 255).astype(np.uint8)
+        frames.append(q[..., 0] if channels == 1 else q)
+        masks.append(inside)
+        Hinv = Hinv @ Hi
+    return np.ascontiguousarray(np.stack(frames)), np.repeat(H[None], n, 0), np.stack(masks[:n])

@@ -5,8 +5,10 @@ sor_wave_kernel: single CTA), a forward-backward case, a P=12 RGB and a P=12 ste
 kernel, stereo SOR), a 70-row level as three bands of the lane kernel and forced into a cluster of bands of the
 wave kernel with 1 and 2 rows per thread (st.async halo exchange), and the 8-bit frame path (pyramid and
 upsampling kernels), and a frame interpolation, a point tracking (advance, seed, block scan, scatter) and a filtered
-disparity (union-find speckles, fill, depth and xyz) checked against their restatements.  Results are checked against
-the oracle so that a clean log means a correct run."""
+disparity (union-find speckles, fill, depth and xyz) and a global motion (correspondences, compaction, hypotheses,
+the bulk-copied score tiles with and without refills, refits, per-pixel outputs) checked against their
+restatements.  Results are checked against the
+oracle so that a clean log means a correct run."""
 import os
 import sys
 
@@ -102,6 +104,49 @@ for k in range(n):
     ok &= all(np.array_equal(np.asarray(g[k]).view(np.uint8), np.asarray(e).view(np.uint8))
               for g, e in zip((got["disp"], got["status"], got["depth"], got["xyz"]), exp))
 print("%-22s %s" % ("disparity_stereo", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# global motion on a two-way RGB flow clip with fb_check and every per-pixel output; a step of 1 gives more
+# correspondences than one 4096-entry score tile
+prm = params.from_cli_numbers("3 1 8 8 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=3, nop=2)
+clip = synth.synthetic_sequence(n + 1, h, w, 3, seed=5, amp=3.0)
+ctx = api.Context(prm, 96, 64, prm.p_samp_s, 2 * n)
+ctx.upload_sequence_bidir_u8(0, n, clip, w, h)
+ctx.run(2 * n)
+full = np.empty((2 * n, h, w, 2), np.float32)
+ctx.get_flow_fullres(0, 2 * n, full, w, h)
+ctx.sync()
+mp = dict(model="homography", step=1, fb_check=1, alpha=0.01, beta=0.5, hypotheses=100, threshold=1.0, refine=3, seed=3)
+mask, res, reg = np.empty((n, h, w), np.uint8), np.empty((n, h, w, 2), np.float32), np.empty((n, h, w, 3), np.uint8)
+models, stats = ctx.global_motion_fullres(0, n, mp, width_org=w, height_org=h, b0=n, i1=clip[1:], mask=mask,
+                                          residual=res, registered=reg)
+ctx.close()
+exp = preprocess.global_motion(full[:n], full[n:], clip[1:], mp)
+ok = all(np.array_equal(np.asarray(g).view(np.uint8), np.asarray(e).view(np.uint8))
+         for g, e in zip((models, stats, mask, res, reg), exp))
+print("%-22s %s" % ("global_motion_rgb", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# and on 128 x 160 gray frames at step 1 without fb_check: more than 8192 correspondences per pair, so the score
+# kernel refills both of its bulk-copied tile buffers
+h2, w2 = 128, 160
+prm = params.from_cli_numbers("3 1 8 8 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=1, nop=2)
+clip = synth.synthetic_sequence(n + 1, h2, w2, 1, seed=6, amp=3.0)
+ctx = api.Context(prm, w2, h2, prm.p_samp_s, n)
+ctx.upload_sequence_u8(0, n, clip, w2, h2)
+ctx.run(n)
+full = np.empty((n, h2, w2, 2), np.float32)
+ctx.get_flow_fullres(0, n, full, w2, h2)
+ctx.sync()
+mp = dict(model="affine", step=1, fb_check=0, alpha=0.01, beta=0.5, hypotheses=70, threshold=1.0, refine=2, seed=4)
+mask, res, reg = np.empty((n, h2, w2), np.uint8), np.empty((n, h2, w2, 2), np.float32), np.empty((n, h2, w2), np.uint8)
+models, stats = ctx.global_motion_fullres(0, n, mp, width_org=w2, height_org=h2, i1=clip[1:], mask=mask, residual=res,
+                                          registered=reg)
+ctx.close()
+exp = preprocess.global_motion(full, None, clip[1:], mp)
+ok = (stats["n_corr"] > 8192).all() and all(np.array_equal(np.asarray(g).view(np.uint8), np.asarray(e).view(np.uint8))
+                                            for g, e in zip((models, stats, mask, res, reg), exp))
+print("%-22s %s" % ("global_motion_tiles", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
