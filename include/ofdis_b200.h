@@ -548,6 +548,77 @@ int ofdis_track_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned c
  * first ofdis_track_begin or with a NULL out. */
 int ofdis_track_stats_get(const ofdis_ctx* ctx, ofdis_track_stats* out);
 
+/* Video stabilisation (extension): a Gaussian-smoothed camera path streamed through a clip, from the per-pair models
+ * of ofdis_global_motion_fullres, and every frame warped onto it on the device (the motion filter of Matsushita et al.,
+ * "Full-frame video stabilization", CVPR 2005, and of OpenCV's videostab).  The context owns one stabiliser: the
+ * params and weights, the index L of the last frame received, the index of the next frame to emit, the models still
+ * needed and the frames not emitted yet.  It persists across calls and across ofdis_run and the other extensions;
+ * ofdis_stab_begin resets it and ofdis_destroy frees it.  float64 in the path, float32 in the per-pixel warp,
+ * everything without contraction and with IEEE division; preprocess.stabilize restates it bit for bit, and its output
+ * does not depend on how the clip is cut into calls.  W = width_org, H = height_org, r = radius, I = the identity.
+ *   Models as received.  Model k (M_k) maps a pixel of frame k to its position in frame k+1.  Its entries are divided
+ *   by its m22; it is replaced by I when m22 is not finite and non-zero, an entry of the divided model is not finite,
+ *   or its adjugate's (2,2) entry a = m00*m11 - m01*m10 is not finite and non-zero (I means "camera still"; the nine
+ *   NaNs of a status != 0 pair are such a model).
+ *   Matrices (3 x 3, row-major, float64).  (A*B)_ij = (A_i0*B_0j + A_i1*B_1j) + A_i2*B_2j.  norm(A): every entry
+ *   divided by A_22.  inv(A) = norm(C) of the adjugate C: C00 = a11*a22 - a12*a21, C01 = a02*a21 - a01*a22,
+ *   C02 = a01*a12 - a02*a11, C10 = a12*a20 - a10*a22, C11 = a00*a22 - a02*a20, C12 = a02*a10 - a00*a12,
+ *   C20 = a10*a21 - a11*a20, C21 = a01*a20 - a00*a21, C22 = a00*a11 - a01*a10 (exact on affine maps, whose products
+ *   keep the row (0, 0, 1)).  A norm or inv whose divisor is zero or not finite, or that yields a non-finite entry,
+ *   makes the frame's path undefined.
+ *   Path of frame t over the window [a, b], a = max(0, t-r); b = t+r in ofdis_stab_push, min(L, t+r) in
+ *   ofdis_stab_finish.  P = I, acc = w0*I (w0 on the diagonal, +0.0 elsewhere), wsum = w0.  Forward, d = 1 .. b-t:
+ *   P = norm(M_{t+d-1} * P), acc_ij = acc_ij + w_d*P_ij, wsum = wsum + w_d.  Backward from P = I, d = 1 .. t-a:
+ *   P = norm(inv(M_{t-d}) * P), the same sums.  S = acc / wsum entry by entry (S_22 is exactly 1: acc_22 and wsum are
+ *   summed in the same order); a non-finite entry of S makes the path undefined.  S maps a pixel of frame t to the
+ *   weighted mean of its positions in the window's frames: the smoothed camera.
+ *   Crop and limit.  s = 1 - 2*(double)crop, c = (0.5*(W-1), 0.5*(H-1)), Z = [s, 0, c_x*(1-s); 0, s, c_y*(1-s);
+ *   0, 0, 1] (an output pixel -> its position in the uncropped stabilised frame).  S(l): off-diagonal entries l*S_ij,
+ *   diagonal entries (1-l) + l*S_ii.  A(l) = norm(inv(S(l)) * Z), a0..a8 = A(l) rounded to float32.  l passes when
+ *   A(l) is defined and each corner (0,0), (W-1,0), (0,H-1), (W-1,H-1) passes the per-pixel test below (wq > 0 and
+ *   (mx/wq, my/wq) in [0, W-1] x [0, H-1]).  limit 0: l = 1; limit 1: l = 1 if it passes, else 20 rounds of bisection
+ *   from lo = 0, hi = 1 with mid = 0.5*(lo + hi) (mid passes: lo = mid, else hi = mid), l = lo (S(0) = I: no correction).
+ *   An undefined path, or limit 0 with A(1) undefined, gives S = I, l = 0 and status 1.
+ *   Per pixel (X, Y) of output frame t, in float32: mx = (a0*X + a1*Y) + a2, my = (a3*X + a4*Y) + a5,
+ *   wq = (a6*X + a7*Y) + a8; with wq > 0 and (mx/wq, my/wq) in the frame, frame t there by the bilinear byte rule and
+ *   rounding of the registered frames of ofdis_global_motion_fullres, else 0. */
+typedef struct ofdis_stab_params {
+  int radius;   /* r, 1 .. 64: frames on each side of the smoothing window */
+  float crop;   /* 0 <= crop < 0.5: the fraction cut from each side, the rest scaled back to the frame */
+  int limit;    /* 0 | 1: shrink each correction so that the cropped frame's corners stay inside the source frame */
+} ofdis_stab_params;
+typedef struct ofdis_stab_frame {
+  long long frame;        /* index in the clip, from 0 */
+  int status;             /* 0, or 1: the window's path is undefined and the correction is the identity */
+  double lambda;          /* l: the share of the correction the limit keeps, 1 without it */
+  double correction[9];   /* S(l), row-major: frame pixel -> stabilised position, before the crop */
+} ofdis_stab_frame;       /* 96 bytes */
+/* Resets the stabiliser: params, weights (host, r+1 finite entries >= 0 with weights[0] > 0; w_d weighs the frames d
+ * away, so the caller picks the kernel -- preprocess.gaussian_weights and the batch command make a Gaussian) and frame 0
+ * ([H][W][noc] bytes in memkind).  Allocates the workspace -- a device ring of r + max_frames frames (W*H*noc bytes
+ * each: 79 x 6.2 MB, about 491 MB, for 1920 x 1080 RGB at r = 15 and 64 frames), a ring of 2r + max_frames models
+ * (72 bytes each) and max(r, max_frames) per-frame records (a0..a8 and the ofdis_stab_frame) -- which grows, never
+ * shrinks and is freed by ofdis_destroy.  A NULL or out-of-range p, bad weights or a NULL frame is OFDIS_ERR_ARG;
+ * frame sizes are checked as in ofdis_get_flow_fullres.  The stabiliser reads no flow: any context may use it. */
+int ofdis_stab_begin(ofdis_ctx* ctx, const ofdis_stab_params* p, const double* weights, const unsigned char* frame0,
+                     int width_org, int height_org, int memkind);
+/* Appends frames L+1 .. L+n: frame k at frames + k*frame_stride (a clip: frames + hwc with stride hwc; the pairs of
+ * ofdis_upload_frames_u8: image2 at stride 2hwc), in memkind, and models = [n][9] float64 in host memory, model k
+ * mapping frame L+k to frame L+k+1 -- exactly what ofdis_global_motion_fullres returns.  Then emits, in order, every
+ * frame t <= L' - r not emitted yet (L' = L+n): at most n frames, exactly n once the clip is longer than r.  Their bytes
+ * go to out ([n][H][W][noc] in memkind), their records to info ([n], host, may be NULL) and their count to *n_out.
+ * n < 1 or n > max_frames, a NULL models, frames, out or n_out, frame_stride below one frame, or no live stabiliser is
+ * OFDIS_ERR_ARG. */
+int ofdis_stab_push(ofdis_ctx* ctx, int n, const double* models, const unsigned char* frames, size_t frame_stride,
+                    unsigned char* out, ofdis_stab_frame* info, int* n_out, int memkind);
+/* Emits the remaining min(r, L+1) frames, each with its window cut at L (out holds r frames), and ends the stabiliser:
+ * a push or finish before the next ofdis_stab_begin is OFDIS_ERR_ARG, as are a NULL out or n_out.
+ * Host frames are copied straight into the ring, host output goes through the full-resolution scratch.  A push or
+ * finish enqueues its copies and, when it emits a frame, 2 kernels, whatever n; it synchronises the context's stream
+ * once, at the end.  Not part of ofdis_run's graph; the flows are not changed.  A call that fails on the way leaves
+ * the stabiliser to a new ofdis_stab_begin. */
+int ofdis_stab_finish(ofdis_ctx* ctx, unsigned char* out, ofdis_stab_frame* info, int* n_out, int memkind);
+
 /* Init flow from a flow of the original frame size (extension; the reference's disabled file input,
  * run_dense.cpp:292-301,355-378).  `flow` = [f1-f0][height_org][width_org][nop] floats.  Prepares the initflow of
  * pairs [f0, f1) that the following ofdis_run(ctx, n, use_initflow = 1) reads: replicate padding to the context,

@@ -14,8 +14,9 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import (DISP_FILTER_FIELDS, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, STEREO_CAMERA_FIELDS,
-                         TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, motion_params)
+from .preprocess import (DISP_FILTER_FIELDS, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, STAB_FRAME_DTYPE,
+                         STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE,
+                         TRACK_STATS_FIELDS, gaussian_weights, motion_params)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("OFDIS_LIB") or os.path.join(_HERE, "lib", "libofdis_b200.so")  # OFDIS_LIB: experiments only
@@ -38,7 +39,7 @@ EXPORTS = [
     "ofdis_consistency_fullres", "ofdis_flow_error_fullres", "ofdis_debug_sor_plan",
     "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres", "ofdis_interpolate_fullres",
     "ofdis_track_begin", "ofdis_track_advance", "ofdis_track_stats_get", "ofdis_disparity_fullres",
-    "ofdis_global_motion_fullres",
+    "ofdis_global_motion_fullres", "ofdis_stab_begin", "ofdis_stab_push", "ofdis_stab_finish",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -98,6 +99,21 @@ class MotionStats(ctypes.Structure):
 
 assert tuple(k for k, _ in MotionParams._fields_) == MOTION_PARAM_FIELDS
 assert ctypes.sizeof(MotionStats) == MOTION_STATS_DTYPE.itemsize
+
+
+class StabParams(ctypes.Structure):
+    """ofdis_stab_params (include/ofdis_b200.h)."""
+    _fields_ = [("radius", ctypes.c_int), ("crop", ctypes.c_float), ("limit", ctypes.c_int)]
+
+
+class StabFrame(ctypes.Structure):
+    """ofdis_stab_frame (include/ofdis_b200.h); STAB_FRAME_DTYPE is the same record as numpy sees it."""
+    _fields_ = [("frame", ctypes.c_longlong), ("status", ctypes.c_int), ("lambda", ctypes.c_double),
+                ("correction", ctypes.c_double * 9)]
+
+
+assert tuple(k for k, _ in StabParams._fields_) == STAB_PARAM_FIELDS
+assert ctypes.sizeof(StabFrame) == STAB_FRAME_DTYPE.itemsize
 
 
 class OfdisError(RuntimeError):
@@ -164,6 +180,11 @@ def lib():
         L.ofdis_global_motion_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
             [ctypes.POINTER(MotionParams), ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 5 + [ctypes.c_int] * 3
         L.ofdis_track_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackStats)]
+        L.ofdis_stab_begin.argtypes = [ctypes.c_void_p, ctypes.POINTER(StabParams)] + [ctypes.c_void_p] * 2 + \
+            [ctypes.c_int] * 3
+        L.ofdis_stab_push.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 2 + [ctypes.c_size_t] + \
+            [ctypes.c_void_p] * 3 + [ctypes.c_int]
+        L.ofdis_stab_finish.argtypes = [ctypes.c_void_p] + [ctypes.c_void_p] * 3 + [ctypes.c_int]
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -634,6 +655,68 @@ class Context:
         if rc != 0:
             raise OfdisError("track_stats: status %d" % rc)
         return {k: int(getattr(st, k)) for k in TRACK_STATS_FIELDS}
+
+    def stab_begin(self, params, frame0, width_org, height_org, weights=None, memkind=MEM_HOST):
+        """Resets the context's stabiliser on frame 0 (ofdis_stab_begin; preprocess.stabilize restates the whole clip).
+        params: a mapping with preprocess.STAB_PARAM_FIELDS or a StabParams; weights: r+1 floats, by default
+        preprocess.gaussian_weights(radius).  Host: frame0 a uint8 (height_org, width_org[, noc]) array; with
+        memkind=MEM_DEVICE a device address the caller owns."""
+        if not isinstance(params, StabParams):
+            params = StabParams(*[params[k] for k in STAB_PARAM_FIELDS])
+        wts = np.ascontiguousarray(gaussian_weights(params.radius) if weights is None else weights, np.float64)
+        if wts.shape != (max(params.radius, 0) + 1,):
+            raise ValueError("stab_begin: weights must hold radius + 1 = %d values" % (params.radius + 1))
+        if memkind == MEM_HOST:
+            self._frames_u8("stab_begin: frame0", np.asarray(frame0)[None], 1, width_org, height_org)
+            frame0 = np.ascontiguousarray(frame0)
+        self._ck(lib().ofdis_stab_begin(self._h, ctypes.byref(params), _ptr(wts), _ptr(frame0), width_org, height_org,
+                                        memkind))
+        self._stab = (params.radius, width_org, height_org)
+
+    def _stab_out(self, frames, out, memkind):
+        _, w, h = getattr(self, "_stab", (0, 0, 0))
+        noc = self.prm.noc
+        shape = (frames, h, w) + ((noc,) if noc > 1 else ())
+        if memkind == MEM_HOST:
+            return np.empty(shape, np.uint8)
+        if out is None:
+            raise ValueError("stab: memkind=MEM_DEVICE needs out, a device address of %s bytes" % (shape,))
+        return out
+
+    def stab_push(self, models, frames, frame_stride=None, memkind=MEM_HOST, out=None):
+        """Appends n frames and their n models (ofdis_stab_push) and returns (out[:n_out], info): the frames whose
+        smoothing window is complete, and their records (n_out,) of STAB_FRAME_DTYPE.  models: (n, 3, 3) float64 on the
+        host, model k mapping the previous frame onto frames[k] -- what global_motion_fullres returns.  Host: frames a
+        uint8 (n, height_org, width_org[, noc]) array whose frames are C-contiguous (clip[1:] or pairs[:, 1]).  With
+        memkind=MEM_DEVICE, frames and out ([n] frames) are device addresses the caller owns, frame_stride the bytes
+        between frames (default one frame), and out is returned as given with n_out."""
+        models = np.ascontiguousarray(models, np.float64).reshape(-1, 9)
+        n = models.shape[0]
+        _, w, h = getattr(self, "_stab", (0, 0, 0))
+        if memkind == MEM_HOST:
+            frame_stride = self._frames_u8("stab_push: frames", frames, n, w, h)
+            pf = frames.ctypes.data
+        else:
+            frame_stride = h * w * self.prm.noc if frame_stride is None else frame_stride
+            pf = frames
+        dst = self._stab_out(max(n, 1), out, memkind)
+        info = np.zeros(max(n, 1), STAB_FRAME_DTYPE)
+        n_out = ctypes.c_int(0)
+        self._ck(lib().ofdis_stab_push(self._h, n, _ptr(models), _ptr(pf), frame_stride, _ptr(dst), _ptr(info),
+                                       ctypes.byref(n_out), memkind))
+        k = n_out.value
+        return (dst[:k] if memkind == MEM_HOST else (dst, k)), info[:k].copy()
+
+    def stab_finish(self, memkind=MEM_HOST, out=None):
+        """Emits the remaining frames and ends the stabiliser (ofdis_stab_finish): (out[:n_out], info) as stab_push,
+        out holding radius frames."""
+        r = getattr(self, "_stab", (0, 0, 0))[0]
+        dst = self._stab_out(max(r, 1), out, memkind)
+        info = np.zeros(max(r, 1), STAB_FRAME_DTYPE)
+        n_out = ctypes.c_int(0)
+        self._ck(lib().ofdis_stab_finish(self._h, _ptr(dst), _ptr(info), ctypes.byref(n_out), memkind))
+        k = n_out.value
+        return (dst[:k] if memkind == MEM_HOST else (dst, k)), info[:k].copy()
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

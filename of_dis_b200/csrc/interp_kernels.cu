@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(256) interp_blend_kernel(InterpSrc s, InterpWo
   unsigned char* q = out + o * NOC;
   for (int c = 0; c < NOC; ++c) {
     const float val = only0 ? s0[c] : only1 ? s1[c] : (1.0f - t) * s0[c] + t * s1[c];
-    q[c] = (unsigned char)(fminf(fmaxf(val, 0.f), 255.f) + 0.5f);
+    q[c] = round_u8(val);
   }
 }
 

@@ -114,10 +114,6 @@ __device__ __forceinline__ bool motion_solve(double (&A)[K][K], double (&b)[K], 
   return ok;
 }
 
-__device__ __forceinline__ bool in_frame_f(float x, float y, int w, int h) {
-  return x >= 0.f && x <= (float)(w - 1) && y >= 0.f && y <= (float)(h - 1);
-}
-
 // ---- 1. correspondences ------------------------------------------------------------------------------------------
 template <bool FB>
 __global__ void __launch_bounds__(kCorrThreads) motion_corr_kernel(LevelGeom g, int fa, int fb, MotionGeom mg,
@@ -470,7 +466,7 @@ __global__ void __launch_bounds__(256) motion_apply_kernel(LevelGeom g, int fa, 
     if (o.registered && wq > 0.f && in_frame_f(xw, yw, w, h)) {
       float v[NOC];
       bil_u8<NOC>(o.i1 + k * o.stride, w, h, xw, yw, v);
-      for (int c = 0; c < NOC; ++c) reg[c] = (unsigned char)(fminf(fmaxf(v[c], 0.f), 255.f) + 0.5f);
+      for (int c = 0; c < NOC; ++c) reg[c] = round_u8(v[c]);
     }
   }
   if (o.residual) {

@@ -92,6 +92,15 @@ struct ofdis_ctx {
   void* d_motion = nullptr;
   size_t motion_cells = 0, motion_hyps = 0;
   MotionWork motion{};
+  // the stabiliser of ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish: its workspace (StabWork: the frame ring,
+  // the model ring, the per-frame records), the geometry and weights of the last begin, L and the next frame to emit;
+  // grows, never shrinks; never touched by ofdis_run
+  void* d_stab = nullptr;
+  size_t stab_bytes = 0;
+  StabWork stab{};
+  StabGeom sgeom{};
+  long long stab_last = 0, stab_next = 0;
+  bool stab_on = false;
   std::vector<float*> d_flow;   // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -462,6 +471,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_track);
   cudaFree(ctx->d_disp);
   cudaFree(ctx->d_motion);
+  cudaFree(ctx->d_stab);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -1450,6 +1460,152 @@ int ofdis_track_stats_get(const ofdis_ctx* ctx, ofdis_track_stats* out) {
   out->dropped = (long long)s.dropped;
   out->alive = s.alive;
   out->next_id = s.next_id;
+  return OFDIS_OK;
+}
+
+// The stabiliser's workspace for frames of hwc bytes at radius r: the frame ring (r + max_frames frames), the model
+// ring (2r + max_frames models) and max(r, max_frames) records.  Grows, never shrinks.
+static int ensure_stab(ofdis_ctx* ctx, size_t hwc, int r) {
+  const int ring = r + ctx->max_frames, mring = 2 * r + ctx->max_frames, nrec = std::max(r, ctx->max_frames);
+  const size_t b_frames = align16(hwc * ring), b_models = align16(sizeof(double) * 9 * mring);
+  const size_t bytes = b_frames + b_models + sizeof(StabRec) * nrec;
+  if (bytes > ctx->stab_bytes) {
+    CK(cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_stab);
+    ctx->d_stab = nullptr;
+    ctx->stab_bytes = 0;
+    if (cudaMalloc(&ctx->d_stab, bytes) != cudaSuccess) {
+      ctx->d_stab = nullptr;
+      return fail(ctx, OFDIS_ERR_NOMEM, "stab workspace");
+    }
+    ctx->stab_bytes = bytes;
+  }
+  char* b = static_cast<char*>(ctx->d_stab);
+  ctx->stab.frames = reinterpret_cast<unsigned char*>(b);
+  ctx->stab.models = reinterpret_cast<double*>(b + b_frames);
+  ctx->stab.rec = reinterpret_cast<StabRec*>(b + b_frames + b_models);
+  ctx->sgeom.ring = ring;
+  ctx->sgeom.mring = mring;
+  return OFDIS_OK;
+}
+
+int ofdis_stab_begin(ofdis_ctx* ctx, const ofdis_stab_params* p, const double* weights, const unsigned char* frame0,
+                     int width_org, int height_org, int memkind) {
+  static_assert(sizeof(ofdis_stab_frame) == 96, "ofdis_stab_frame: 96 bytes, as preprocess.STAB_FRAME_DTYPE");
+  if (!ctx) return OFDIS_ERR_ARG;
+  bool ok = p && p->radius >= 1 && p->radius <= STAB_MAX_RADIUS && p->crop >= 0.f && p->crop < 0.5f &&
+            (p->limit == 0 || p->limit == 1) && weights && frame0 && weights[0] > 0.0;
+  for (int d = 0; ok && d <= p->radius; ++d) ok = weights[d] >= 0.0 && weights[d] <= DBL_MAX;
+  if (!ok) return fail(ctx, OFDIS_ERR_ARG, "stab_begin: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("stab", -1);
+  CK(cudaSetDevice(ctx->device));
+  ctx->stab_on = false;
+  const size_t hwc = (size_t)width_org * height_org * ctx->prm.noc;
+  rc = ensure_stab(ctx, hwc, p->radius);
+  if (rc) return rc;
+  StabGeom& sg = ctx->sgeom;
+  sg.w = width_org;
+  sg.h = height_org;
+  sg.noc = ctx->prm.noc;
+  sg.radius = p->radius;
+  sg.limit = p->limit;
+  sg.crop = p->crop;
+  for (int d = 0; d <= STAB_MAX_RADIUS; ++d) sg.wt[d] = d <= p->radius ? weights[d] : 0.0;
+  CK(cudaMemcpyAsync(ctx->stab.frames, frame0, hwc,
+                     memkind == OFDIS_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->stab_last = ctx->stab_next = 0;
+  ctx->stab_on = true;
+  return OFDIS_OK;
+}
+
+// Emits frames stab_next .. stab_next + count - 1 (windows cut at L with cut) to out and info, then synchronises.
+static int stab_emit(ofdis_ctx* ctx, int count, int cut, unsigned char* out, ofdis_stab_frame* info, int memkind) {
+  StabGeom sg = ctx->sgeom;
+  sg.count = count;
+  sg.cut = cut;
+  sg.next = ctx->stab_next;
+  sg.last = ctx->stab_last;
+  sg.slot0 = (int)(ctx->stab_next % sg.ring);
+  const size_t pix = (size_t)sg.w * sg.h, hwc = pix * sg.noc;
+  std::vector<StabRec> rec(count);
+  if (count > 0) {
+    unsigned char* dout = out;
+    if (memkind != OFDIS_MEM_DEVICE) {
+      // the full-resolution scratch, at least what ofdis_get_flow_fullres asks for
+      const size_t frames = (size_t)std::max(sg.radius, ctx->max_frames);
+      int rc = ensure_full(ctx, std::max(pix * ctx->nop * (size_t)ctx->max_frames, (hwc * frames + 3) / 4));
+      if (rc) return rc;
+      dout = reinterpret_cast<unsigned char*>(ctx->d_full);
+    }
+    sg.vec = sg.w % 4 == 0 && reinterpret_cast<uintptr_t>(dout) % 4 == 0;
+    const int k = launch_stab(sg, ctx->stab, dout, ctx->stream);
+    if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "stab kernel launch", cudaGetLastError());
+    ctx->launches += k;
+    if (memkind != OFDIS_MEM_DEVICE) CK(cudaMemcpyAsync(out, dout, hwc * count, cudaMemcpyDeviceToHost, ctx->stream));
+    if (info) CK(cudaMemcpyAsync(rec.data(), ctx->stab.rec, sizeof(StabRec) * count, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (int i = 0; i < count && info; ++i) info[i] = rec[i].info;
+  return OFDIS_OK;
+}
+
+int ofdis_stab_push(ofdis_ctx* ctx, int n, const double* models, const unsigned char* frames, size_t frame_stride,
+                    unsigned char* out, ofdis_stab_frame* info, int* n_out, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (n < 1 || n > ctx->max_frames || !models || !frames || !out || !n_out)
+    return fail(ctx, OFDIS_ERR_ARG, "stab_push: bad argument");
+  if (!ctx->stab_on) return fail(ctx, OFDIS_ERR_ARG, "stab_push: no live stabiliser (ofdis_stab_begin)");
+  const StabGeom& sg = ctx->sgeom;
+  const size_t hwc = (size_t)sg.w * sg.h * sg.noc;
+  if (frame_stride < hwc) return fail(ctx, OFDIS_ERR_ARG, "stab_push: frame_stride below one frame");
+  NvtxRange nvtx("stab", -1);
+  CK(cudaSetDevice(ctx->device));
+  *n_out = 0;
+  // a call that fails on the way leaves the stabiliser to a new ofdis_stab_begin
+  ctx->stab_on = false;
+  const long long L = ctx->stab_last;
+  const cudaMemcpyKind kin = memkind == OFDIS_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  // frames L+1 .. L+n and models L .. L+n-1 into their rings, in at most two runs each across the wrap
+  for (int k = 0, run; k < n; k += run) {
+    const int slot = (int)((L + 1 + k) % sg.ring);
+    run = std::min(n - k, sg.ring - slot);
+    CK(cudaMemcpy2DAsync(ctx->stab.frames + (size_t)slot * hwc, hwc, frames + (size_t)k * frame_stride, frame_stride,
+                         hwc, run, kin, ctx->stream));
+  }
+  for (int k = 0, run; k < n; k += run) {
+    const int slot = (int)((L + k) % sg.mring);
+    run = std::min(n - k, sg.mring - slot);
+    CK(cudaMemcpyAsync(ctx->stab.models + (size_t)slot * 9, models + (size_t)k * 9, sizeof(double) * 9 * run,
+                       cudaMemcpyHostToDevice, ctx->stream));
+  }
+  ctx->stab_last = L + n;
+  const long long last_emitted = ctx->stab_last - sg.radius;
+  const int count = last_emitted >= ctx->stab_next ? (int)(last_emitted - ctx->stab_next + 1) : 0;
+  const int rc = stab_emit(ctx, count, 0, out, info, memkind);
+  if (rc) return rc;
+  ctx->stab_next += count;
+  *n_out = count;
+  ctx->stab_on = true;
+  return OFDIS_OK;
+}
+
+int ofdis_stab_finish(ofdis_ctx* ctx, unsigned char* out, ofdis_stab_frame* info, int* n_out, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!out || !n_out) return fail(ctx, OFDIS_ERR_ARG, "stab_finish: bad argument");
+  if (!ctx->stab_on) return fail(ctx, OFDIS_ERR_ARG, "stab_finish: no live stabiliser (ofdis_stab_begin)");
+  NvtxRange nvtx("stab", -1);
+  CK(cudaSetDevice(ctx->device));
+  *n_out = 0;
+  ctx->stab_on = false;
+  const int count = (int)(ctx->stab_last - ctx->stab_next + 1);
+  const int rc = stab_emit(ctx, count, 1, out, info, memkind);
+  if (rc) return rc;
+  ctx->stab_next += count;
+  *n_out = count;
   return OFDIS_OK;
 }
 

@@ -626,6 +626,16 @@ int main(int argc, char** argv) {
 // 255 where it moves on its own and 128 where its flow is unknown, leaves the frame or (with --bidirectional) is
 // inconsistent, the code of _occ.pgm; and <stem>_registered.png, image2 sampled at the model's position of every
 // pixel of image1 (0 outside image2).  Every other output keeps its bytes.  Not with --warm-start.
+//
+// --stabilize RADIUS CROP DIR (needs --global-motion, whose models it smooths; flow binaries only): every clip
+// stabilised on the device (ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish).  Clips are the runs of pairs of
+// --tracks, across batches: the stabiliser begins on a clip's first image1, every batch pushes the image2 frames of
+// its run with their models and the clip's end emits the rest.  Settings: radius RADIUS (1 .. 64), Gaussian weights
+// exp(-d*d / (2 RADIUS)) (sigma^2 = RADIUS, OpenCV videostab's default), crop CROP (0 <= CROP < 0.5) with the limit on
+// when CROP > 0.  Every frame of every clip goes to DIR/stab_<clip %04d>_<frame %06d>.png (8-bit gray, or RGB from the
+// *_RGB binaries), clips and frames counted from 0, and DIR/stab.txt gets one line per frame,
+// `clip frame s00 s01 s02 s10 s11 s12 s20 s21 s22 lambda status`, the correction and its share printed with %.17g.
+// Every other output keeps its bytes.  Not with --warm-start.
 
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
@@ -839,7 +849,7 @@ int main(int argc, char** argv) {
             "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
             "       [--color [--color-max M]] [--interpolate T] [--tracks PATH]\n"
             "       [--lr-check] [--speckle N R] [--fill] [--camera fx,fy,cx,cy,baseline,doffs]\n"
-            "       [--global-motion similarity|affine|homography PATH]\n"
+            "       [--global-motion similarity|affine|homography PATH [--stabilize RADIUS CROP DIR]]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -863,7 +873,10 @@ int main(int argc, char** argv) {
             "  holes filled with the background disparity, and with --camera <stem>_depth.pfm and <stem>.ply;\n"
             "  not with --warm-start\n"
             "  --global-motion MODEL PATH: flow only; the camera motion of every pair, one line per pair in PATH, and\n"
-            "  <stem>_residual<ext>, <stem>_moving.pgm and <stem>_registered.png; not with --warm-start\n",
+            "  <stem>_residual<ext>, <stem>_moving.pgm and <stem>_registered.png; not with --warm-start\n"
+            "  --stabilize RADIUS CROP DIR: flow only, with --global-motion; every clip stabilised along its smoothed\n"
+            "  camera path (RADIUS 1..64 frames each side, CROP 0 <= CROP < 0.5 cut from each side), written to\n"
+            "  DIR/stab_<clip>_<frame>.png, the corrections to DIR/stab.txt; not with --warm-start\n",
             argv[0]);
     return 2;
   }
@@ -879,6 +892,7 @@ int main(int argc, char** argv) {
   const char* speckle_arg[2] = {nullptr, nullptr};  // --speckle N R
   const char* camera_arg = nullptr;  // --camera fx,fy,cx,cy,baseline,doffs
   const char* gm_arg[2] = {nullptr, nullptr};  // --global-motion MODEL PATH
+  const char* stab_arg[3] = {nullptr, nullptr, nullptr};  // --stabilize RADIUS CROP DIR
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -946,6 +960,15 @@ int main(int argc, char** argv) {
       gm_arg[0] = argv[first_num + 1];
       gm_arg[1] = argv[first_num + 2];
       first_num += 3;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--stabilize")) {
+      if (argc < first_num + 4 || stab_arg[0]) {
+        fprintf(stderr, "error: --stabilize takes a radius, a crop and an output directory\n");
+        return 2;
+      }
+      stab_arg[0] = argv[first_num + 1];
+      stab_arg[1] = argv[first_num + 2];
+      stab_arg[2] = argv[first_num + 3];
+      first_num += 4;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
         fprintf(stderr, "error: --gt takes one ground-truth list file\n");
@@ -1001,6 +1024,35 @@ int main(int argc, char** argv) {
       fprintf(stderr, "error: --global-motion takes the model similarity, affine or homography, got %s\n", gm_arg[0]);
       return 2;
     }
+  }
+  ofdis_stab_params stp;  // --stabilize
+  memset(&stp, 0, sizeof(stp));
+  vector<double> stab_wts;
+  if (stab_arg[0]) {
+    if (SELECTMODE != 1) {
+      fprintf(stderr, "error: --stabilize smooths the camera motion of flows; the stereo binaries take no --stabilize\n");
+      return 2;
+    }
+    if (warm) {
+      fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --stabilize\n");
+      return 2;
+    }
+    if (!gm_arg[0]) {
+      fprintf(stderr, "error: --stabilize smooths the models of --global-motion; give --global-motion too\n");
+      return 2;
+    }
+    char *e0 = nullptr, *e1 = nullptr;
+    const long r = strtol(stab_arg[0], &e0, 10);
+    const float crop = strtof(stab_arg[1], &e1);
+    if (e0 == stab_arg[0] || *e0 || r < 1 || r > 64 || e1 == stab_arg[1] || *e1 || !(crop >= 0.0f && crop < 0.5f)) {
+      fprintf(stderr, "error: --stabilize takes a radius 1..64 and a crop 0 <= CROP < 0.5, got %s %s\n", stab_arg[0],
+              stab_arg[1]);
+      return 2;
+    }
+    stp.radius = (int)r;
+    stp.crop = crop;
+    stp.limit = crop > 0.0f ? 1 : 0;
+    for (int d = 0; d <= stp.radius; ++d) stab_wts.push_back(exp(-(double)(d * d) / (2.0 * stp.radius)));
   }
   ofdis_disp_filter dfilt;
   memset(&dfilt, 0, sizeof(dfilt));
@@ -1122,12 +1174,23 @@ int main(int argc, char** argv) {
     }
     fprintf(tracks_file, "# clip frame id x y\n");
   }
+  FILE* stab_file = nullptr;
+  const string stab_txt = stab_arg[0] ? string(stab_arg[2]) + "/stab.txt" : string();
+  if (stab_arg[0]) {
+    stab_file = fopen(stab_txt.c_str(), "w");
+    if (!stab_file) {
+      fprintf(stderr, "error: cannot write %s\n", stab_txt.c_str());
+      if (tracks_file) fclose(tracks_file);
+      return 1;
+    }
+  }
   FILE* gm_file = nullptr;
   if (gm_model) {
     gm_file = fopen(gm_arg[1], "w");
     if (!gm_file) {
       fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
       if (tracks_file) fclose(tracks_file);
+      if (stab_file) fclose(stab_file);
       return 1;
     }
   }
@@ -1169,6 +1232,44 @@ int main(int argc, char** argv) {
     ttotal.ended_inconsistent += st.ended_inconsistent;
     ttotal.ended_boundary += st.ended_boundary;
     ttotal.dropped += st.dropped;
+  };
+  // --stabilize: the emitted frames and records, the clip being stabilised (-1 none), whether its stabiliser is live
+  // and its frame size
+  vector<uint8_t> sbuf, spng;
+  vector<ofdis_stab_frame> sinfo;
+  int sclip = -1, sw = 0, sh = 0;
+  bool stab_live = false;
+  auto write_stab = [&](int count) {
+    const size_t shwc = (size_t)sw * sh * nochannels;
+    for (int i = 0; i < count; ++i) {
+      const ofdis_stab_frame& f = sinfo[i];
+      fprintf(stab_file, "%d %lld", sclip, f.frame);
+      for (int e = 0; e < 9; ++e) fprintf(stab_file, " %.17g", f.correction[e]);
+      fprintf(stab_file, " %.17g %d\n", f.lambda, f.status);
+      const uint8_t* im = sbuf.data() + (size_t)i * shwc;
+      if (nochannels == 3) {  // the decoder's BGR -> RGB
+        spng.resize(shwc);
+        for (size_t q = 0; q < shwc; q += 3) {
+          spng[q] = im[q + 2];
+          spng[q + 1] = im[q + 1];
+          spng[q + 2] = im[q];
+        }
+        im = spng.data();
+      }
+      char name[64];
+      snprintf(name, sizeof(name), "/stab_%04d_%06lld.png", sclip, f.frame);
+      save_png(im, sw, sh, nochannels, 8, (string(stab_arg[2]) + name).c_str());
+    }
+  };
+  auto stab_end = [&]() -> int {  // emits the rest of the clip being stabilised
+    if (!stab_live) return OFDIS_OK;
+    stab_live = false;
+    sbuf.resize((size_t)stp.radius * sw * sh * nochannels);
+    sinfo.resize(stp.radius);
+    int count = 0;
+    const int rc = ofdis_stab_finish(ctx, sbuf.data(), sinfo.data(), &count, OFDIS_MEM_HOST);
+    if (rc == OFDIS_OK) write_stab(count);
+    return rc;
   };
   auto write_tracks = [&](const ofdis_track_point* p, int count) {
     for (int i = 0; i < count; ++i)
@@ -1233,6 +1334,11 @@ int main(int argc, char** argv) {
     verbosity = P.verbosity;
     if (w != ctx_w || h != ctx_h) {
       end_clip();  // a pair of another size never continues the previous one
+      if (stab_end() != OFDIS_OK) {
+        fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
+        ofdis_destroy(ctx);
+        return 1;
+      }
       if (ctx) ofdis_destroy(ctx);
       ctx = nullptr;
       ofdis_params p;
@@ -1358,6 +1464,30 @@ int main(int argc, char** argv) {
       if (rc == OFDIS_OK)
         rc = ofdis_track_advance(ctx, k0, k1, n + k0, im2, fs, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
       for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k) write_tracks(tpoints.data() + (size_t)k * tp.capacity, tcounts[k]);
+    }
+    // --stabilize: the runs of --tracks; a clip begins on its first image1, every run pushes its image2 frames with
+    // their --global-motion models
+    for (int k0 = 0, k1; k0 < n && stab_file && rc == OFDIS_OK; k0 = k1) {
+      for (k1 = k0 + 1; k1 < n && jobs[j0 + k1].a == jobs[j0 + k1 - 1].b;) ++k1;
+      const size_t fs = seq ? hwc : 2 * hwc;  // image1 of pair k at k * fs, its image2 one frame later
+      const uint8_t* im1 = frames.data() + (size_t)k0 * fs;
+      if (j0 + k0 == 0 || jobs[j0 + k0].a != jobs[j0 + k0 - 1].b) {
+        rc = stab_end();
+        if (rc == OFDIS_OK) rc = ofdis_stab_begin(ctx, &stp, stab_wts.data(), im1, w, h, OFDIS_MEM_HOST);
+        if (rc == OFDIS_OK) {
+          stab_live = true;
+          ++sclip;
+          sw = w;
+          sh = h;
+        }
+      }
+      if (rc != OFDIS_OK) break;
+      sbuf.resize((size_t)(k1 - k0) * hwc);
+      sinfo.resize(k1 - k0);
+      int count = 0;
+      rc = ofdis_stab_push(ctx, k1 - k0, gm_models.data() + (size_t)9 * k0, im1 + hwc, fs, sbuf.data(), sinfo.data(),
+                           &count, OFDIS_MEM_HOST);
+      if (rc == OFDIS_OK) write_stab(count);
     }
     if (rc == OFDIS_OK) rc = ofdis_sync(ctx);
     if (rc == OFDIS_OK && gtlist) {
@@ -1514,7 +1644,16 @@ int main(int argc, char** argv) {
     done += n;
   }
   end_clip();
+  if (stab_end() != OFDIS_OK) {
+    fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
+    ofdis_destroy(ctx);
+    return 1;
+  }
   if (ctx) ofdis_destroy(ctx);
+  if (stab_file && fclose(stab_file) != 0) {
+    fprintf(stderr, "error: cannot write %s\n", stab_txt.c_str());
+    return 1;
+  }
   if (tracks_file && fclose(tracks_file) != 0) {
     fprintf(stderr, "error: cannot write %s\n", tracks_path);
     return 1;

@@ -1254,15 +1254,182 @@ def _motion_pair(F, B, I1, p):
     residual = np.stack([rx, ry], -1).astype(f32)
     residual = np.where(np.isnan(residual), _QNAN, residual).astype(f32)
     mask = np.where(valid, np.where(close, 0, 1), 2).astype(np.uint8)
-    reg = None
-    if I1 is not None:
-        img = I1.reshape(h, w, -1).astype(f32)
-        with np.errstate(invalid="ignore"):
-            ins = (wq > 0) & (xw >= 0) & (xw <= f32(w - 1)) & (yw >= 0) & (yw <= f32(h - 1))
-        val = _bilinear_frame(img, np.where(ins, xw, f32(0)), np.where(ins, yw, f32(0)))
-        out = (np.fmin(np.fmax(val, f32(0)), f32(255)) + f32(0.5)).astype(np.uint8)
-        reg = np.where(ins[..., None], out, np.uint8(0)).reshape(I1.shape)
+    reg = None if I1 is None else _sample_u8(I1, wq, xw, yw)
     return M, st, mask, residual, reg
+
+
+def _sample_u8(I: np.ndarray, wq: np.ndarray, xw: np.ndarray, yw: np.ndarray) -> np.ndarray:
+    """The registered frames' rule: the 8-bit frame I (h, w[, noc]) at (xw, yw) (float32 (h, w)) by the bilinear byte
+    rule and its rounding where wq > 0 and the position lies in the frame, else 0."""
+    f32 = np.float32
+    h, w = wq.shape
+    img = I.reshape(h, w, -1).astype(f32)
+    with np.errstate(invalid="ignore"):
+        ins = (wq > 0) & (xw >= 0) & (xw <= f32(w - 1)) & (yw >= 0) & (yw <= f32(h - 1))
+    val = _bilinear_frame(img, np.where(ins, xw, f32(0)), np.where(ins, yw, f32(0)))
+    out = (np.fmin(np.fmax(val, f32(0)), f32(255)) + f32(0.5)).astype(np.uint8)
+    return np.where(ins[..., None], out, np.uint8(0)).reshape(I.shape)
+
+
+# ---- video stabilisation (ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish) ---------------------------------
+STAB_PARAM_FIELDS = ("radius", "crop", "limit")
+# ofdis_stab_frame, field for field (96 bytes)
+STAB_FRAME_DTYPE = np.dtype({"names": ["frame", "status", "lambda", "correction"],
+                             "formats": ["<i8", "<i4", "<f8", ("<f8", (9,))], "offsets": [0, 8, 16, 24],
+                             "itemsize": 96})
+_EYE = (1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0)
+
+
+def gaussian_weights(r: int, sigma: float | None = None) -> list:
+    """w_d = exp(-d*d / (2 sigma^2)) for d = 0 .. r; sigma^2 = r by default (OpenCV videostab's stdev sqrt(r))."""
+    s2 = float(r) if sigma is None else float(sigma) * float(sigma)
+    return [math.exp(-d * d / (2 * s2)) for d in range(int(r) + 1)]
+
+
+def _mat_mul(A, B):
+    return tuple((A[3 * i] * B[j] + A[3 * i + 1] * B[3 + j]) + A[3 * i + 2] * B[6 + j]
+                 for i in range(3) for j in range(3))
+
+
+def _mat_norm(A):
+    d = A[8]
+    if not (math.isfinite(d) and d != 0.0):
+        return None
+    R = tuple(v / d for v in A)
+    return R if all(math.isfinite(v) for v in R) else None
+
+
+def _mat_inv(a):
+    C = (a[4] * a[8] - a[5] * a[7], a[2] * a[7] - a[1] * a[8], a[1] * a[5] - a[2] * a[4],
+         a[5] * a[6] - a[3] * a[8], a[0] * a[8] - a[2] * a[6], a[2] * a[3] - a[0] * a[5],
+         a[3] * a[7] - a[4] * a[6], a[1] * a[6] - a[0] * a[7], a[0] * a[4] - a[1] * a[3])
+    return _mat_norm(C)
+
+
+def stab_model(m) -> tuple:
+    """A model as received: its 9 entries divided by m22, or the identity (m22 not finite and non-zero, a non-finite
+    entry, or m00*m11 - m01*m10 of the divided model not finite and non-zero)."""
+    m = [float(v) for v in np.asarray(m, np.float64).reshape(-1)]
+    d = m[8]
+    if not (math.isfinite(d) and d != 0.0):
+        return _EYE
+    q = tuple(v / d for v in m)
+    if not all(math.isfinite(v) for v in q):
+        return _EYE
+    a = q[0] * q[4] - q[1] * q[3]
+    return q if math.isfinite(a) and a != 0.0 else _EYE
+
+
+def stab_path(models, t: int, a: int, b: int, weights):
+    """S of frame t over the window [a, b] (9 floats), or None where the path is undefined.  models[k] is M_k as
+    received (stab_model) for k in [a, b-1]; any mapping of those indices will do."""
+    w0 = float(weights[0])
+    acc = [w0 if i % 4 == 0 else 0.0 for i in range(9)]
+    wsum = w0
+    for sign in (1, -1):
+        P = _EYE
+        for d in range(1, (b - t if sign > 0 else t - a) + 1):
+            if sign > 0:
+                P = _mat_norm(_mat_mul(models[t + d - 1], P))
+            else:
+                Q = _mat_inv(models[t - d])
+                P = None if Q is None else _mat_norm(_mat_mul(Q, P))
+            if P is None:
+                return None
+            wd = float(weights[d])
+            acc = [acc[i] + wd * P[i] for i in range(9)]
+            wsum = wsum + wd
+    S = tuple(v / wsum for v in acc)
+    return S if all(math.isfinite(v) for v in S) else None
+
+
+def _stab_map(S, lam, crop, w, h):
+    """(S(lam), A(lam) rounded to float32 or None)."""
+    SL = tuple((1.0 - lam) + lam * S[i] if i % 4 == 0 else lam * S[i] for i in range(9))
+    s = 1.0 - 2.0 * float(np.float32(crop))
+    cx, cy = 0.5 * float(w - 1), 0.5 * float(h - 1)
+    Si = _mat_inv(SL)
+    A = None if Si is None else _mat_norm(_mat_mul(Si, (s, 0.0, cx * (1.0 - s), 0.0, s, cy * (1.0 - s), 0.0, 0.0, 1.0)))
+    return SL, None if A is None else np.array(A).astype(np.float32)
+
+
+def _stab_project(a, X, Y):
+    """(wq, mx/wq, my/wq) of the per-pixel rule, float32."""
+    with np.errstate(all="ignore"):
+        mx = (a[0] * X + a[1] * Y) + a[2]
+        my = (a[3] * X + a[4] * Y) + a[5]
+        wq = (a[6] * X + a[7] * Y) + a[8]
+        return wq, mx / wq, my / wq
+
+
+def stab_correction(S, params, w: int, h: int):
+    """The crop and limit of frame t's S (None: an undefined path): (status, lambda, S(lambda) (9 floats), a0..a8
+    (9,) float32)."""
+    f32 = np.float32
+    crop, limit = params["crop"], int(params["limit"])
+    X = np.array([0, w - 1, 0, w - 1], f32)
+    Y = np.array([0, 0, h - 1, h - 1], f32)
+
+    def passes(lam):
+        SL, a = _stab_map(S, lam, crop, w, h)
+        if a is None:
+            return False
+        wq, xw, yw = _stab_project(a, X, Y)
+        with np.errstate(invalid="ignore"):
+            return bool(((wq > 0) & (xw >= 0) & (xw <= f32(w - 1)) & (yw >= 0) & (yw <= f32(h - 1))).all())
+
+    if S is not None:
+        lam = 1.0
+        if limit and not passes(1.0):
+            lo, hi = 0.0, 1.0
+            for _ in range(20):
+                mid = 0.5 * (lo + hi)
+                if passes(mid):
+                    lo = mid
+                else:
+                    hi = mid
+            lam = lo
+        SL, a = _stab_map(S, lam, crop, w, h)
+        if a is not None:
+            return 0, lam, SL, a
+    SL, a = _stab_map(_EYE, 0.0, crop, w, h)
+    return 1, 0.0, SL, a
+
+
+def stab_warp(frame: np.ndarray, a: np.ndarray) -> np.ndarray:
+    """The stabilised bytes of one frame (h, w[, noc]) under a0..a8."""
+    h, w = frame.shape[:2]
+    X = np.arange(w, dtype=np.float32)[None, :]
+    Y = np.arange(h, dtype=np.float32)[:, None]
+    wq, xw, yw = _stab_project(a, X, Y)
+    return _sample_u8(frame, wq, xw, yw)
+
+
+def stab_params(params) -> dict:
+    return {k: params[k] for k in STAB_PARAM_FIELDS}
+
+
+def stabilize(frames: np.ndarray, models: np.ndarray, params, weights):
+    """ofdis_stab_begin on frames[0], pushes of the others and ofdis_stab_finish, bit for bit, however the clip is cut
+    into pushes: float64 path, float32 warp, without contraction.  frames (N, h, w[, noc]) uint8, models (N-1, 3, 3)
+    (model k maps frame k to frame k+1, as ofdis_global_motion_fullres returns it), params a mapping with
+    STAB_PARAM_FIELDS, weights r+1 floats.  Returns (stabilised frames (N, h, w[, noc]) uint8, records (N,) of
+    STAB_FRAME_DTYPE)."""
+    p = stab_params(params)
+    frames = np.asarray(frames, np.uint8)
+    n = frames.shape[0]
+    h, w = frames.shape[1:3]
+    r = int(p["radius"])
+    M = [stab_model(m) for m in np.asarray(models, np.float64).reshape(-1, 9)]
+    assert len(M) == n - 1
+    out = np.empty_like(frames)
+    info = np.zeros(n, STAB_FRAME_DTYPE)
+    for t in range(n):
+        S = stab_path(M, t, max(0, t - r), min(n - 1, t + r), weights)
+        status, lam, SL, a = stab_correction(S, p, w, h)
+        out[t] = stab_warp(frames[t], a)
+        info[t] = (t, status, lam, SL)
+    return out, info
 
 
 def global_motion(F: np.ndarray, B: np.ndarray | None, frames1: np.ndarray | None, params):

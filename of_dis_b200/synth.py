@@ -152,3 +152,36 @@ def global_motion_clip(n: int, h: int, w: int, channels: int = 1, seed: int = 0,
         masks.append(inside)
         Hinv = Hinv @ Hi
     return np.ascontiguousarray(np.stack(frames)), np.repeat(H[None], n, 0), np.stack(masks[:n])
+
+
+def shaky_clip(n: int, h: int, w: int, channels: int = 1, seed: int = 0, pan=(1.0, 0.0), jitter: float = 2.0):
+    """A clip of n uint8 frames filmed by a camera that pans by `pan` = (dx, dy) pixels per frame and shakes at random
+    about that path: frame t shows the canvas of _canvas through the pose C_t = J_t P_t, P_t the shift by t * pan and
+    J_t a random rotation (up to jitter / 4 degrees) about the frame's centre plus a random shift of up to `jitter`
+    pixels in x and y, i.e. frame t is the canvas sampled at C_t^-1 x (cubic).  Returns (frames, models, smooth):
+    frames (n, h, w[, 3]), models (n - 1, 3, 3) float64, model t = C_{t+1} C_t^-1 mapping a pixel of frame t to its
+    position in frame t + 1, and smooth (n, 3, 3) the corrections P_t C_t^-1 = J_t^-1 that move frame t onto the
+    shake-free path."""
+    from scipy import ndimage
+
+    rng = np.random.default_rng(seed + 7)
+    bg, m = _canvas(h, w, channels, seed)
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    poses, frames = [], []
+    for t in range(n):
+        J = similarity_about_centre(h, w, rng.uniform(-0.25, 0.25) * jitter, 1.0,
+                                    (rng.uniform(-1, 1) * jitter, rng.uniform(-1, 1) * jitter))
+        P = np.array([[1.0, 0.0, t * pan[0]], [0.0, 1.0, t * pan[1]], [0.0, 0.0, 1.0]])
+        C = J @ P
+        Ci = np.linalg.inv(C)
+        sx = Ci[0, 0] * xx + Ci[0, 1] * yy + Ci[0, 2]
+        sy = Ci[1, 0] * xx + Ci[1, 1] * yy + Ci[1, 2]
+        img = np.empty((h, w, channels))
+        for c in range(channels):
+            img[..., c] = ndimage.map_coordinates(bg[..., c], [sy + m, sx + m], order=3, mode="nearest")
+        q = np.clip(np.rint(img), 0, 255).astype(np.uint8)
+        frames.append(q[..., 0] if channels == 1 else q)
+        poses.append((C, J))
+    models = np.stack([poses[t + 1][0] @ np.linalg.inv(poses[t][0]) for t in range(n - 1)])
+    smooth = np.stack([np.linalg.inv(J) for _, J in poses])
+    return np.ascontiguousarray(np.stack(frames)), models, smooth
