@@ -548,6 +548,98 @@ int ofdis_track_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned c
  * first ofdis_track_begin or with a NULL out. */
 int ofdis_track_stats_get(const ofdis_ctx* ctx, ofdis_track_stats* out);
 
+/* Trajectory descriptors (extension): the single-scale pipeline of Wang and Schmid's improved dense trajectories
+ * ("Action recognition with improved trajectories", ICCV 2013) on the tracker above.  The tracks are the tracker's,
+ * bit for bit (the raw flow F moves them); the descriptors describe the camera-compensated residual flow R.  The
+ * context owns one descriptor stage on top of its tracker; ofdis_traj_begin starts both, ofdis_track_begin and
+ * ofdis_track_advance end it.  Float32 without contraction, IEEE division and square root, every sum from +0.0f in
+ * the order given; preprocess.traj_descriptors restates it bit for bit.  W = width_org, H = height_org.
+ *   Segments.  A track seeded at frame b (counted from ofdis_traj_begin's frame, 0) emits one descriptor per complete
+ *   segment [b + (j-1)L, b + jL], j = 1, 2, ...: L + 1 positions p_0..p_L, L steps, and the frame histograms of its L
+ *   source frames.  The next segment starts at the last point of the previous one; a track that ends partway through
+ *   a segment discards it.
+ *   Residual flow of pair k.  models[k] (9 float64, ofdis_global_motion_fullres's model) goes through the
+ *   stabiliser's validity rule (divided by m22, or the identity; ofdis_stab_push), then each entry is rounded to
+ *   float32: m0..m8; models == NULL is the identity (R = F).  F = slot f0+k's full-resolution flow (exactly what
+ *   ofdis_get_flow_fullres returns).  At pixel (X, Y): mx = (m0*X + m1*Y) + m2, my = (m3*X + m4*Y) + m5,
+ *   wq = (m6*X + m7*Y) + m8, R = (u - (mx/wq - X), v - (my/wq - Y)).  R is unknown where |u| > 1e9, |v| > 1e9 or
+ *   either is NaN (F unknown), where wq is not > 0, or where a component of R is not finite.
+ *   Vector fields of source frame k (pair k's I0: ofdis_traj_begin's frame, then the previous pair's target frame).
+ *   Central differences are clamped: dx(f)(X, Y) = (f(min(X+1, W-1), Y) - f(max(X-1, 0), Y)) * 0.5f, dy the same in y.
+ *     HOG:  (dx(g), dy(g)) of the tracker's brightness g.
+ *     HOF:  R; unknown where R is.
+ *     MBHx: (dx(R_u), dy(R_u)); MBHy: (dx(R_v), dy(R_v)); unknown where R is unknown at one of the four neighbours.
+ *   Orientation bins of a vector (a, b).  mag = sqrtf(a*a + b*b); an unknown vector or a non-finite mag gives no
+ *   bin.  angle = atan2_f32(b, a) (the color wheel's polynomial, preprocess.atan2_f32); angle < 0: angle + 6.2831855f;
+ *   fbin = angle * 1.2732395f (8 / 2pi); bin0 = floorf(fbin), 8 wraps to 0; bin1 = (bin0 + 1) % 8;
+ *   mag1 = (fbin - floorf(fbin)) * mag, mag0 = mag - mag1.  HOF with mag <= min_flow: weight 1 into its zero bin 8
+ *   instead (HOF has 9 bins, the others 8).
+ *   Frame histogram of a track at its position (x, y) before pair k's advance.  (xr, yr) = ((int)floorf(x + 0.5f),
+ *   (int)floorf(y + 0.5f)); the N x N patch at ox = min(max(xr - N/2, 0), W - N), oy the same with H; ns x ns cells of
+ *   c = N/ns pixels.  In cell (cx, cy) a bin's sum runs over the cell's pixels q = py*c + px (row-major): q mod 32 = l
+ *   gives lane l, which sums its pixels in increasing q (mag0 into bin0, mag1 into bin1, for HOG, HOF, MBHx, MBHy);
+ *   the cell's sum is lane 0's + lane 1's + ... + lane 31's, and v = sum + eps.  Each descriptor's entries, in the
+ *   order (cx, cy, bin), sum to s = v_0 + v_1 + ...; each becomes sqrtf(v / s) (RootSIFT).
+ *   Temporal cells: step i of the segment (0 .. L-1) adds its frame histograms to cell i / (L/nt), in step order;
+ *   the descriptor holds that sum / (float)(L/nt).
+ *   Tests of a completed segment, in order, each counted in its counter: with n = (float)(L+1), mean_x = (x_0 + ...
+ *   + x_L) / n, sd_x = sqrtf(((x_0 - mean_x)^2 + ... ) / n), the same in y; *static* if sd_x < min_var and sd_y <
+ *   min_var; *erratic* if sd_x > max_var or sd_y > max_var; with steps s_i = |p_{i+1} - p_i|, length = s_0 + ... +
+ *   s_{L-1} and smax their largest, *jump* if smax > max_dis and smax > 0.7f*length; with d_i = R at (xr, yr) of p_i
+ *   (the step's source pixel), *camera* if any d_i is unknown or not finite in magnitude |d_i| = sqrtf(du*du + dv*dv),
+ *   or max |d_i| <= min_disp (the track moves with the camera).  Otherwise the segment is emitted.
+ *   Descriptor (dim = 2L + ns*ns*nt*33 floats; 426 with the defaults): the shape d_i / (|d_0| + ... + |d_{L-1}|) as
+ *   (du_0, dv_0, du_1, ...), then HOG [nt][ns][ns][8], HOF [nt][ns][ns][9], MBHx and MBHy [nt][ns][ns][8], the
+ *   temporal cell outermost, then the x cell, the y cell and the bin.
+ *   Order and bound.  Segments are emitted pair by pair, within a pair in list order (id order).  Each takes L (track,
+ *   pair) incidences: at most n*capacity fall in a call of n pairs and at most (L-1)*capacity come from before it, so a
+ *   call emits at most capacity * ceil((n + L - 1) / L) segments (the caller's output size).
+ *   Wang and Schmid use L 15, nt 3, N 32, ns 2, min_flow 0.4, eps 0.05, min_disp 1 (their camera test in pixels at
+ *   full resolution), min_var sqrt(3), max_var 50 and max_dis 20. */
+typedef struct ofdis_traj_params {
+  int L;             /* steps per segment, 1 .. 64, a multiple of nt */
+  int nt;            /* temporal cells, >= 1 */
+  int N;             /* patch side, a multiple of ns, at most min(W, H) */
+  int ns;            /* spatial cells per side, 1 .. 4 */
+  float min_flow;    /* HOF's zero-bin magnitude; finite */
+  float eps;         /* added to every bin sum; finite and > 0 */
+  float min_disp;    /* the camera test; finite and >= 0 */
+  float min_var, max_var, max_dis;  /* the static, erratic and jump tests; finite */
+} ofdis_traj_params;
+typedef struct ofdis_traj_record {
+  int id;            /* the track's id */
+  int start;         /* the segment's first frame, counted from ofdis_traj_begin's frame */
+  float mean_x, mean_y, sd_x, sd_y, length;
+} ofdis_traj_record;  /* 28 bytes */
+typedef struct ofdis_traj_stats {
+  long long emitted, rejected_static, rejected_erratic, rejected_jump, rejected_camera;  /* since ofdis_traj_begin */
+} ofdis_traj_stats;
+/* ofdis_track_begin (same arguments, outputs and errors) followed by a reset of the descriptor stage, which keeps a
+ * device copy of `frame`: pair 0's source frame.  Flow contexts only.  Allocates the descriptor workspace -- per track
+ * slot and list (two lists): (2(L+1) + 2L + nt*ns*ns*33 floats rounded up to 16 bytes) + 8 bytes of state, per slot
+ * 40 bytes of scan state, per pixel 44 bytes of fields, one frame, and the records and descriptors of max_frames pairs
+ * for host outputs (capacity * ceil((max_frames + L - 1) / L) * (28 + 4*dim) bytes) -- which grows, never shrinks and
+ * is freed by ofdis_destroy.  The batch command's tracker settings (1024 x 436 gray, capacity 4 x 7040 cells, 64
+ * frames) with the defaults: about 420 MB, of which 106 MB the per-track state, 20 MB the fields and 293 MB the host
+ * outputs.  A NULL or out-of-range traj, or a stereo context, is OFDIS_ERR_ARG. */
+int ofdis_traj_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const ofdis_traj_params* traj,
+                     const unsigned char* frame, ofdis_track_point* points, int* count, int width_org, int height_org,
+                     int memkind);
+/* ofdis_track_advance (same frames, slots, outputs and errors) with the descriptors of every pair: the source frame of
+ * pair 0 is the kept frame, of pair k >= 1 frames + (k-1)*frame_stride; the last target frame is kept for the next
+ * call.  models: [f1-f0][9] float64 in host memory, or NULL.  The emitted segments' records go to records and their
+ * descriptors to desc ([bound][dim] floats), bound = capacity * ceil((f1-f0 + L - 1) / L), both in memkind; pair k's
+ * count goes to n_desc[k] (host).  Per pair 5 launches beyond the tracker's 5; no host round trip between pairs; one
+ * synchronise at the end (host outputs: a second one after their copies).  A call before ofdis_traj_begin or after an
+ * ofdis_track_begin or ofdis_track_advance, NULL records, desc or n_desc, or device outputs not 4-byte aligned is
+ * OFDIS_ERR_ARG.  A call that fails on the way leaves the stage to a new ofdis_traj_begin. */
+int ofdis_traj_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames, size_t frame_stride,
+                       const double* models, ofdis_track_point* points, int* counts, ofdis_traj_record* records,
+                       float* desc, int* n_desc, int width_org, int height_org, int memkind);
+/* The descriptor stage's counters since ofdis_traj_begin (synchronises the context's stream); OFDIS_ERR_ARG without a
+ * live stage or with a NULL out. */
+int ofdis_traj_stats_get(const ofdis_ctx* ctx, ofdis_traj_stats* out);
+
 /* Video stabilisation (extension): a Gaussian-smoothed camera path streamed through a clip, from the per-pair models
  * of ofdis_global_motion_fullres, and every frame warped onto it on the device (the motion filter of Matsushita et al.,
  * "Full-frame video stabilization", CVPR 2005, and of OpenCV's videostab).  The context owns one stabiliser: the

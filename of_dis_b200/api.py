@@ -16,7 +16,8 @@ import numpy as np
 from .params import CParams, DisParams
 from .preprocess import (DISP_FILTER_FIELDS, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, STAB_FRAME_DTYPE,
                          STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE,
-                         TRACK_STATS_FIELDS, gaussian_weights, motion_params)
+                         TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
+                         gaussian_weights, motion_params, traj_bound, traj_dim)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("OFDIS_LIB") or os.path.join(_HERE, "lib", "libofdis_b200.so")  # OFDIS_LIB: experiments only
@@ -40,6 +41,7 @@ EXPORTS = [
     "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres", "ofdis_interpolate_fullres",
     "ofdis_track_begin", "ofdis_track_advance", "ofdis_track_stats_get", "ofdis_disparity_fullres",
     "ofdis_global_motion_fullres", "ofdis_stab_begin", "ofdis_stab_push", "ofdis_stab_finish",
+    "ofdis_traj_begin", "ofdis_traj_advance", "ofdis_traj_stats_get",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -116,6 +118,16 @@ assert tuple(k for k, _ in StabParams._fields_) == STAB_PARAM_FIELDS
 assert ctypes.sizeof(StabFrame) == STAB_FRAME_DTYPE.itemsize
 
 
+class TrajParams(ctypes.Structure):
+    """ofdis_traj_params (include/ofdis_b200.h)."""
+    _fields_ = [(k, ctypes.c_int) for k in TRAJ_PARAM_FIELDS[:4]] + [(k, ctypes.c_float) for k in TRAJ_PARAM_FIELDS[4:]]
+
+
+class TrajStats(ctypes.Structure):
+    """ofdis_traj_stats (include/ofdis_b200.h)."""
+    _fields_ = [(k, ctypes.c_longlong) for k in TRAJ_STATS_FIELDS]
+
+
 class OfdisError(RuntimeError):
     pass
 
@@ -180,6 +192,11 @@ def lib():
         L.ofdis_global_motion_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
             [ctypes.POINTER(MotionParams), ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 5 + [ctypes.c_int] * 3
         L.ofdis_track_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackStats)]
+        L.ofdis_traj_begin.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackParams), ctypes.POINTER(TrajParams)] + \
+            [ctypes.c_void_p] * 3 + [ctypes.c_int] * 3
+        L.ofdis_traj_advance.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p, ctypes.c_size_t] + \
+            [ctypes.c_void_p] * 6 + [ctypes.c_int] * 3
+        L.ofdis_traj_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrajStats)]
         L.ofdis_stab_begin.argtypes = [ctypes.c_void_p, ctypes.POINTER(StabParams)] + [ctypes.c_void_p] * 2 + \
             [ctypes.c_int] * 3
         L.ofdis_stab_push.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 2 + [ctypes.c_size_t] + \
@@ -655,6 +672,75 @@ class Context:
         if rc != 0:
             raise OfdisError("track_stats: status %d" % rc)
         return {k: int(getattr(st, k)) for k in TRACK_STATS_FIELDS}
+
+    def traj_begin(self, track_params, traj_params, frame, width_org, height_org, memkind=MEM_HOST, points=None):
+        """Resets the context's tracker and its descriptor stage and seeds `frame` (ofdis_traj_begin;
+        preprocess.traj_descriptors restates the whole stage).  track_params as track_begin's; traj_params a mapping
+        with the keys of preprocess.TRAJ_PARAM_FIELDS (or a TrajParams).  Returns what track_begin returns."""
+        if not isinstance(track_params, TrackParams):
+            track_params = TrackParams(*[track_params[k] for k in TRACK_PARAM_FIELDS])
+        if not isinstance(traj_params, TrajParams):
+            traj_params = TrajParams(*[traj_params[k] for k in TRAJ_PARAM_FIELDS])
+        count = ctypes.c_int(0)
+        if memkind == MEM_HOST:
+            self._frames_u8("traj_begin: frame", np.asarray(frame)[None], 1, width_org, height_org)
+            frame = np.ascontiguousarray(frame)
+            points = np.empty(max(track_params.capacity, 0), TRACK_POINT_DTYPE)
+        self._ck(lib().ofdis_traj_begin(self._h, ctypes.byref(track_params), ctypes.byref(traj_params), _ptr(frame),
+                                        _ptr(points), ctypes.byref(count), width_org, height_org, memkind))
+        # only a stage the library accepted sizes the host outputs of traj_advance: a refused begin leaves the
+        # previous stage, and its parameters, live
+        self._track_capacity = track_params.capacity
+        self._traj = {k: getattr(traj_params, k) for k in TRAJ_PARAM_FIELDS}
+        return points[:count.value].copy() if memkind == MEM_HOST else count.value
+
+    def traj_advance(self, f0, f1, b0, frames, width_org, height_org, models=None, frame_stride=None,
+                     memkind=MEM_HOST, points=None, records=None, desc=None):
+        """track_advance with the descriptors of every pair (ofdis_traj_advance).  models: None (no compensation) or
+        (f1-f0, 9) float64 as global_motion_fullres returns them, always on the host.  Host: returns (lists, records,
+        desc, n_desc) -- the tracker's lists, the emitted segments' TRAJ_RECORD_DTYPE records and (count, dim) float32
+        descriptors, and the int32 segments per pair.  With memkind=MEM_DEVICE frames, points, records and desc are
+        device addresses the caller owns (records and desc: preprocess.traj_bound(capacity, f1-f0, L) entries) and
+        (counts, n_desc) is returned."""
+        n = max(f1 - f0, 0)
+        cap = getattr(self, "_track_capacity", 0)
+        tp = getattr(self, "_traj", None)
+        L = tp["L"] if tp else 1
+        dim = traj_dim(tp) if tp else 0
+        bound = traj_bound(cap, n, L)
+        counts = np.zeros(n, np.int32)
+        n_desc = np.zeros(n, np.int32)
+        pm = None
+        if models is not None:
+            pm = np.ascontiguousarray(models, np.float64)
+            if pm.shape != (n, 9) and pm.shape != (n, 3, 3):
+                raise ValueError("traj_advance: models must be (%d, 9) float64" % n)
+        if memkind == MEM_HOST:
+            frame_stride = self._frames_u8("traj_advance: frames", frames, n, width_org, height_org)
+            points = np.empty(n * cap, TRACK_POINT_DTYPE)
+            records = np.empty(bound, TRAJ_RECORD_DTYPE)
+            desc = np.empty((bound, dim), np.float32)
+            pf = frames.ctypes.data
+        else:
+            frame_stride = height_org * width_org * self.prm.noc if frame_stride is None else frame_stride
+            pf = frames
+        self._ck(lib().ofdis_traj_advance(self._h, f0, f1, b0, _ptr(pf), frame_stride, _ptr(pm), _ptr(points),
+                                          _ptr(counts), _ptr(records), _ptr(desc), _ptr(n_desc), width_org,
+                                          height_org, memkind))
+        if memkind != MEM_HOST:
+            return counts, n_desc
+        total = int(n_desc.sum())
+        lists = [points[k * cap:k * cap + counts[k]].copy() for k in range(n)]
+        return lists, records[:total].copy(), desc[:total].copy(), n_desc
+
+    def traj_stats(self):
+        """The descriptor stage's counters since traj_begin (ofdis_traj_stats_get): a dict of
+        preprocess.TRAJ_STATS_FIELDS."""
+        st = TrajStats()
+        rc = lib().ofdis_traj_stats_get(self._h, ctypes.byref(st))
+        if rc != 0:
+            raise OfdisError("traj_stats: status %d" % rc)
+        return {k: int(getattr(st, k)) for k in TRAJ_STATS_FIELDS}
 
     def stab_begin(self, params, frame0, width_org, height_org, weights=None, memkind=MEM_HOST):
         """Resets the context's stabiliser on frame 0 (ofdis_stab_begin; preprocess.stabilize restates the whole clip).

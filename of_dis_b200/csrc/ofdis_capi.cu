@@ -84,6 +84,17 @@ struct ofdis_ctx {
   TrackGeom tgeom{};
   int track_cur = 0;
   bool track_on = false;
+  // the descriptor stage of ofdis_traj_begin / ofdis_traj_advance on top of the tracker: its workspace (TrajWork, then
+  // the host-output records and descriptors of max_frames pairs), the geometry of the last begin and the frames seen
+  // since it; ended by ofdis_track_begin and ofdis_track_advance; never touched by ofdis_run
+  void* d_traj = nullptr;
+  size_t traj_bytes = 0;
+  TrajWork traj{};
+  TrajGeom trgeom{};
+  ofdis_traj_record* traj_rec = nullptr;
+  float* traj_desc = nullptr;
+  int traj_frame = 0;
+  bool traj_on = false;
   // lazily allocated workspace of ofdis_disparity_fullres (DispWork for max_frames pairs of width x height pixels);
   // never touched by ofdis_run
   void* d_disp = nullptr;
@@ -471,6 +482,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_track);
   cudaFree(ctx->d_disp);
   cudaFree(ctx->d_motion);
+  cudaFree(ctx->d_traj);
   cudaFree(ctx->d_stab);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
@@ -1343,6 +1355,7 @@ int ofdis_track_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const un
   NvtxRange nvtx("track", -1);
   CK(cudaSetDevice(ctx->device));
   ctx->track_on = false;
+  ctx->traj_on = false;
   TrackGeom t{};
   t.w = width_org;
   t.h = height_org;
@@ -1397,6 +1410,7 @@ int ofdis_track_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned c
       !points || !counts || (memkind == OFDIS_MEM_DEVICE && reinterpret_cast<uintptr_t>(points) % 4))
     return fail(ctx, OFDIS_ERR_ARG, "track_advance: bad argument");
   if (!ctx->track_on) return fail(ctx, OFDIS_ERR_ARG, "track_advance: no ofdis_track_begin");
+  ctx->traj_on = false;
   int cx, cy;
   int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
   if (rc) return rc;
@@ -1460,6 +1474,234 @@ int ofdis_track_stats_get(const ofdis_ctx* ctx, ofdis_track_stats* out) {
   out->dropped = (long long)s.dropped;
   out->alive = s.alive;
   out->next_id = s.next_id;
+  return OFDIS_OK;
+}
+
+// A received model through the stabiliser's validity rule (stab_kernels.cu): divided by its m22 into q, which stays
+// as it is (the identity) when m22 is not finite and non-zero, an entry is not finite or m00*m11 - m01*m10 is not
+// finite and non-zero
+static void stab_valid_model(const double* m, double* q) {
+  const double d = m[8];
+  double M[9];
+  bool ok = std::isfinite(d) && d != 0.0;
+  for (int i = 0; i < 9; ++i) {
+    M[i] = m[i] / d;
+    ok = ok && std::isfinite(M[i]);
+  }
+  if (ok) {
+    const double a = M[0] * M[4] - M[1] * M[3];
+    ok = std::isfinite(a) && a != 0.0;
+  }
+  if (ok) std::memcpy(q, M, sizeof(M));
+}
+
+// The bound of the segments a call of n pairs emits (ofdis_traj_advance's header)
+static size_t traj_bound(const TrajGeom& tg, int capacity, int n) {
+  return (size_t)capacity * (size_t)((n + tg.L - 1 + tg.L - 1) / tg.L);
+}
+
+// The descriptor stage's workspace for tracker geometry t and descriptor geometry tg: the state, two state lists and
+// their metadata, the per-slot scan arrays, the per-pixel fields, the models of max_frames pairs, the kept frame,
+// then the host-output records and descriptors of max_frames pairs.  Grows, never shrinks.
+static int ensure_traj(ofdis_ctx* ctx, const TrackGeom& t, const TrajGeom& tg) {
+  const size_t cp = (size_t)t.cap_pad, px = (size_t)tg.w * tg.h, nb = cp / TRACK_BLOCK;
+  const size_t bound = traj_bound(tg, t.capacity, ctx->max_frames);
+  const size_t part[14] = {align16(sizeof(TrajState)), sizeof(float) * tg.ss * cp, sizeof(float) * tg.ss * cp,
+                           sizeof(int2) * cp, sizeof(int2) * cp, align16(sizeof(uchar4) * px),
+                           sizeof(float4) * 2 * px, align16(sizeof(float2) * px),
+                           align16(sizeof(float) * 9 * ctx->max_frames),
+                           align16(sizeof(int) * cp), align16(sizeof(int) * cp), align16(sizeof(TrajSeg) * cp),
+                           align16(sizeof(unsigned int) * nb), align16(sizeof(int) * ctx->max_frames)};
+  const size_t frame = align16(px * ctx->prm.noc), rec = align16(sizeof(ofdis_traj_record) * bound);
+  size_t bytes = frame + rec + sizeof(float) * tg.dim * bound;
+  for (size_t p : part) bytes += p;
+  if (bytes > ctx->traj_bytes) {
+    CK(cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_traj);
+    ctx->d_traj = nullptr;
+    ctx->traj_bytes = 0;
+    if (cudaMalloc(&ctx->d_traj, bytes) != cudaSuccess) {
+      ctx->d_traj = nullptr;
+      return fail(ctx, OFDIS_ERR_NOMEM, "traj workspace");
+    }
+    ctx->traj_bytes = bytes;
+  }
+  char* b = static_cast<char*>(ctx->d_traj);
+  TrajWork& tw = ctx->traj;
+  auto take = [&b](size_t n) { char* r = b; b += n; return r; };
+  tw.state = reinterpret_cast<TrajState*>(take(part[0]));
+  tw.st[0] = reinterpret_cast<float*>(take(part[1]));
+  tw.st[1] = reinterpret_cast<float*>(take(part[2]));
+  tw.meta[0] = reinterpret_cast<int2*>(take(part[3]));
+  tw.meta[1] = reinterpret_cast<int2*>(take(part[4]));
+  tw.bins = reinterpret_cast<uchar4*>(take(part[5]));
+  tw.mag = reinterpret_cast<float4*>(take(part[6]));
+  tw.res = reinterpret_cast<float2*>(take(part[7]));
+  tw.models = reinterpret_cast<float*>(take(part[8]));
+  tw.dst = reinterpret_cast<int*>(take(part[9]));
+  tw.eoff = reinterpret_cast<int*>(take(part[10]));
+  tw.seg = reinterpret_cast<TrajSeg*>(take(part[11]));
+  tw.ebsum = reinterpret_cast<unsigned int*>(take(part[12]));
+  tw.ndesc = reinterpret_cast<int*>(take(part[13]));
+  tw.frame = reinterpret_cast<unsigned char*>(take(frame));
+  ctx->traj_rec = reinterpret_cast<ofdis_traj_record*>(take(rec));
+  ctx->traj_desc = reinterpret_cast<float*>(b);
+  return OFDIS_OK;
+}
+
+int ofdis_traj_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const ofdis_traj_params* traj,
+                     const unsigned char* frame, ofdis_track_point* points, int* count, int width_org, int height_org,
+                     int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  auto finite = [](float v) { return std::isfinite(v); };
+  if (ctx->nop != 2 || !traj || traj->L < 1 || traj->L > 64 || traj->nt < 1 || traj->L % traj->nt ||
+      traj->ns < 1 || traj->ns > TRAJ_MAX_NS || traj->N < 1 || traj->N % traj->ns ||
+      traj->N > std::min(width_org, height_org) || !finite(traj->min_flow) || !finite(traj->eps) ||
+      !(traj->eps > 0.f) || !finite(traj->min_disp) || !(traj->min_disp >= 0.f) || !finite(traj->min_var) ||
+      !finite(traj->max_var) || !finite(traj->max_dis))
+    return fail(ctx, OFDIS_ERR_ARG, "traj_begin: bad argument");
+  int rc = ofdis_track_begin(ctx, params, frame, points, count, width_org, height_org, memkind);
+  if (rc) return rc;
+  NvtxRange nvtx("traj", -1);
+  TrajGeom tg{};
+  tg.w = width_org;
+  tg.h = height_org;
+  tg.L = traj->L;
+  tg.nt = traj->nt;
+  tg.N = traj->N;
+  tg.ns = traj->ns;
+  tg.c = traj->N / traj->ns;
+  tg.tl = traj->L / traj->nt;
+  tg.pos = 2 * (tg.L + 1);
+  tg.dis = 2 * tg.L;
+  tg.nacc = tg.nt * tg.ns * tg.ns * TRAJ_BINS;
+  tg.ss = (tg.pos + tg.dis + tg.nacc + 3) / 4 * 4;
+  tg.dim = tg.dis + tg.nacc;
+  tg.min_flow = traj->min_flow;
+  tg.eps = traj->eps;
+  tg.min_disp = traj->min_disp;
+  tg.min_var = traj->min_var;
+  tg.max_var = traj->max_var;
+  tg.max_dis = traj->max_dis;
+  const TrackGeom& t = ctx->tgeom;
+  rc = ensure_traj(ctx, t, tg);
+  if (rc) return rc;
+  ctx->trgeom = tg;
+  const TrajWork& tw = ctx->traj;
+  const size_t hwc = (size_t)width_org * height_org * ctx->prm.noc;
+  // frame 0's tracks start their first segment at frame 0; track_begin staged a host frame in d_stage
+  CK(cudaMemsetAsync(tw.state, 0, sizeof(TrajState), ctx->stream));
+  CK(cudaMemsetAsync(tw.meta[ctx->track_cur], 0, sizeof(int2) * t.cap_pad, ctx->stream));
+  CK(cudaMemcpyAsync(tw.frame, memkind == OFDIS_MEM_DEVICE ? frame : static_cast<const unsigned char*>(ctx->d_stage),
+                     hwc, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->traj_frame = 0;
+  ctx->traj_on = true;
+  return OFDIS_OK;
+}
+
+int ofdis_traj_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames, size_t frame_stride,
+                       const double* models, ofdis_track_point* points, int* counts, ofdis_traj_record* records,
+                       float* desc, int* n_desc, int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (ctx->nop != 2 || f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || b0 < 0 || b0 > ctx->max_frames - (f1 - f0) ||
+      !frames || !points || !counts || !records || !desc || !n_desc ||
+      (memkind == OFDIS_MEM_DEVICE && (reinterpret_cast<uintptr_t>(points) % 4 ||
+                                       reinterpret_cast<uintptr_t>(records) % 4 ||
+                                       reinterpret_cast<uintptr_t>(desc) % 4)))
+    return fail(ctx, OFDIS_ERR_ARG, "traj_advance: bad argument");
+  if (!ctx->traj_on || !ctx->track_on) return fail(ctx, OFDIS_ERR_ARG, "traj_advance: no ofdis_traj_begin");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  const TrackGeom& t = ctx->tgeom;
+  const TrajGeom& tg = ctx->trgeom;
+  if (width_org != t.w || height_org != t.h)
+    return fail(ctx, OFDIS_ERR_ARG, "traj_advance: frame size differs from ofdis_traj_begin's");
+  const size_t hwc = (size_t)width_org * height_org * ctx->prm.noc;
+  if (frame_stride < hwc) return fail(ctx, OFDIS_ERR_ARG, "traj_advance: frame_stride below one frame");
+  NvtxRange nvtx("traj", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0, D = ctx->dirs;
+  // the models through the stabiliser's validity rule, rounded to float32 (models == NULL: the identity)
+  std::vector<float> m32(9 * (size_t)n);
+  for (int k = 0; k < n; ++k) {
+    double q[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    if (models) stab_valid_model(models + 9 * (size_t)k, q);
+    for (int i = 0; i < 9; ++i) m32[9 * (size_t)k + i] = (float)q[i];
+  }
+  const TrackWork& ws = ctx->track;
+  const TrajWork& tw = ctx->traj;
+  const unsigned char* src = frames;
+  size_t stride = frame_stride;
+  if (memkind != OFDIS_MEM_DEVICE) {
+    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    CK(cudaMemcpy2DAsync(ctx->d_stage, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    src = static_cast<const unsigned char*>(ctx->d_stage);
+    stride = hwc;
+  }
+  ofdis_track_point* out = memkind == OFDIS_MEM_DEVICE ? points : ctx->track_out;
+  ofdis_traj_record* rout = memkind == OFDIS_MEM_DEVICE ? records : ctx->traj_rec;
+  float* dout = memkind == OFDIS_MEM_DEVICE ? desc : ctx->traj_desc;
+  const LevelGeom g = stepped(ctx->lev[0], D);
+  // a call that fails on the way leaves the tracker and the descriptor stage to a new ofdis_traj_begin
+  ctx->track_on = false;
+  ctx->traj_on = false;
+  CK(cudaMemcpyAsync(tw.models, m32.data(), sizeof(float) * m32.size(), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemsetAsync(&tw.state->total, 0, sizeof(int), ctx->stream));
+  int cur = ctx->track_cur;
+  for (int k = 0; k < n; ++k) {
+    const unsigned char* I = k == 0 ? tw.frame : src + (k - 1) * stride;
+    const int l0 = launch_traj_frame(g, (f0 + k) * D, tg, t, tw, ws, ctx->prm.noc, I, tw.models + 9 * k, cur, cx, cy,
+                                     ctx->stream);
+    if (l0 < 0) return fail(ctx, OFDIS_ERR_CUDA, "traj_field_kernel launch", cudaGetLastError());
+    if (launch_track_advance(g, (f0 + k) * D, (b0 + k) * D, t, ws, cur, cx, cy, ctx->stream) < 0)
+      return fail(ctx, OFDIS_ERR_CUDA, "track_advance_kernel launch", cudaGetLastError());
+    const int l = launch_track_seed_compact(t, ws, ctx->prm.noc, src + k * stride, cur, out + (size_t)k * t.capacity,
+                                            k, ctx->stream);
+    if (l < 0) return fail(ctx, OFDIS_ERR_CUDA, "track_seed_kernel launch", cudaGetLastError());
+    const int l1 = launch_traj_step(tg, t, tw, ws, cur, ctx->traj_frame + k, k, rout, dout, ctx->stream);
+    if (l1 < 0) return fail(ctx, OFDIS_ERR_CUDA, "traj_flag_kernel launch", cudaGetLastError());
+    ctx->launches += l0 + 1 + l + l1;
+    cur ^= 1;
+  }
+  ctx->track_cur = cur;
+  CK(cudaMemcpyAsync(tw.frame, src + (n - 1) * stride, hwc, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(counts, ws.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(n_desc, tw.ndesc, sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (memkind != OFDIS_MEM_DEVICE) {
+    for (int k = 0; k < n; ++k)
+      if (counts[k] > 0)
+        CK(cudaMemcpyAsync(points + (size_t)k * t.capacity, out + (size_t)k * t.capacity,
+                           sizeof(ofdis_track_point) * counts[k], cudaMemcpyDeviceToHost, ctx->stream));
+    size_t total = 0;
+    for (int k = 0; k < n; ++k) total += (size_t)n_desc[k];
+    if (total) {
+      CK(cudaMemcpyAsync(records, rout, sizeof(ofdis_traj_record) * total, cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaMemcpyAsync(desc, dout, sizeof(float) * tg.dim * total, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  ctx->traj_frame += n;
+  ctx->track_on = true;
+  ctx->traj_on = true;
+  return OFDIS_OK;
+}
+
+int ofdis_traj_stats_get(const ofdis_ctx* ctx, ofdis_traj_stats* out) {
+  if (!ctx || !out || !ctx->traj_on) return OFDIS_ERR_ARG;
+  TrajState s;
+  if (cudaSetDevice(ctx->device) != cudaSuccess ||
+      cudaMemcpyAsync(&s, ctx->traj.state, sizeof(s), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+      cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+    return OFDIS_ERR_CUDA;
+  out->emitted = (long long)s.emitted;
+  out->rejected_static = (long long)s.reason[0];
+  out->rejected_erratic = (long long)s.reason[1];
+  out->rejected_jump = (long long)s.reason[2];
+  out->rejected_camera = (long long)s.reason[3];
   return OFDIS_OK;
 }
 

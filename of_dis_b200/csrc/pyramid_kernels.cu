@@ -222,7 +222,7 @@ __global__ void __launch_bounds__(256) flow_encode_kernel(LevelGeom g, int f0, u
 // preprocess.atan2_f32 / flow_to_color / disp_to_color restate it bit for bit).  The tables, built once at compile
 // time in float32: Middlebury's color wheel (makecolorwheel, integer division) divided by 255, and the eight-entry
 // map of KITTI's stereo devkit (disp_to_color) with its bin weights and cumulative bin edges.
-constexpr float PI_F = 3.14159265358979323846f;
+constexpr float PI_F = OFDIS_PI_F;
 constexpr int WHEEL = 55;
 struct ColorTables {
   float wheel[WHEEL][3];  // W[k][b] / 255.0f
@@ -251,28 +251,14 @@ constexpr ColorTables make_color_tables() {
     t.disp_cum[i + 1] = t.disp_cum[i] + (float)M[i][3] / 1000.0f;
   }
   // atan(t) ~ t * (C0 + s * (C1 + ... + s * C7)), s = t * t, fitted on [0, 1] (|error| < 4e-8 before rounding)
-  constexpr float C[8] = {0.99999934f, -0.3332986f, 0.19946565f, -0.13908629f,
-                          0.09642195f, -0.055912293f, 0.021862935f, -0.0040545613f};
+  constexpr float C[8] = {OFDIS_ATAN2_C};
   for (int k = 0; k < 8; ++k) t.atan_c[k] = C[k];
   return t;
 }
 __constant__ ColorTables kColor = make_color_tables();
 
-// The library's float32 atan2: octant reduction to t = min / max in [0, 1] (0 where both are 0), the odd degree-15
-// polynomial kColor.atan_c (Horner in s = t * t), then pi/2 - p, pi - p and the sign, all on the sign bits,
-// so the signed zeros and the axes follow C.  |error| <= 1e-6 against float64 atan2; every finite input gives a value
-// in [-PI_F, PI_F].
-__device__ __forceinline__ float atan2_f32(float y, float x) {
-  const float ax = fabsf(x), ay = fabsf(y), mx = fmaxf(ax, ay), mn = fminf(ax, ay);
-  const float t = mx > 0.0f ? mn / mx : 0.0f, s = t * t;
-  float q = kColor.atan_c[7];
-#pragma unroll
-  for (int k = 6; k >= 0; --k) q = q * s + kColor.atan_c[k];
-  float p = t * q;
-  p = ay > ax ? PI_F * 0.5f - p : p;
-  p = signbit(x) ? PI_F - p : p;
-  return signbit(y) ? -p : p;
-}
+// The library's float32 atan2 (ofdis_internal.cuh) on the color tables' coefficients
+__device__ __forceinline__ float atan2_f32(float y, float x) { return ofdis::atan2_f32(y, x, kColor.atan_c); }
 
 // What the automatic scale is the maximum of: flow the radius of a known pixel (|u|, |v| <= 1e9, so NaN and the
 // infinities are unknown), stereo the valid disparity d (0 <= d <= 1e9; d = -F, +F in a slot marked swapped).  +0

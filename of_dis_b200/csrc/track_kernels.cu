@@ -25,43 +25,6 @@ namespace {
 constexpr int TRACK_THREADS = 256;  // threads of every kernel but the scan; a scan block is 4 flags per thread
 static_assert(TRACK_BLOCK == 4 * TRACK_THREADS, "a scan block is one 32-bit word of flags per thread");
 
-// Exclusive scan of one value per thread over a CTA of NT threads; `total` gets the CTA's sum.  sw: NT / 32 words of
-// shared memory.  Ends with a barrier, so it can run in a loop.
-template <int NT>
-__device__ __forceinline__ unsigned int block_exclusive_scan(unsigned int v, unsigned int* sw, unsigned int& total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) sw[warp] = x;
-  __syncthreads();
-  if (warp == 0) {
-    unsigned int s = lane < NT / 32 ? sw[lane] : 0u;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned int y = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += y;
-    }
-    if (lane < NT / 32) sw[lane] = s;
-  }
-  __syncthreads();
-  const unsigned int ex = x - v + (warp ? sw[warp - 1] : 0u);
-  total = sw[NT / 32 - 1];
-  __syncthreads();
-  return ex;
-}
-
-// brightness of pixel (x, y) of an 8-bit frame: the byte, or the mean of three channels in memory order
-template <int NOC>
-__device__ __forceinline__ float gray_at(const unsigned char* I, int w, int x, int y) {
-  const unsigned char* p = I + ((size_t)y * w + x) * NOC;
-  if (NOC == 1) return (float)p[0];
-  return ((float)p[0] + (float)p[1] + (float)p[2]) / 3.0f;
-}
-
 template <int NOP>
 __global__ void __launch_bounds__(TRACK_THREADS) track_advance_kernel(LevelGeom g, int fa, int fb, TrackGeom t,
                                                                       TrackWork ws, ofdis_track_point* list,

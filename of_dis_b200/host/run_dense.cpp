@@ -627,6 +627,16 @@ int main(int argc, char** argv) {
 // inconsistent, the code of _occ.pgm; and <stem>_registered.png, image2 sampled at the model's position of every
 // pixel of image1 (0 outside image2).  Every other output keeps its bytes.  Not with --warm-start.
 //
+// --descriptors PATH (needs --tracks, whose clips it describes; flow binaries only): the trajectory descriptors of
+// every clip's tracks (ofdis_traj_begin / ofdis_traj_advance in place of the tracker's calls, whose tracks they keep
+// bit for bit), with the --global-motion models when that flag is given and without camera compensation otherwise.
+// Settings: Wang and Schmid's, L 15, nt 3, N 32, ns 2, min_flow 0.4, eps 0.05, min_disp 1, min_var sqrt(3), max_var 50,
+// max_dis 20.  PATH gets the header `# clip id start mean_x mean_y sd_x sd_y length d0 .. d425`, then one line per
+// emitted segment in the order of the calls, clips counted from 0 and start from the clip's first frame, every float
+// printed with %.9g (which round-trips float32).  With verbosity > 0 a line `DESCRIPTORS clips C emitted E static S
+// erratic R jump J camera K` follows the TRACKS line.  Frames smaller than N are refused before any device work; every
+// other output, the --tracks file included, keeps its bytes.  Not with --warm-start.
+//
 // --stabilize RADIUS CROP DIR (needs --global-motion, whose models it smooths; flow binaries only): every clip
 // stabilised on the device (ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish).  Clips are the runs of pairs of
 // --tracks, across batches: the stabiliser begins on a clip's first image1, every batch pushes the image2 frames of
@@ -847,7 +857,7 @@ int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr,
             "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
-            "       [--color [--color-max M]] [--interpolate T] [--tracks PATH]\n"
+            "       [--color [--color-max M]] [--interpolate T] [--tracks PATH [--descriptors PATH]]\n"
             "       [--lr-check] [--speckle N R] [--fill] [--camera fx,fy,cx,cy,baseline,doffs]\n"
             "       [--global-motion similarity|affine|homography PATH [--stabilize RADIUS CROP DIR]]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
@@ -868,6 +878,10 @@ int main(int argc, char** argv) {
             "  synthesised on the device from the forward and backward flows; not with --warm-start\n"
             "  --tracks PATH: dense point trajectories through every clip of the list, written to PATH as lines\n"
             "  `clip frame id x y`; not with --warm-start\n"
+            "  --descriptors PATH: flow only, with --tracks; the trajectory descriptors (shape, HOG, HOF, MBH) of every\n"
+            "  15-frame segment of the tracks, camera-compensated with the --global-motion models when given, written to\n"
+            "  PATH as lines `clip id start mean_x mean_y sd_x sd_y length` and 426 floats; frames of at least 32 x 32;\n"
+            "  not with --warm-start\n"
             "  --lr-check, --speckle N R, --fill, --camera ...: stereo only; also write <stem>_filtered<ext>, the\n"
             "  disparity without the pixels that fail the left-right check and the speckles of at most N pixels (R px),\n"
             "  holes filled with the background disparity, and with --camera <stem>_depth.pfm and <stem>.ply;\n"
@@ -888,6 +902,7 @@ int main(int argc, char** argv) {
   float interp_t = 0.0f;
   const char* gtlist = nullptr;
   const char* tracks_path = nullptr;  // --tracks PATH
+  const char* desc_path = nullptr;    // --descriptors PATH
   bool lr_check = false, disp_fill = false;  // --lr-check, --fill
   const char* speckle_arg[2] = {nullptr, nullptr};  // --speckle N R
   const char* camera_arg = nullptr;  // --camera fx,fy,cx,cy,baseline,doffs
@@ -930,6 +945,13 @@ int main(int argc, char** argv) {
         return 2;
       }
       tracks_path = argv[first_num + 1];
+      first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--descriptors")) {
+      if (argc < first_num + 2 || desc_path) {
+        fprintf(stderr, "error: --descriptors takes one output path\n");
+        return 2;
+      }
+      desc_path = argv[first_num + 1];
       first_num += 2;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--lr-check")) {
       lr_check = true;
@@ -1025,6 +1047,33 @@ int main(int argc, char** argv) {
       return 2;
     }
   }
+  if (desc_path) {
+    if (SELECTMODE != 1) {
+      fprintf(stderr, "error: --descriptors describes the tracks of flows; the stereo binaries take no --descriptors\n");
+      return 2;
+    }
+    if (warm) {
+      fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --descriptors\n");
+      return 2;
+    }
+    if (!tracks_path) {
+      fprintf(stderr, "error: --descriptors describes the clips of --tracks; give --tracks too\n");
+      return 2;
+    }
+  }
+  ofdis_traj_params trp;  // --descriptors: Wang and Schmid's settings
+  memset(&trp, 0, sizeof(trp));
+  trp.L = 15;
+  trp.nt = 3;
+  trp.N = 32;
+  trp.ns = 2;
+  trp.min_flow = 0.4f;
+  trp.eps = 0.05f;
+  trp.min_disp = 1.0f;
+  trp.min_var = (float)std::sqrt(3.0);
+  trp.max_var = 50.0f;
+  trp.max_dis = 20.0f;
+  const int tdim = 2 * trp.L + trp.ns * trp.ns * trp.nt * 33;
   ofdis_stab_params stp;  // --stabilize
   memset(&stp, 0, sizeof(stp));
   vector<double> stab_wts;
@@ -1165,11 +1214,35 @@ int main(int argc, char** argv) {
       }
     }
   }
+  // --descriptors: every pair's frames hold an N x N patch, checked before any device work
+  for (size_t k = 0; k < jobs.size() && desc_path; ++k) {
+    int iw = 0, ih = 0;
+    if (!image_size(jobs[k].a.c_str(), iw, ih)) {
+      fprintf(stderr, "error: cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)\n",
+              jobs[k].a.c_str(), jobs[k].b.c_str());
+      return 1;
+    }
+    if (iw < trp.N || ih < trp.N) {
+      fprintf(stderr, "error: --descriptors needs frames of at least %d x %d, %s is %d x %d\n", trp.N, trp.N,
+              jobs[k].a.c_str(), iw, ih);
+      return 2;
+    }
+  }
+  FILE* desc_file = nullptr;
+  if (desc_path) {
+    desc_file = fopen(desc_path, "w");
+    if (!desc_file) {
+      fprintf(stderr, "error: cannot write %s\n", desc_path);
+      return 1;
+    }
+    fprintf(desc_file, "# clip id start mean_x mean_y sd_x sd_y length d0 .. d%d\n", tdim - 1);
+  }
   FILE* tracks_file = nullptr;
   if (tracks_path) {
     tracks_file = fopen(tracks_path, "w");
     if (!tracks_file) {
       fprintf(stderr, "error: cannot write %s\n", tracks_path);
+      if (desc_file) fclose(desc_file);
       return 1;
     }
     fprintf(tracks_file, "# clip frame id x y\n");
@@ -1181,6 +1254,7 @@ int main(int argc, char** argv) {
     if (!stab_file) {
       fprintf(stderr, "error: cannot write %s\n", stab_txt.c_str());
       if (tracks_file) fclose(tracks_file);
+      if (desc_file) fclose(desc_file);
       return 1;
     }
   }
@@ -1190,6 +1264,7 @@ int main(int argc, char** argv) {
     if (!gm_file) {
       fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
       if (tracks_file) fclose(tracks_file);
+      if (desc_file) fclose(desc_file);
       if (stab_file) fclose(stab_file);
       return 1;
     }
@@ -1224,6 +1299,12 @@ int main(int argc, char** argv) {
   size_t tframes = 0;
   ofdis_track_stats ttotal;
   memset(&ttotal, 0, sizeof(ttotal));
+  // --descriptors: the segments of a call and the totals of the finished clips
+  vector<ofdis_traj_record> trec;
+  vector<float> tdesc;
+  vector<int> tndesc;
+  ofdis_traj_stats dtotal;
+  memset(&dtotal, 0, sizeof(dtotal));
   auto end_clip = [&]() {  // adds the tracked clip's counters to the totals
     ofdis_track_stats st;
     if (tclip < 0 || ofdis_track_stats_get(ctx, &st) != OFDIS_OK) return;
@@ -1232,6 +1313,23 @@ int main(int argc, char** argv) {
     ttotal.ended_inconsistent += st.ended_inconsistent;
     ttotal.ended_boundary += st.ended_boundary;
     ttotal.dropped += st.dropped;
+    ofdis_traj_stats ds;
+    if (!desc_file || ofdis_traj_stats_get(ctx, &ds) != OFDIS_OK) return;
+    dtotal.emitted += ds.emitted;
+    dtotal.rejected_static += ds.rejected_static;
+    dtotal.rejected_erratic += ds.rejected_erratic;
+    dtotal.rejected_jump += ds.rejected_jump;
+    dtotal.rejected_camera += ds.rejected_camera;
+  };
+  auto write_desc = [&](int count) {
+    for (int i = 0; i < count; ++i) {
+      const ofdis_traj_record& r = trec[i];
+      fprintf(desc_file, "%d %d %d %.9g %.9g %.9g %.9g %.9g", tclip, r.id, r.start, (double)r.mean_x, (double)r.mean_y,
+              (double)r.sd_x, (double)r.sd_y, (double)r.length);
+      const float* d = tdesc.data() + (size_t)i * tdim;
+      for (int e = 0; e < tdim; ++e) fprintf(desc_file, " %.9g", (double)d[e]);
+      fprintf(desc_file, "\n");
+    }
   };
   // --stabilize: the emitted frames and records, the clip being stabilised (-1 none), whether its stabiliser is live
   // and its frame size
@@ -1458,11 +1556,24 @@ int main(int argc, char** argv) {
         end_clip();
         ++tclip;
         tframe = 0;
-        rc = ofdis_track_begin(ctx, &tp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
+        rc = desc_file ? ofdis_traj_begin(ctx, &tp, &trp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST)
+                       : ofdis_track_begin(ctx, &tp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
         if (rc == OFDIS_OK) write_tracks(tpoints.data(), tcounts[0]);
       }
-      if (rc == OFDIS_OK)
+      if (rc == OFDIS_OK && desc_file) {
+        const size_t bound = (size_t)tp.capacity * ((k1 - k0 + 2 * trp.L - 2) / trp.L);
+        trec.resize(bound);
+        tdesc.resize(bound * tdim);
+        tndesc.resize(k1 - k0);
+        rc = ofdis_traj_advance(ctx, k0, k1, n + k0, im2, fs, gm_model ? gm_models.data() + (size_t)9 * k0 : nullptr,
+                                tpoints.data(), tcounts.data(), trec.data(), tdesc.data(), tndesc.data(), w, h,
+                                OFDIS_MEM_HOST);
+        int total = 0;
+        for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k) total += tndesc[k];
+        if (rc == OFDIS_OK) write_desc(total);
+      } else if (rc == OFDIS_OK) {
         rc = ofdis_track_advance(ctx, k0, k1, n + k0, im2, fs, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
+      }
       for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k) write_tracks(tpoints.data() + (size_t)k * tp.capacity, tcounts[k]);
     }
     // --stabilize: the runs of --tracks; a clip begins on its first image1, every run pushes its image2 frames with
@@ -1658,6 +1769,10 @@ int main(int argc, char** argv) {
     fprintf(stderr, "error: cannot write %s\n", tracks_path);
     return 1;
   }
+  if (desc_file && fclose(desc_file) != 0) {
+    fprintf(stderr, "error: cannot write %s\n", desc_path);
+    return 1;
+  }
   if (gm_file && fclose(gm_file) != 0) {
     fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
     return 1;
@@ -1668,6 +1783,9 @@ int main(int argc, char** argv) {
   if (verbosity > 0 && tracks_path)
     printf("TRACKS clips %d frames %zu seeded %lld leaves %lld inconsistent %lld boundary %lld dropped %lld\n", tclip + 1,
            tframes, ttotal.seeded, ttotal.ended_leaves, ttotal.ended_inconsistent, ttotal.ended_boundary, ttotal.dropped);
+  if (verbosity > 0 && desc_path)
+    printf("DESCRIPTORS clips %d emitted %lld static %lld erratic %lld jump %lld camera %lld\n", tclip + 1,
+           dtotal.emitted, dtotal.rejected_static, dtotal.rejected_erratic, dtotal.rejected_jump, dtotal.rejected_camera);
   if (verbosity > 0 && gtlist) {
     static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
     print_eval("", done, eval_total[0]);

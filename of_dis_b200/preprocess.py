@@ -1457,3 +1457,332 @@ def global_motion(F: np.ndarray, B: np.ndarray | None, frames1: np.ndarray | Non
     if one:
         return models[0], stats[0], mask[0], residual[0], None if reg is None else reg[0]
     return models, stats, mask, residual, reg
+
+
+# ---- trajectory descriptors (ofdis_traj_begin / ofdis_traj_advance) -------------------------------------------------
+# ofdis_traj_params, ofdis_traj_record and ofdis_traj_stats, field for field
+TRAJ_PARAM_FIELDS = ("L", "nt", "N", "ns", "min_flow", "eps", "min_disp", "min_var", "max_var", "max_dis")
+TRAJ_RECORD_DTYPE = np.dtype([("id", "<i4"), ("start", "<i4"), ("mean_x", "<f4"), ("mean_y", "<f4"),
+                              ("sd_x", "<f4"), ("sd_y", "<f4"), ("length", "<f4")])
+TRAJ_STATS_FIELDS = ("emitted", "rejected_static", "rejected_erratic", "rejected_jump", "rejected_camera")
+# Wang and Schmid's improved dense trajectories (ICCV 2013)
+TRAJ_DEFAULTS = {"L": 15, "nt": 3, "N": 32, "ns": 2, "min_flow": 0.4, "eps": 0.05, "min_disp": 1.0,
+                 "min_var": math.sqrt(3.0), "max_var": 50.0, "max_dis": 20.0}
+TRAJ_BINS = 33                   # HOG 8, HOF 9, MBHx 8, MBHy 8 per spatial cell
+_TRAJ_LO = (0, 8, 17, 25)        # first entry of each in a cell's 33
+_TRAJ_NB = (8, 9, 8, 8)
+_TWO_PI_F = np.float32(6.2831855)
+_BIN_SCALE = np.float32(1.2732395)  # 8 / (2 pi)
+_NO_BIN = 255
+_FLT_MAX = np.float32(np.finfo(np.float32).max)
+
+
+def traj_dim(p) -> int:
+    """Floats per descriptor: 2L + ns^2 nt 33 (426 with TRAJ_DEFAULTS)."""
+    return 2 * int(p["L"]) + int(p["ns"]) ** 2 * int(p["nt"]) * TRAJ_BINS
+
+
+def traj_bound(capacity: int, n: int, L: int) -> int:
+    """The most segments a call of n pairs emits: capacity * ceil((n + L - 1) / L)."""
+    return int(capacity) * ((int(n) + 2 * int(L) - 2) // int(L)) if n > 0 else 0
+
+
+def orientation_bins(a, b):
+    """The orientation bins of the vectors (a, b) (ofdis_traj_params' header): (bin0, mag0, mag1), bin0 uint8 with
+    255 where mag = sqrtf(a*a + b*b) is not finite (mag0 = mag1 = 0 there); bin1 = (bin0 + 1) % 8."""
+    f32 = np.float32
+    a, b = np.asarray(a, f32), np.asarray(b, f32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        mag = np.sqrt(a * a + b * b)
+        ok = mag <= _FLT_MAX
+        ang = atan2_f32(b, a)
+        ang = np.where(ang < 0, ang + _TWO_PI_F, ang).astype(f32)
+        fbin = (ang * _BIN_SCALE).astype(f32)
+        fb0 = np.floor(fbin)
+        m1 = ((fbin - fb0) * mag).astype(f32)
+        m0 = (mag - m1).astype(f32)
+    b0 = np.where(ok, fb0, 0).astype(np.int64)
+    b0 = np.where(b0 >= 8, 0, b0)
+    return (np.where(ok, b0, _NO_BIN).astype(np.uint8), np.where(ok, m0, f32(0)).astype(f32),
+            np.where(ok, m1, f32(0)).astype(f32))
+
+
+def traj_model(m) -> np.ndarray:
+    """A received model (9 float64, or None) as the descriptors apply it: stab_model, then float32."""
+    return np.array(_EYE if m is None else stab_model(m), np.float32)
+
+
+def traj_residual(F: np.ndarray, m32: np.ndarray):
+    """(R, known): the residual flow F - the model's flow, (h, w, 2) float32, and where it is known."""
+    f32 = np.float32
+    F = np.asarray(F, f32)
+    h, w = F.shape[:2]
+    m = [f32(v) for v in np.asarray(m32, f32).reshape(9)]
+    X = np.broadcast_to(np.arange(w, dtype=f32)[None, :], (h, w))
+    Y = np.broadcast_to(np.arange(h, dtype=f32)[:, None], (h, w))
+    u, v = F[..., 0], F[..., 1]
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        mx = (m[0] * X + m[1] * Y) + m[2]
+        my = (m[3] * X + m[4] * Y) + m[5]
+        wq = (m[6] * X + m[7] * Y) + m[8]
+        ru = u - (mx / wq - X)
+        rv = v - (my / wq - Y)
+        known = (np.abs(u) <= f32(1e9)) & (np.abs(v) <= f32(1e9)) & (wq > 0) & (np.abs(ru) <= _FLT_MAX) & \
+            (np.abs(rv) <= _FLT_MAX)
+    return np.stack([ru, rv], -1).astype(f32), known
+
+
+def _brightness(frame: np.ndarray) -> np.ndarray:
+    f32 = np.float32
+    I = np.asarray(frame, np.uint8)
+    if I.ndim == 3 and I.shape[2] == 3:
+        return (I[..., 0].astype(f32) + I[..., 1].astype(f32) + I[..., 2].astype(f32)) / f32(3)
+    return I.reshape(I.shape[:2]).astype(f32)
+
+
+def _cdiff(f: np.ndarray):
+    """The tracker's clamped central differences of an (h, w) plane: (dx, dy)."""
+    h, w = f.shape
+    xs, ys = np.arange(w), np.arange(h)
+    with np.errstate(invalid="ignore", over="ignore"):
+        dx = (f[:, np.minimum(xs + 1, w - 1)] - f[:, np.maximum(xs - 1, 0)]) * np.float32(0.5)
+        dy = (f[np.minimum(ys + 1, h - 1), :] - f[np.maximum(ys - 1, 0), :]) * np.float32(0.5)
+    return dx, dy
+
+
+def traj_fields(frame: np.ndarray, F: np.ndarray, m32: np.ndarray, min_flow):
+    """The per-pixel fields of one source frame: (contrib, R, known).  contrib (h, w, 33) float32 is what the pixel
+    adds to each of a cell's 33 bins (HOG 0-7, HOF 8-16 with the zero bin 16, MBHx 17-24, MBHy 25-32), 0 elsewhere."""
+    f32 = np.float32
+    R, known = traj_residual(F, m32)
+    h, w = known.shape
+    gx, gy = _cdiff(_brightness(frame))
+    xs, ys = np.arange(w), np.arange(h)
+    xl, xr = np.maximum(xs - 1, 0), np.minimum(xs + 1, w - 1)
+    yu, yd = np.maximum(ys - 1, 0), np.minimum(ys + 1, h - 1)
+    kn = known[:, xl] & known[:, xr] & known[yu, :] & known[yd, :]
+    fields = [(gx, gy, np.ones((h, w), bool))]
+    fields.append((R[..., 0], R[..., 1], known))
+    for c in range(2):
+        dx, dy = _cdiff(R[..., c])
+        fields.append((dx, dy, kn))
+    contrib = np.zeros((h, w, TRAJ_BINS), f32)
+    rows, cols = np.indices((h, w))
+    for q, (a, b, ok) in enumerate(fields):
+        b0, m0, m1 = orientation_bins(np.where(ok, a, f32(0)), np.where(ok, b, f32(0)))
+        has = ok & (b0 != _NO_BIN)
+        if q == 1:
+            with np.errstate(invalid="ignore", over="ignore"):
+                zero = has & (np.sqrt(R[..., 0] * R[..., 0] + R[..., 1] * R[..., 1]) <= f32(min_flow))
+            b0 = np.where(zero, 8, b0)
+            m0 = np.where(zero, f32(1), m0)
+            m1 = np.where(zero, f32(0), m1)
+        lo = _TRAJ_LO[q]
+        b1 = np.where(b0 == 8, 1, (b0.astype(np.int64) + 1) % 8)
+        contrib[rows[has], cols[has], lo + b0[has].astype(np.int64)] = m0[has]
+        contrib[rows[has], cols[has], lo + b1[has]] += m1[has]
+    return contrib, R, known
+
+
+def traj_frame_hist(contrib: np.ndarray, xs: np.ndarray, ys: np.ndarray, p) -> np.ndarray:
+    """The RootSIFT-normalised frame histograms of tracks at (xs, ys): (T, ns*ns, 33) float32, cells (cx, cy) as
+    cx * ns + cy; each cell's sums in the lane order of the header."""
+    f32 = np.float32
+    h, w = contrib.shape[:2]
+    N, ns = int(p["N"]), int(p["ns"])
+    c = N // ns
+    T = xs.size
+    xr = np.floor(xs.astype(f32) + f32(0.5)).astype(np.int64)
+    yr = np.floor(ys.astype(f32) + f32(0.5)).astype(np.int64)
+    ox = np.minimum(np.maximum(xr - N // 2, 0), w - N)
+    oy = np.minimum(np.maximum(yr - N // 2, 0), h - N)
+    cc = c * c
+    rounds = (cc + 31) // 32
+    q = np.arange(cc)
+    v = np.empty((T, ns * ns, TRAJ_BINS), f32)
+    for cx in range(ns):
+        for cy in range(ns):
+            px = ox[:, None] + cx * c + q[None, :] % c
+            py = oy[:, None] + cy * c + q[None, :] // c
+            a = np.zeros((T, rounds * 32, TRAJ_BINS), f32)
+            a[:, :cc] = contrib[py, px]
+            a = a.reshape(T, rounds, 32, TRAJ_BINS)
+            lane = a[:, 0]
+            for r in range(1, rounds):
+                lane = lane + a[:, r]
+            s = lane[:, 0]
+            for l in range(1, 32):
+                s = s + lane[:, l]
+            v[:, cx * ns + cy] = s + f32(p["eps"])
+    out = np.empty_like(v)
+    for d in range(4):
+        lo, nb = _TRAJ_LO[d], _TRAJ_NB[d]
+        s = np.zeros(T, f32)
+        for cell in range(ns * ns):
+            for k in range(nb):
+                s = s + v[:, cell, lo + k]
+        out[:, :, lo:lo + nb] = np.sqrt(v[:, :, lo:lo + nb] / s[:, None, None])
+    return out
+
+
+def traj_segment_test(pos: np.ndarray, disp: np.ndarray, p):
+    """The tests of one completed segment: pos (L+1, 2), disp (L, 2) float32.  Returns (why, stats, dsum): why 0
+    emitted, 1 static, 2 erratic, 3 jump, 4 camera; stats (mean_x, mean_y, sd_x, sd_y, length)."""
+    f32 = np.float32
+    L = disp.shape[0]
+    fn = f32(L + 1)
+    with np.errstate(invalid="ignore", over="ignore"):
+        sx = sy = f32(0)
+        for j in range(L + 1):
+            sx = f32(sx + pos[j, 0])
+            sy = f32(sy + pos[j, 1])
+        mx, my = f32(sx / fn), f32(sy / fn)
+        vx = vy = f32(0)
+        for j in range(L + 1):
+            dx, dy = f32(pos[j, 0] - mx), f32(pos[j, 1] - my)
+            vx = f32(vx + dx * dx)
+            vy = f32(vy + dy * dy)
+        sdx, sdy = np.sqrt(f32(vx / fn)), np.sqrt(f32(vy / fn))
+        length = smax = f32(0)
+        for j in range(L):
+            dx, dy = f32(pos[j + 1, 0] - pos[j, 0]), f32(pos[j + 1, 1] - pos[j, 1])
+            s = np.sqrt(f32(dx * dx + dy * dy))
+            length = f32(length + s)
+            if s > smax:
+                smax = s
+        dsum = dmax = f32(0)
+        known = True
+        for j in range(L):
+            du, dv = disp[j, 0], disp[j, 1]
+            a = np.sqrt(f32(du * du + dv * dv))
+            known = known and bool(a <= _FLT_MAX)
+            dsum = f32(dsum + a)
+            if a > dmax:
+                dmax = a
+    stats = (mx, my, sdx, sdy, length)
+    if sdx < f32(p["min_var"]) and sdy < f32(p["min_var"]):
+        return 1, stats, dsum
+    if sdx > f32(p["max_var"]) or sdy > f32(p["max_var"]):
+        return 2, stats, dsum
+    if smax > f32(p["max_dis"]) and smax > f32(0.7) * length:
+        return 3, stats, dsum
+    if not known or dmax <= f32(p["min_disp"]):
+        return 4, stats, dsum
+    return 0, stats, dsum
+
+
+class TrajStream:
+    """ofdis_traj_begin / ofdis_traj_advance restated bit for bit, one call at a time, on the tracker of
+    track_points: begin(frame), then advance(frames, fw, bw, models) for every call with the call's target frames
+    (n, h, w[, noc]), full-resolution flows (n, h, w, 2) and models (n, 9) float64 or None."""
+
+    def __init__(self, track_params, traj_params):
+        self.tp = {k: track_params[k] for k in TRACK_PARAM_FIELDS}
+        self.p = {k: traj_params[k] for k in TRAJ_PARAM_FIELDS}
+        L, nt, ns = int(self.p["L"]), int(self.p["nt"]), int(self.p["ns"])
+        assert L % nt == 0 and int(self.p["N"]) % ns == 0
+        self.L, self.nt, self.ns, self.tl = L, nt, ns, L // nt
+
+    def _fresh(self, n):
+        return (np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros((n, self.L + 1, 2), np.float32),
+                np.zeros((n, self.L, 2), np.float32), np.zeros((n, self.nt, self.ns * self.ns, TRAJ_BINS), np.float32))
+
+    def begin(self, frame):
+        self.stats = dict.fromkeys(TRACK_STATS_FIELDS, 0)
+        self.tstats = dict.fromkeys(TRAJ_STATS_FIELDS, 0)
+        self.tracks, self.next_id = _track_seed(np.asarray(frame, np.uint8), np.empty(0, TRACK_POINT_DTYPE), 0,
+                                                self.stats, self.tp)
+        self.step, self.start, self.pos, self.disp, self.acc = self._fresh(self.tracks.size)
+        self.frame = np.asarray(frame, np.uint8)
+        self.fr = 0
+        return self.tracks
+
+    def _emit(self, disp, a, dsum):
+        f32 = np.float32
+        shape = (disp / dsum).astype(f32).reshape(-1)
+        parts = [shape]
+        for d in range(4):
+            lo, nb = _TRAJ_LO[d], _TRAJ_NB[d]
+            parts.append((a[:, :, lo:lo + nb] / f32(self.tl)).astype(f32).reshape(-1))
+        return np.concatenate(parts)
+
+    def advance(self, frames, fw, bw, models=None):
+        """Returns (lists, records, desc, n_desc), as Context.traj_advance on the host."""
+        f32 = np.float32
+        clip = np.asarray(frames, np.uint8)
+        F = np.asarray(fw, f32)
+        B = np.asarray(bw, f32)
+        n = F.shape[0]
+        lists, recs, descs, n_desc = [], [], [], []
+        p, L, tkeys = self.p, self.L, ("mean_x", "mean_y", "sd_x", "sd_y", "length")
+        for k in range(n):
+            m32 = traj_model(None if models is None else models[k])
+            contrib, R, known = traj_fields(self.frame, F[k], m32, p["min_flow"])
+            tr = self.tracks
+            T = tr.size
+            if T:
+                xs, ys = tr["x"], tr["y"]
+                xr = np.floor(xs + f32(0.5)).astype(np.int64)
+                yr = np.floor(ys + f32(0.5)).astype(np.int64)
+                hist = traj_frame_hist(contrib, xs, ys, p)
+                idx = np.arange(T)
+                t = self.step
+                self.pos[idx, t, 0], self.pos[idx, t, 1] = xs, ys
+                d = np.where(known[yr, xr][:, None], R[yr, xr], f32(np.nan))
+                self.disp[idx, t] = d
+                tc = t // self.tl
+                first = (t % self.tl) == 0
+                cur = self.acc[idx, tc]
+                self.acc[idx, tc] = np.where(first[:, None, None], hist, cur + hist)
+            adv = _track_advance(tr, F[k], B[k], self.stats, self.tp)
+            keep = np.isin(tr["id"], adv["id"])
+            step, start, pos, disp, acc = (a[keep] for a in (self.step, self.start, self.pos, self.disp, self.acc))
+            step = step + 1
+            ne = 0
+            for i in np.flatnonzero(step == L):
+                pos[i, L, 0], pos[i, L, 1] = adv["x"][i], adv["y"][i]
+                why, st, dsum = traj_segment_test(pos[i], disp[i], p)
+                if why:
+                    self.tstats[TRAJ_STATS_FIELDS[why]] += 1
+                else:
+                    rec = np.zeros(1, TRAJ_RECORD_DTYPE)
+                    rec["id"], rec["start"] = adv["id"][i], start[i]
+                    for key, val in zip(tkeys, st):
+                        rec[key] = val
+                    recs.append(rec)
+                    descs.append(self._emit(disp[i], acc[i], dsum))
+                    ne += 1
+                step[i] = 0
+                start[i] += L
+            self.tstats["emitted"] += ne
+            n_desc.append(ne)
+            tracks, self.next_id = _track_seed(clip[k], adv, self.next_id, self.stats, self.tp)
+            ns_ = tracks.size - adv.size
+            fresh = self._fresh(ns_)
+            fresh[1][:] = self.fr + 1
+            self.step, self.start, self.pos, self.disp, self.acc = (np.concatenate([a, b]) for a, b in
+                                                                    zip((step, start, pos, disp, acc), fresh))
+            self.tracks = tracks
+            lists.append(tracks)
+            self.frame = clip[k]
+            self.fr += 1
+        dim = traj_dim(p)
+        records = np.concatenate(recs) if recs else np.zeros(0, TRAJ_RECORD_DTYPE)
+        desc = np.stack(descs).astype(f32) if descs else np.zeros((0, dim), f32)
+        return lists, records, desc, np.array(n_desc, np.int32)
+
+    def track_stats(self):
+        st = dict(self.stats)
+        st["alive"], st["next_id"] = int(self.tracks.size), int(self.next_id)
+        return st
+
+
+def traj_descriptors(frames: np.ndarray, fw: np.ndarray, bw: np.ndarray, models, track_params, traj_params):
+    """ofdis_traj_begin on frames[0] followed by one ofdis_traj_advance through the n pairs, bit for bit.  frames: the
+    clip (n + 1, h, w[, noc]) uint8; fw, bw: the full-resolution forward flows and their backward partners (n, h, w, 2)
+    float32; models: (n, 9) float64 or None.  Returns (lists, records, desc, n_desc, track_stats, traj_stats)."""
+    clip = np.asarray(frames, np.uint8)
+    s = TrajStream(track_params, traj_params)
+    first = s.begin(clip[0])
+    lists, records, desc, n_desc = s.advance(clip[1:], fw, bw, models)
+    return [first] + lists, records, desc, n_desc, s.track_stats(), dict(s.tstats)
