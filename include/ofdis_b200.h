@@ -399,6 +399,65 @@ int ofdis_disparity_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
                             const ofdis_stereo_camera* cam, float* disp, unsigned char* status, float* depth,
                             float* xyz, int width_org, int height_org, int memkind);
 
+/* Scene flow from a flow and two disparity maps (extension, flow contexts only): the second disparity warped to the
+ * first frame, the 3-D motion of every pixel and KITTI 2015's D1, D2, Fl and SF outlier counts.  Everything is
+ * float32 without contraction, with IEEE division; preprocess.scene_flow restates it bit for bit.  W = width_org,
+ * H = height_org, qNaN = the quiet NaN 0x7fc00000, known(d) = 0 <= d <= 1e9 (NaN fails, -0 passes).  For every pair
+ * k < f1-f0 and pixel (x, y):
+ *   F = (u, v): slot f0+k's full-resolution flow, exactly what ofdis_get_flow_fullres returns (computed from the level
+ *     flows without a full-resolution copy).  d0 = D0(x, y) with D0 = disp0 + k*disp_stride, D1 = disp1 + k*disp_stride,
+ *     both [H][W] positive disparities with NaN for unknown (the disp output of ofdis_disparity_fullres, or a decoded
+ *     KITTI PNG); disp_stride >= W*H floats, so a clip of n+1 maps passes disp1 = disp0 + W*H.
+ *   1. Target.  (xs, ys) = ((float)x + u, (float)y + v); it fails outside [0, W-1] x [0, H-1] (or NaN).
+ *   2. d1, the second disparity at the target.  x0 = floor(xs), x1 = min(x0 + 1, W-1), fx = xs - x0 (the same in y).
+ *      When the four corners are known and max - min of them <= edge_diff: the bilinear value of
+ *      ofdis_consistency_fullres, r0 = D1(x0,y0)*(1-fx) + D1(x1,y0)*fx, r1 = D1(x0,y1)*(1-fx) + D1(x1,y1)*fx,
+ *      d1 = r0*(1-fy) + r1*fy.  Otherwise the nearest corner, D1(fx >= 0.5f ? x1 : x0, fy >= 0.5f ? y1 : y0), so that a
+ *      depth edge gives one of its sides rather than a "flying" disparity between them.  edge_diff = +inf always blends.
+ *   3. status (bytes): bit 0 d0 is not known, bit 1 the target fails, bit 2 d1 is not known (only when bit 1 is clear).
+ *   4. disp1_warped = d1 where bits 1 and 2 are clear, else qNaN: KITTI's D2 (disp_occ_1) in frame-t coordinates.
+ *   5. motion = [n][H][W][3], needs cam: fb = fx * baseline rounded once; where status = 0, s0 = d0 + doffs > 0 and
+ *      s1 = d1 + doffs > 0: Z0 = fb / s0, X0 = (((float)x - cx) * Z0) / fx, Y0 = (((float)y - cy) * Z0) / fy (the xyz of
+ *      ofdis_disparity_fullres bit for bit), Z1 = fb / s1, X1 = ((xs - cx) * Z1) / fx, Y1 = ((ys - cy) * Z1) / fy, and
+ *      motion = (X1 - X0, Y1 - Y0, Z1 - Z0); elsewhere (qNaN, qNaN, qNaN).  Every NaN written is qNaN.
+ *   6. Evaluation (gt and stats).  Ground truth is known as above for gt.disp0 and gt.disp1, and as in
+ *      ofdis_flow_error_fullres (|G_u|, |G_v| <= 1e9) for gt.flow.  D1 compares d0 with gt.disp0, D2 disp1_warped with
+ *      gt.disp1: e = fabsf(est - G), g = fabsf(G).  Fl compares F with gt.flow: e = sqrtf(du*du + dv*dv) with
+ *      (du, dv) = F - G, g = sqrtf(G_u*G_u + G_v*G_v).  An unknown estimate (a disparity that is not known, a flow with
+ *      |u| or |v| not <= 1e9) has e = +inf.  A component is an outlier when e > 3.0f && e > 0.05f * g (the KITTI
+ *      expression of ofdis_flow_error_fullres), so an unknown estimate is always one.  KITTI's devkit instead fills
+ *      unknown estimates from the background before it compares; pass filled disparities (ofdis_disparity_fullres with
+ *      fill) for its behaviour.  Each component counts where its ground truth is known; a pixel counts for SF where
+ *      all three are known, and is an SF outlier where any of its three components is an outlier.  A pixel counts for
+ *      (pair k, class c) with c = classes[k][y][x] < nclasses (classes NULL: class 0), as ofdis_flow_error_fullres.
+ * stats = [f1-f0][nclasses] exact counts, always host memory.  disp0, disp1, gt's three arrays ([n][H][W], [n][H][W]
+ * and [n][H][W][2], this library's flow convention), classes ([n][H][W] bytes) and the outputs disp1_warped
+ * ([n][H][W]), status and motion are in memkind; each output may be NULL, but not all three when stats is NULL.  Host
+ * inputs go through the context's staging buffer, host outputs through its full-resolution scratch.  Device
+ * disparities may come from another context on the same device (a stereo context's ofdis_disparity_fullres); the
+ * caller orders that work before this call, by sharing the stream or with an event.  OFDIS_ERR_ARG: a stereo context,
+ * slots outside the context, NULL disp0 or disp1, disp_stride < W*H, edge_diff NaN or negative, all outputs and stats
+ * NULL, gt and stats not given together (or a NULL array in gt), nclasses not in 1..16, classes NULL when nclasses > 1,
+ * motion without cam, a cam whose fx, fy, baseline are not finite and > 0 or whose cx, cy, doffs are not finite, or a
+ * device pointer that is not aligned to its element; frame sizes as ofdis_get_flow_fullres checks them.  The counters,
+ * 64 bytes per (pair, class) for max_frames x 16, are allocated on the first call and freed by ofdis_destroy.
+ * Enqueued on the context's stream as one kernel, plus one memset of the counters with stats, whatever the number of
+ * pairs; host outputs or stats synchronise the stream.  Not part of ofdis_run's graph; the flows are not changed. */
+typedef struct ofdis_sf_gt {            /* all three [n][H][W](...) in memkind */
+  const float* disp0;                   /* positive disparity at t, NaN = unknown */
+  const float* disp1;                   /* positive disparity at t+1 of the point seen at (x, y) in frame t (KITTI disp_occ_1) */
+  const float* flow;                    /* [n][H][W][2], this library's convention */
+} ofdis_sf_gt;
+typedef struct ofdis_sf_stats {         /* per (pair, class), 64 bytes, exact counts */
+  long long n_d1, n_d2, n_fl, n_sf;     /* pixels counted */
+  long long out_d1, out_d2, out_fl, out_sf;
+} ofdis_sf_stats;
+int ofdis_scene_flow_fullres(ofdis_ctx* ctx, int f0, int f1, const float* disp0, const float* disp1,
+                             size_t disp_stride, float edge_diff, const ofdis_stereo_camera* cam,
+                             float* disp1_warped, unsigned char* status, float* motion,
+                             const ofdis_sf_gt* gt, const unsigned char* classes, int nclasses,
+                             ofdis_sf_stats* stats, int width_org, int height_org, int memkind);
+
 /* Global camera motion from dense flows (extension, flow contexts only): a RANSAC fit of one similarity, affine map
  * or homography per pair, its least-squares refits on the inliers, and from the model per pixel the residual flow, a
  * moving-pixel mask and I1 registered onto I0.  preprocess.global_motion restates it bit for bit.  float32 where

@@ -14,9 +14,9 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import (DISP_FILTER_FIELDS, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, STAB_FRAME_DTYPE,
-                         STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS, TRACK_POINT_DTYPE,
-                         TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
+from .preprocess import (DISP_FILTER_FIELDS, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
+                         STAB_FRAME_DTYPE, STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS,
+                         TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
                          gaussian_weights, motion_params, traj_bound, traj_dim)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -41,11 +41,14 @@ EXPORTS = [
     "ofdis_get_flow_fullres_encoded", "ofdis_flow_color_fullres", "ofdis_interpolate_fullres",
     "ofdis_track_begin", "ofdis_track_advance", "ofdis_track_stats_get", "ofdis_disparity_fullres",
     "ofdis_global_motion_fullres", "ofdis_stab_begin", "ofdis_stab_push", "ofdis_stab_finish",
-    "ofdis_traj_begin", "ofdis_traj_advance", "ofdis_traj_stats_get",
+    "ofdis_traj_begin", "ofdis_traj_advance", "ofdis_traj_stats_get", "ofdis_scene_flow_fullres",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
 DISP_OUTPUTS = ("disp", "status", "depth", "xyz")
+
+# outputs of scene_flow_fullres, in the C-ABI's argument order
+SF_OUTPUTS = ("disp1", "status", "motion")
 
 # encodings of get_flow_fullres_encoded (OFDIS_ENC_F16, OFDIS_ENC_KITTI)
 ENCODINGS = {"f16": 1, "kitti": 2}
@@ -85,6 +88,11 @@ class StereoCamera(ctypes.Structure):
 
 
 assert tuple(k for k, _ in DispFilter._fields_) == DISP_FILTER_FIELDS
+
+
+class SfGt(ctypes.Structure):
+    """ofdis_sf_gt (include/ofdis_b200.h)."""
+    _fields_ = [("disp0", ctypes.c_void_p), ("disp1", ctypes.c_void_p), ("flow", ctypes.c_void_p)]
 
 
 class MotionParams(ctypes.Structure):
@@ -189,6 +197,9 @@ def lib():
             [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
         L.ofdis_disparity_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
             [ctypes.POINTER(DispFilter), ctypes.POINTER(StereoCamera)] + [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3
+        L.ofdis_scene_flow_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 2 + \
+            [ctypes.c_size_t, ctypes.c_float, ctypes.POINTER(StereoCamera)] + [ctypes.c_void_p] * 3 + \
+            [ctypes.POINTER(SfGt), ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p] + [ctypes.c_int] * 3
         L.ofdis_global_motion_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
             [ctypes.POINTER(MotionParams), ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 5 + [ctypes.c_int] * 3
         L.ofdis_track_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackStats)]
@@ -430,6 +441,78 @@ class Context:
         self._ck(lib().ofdis_disparity_fullres(self._h, f0, f1, b0, ctypes.byref(filt), cam, *ptrs, width_org,
                                                height_org, memkind))
         return {k: out.get(k) for k in outputs}
+
+    def scene_flow_fullres(self, f0, f1, disp0, disp1, *, width_org, height_org, edge_diff=1.0, camera=None,
+                           outputs=("disp1", "status"), gt=None, classes=None, nclasses=None, memkind=MEM_HOST,
+                           out=None, disp_stride=None):
+        """Scene flow of the last run's flow slots [f0, f1) (ofdis_scene_flow_fullres; preprocess.scene_flow restates
+        it): pair k's flow F with the disparities disp0[k] at t and disp1[k] at t+1 (positive, NaN unknown) gives
+        "disp1" (the t+1 disparity warped to frame t), "status" and, with a camera (a mapping with
+        STEREO_CAMERA_FIELDS), "motion" (the 3-D motion).  gt: None or (disp0, disp1, flow) ground truth, with classes
+        and nclasses as flow_error_fullres takes them.  Returns (outs, stats): a dict of the requested SF_OUTPUTS and,
+        with gt, a (f1-f0, nclasses) array of SF_STATS_DTYPE (else None), always on the host.
+        Host: disp0 and disp1 float32 (f1-f0, height_org, width_org) arrays whose frames are C-contiguous and equally
+        spaced (a clip's maps[:-1] and maps[1:] qualify); gt and classes C-contiguous float32 / uint8 arrays; the
+        outputs new or given in `out` as numpy arrays of exactly their dtype and shape ("motion" has a last axis of 3);
+        the call synchronises the stream.  With memkind=MEM_DEVICE every array is a device address the caller owns,
+        disp_stride the floats between consecutive maps (default one frame), and the call only synchronises for
+        stats."""
+        unknown = set(outputs) - set(SF_OUTPUTS)
+        if unknown:
+            raise ValueError("scene_flow_fullres: unknown outputs %s" % sorted(unknown))
+        if nclasses is None:
+            if classes is not None:
+                raise ValueError("scene_flow_fullres: nclasses is required with classes")
+            nclasses = 1
+        n = max(f1 - f0, 0)
+        shape = (n, height_org, width_org)
+        out = dict(out or {})
+        if gt is not None:
+            gt = tuple(gt)
+            if len(gt) != 3:
+                raise ValueError("scene_flow_fullres: gt is (disp0, disp1, flow)")
+        if memkind == MEM_HOST:
+            strides = []
+            for name, arr in (("disp0", disp0), ("disp1", disp1)):
+                if not (isinstance(arr, np.ndarray) and arr.dtype == np.float32 and arr.shape == shape
+                        and (n == 0 or arr[0].flags["C_CONTIGUOUS"])):
+                    raise ValueError("scene_flow_fullres: %s must be a float32 array of shape %s whose frames are "
+                                     "C-contiguous" % (name, shape))
+                strides.append(arr.strides[0] // 4 if n > 1 else height_org * width_org)
+            if strides[0] != strides[1] or (n > 1 and disp0.strides[0] % 4):
+                raise ValueError("scene_flow_fullres: disp0 and disp1 must space their frames equally")
+            disp_stride = strides[0]
+            inputs = (("classes", classes, np.uint8, shape),)
+            if gt is not None:
+                inputs += (("gt disp0", gt[0], np.float32, shape), ("gt disp1", gt[1], np.float32, shape),
+                           ("gt flow", gt[2], np.float32, shape + (2,)))
+            for name, arr, dt, shp in inputs:
+                if arr is not None and not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape == shp
+                                            and arr.flags["C_CONTIGUOUS"]):
+                    raise ValueError("scene_flow_fullres: %s must be a C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shp))
+            for name in outputs:
+                shp = shape + ((3,) if name == "motion" else ())
+                dt = np.uint8 if name == "status" else np.float32
+                arr = out.setdefault(name, np.empty(shp, dt))
+                if not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape == shp
+                        and arr.flags["C_CONTIGUOUS"] and arr.flags["WRITEABLE"]):
+                    raise ValueError("scene_flow_fullres: %s must be a writeable C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shp))
+        else:
+            missing = [name for name in outputs if out.get(name) is None]
+            if missing:
+                raise ValueError("scene_flow_fullres: no device address for the requested outputs %s" % missing)
+            if disp_stride is None:
+                disp_stride = height_org * width_org
+        cam = None if camera is None else ctypes.byref(StereoCamera(*[camera[k] for k in STEREO_CAMERA_FIELDS]))
+        gts = None if gt is None else ctypes.byref(SfGt(*[_ptr(a) for a in gt]))
+        stats = None if gt is None else np.zeros((n, max(nclasses, 0)), SF_STATS_DTYPE)
+        ptrs = [_ptr(out.get(k)) if k in outputs else None for k in SF_OUTPUTS]
+        self._ck(lib().ofdis_scene_flow_fullres(self._h, f0, f1, _ptr(disp0), _ptr(disp1), disp_stride, edge_diff, cam,
+                                                *ptrs, gts, _ptr(classes), nclasses, _ptr(stats), width_org,
+                                                height_org, memkind))
+        return {k: out.get(k) for k in outputs}, stats
 
     def global_motion_fullres(self, f0, f1, params, *, width_org, height_org, b0=None, i1=None, frame_stride=None,
                               mask=None, residual=None, registered=None, memkind=MEM_HOST):

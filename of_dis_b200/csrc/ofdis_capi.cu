@@ -98,6 +98,8 @@ struct ofdis_ctx {
   // lazily allocated workspace of ofdis_disparity_fullres (DispWork for max_frames pairs of width x height pixels);
   // never touched by ofdis_run
   void* d_disp = nullptr;
+  // lazily allocated counters of ofdis_scene_flow_fullres ([max_frames][16] ofdis_sf_stats); never touched by ofdis_run
+  ofdis_sf_stats* d_sf = nullptr;
   // lazily allocated workspace of ofdis_global_motion_fullres (MotionWork for max_frames pairs of motion_cells cells
   // and motion_hyps hypotheses); grows, never shrinks; never touched by ofdis_run
   void* d_motion = nullptr;
@@ -481,6 +483,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_interp);
   cudaFree(ctx->d_track);
   cudaFree(ctx->d_disp);
+  cudaFree(ctx->d_sf);
   cudaFree(ctx->d_motion);
   cudaFree(ctx->d_traj);
   cudaFree(ctx->d_stab);
@@ -1906,6 +1909,103 @@ int ofdis_flow_error_fullres(ofdis_ctx* ctx, int f0, int f1, const float* gt, co
     CK(cudaMemcpyAsync(err, derr, sizeof(float) * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(stats, dstats, sizeof(ofdis_error_stats) * n * nclasses, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
+  return OFDIS_OK;
+}
+
+int ofdis_scene_flow_fullres(ofdis_ctx* ctx, int f0, int f1, const float* disp0, const float* disp1,
+                             size_t disp_stride, float edge_diff, const ofdis_stereo_camera* cam,
+                             float* disp1_warped, unsigned char* status, float* motion,
+                             const ofdis_sf_gt* gt, const unsigned char* classes, int nclasses,
+                             ofdis_sf_stats* stats, int width_org, int height_org, int memkind) {
+  static_assert(sizeof(ofdis_sf_stats) == 64, "ofdis_sf_stats: 64 bytes, as api.SF_STATS_DTYPE");
+  if (!ctx) return OFDIS_ERR_ARG;
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  auto misaligned = [dev](const float* p) { return dev && reinterpret_cast<uintptr_t>(p) % sizeof(float); };
+  const size_t pix = (size_t)std::max(width_org, 0) * std::max(height_org, 0);
+  if (ctx->nop != 2 || f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !disp0 || !disp1 || disp_stride < pix ||
+      !(edge_diff >= 0.f) || (!disp1_warped && !status && !motion && !stats) || (!gt != !stats) ||
+      (gt && (!gt->disp0 || !gt->disp1 || !gt->flow)) || nclasses < 1 || nclasses > kEvalMaxClasses ||
+      (!classes && nclasses > 1) ||
+      (motion && (!cam || !finite_gt0(cam->fx) || !finite_gt0(cam->fy) || !finite_gt0(cam->baseline) ||
+                  !finite_f32(cam->cx) || !finite_f32(cam->cy) || !finite_f32(cam->doffs))) ||
+      misaligned(disp0) || misaligned(disp1) || misaligned(disp1_warped) || misaligned(motion) ||
+      (gt && (misaligned(gt->disp0) || misaligned(gt->disp1) || misaligned(gt->flow))))
+    return fail(ctx, OFDIS_ERR_ARG, "scene_flow_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("sceneflow", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0, D = ctx->dirs;
+  const size_t np = pix * n;
+  if (stats && !ctx->d_sf &&
+      cudaMalloc((void**)&ctx->d_sf, sizeof(ofdis_sf_stats) * ctx->max_frames * kEvalMaxClasses) != cudaSuccess) {
+    ctx->d_sf = nullptr;
+    return fail(ctx, OFDIS_ERR_NOMEM, "scene_flow_fullres counters");
+  }
+  SfArgs a{};
+  a.disp0 = disp0;
+  a.disp1 = disp1;
+  a.stride = disp_stride;
+  a.edge_diff = edge_diff;
+  if (motion) a.cam = DispCamera{cam->fx * cam->baseline, cam->fx, cam->fy, cam->cx, cam->cy, cam->doffs};
+  a.disp1w = disp1_warped;
+  a.status = status;
+  a.motion = motion;
+  if (gt) {
+    a.gt_d0 = gt->disp0;
+    a.gt_d1 = gt->disp1;
+    a.gt_flow = gt->flow;
+    a.classes = classes;
+    a.stats = ctx->d_sf;
+  }
+  a.nclasses = nclasses;
+  if (!dev) {
+    // the staging buffer: disp0 and disp1 packed to one map per pair, then gt's disp0, disp1 and flow and the classes
+    // (those given); sized for max_frames
+    rc = ensure_stage(ctx, (sizeof(float) * 6 + 1) * pix * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    float* s = static_cast<float*>(ctx->d_stage);
+    const size_t row = sizeof(float) * pix, pitch = sizeof(float) * disp_stride;
+    CK(cudaMemcpy2DAsync(s, row, disp0, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(s + np, row, disp1, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
+    a.disp0 = s;
+    a.disp1 = s + np;
+    a.stride = pix;
+    s += 2 * np;
+    if (gt) {
+      CK(cudaMemcpyAsync(s, gt->disp0, sizeof(float) * np, cudaMemcpyHostToDevice, ctx->stream));
+      CK(cudaMemcpyAsync(s + np, gt->disp1, sizeof(float) * np, cudaMemcpyHostToDevice, ctx->stream));
+      CK(cudaMemcpyAsync(s + 2 * np, gt->flow, sizeof(float) * 2 * np, cudaMemcpyHostToDevice, ctx->stream));
+      a.gt_d0 = s;
+      a.gt_d1 = s + np;
+      a.gt_flow = s + 2 * np;
+      if (classes) {
+        CK(cudaMemcpyAsync(s + 4 * np, classes, np, cudaMemcpyHostToDevice, ctx->stream));
+        a.classes = reinterpret_cast<const unsigned char*>(s + 4 * np);
+      }
+    }
+    // the full-resolution scratch: disp1_warped and motion floats (those asked for), then the status bytes; sized for
+    // max_frames, and at least what ofdis_get_flow_fullres asks for
+    rc = ensure_full(ctx, std::max(pix * ctx->nop, pix * 4 + (pix + 3) / 4) * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    float* q = ctx->d_full;
+    if (disp1_warped) a.disp1w = q, q += np;
+    if (motion) a.motion = q, q += 3 * np;
+    a.status = status ? reinterpret_cast<unsigned char*>(q) : nullptr;
+  }
+  if (stats) CK(cudaMemsetAsync(ctx->d_sf, 0, sizeof(ofdis_sf_stats) * n * nclasses, ctx->stream));
+  if (launch_scene_flow(stepped(ctx->lev[0], D), f0 * D, n, a, width_org, height_org, cx, cy, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "sceneflow_kernel launch", cudaGetLastError());
+  ctx->launches += 1;
+  if (!dev) {
+    if (disp1_warped) CK(cudaMemcpyAsync(disp1_warped, a.disp1w, sizeof(float) * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (motion) CK(cudaMemcpyAsync(motion, a.motion, sizeof(float) * 3 * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (status) CK(cudaMemcpyAsync(status, a.status, np, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if (stats)
+    CK(cudaMemcpyAsync(stats, ctx->d_sf, sizeof(ofdis_sf_stats) * n * nclasses, cudaMemcpyDeviceToHost, ctx->stream));
+  if (!dev || stats) CK(cudaStreamSynchronize(ctx->stream));
   return OFDIS_OK;
 }
 

@@ -647,6 +647,21 @@ int main(int argc, char** argv) {
 // `clip frame s00 s01 s02 s10 s11 s12 s20 s21 s22 lambda status`, the correction and its share printed with %.17g.
 // Every other output keeps its bytes.  Not with --warm-start.
 
+// --scene-flow DISPLIST (flow binaries only): scene flow (ofdis_scene_flow_fullres, edge_diff 1) of every pair from
+// its forward flow and two disparity maps.  DISPLIST holds two files per pair, in list order: the disparity of image1
+// and that of image2, each a PFM of the positive disparity (what run_DE_*_batch writes, <stem>_filtered.pfm included;
+// NaN unknown) or KITTI's 16-bit disparity PNG (0 unknown).  Every pair gets <stem>_disp1.pfm, image2's disparity
+// warped to image1 (PFM of the positive disparity, NaN unknown); with --kitti <stem>_disp1<ext>, KITTI's 16-bit
+// disparity PNG (NaN as 0), so that <stem><ext>, the disparity of image1 and this file form a KITTI scene-flow
+// submission.  With --camera fx,fy,cx,cy,baseline,doffs also <stem>_sceneflow.pfm, a 3-channel PFM ("PF", rows
+// bottom-up) of the 3-D motion, NaN where unknown.  --gt-scene-flow GTLIST holds three files per pair: the ground-truth
+// disparities at t and at t+1 (KITTI's disp_occ_0 and disp_occ_1, PFM or PNG as above) and the flow (KITTI PNG or
+// .flo).  With verbosity > 0 every pair prints `SFEVAL <out> d1 O N P d2 O N P fl O N P sf O N P` (outliers, pixels
+// counted, percentage; KITTI's D1, D2, Fl and SF with an unknown estimate counted as an outlier) and the end
+// `SFEVAL (<P> pairs) ...`, with --bidirectional also per class of the forward consistency mask as EVAL.  A list
+// whose count or files do not match the pairs is refused before any device work; every other output keeps its
+// bytes.  Not with --warm-start; --camera on a flow binary needs --scene-flow.
+
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
   const size_t slash = path.find_last_of('/'), dot = path.find_last_of('.');
@@ -689,6 +704,38 @@ static void add_stats(ofdis_error_stats& t, const ofdis_error_stats& s) {
   for (int k = 0; k < 3; ++k) t.n_over[k] += s.n_over[k];
   t.n_outlier += s.n_outlier;
   t.sum_err += s.sum_err;
+}
+
+static void add_sf_stats(ofdis_sf_stats& t, const ofdis_sf_stats& s) {
+  t.n_d1 += s.n_d1; t.n_d2 += s.n_d2; t.n_fl += s.n_fl; t.n_sf += s.n_sf;
+  t.out_d1 += s.out_d1; t.out_d2 += s.out_d2; t.out_fl += s.out_fl; t.out_sf += s.out_sf;
+}
+
+// one SFEVAL line: a pair's output path (pairs 0), or the total of `pairs` pairs with the class name (empty: all)
+static void print_sfeval(const char* label, size_t pairs, const ofdis_sf_stats& s) {
+  if (pairs) printf("SFEVAL %s%s(%zu pairs)", label, *label ? " " : "", pairs);
+  else printf("SFEVAL %s", label);
+  const long long n[4] = {s.n_d1, s.n_d2, s.n_fl, s.n_sf}, o[4] = {s.out_d1, s.out_d2, s.out_fl, s.out_sf};
+  static const char* const kNames[4] = {"d1", "d2", "fl", "sf"};
+  for (int i = 0; i < 4; ++i) {
+    if (n[i]) printf(" %s %lld %lld %.6f", kNames[i], o[i], n[i], 100.0 * (double)o[i] / (double)n[i]);
+    else printf(" %s %lld %lld nan", kNames[i], o[i], n[i]);
+  }
+  printf("\n");
+}
+
+// a 3-channel PFM ("PF", w h, scale -1: little endian, rows bottom-up) of [h][w][3] floats, written as they are
+static void save_pfm3(const float* v, int w, int h, const char* filename) {
+  FILE* f = fopen(filename, "wb");
+  if (!f) {
+    cout << "WriteFile: could not open file" << endl;
+    return;
+  }
+  fprintf(f, "PF\n%d %d\n%f\n", w, h, -1.0f);
+  for (int y = h - 1; y >= 0; --y)
+    if (fwrite(v + (size_t)y * w * 3, sizeof(float), (size_t)w * 3, f) != (size_t)w * 3)
+      cout << "WriteFile: problem writing data" << endl;
+  fclose(f);
 }
 
 static const uint8_t kPngSig[8] = {0x89, 'P', 'N', 'G', 0x0d, 0x0a, 0x1a, 0x0a};
@@ -860,6 +907,7 @@ int main(int argc, char** argv) {
             "       [--color [--color-max M]] [--interpolate T] [--tracks PATH [--descriptors PATH]]\n"
             "       [--lr-check] [--speckle N R] [--fill] [--camera fx,fy,cx,cy,baseline,doffs]\n"
             "       [--global-motion similarity|affine|homography PATH [--stabilize RADIUS CROP DIR]]\n"
+            "       [--scene-flow DISPLIST [--gt-scene-flow GTLIST]]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -890,7 +938,10 @@ int main(int argc, char** argv) {
             "  <stem>_residual<ext>, <stem>_moving.pgm and <stem>_registered.png; not with --warm-start\n"
             "  --stabilize RADIUS CROP DIR: flow only, with --global-motion; every clip stabilised along its smoothed\n"
             "  camera path (RADIUS 1..64 frames each side, CROP 0 <= CROP < 0.5 cut from each side), written to\n"
-            "  DIR/stab_<clip>_<frame>.png, the corrections to DIR/stab.txt; not with --warm-start\n",
+            "  DIR/stab_<clip>_<frame>.png, the corrections to DIR/stab.txt; not with --warm-start\n"
+            "  --scene-flow DISPLIST (flow binaries): the disparities of image1 and image2 of every pair (PFM or KITTI\n"
+            "  PNG) give <stem>_disp1.pfm (<stem>_disp1<ext> with --kitti), and with --camera <stem>_sceneflow.pfm;\n"
+            "  --gt-scene-flow GTLIST: disp0, disp1 and flow ground truth per pair, SFEVAL lines; not with --warm-start\n",
             argv[0]);
     return 2;
   }
@@ -908,6 +959,8 @@ int main(int argc, char** argv) {
   const char* camera_arg = nullptr;  // --camera fx,fy,cx,cy,baseline,doffs
   const char* gm_arg[2] = {nullptr, nullptr};  // --global-motion MODEL PATH
   const char* stab_arg[3] = {nullptr, nullptr, nullptr};  // --stabilize RADIUS CROP DIR
+  const char* sf_list = nullptr;    // --scene-flow DISPLIST
+  const char* sf_gtlist = nullptr;  // --gt-scene-flow GTLIST
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -991,6 +1044,20 @@ int main(int argc, char** argv) {
       stab_arg[1] = argv[first_num + 2];
       stab_arg[2] = argv[first_num + 3];
       first_num += 4;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--scene-flow")) {
+      if (argc < first_num + 2 || sf_list) {
+        fprintf(stderr, "error: --scene-flow takes one disparity list file\n");
+        return 2;
+      }
+      sf_list = argv[first_num + 1];
+      first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt-scene-flow")) {
+      if (argc < first_num + 2 || sf_gtlist) {
+        fprintf(stderr, "error: --gt-scene-flow takes one ground-truth list file\n");
+        return 2;
+      }
+      sf_gtlist = argv[first_num + 1];
+      first_num += 2;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
         fprintf(stderr, "error: --gt takes one ground-truth list file\n");
@@ -1018,7 +1085,20 @@ int main(int argc, char** argv) {
     fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --tracks\n");
     return 2;
   }
-  const bool disp_on = lr_check || disp_fill || speckle_arg[0] || camera_arg;
+  if (sf_list && SELECTMODE != 1) {
+    fprintf(stderr, "error: --scene-flow joins flows with disparities; the stereo binaries take no --scene-flow\n");
+    return 2;
+  }
+  if (sf_list && warm) {
+    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --scene-flow\n");
+    return 2;
+  }
+  if (sf_gtlist && !sf_list) {
+    fprintf(stderr, "error: --gt-scene-flow evaluates the scene flow of --scene-flow; give --scene-flow too\n");
+    return 2;
+  }
+  // --camera on a flow binary belongs to --scene-flow
+  const bool disp_on = lr_check || disp_fill || speckle_arg[0] || (camera_arg && !sf_list);
   if (disp_on && SELECTMODE == 1) {
     fprintf(stderr, "error: --lr-check, --speckle, --fill and --camera filter stereo disparities; the flow binaries "
                     "take none of them\n");
@@ -1214,6 +1294,43 @@ int main(int argc, char** argv) {
       }
     }
   }
+  // --scene-flow / --gt-scene-flow: two and three files per pair, each checked against its pair's image size before
+  // any device work
+  vector<string> sf_files, sf_gts;
+  for (int li = 0; li < 2; ++li) {
+    const char* list = li ? sf_gtlist : sf_list;
+    vector<string>& files = li ? sf_gts : sf_files;
+    const size_t per = li ? 3 : 2;
+    if (!list) continue;
+    FILE* f = fopen(list, "r");
+    if (!f) {
+      fprintf(stderr, "error: cannot read %s\n", list);
+      return 1;
+    }
+    char g[4096];
+    while (fscanf(f, "%4095s", g) == 1) files.push_back(g);
+    fclose(f);
+    if (files.size() != per * jobs.size()) {
+      fprintf(stderr, "error: %s: %s lists %zu files for %zu pairs (%zu per pair)\n",
+              li ? "--gt-scene-flow" : "--scene-flow", list, files.size(), jobs.size(), per);
+      return 2;
+    }
+    vector<float> tmp;
+    for (size_t k = 0; k < files.size(); ++k) {
+      int iw = 0, ih = 0;
+      string err;
+      const Job& jb = jobs[k / per];
+      if (!image_size(jb.a.c_str(), iw, ih)) {
+        fprintf(stderr, "error: cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)\n", jb.a.c_str(),
+                jb.b.c_str());
+        return 1;
+      }
+      if (!read_gt_file(files[k].c_str(), iw, ih, li && k % 3 == 2 ? 2 : 1, tmp, err)) {
+        fprintf(stderr, "error: %s: %s\n", files[k].c_str(), err.c_str());
+        return 2;
+      }
+    }
+  }
   // --descriptors: every pair's frames hold an N x N patch, checked before any device work
   for (size_t k = 0; k < jobs.size() && desc_path; ++k) {
     int iw = 0, ih = 0;
@@ -1273,6 +1390,10 @@ int main(int argc, char** argv) {
   vector<ofdis_error_stats> eval_total(nclasses + 1), eval_pairs;  // [0]: all pixels, [1 + c]: class c
   memset(eval_total.data(), 0, sizeof(ofdis_error_stats) * eval_total.size());
   vector<float> gt_batch, gt_one;
+  // --scene-flow: the batch's disparities, ground truth and outputs; the totals ([0]: all pixels, [1 + c]: class c)
+  vector<float> sf_d0, sf_d1, sf_g0, sf_g1, sf_gf, sf_w, sf_m;
+  vector<ofdis_sf_stats> sf_pairs, sf_total(nclasses + 1);
+  memset(sf_total.data(), 0, sizeof(ofdis_sf_stats) * sf_total.size());
   timeval tv;
   gettimeofday(&tv, NULL);
   size_t done = 0, seq_pairs = 0, seq_decoded = 0, warm_pairs = 0;
@@ -1621,6 +1742,70 @@ int main(int argc, char** argv) {
           if (bidir) add_stats(eval_total[1 + c], eval_pairs[(size_t)k * nclasses + c]);
         }
     }
+    if (rc == OFDIS_OK && sf_list) {
+      const size_t pix = (size_t)w * h;
+      // positive disparities: the readers return this library's stereo convention, -d
+      auto load = [&](const string& path, int fnop, float sign, float* dst) {
+        string err;
+        if (!read_gt_file(path.c_str(), w, h, fnop, gt_one, err)) {
+          fprintf(stderr, "error: %s: %s\n", path.c_str(), err.c_str());
+          return false;
+        }
+        for (size_t i = 0; i < gt_one.size(); ++i) dst[i] = sign * gt_one[i];
+        return true;
+      };
+      sf_d0.resize(n * pix);
+      sf_d1.resize(n * pix);
+      sf_w.resize(n * pix);
+      sf_m.resize(camera_arg ? 3 * n * pix : 0);
+      bool ok = true;
+      for (int k = 0; k < n && ok; ++k)
+        ok = load(sf_files[2 * (j0 + k)], 1, -1.0f, &sf_d0[k * pix]) && load(sf_files[2 * (j0 + k) + 1], 1, -1.0f, &sf_d1[k * pix]);
+      if (sf_gtlist) {
+        sf_g0.resize(n * pix);
+        sf_g1.resize(n * pix);
+        sf_gf.resize(2 * n * pix);
+        for (int k = 0; k < n && ok; ++k)
+          ok = load(sf_gts[3 * (j0 + k)], 1, -1.0f, &sf_g0[k * pix]) && load(sf_gts[3 * (j0 + k) + 1], 1, -1.0f, &sf_g1[k * pix]) &&
+               load(sf_gts[3 * (j0 + k) + 2], 2, 1.0f, &sf_gf[2 * k * pix]);
+        sf_pairs.resize((size_t)n * nclasses);
+      }
+      if (!ok) {
+        ofdis_destroy(ctx);
+        return 1;
+      }
+      const ofdis_sf_gt sgt{sf_g0.data(), sf_g1.data(), sf_gf.data()};
+      rc = ofdis_scene_flow_fullres(ctx, 0, n, sf_d0.data(), sf_d1.data(), pix, 1.0f, camera_arg ? &dcam : nullptr,
+                                    sf_w.data(), nullptr, camera_arg ? sf_m.data() : nullptr, sf_gtlist ? &sgt : nullptr,
+                                    bidir ? masks.data() : nullptr, nclasses, sf_gtlist ? sf_pairs.data() : nullptr, w, h,
+                                    OFDIS_MEM_HOST);
+      for (int k = 0; k < n && rc == OFDIS_OK && sf_gtlist; ++k) {
+        ofdis_sf_stats all;
+        memset(&all, 0, sizeof(all));
+        for (int c = 0; c < nclasses; ++c) {
+          add_sf_stats(all, sf_pairs[(size_t)k * nclasses + c]);
+          add_sf_stats(sf_total[1 + c], sf_pairs[(size_t)k * nclasses + c]);
+        }
+        add_sf_stats(sf_total[0], all);
+        if (verbosity > 0) print_sfeval(jobs[j0 + k].out.c_str(), 0, all);
+      }
+      for (int k = 0; k < n && rc == OFDIS_OK; ++k) {
+        const float* d = &sf_w[k * pix];
+        if (kitti) {
+          vector<uint16_t> enc(pix);
+          for (size_t i = 0; i < pix; ++i)  // NaN fails d >= 0 and is written as 0
+            enc[i] = d[i] >= 0.0f ? (uint16_t)fminf(fmaxf(d[i] * 256.0f, 1.0f), 65535.0f) : (uint16_t)0;
+          save_png(enc.data(), w, h, 1, 16, with_suffix(jobs[j0 + k].out, "_disp1").c_str());
+        } else {
+          ImageF f;  // SavePFMFile writes -value: the positive disparity goes in as -d
+          f.w = w; f.h = h; f.c = 1;
+          f.px.resize(pix);
+          for (size_t i = 0; i < pix; ++i) f.px[i] = -d[i];
+          SavePFMFile(f, with_suffix(jobs[j0 + k].out, "_disp1", ".pfm").c_str());
+        }
+        if (camera_arg) save_pfm3(&sf_m[3 * k * pix], w, h, with_suffix(jobs[j0 + k].out, "_sceneflow", ".pfm").c_str());
+      }
+    }
     if (rc != OFDIS_OK) {
       fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
       ofdis_destroy(ctx);
@@ -1790,6 +1975,11 @@ int main(int argc, char** argv) {
     static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
     print_eval("", done, eval_total[0]);
     for (int c = 0; c < nclasses && bidir; ++c) print_eval(kClassNames[c], done, eval_total[1 + c]);
+  }
+  if (verbosity > 0 && sf_gtlist) {
+    static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
+    print_sfeval("", done, sf_total[0]);
+    for (int c = 0; c < nclasses && bidir; ++c) print_sfeval(kClassNames[c], done, sf_total[1 + c]);
   }
   return 0;
 }

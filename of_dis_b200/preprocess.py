@@ -1007,6 +1007,119 @@ def disparity_filter(F: np.ndarray, B: np.ndarray | None = None, swapped: bool =
     return disp, status, depth, xyz
 
 
+# ofdis_sf_stats (include/ofdis_b200.h), field for field
+SF_STATS_FIELDS = ("n_d1", "n_d2", "n_fl", "n_sf", "out_d1", "out_d2", "out_fl", "out_sf")
+SF_STATS_DTYPE = np.dtype([(k, "<i8") for k in SF_STATS_FIELDS])
+
+
+def _known_disp(d: np.ndarray) -> np.ndarray:
+    """0 <= d <= 1e9: NaN fails, -0 passes."""
+    return (d >= 0) & (d <= np.float32(1e9))
+
+
+def scene_flow(F: np.ndarray, disp0: np.ndarray, disp1: np.ndarray, edge_diff: float = 1.0, camera=None, gt=None,
+               classes: np.ndarray | None = None, nclasses: int = 1):
+    """ofdis_scene_flow_fullres bit for bit, float32 without contraction.  F: full-resolution flows, (h, w, 2) for one
+    pair or (n, h, w, 2), exactly what ofdis_get_flow_fullres returns; disp0, disp1: the positive disparities at t and
+    t+1, (h, w) or (n, h, w) float32 with NaN for unknown; camera: None or a mapping with STEREO_CAMERA_FIELDS; gt: None
+    or (disp0, disp1, flow) of the same shapes, with classes (uint8, the shape of disp0; None: class 0) and nclasses.
+    Returns (disp1_warped, status, motion, stats): float32 and uint8 of disp0's shape, motion (..., 3) float32 (None
+    without a camera), stats of SF_STATS_DTYPE, (nclasses,) for one pair or (n, nclasses) (None without gt).
+
+        target       (xs, ys) = (x + u, y + v); fails outside [0, w-1] x [0, h-1] or NaN
+        d1           corners x0 = floor(xs), x1 = min(x0 + 1, w - 1) (and y); four known corners with max - min <=
+                     edge_diff: bilinear, rows first; else the corner (fx >= 0.5 ? x1 : x0, fy >= 0.5 ? y1 : y0)
+        status       bit 0 d0 unknown, bit 1 the target fails, bit 2 d1 unknown (bit 1 clear)
+        disp1_warped d1 where bits 1 and 2 are clear, else qNaN
+        motion       P1 - P0 where status = 0 and d + doffs > 0 for both, P = (((x - cx) Z) / fx, ((y - cy) Z) / fy, Z)
+                     with Z = (fx * baseline) / (d + doffs) and P1 at (xs, ys); else qNaN
+        outliers     e > 3 and e > 0.05 g; D1 |d0 - G|, D2 |disp1_warped - G|, Fl |F - G|; an unknown estimate has
+                     e = +inf; each counts where its ground truth is known, SF where all three are, as any of them"""
+    f32 = np.float32
+    Fa = np.asarray(F, f32)
+    single = Fa.ndim == 3
+    if single:
+        Fa = Fa[None]
+    n, h, w, _ = Fa.shape
+    D0 = np.asarray(disp0, f32).reshape(n, h, w)
+    D1 = np.asarray(disp1, f32).reshape(n, h, w)
+    u, v = Fa[..., 0], Fa[..., 1]
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        xs = np.arange(w, dtype=f32)[None, None, :] + u
+        ys = np.arange(h, dtype=f32)[None, :, None] + v
+        inside = (xs >= 0) & (xs <= f32(w - 1)) & (ys >= 0) & (ys <= f32(h - 1))
+        xc = np.where(inside, xs, f32(0))
+        yc = np.where(inside, ys, f32(0))
+        x0 = np.floor(xc).astype(np.int64)
+        y0 = np.floor(yc).astype(np.int64)
+        x1 = np.minimum(x0 + 1, w - 1)
+        y1 = np.minimum(y0 + 1, h - 1)
+        fx = (xc - x0.astype(f32)).astype(f32)
+        fy = (yc - y0.astype(f32)).astype(f32)
+        k = np.arange(n)[:, None, None]
+        c00, c10, c01, c11 = D1[k, y0, x0], D1[k, y0, x1], D1[k, y1, x0], D1[k, y1, x1]
+        corners_known = _known_disp(c00) & _known_disp(c10) & _known_disp(c01) & _known_disp(c11)
+        hi = np.maximum(np.maximum(c00, c10), np.maximum(c01, c11))
+        lo = np.minimum(np.minimum(c00, c10), np.minimum(c01, c11))
+        blend = corners_known & ((hi - lo) <= f32(edge_diff))
+        gx, gy = f32(1) - fx, f32(1) - fy
+        r0 = c00 * gx + c10 * fx
+        r1 = c01 * gx + c11 * fx
+        near = np.where(fy >= f32(0.5), np.where(fx >= f32(0.5), c11, c01), np.where(fx >= f32(0.5), c10, c00))
+        d1 = np.where(blend, r0 * gy + r1 * fy, near).astype(f32)
+        k0 = _known_disp(D0)
+        k1 = inside & _known_disp(d1)
+        status = (np.where(k0, 0, 1) | np.where(inside, 0, 2) | np.where(inside & ~k1, 4, 0)).astype(np.uint8)
+        d1w = np.where(k1, d1, _QNAN).astype(f32)
+        motion = None
+        if camera is not None:
+            cam = {key: f32(camera[key]) for key in STEREO_CAMERA_FIELDS}
+            fb = f32(cam["fx"] * cam["baseline"])
+            s0 = (D0 + cam["doffs"]).astype(f32)
+            s1 = (d1 + cam["doffs"]).astype(f32)
+            ok = (status == 0) & (s0 > 0) & (s1 > 0)
+            Z0 = fb / np.where(ok, s0, f32(1))
+            Z1 = fb / np.where(ok, s1, f32(1))
+            X0 = ((np.arange(w, dtype=f32)[None, None, :] - cam["cx"]) * Z0) / cam["fx"]
+            Y0 = ((np.arange(h, dtype=f32)[None, :, None] - cam["cy"]) * Z0) / cam["fy"]
+            X1 = ((xs - cam["cx"]) * Z1) / cam["fx"]
+            Y1 = ((ys - cam["cy"]) * Z1) / cam["fy"]
+            motion = np.stack([X1 - X0, Y1 - Y0, Z1 - Z0], axis=-1).astype(f32)
+            motion = np.where(ok[..., None] & ~np.isnan(motion), motion, _QNAN).astype(f32)
+        stats = None
+        if gt is not None:
+            G0, G1, GF = (np.asarray(a, f32) for a in gt)
+            G0, G1, GF = G0.reshape(n, h, w), G1.reshape(n, h, w), GF.reshape(n, h, w, 2)
+            cls = np.zeros((n, h, w), np.uint8) if classes is None else np.asarray(classes, np.uint8).reshape(n, h, w)
+            assert classes is not None or nclasses == 1
+            lim, inf = f32(1e9), f32(np.inf)
+            kg0, kg1 = _known_disp(G0), _known_disp(G1)
+            Gu, Gv = GF[..., 0], GF[..., 1]
+            kgf = (np.abs(Gu) <= lim) & (np.abs(Gv) <= lim)
+            kf = (np.abs(u) <= lim) & (np.abs(v) <= lim)
+            du, dv = u - Gu, v - Gv
+            e0 = np.where(k0, np.abs(D0 - G0), inf)
+            e1 = np.where(k1, np.abs(d1w - G1), inf)
+            ef = np.where(kf, np.sqrt(du * du + dv * dv), inf)
+            gf = np.sqrt(Gu * Gu + Gv * Gv)
+
+            def out(e, g):
+                return (e > f32(3)) & (e > f32(0.05) * g)
+
+            o0, o1, of = out(e0, np.abs(G0)), out(e1, np.abs(G1)), out(ef, gf)
+            ksf = kg0 & kg1 & kgf
+            masks = (kg0, kg1, kgf, ksf, kg0 & o0, kg1 & o1, kgf & of, ksf & (o0 | o1 | of))
+            stats = np.zeros((n, nclasses), SF_STATS_DTYPE)
+            for p in range(n):
+                for c in range(nclasses):
+                    sel = cls[p] == c
+                    for name, m in zip(SF_STATS_FIELDS, masks):
+                        stats[p, c][name] = int((m[p] & sel).sum())
+    if single:
+        return d1w[0], status[0], None if motion is None else motion[0], None if stats is None else stats[0]
+    return d1w, status, motion, stats
+
+
 # ofdis_motion_params / ofdis_motion_stats (include/ofdis_b200.h), field for field
 MOTION_MODELS = {"similarity": 1, "affine": 2, "homography": 3}
 MOTION_PARAM_FIELDS = ("model", "step", "fb_check", "alpha", "beta", "hypotheses", "threshold", "refine", "seed")

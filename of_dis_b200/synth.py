@@ -110,6 +110,63 @@ def layered_stereo(h: int, w: int, channels: int = 1, seed: int = 0, d_bg: int =
     return q(left), q(right), gt, occluded
 
 
+def layered_scene_flow(h: int, w: int, channels: int = 1, seed: int = 0, d_bg: int = 8, d_fg=(24, 30), dx: int = 6,
+                       block=(0.3, 0.25, 0.6, 0.75)):
+    """Two stereo pairs, at t and t+1, of layered_stereo's scene in which the foreground rectangle moves: at t it covers
+    the fractions `block` = (x0, y0, x1, y1) of the left view at the integer disparity d_fg[0]; at t+1 it has moved
+    sideways by the integer dx pixels and has the disparity d_fg[1] (it came nearer or went away).  The background
+    stays at d_bg.  Both layers are crops of independent canvases (_canvas) sampled at integer positions, the
+    foreground's texture moving with it, so every visible point has exactly the same bytes in all four views.
+    Returns (frames, gt): frames (4, h, w[, 3]) uint8, L_t, R_t, L_t+1, R_t+1; gt a dict of (h, w) arrays in frame-t
+    coordinates: "disp0" the positive disparity at t, "disp1" that of the same point at t+1 (KITTI's disp_occ_1),
+    "flow" (h, w, 2) the left view's flow, all float32; "occluded" bool where the point's match in R_t, L_t+1 or
+    R_t+1 is hidden or outside the frame; and "disp_t1", L_t+1's own disparity map (frame-t+1 coordinates)."""
+    assert 0 <= d_bg < min(d_fg)
+    pad = max(d_fg) + abs(dx)
+    bg, m = _canvas(h, w + pad, channels, seed)
+    fg, _ = _canvas(h, w + pad, channels, seed + 1)
+    X0, Y0, X1, Y1 = int(block[0] * w), int(block[1] * h), int(block[2] * w), int(block[3] * h)
+    y, x = np.mgrid[0:h, 0:w]
+    in_rows = (y >= Y0) & (y < Y1)
+    wc = bg.shape[1]
+
+    def col(c):
+        return np.clip(m + c, 0, wc - 1)
+
+    def view(shift, d_f):
+        """The stereo pair with the rectangle moved by `shift`: left, right, the left view's disparity and where its
+        match in the right view is hidden or outside, and the rectangle's pixels."""
+        bx0, bx1 = X0 + shift, X1 + shift
+        in_fg = in_rows & (x >= bx0) & (x < bx1)
+        left = np.where(in_fg[..., None], fg[m + y, col(x - shift)], bg[m + y, col(x)])
+        xf = x + d_f
+        right_fg = in_rows & (xf >= bx0) & (xf < bx1)
+        right = np.where(right_fg[..., None], fg[m + y, col(xf - shift)], bg[m + y, col(x + d_bg)])
+        disp = np.where(in_fg, d_f, d_bg)
+        xr = x - disp
+        hidden = ~in_fg & in_rows & (xr + d_f >= bx0) & (xr + d_f < bx1)
+        return left, right, disp, (xr < 0) | hidden, in_fg
+
+    l0, r0, disp_t, occ0, fg0 = view(0, d_fg[0])
+    l1, r1, disp_t1, occ1, fg1 = view(dx, d_fg[1])
+    u = np.where(fg0, dx, 0)
+    xt = x + u
+    out = (xt < 0) | (xt > w - 1)
+    xtc = np.clip(xt, 0, w - 1)
+    covered = ~fg0 & fg1[y, xtc]  # a background point behind the rectangle at t+1
+    occluded = occ0 | out | covered | occ1[y, xtc]
+
+    def q(img):
+        img = np.clip(np.rint(img), 0, 255).astype(np.uint8)
+        return np.ascontiguousarray(img[..., 0] if channels == 1 else img)
+
+    frames = np.stack([q(l0), q(r0), q(l1), q(r1)])
+    gt = {"disp0": disp_t.astype(np.float32), "disp1": np.where(fg0, d_fg[1], d_bg).astype(np.float32),
+          "flow": np.stack([u, np.zeros_like(u)], -1).astype(np.float32), "occluded": occluded,
+          "disp_t1": disp_t1.astype(np.float32)}
+    return frames, gt
+
+
 def similarity_about_centre(h: int, w: int, angle_deg: float = 0.0, zoom: float = 1.0, shift=(0.0, 0.0)):
     """The 3 x 3 float64 map of pixel positions that rotates by angle_deg and scales by zoom about the frame's centre
     ((w-1)/2, (h-1)/2), then shifts by (dx, dy)."""
