@@ -271,14 +271,14 @@ void sor_workspace_need(const ofdis_ctx* c, int mc_lo, int mc_hi, size_t* recf4,
           }
 }
 
-// (Re)allocates the refinement planes of the finest level (mask, avg[C], 8 x deriv[C]) behind `recf4` float4 of SOR
+// (Re)allocates the refinement planes of the finest level (mask, 8 x deriv[C]) behind `recf4` float4 of SOR
 // lane rows per frame, and the chain's scratch for `chain_nb` bands per frame; all of it zeroed.  On failure the
 // previous buffers stay in place.
 bool alloc_refinement(ofdis_ctx* ctx, size_t recf4, int chain_nb) {
   const LevelGeom& Lf = ctx->lev[0];
   const size_t plane = (size_t)Lf.pitch * Lf.h, cap = (size_t)ctx->cap;
   const int C = ctx->prm.noc;
-  const size_t per_frame = plane * (1 + C + 8 * C) + recf4 * 4, chain_ints = 1 + (size_t)chain_nb * cap;
+  const size_t per_frame = plane * (1 + 8 * C) + recf4 * 4, chain_ints = 1 + (size_t)chain_nb * cap;
   float* planes = nullptr;
   int* chain = nullptr;
   if (cudaMalloc((void**)&planes, sizeof(float) * per_frame * cap) != cudaSuccess) return false;
@@ -298,7 +298,6 @@ bool alloc_refinement(ofdis_ctx* ctx, size_t recf4, int chain_nb) {
   VarRefPlanes& P = ctx->planes;
   P.rec = reinterpret_cast<float4*>(q); q += recf4 * 4 * cap;   // first (alignment)
   P.mask = q; q += plane * cap;
-  P.avg = q; q += plane * C * cap;
   for (int k = 0; k < 8; ++k) { P.deriv[k] = q; q += plane * C * cap; }
   P.plane = plane;
   ctx->rec_f4 = recf4;

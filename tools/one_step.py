@@ -1,4 +1,4 @@
-"""One eager step (48 launches at operating point 2) of a B-pair batch, for ncu launch lists:
+"""One eager step (39 launches at operating point 2) of a B-pair batch, for ncu launch lists:
    ncu --metrics gpu__time_duration.sum,smsp__inst_executed.sum --clock-control none --csv \
        --log-file x.csv python tools/one_step.py [B] [steps]"""
 import sys
