@@ -1705,6 +1705,10 @@ def traj_frame_hist(contrib: np.ndarray, xs: np.ndarray, ys: np.ndarray, p) -> n
     N, ns = int(p["N"]), int(p["ns"])
     c = N // ns
     T = xs.size
+    chunk = max(1, (1 << 24) // (((c * c + 31) // 32) * 32 * TRAJ_BINS))  # tracks per 64 MB of lane sums
+    if T > chunk:
+        return np.concatenate([traj_frame_hist(contrib, xs[i:i + chunk], ys[i:i + chunk], p)
+                               for i in range(0, T, chunk)])
     xr = np.floor(xs.astype(f32) + f32(0.5)).astype(np.int64)
     yr = np.floor(ys.astype(f32) + f32(0.5)).astype(np.int64)
     ox = np.minimum(np.maximum(xr - N // 2, 0), w - N)
@@ -1738,50 +1742,51 @@ def traj_frame_hist(contrib: np.ndarray, xs: np.ndarray, ys: np.ndarray, p) -> n
     return out
 
 
-def traj_segment_test(pos: np.ndarray, disp: np.ndarray, p):
-    """The tests of one completed segment: pos (L+1, 2), disp (L, 2) float32.  Returns (why, stats, dsum): why 0
-    emitted, 1 static, 2 erratic, 3 jump, 4 camera; stats (mean_x, mean_y, sd_x, sd_y, length)."""
+def traj_segment_tests(pos: np.ndarray, disp: np.ndarray, p):
+    """The tests of S completed segments: pos (S, L+1, 2), disp (S, L, 2) float32.  Returns (why, stats, dsum): why
+    (S,) 0 emitted, 1 static, 2 erratic, 3 jump, 4 camera; stats (mean_x, mean_y, sd_x, sd_y, length) and dsum (S,)
+    float32, each sum over j in order."""
     f32 = np.float32
-    L = disp.shape[0]
+    S, L = disp.shape[:2]
     fn = f32(L + 1)
+    z = lambda: np.zeros(S, f32)  # noqa: E731
     with np.errstate(invalid="ignore", over="ignore"):
-        sx = sy = f32(0)
+        sx, sy = z(), z()
         for j in range(L + 1):
-            sx = f32(sx + pos[j, 0])
-            sy = f32(sy + pos[j, 1])
-        mx, my = f32(sx / fn), f32(sy / fn)
-        vx = vy = f32(0)
+            sx = sx + pos[:, j, 0]
+            sy = sy + pos[:, j, 1]
+        mx, my = sx / fn, sy / fn
+        vx, vy = z(), z()
         for j in range(L + 1):
-            dx, dy = f32(pos[j, 0] - mx), f32(pos[j, 1] - my)
-            vx = f32(vx + dx * dx)
-            vy = f32(vy + dy * dy)
-        sdx, sdy = np.sqrt(f32(vx / fn)), np.sqrt(f32(vy / fn))
-        length = smax = f32(0)
+            dx, dy = pos[:, j, 0] - mx, pos[:, j, 1] - my
+            vx = vx + dx * dx
+            vy = vy + dy * dy
+        sdx, sdy = np.sqrt(vx / fn), np.sqrt(vy / fn)
+        length, smax = z(), z()
         for j in range(L):
-            dx, dy = f32(pos[j + 1, 0] - pos[j, 0]), f32(pos[j + 1, 1] - pos[j, 1])
-            s = np.sqrt(f32(dx * dx + dy * dy))
-            length = f32(length + s)
-            if s > smax:
-                smax = s
-        dsum = dmax = f32(0)
-        known = True
+            dx, dy = pos[:, j + 1, 0] - pos[:, j, 0], pos[:, j + 1, 1] - pos[:, j, 1]
+            s = np.sqrt(dx * dx + dy * dy)
+            length = length + s
+            smax = np.where(s > smax, s, smax)
+        dsum, dmax = z(), z()
+        known = np.ones(S, bool)
         for j in range(L):
-            du, dv = disp[j, 0], disp[j, 1]
-            a = np.sqrt(f32(du * du + dv * dv))
-            known = known and bool(a <= _FLT_MAX)
-            dsum = f32(dsum + a)
-            if a > dmax:
-                dmax = a
-    stats = (mx, my, sdx, sdy, length)
-    if sdx < f32(p["min_var"]) and sdy < f32(p["min_var"]):
-        return 1, stats, dsum
-    if sdx > f32(p["max_var"]) or sdy > f32(p["max_var"]):
-        return 2, stats, dsum
-    if smax > f32(p["max_dis"]) and smax > f32(0.7) * length:
-        return 3, stats, dsum
-    if not known or dmax <= f32(p["min_disp"]):
-        return 4, stats, dsum
-    return 0, stats, dsum
+            du, dv = disp[:, j, 0], disp[:, j, 1]
+            a = np.sqrt(du * du + dv * dv)
+            known &= a <= _FLT_MAX
+            dsum = dsum + a
+            dmax = np.where(a > dmax, a, dmax)
+        why = np.where(~known | (dmax <= f32(p["min_disp"])), 4, 0)
+        why = np.where((smax > f32(p["max_dis"])) & (smax > f32(0.7) * length), 3, why)
+        why = np.where((sdx > f32(p["max_var"])) | (sdy > f32(p["max_var"])), 2, why)
+        why = np.where((sdx < f32(p["min_var"])) & (sdy < f32(p["min_var"])), 1, why)
+    return why, (mx, my, sdx, sdy, length), dsum
+
+
+def traj_segment_test(pos: np.ndarray, disp: np.ndarray, p):
+    """traj_segment_tests of one segment: pos (L+1, 2), disp (L, 2) float32; why an int, the rest float32 scalars."""
+    why, stats, dsum = traj_segment_tests(np.asarray(pos, np.float32)[None], np.asarray(disp, np.float32)[None], p)
+    return int(why[0]), tuple(v[0] for v in stats), dsum[0]
 
 
 class TrajStream:
@@ -1811,13 +1816,14 @@ class TrajStream:
         return self.tracks
 
     def _emit(self, disp, a, dsum):
+        """The descriptors (S, dim) of S segments: disp (S, L, 2), a (S, nt, ns^2, 33), dsum (S,)."""
         f32 = np.float32
-        shape = (disp / dsum).astype(f32).reshape(-1)
-        parts = [shape]
+        S = dsum.size
+        parts = [(disp / dsum[:, None, None]).astype(f32).reshape(S, -1)]
         for d in range(4):
             lo, nb = _TRAJ_LO[d], _TRAJ_NB[d]
-            parts.append((a[:, :, lo:lo + nb] / f32(self.tl)).astype(f32).reshape(-1))
-        return np.concatenate(parts)
+            parts.append((a[..., lo:lo + nb] / f32(self.tl)).astype(f32).reshape(S, -1))
+        return np.concatenate(parts, 1)
 
     def advance(self, frames, fw, bw, models=None):
         """Returns (lists, records, desc, n_desc), as Context.traj_advance on the host."""
@@ -1851,22 +1857,23 @@ class TrajStream:
             keep = np.isin(tr["id"], adv["id"])
             step, start, pos, disp, acc = (a[keep] for a in (self.step, self.start, self.pos, self.disp, self.acc))
             step = step + 1
-            ne = 0
-            for i in np.flatnonzero(step == L):
-                pos[i, L, 0], pos[i, L, 1] = adv["x"][i], adv["y"][i]
-                why, st, dsum = traj_segment_test(pos[i], disp[i], p)
-                if why:
-                    self.tstats[TRAJ_STATS_FIELDS[why]] += 1
-                else:
-                    rec = np.zeros(1, TRAJ_RECORD_DTYPE)
-                    rec["id"], rec["start"] = adv["id"][i], start[i]
-                    for key, val in zip(tkeys, st):
-                        rec[key] = val
-                    recs.append(rec)
-                    descs.append(self._emit(disp[i], acc[i], dsum))
-                    ne += 1
-                step[i] = 0
-                start[i] += L
+            done = np.flatnonzero(step == L)  # in list order, the order of the records
+            pos[done, L, 0], pos[done, L, 1] = adv["x"][done], adv["y"][done]
+            why, st, dsum = traj_segment_tests(pos[done], disp[done], p)
+            for r in range(1, len(TRAJ_STATS_FIELDS)):
+                self.tstats[TRAJ_STATS_FIELDS[r]] += int((why == r).sum())
+            em = why == 0
+            ne = int(em.sum())
+            if ne:
+                e = done[em]
+                rec = np.zeros(ne, TRAJ_RECORD_DTYPE)
+                rec["id"], rec["start"] = adv["id"][e], start[e]
+                for key, val in zip(tkeys, st):
+                    rec[key] = val[em]
+                recs.append(rec)
+                descs.append(self._emit(disp[e], acc[e], dsum[em]))
+            step[done] = 0
+            start[done] += L
             self.tstats["emitted"] += ne
             n_desc.append(ne)
             tracks, self.next_id = _track_seed(clip[k], adv, self.next_id, self.stats, self.tp)
@@ -1881,7 +1888,7 @@ class TrajStream:
             self.fr += 1
         dim = traj_dim(p)
         records = np.concatenate(recs) if recs else np.zeros(0, TRAJ_RECORD_DTYPE)
-        desc = np.stack(descs).astype(f32) if descs else np.zeros((0, dim), f32)
+        desc = np.concatenate(descs).astype(f32) if descs else np.zeros((0, dim), f32)
         return lists, records, desc, np.array(n_desc, np.int32)
 
     def track_stats(self):
