@@ -699,6 +699,79 @@ int ofdis_traj_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned ch
  * live stage or with a NULL out. */
 int ofdis_traj_stats_get(const ofdis_ctx* ctx, ofdis_traj_stats* out);
 
+/* Fisher vectors of descriptors (extension): one fixed-length vector per clip from its descriptors, the encoding of
+ * Wang and Schmid's improved dense trajectories -- PCA per descriptor block, a diagonal GMM per block and the improved
+ * Fisher vector (Perronnin, Sanchez and Mensink, ECCV 2010).  The context owns one encoder: the device codebook, the
+ * float64 statistics of the clip being encoded and its counters.  It persists across calls and across ofdis_run and the
+ * other extensions; ofdis_fisher_begin resets it and ofdis_destroy frees it.  It reads no flow: any context may use
+ * it.  Float32 without contraction, IEEE division and square root; the statistics and the normalisation float64;
+ * preprocess.FisherStream restates it bit for bit.  Per descriptor x and block b (offset o, dim_in D, dim P):
+ *   Projection.  y_d = sum_i proj[d][i] * (x[o+i] - mean[i]), from +0.0f in increasing i.
+ *   Log-likelihood.  z_kd = (y_d - mu[k][d]) * isig[k][d]; q_k = sum_d z_kd * z_kd from +0.0f in increasing d;
+ *   ll_k = c_k - 0.5f * q_k.
+ *   Posteriors.  m = max_k ll_k; e_k = exp_f32(ll_k - m); s = sum_k e_k from +0.0f in increasing k; g_k = e_k / s.
+ *   exp_f32 (preprocess.exp_f32): n = rintf(x * 1.44269504f), r = (x - n * 0.693145751953125f) - n * 1.42860677e-06f,
+ *   p = 1/k! for k = 7 .. 0 in Horner form (p = p * r + c_k, c_7 .. c_3 = 0.000198412701f, 0.00138888892f,
+ *   0.00833333377f, 0.0416666679f, 0.166666672f, then 0.5f, 1, 1), times 2^n built in the exponent field; +0 for x
+ *   < -87 (e^x below FLT_MIN), exactly 1 at 0; within 2 ulp of float64 exp on [-87, 0].
+ *   Skipped.  The block of x is skipped when some y_d, some q_k or m is not finite (a non-finite z makes q_k infinite;
+ *   skipping it keeps 0 * inf out of the sums).  It is counted in the block's `skipped` and adds nothing.
+ *   Statistics, float64, per block and Gaussian, plain sequential sums over the clip's descriptors in push order (so
+ *   they do not depend on how the clip is cut into pushes): S0_k += (double)g_k; S1_kd += (double)g_k * (double)z_kd;
+ *   S2_kd += (double)g_k * ((double)z_kd * (double)z_kd).  N_b counts the descriptors block b did not skip.
+ *   Vector, per block, float64: u_kd = S1_kd / (N_b * sqrt(w_k)), v_kd = (S2_kd - S0_k) / (N_b * sqrt(2 * w_k)),
+ *   laid out [u (K x P), v (K x P)]; each entry t becomes t < 0 ? -sqrt(|t|) : sqrt(|t|); then the sum of squares,
+ *   256 partial sums over the indices = j (mod 256) in increasing index, then the partials in increasing j; each
+ *   entry is divided by its square root when that is > 0 and rounded to float32.  N_b = 0 gives a block of zeros.
+ *   The clip's vector is the blocks in order, 2K * sum P floats (109,056 with IDT's blocks, P = D / 2, at K = 256).
+ *   Departures from VLFeat's vl_fisher: every posterior counts (VLFeat drops those below 1e-6), and the sums are
+ *   float64 and sequential.
+ * IDT's blocks follow from ofdis_traj_params, as preprocess.fisher_blocks gives them: shape 2L, HOG nt*ns*ns*8, HOF nt*ns*ns*9, MBHx and
+ * MBHy nt*ns*ns*8 each -- 30/96/108/96/96 of the 426 floats with the defaults. */
+#define OFDIS_FISHER_MAX_BLOCKS 8
+typedef struct ofdis_fisher_block { int offset, dim_in, dim; } ofdis_fisher_block;
+typedef struct ofdis_fisher_codebook {
+  int K;             /* Gaussians per block, 1 .. 256 */
+  int desc_dim;      /* floats per descriptor, >= 1 */
+  int nblocks;       /* 1 .. OFDIS_FISHER_MAX_BLOCKS */
+  ofdis_fisher_block blocks[OFDIS_FISHER_MAX_BLOCKS];  /* 1 <= dim <= dim_in <= 512, offset >= 0, offset + dim_in
+                                                         <= desc_dim */
+  /* host float32, per block in order: mean[dim_in], proj[dim][dim_in], mu[K][dim], isig[K][dim] (1/sigma, finite,
+   * > 0), c[K] (log w_k - sum_d log sigma_kd, finite), w[K] (finite, > 0) -- the body of the codebook file
+   * (preprocess.write_fisher_codebook: "OFDISFV1", int32 K, nblocks, desc_dim, offset/dim_in/dim per block, body) */
+  const float* params;
+} ofdis_fisher_codebook;
+typedef struct ofdis_fisher_stats {
+  long long pushed;                            /* descriptors pushed since the last begin or take */
+  long long n[OFDIS_FISHER_MAX_BLOCKS];        /* N_b */
+  long long skipped[OFDIS_FISHER_MAX_BLOCKS];  /* the skipped, per block */
+} ofdis_fisher_stats;  /* 136 bytes */
+/* Validates the codebook on the host (every range above, every array finite, isig and w > 0, else OFDIS_ERR_ARG,
+ * which leaves a live encoder as it was), uploads it and resets the statistics.  Allocates the workspace -- the codebook, 8 * K * sum(1 + 2P) bytes of
+ * statistics, and per chunk of 4096 descriptors the host-input staging (4 * desc_dim bytes each), y (4 * sum P),
+ * the posteriors (4 * K * nblocks) and the skip flags (nblocks), plus the host-output vector: about 30 MB with IDT's
+ * blocks at K = 256 -- which grows, never shrinks and is freed by ofdis_destroy. */
+int ofdis_fisher_begin(ofdis_ctx* ctx, const ofdis_fisher_codebook* cb);
+/* Adds n descriptors desc ([n][desc_dim] float32 in memkind) to the clip, in order; host input goes through the
+ * staging in chunks of 4096.  3 launches per chunk of 4096 descriptors, no host round trip inside the call, one
+ * synchronise at the end; n = 0 does nothing.  n < 0, a NULL desc with n > 0, a device desc that is not 4-byte aligned,
+ * or no live encoder is OFDIS_ERR_ARG.  A call that fails on the way leaves the encoder to a new ofdis_fisher_begin. */
+int ofdis_fisher_push(ofdis_ctx* ctx, const float* desc, long n, int memkind);
+/* Ends the clip: its vector to fv (2K * sum P floats, may be NULL), the raw statistics [nblocks]{S0[K], S1[K][P],
+ * S2[K][P]} float64 to stats (may be NULL; what an EM step needs), both in memkind (device: fv 4-byte, stats 8-byte
+ * aligned, else OFDIS_ERR_ARG), and the counters to *out (host, may be NULL).  Then resets the statistics and
+ * counters for the next clip; the codebook stays.  One launch when fv is given, none without; one synchronise at the end.  No live encoder is
+ * OFDIS_ERR_ARG; a call that fails on the way leaves the encoder to a new ofdis_fisher_begin. */
+int ofdis_fisher_take(ofdis_ctx* ctx, float* fv, double* stats, ofdis_fisher_stats* out, int memkind);
+/* ofdis_traj_advance (same frames, slots, points, counts, n_desc and errors) whose emitted segments go, in the order
+ * of ofdis_traj_advance's output, straight into the live encoder as an ofdis_fisher_push would take them: the
+ * descriptors stay in the descriptor stage's device output and never cross to the host.  Adds 3 launches per chunk of
+ * 4096 segments and one synchronise to ofdis_traj_advance's.  No live encoder, or one whose desc_dim is not the
+ * descriptors' dim, is OFDIS_ERR_ARG; a call that fails on the way leaves both stages to a new begin. */
+int ofdis_traj_advance_fisher(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames,
+                              size_t frame_stride, const double* models, ofdis_track_point* points, int* counts,
+                              int* n_desc, int width_org, int height_org, int memkind);
+
 /* Video stabilisation (extension): a Gaussian-smoothed camera path streamed through a clip, from the per-pair models
  * of ofdis_global_motion_fullres, and every frame warped onto it on the device (the motion filter of Matsushita et al.,
  * "Full-frame video stabilization", CVPR 2005, and of OpenCV's videostab).  The context owns one stabiliser: the

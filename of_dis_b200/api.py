@@ -14,10 +14,11 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import (DISP_FILTER_FIELDS, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
+from .preprocess import (DISP_FILTER_FIELDS, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
                          STAB_FRAME_DTYPE, STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS,
                          TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
-                         gaussian_weights, motion_params, traj_bound, traj_dim)
+                         fisher_fit, fisher_pack, fisher_sizes, gaussian_weights, motion_params,
+                         traj_bound, traj_dim)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("OFDIS_LIB") or os.path.join(_HERE, "lib", "libofdis_b200.so")  # OFDIS_LIB: experiments only
@@ -42,6 +43,7 @@ EXPORTS = [
     "ofdis_track_begin", "ofdis_track_advance", "ofdis_track_stats_get", "ofdis_disparity_fullres",
     "ofdis_global_motion_fullres", "ofdis_stab_begin", "ofdis_stab_push", "ofdis_stab_finish",
     "ofdis_traj_begin", "ofdis_traj_advance", "ofdis_traj_stats_get", "ofdis_scene_flow_fullres",
+    "ofdis_fisher_begin", "ofdis_fisher_push", "ofdis_fisher_take", "ofdis_traj_advance_fisher",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -136,6 +138,26 @@ class TrajStats(ctypes.Structure):
     _fields_ = [(k, ctypes.c_longlong) for k in TRAJ_STATS_FIELDS]
 
 
+class FisherBlock(ctypes.Structure):
+    """ofdis_fisher_block (include/ofdis_b200.h)."""
+    _fields_ = [("offset", ctypes.c_int), ("dim_in", ctypes.c_int), ("dim", ctypes.c_int)]
+
+
+class FisherCodebook(ctypes.Structure):
+    """ofdis_fisher_codebook (include/ofdis_b200.h); params points at a packed float32 body the caller keeps alive."""
+    _fields_ = [("K", ctypes.c_int), ("desc_dim", ctypes.c_int), ("nblocks", ctypes.c_int),
+                ("blocks", FisherBlock * FISHER_MAX_BLOCKS), ("params", ctypes.c_void_p)]
+
+
+class FisherStats(ctypes.Structure):
+    """ofdis_fisher_stats (include/ofdis_b200.h); FISHER_STATS_DTYPE is the same record as numpy sees it."""
+    _fields_ = [("pushed", ctypes.c_longlong), ("n", ctypes.c_longlong * FISHER_MAX_BLOCKS),
+                ("skipped", ctypes.c_longlong * FISHER_MAX_BLOCKS)]
+
+
+assert ctypes.sizeof(FisherStats) == FISHER_STATS_DTYPE.itemsize
+
+
 class OfdisError(RuntimeError):
     pass
 
@@ -213,6 +235,11 @@ def lib():
         L.ofdis_stab_push.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 2 + [ctypes.c_size_t] + \
             [ctypes.c_void_p] * 3 + [ctypes.c_int]
         L.ofdis_stab_finish.argtypes = [ctypes.c_void_p] + [ctypes.c_void_p] * 3 + [ctypes.c_int]
+        L.ofdis_fisher_begin.argtypes = [ctypes.c_void_p, ctypes.POINTER(FisherCodebook)]
+        L.ofdis_fisher_push.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_long, ctypes.c_int]
+        L.ofdis_fisher_take.argtypes = [ctypes.c_void_p] + [ctypes.c_void_p] * 3 + [ctypes.c_int]
+        L.ofdis_traj_advance_fisher.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
+            [ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -886,6 +913,63 @@ class Context:
         self._ck(lib().ofdis_stab_finish(self._h, _ptr(dst), _ptr(info), ctypes.byref(n_out), memkind))
         k = n_out.value
         return (dst[:k] if memkind == MEM_HOST else (dst, k)), info[:k].copy()
+
+    def fisher_begin(self, codebook):
+        """Resets the context's Fisher encoder on `codebook` (ofdis_fisher_begin; preprocess.FisherStream restates the
+        encoder): a dict of preprocess.fisher_unpack / read_fisher_codebook."""
+        K, blocks = int(codebook["K"]), [tuple(int(v) for v in b) for b in codebook["blocks"]]
+        body = np.ascontiguousarray(fisher_pack(codebook), np.float32)
+        c = FisherCodebook()
+        c.K, c.desc_dim, c.nblocks = K, int(codebook["desc_dim"]), len(blocks)
+        if len(blocks) > FISHER_MAX_BLOCKS or body.size != fisher_sizes(K, blocks)["body"]:
+            raise ValueError("fisher_begin: %d blocks, body of %d floats" % (len(blocks), body.size))
+        for b, (o, di, d) in enumerate(blocks):
+            c.blocks[b] = FisherBlock(o, di, d)
+        c.params = body.ctypes.data
+        self._ck(lib().ofdis_fisher_begin(self._h, ctypes.byref(c)))
+        self._fisher = (K, blocks, int(codebook["desc_dim"]))
+
+    def fisher_push(self, desc, memkind=MEM_HOST, n=None):
+        """Adds descriptors to the clip (ofdis_fisher_push): host (n, desc_dim) float32, or with memkind=MEM_DEVICE
+        a device address of n descriptors."""
+        if memkind == MEM_HOST:
+            D = getattr(self, "_fisher", (0, [], 0))[2]
+            desc = np.ascontiguousarray(desc, np.float32)
+            if desc.size and (desc.ndim != 2 or desc.shape[1] != D):
+                raise ValueError("fisher_push: desc must be (n, %d) float32" % D)
+            n = desc.shape[0] if desc.ndim == 2 else 0
+        elif n is None:
+            raise ValueError("fisher_push: device input needs n, the number of descriptors at the address")
+        self._ck(lib().ofdis_fisher_push(self._h, _ptr(desc), int(n), memkind))
+
+    def fisher_take(self, memkind=MEM_HOST, fv=None, stats=None, with_fv=True, with_stats=True):
+        """Ends the clip (ofdis_fisher_take).  Host: returns (fv float32 (2K sum dim,), stats float64, counters) --
+        counters a dict with `pushed` and per-block `n` and `skipped` arrays -- fv or stats None where not asked for.
+        With memkind=MEM_DEVICE fv and stats are device addresses the caller owns (or None) and counters is returned."""
+        K, blocks, _ = getattr(self, "_fisher", (1, [(0, 1, 1)], 1))
+        sz = fisher_sizes(K, blocks)
+        if memkind == MEM_HOST:
+            fv = np.empty(sz["fv"], np.float32) if with_fv else None
+            stats = np.empty(sz["stats"], np.float64) if with_stats else None
+        st = FisherStats()
+        self._ck(lib().ofdis_fisher_take(self._h, _ptr(fv), _ptr(stats), ctypes.byref(st), memkind))
+        nb = len(blocks)
+        counters = {"pushed": int(st.pushed), "n": np.array(st.n[:nb], np.int64),
+                    "skipped": np.array(st.skipped[:nb], np.int64)}
+        return counters if memkind != MEM_HOST else (fv, stats, counters)
+
+    def fisher_fit(self, samples, blocks, dims, K=256, iters=10, seed=0, var_floor=1e-3):
+        """preprocess.fisher_fit with the E-step on the device: each iteration is a fisher_begin, one push of the
+        samples and a take of the statistics; the M-step runs on the host.  Returns the same codebook bytes as
+        preprocess.fisher_fit."""
+        x = np.ascontiguousarray(samples, np.float32)
+
+        def estep(cb, xs):
+            self.fisher_begin(cb)
+            self.fisher_push(xs)
+            return self.fisher_take(with_fv=False)[1]
+
+        return fisher_fit(x, blocks, dims, K, iters, seed, var_floor, estep=estep)
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

@@ -114,6 +114,15 @@ struct ofdis_ctx {
   StabGeom sgeom{};
   long long stab_last = 0, stab_next = 0;
   bool stab_on = false;
+  // the Fisher encoder of ofdis_fisher_begin / ofdis_fisher_push / ofdis_fisher_take: its workspace (FisherWork), the
+  // geometry of the last begin and the descriptors pushed since it or the last take; grows, never shrinks; never
+  // touched by ofdis_run
+  void* d_fisher = nullptr;
+  size_t fisher_bytes = 0;
+  FisherWork fisher{};
+  FisherGeom fgeom{};
+  long long fisher_pushed = 0;
+  bool fisher_on = false;
   std::vector<float*> d_flow;   // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -486,6 +495,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_motion);
   cudaFree(ctx->d_traj);
   cudaFree(ctx->d_stab);
+  cudaFree(ctx->d_fisher);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -1602,17 +1612,23 @@ int ofdis_traj_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const ofd
   return OFDIS_OK;
 }
 
-int ofdis_traj_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames, size_t frame_stride,
-                       const double* models, ofdis_track_point* points, int* counts, ofdis_traj_record* records,
-                       float* desc, int* n_desc, int width_org, int height_org, int memkind) {
+static int fisher_push_chunks(ofdis_ctx* ctx, const float* desc, long n, bool host);
+
+// ofdis_traj_advance, and with to_fisher (records and desc unused) ofdis_traj_advance_fisher: the emitted segments'
+// descriptors stay in the stage's device output and go into the live encoder
+static int traj_advance_impl(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames, size_t frame_stride,
+                             const double* models, ofdis_track_point* points, int* counts, ofdis_traj_record* records,
+                             float* desc, int* n_desc, int width_org, int height_org, int memkind, bool to_fisher) {
   if (!ctx) return OFDIS_ERR_ARG;
   if (ctx->nop != 2 || f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || b0 < 0 || b0 > ctx->max_frames - (f1 - f0) ||
-      !frames || !points || !counts || !records || !desc || !n_desc ||
+      !frames || !points || !counts || (!to_fisher && (!records || !desc)) || !n_desc ||
       (memkind == OFDIS_MEM_DEVICE && (reinterpret_cast<uintptr_t>(points) % 4 ||
                                        reinterpret_cast<uintptr_t>(records) % 4 ||
                                        reinterpret_cast<uintptr_t>(desc) % 4)))
     return fail(ctx, OFDIS_ERR_ARG, "traj_advance: bad argument");
   if (!ctx->traj_on || !ctx->track_on) return fail(ctx, OFDIS_ERR_ARG, "traj_advance: no ofdis_traj_begin");
+  if (to_fisher && (!ctx->fisher_on || ctx->fgeom.desc_dim != ctx->trgeom.dim))
+    return fail(ctx, OFDIS_ERR_ARG, "traj_advance_fisher: no live encoder of the descriptors' size");
   int cx, cy;
   int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
   if (rc) return rc;
@@ -1644,8 +1660,8 @@ int ofdis_traj_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned ch
     stride = hwc;
   }
   ofdis_track_point* out = memkind == OFDIS_MEM_DEVICE ? points : ctx->track_out;
-  ofdis_traj_record* rout = memkind == OFDIS_MEM_DEVICE ? records : ctx->traj_rec;
-  float* dout = memkind == OFDIS_MEM_DEVICE ? desc : ctx->traj_desc;
+  ofdis_traj_record* rout = memkind == OFDIS_MEM_DEVICE && !to_fisher ? records : ctx->traj_rec;
+  float* dout = memkind == OFDIS_MEM_DEVICE && !to_fisher ? desc : ctx->traj_desc;
   const LevelGeom g = stepped(ctx->lev[0], D);
   // a call that fails on the way leaves the tracker and the descriptor stage to a new ofdis_traj_begin
   ctx->track_on = false;
@@ -1680,16 +1696,36 @@ int ofdis_traj_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned ch
                            sizeof(ofdis_track_point) * counts[k], cudaMemcpyDeviceToHost, ctx->stream));
     size_t total = 0;
     for (int k = 0; k < n; ++k) total += (size_t)n_desc[k];
-    if (total) {
+    if (total && !to_fisher) {
       CK(cudaMemcpyAsync(records, rout, sizeof(ofdis_traj_record) * total, cudaMemcpyDeviceToHost, ctx->stream));
       CK(cudaMemcpyAsync(desc, dout, sizeof(float) * tg.dim * total, cudaMemcpyDeviceToHost, ctx->stream));
     }
     CK(cudaStreamSynchronize(ctx->stream));
   }
+  if (to_fisher) {
+    long total = 0;
+    for (int k = 0; k < n; ++k) total += n_desc[k];
+    rc = fisher_push_chunks(ctx, dout, total, false);
+    if (rc) return rc;
+  }
   ctx->traj_frame += n;
   ctx->track_on = true;
   ctx->traj_on = true;
   return OFDIS_OK;
+}
+
+int ofdis_traj_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames, size_t frame_stride,
+                       const double* models, ofdis_track_point* points, int* counts, ofdis_traj_record* records,
+                       float* desc, int* n_desc, int width_org, int height_org, int memkind) {
+  return traj_advance_impl(ctx, f0, f1, b0, frames, frame_stride, models, points, counts, records, desc, n_desc,
+                           width_org, height_org, memkind, false);
+}
+
+int ofdis_traj_advance_fisher(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* frames,
+                              size_t frame_stride, const double* models, ofdis_track_point* points, int* counts,
+                              int* n_desc, int width_org, int height_org, int memkind) {
+  return traj_advance_impl(ctx, f0, f1, b0, frames, frame_stride, models, points, counts, nullptr, nullptr, n_desc,
+                           width_org, height_org, memkind, true);
 }
 
 int ofdis_traj_stats_get(const ofdis_ctx* ctx, ofdis_traj_stats* out) {
@@ -1850,6 +1886,178 @@ int ofdis_stab_finish(ofdis_ctx* ctx, unsigned char* out, ofdis_stab_frame* info
   if (rc) return rc;
   ctx->stab_next += count;
   *n_out = count;
+  return OFDIS_OK;
+}
+
+// The encoder's workspace for geometry g: the codebook (body floats), the statistics, the counts, per chunk the
+// staging, y, the posteriors and the skip flags, then the host-output vector.  Grows, never shrinks.
+static int ensure_fisher(ofdis_ctx* ctx, const FisherGeom& g, size_t body, size_t nstats) {
+  const size_t C = FISHER_CHUNK;
+  const size_t b_cb = align16(sizeof(float) * body), b_st = align16(sizeof(double) * nstats);
+  const size_t b_cnt = align16(sizeof(unsigned long long) * 2 * FISHER_MAX_BLOCKS);
+  const size_t b_x = align16(sizeof(float) * C * g.desc_dim), b_y = align16(sizeof(float) * C * g.ydim);
+  const size_t b_g = align16(sizeof(float) * C * g.nblocks * g.K), b_sk = align16(C * g.nblocks);
+  const size_t b_fv = align16(sizeof(float) * 2 * g.K * g.ydim);
+  const size_t bytes = b_cb + b_st + b_cnt + b_x + b_y + b_g + b_sk + b_fv;
+  if (bytes > ctx->fisher_bytes) {
+    CK(cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_fisher);
+    ctx->d_fisher = nullptr;
+    ctx->fisher_bytes = 0;
+    if (cudaMalloc(&ctx->d_fisher, bytes) != cudaSuccess) {
+      ctx->d_fisher = nullptr;
+      return fail(ctx, OFDIS_ERR_NOMEM, "fisher workspace");
+    }
+    ctx->fisher_bytes = bytes;
+  }
+  char* p = static_cast<char*>(ctx->d_fisher);
+  FisherWork& w = ctx->fisher;
+  w.cb = reinterpret_cast<float*>(p);
+  w.stats = reinterpret_cast<double*>(p += b_cb);
+  w.count = reinterpret_cast<unsigned long long*>(p += b_st);
+  w.x = reinterpret_cast<float*>(p += b_cnt);
+  w.y = reinterpret_cast<float*>(p += b_x);
+  w.gamma = reinterpret_cast<float*>(p += b_y);
+  w.skip = reinterpret_cast<unsigned char*>(p += b_g);
+  w.fv = reinterpret_cast<float*>(p += b_sk);
+  return OFDIS_OK;
+}
+
+static size_t fisher_nstats(const FisherGeom& g) {
+  size_t n = 0;
+  for (int b = 0; b < g.nblocks; ++b) n += (size_t)g.K * (1 + 2 * g.dim[b]);
+  return n;
+}
+
+// zero statistics and counts for a new clip (enqueued)
+static int fisher_reset(ofdis_ctx* ctx) {
+  CK(cudaMemsetAsync(ctx->fisher.stats, 0, sizeof(double) * fisher_nstats(ctx->fgeom), ctx->stream));
+  CK(cudaMemsetAsync(ctx->fisher.count, 0, sizeof(unsigned long long) * 2 * FISHER_MAX_BLOCKS, ctx->stream));
+  ctx->fisher_pushed = 0;
+  return OFDIS_OK;
+}
+
+int ofdis_fisher_begin(ofdis_ctx* ctx, const ofdis_fisher_codebook* cb) {
+  static_assert(sizeof(ofdis_fisher_stats) == 136, "ofdis_fisher_stats: 136 bytes, as preprocess.FISHER_STATS_DTYPE");
+  static_assert(OFDIS_FISHER_MAX_BLOCKS == FISHER_MAX_BLOCKS, "one block limit");
+  if (!ctx) return OFDIS_ERR_ARG;
+  bool ok = cb && cb->params && cb->K >= 1 && cb->K <= FISHER_MAX_K && cb->nblocks >= 1 &&
+            cb->nblocks <= FISHER_MAX_BLOCKS && cb->desc_dim >= 1;
+  FisherGeom g{};
+  size_t body = 0, fv = 0, nst = 0;
+  for (int b = 0; ok && b < cb->nblocks; ++b) {
+    const ofdis_fisher_block& bl = cb->blocks[b];
+    ok = bl.dim >= 1 && bl.dim <= bl.dim_in && bl.dim_in <= FISHER_MAX_DIM && bl.offset >= 0 &&
+         (long long)bl.offset + bl.dim_in <= cb->desc_dim;
+    if (!ok) break;
+    const size_t K = cb->K, D = bl.dim_in, P = bl.dim;
+    g.off[b] = bl.offset;
+    g.din[b] = bl.dim_in;
+    g.dim[b] = bl.dim;
+    g.yoff[b] = g.ydim;
+    g.ydim += bl.dim;
+    g.poff[b] = (long long)body;
+    g.foff[b] = (long long)fv;
+    g.soff[b] = (long long)nst;
+    // mean, proj and mu finite; isig finite and > 0; c finite; w finite and > 0
+    const float* a = cb->params + body;
+    for (size_t i = 0; ok && i < D + P * D + K * P; ++i) ok = finite_f32(a[i]);
+    a += D + P * D + K * P;
+    for (size_t i = 0; ok && i < K * P; ++i) ok = finite_gt0(a[i]);
+    a += K * P;
+    for (size_t i = 0; ok && i < K; ++i) ok = finite_f32(a[i]);
+    a += K;
+    for (size_t i = 0; ok && i < K; ++i) ok = finite_gt0(a[i]);
+    body += D + P * D + 2 * K * P + 2 * K;
+    fv += 2 * K * P;
+    nst += K * (1 + 2 * P);
+  }
+  if (!ok) return fail(ctx, OFDIS_ERR_ARG, "fisher_begin: bad codebook");
+  g.K = cb->K;
+  g.nblocks = cb->nblocks;
+  g.desc_dim = cb->desc_dim;
+  NvtxRange nvtx("fisher", -1);
+  CK(cudaSetDevice(ctx->device));
+  ctx->fisher_on = false;
+  int rc = ensure_fisher(ctx, g, body, nst);
+  if (rc) return rc;
+  ctx->fgeom = g;
+  CK(cudaMemcpyAsync(ctx->fisher.cb, cb->params, sizeof(float) * body, cudaMemcpyHostToDevice, ctx->stream));
+  rc = fisher_reset(ctx);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->fisher_on = true;
+  return OFDIS_OK;
+}
+
+// n descriptors into the live encoder, in chunks (host input through the staging buffer), one synchronise at the end
+static int fisher_push_chunks(ofdis_ctx* ctx, const float* desc, long n, bool host) {
+  // a call that fails on the way leaves the encoder to a new ofdis_fisher_begin
+  ctx->fisher_on = false;
+  const FisherGeom& g = ctx->fgeom;
+  for (long c0 = 0; c0 < n; c0 += FISHER_CHUNK) {
+    const int m = (int)std::min<long>(FISHER_CHUNK, n - c0);
+    const float* x = desc + (size_t)c0 * g.desc_dim;
+    if (host) {
+      CK(cudaMemcpyAsync(ctx->fisher.x, x, sizeof(float) * (size_t)m * g.desc_dim, cudaMemcpyHostToDevice,
+                         ctx->stream));
+      x = ctx->fisher.x;
+    }
+    const int k = launch_fisher_chunk(g, ctx->fisher, x, m, ctx->stream);
+    if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fisher kernel launch", cudaGetLastError());
+    ctx->launches += k;
+  }
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->fisher_pushed += n;
+  ctx->fisher_on = true;
+  return OFDIS_OK;
+}
+
+int ofdis_fisher_push(ofdis_ctx* ctx, const float* desc, long n, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (n < 0 || (!desc && n > 0) || (memkind == OFDIS_MEM_DEVICE && reinterpret_cast<uintptr_t>(desc) % 4 != 0))
+    return fail(ctx, OFDIS_ERR_ARG, "fisher_push: bad argument");
+  if (!ctx->fisher_on) return fail(ctx, OFDIS_ERR_ARG, "fisher_push: no live encoder (ofdis_fisher_begin)");
+  if (n == 0) return OFDIS_OK;
+  NvtxRange nvtx("fisher", -1);
+  CK(cudaSetDevice(ctx->device));
+  return fisher_push_chunks(ctx, desc, n, memkind != OFDIS_MEM_DEVICE);
+}
+
+int ofdis_fisher_take(ofdis_ctx* ctx, float* fv, double* stats, ofdis_fisher_stats* out, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  if (dev && (reinterpret_cast<uintptr_t>(fv) % 4 != 0 || reinterpret_cast<uintptr_t>(stats) % 8 != 0))
+    return fail(ctx, OFDIS_ERR_ARG, "fisher_take: bad argument");
+  if (!ctx->fisher_on) return fail(ctx, OFDIS_ERR_ARG, "fisher_take: no live encoder (ofdis_fisher_begin)");
+  NvtxRange nvtx("fisher", -1);
+  CK(cudaSetDevice(ctx->device));
+  ctx->fisher_on = false;
+  const FisherGeom& g = ctx->fgeom;
+  const cudaMemcpyKind kout = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  if (fv) {
+    float* dfv = dev ? fv : ctx->fisher.fv;
+    const int k = launch_fisher_take(g, ctx->fisher, dfv, ctx->stream);
+    if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fisher kernel launch", cudaGetLastError());
+    ctx->launches += k;
+    if (!dev) CK(cudaMemcpyAsync(fv, dfv, sizeof(float) * 2 * g.K * g.ydim, kout, ctx->stream));
+  }
+  if (stats) CK(cudaMemcpyAsync(stats, ctx->fisher.stats, sizeof(double) * fisher_nstats(g), kout, ctx->stream));
+  unsigned long long cnt[2 * FISHER_MAX_BLOCKS];
+  CK(cudaMemcpyAsync(cnt, ctx->fisher.count, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
+  const long long pushed = ctx->fisher_pushed;
+  const int rc = fisher_reset(ctx);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (out) {
+    std::memset(out, 0, sizeof(*out));
+    out->pushed = pushed;
+    for (int b = 0; b < g.nblocks; ++b) {
+      out->n[b] = (long long)cnt[b];
+      out->skipped[b] = (long long)cnt[FISHER_MAX_BLOCKS + b];
+    }
+  }
+  ctx->fisher_on = true;
   return OFDIS_OK;
 }
 

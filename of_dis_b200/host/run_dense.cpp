@@ -637,6 +637,17 @@ int main(int argc, char** argv) {
 // erratic R jump J camera K` follows the TRACKS line.  Frames smaller than N are refused before any device work; every
 // other output, the --tracks file included, keeps its bytes.  Not with --warm-start.
 //
+// --fisher CODEBOOK PATH (needs --tracks; flow binaries only): one improved Fisher vector per clip of --tracks from the
+// descriptors of --descriptors' stage (run whether or not --descriptors is given), encoded on the device with the
+// codebook file CODEBOOK (preprocess.write_fisher_codebook's format, whose desc_dim and block ranges must be the
+// descriptors': 426 floats, blocks 0+30, 30+96, 126+108, 234+96, 330+96).  Without --descriptors the descriptors go
+// from the descriptor stage to the encoder on the device (ofdis_traj_advance_fisher); with it they are pushed from the
+// host copy that --descriptors writes.  PATH gets the header `# clip n_desc n_0 .. n_{B-1} fv0 .. fv{F-1}`, then at
+// every clip's end one line: the clip, the descriptors pushed, each block's N_b and the vector's F floats with %.9g.
+// With verbosity > 0 a line `FISHER clips C descriptors N skipped s_0 .. s_{B-1}` follows the DESCRIPTORS line.  The
+// stereo binaries, --warm-start, a missing --tracks, an unreadable, malformed or mismatched codebook and an unwritable
+// PATH are refused before any device work; every other output keeps its bytes.
+//
 // --stabilize RADIUS CROP DIR (needs --global-motion, whose models it smooths; flow binaries only): every clip
 // stabilised on the device (ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish).  Clips are the runs of pairs of
 // --tracks, across batches: the stabiliser begins on a clip's first image1, every batch pushes the image2 frames of
@@ -900,11 +911,82 @@ static void save_mask_pgm(const uint8_t* mask, int w, int h, const char* filenam
   fclose(f);
 }
 
+// --fisher: a codebook file of preprocess.write_fisher_codebook ("OFDISFV1", int32 K, nblocks, desc_dim,
+// offset/dim_in/dim per block, the float32 body), checked as ofdis_fisher_begin checks it
+struct FisherBook {
+  ofdis_fisher_codebook cb;
+  vector<float> body;
+};
+static bool read_fisher_book(const char* path, FisherBook& fb, string& err) {
+  FILE* f = fopen(path, "rb");
+  if (!f) {
+    err = "cannot read the codebook";
+    return false;
+  }
+  vector<unsigned char> raw;
+  unsigned char buf[65536];
+  for (size_t got; (got = fread(buf, 1, sizeof(buf), f)) > 0;) raw.insert(raw.end(), buf, buf + got);
+  fclose(f);
+  auto i32 = [&raw](size_t at) {
+    int32_t v;
+    memcpy(&v, raw.data() + at, 4);
+    return (int)v;
+  };
+  if (raw.size() < 20 || memcmp(raw.data(), "OFDISFV1", 8) != 0) {
+    err = "not a codebook file (OFDISFV1)";
+    return false;
+  }
+  memset(&fb.cb, 0, sizeof(fb.cb));
+  fb.cb.K = i32(8);
+  fb.cb.nblocks = i32(12);
+  fb.cb.desc_dim = i32(16);
+  if (fb.cb.K < 1 || fb.cb.K > 256 || fb.cb.nblocks < 1 || fb.cb.nblocks > OFDIS_FISHER_MAX_BLOCKS ||
+      fb.cb.desc_dim < 1 || raw.size() < 20 + 12 * (size_t)fb.cb.nblocks) {
+    err = "bad codebook header";
+    return false;
+  }
+  const size_t K = fb.cb.K;
+  size_t body = 0;
+  for (int b = 0; b < fb.cb.nblocks; ++b) {
+    ofdis_fisher_block& bl = fb.cb.blocks[b];
+    bl.offset = i32(20 + 12 * b);
+    bl.dim_in = i32(24 + 12 * b);
+    bl.dim = i32(28 + 12 * b);
+    if (bl.dim < 1 || bl.dim > bl.dim_in || bl.dim_in > 512 || bl.offset < 0 ||
+        (long long)bl.offset + bl.dim_in > fb.cb.desc_dim) {
+      err = "bad codebook block";
+      return false;
+    }
+    body += bl.dim_in + (size_t)bl.dim * bl.dim_in + 2 * K * bl.dim + 2 * K;
+  }
+  const size_t at = 20 + 12 * (size_t)fb.cb.nblocks;
+  if (raw.size() != at + 4 * body) {
+    err = "codebook body does not match its header";
+    return false;
+  }
+  fb.body.resize(body);
+  memcpy(fb.body.data(), raw.data() + at, 4 * body);
+  const float* a = fb.body.data();
+  for (int b = 0; b < fb.cb.nblocks; ++b) {
+    const size_t D = fb.cb.blocks[b].dim_in, P = fb.cb.blocks[b].dim;
+    const size_t n[4] = {D + P * D + K * P, K * P, K, K};  // finite; isig > 0; c finite; w > 0
+    for (int part = 0; part < 4; ++part)
+      for (size_t i = 0; i < n[part]; ++i, ++a)
+        if (!(std::fabs(*a) <= FLT_MAX) || (part % 2 == 1 && !(*a > 0.f))) {
+          err = "codebook entries must be finite, isig and w > 0";
+          return false;
+        }
+  }
+  fb.cb.params = fb.body.data();
+  return true;
+}
+
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr,
             "usage: %s listfile [--batch N | --warm-start] [--bidirectional] [--gt gtlist] [--kitti]\n"
-            "       [--color [--color-max M]] [--interpolate T] [--tracks PATH [--descriptors PATH]]\n"
+            "       [--color [--color-max M]] [--interpolate T]\n"
+            "       [--tracks PATH [--descriptors PATH] [--fisher CODEBOOK PATH]]\n"
             "       [--lr-check] [--speckle N R] [--fill] [--camera fx,fy,cx,cy,baseline,doffs]\n"
             "       [--global-motion similarity|affine|homography PATH [--stabilize RADIUS CROP DIR]]\n"
             "       [--scene-flow DISPLIST [--gt-scene-flow GTLIST]]\n"
@@ -930,6 +1012,9 @@ int main(int argc, char** argv) {
             "  15-frame segment of the tracks, camera-compensated with the --global-motion models when given, written to\n"
             "  PATH as lines `clip id start mean_x mean_y sd_x sd_y length` and 426 floats; frames of at least 32 x 32;\n"
             "  not with --warm-start\n"
+            "  --fisher CODEBOOK PATH: flow only, with --tracks; one Fisher vector per clip of the descriptors above,\n"
+            "  encoded on the device with the codebook file CODEBOOK (python -m of_dis_b200.fisher_fit), written to\n"
+            "  PATH as lines `clip n_desc n_0 .. n_4` and the vector; not with --warm-start\n"
             "  --lr-check, --speckle N R, --fill, --camera ...: stereo only; also write <stem>_filtered<ext>, the\n"
             "  disparity without the pixels that fail the left-right check and the speckles of at most N pixels (R px),\n"
             "  holes filled with the background disparity, and with --camera <stem>_depth.pfm and <stem>.ply;\n"
@@ -954,6 +1039,7 @@ int main(int argc, char** argv) {
   const char* gtlist = nullptr;
   const char* tracks_path = nullptr;  // --tracks PATH
   const char* desc_path = nullptr;    // --descriptors PATH
+  const char* fisher_arg[2] = {nullptr, nullptr};  // --fisher CODEBOOK PATH
   bool lr_check = false, disp_fill = false;  // --lr-check, --fill
   const char* speckle_arg[2] = {nullptr, nullptr};  // --speckle N R
   const char* camera_arg = nullptr;  // --camera fx,fy,cx,cy,baseline,doffs
@@ -1006,6 +1092,14 @@ int main(int argc, char** argv) {
       }
       desc_path = argv[first_num + 1];
       first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--fisher")) {
+      if (argc < first_num + 3 || fisher_arg[0]) {
+        fprintf(stderr, "error: --fisher takes a codebook file and an output path\n");
+        return 2;
+      }
+      fisher_arg[0] = argv[first_num + 1];
+      fisher_arg[1] = argv[first_num + 2];
+      first_num += 3;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--lr-check")) {
       lr_check = true;
       first_num += 1;
@@ -1141,7 +1235,21 @@ int main(int argc, char** argv) {
       return 2;
     }
   }
-  ofdis_traj_params trp;  // --descriptors: Wang and Schmid's settings
+  if (fisher_arg[0]) {
+    if (SELECTMODE != 1) {
+      fprintf(stderr, "error: --fisher encodes the descriptors of flows; the stereo binaries take no --fisher\n");
+      return 2;
+    }
+    if (warm) {
+      fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --fisher\n");
+      return 2;
+    }
+    if (!tracks_path) {
+      fprintf(stderr, "error: --fisher encodes the clips of --tracks; give --tracks too\n");
+      return 2;
+    }
+  }
+  ofdis_traj_params trp;  // --descriptors, --fisher: Wang and Schmid's settings
   memset(&trp, 0, sizeof(trp));
   trp.L = 15;
   trp.nt = 3;
@@ -1154,6 +1262,25 @@ int main(int argc, char** argv) {
   trp.max_var = 50.0f;
   trp.max_dis = 20.0f;
   const int tdim = 2 * trp.L + trp.ns * trp.ns * trp.nt * 33;
+  FisherBook fbook;  // --fisher: the codebook, whose blocks must be the descriptors' (shape, HOG, HOF, MBHx, MBHy)
+  if (fisher_arg[0]) {
+    string err;
+    if (!read_fisher_book(fisher_arg[0], fbook, err)) {
+      fprintf(stderr, "error: %s: %s\n", fisher_arg[0], err.c_str());
+      return 2;
+    }
+    const int c = trp.nt * trp.ns * trp.ns, din[5] = {2 * trp.L, 8 * c, 9 * c, 8 * c, 8 * c};
+    bool match = fbook.cb.desc_dim == tdim && fbook.cb.nblocks == 5;
+    for (int b = 0, off = 0; match && b < 5; off += din[b++])
+      match = fbook.cb.blocks[b].offset == off && fbook.cb.blocks[b].dim_in == din[b];
+    if (!match) {
+      fprintf(stderr, "error: %s: the codebook's blocks are not the descriptors' (desc_dim %d, blocks 0+%d, %d+%d, "
+                      "%d+%d, %d+%d, %d+%d)\n", fisher_arg[0], tdim, din[0], din[0], din[1], din[0] + din[1], din[2],
+              din[0] + din[1] + din[2], din[3], tdim - din[4], din[4]);
+      return 2;
+    }
+  }
+  const bool traj_stage = desc_path || fisher_arg[0];  // the descriptor stage runs in place of the tracker's calls
   ofdis_stab_params stp;  // --stabilize
   memset(&stp, 0, sizeof(stp));
   vector<double> stab_wts;
@@ -1331,8 +1458,8 @@ int main(int argc, char** argv) {
       }
     }
   }
-  // --descriptors: every pair's frames hold an N x N patch, checked before any device work
-  for (size_t k = 0; k < jobs.size() && desc_path; ++k) {
+  // --descriptors, --fisher: every pair's frames hold an N x N patch, checked before any device work
+  for (size_t k = 0; k < jobs.size() && traj_stage; ++k) {
     int iw = 0, ih = 0;
     if (!image_size(jobs[k].a.c_str(), iw, ih)) {
       fprintf(stderr, "error: cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)\n",
@@ -1340,8 +1467,8 @@ int main(int argc, char** argv) {
       return 1;
     }
     if (iw < trp.N || ih < trp.N) {
-      fprintf(stderr, "error: --descriptors needs frames of at least %d x %d, %s is %d x %d\n", trp.N, trp.N,
-              jobs[k].a.c_str(), iw, ih);
+      fprintf(stderr, "error: --%s needs frames of at least %d x %d, %s is %d x %d\n",
+              desc_path ? "descriptors" : "fisher", trp.N, trp.N, jobs[k].a.c_str(), iw, ih);
       return 2;
     }
   }
@@ -1354,12 +1481,25 @@ int main(int argc, char** argv) {
     }
     fprintf(desc_file, "# clip id start mean_x mean_y sd_x sd_y length d0 .. d%d\n", tdim - 1);
   }
+  FILE* fisher_file = nullptr;
+  int fv_floats = 0;
+  if (fisher_arg[0]) {
+    fisher_file = fopen(fisher_arg[1], "w");
+    if (!fisher_file) {
+      fprintf(stderr, "error: cannot write %s\n", fisher_arg[1]);
+      if (desc_file) fclose(desc_file);
+      return 1;
+    }
+    for (int b = 0; b < fbook.cb.nblocks; ++b) fv_floats += 2 * fbook.cb.K * fbook.cb.blocks[b].dim;
+    fprintf(fisher_file, "# clip n_desc n_0 .. n_%d fv0 .. fv%d\n", fbook.cb.nblocks - 1, fv_floats - 1);
+  }
   FILE* tracks_file = nullptr;
   if (tracks_path) {
     tracks_file = fopen(tracks_path, "w");
     if (!tracks_file) {
       fprintf(stderr, "error: cannot write %s\n", tracks_path);
       if (desc_file) fclose(desc_file);
+      if (fisher_file) fclose(fisher_file);
       return 1;
     }
     fprintf(tracks_file, "# clip frame id x y\n");
@@ -1372,6 +1512,7 @@ int main(int argc, char** argv) {
       fprintf(stderr, "error: cannot write %s\n", stab_txt.c_str());
       if (tracks_file) fclose(tracks_file);
       if (desc_file) fclose(desc_file);
+      if (fisher_file) fclose(fisher_file);
       return 1;
     }
   }
@@ -1382,6 +1523,7 @@ int main(int argc, char** argv) {
       fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
       if (tracks_file) fclose(tracks_file);
       if (desc_file) fclose(desc_file);
+      if (fisher_file) fclose(fisher_file);
       if (stab_file) fclose(stab_file);
       return 1;
     }
@@ -1426,7 +1568,26 @@ int main(int argc, char** argv) {
   vector<int> tndesc;
   ofdis_traj_stats dtotal;
   memset(&dtotal, 0, sizeof(dtotal));
-  auto end_clip = [&]() {  // adds the tracked clip's counters to the totals
+  // --fisher: whether the clip's encoder is live, the vector of a take, the totals, the status of the last take
+  bool fisher_live = false;
+  vector<float> fvec(fv_floats);
+  long long fpushed = 0, fskipped[OFDIS_FISHER_MAX_BLOCKS] = {0};
+  int fclips = 0, fisher_rc = OFDIS_OK;
+  auto end_clip = [&]() {  // adds the tracked clip's counters to the totals; --fisher: takes the clip's vector
+    if (fisher_live) {
+      fisher_live = false;
+      ofdis_fisher_stats fs;
+      fisher_rc = ofdis_fisher_take(ctx, fvec.data(), nullptr, &fs, OFDIS_MEM_HOST);
+      if (fisher_rc == OFDIS_OK) {
+        fprintf(fisher_file, "%d %lld", tclip, fs.pushed);
+        for (int b = 0; b < fbook.cb.nblocks; ++b) fprintf(fisher_file, " %lld", fs.n[b]);
+        for (int i = 0; i < fv_floats; ++i) fprintf(fisher_file, " %.9g", (double)fvec[i]);
+        fprintf(fisher_file, "\n");
+        ++fclips;
+        fpushed += fs.pushed;
+        for (int b = 0; b < fbook.cb.nblocks; ++b) fskipped[b] += fs.skipped[b];
+      }
+    }
     ofdis_track_stats st;
     if (tclip < 0 || ofdis_track_stats_get(ctx, &st) != OFDIS_OK) return;
     ttotal.seeded += st.seeded;
@@ -1435,7 +1596,7 @@ int main(int argc, char** argv) {
     ttotal.ended_boundary += st.ended_boundary;
     ttotal.dropped += st.dropped;
     ofdis_traj_stats ds;
-    if (!desc_file || ofdis_traj_stats_get(ctx, &ds) != OFDIS_OK) return;
+    if (!traj_stage || ofdis_traj_stats_get(ctx, &ds) != OFDIS_OK) return;
     dtotal.emitted += ds.emitted;
     dtotal.rejected_static += ds.rejected_static;
     dtotal.rejected_erratic += ds.rejected_erratic;
@@ -1553,7 +1714,7 @@ int main(int argc, char** argv) {
     verbosity = P.verbosity;
     if (w != ctx_w || h != ctx_h) {
       end_clip();  // a pair of another size never continues the previous one
-      if (stab_end() != OFDIS_OK) {
+      if (fisher_rc != OFDIS_OK || stab_end() != OFDIS_OK) {
         fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
         ofdis_destroy(ctx);
         return 1;
@@ -1675,13 +1836,24 @@ int main(int argc, char** argv) {
       tcounts.resize(n);
       if (j0 + k0 == 0 || jobs[j0 + k0].a != jobs[j0 + k0 - 1].b) {
         end_clip();
+        rc = fisher_rc;
         ++tclip;
         tframe = 0;
-        rc = desc_file ? ofdis_traj_begin(ctx, &tp, &trp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST)
-                       : ofdis_track_begin(ctx, &tp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
+        if (rc == OFDIS_OK)
+          rc = traj_stage ? ofdis_traj_begin(ctx, &tp, &trp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST)
+                          : ofdis_track_begin(ctx, &tp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
+        if (rc == OFDIS_OK && fisher_file) {
+          rc = ofdis_fisher_begin(ctx, &fbook.cb);
+          fisher_live = rc == OFDIS_OK;
+        }
         if (rc == OFDIS_OK) write_tracks(tpoints.data(), tcounts[0]);
       }
-      if (rc == OFDIS_OK && desc_file) {
+      if (rc == OFDIS_OK && traj_stage && !desc_file) {  // --fisher alone: the descriptors stay on the device
+        tndesc.resize(k1 - k0);
+        rc = ofdis_traj_advance_fisher(ctx, k0, k1, n + k0, im2, fs,
+                                       gm_model ? gm_models.data() + (size_t)9 * k0 : nullptr, tpoints.data(),
+                                       tcounts.data(), tndesc.data(), w, h, OFDIS_MEM_HOST);
+      } else if (rc == OFDIS_OK && desc_file) {
         const size_t bound = (size_t)tp.capacity * ((k1 - k0 + 2 * trp.L - 2) / trp.L);
         trec.resize(bound);
         tdesc.resize(bound * tdim);
@@ -1692,6 +1864,7 @@ int main(int argc, char** argv) {
         int total = 0;
         for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k) total += tndesc[k];
         if (rc == OFDIS_OK) write_desc(total);
+        if (rc == OFDIS_OK && fisher_file) rc = ofdis_fisher_push(ctx, tdesc.data(), total, OFDIS_MEM_HOST);
       } else if (rc == OFDIS_OK) {
         rc = ofdis_track_advance(ctx, k0, k1, n + k0, im2, fs, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
       }
@@ -1940,7 +2113,7 @@ int main(int argc, char** argv) {
     done += n;
   }
   end_clip();
-  if (stab_end() != OFDIS_OK) {
+  if (fisher_rc != OFDIS_OK || stab_end() != OFDIS_OK) {
     fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
     ofdis_destroy(ctx);
     return 1;
@@ -1958,6 +2131,10 @@ int main(int argc, char** argv) {
     fprintf(stderr, "error: cannot write %s\n", desc_path);
     return 1;
   }
+  if (fisher_file && fclose(fisher_file) != 0) {
+    fprintf(stderr, "error: cannot write %s\n", fisher_arg[1]);
+    return 1;
+  }
   if (gm_file && fclose(gm_file) != 0) {
     fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
     return 1;
@@ -1971,6 +2148,11 @@ int main(int argc, char** argv) {
   if (verbosity > 0 && desc_path)
     printf("DESCRIPTORS clips %d emitted %lld static %lld erratic %lld jump %lld camera %lld\n", tclip + 1,
            dtotal.emitted, dtotal.rejected_static, dtotal.rejected_erratic, dtotal.rejected_jump, dtotal.rejected_camera);
+  if (verbosity > 0 && fisher_arg[0]) {
+    printf("FISHER clips %d descriptors %lld skipped", fclips, fpushed);
+    for (int b = 0; b < fbook.cb.nblocks; ++b) printf(" %lld", fskipped[b]);
+    printf("\n");
+  }
   if (verbosity > 0 && gtlist) {
     static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
     print_eval("", done, eval_total[0]);

@@ -1906,3 +1906,345 @@ def traj_descriptors(frames: np.ndarray, fw: np.ndarray, bw: np.ndarray, models,
     first = s.begin(clip[0])
     lists, records, desc, n_desc = s.advance(clip[1:], fw, bw, models)
     return [first] + lists, records, desc, n_desc, s.track_stats(), dict(s.tstats)
+
+
+# ---- Fisher vectors of descriptors (ofdis_fisher_begin / ofdis_fisher_push / ofdis_fisher_take) ----------------------
+# The library's float32 exp (exp_f32, ofdis_internal.cuh): Cody-Waite reduction by ln 2 (ln2_hi has 15 significant bits,
+# so n * ln2_hi is exact for |n| <= 256), the degree-7 Taylor polynomial of e^r in Horner form, then the exact scale by
+# 2^n.  +0 below EXP_CUTOFF (where e^x would leave the normal range), exactly 1 at +-0; within 2 ulp of float64 exp on
+# [EXP_CUTOFF, 0] (1.21 ulp at most over every third float32 there).
+EXP_CUTOFF = np.float32(-87.0)
+_EXP_LOG2E = np.float32(1.44269504)
+_EXP_LN2_HI = np.float32(0.693145751953125)
+_EXP_LN2_LO = np.float32(1.42860677e-06)
+_EXP_C = np.array([1.0, 1.0, 0.5, 0.166666672, 0.0416666679, 0.00833333377, 0.00138888892, 0.000198412701],
+                  np.float32)  # 1/k!
+FISHER_MAX_K = 256
+FISHER_MAX_BLOCKS = 8
+FISHER_MAX_DIM = 512
+FISHER_MAGIC = b"OFDISFV1"
+# ofdis_fisher_stats, field for field (136 bytes)
+FISHER_STATS_DTYPE = np.dtype([("pushed", "<i8"), ("n", "<i8", (FISHER_MAX_BLOCKS,)),
+                               ("skipped", "<i8", (FISHER_MAX_BLOCKS,))])
+FISHER_PARTS = ("mean", "proj", "mu", "isig", "c", "w")  # the packed order of a block's float32 arrays
+
+
+def exp_f32(x) -> np.ndarray:
+    """exp_f32 of float32 x <= 0 (or -inf), elementwise, bit for bit."""
+    f32 = np.float32
+    x = np.asarray(x, f32)
+    with np.errstate(all="ignore"):
+        n = np.rint(x * _EXP_LOG2E)
+        r = (x - n * _EXP_LN2_HI) - n * _EXP_LN2_LO
+        p = np.full(x.shape, _EXP_C[7], f32)
+        for k in range(6, -1, -1):
+            p = p * r + _EXP_C[k]
+        ni = np.fmin(np.fmax(n, np.float32(-126)), np.float32(128)).astype(np.int32)
+        scale = ((ni + 127) << 23).astype(np.int32).view(f32)
+        return np.where(x < EXP_CUTOFF, f32(0), p * scale).astype(f32)
+
+
+def fisher_blocks(traj_params):
+    """The descriptor blocks of ofdis_traj_advance's descriptors, [(offset, dim_in)]: shape 2L, HOG nt ns^2 8, HOF
+    nt ns^2 9, MBHx and MBHy nt ns^2 8 each (30/96/108/96/96 with TRAJ_DEFAULTS)."""
+    L, c = int(traj_params["L"]), int(traj_params["nt"]) * int(traj_params["ns"]) ** 2
+    out, off = [], 0
+    for d in (2 * L, 8 * c, 9 * c, 8 * c, 8 * c):
+        out.append((off, d))
+        off += d
+    return out
+
+
+def fisher_sizes(K: int, blocks) -> dict:
+    """Floats of the packed body, of the vector (2K sum dim) and doubles of the statistics (sum K(1 + 2 dim))."""
+    body = sum(di + d * di + 2 * K * d + 2 * K for _, di, d in blocks)
+    return {"body": body, "fv": 2 * K * sum(d for _, _, d in blocks),
+            "stats": sum(K * (1 + 2 * d) for _, _, d in blocks)}
+
+
+def fisher_pack(cb) -> np.ndarray:
+    """The codebook's float32 body: per block mean[dim_in], proj[dim][dim_in], mu[K][dim], isig[K][dim], c[K], w[K]."""
+    return np.concatenate([np.asarray(cb[k][b], np.float32).ravel() for b in range(len(cb["blocks"]))
+                           for k in FISHER_PARTS]).astype(np.float32)
+
+
+def fisher_unpack(K: int, desc_dim: int, blocks, body) -> dict:
+    """A codebook dict from its header fields and packed body (fisher_pack's inverse)."""
+    body = np.asarray(body, np.float32).ravel()
+    blocks = [tuple(int(v) for v in b) for b in blocks]
+    if body.size != fisher_sizes(K, blocks)["body"]:
+        raise ValueError("fisher codebook: body of %d floats, %d expected" % (body.size, fisher_sizes(K, blocks)["body"]))
+    cb = {"K": int(K), "desc_dim": int(desc_dim), "blocks": blocks}
+    for k in FISHER_PARTS:
+        cb[k] = []
+    p = 0
+    for _, di, d in blocks:
+        for k, shape in zip(FISHER_PARTS, ((di,), (d, di), (K, d), (K, d), (K,), (K,))):
+            n = int(np.prod(shape))
+            cb[k].append(body[p:p + n].reshape(shape).copy())
+            p += n
+    return cb
+
+
+def fisher_check(cb) -> None:
+    """Raises ValueError where ofdis_fisher_begin answers OFDIS_ERR_ARG."""
+    K, D, blocks = cb["K"], cb["desc_dim"], cb["blocks"]
+    if not (1 <= K <= FISHER_MAX_K and 1 <= len(blocks) <= FISHER_MAX_BLOCKS and D >= 1):
+        raise ValueError("fisher codebook: K %d, %d blocks, desc_dim %d out of range" % (K, len(blocks), D))
+    for b, (o, di, d) in enumerate(blocks):
+        if not (1 <= d <= di <= FISHER_MAX_DIM and o >= 0 and o + di <= D):
+            raise ValueError("fisher codebook: block %d (%d, %d, %d) out of range" % (b, o, di, d))
+        arrs = [np.asarray(cb[k][b], np.float32) for k in FISHER_PARTS]
+        if not all(np.isfinite(a).all() for a in arrs) or not (arrs[3] > 0).all() or not (arrs[5] > 0).all():
+            raise ValueError("fisher codebook: block %d has non-finite entries or isig, w not > 0" % b)
+
+
+def write_fisher_codebook(path: str, cb) -> None:
+    """The codebook file: OFDISFV1, int32 K, nblocks, desc_dim, (offset, dim_in, dim) per block, the float32 body,
+    all little-endian."""
+    hdr = [cb["K"], len(cb["blocks"]), cb["desc_dim"]] + [v for b in cb["blocks"] for v in b]
+    with open(path, "wb") as f:
+        f.write(FISHER_MAGIC + np.asarray(hdr, "<i4").tobytes() + fisher_pack(cb).astype("<f4").tobytes())
+
+
+def read_fisher_codebook(path: str) -> dict:
+    """write_fisher_codebook's file back; ValueError on a malformed file."""
+    with open(path, "rb") as f:
+        raw = f.read()
+    if raw[:8] != FISHER_MAGIC or len(raw) < 20:
+        raise ValueError("%s: not a fisher codebook" % path)
+    K, nb, D = (int(v) for v in np.frombuffer(raw, "<i4", 3, 8))
+    if not 1 <= nb <= FISHER_MAX_BLOCKS or len(raw) < 20 + 12 * nb:
+        raise ValueError("%s: bad block count %d" % (path, nb))
+    blocks = [tuple(int(v) for v in r) for r in np.frombuffer(raw, "<i4", 3 * nb, 20).reshape(nb, 3)]
+    if K < 1 or any(di < 1 or d < 1 for _, di, d in blocks):
+        raise ValueError("%s: bad header" % path)
+    body = np.frombuffer(raw, "<f4", offset=20 + 12 * nb) if (len(raw) - 20 - 12 * nb) % 4 == 0 else None
+    if body is None or body.size != fisher_sizes(K, blocks)["body"]:
+        raise ValueError("%s: body size does not match the header" % path)
+    cb = fisher_unpack(K, D, blocks, body.astype(np.float32))
+    fisher_check(cb)
+    return cb
+
+
+def fisher_project(x: np.ndarray, mean: np.ndarray, proj: np.ndarray) -> np.ndarray:
+    """y_d = sum_i proj[d][i] * (x_i - mean_i), float32, from +0.0f in increasing i; x (n, dim_in) -> (n, dim)."""
+    f32 = np.float32
+    with np.errstate(all="ignore"):
+        t = (np.asarray(x, f32) - np.asarray(mean, f32)[None]).astype(f32)
+        y = np.zeros((t.shape[0], proj.shape[0]), f32)
+        for i in range(t.shape[1]):
+            y = y + proj[:, i][None, :] * t[:, i:i + 1]
+    return y
+
+
+def fisher_posteriors(y: np.ndarray, mu: np.ndarray, isig: np.ndarray, c: np.ndarray):
+    """(gamma (n, K) float32, skipped (n,) bool) of projected descriptors y (n, dim): q_k = sum_d z_kd^2 in increasing
+    d, z_kd = (y_d - mu_kd) * isig_kd, ll_k = c_k - 0.5f q_k, m = max ll, e_k = exp_f32(ll_k - m), s = sum_k e_k in
+    increasing k, gamma_k = e_k / s; skipped where a y_d, a q_k or m is not finite."""
+    f32 = np.float32
+    n, K = y.shape[0], mu.shape[0]
+    with np.errstate(all="ignore"):
+        q = np.zeros((n, K), f32)
+        for d in range(y.shape[1]):
+            z = (y[:, d:d + 1] - mu[:, d][None, :]) * isig[:, d][None, :]
+            q = q + z * z
+        ll = (c[None, :] - f32(0.5) * q).astype(f32)
+        m = ll.max(axis=1) if K else np.zeros(n, f32)
+        skipped = ~np.isfinite(y).all(axis=1) | ~np.isfinite(q).all(axis=1) | ~np.isfinite(m)
+        e = exp_f32(np.where(skipped[:, None], f32(0), ll - m[:, None]))
+        s = np.cumsum(e, axis=1, dtype=f32)[:, -1]
+        g = (e / s[:, None]).astype(f32)
+    return g, skipped
+
+
+class FisherStream:
+    """ofdis_fisher_begin / push / take restated bit for bit: begin(codebook), push(desc) any number of times, then
+    take() -> (fv, stats, counters) as Context.fisher_take, which resets the clip."""
+
+    def __init__(self, cb):
+        self.begin(cb)
+
+    def begin(self, cb):
+        fisher_check(cb)
+        self.cb = cb
+        self._reset()
+
+    def _reset(self):
+        K = self.cb["K"]
+        self.S0 = [np.zeros(K) for _ in self.cb["blocks"]]
+        self.S1 = [np.zeros((K, d)) for _, _, d in self.cb["blocks"]]
+        self.S2 = [np.zeros((K, d)) for _, _, d in self.cb["blocks"]]
+        self.pushed = 0
+        self.n = np.zeros(len(self.cb["blocks"]), np.int64)
+        self.skipped = np.zeros(len(self.cb["blocks"]), np.int64)
+
+    def push(self, desc):
+        cb = self.cb
+        x = np.asarray(desc, np.float32).reshape(-1, cb["desc_dim"])
+        self.pushed += x.shape[0]
+        for b, (o, di, d) in enumerate(cb["blocks"]):
+            mu, isig = cb["mu"][b], cb["isig"][b]
+            y = fisher_project(x[:, o:o + di], cb["mean"][b], cb["proj"][b])
+            g, skip = fisher_posteriors(y, mu, isig, cb["c"][b])
+            keep = ~skip
+            self.n[b] += int(keep.sum())
+            self.skipped[b] += int(skip.sum())
+            y, g = y[keep], g[keep].astype(np.float64)
+            step = max(1, (1 << 21) // (cb["K"] * d))
+            for a in range(0, y.shape[0], step):
+                z = ((y[a:a + step, None, :] - mu[None]) * isig[None]).astype(np.float64)
+                ga = g[a:a + step]
+                # sequential sums over the descriptors: cumsum from the running value
+                self.S0[b] = np.cumsum(np.concatenate([self.S0[b][None], ga]), axis=0)[-1]
+                self.S1[b] = np.cumsum(np.concatenate([self.S1[b][None], ga[:, :, None] * z]), axis=0)[-1]
+                self.S2[b] = np.cumsum(np.concatenate([self.S2[b][None], ga[:, :, None] * (z * z)]), axis=0)[-1]
+
+    def take(self):
+        cb, K = self.cb, self.cb["K"]
+        fv, stats = [], []
+        for b, (_, _, d) in enumerate(cb["blocks"]):
+            fv.append(fisher_normalize(self.S0[b], self.S1[b], self.S2[b], cb["w"][b], int(self.n[b])))
+            stats += [self.S0[b], self.S1[b].ravel(), self.S2[b].ravel()]
+        counters = {"pushed": int(self.pushed), "n": self.n.copy(), "skipped": self.skipped.copy()}
+        out = np.concatenate(fv).astype(np.float32), np.concatenate(stats), counters
+        self._reset()
+        return out
+
+
+def fisher_normalize(S0, S1, S2, w, N: int) -> np.ndarray:
+    """One block's vector, float32 [u (K x dim), v (K x dim)]: u = S1 / (N sqrt(w)), v = (S2 - S0) / (N sqrt(2w)) in
+    float64, t < 0 ? -sqrt(|t|) : sqrt(|t|), then divided by sqrt of the sum of squares (256 partials over the indices = j mod 256
+    in increasing index, then the partials in increasing j) when that is > 0; zeros when N = 0."""
+    K, d = S1.shape
+    if N == 0:
+        return np.zeros(2 * K * d, np.float32)
+    wd = np.asarray(w, np.float32).astype(np.float64)
+    u = S1 / (float(N) * np.sqrt(wd))[:, None]
+    v = (S2 - S0[:, None]) / (float(N) * np.sqrt(2.0 * wd))[:, None]
+    f = np.concatenate([u.ravel(), v.ravel()])
+    r = np.sqrt(np.abs(f))
+    f = np.where(f < 0, -r, r)
+    sq = np.zeros(-(-f.size // 256) * 256)
+    sq[:f.size] = f * f
+    part = np.cumsum(sq.reshape(-1, 256), axis=0)[-1]
+    norm = np.sqrt(np.cumsum(part)[-1])
+    return (f / norm if norm > 0 else f).astype(np.float32)
+
+
+def fisher_encode(desc, cb):
+    """One clip's Fisher vector, bit for bit what one push of desc (n, desc_dim) and a take give: (fv, stats,
+    counters)."""
+    s = FisherStream(cb)
+    s.push(desc)
+    return s.take()
+
+
+def fisher_pca(samples, blocks, dims):
+    """Per block (offset, dim_in) with output size dims[b]: (mean float32, proj float32 (dim, dim_in), eigenvalues
+    float64 (dim,)) -- float64 mean and covariance, eigh, the top dim components by eigenvalue (descending), each
+    with the sign that makes its largest-magnitude entry positive (the first such entry on a tie)."""
+    x = np.asarray(samples, np.float32).astype(np.float64)
+    out = []
+    for (o, di), d in zip(blocks, dims):
+        xb = x[:, o:o + di]
+        mean = xb.mean(axis=0)
+        xc = xb - mean
+        cov = xc.T @ xc / max(xb.shape[0] - 1, 1)
+        ev, V = np.linalg.eigh(cov)
+        order = np.argsort(-ev, kind="stable")[:d]
+        P = V[:, order].T
+        big = np.argmax(np.abs(P), axis=1)
+        P = P * np.where(P[np.arange(d), big] < 0, -1.0, 1.0)[:, None]
+        out.append((mean.astype(np.float32), P.astype(np.float32), ev[order]))
+    return out
+
+
+def _fisher_cb_params(K, mu, var, w):
+    """isig, c, w of a block as float32 from float64 variances and weights: isig = 1/sqrt(var), c = log w - sum_d
+    log sqrt(var)."""
+    sig = np.sqrt(var)
+    return ((1.0 / sig).astype(np.float32), (np.log(w) - np.log(sig).sum(axis=1)).astype(np.float32),
+            np.asarray(w).astype(np.float32))
+
+
+FISHER_EIG_FLOOR = 1e-12  # eigenvalues below this (degenerate data) are raised to it before they become variances
+
+
+def fisher_init(samples, blocks, dims, K: int, seed: int):
+    """The fit's initial codebook: PCA as fisher_pca; as means, the projections of K distinct samples drawn with
+    splitmix64 from the seed (draw t = ((splitmix64(seed + (t+1) 0x9E3779B97F4A7C15) >> 32) * n) >> 32, repeats
+    skipped); the eigenvalues as every Gaussian's variances; w = 1/K.  Returns (codebook, eigenvalues per block)."""
+    x = np.asarray(samples, np.float32)
+    n = x.shape[0]
+    if n < K:
+        raise ValueError("fisher_init: %d samples for K = %d" % (n, K))
+    idx, seen, t = [], set(), 0
+    while len(idx) < K:
+        batch = np.arange(t + 1, t + 1 + 4 * K, dtype=np.uint64)
+        with np.errstate(over="ignore"):
+            z = splitmix64(np.uint64(seed % 2 ** 64) + batch * np.uint64(_SPLITMIX_GAMMA))
+        for j in ((z >> np.uint64(32)) * np.uint64(n)) >> np.uint64(32):
+            j = int(j)
+            if j not in seen and len(idx) < K:
+                seen.add(j)
+                idx.append(j)
+        t += 4 * K
+    pca = fisher_pca(x, blocks, dims)
+    cb = {"K": int(K), "desc_dim": int(x.shape[1]), "blocks": [(o, di, d) for (o, di), d in zip(blocks, dims)]}
+    for k in FISHER_PARTS:
+        cb[k] = []
+    eigs = []
+    for (o, di), (mean, P, ev) in zip(blocks, pca):
+        ev = np.maximum(ev, FISHER_EIG_FLOOR)
+        mu = fisher_project(x[idx, o:o + di], mean, P)
+        isig, c, w = _fisher_cb_params(K, mu, np.tile(ev, (K, 1)), np.full(K, 1.0 / K))
+        for k, v in zip(FISHER_PARTS, (mean, P, mu, isig, c, w)):
+            cb[k].append(v)
+        eigs.append(ev)
+    return cb, eigs
+
+
+def fisher_mstep(cb, stats, eigvals, var_floor: float):
+    """The M-step from take's statistics, float64, with y = mu + z / isig: mu += (S1/S0) / isig, var = (S2/S0 -
+    (S1/S0)^2) / isig^2 floored at var_floor * eigenvalue, w = S0 / sum S0; isig and c recomputed.  A Gaussian with
+    S0 = 0 keeps its parameters."""
+    K = cb["K"]
+    out = {k: cb[k] for k in ("K", "desc_dim", "blocks", "mean", "proj")}
+    for k in ("mu", "isig", "c", "w"):
+        out[k] = []
+    stats = np.asarray(stats, np.float64)
+    p = 0
+    for b, (_, _, d) in enumerate(cb["blocks"]):
+        S0 = stats[p:p + K]
+        S1 = stats[p + K:p + K + K * d].reshape(K, d)
+        S2 = stats[p + K + K * d:p + K + 2 * K * d].reshape(K, d)
+        p += K * (1 + 2 * d)
+        mu0 = cb["mu"][b].astype(np.float64)
+        is0 = cb["isig"][b].astype(np.float64)
+        live = S0 > 0
+        s0 = np.where(live, S0, 1.0)[:, None]
+        r1, r2 = S1 / s0, S2 / s0
+        mu = mu0 + r1 / is0
+        var = np.maximum((r2 - r1 * r1) / (is0 * is0), var_floor * np.asarray(eigvals[b])[None, :])
+        tot = S0.sum()
+        w = S0 / tot if tot > 0 else np.full(K, 1.0 / K)
+        isig, c, w32 = _fisher_cb_params(K, mu, var, np.where(live, w, 1.0))
+        out["mu"].append(np.where(live[:, None], mu.astype(np.float32), cb["mu"][b]))
+        out["isig"].append(np.where(live[:, None], isig, cb["isig"][b]))
+        out["c"].append(np.where(live, c, cb["c"][b]))
+        out["w"].append(np.where(live, w32, cb["w"][b]))
+    return out
+
+
+def fisher_fit(samples, blocks, dims, K: int = 256, iters: int = 10, seed: int = 0, var_floor: float = 1e-3,
+               estep=None):
+    """EM for a diagonal GMM per block on the PCA-projected samples: fisher_init, then `iters` rounds of an E-step
+    (estep(codebook, samples) -> take's statistics; fisher_encode's by default) and fisher_mstep.  Context.fisher_fit
+    runs the same loop with the E-step on the device, so both return the same codebook bytes."""
+    x = np.asarray(samples, np.float32)
+    cb, eigs = fisher_init(x, blocks, dims, K, seed)
+    for _ in range(iters):
+        stats = estep(cb, x) if estep is not None else fisher_encode(x, cb)[1]
+        cb = fisher_mstep(cb, stats, eigs, var_floor)
+    return cb

@@ -6,8 +6,8 @@ kernel, stereo SOR), a 70-row level as three bands of the lane kernel and forced
 wave kernel with 1 and 2 rows per thread (st.async halo exchange), and the 8-bit frame path (pyramid and
 upsampling kernels), and a frame interpolation, a point tracking (advance, seed, block scan, scatter) and a filtered
 disparity (union-find speckles, fill, depth and xyz) and a global motion (correspondences, compaction, hypotheses,
-the bulk-copied score tiles with and without refills, refits, per-pixel outputs) checked against their
-restatements.  Results are checked against the
+the bulk-copied score tiles with and without refills, refits, per-pixel outputs) and a Fisher encoding (projection,
+posteriors, float64 statistics, the take) checked against their restatements.  Results are checked against the
 oracle so that a clean log means a correct run."""
 import os
 import sys
@@ -147,6 +147,35 @@ exp = preprocess.global_motion(full, None, clip[1:], mp)
 ok = (stats["n_corr"] > 8192).all() and all(np.array_equal(np.asarray(g).view(np.uint8), np.asarray(e).view(np.uint8))
                                             for g, e in zip((models, stats, mask, res, reg), exp))
 print("%-22s %s" % ("global_motion_tiles", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# Fisher encoder (projection GEMM, posteriors, float64 statistics, the take): two chunks of descriptors with IDT's
+# blocks, non-finite entries among them, K = 24 (a partial Gaussian tile) against preprocess.fisher_encode
+rng = np.random.default_rng(7)
+blocks = [(o, di, di // 2) for o, di in preprocess.fisher_blocks(preprocess.TRAJ_DEFAULTS)]
+K, D = 24, preprocess.traj_dim(preprocess.TRAJ_DEFAULTS)
+cb = {"K": K, "desc_dim": D, "blocks": blocks}
+for part in preprocess.FISHER_PARTS:
+    cb[part] = []
+for _, di, d in blocks:
+    cb["mean"].append(rng.uniform(0, 0.1, di).astype(np.float32))
+    cb["proj"].append(rng.normal(0, di ** -0.5, (d, di)).astype(np.float32))
+    cb["mu"].append(rng.normal(0, 0.2, (K, d)).astype(np.float32))
+    cb["isig"].append(rng.uniform(1.0, 3.0, (K, d)).astype(np.float32))
+    cb["c"].append(rng.normal(0, 1.0, K).astype(np.float32))
+    cb["w"].append(np.full(K, 1.0 / K, np.float32))
+x = np.abs(rng.normal(0, 0.3, (4096 + 77, D))).astype(np.float32)
+x[5, 3], x[9, 100] = np.nan, np.inf
+prm = params.from_cli_numbers("3 1 8 8 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=1, nop=2)
+ctx = api.Context(prm, 64, 64, prm.p_samp_s, 1)
+ctx.fisher_begin(cb)
+ctx.fisher_push(x)
+got = ctx.fisher_take()
+ctx.close()
+exp = preprocess.fisher_encode(x, cb)
+ok = all(np.array_equal(g.view(np.uint8), e.view(np.uint8)) for g, e in zip(got[:2], exp[:2])) and \
+    np.array_equal(got[2]["n"], exp[2]["n"]) and np.array_equal(got[2]["skipped"], exp[2]["skipped"])
+print("%-22s %s" % ("fisher_idt_k24", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
