@@ -542,6 +542,90 @@ int ofdis_global_motion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const of
                                 ofdis_motion_stats* stats, unsigned char* mask, float* residual,
                                 unsigned char* registered, int width_org, int height_org, int memkind);
 
+/* Stereo ego-motion from flows and disparities (extension, flow contexts only): a RANSAC fit of one rigid transform
+ * [R | t] per pair from the camera at t to the camera at t+1, its Gauss-Newton refits on the inliers, and from the pose
+ * per pixel an independent-motion mask, the residual flow and the object motion.  preprocess.egomotion restates it
+ * bit for bit.  float32 where marked, float64 in the solver, everything without contraction and with IEEE division
+ * and square root; no transcendental function.  W = width_org, H = height_org, s = step, qNaN = the quiet NaN
+ * 0x7fc00000, known(d) = 0 <= d <= 1e9, fb = fx * baseline rounded once to float32.  For every pair k < f1-f0, slot
+ * a = f0+k, D0 = disp0 + k*disp_stride, D1 = disp1 + k*disp_stride ([H][W] positive disparities, NaN unknown, as
+ * ofdis_scene_flow_fullres takes them):
+ *   1. Correspondences.  The cells of ofdis_global_motion_fullres at step s, cell (i, j) read at its pixel (px, py).
+ *      F = (u, v) is slot a's flow there (ofdis_get_flow_fullres's value), (xs, ys) = ((float)px + u, (float)py + v),
+ *      d0 = D0(px, py), d1 = D1 gathered at (xs, ys) by step 2 of ofdis_scene_flow_fullres with edge_diff (when the
+ *      target lies in [0, W-1] x [0, H-1]), s0 = d0 + doffs, s1 = d1 + doffs.  A cell is valid when d0 is known,
+ *      s0 > 0, the target lies in the frame, d1 is known, s1 > 0 and, with fb_check, the mask of
+ *      ofdis_consistency_fullres(alpha, beta) of slot a against slot b0+k is 0 there.  It gives P = (X, Y, Z), the
+ *      xyz of scene flow's step 5 (Z = fb / s0, X = (((float)px - cx) * Z) / fx, Y = (((float)py - cy) * Z) / fy) and
+ *      the observation (xs, ys, d1).  The valid cells in cell order are the m correspondences; m < 3: status 1.
+ *   2. Hypotheses h = 0 .. hypotheses-1.  Draws d = 0, 1, 2 by ofdis_global_motion_fullres's SplitMix64 rule give
+ *      correspondences a, b, c.  Q, the t+1 point of an observation, is scene flow's Z1 = fb / s1,
+ *      X1 = ((xs - cx) * Z1) / fx, Y1 = ((ys - cy) * Z1) / fy (float32).  In float64 of the float32 values, the triad
+ *      of three points A, B, C: u = B - A, L = sqrt((u0*u0 + u1*u1) + u2*u2), e1 = u / L (per component),
+ *      n' = e1 x (C - A) with x the cross product (a1*b2 - a2*b1, a2*b0 - a0*b2, a0*b1 - a1*b0),
+ *      Ln = sqrt(n'.n') as L, n = n' / Ln, e2 = n x e1.  The triads (e1, e2, n) of P and (f1, f2, q) of Q give
+ *      R_ij = ((f1_i*e1_j) + (f2_i*e2_j)) + (q_i*n_j) and t_i = cQ_i - (((R_i0*cP_0) + (R_i1*cP_1)) + (R_i2*cP_2)),
+ *      with the centroids c_i = ((a_i + b_i) + c_i) / 3.0.  A length that is not > 0 or a non-finite entry of R or t
+ *      makes the hypothesis unsolvable (repeated or collinear draws).
+ *   3. Scoring.  g = [R | t] rounded to float32 (row-major, 12), P' = (X', Y', Z') with X' = ((g0*X + g1*Y) + g2*Z)
+ *      + g3 (rows 4..7, 8..11 the same).  A correspondence is an inlier iff Z' > 0 and (ex*ex + ey*ey) + ed*ed <=
+ *      tz*tz with ex = (fx*X' + cx*Z') - xs*Z', ey = (fy*Y' + cy*Z') - ys*Z', ed = fb - s1*Z', tz = threshold*Z'
+ *      (float32): the left-image and disparity reprojection error <= threshold, without a division.  The best
+ *      solvable hypothesis has the most inliers, the lowest h on a tie (the largest (count << 32) | (0xFFFFFFFF - h)).
+ *      No solvable hypothesis: status 2.
+ *   4. Refits, rounds 1 .. refine: the inliers of the current model by the test above; fewer than 3: stop.  For each
+ *      inlier, in float64 with P' = R P + t (P'_i = (((R_i0*X) + (R_i1*Y)) + (R_i2*Z)) + t_i), iz = 1.0 / Z',
+ *      u = X' * iz, v = Y' * iz, three residuals and their gradients a = d(residual)/dP':
+ *        x: r = ((fx*u) + cx) - xs,        a = (fx*iz, 0, -((fx*iz)*u))
+ *        y: r = ((fy*v) + cy) - ys,        a = (0, fy*iz, -((fy*iz)*v))
+ *        d: r = ((fb*iz) - doffs) - d1,    a = (0, 0, -((fb*iz)*iz))
+ *      and the Jacobian row of (omega, tau) with w = 2 P' per component: ((a1*-w2) + (a2*w1), (a0*w2) + (a2*-w0),
+ *      (a0*-w1) + (a1*w0), a0, a1, a2).  N_ij = ((Jx_i*Jx_j) + (Jy_i*Jy_j)) + (Jd_i*Jd_j) for i <= j and
+ *      b_i = -(((Jx_i*rx) + (Jy_i*ry)) + (Jd_i*rd)), summed as ofdis_global_motion_fullres's refits sum (chunks of 32
+ *      from +0.0, then the pairwise tree), mirrored and solved by its elimination.  A failure stops and keeps the
+ *      model; else with (omega, tau) = x, q = (w0*w0 + w1*w1) + w2*w2 (w = omega), the Cayley rotation
+ *      C_ij = (((i == j ? 1.0 - q : 0.0) + (2.0*(w_i*w_j))) + (2.0*K_ij)) / (1.0 + q) with K = [omega]x =
+ *      [0, -w2, w1; w2, 0, -w0; -w1, w0, 0], then [R | t]_ij = ((C_i0*M_0j) + (C_i1*M_1j)) + (C_i2*M_2j) of the old
+ *      [R | t] = M for j = 0..3, and t_i = t_i + tau_i.
+ *   5. pose = [n][12] float64 row-major [R | t]: camera-t coordinates to camera-t+1 coordinates.  Status != 0: twelve
+ *      float64 qNaN 0x7ff8000000000000.
+ *   6. Per pixel (X, Y), with g = the pose rounded to float32 and step 1's values at the pixel: mask 2 where the pixel
+ *      is not valid by step 1 or Z' <= 0 (or NaN), 0 where it passes step 3's test, else 1 (moves independently).
+ *      residual = (u - (((fx*X')/Z' + cx) - (float)X), v - (((fy*Y')/Z' + cy) - (float)Y)) where d0 is known and
+ *      s0 > 0, else qNaN: F minus the flow the pose induces.  object_motion = (X1 - X', Y1 - Y', Z1 - Z') with Q as in
+ *      step 2, where mask != 2, else qNaN: the pixel's 3-D motion relative to the static scene.  Every NaN written is
+ *      qNaN; a pair of status != 0 writes mask 2 and qNaN.
+ * stats per pair: the ofdis_motion_stats of ofdis_global_motion_fullres (status, n_corr = m, best_hypothesis,
+ * ransac_inliers, refits that replaced the model, n_inliers of the final model).  pose and stats are host memory;
+ * mask [n][H][W] bytes, residual [n][H][W][2] and object_motion [n][H][W][3] float32 are optional (NULL skips them)
+ * and in memkind, as disp0 and disp1 are.  Host inputs go through the context's staging buffer, host outputs through
+ * its full-resolution scratch.  Device disparities may come from another context on the same device; the caller
+ * orders that work before this call.  OFDIS_ERR_ARG: a stereo context, slots outside the context (b0 only with
+ * fb_check), a NULL p or one out of range (step >= 1, fb_check 0|1, alpha and beta finite and >= 0, edge_diff >= 0
+ * (+inf allowed), hypotheses 1..65536, threshold finite and > 0, refine 0..16), a NULL or bad cam (as
+ * ofdis_scene_flow_fullres checks it), NULL disp0, disp1, pose or stats, disp_stride < W*H, a device pointer that is
+ * not aligned to its element, or more than 2^24 cells per pair; frame sizes as ofdis_get_flow_fullres checks them.
+ * The workspace -- per cell and pair 39.75 bytes (the 32-byte correspondence, its flag, the refit's 27 chunk sums per
+ * 32 cells), per hypothesis and pair 160 (its float64 [R | t] and the float32 record) and 140 per pair -- is allocated
+ * on the first call, grows, never shrinks and is freed by ofdis_destroy.  Enqueued on the context's stream as 5
+ * kernels, plus one when a per-pixel output is asked for, whatever the number of pairs; the call synchronises the
+ * stream once, at the end, for pose and stats.  Not part of ofdis_run's graph; the flows are not changed. */
+typedef struct ofdis_egomotion_params {
+  int step;                  /* correspondence grid step s >= 1 (the seed grid of ofdis_track_begin) */
+  int fb_check;              /* 0 | 1: only correspondences whose consistency mask against slot b0+k is 0 */
+  float alpha, beta;         /* the rule of ofdis_consistency_fullres; finite, >= 0 */
+  float edge_diff;           /* the d1 gather of ofdis_scene_flow_fullres; >= 0, +inf allowed */
+  int hypotheses;            /* 1 .. 65536 */
+  float threshold;           /* inlier stereo reprojection error in pixels; finite, > 0 */
+  int refine;                /* 0 .. 16 Gauss-Newton rounds on the inliers */
+  unsigned long long seed;
+} ofdis_egomotion_params;
+int ofdis_egomotion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_egomotion_params* p,
+                            const float* disp0, const float* disp1, size_t disp_stride,
+                            const ofdis_stereo_camera* cam, double* pose, ofdis_motion_stats* stats,
+                            unsigned char* mask, float* residual, float* object_motion,
+                            int width_org, int height_org, int memkind);
+
 /* Dense point trajectories (extension): the tracker of Sundaram, Brox and Keutzer ("Dense point trajectories by
  * GPU-accelerated large displacement optical flow", ECCV 2010) through consecutive pairs of bidirectional flows.
  * The context owns one tracker: the list of live tracks (sorted by id), the next id and the counters.  It persists

@@ -14,7 +14,7 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import (DISP_FILTER_FIELDS, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
+from .preprocess import (DISP_FILTER_FIELDS, EGO_PARAM_FIELDS, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
                          STAB_FRAME_DTYPE, STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS,
                          TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
                          fisher_fit, fisher_pack, fisher_sizes, gaussian_weights, motion_params,
@@ -44,6 +44,7 @@ EXPORTS = [
     "ofdis_global_motion_fullres", "ofdis_stab_begin", "ofdis_stab_push", "ofdis_stab_finish",
     "ofdis_traj_begin", "ofdis_traj_advance", "ofdis_traj_stats_get", "ofdis_scene_flow_fullres",
     "ofdis_fisher_begin", "ofdis_fisher_push", "ofdis_fisher_take", "ofdis_traj_advance_fisher",
+    "ofdis_egomotion_fullres",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -51,6 +52,9 @@ DISP_OUTPUTS = ("disp", "status", "depth", "xyz")
 
 # outputs of scene_flow_fullres, in the C-ABI's argument order
 SF_OUTPUTS = ("disp1", "status", "motion")
+
+# per-pixel outputs of egomotion_fullres, in the C-ABI's argument order
+EGO_OUTPUTS = ("mask", "residual", "object_motion")
 
 # encodings of get_flow_fullres_encoded (OFDIS_ENC_F16, OFDIS_ENC_KITTI)
 ENCODINGS = {"f16": 1, "kitti": 2}
@@ -111,6 +115,16 @@ class MotionStats(ctypes.Structure):
 
 assert tuple(k for k, _ in MotionParams._fields_) == MOTION_PARAM_FIELDS
 assert ctypes.sizeof(MotionStats) == MOTION_STATS_DTYPE.itemsize
+
+
+class EgoParams(ctypes.Structure):
+    """ofdis_egomotion_params (include/ofdis_b200.h)."""
+    _fields_ = [("step", ctypes.c_int), ("fb_check", ctypes.c_int), ("alpha", ctypes.c_float),
+                ("beta", ctypes.c_float), ("edge_diff", ctypes.c_float), ("hypotheses", ctypes.c_int),
+                ("threshold", ctypes.c_float), ("refine", ctypes.c_int), ("seed", ctypes.c_ulonglong)]
+
+
+assert tuple(k for k, _ in EgoParams._fields_) == EGO_PARAM_FIELDS
 
 
 class StabParams(ctypes.Structure):
@@ -224,6 +238,9 @@ def lib():
             [ctypes.POINTER(SfGt), ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p] + [ctypes.c_int] * 3
         L.ofdis_global_motion_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
             [ctypes.POINTER(MotionParams), ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 5 + [ctypes.c_int] * 3
+        L.ofdis_egomotion_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
+            [ctypes.POINTER(EgoParams)] + [ctypes.c_void_p] * 2 + [ctypes.c_size_t, ctypes.POINTER(StereoCamera)] + \
+            [ctypes.c_void_p] * 5 + [ctypes.c_int] * 3
         L.ofdis_track_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackStats)]
         L.ofdis_traj_begin.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackParams), ctypes.POINTER(TrajParams)] + \
             [ctypes.c_void_p] * 3 + [ctypes.c_int] * 3
@@ -579,6 +596,61 @@ class Context:
                                                    _ptr(i1), frame_stride, _ptr(models), _ptr(stats), _ptr(mask),
                                                    _ptr(residual), _ptr(registered), width_org, height_org, memkind))
         return models, stats
+
+    def egomotion_fullres(self, f0, f1, disp0, disp1, params, *, camera, width_org, height_org, b0=None,
+                          disp_stride=None, outputs=(), out=None, memkind=MEM_HOST):
+        """The stereo ego-motion of the last run's flow slots [f0, f1) (ofdis_egomotion_fullres;
+        preprocess.egomotion restates it): pair k's flow with the disparities disp0[k] at t and disp1[k] at t+1
+        (positive, NaN unknown) and the stereo camera (a mapping with STEREO_CAMERA_FIELDS) give one rigid pose per
+        pair, camera t to camera t+1.  params: a mapping with preprocess.EGO_PARAM_FIELDS or an EgoParams; b0: the
+        partner slots of fb_check.  outputs: any of EGO_OUTPUTS ("mask" uint8 (n, H, W), "residual" float32
+        (n, H, W, 2), "object_motion" float32 (n, H, W, 3)).  Returns (pose (n, 3, 4) float64, stats (n,) of
+        MOTION_STATS_DTYPE, outs), pose and stats always on the host; the call synchronises the stream.  Host: disp0
+        and disp1 float32 (n, H, W) arrays whose frames are C-contiguous and equally spaced (a clip's maps[:-1] and
+        maps[1:] qualify); the outputs new or given in `out` as numpy arrays of exactly their dtype and shape.  With
+        memkind=MEM_DEVICE every array is a device address the caller owns and disp_stride the floats between
+        consecutive maps (default one frame)."""
+        unknown = set(outputs) - set(EGO_OUTPUTS)
+        if unknown:
+            raise ValueError("egomotion_fullres: unknown outputs %s" % sorted(unknown))
+        if not isinstance(params, EgoParams):
+            params = EgoParams(*[params[k] for k in EGO_PARAM_FIELDS])
+        n = max(f1 - f0, 0)
+        shape = (n, height_org, width_org)
+        out = dict(out or {})
+        if memkind == MEM_HOST:
+            strides = []
+            for name, arr in (("disp0", disp0), ("disp1", disp1)):
+                if not (isinstance(arr, np.ndarray) and arr.dtype == np.float32 and arr.shape == shape
+                        and (n == 0 or arr[0].flags["C_CONTIGUOUS"])):
+                    raise ValueError("egomotion_fullres: %s must be a float32 array of shape %s whose frames are "
+                                     "C-contiguous" % (name, shape))
+                strides.append(arr.strides[0] // 4 if n > 1 else height_org * width_org)
+            if strides[0] != strides[1] or (n > 1 and disp0.strides[0] % 4):
+                raise ValueError("egomotion_fullres: disp0 and disp1 must space their frames equally")
+            disp_stride = strides[0]
+            for name in outputs:
+                shp = shape + {"mask": (), "residual": (2,), "object_motion": (3,)}[name]
+                dt = np.uint8 if name == "mask" else np.float32
+                arr = out.setdefault(name, np.empty(shp, dt))
+                if not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape == shp
+                        and arr.flags["C_CONTIGUOUS"] and arr.flags["WRITEABLE"]):
+                    raise ValueError("egomotion_fullres: %s must be a writeable C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shp))
+        else:
+            missing = [name for name in outputs if out.get(name) is None]
+            if missing:
+                raise ValueError("egomotion_fullres: no device address for the requested outputs %s" % missing)
+            if disp_stride is None:
+                disp_stride = height_org * width_org
+        cam = None if camera is None else ctypes.byref(StereoCamera(*[camera[k] for k in STEREO_CAMERA_FIELDS]))
+        pose = np.empty((n, 3, 4), np.float64)
+        stats = np.zeros(n, MOTION_STATS_DTYPE)
+        ptrs = [_ptr(out.get(k)) if k in outputs else None for k in EGO_OUTPUTS]
+        self._ck(lib().ofdis_egomotion_fullres(self._h, f0, f1, -1 if b0 is None else b0, ctypes.byref(params),
+                                               _ptr(disp0), _ptr(disp1), disp_stride, cam, _ptr(pose), _ptr(stats),
+                                               *ptrs, width_org, height_org, memkind))
+        return pose, stats, {k: out.get(k) for k in outputs}
 
     def flow_error_fullres(self, f0, f1, gt, width_org, height_org, classes=None, nclasses=None, with_err=False,
                            memkind=MEM_HOST, err=None):

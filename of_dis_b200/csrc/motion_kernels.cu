@@ -13,11 +13,14 @@
 // without contraction (-fmad=false), IEEE division.
 #include <cuda_runtime.h>
 
+#include "bulk_tile.cuh"
 #include "ofdis_internal.cuh"
 
 namespace ofdis {
 
 namespace {
+
+using namespace tiles;
 
 constexpr int kCorrThreads = 256;
 constexpr int kCompactThreads = 1024;
@@ -27,12 +30,6 @@ constexpr int kTile = 4096;                                                     
 constexpr size_t kScoreSmem = 2 * kTile * sizeof(float4) + 16;                       // two tiles, two mbarriers
 constexpr int kRefitThreads = 256;
 constexpr int kChunk = 32;
-
-__device__ __forceinline__ unsigned long long splitmix64(unsigned long long z) {
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
 
 // the two rows r1 | b1, r2 | b2 of correspondence c (float64 of its float32 values)
 template <int MODEL>
@@ -64,54 +61,6 @@ __device__ __forceinline__ void motion_hmat(const double* x, double* H) {
     H[7] = MODEL == OFDIS_MOTION_HOMOGRAPHY ? x[7] : 0.0;
   }
   H[8] = 1.0;
-}
-
-// The elimination of the header: partial pivoting (the first row of the largest |a_ij|), then back substitution.
-// Returns false on a pivot that is not > 0 in magnitude or a non-finite solution.
-template <int K>
-__device__ __forceinline__ bool motion_solve(double (&A)[K][K], double (&b)[K], double (&x)[K]) {
-#pragma unroll
-  for (int j = 0; j < K; ++j) {
-    int p = j;
-    double best = fabs(A[j][j]);
-#pragma unroll
-    for (int i = j + 1; i < K; ++i) {
-      const double a = fabs(A[i][j]);
-      if (a > best) best = a, p = i;
-    }
-    if (!(best > 0.0)) return false;
-#pragma unroll
-    for (int i = j + 1; i < K; ++i) {
-      if (i == p) {
-#pragma unroll
-        for (int c = j; c < K; ++c) {
-          const double t = A[j][c];
-          A[j][c] = A[i][c];
-          A[i][c] = t;
-        }
-        const double t = b[j];
-        b[j] = b[i];
-        b[i] = t;
-      }
-    }
-#pragma unroll
-    for (int i = j + 1; i < K; ++i) {
-      const double f = A[i][j] / A[j][j];
-#pragma unroll
-      for (int c = j + 1; c < K; ++c) A[i][c] = A[i][c] - f * A[j][c];
-      b[i] = b[i] - f * b[j];
-    }
-  }
-  bool ok = true;
-#pragma unroll
-  for (int i = K - 1; i >= 0; --i) {
-    double s = b[i];
-#pragma unroll
-    for (int c = i + 1; c < K; ++c) s = s - A[i][c] * x[c];
-    x[i] = s / A[i][i];
-    ok = ok && isfinite(x[i]);
-  }
-  return ok;
 }
 
 // ---- 1. correspondences ------------------------------------------------------------------------------------------
@@ -211,25 +160,6 @@ __global__ void __launch_bounds__(kHypThreads) motion_hyp_kernel(MotionGeom mg, 
 }
 
 // ---- 4. scoring (the hot path) ----------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned a, unsigned count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned a, unsigned parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tWAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}" ::"r"(a), "r"(parity)
-      : "memory");
-}
-// one bulk copy of `bytes` (a multiple of 16) into shared memory, completing on mbarrier `mbar`
-__device__ __forceinline__ void bulk_tile(unsigned dst, const void* src, unsigned bytes, unsigned mbar) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(bytes) : "memory");
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(mbar)
-               : "memory");
-}
-
 // the inlier test of the header; without a perspective row W' is exactly 1, so the test reduces to its float32 value
 template <bool PERSP>
 __device__ __forceinline__ int motion_inlier(const float* g, float4 c, float t) {

@@ -105,6 +105,11 @@ struct ofdis_ctx {
   void* d_motion = nullptr;
   size_t motion_cells = 0, motion_hyps = 0;
   MotionWork motion{};
+  // lazily allocated workspace of ofdis_egomotion_fullres (EgoWork for max_frames pairs of ego_cells cells and
+  // ego_hyps hypotheses); grows, never shrinks; never touched by ofdis_run
+  void* d_ego = nullptr;
+  size_t ego_cells = 0, ego_hyps = 0;
+  EgoWork ego{};
   // the stabiliser of ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish: its workspace (StabWork: the frame ring,
   // the model ring, the per-frame records), the geometry and weights of the last begin, L and the next frame to emit;
   // grows, never shrinks; never touched by ofdis_run
@@ -493,6 +498,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_disp);
   cudaFree(ctx->d_sf);
   cudaFree(ctx->d_motion);
+  cudaFree(ctx->d_ego);
   cudaFree(ctx->d_traj);
   cudaFree(ctx->d_stab);
   cudaFree(ctx->d_fisher);
@@ -1307,6 +1313,127 @@ int ofdis_global_motion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const of
   CK(cudaStreamSynchronize(ctx->stream));
   for (int q = 0; q < n; ++q) {
     std::memcpy(model + 9 * (size_t)q, res[q].M, sizeof(res[q].M));
+    stats[q] = res[q].st;
+  }
+  return OFDIS_OK;
+}
+
+// The workspace of ofdis_egomotion_fullres for max_frames pairs of at least `cells` cells and `hyps` hypotheses: per
+// cell the correspondence (32 bytes), its flag (1) and the refit's chunk sums (27 doubles per 32 cells); per hypothesis
+// its float64 [R | t] (96) and EgoHyp (64); per pair EgoOut, the key and the count.  Grows, never shrinks.
+static int ensure_ego(ofdis_ctx* ctx, size_t cells, size_t hyps) {
+  cells = (cells + 31) / 32 * 32;
+  const size_t n = (size_t)ctx->max_frames;
+  if (ctx->d_ego && cells <= ctx->ego_cells && hyps <= ctx->ego_hyps) return OFDIS_OK;
+  cells = std::max(cells, ctx->ego_cells);
+  hyps = std::max(hyps, ctx->ego_hyps);
+  const size_t b_corr = n * cells * sizeof(EgoCorr), b_chunk = n * (cells / 32) * EGO_NE * sizeof(double);
+  const size_t b_hp = n * hyps * 12 * sizeof(double), b_hg = n * hyps * sizeof(EgoHyp);
+  const size_t b_out = align16(n * sizeof(EgoOut)), b_key = align16(n * 8), b_m = align16(n * 4);
+  CK(cudaStreamSynchronize(ctx->stream));
+  cudaFree(ctx->d_ego);
+  ctx->d_ego = nullptr;
+  ctx->ego_cells = ctx->ego_hyps = 0;
+  if (cudaMalloc(&ctx->d_ego, b_corr + b_chunk + b_hp + b_hg + b_out + b_key + b_m + n * cells) != cudaSuccess) {
+    ctx->d_ego = nullptr;
+    return fail(ctx, OFDIS_ERR_NOMEM, "egomotion_fullres workspace");
+  }
+  char* b = static_cast<char*>(ctx->d_ego);
+  EgoWork& ws = ctx->ego;
+  ws.corr = reinterpret_cast<EgoCorr*>(b);
+  b += b_corr;
+  ws.chunk = reinterpret_cast<double*>(b);
+  b += b_chunk;
+  ws.hp = reinterpret_cast<double*>(b);
+  b += b_hp;
+  ws.hg = reinterpret_cast<EgoHyp*>(b);
+  b += b_hg;
+  ws.out = reinterpret_cast<EgoOut*>(b);
+  b += b_out;
+  ws.key = reinterpret_cast<unsigned long long*>(b);
+  b += b_key;
+  ws.m = reinterpret_cast<int*>(b);
+  b += b_m;
+  ws.flag = reinterpret_cast<unsigned char*>(b);
+  ctx->ego_cells = cells;
+  ctx->ego_hyps = hyps;
+  return OFDIS_OK;
+}
+
+int ofdis_egomotion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_egomotion_params* p,
+                            const float* disp0, const float* disp1, size_t disp_stride,
+                            const ofdis_stereo_camera* cam, double* pose, ofdis_motion_stats* stats,
+                            unsigned char* mask, float* residual, float* object_motion,
+                            int width_org, int height_org, int memkind) {
+  static_assert(sizeof(EgoCorr) == 32 && sizeof(EgoHyp) == 64 && sizeof(EgoOut) == 128, "egomotion records");
+  if (!ctx) return OFDIS_ERR_ARG;
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  auto misaligned = [dev](const float* q) { return dev && reinterpret_cast<uintptr_t>(q) % sizeof(float); };
+  const size_t pix = (size_t)std::max(width_org, 0) * std::max(height_org, 0);
+  if (ctx->nop != 2 || f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !p ||
+      (p->fb_check && (b0 < 0 || b0 > ctx->max_frames - (f1 - f0))) || p->step < 1 ||
+      (p->fb_check != 0 && p->fb_check != 1) || !finite_ge0(p->alpha) || !finite_ge0(p->beta) ||
+      !(p->edge_diff >= 0.f) || p->hypotheses < 1 || p->hypotheses > 65536 || !finite_gt0(p->threshold) ||
+      p->refine < 0 || p->refine > 16 || !cam || !finite_gt0(cam->fx) || !finite_gt0(cam->fy) ||
+      !finite_gt0(cam->baseline) || !finite_f32(cam->cx) || !finite_f32(cam->cy) || !finite_f32(cam->doffs) ||
+      !disp0 || !disp1 || !pose || !stats || disp_stride < pix || misaligned(disp0) || misaligned(disp1) ||
+      misaligned(residual) || misaligned(object_motion))
+    return fail(ctx, OFDIS_ERR_ARG, "egomotion_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  const int s = p->step, ncx = (width_org - 1) / s + 1, ncy = (height_org - 1) / s + 1;
+  if ((long long)ncx * ncy > (1ll << 24)) return fail(ctx, OFDIS_ERR_ARG, "egomotion_fullres: more than 2^24 cells");
+  NvtxRange nvtx("egomotion", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0, D = ctx->dirs;
+  const size_t np = pix * n;
+  rc = ensure_ego(ctx, (size_t)ncx * ncy, (size_t)p->hypotheses);
+  if (rc) return rc;
+  EgoGeom eg{};
+  eg.w = width_org, eg.h = height_org, eg.s = s, eg.ncx = ncx, eg.cells = ncx * ncy, eg.nh = p->hypotheses;
+  eg.fb_check = p->fb_check, eg.refine = p->refine, eg.crop_x = cx, eg.crop_y = cy;
+  eg.alpha = p->alpha, eg.beta = p->beta, eg.edge_diff = p->edge_diff, eg.thr = p->threshold;
+  eg.cam = DispCamera{cam->fx * cam->baseline, cam->fx, cam->fy, cam->cx, cam->cy, cam->doffs};
+  eg.seed = p->seed;
+  eg.cell_cap = ctx->ego_cells, eg.chunk_cap = ctx->ego_cells / 32, eg.hyp_cap = ctx->ego_hyps;
+  eg.disp0 = disp0, eg.disp1 = disp1, eg.stride = disp_stride;
+  EgoOutputs o{mask, residual, object_motion};
+  if (!dev) {
+    // the staging buffer: disp0 and disp1 packed to one map per pair; sized for max_frames
+    rc = ensure_stage(ctx, sizeof(float) * 2 * pix * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    float* st = static_cast<float*>(ctx->d_stage);
+    const size_t row = sizeof(float) * pix, pitch = sizeof(float) * disp_stride;
+    CK(cudaMemcpy2DAsync(st, row, disp0, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(st + np, row, disp1, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
+    eg.disp0 = st, eg.disp1 = st + np, eg.stride = pix;
+    if (mask || residual || object_motion) {
+      // the full-resolution scratch: residual and object_motion floats (those asked for), then the mask bytes; sized
+      // for max_frames, and at least what ofdis_get_flow_fullres asks for
+      rc = ensure_full(ctx, std::max(pix * ctx->nop, 5 * pix + (pix + 3) / 4) * (size_t)ctx->max_frames);
+      if (rc) return rc;
+      float* q = ctx->d_full;
+      if (residual) o.residual = q, q += 2 * np;
+      if (object_motion) o.object_motion = q, q += 3 * np;
+      if (mask) o.mask = reinterpret_cast<unsigned char*>(q);
+    }
+  }
+  const int k = launch_egomotion(stepped(ctx->lev[0], D), f0 * D, (p->fb_check ? b0 : f0) * D, n, eg, ctx->ego, o,
+                                 ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "egomotion kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  if (!dev) {
+    if (residual) CK(cudaMemcpyAsync(residual, o.residual, sizeof(float) * 2 * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (object_motion)
+      CK(cudaMemcpyAsync(object_motion, o.object_motion, sizeof(float) * 3 * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (mask) CK(cudaMemcpyAsync(mask, o.mask, np, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  std::vector<EgoOut> res(n);
+  CK(cudaMemcpyAsync(res.data(), ctx->ego.out, sizeof(EgoOut) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (int q = 0; q < n; ++q) {
+    std::memcpy(pose + 12 * (size_t)q, res[q].pose, sizeof(res[q].pose));
     stats[q] = res[q].st;
   }
   return OFDIS_OK;

@@ -18,8 +18,6 @@ constexpr int SF_ROWS = 32;  // rows of a CTA (32 x SF_ROWS threads)
 
 __device__ __forceinline__ float qnan() { return __int_as_float(0x7fc00000); }
 __device__ __forceinline__ float canon(float v) { return isnan(v) ? qnan() : v; }
-// a disparity is known in [0, 1e9]: NaN fails, -0 passes
-__device__ __forceinline__ bool known_d(float d) { return d >= 0.0f && d <= 1e9f; }
 // KITTI's outlier rule of ofdis_flow_error_fullres
 __device__ __forceinline__ bool outlier(float e, float g) { return e > 3.0f && e > 0.05f * g; }
 
@@ -43,23 +41,7 @@ __global__ void __launch_bounds__(32 * SF_ROWS) sceneflow_kernel(LevelGeom g, in
     const float xs = (float)X + f[0], ys = (float)Y + f[1];
     const bool in = in_frame_f(xs, ys, w_org, h_org);
     float d1 = qnan();
-    if (in) {
-      const int x0 = (int)floorf(xs), y0 = (int)floorf(ys);
-      const int x1 = min(x0 + 1, w_org - 1), y1 = min(y0 + 1, h_org - 1);
-      const float fx = xs - (float)x0, fy = ys - (float)y0;
-      const float c00 = D1[(size_t)y0 * w_org + x0], c10 = D1[(size_t)y0 * w_org + x1];
-      const float c01 = D1[(size_t)y1 * w_org + x0], c11 = D1[(size_t)y1 * w_org + x1];
-      const bool all = known_d(c00) && known_d(c10) && known_d(c01) && known_d(c11);
-      const float hi = fmaxf(fmaxf(c00, c10), fmaxf(c01, c11)), lo = fminf(fminf(c00, c10), fminf(c01, c11));
-      if (all && hi - lo <= a.edge_diff) {
-        const float gx = 1.0f - fx, gy = 1.0f - fy;
-        const float r0 = c00 * gx + c10 * fx, r1 = c01 * gx + c11 * fx;
-        d1 = r0 * gy + r1 * fy;
-      } else {
-        const bool rx = fx >= 0.5f, ry = fy >= 0.5f;
-        d1 = ry ? (rx ? c11 : c01) : (rx ? c10 : c00);
-      }
-    }
+    if (in) d1 = sf_d1_at(D1, xs, ys, w_org, h_org, a.edge_diff);
     const bool k0 = known_d(d0), k1 = in && known_d(d1);
     const unsigned char st = (unsigned char)((k0 ? 0 : 1) | (in ? 0 : 2) | (in && !k1 ? 4 : 0));
     const float d1w = k1 ? d1 : qnan();

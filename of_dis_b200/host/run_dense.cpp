@@ -673,6 +673,55 @@ int main(int argc, char** argv) {
 // whose count or files do not match the pairs is refused before any device work; every other output keeps its
 // bytes.  Not with --warm-start; --camera on a flow binary needs --scene-flow.
 
+// --odometry DIR (flow binaries only, with --scene-flow and --camera, which give both disparities of every pair and the
+// stereo camera): the rig's ego-motion of every pair (ofdis_egomotion_fullres) with step 8, 1024 hypotheses, a 1 px
+// threshold, 5 Gauss-Newton rounds, seed 0 and edge_diff 1; with --bidirectional only correspondences whose forward
+// consistency mask (the thresholds of _occ.pgm) is 0.  A clip is a run of pairs whose image1 is the previous pair's
+// image2; clips and their frames count from 0.  DIR/odometry.txt gets one line per pair, `clip frame status n_corr
+// ransac_inliers n_inliers` and the 12 numbers of the relative pose [R | t] (camera t to camera t+1, row-major, %.17g);
+// DIR/poses_<clip %04d>.txt the clip's camera-to-world poses in KITTI's odometry format, n+1 lines from the identity,
+// T_(k+1) = T_k inv([R | t]_k).  Every pair gets <stem>_objects.pgm (0 static, 255 moves on its own, 128 unknown: the
+// code of _occ.pgm) and <stem>_objmotion.pfm (3-channel PFM as _sceneflow.pfm, the object's own 3-D motion, NaN where
+// unknown).  --gt-poses LIST holds one KITTI poses file per clip, with at least n+1 lines for a clip of n pairs; with
+// verbosity > 0 every pair prints `ODOEVAL clip frame t_err r_err` (the relative pose error in metres and degrees, as
+// KITTI's devkit forms it) and the end `ODOEVAL (<P> pairs) t_err <mean> r_err <mean>`.  Refused before any device
+// work: the stereo binaries, --warm-start, --odometry without --scene-flow or --camera, --gt-poses without
+// --odometry, a list that does not match the clips or a file with too few lines, and a DIR that cannot be written.
+// Every other output keeps its bytes.
+
+// Rigid poses as 12 doubles, row-major [R | t].  T <- T inv(P): the next camera-to-world pose of a clip (KITTI's
+// odometry convention) from the relative pose P, camera t to camera t+1.
+static void chain_pose(double* T, const double* P) {
+  double I[12];  // inv(P) = [R^T | -R^T t]
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) I[4 * i + j] = P[4 * j + i];
+    I[4 * i + 3] = -(P[i] * P[3] + P[4 + i] * P[7] + P[8 + i] * P[11]);
+  }
+  double N[12];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 4; ++j)
+      N[4 * i + j] = T[4 * i] * I[j] + T[4 * i + 1] * I[4 + j] + T[4 * i + 2] * I[8 + j] + (j == 3 ? T[4 * i + 3] : 0.0);
+  memcpy(T, N, sizeof(N));
+}
+
+// The relative pose error of the estimate P (camera t to t+1) against the ground-truth camera-to-world poses G0, G1,
+// as KITTI's devkit forms it: E = inv(inv(G0) G1) inv(P), t_err = |E_t| (metres), r_err = acos((trace(E_R) - 1) / 2)
+// in degrees.
+static void pose_error(const double* G0, const double* G1, const double* P, double* t_err, double* r_err) {
+  // inv(inv(G0) G1) = inv(G1) G0; then E = inv(G1) G0 inv(P): chain G0 by P gives G0 inv(P)
+  double A[12], Gi[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+  memcpy(A, G0, sizeof(A));
+  chain_pose(A, P);   // A = G0 inv(P)
+  chain_pose(Gi, G1);  // Gi = inv(G1)
+  double E[12];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 4; ++j)
+      E[4 * i + j] = Gi[4 * i] * A[j] + Gi[4 * i + 1] * A[4 + j] + Gi[4 * i + 2] * A[8 + j] + (j == 3 ? Gi[4 * i + 3] : 0.0);
+  *t_err = sqrt(E[3] * E[3] + E[7] * E[7] + E[11] * E[11]);
+  const double c = 0.5 * (E[0] + E[5] + E[10] - 1.0);
+  *r_err = acos(fmin(1.0, fmax(-1.0, c))) * (180.0 / M_PI);
+}
+
 // <stem><ext> -> <stem><suffix><ext> (ext: from the last '.' of the file name, empty if it has none)
 static string with_suffix(const string& path, const char* suffix, const char* new_ext = nullptr) {
   const size_t slash = path.find_last_of('/'), dot = path.find_last_of('.');
@@ -1026,7 +1075,10 @@ int main(int argc, char** argv) {
             "  DIR/stab_<clip>_<frame>.png, the corrections to DIR/stab.txt; not with --warm-start\n"
             "  --scene-flow DISPLIST (flow binaries): the disparities of image1 and image2 of every pair (PFM or KITTI\n"
             "  PNG) give <stem>_disp1.pfm (<stem>_disp1<ext> with --kitti), and with --camera <stem>_sceneflow.pfm;\n"
-            "  --gt-scene-flow GTLIST: disp0, disp1 and flow ground truth per pair, SFEVAL lines; not with --warm-start\n",
+            "  --gt-scene-flow GTLIST: disp0, disp1 and flow ground truth per pair, SFEVAL lines; not with --warm-start\n"
+            "  --odometry DIR (flow binaries, with --scene-flow and --camera): the rig's ego-motion of every pair to\n"
+            "  DIR/odometry.txt, each clip's KITTI poses to DIR/poses_<clip>.txt, <stem>_objects.pgm and\n"
+            "  <stem>_objmotion.pfm; --gt-poses LIST: one KITTI poses file per clip, ODOEVAL lines; not with --warm-start\n",
             argv[0]);
     return 2;
   }
@@ -1047,6 +1099,8 @@ int main(int argc, char** argv) {
   const char* stab_arg[3] = {nullptr, nullptr, nullptr};  // --stabilize RADIUS CROP DIR
   const char* sf_list = nullptr;    // --scene-flow DISPLIST
   const char* sf_gtlist = nullptr;  // --gt-scene-flow GTLIST
+  const char* odo_dir = nullptr;     // --odometry DIR
+  const char* odo_gtlist = nullptr;  // --gt-poses LIST
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -1152,6 +1206,20 @@ int main(int argc, char** argv) {
       }
       sf_gtlist = argv[first_num + 1];
       first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--odometry")) {
+      if (argc < first_num + 2 || odo_dir) {
+        fprintf(stderr, "error: --odometry takes one output directory\n");
+        return 2;
+      }
+      odo_dir = argv[first_num + 1];
+      first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt-poses")) {
+      if (argc < first_num + 2 || odo_gtlist) {
+        fprintf(stderr, "error: --gt-poses takes one list of KITTI poses files\n");
+        return 2;
+      }
+      odo_gtlist = argv[first_num + 1];
+      first_num += 2;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
       if (argc < first_num + 2 || gtlist) {
         fprintf(stderr, "error: --gt takes one ground-truth list file\n");
@@ -1189,6 +1257,22 @@ int main(int argc, char** argv) {
   }
   if (sf_gtlist && !sf_list) {
     fprintf(stderr, "error: --gt-scene-flow evaluates the scene flow of --scene-flow; give --scene-flow too\n");
+    return 2;
+  }
+  if (odo_dir && SELECTMODE != 1) {
+    fprintf(stderr, "error: --odometry fits the rig's motion from flows; the stereo binaries take no --odometry\n");
+    return 2;
+  }
+  if (odo_dir && warm) {
+    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --odometry\n");
+    return 2;
+  }
+  if (odo_dir && (!sf_list || !camera_arg)) {
+    fprintf(stderr, "error: --odometry needs the disparities of --scene-flow and the stereo camera of --camera\n");
+    return 2;
+  }
+  if (odo_gtlist && !odo_dir) {
+    fprintf(stderr, "error: --gt-poses evaluates the poses of --odometry; give --odometry too\n");
     return 2;
   }
   // --camera on a flow binary belongs to --scene-flow
@@ -1458,6 +1542,68 @@ int main(int argc, char** argv) {
       }
     }
   }
+  // --odometry: the clip and frame of every pair, the ground-truth poses of every clip and the output files, before
+  // any device work
+  vector<int> odo_clip(jobs.size(), 0), odo_frame(jobs.size(), 0);
+  vector<vector<double>> odo_gt;  // per clip, 12 numbers per line
+  vector<vector<double>> odo_rel;  // per clip, 12 numbers per pair (filled as the pairs are computed)
+  FILE* odo_file = nullptr;
+  if (odo_dir) {
+    int nclips = 0;
+    for (size_t k = 0; k < jobs.size(); ++k) {
+      const bool cont = k > 0 && jobs[k].a == jobs[k - 1].b;
+      odo_clip[k] = cont ? odo_clip[k - 1] : nclips++;
+      odo_frame[k] = cont ? odo_frame[k - 1] + 1 : 0;
+    }
+    odo_rel.resize(nclips);
+    if (odo_gtlist) {
+      FILE* f = fopen(odo_gtlist, "r");
+      if (!f) {
+        fprintf(stderr, "error: cannot read %s\n", odo_gtlist);
+        return 2;
+      }
+      vector<string> files;
+      char g[4096];
+      while (fscanf(f, "%4095s", g) == 1) files.push_back(g);
+      fclose(f);
+      if ((int)files.size() != nclips) {
+        fprintf(stderr, "error: --gt-poses: %s lists %zu poses files for %d clips\n", odo_gtlist, files.size(), nclips);
+        return 2;
+      }
+      vector<int> need(nclips, 0);
+      for (size_t k = 0; k < jobs.size(); ++k) need[odo_clip[k]] = odo_frame[k] + 2;
+      for (int c = 0; c < nclips; ++c) {
+        FILE* pf = fopen(files[c].c_str(), "r");
+        if (!pf) {
+          fprintf(stderr, "error: cannot read %s\n", files[c].c_str());
+          return 2;
+        }
+        vector<double> v;
+        double x;
+        while (fscanf(pf, "%lf", &x) == 1) v.push_back(x);
+        const bool eof = feof(pf);
+        fclose(pf);
+        if (!eof || v.size() % 12 || (int)(v.size() / 12) < need[c]) {
+          fprintf(stderr, "error: %s: a KITTI poses file of at least %d lines of 12 numbers, got %zu numbers\n",
+                  files[c].c_str(), need[c], v.size());
+          return 2;
+        }
+        odo_gt.push_back(v);
+      }
+    }
+    const string path = string(odo_dir) + "/odometry.txt";
+    odo_file = fopen(path.c_str(), "w");
+    if (!odo_file) {
+      fprintf(stderr, "error: --odometry: cannot write %s\n", path.c_str());
+      return 2;
+    }
+  }
+  double odo_terr = 0.0, odo_rerr = 0.0;
+  size_t odo_eval = 0;
+  vector<double> odo_pose;
+  vector<ofdis_motion_stats> odo_stats;
+  vector<uint8_t> odo_mask;
+  vector<float> odo_om;
   // --descriptors, --fisher: every pair's frames hold an N x N patch, checked before any device work
   for (size_t k = 0; k < jobs.size() && traj_stage; ++k) {
     int iw = 0, ih = 0;
@@ -1978,6 +2124,43 @@ int main(int argc, char** argv) {
         }
         if (camera_arg) save_pfm3(&sf_m[3 * k * pix], w, h, with_suffix(jobs[j0 + k].out, "_sceneflow", ".pfm").c_str());
       }
+      if (rc == OFDIS_OK && odo_dir) {
+        ofdis_egomotion_params ep;
+        memset(&ep, 0, sizeof(ep));
+        ep.step = 8;
+        ep.fb_check = bidir ? 1 : 0;
+        ep.alpha = 0.01f;
+        ep.beta = 0.5f;
+        ep.edge_diff = 1.0f;
+        ep.hypotheses = 1024;
+        ep.threshold = 1.0f;
+        ep.refine = 5;
+        ep.seed = 0;
+        odo_pose.resize((size_t)12 * n);
+        odo_stats.resize(n);
+        odo_mask.resize(n * pix);
+        odo_om.resize(3 * n * pix);
+        rc = ofdis_egomotion_fullres(ctx, 0, n, n, &ep, sf_d0.data(), sf_d1.data(), pix, &dcam, odo_pose.data(),
+                                     odo_stats.data(), odo_mask.data(), nullptr, odo_om.data(), w, h, OFDIS_MEM_HOST);
+        for (int k = 0; k < n && rc == OFDIS_OK; ++k) {
+          const int c = odo_clip[j0 + k], fr = odo_frame[j0 + k];
+          const ofdis_motion_stats& st = odo_stats[k];
+          const double* P = odo_pose.data() + (size_t)12 * k;
+          fprintf(odo_file, "%d %d %d %d %d %d", c, fr, st.status, st.n_corr, st.ransac_inliers, st.n_inliers);
+          for (int i = 0; i < 12; ++i) fprintf(odo_file, " %.17g", P[i]);
+          fprintf(odo_file, "\n");
+          odo_rel[c].insert(odo_rel[c].end(), P, P + 12);
+          save_mask_pgm(odo_mask.data() + k * pix, w, h, with_suffix(jobs[j0 + k].out, "_objects", ".pgm").c_str());
+          save_pfm3(&odo_om[3 * k * pix], w, h, with_suffix(jobs[j0 + k].out, "_objmotion", ".pfm").c_str());
+          if (!odo_gtlist) continue;
+          double te, re;
+          pose_error(&odo_gt[c][(size_t)12 * fr], &odo_gt[c][(size_t)12 * (fr + 1)], P, &te, &re);
+          odo_terr += te;
+          odo_rerr += re;
+          ++odo_eval;
+          if (verbosity > 0) printf("ODOEVAL %d %d %.9g %.9g\n", c, fr, te, re);
+        }
+      }
     }
     if (rc != OFDIS_OK) {
       fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
@@ -2139,6 +2322,26 @@ int main(int argc, char** argv) {
     fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
     return 1;
   }
+  if (odo_file && fclose(odo_file) != 0) {
+    fprintf(stderr, "error: cannot write %s/odometry.txt\n", odo_dir);
+    return 1;
+  }
+  for (size_t c = 0; c < odo_rel.size(); ++c) {
+    char name[32];
+    snprintf(name, sizeof(name), "/poses_%04zu.txt", c);
+    const string path = string(odo_dir) + name;
+    FILE* f = fopen(path.c_str(), "w");
+    double T[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+    for (size_t k = 0; f && k <= odo_rel[c].size() / 12; ++k) {
+      if (k > 0) chain_pose(T, &odo_rel[c][12 * (k - 1)]);
+      for (int i = 0; i < 12; ++i) fprintf(f, i ? " %.17g" : "%.17g", T[i]);
+      fprintf(f, "\n");
+    }
+    if (!f || fclose(f) != 0) {
+      fprintf(stderr, "error: cannot write %s\n", path.c_str());
+      return 1;
+    }
+  }
   if (verbosity > 0) printf("TIME (%zu pairs, load + flow + save) (ms): %3g\n", done, elapsed_ms(tv));
   if (verbosity > 0 && seq_pairs) printf("SEQUENCE (%zu of %zu pairs from %zu decoded frames)\n", seq_pairs, done, seq_decoded);
   if (verbosity > 0 && warm) printf("WARM START (%zu of %zu pairs from the previous pair's flow)\n", warm_pairs, done);
@@ -2158,6 +2361,9 @@ int main(int argc, char** argv) {
     print_eval("", done, eval_total[0]);
     for (int c = 0; c < nclasses && bidir; ++c) print_eval(kClassNames[c], done, eval_total[1 + c]);
   }
+  if (verbosity > 0 && odo_gtlist)
+    printf("ODOEVAL (%zu pairs) t_err %.9g r_err %.9g\n", odo_eval, odo_eval ? odo_terr / odo_eval : 0.0,
+           odo_eval ? odo_rerr / odo_eval : 0.0);
   if (verbosity > 0 && sf_gtlist) {
     static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
     print_sfeval("", done, sf_total[0]);

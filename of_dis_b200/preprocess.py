@@ -1017,6 +1017,34 @@ def _known_disp(d: np.ndarray) -> np.ndarray:
     return (d >= 0) & (d <= np.float32(1e9))
 
 
+def sf_gather_d1(D1: np.ndarray, xs: np.ndarray, ys: np.ndarray, inside: np.ndarray, edge_diff) -> np.ndarray:
+    """Step 2 of ofdis_scene_flow_fullres: the second disparity D1 (n, h, w) gathered at the targets (xs, ys) (float32,
+    (n, ...)) that lie in the frame (`inside`; the value elsewhere is meaningless).  Four known corners spread by at
+    most edge_diff blend bilinearly, rows first; otherwise the nearest corner."""
+    f32 = np.float32
+    n, h, w = D1.shape
+    with np.errstate(invalid="ignore", over="ignore"):
+        xc = np.where(inside, xs, f32(0))
+        yc = np.where(inside, ys, f32(0))
+        x0 = np.floor(xc).astype(np.int64)
+        y0 = np.floor(yc).astype(np.int64)
+        x1 = np.minimum(x0 + 1, w - 1)
+        y1 = np.minimum(y0 + 1, h - 1)
+        fx = (xc - x0.astype(f32)).astype(f32)
+        fy = (yc - y0.astype(f32)).astype(f32)
+        k = np.arange(n).reshape((n,) + (1,) * (xs.ndim - 1))
+        c00, c10, c01, c11 = D1[k, y0, x0], D1[k, y0, x1], D1[k, y1, x0], D1[k, y1, x1]
+        corners_known = _known_disp(c00) & _known_disp(c10) & _known_disp(c01) & _known_disp(c11)
+        hi = np.maximum(np.maximum(c00, c10), np.maximum(c01, c11))
+        lo = np.minimum(np.minimum(c00, c10), np.minimum(c01, c11))
+        blend = corners_known & ((hi - lo) <= f32(edge_diff))
+        gx, gy = f32(1) - fx, f32(1) - fy
+        r0 = c00 * gx + c10 * fx
+        r1 = c01 * gx + c11 * fx
+        near = np.where(fy >= f32(0.5), np.where(fx >= f32(0.5), c11, c01), np.where(fx >= f32(0.5), c10, c00))
+        return np.where(blend, r0 * gy + r1 * fy, near).astype(f32)
+
+
 def scene_flow(F: np.ndarray, disp0: np.ndarray, disp1: np.ndarray, edge_diff: float = 1.0, camera=None, gt=None,
                classes: np.ndarray | None = None, nclasses: int = 1):
     """ofdis_scene_flow_fullres bit for bit, float32 without contraction.  F: full-resolution flows, (h, w, 2) for one
@@ -1048,25 +1076,7 @@ def scene_flow(F: np.ndarray, disp0: np.ndarray, disp1: np.ndarray, edge_diff: f
         xs = np.arange(w, dtype=f32)[None, None, :] + u
         ys = np.arange(h, dtype=f32)[None, :, None] + v
         inside = (xs >= 0) & (xs <= f32(w - 1)) & (ys >= 0) & (ys <= f32(h - 1))
-        xc = np.where(inside, xs, f32(0))
-        yc = np.where(inside, ys, f32(0))
-        x0 = np.floor(xc).astype(np.int64)
-        y0 = np.floor(yc).astype(np.int64)
-        x1 = np.minimum(x0 + 1, w - 1)
-        y1 = np.minimum(y0 + 1, h - 1)
-        fx = (xc - x0.astype(f32)).astype(f32)
-        fy = (yc - y0.astype(f32)).astype(f32)
-        k = np.arange(n)[:, None, None]
-        c00, c10, c01, c11 = D1[k, y0, x0], D1[k, y0, x1], D1[k, y1, x0], D1[k, y1, x1]
-        corners_known = _known_disp(c00) & _known_disp(c10) & _known_disp(c01) & _known_disp(c11)
-        hi = np.maximum(np.maximum(c00, c10), np.maximum(c01, c11))
-        lo = np.minimum(np.minimum(c00, c10), np.minimum(c01, c11))
-        blend = corners_known & ((hi - lo) <= f32(edge_diff))
-        gx, gy = f32(1) - fx, f32(1) - fy
-        r0 = c00 * gx + c10 * fx
-        r1 = c01 * gx + c11 * fx
-        near = np.where(fy >= f32(0.5), np.where(fx >= f32(0.5), c11, c01), np.where(fx >= f32(0.5), c10, c00))
-        d1 = np.where(blend, r0 * gy + r1 * fy, near).astype(f32)
+        d1 = sf_gather_d1(D1, xs, ys, inside, edge_diff)
         k0 = _known_disp(D0)
         k1 = inside & _known_disp(d1)
         status = (np.where(k0, 0, 1) | np.where(inside, 0, 2) | np.where(inside & ~k1, 4, 0)).astype(np.uint8)
@@ -1382,6 +1392,346 @@ def _sample_u8(I: np.ndarray, wq: np.ndarray, xw: np.ndarray, yw: np.ndarray) ->
     val = _bilinear_frame(img, np.where(ins, xw, f32(0)), np.where(ins, yw, f32(0)))
     out = (np.fmin(np.fmax(val, f32(0)), f32(255)) + f32(0.5)).astype(np.uint8)
     return np.where(ins[..., None], out, np.uint8(0)).reshape(I.shape)
+
+
+# ---- stereo ego-motion (ofdis_egomotion_fullres) ---------------------------------------------------------------------
+# ofdis_egomotion_params, field for field; the stats are MOTION_STATS_DTYPE
+EGO_PARAM_FIELDS = ("step", "fb_check", "alpha", "beta", "edge_diff", "hypotheses", "threshold", "refine", "seed")
+
+
+def _ego_cam(camera) -> dict:
+    cam = {key: np.float32(camera[key]) for key in STEREO_CAMERA_FIELDS}
+    cam["fb"] = np.float32(cam["fx"] * cam["baseline"])
+    return cam
+
+
+def ego_pixels(F: np.ndarray, D0: np.ndarray, D1: np.ndarray, cam: dict, edge_diff, valid_fb=None) -> dict:
+    """Step 1 of ofdis_egomotion_fullres at every pixel of one pair: F (h, w, 2), D0 and D1 (h, w) float32.  Returns
+    float32 arrays xs, ys, d0, d1, s0, s1, X, Y, Z (P), the bool arrays usable0 (d0 known, s0 > 0) and valid (the pixel
+    would be a correspondence; valid_fb, the consistency mask == 0, joins it where given)."""
+    f32 = np.float32
+    h, w = D0.shape
+    u, v = F[..., 0], F[..., 1]
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        xs = np.arange(w, dtype=f32)[None, :] + u
+        ys = np.arange(h, dtype=f32)[:, None] + v
+        inside = (xs >= 0) & (xs <= f32(w - 1)) & (ys >= 0) & (ys <= f32(h - 1))
+        d1 = sf_gather_d1(D1[None], xs[None], ys[None], inside[None], edge_diff)[0]
+        d1 = np.where(inside, d1, _QNAN).astype(f32)
+        s0 = (D0 + cam["doffs"]).astype(f32)
+        s1 = (d1 + cam["doffs"]).astype(f32)
+        usable0 = _known_disp(D0) & (s0 > 0)
+        Z = (cam["fb"] / s0).astype(f32)
+        X = (((np.arange(w, dtype=f32)[None, :] - cam["cx"]) * Z) / cam["fx"]).astype(f32)
+        Y = (((np.arange(h, dtype=f32)[:, None] - cam["cy"]) * Z) / cam["fy"]).astype(f32)
+        valid = usable0 & inside & _known_disp(d1) & (s1 > 0)
+    if valid_fb is not None:
+        valid &= valid_fb
+    return dict(xs=xs, ys=ys, d0=D0, d1=d1, s0=s0, s1=s1, X=X, Y=Y, Z=Z, usable0=usable0, valid=valid)
+
+
+def ego_q(cam: dict, xs, ys, s1):
+    """Q, the t+1 point of observations (xs, ys, s1 = d1 + doffs): scene flow's (X1, Y1, Z1), float32."""
+    with np.errstate(all="ignore"):
+        Z1 = (cam["fb"] / np.asarray(s1, np.float32)).astype(np.float32)
+        X1 = (((np.asarray(xs, np.float32) - cam["cx"]) * Z1) / cam["fx"]).astype(np.float32)
+        Y1 = (((np.asarray(ys, np.float32) - cam["cy"]) * Z1) / cam["fy"]).astype(np.float32)
+    return X1, Y1, Z1
+
+
+def _cross(a, b):
+    return np.stack([a[..., 1] * b[..., 2] - a[..., 2] * b[..., 1], a[..., 2] * b[..., 0] - a[..., 0] * b[..., 2],
+                     a[..., 0] * b[..., 1] - a[..., 1] * b[..., 0]], -1)
+
+
+def _triad(A, B, C):
+    """The triads (e1, e2, n) of point triples A, B, C (..., 3) float64: (..., 3 rows, 3) and whether both lengths are
+    > 0."""
+    with np.errstate(all="ignore"):
+        u, v = B - A, C - A
+        L = np.sqrt((u[..., 0] * u[..., 0] + u[..., 1] * u[..., 1]) + u[..., 2] * u[..., 2])
+        e1 = u / L[..., None]
+        nn = _cross(e1, v)
+        Ln = np.sqrt((nn[..., 0] * nn[..., 0] + nn[..., 1] * nn[..., 1]) + nn[..., 2] * nn[..., 2])
+        n = nn / Ln[..., None]
+        e2 = _cross(n, e1)
+    return np.stack([e1, e2, n], -2), (L > 0) & (Ln > 0)
+
+
+def ego_fit3(P: np.ndarray, Q: np.ndarray):
+    """The closed-form rigid fit of ofdis_egomotion_fullres's step 2 from three point pairs P, Q (..., 3, 3) float64:
+    returns ([R | t] (..., 12) float64, ok (...,))."""
+    E, okp = _triad(P[..., 0, :], P[..., 1, :], P[..., 2, :])
+    G, okq = _triad(Q[..., 0, :], Q[..., 1, :], Q[..., 2, :])
+    with np.errstate(all="ignore"):
+        R = ((G[..., 0, :, None] * E[..., 0, None, :]) + (G[..., 1, :, None] * E[..., 1, None, :])) + \
+            (G[..., 2, :, None] * E[..., 2, None, :])
+        cP = ((P[..., 0, :] + P[..., 1, :]) + P[..., 2, :]) / 3.0
+        cQ = ((Q[..., 0, :] + Q[..., 1, :]) + Q[..., 2, :]) / 3.0
+        t = cQ - (((R[..., 0] * cP[..., 0, None]) + (R[..., 1] * cP[..., 1, None])) + (R[..., 2] * cP[..., 2, None]))
+    M = np.concatenate([R, t[..., None]], -1).reshape(P.shape[:-2] + (12,))
+    return M, okp & okq & np.isfinite(M).all(axis=-1)
+
+
+def ego_transform(g: np.ndarray, X, Y, Z):
+    """P' = g P in float32 for g (..., 12) against points (m,): (X', Y', Z') each (..., m)."""
+    g = np.asarray(g, np.float32)[..., None, :]
+    with np.errstate(all="ignore"):
+        Xp = ((g[..., 0] * X + g[..., 1] * Y) + g[..., 2] * Z) + g[..., 3]
+        Yp = ((g[..., 4] * X + g[..., 5] * Y) + g[..., 6] * Z) + g[..., 7]
+        Zp = ((g[..., 8] * X + g[..., 9] * Y) + g[..., 10] * Z) + g[..., 11]
+    return Xp, Yp, Zp
+
+
+def ego_inliers(g: np.ndarray, c: np.ndarray, cam: dict, threshold) -> np.ndarray:
+    """The inlier test of ofdis_egomotion_fullres, float32: g (..., 12) against the correspondences c (m, 8) (X, Y, Z,
+    xs, ys, d1, s1, 0); returns (..., m) bool."""
+    f32 = np.float32
+    Xp, Yp, Zp = ego_transform(g, c[:, 0], c[:, 1], c[:, 2])
+    with np.errstate(all="ignore"):
+        ex = (cam["fx"] * Xp + cam["cx"] * Zp) - c[:, 3] * Zp
+        ey = (cam["fy"] * Yp + cam["cy"] * Zp) - c[:, 4] * Zp
+        ed = cam["fb"] - c[:, 6] * Zp
+        tz = f32(threshold) * Zp
+        return (Zp > 0) & ((ex * ex + ey * ey) + ed * ed <= tz * tz)
+
+
+def _chunk_tree(T: np.ndarray) -> np.ndarray:
+    """Sums of the rows of T (m, ne) float64 in chunks of 32 from +0.0, then a pairwise tree over the chunk sums padded
+    with +0.0 to a power of two."""
+    m, ne = T.shape
+    nc = (m + 31) // 32
+    T = np.concatenate([T, np.zeros((nc * 32 - m, ne))]).reshape(nc, 32, ne)
+    v = np.zeros((nc, ne))
+    for e in range(32):
+        v = v + T[:, e]
+    P = 1
+    while P < nc:
+        P *= 2
+    v = np.concatenate([v, np.zeros((P - nc, ne))])
+    while v.shape[0] > 1:
+        v = v[0::2] + v[1::2]
+    return v[0]
+
+
+def ego_rows(M: np.ndarray, c: np.ndarray, cam: dict):
+    """The refit's Jacobian rows J (m, 3, 6) and residuals r (m, 3) (x, y, disparity) of the correspondences c at the
+    float64 model M (12,), in the header's expression order."""
+    X, Y, Z = (c[:, i].astype(np.float64) for i in range(3))
+    Pp = [(((M[4 * i] * X) + (M[4 * i + 1] * Y)) + (M[4 * i + 2] * Z)) + M[4 * i + 3] for i in range(3)]
+    fx, fy, cx, cy, fb, doffs = (float(cam[k]) for k in ("fx", "fy", "cx", "cy", "fb", "doffs"))
+    zero = np.zeros_like(X)
+    with np.errstate(all="ignore"):
+        iz = 1.0 / Pp[2]
+        u, v = Pp[0] * iz, Pp[1] * iz
+        ax = (fx * iz, zero, -((fx * iz) * u))
+        ay = (zero, fy * iz, -((fy * iz) * v))
+        ad = (zero, zero, -((fb * iz) * iz))
+        r = np.stack([((fx * u) + cx) - c[:, 3].astype(np.float64), ((fy * v) + cy) - c[:, 4].astype(np.float64),
+                      ((fb * iz) - doffs) - c[:, 5].astype(np.float64)], -1)
+        w0, w1, w2 = 2.0 * Pp[0], 2.0 * Pp[1], 2.0 * Pp[2]
+        J = np.stack([np.stack([(a[1] * -w2) + (a[2] * w1), (a[0] * w2) + (a[2] * -w0), (a[0] * -w1) + (a[1] * w0),
+                                a[0], a[1], a[2]], -1) for a in (ax, ay, ad)], 1)
+    return J, r
+
+
+def ego_normal_sums(M: np.ndarray, c: np.ndarray, inl: np.ndarray, cam: dict):
+    """The refit's normal equations (A (6, 6), b (6,)) from the inliers `inl` of c (m, 8) at the model M."""
+    J, r = ego_rows(M, c, cam)
+    with np.errstate(all="ignore"):
+        terms = [((J[:, 0, a] * J[:, 0, b]) + (J[:, 1, a] * J[:, 1, b])) + (J[:, 2, a] * J[:, 2, b])
+                 for a in range(6) for b in range(a, 6)]
+        terms += [-(((J[:, 0, a] * r[:, 0]) + (J[:, 1, a] * r[:, 1])) + (J[:, 2, a] * r[:, 2])) for a in range(6)]
+    T = np.where(inl[:, None], np.stack(terms, -1), 0.0)
+    v = _chunk_tree(T)
+    A = np.zeros((6, 6))
+    e = 0
+    for a in range(6):
+        for b in range(a, 6):
+            A[a, b] = A[b, a] = v[e]
+            e += 1
+    return A, v[e:]
+
+
+def ego_update(M: np.ndarray, x: np.ndarray) -> np.ndarray:
+    """[R | t] <- [C R | C t + tau] with the Cayley rotation C of omega = x[:3] and tau = x[3:]."""
+    w = x[:3]
+    q = (w[0] * w[0] + w[1] * w[1]) + w[2] * w[2]
+    dg, dn = 1.0 - q, 1.0 + q
+    K = ((0.0, -w[2], w[1]), (w[2], 0.0, -w[0]), (-w[1], w[0], 0.0))
+    C = [[(((dg if i == j else 0.0) + (2.0 * (w[i] * w[j]))) + (2.0 * K[i][j])) / dn for j in range(3)]
+         for i in range(3)]
+    Mn = np.zeros(12)
+    for i in range(3):
+        for j in range(4):
+            Mn[4 * i + j] = ((C[i][0] * M[j]) + (C[i][1] * M[4 + j])) + (C[i][2] * M[8 + j])
+        Mn[4 * i + 3] = Mn[4 * i + 3] + x[3 + i]
+    return Mn
+
+
+def ego_correspondences(px: dict, step: int) -> np.ndarray:
+    """The compacted correspondences (m, 8) float32 (X, Y, Z, xs, ys, d1, s1, 0) of step 1 from ego_pixels' arrays."""
+    h, w = px["valid"].shape
+    s = int(step)
+    ncx, ncy = (w - 1) // s + 1, (h - 1) // s + 1
+    cell = np.arange(ncx * ncy)
+    cxs = np.minimum((cell % ncx) * s + s // 2, w - 1)
+    cys = np.minimum((cell // ncx) * s + s // 2, h - 1)
+    sel = px["valid"][cys, cxs]
+    cxs, cys = cxs[sel], cys[sel]
+    cols = [px[k][cys, cxs] for k in ("X", "Y", "Z", "xs", "ys", "d1", "s1")]
+    return np.stack(cols + [np.zeros(cxs.shape[0], np.float32)], -1).astype(np.float32)
+
+
+def _ego_pair(F, B, D0, D1, cam, p):
+    f32 = np.float32
+    h, w = D0.shape
+    fbm = consistency_check(F, B, p["alpha"], p["beta"])[0] == 0 if p["fb_check"] else None
+    px = ego_pixels(F, D0, D1, cam, p["edge_diff"], fbm)
+    corr = ego_correspondences(px, p["step"])
+    m = corr.shape[0]
+    st = np.zeros((), MOTION_STATS_DTYPE)
+    st["n_corr"], st["best_hypothesis"] = m, -1
+    status = 1 if m < 3 else 0
+    thr = p["threshold"]
+    if not status:
+        idx = motion_draws(int(p["seed"]), int(p["hypotheses"]), 3, m)
+        c = corr[idx]  # (nh, 3, 8)
+        P = c[..., 0:3].astype(np.float64)
+        Q = np.stack(ego_q(cam, c[..., 3], c[..., 4], c[..., 6]), -1).astype(np.float64)
+        Ms, ok = ego_fit3(P, Q)
+        g = Ms.astype(f32)
+        counts = np.zeros(idx.shape[0], np.int64)
+        for h0 in range(0, idx.shape[0], 256):
+            counts[h0:h0 + 256] = ego_inliers(g[h0:h0 + 256], corr, cam, thr).sum(axis=1)
+        if not ok.any():
+            status = 2
+    if status:
+        pose = np.full(12, _QNAN64)
+    else:
+        keys = np.where(ok, (counts << 32) | (0xFFFFFFFF - np.arange(idx.shape[0])), -1)
+        best = int(np.argmax(keys))
+        st["best_hypothesis"], st["ransac_inliers"] = best, counts[best]
+        M = Ms[best]
+        refits = 0
+        for r in range(int(p["refine"]) + 1):
+            inl = ego_inliers(M.astype(f32), corr, cam, thr)
+            cnt = int(inl.sum())
+            if r == int(p["refine"]) or cnt < 3:
+                break
+            A, b = ego_normal_sums(M, corr, inl, cam)
+            x, okn = motion_solve(A[None], b[None])
+            if not okn[0]:
+                break
+            M, refits = ego_update(M, x[0]), refits + 1
+        st["refits"], st["n_inliers"] = refits, cnt
+        pose = np.where(np.isnan(M), _QNAN64, M)
+    st["status"] = status
+    # per pixel
+    mask = np.full((h, w), 2, np.uint8)
+    residual = np.full((h, w, 2), _QNAN, f32)
+    objm = np.full((h, w, 3), _QNAN, f32)
+    if status:
+        return pose, st, mask, residual, objm
+    g = pose.astype(f32)
+    X, Y, Z = px["X"].ravel(), px["Y"].ravel(), px["Z"].ravel()
+    Xp, Yp, Zp = (a.reshape(h, w) for a in ego_transform(g, X, Y, Z))
+    with np.errstate(all="ignore"):
+        xi = (cam["fx"] * Xp) / Zp + cam["cx"]
+        yi = (cam["fy"] * Yp) / Zp + cam["cy"]
+        rx = F[..., 0] - (xi - np.arange(w, dtype=f32)[None, :])
+        ry = F[..., 1] - (yi - np.arange(h, dtype=f32)[:, None])
+    res = np.stack([rx, ry], -1).astype(f32)
+    res = np.where(np.isnan(res), _QNAN, res)
+    residual = np.where(px["usable0"][..., None], res, _QNAN).astype(f32)
+    cflat = np.stack([px[k].ravel() for k in ("X", "Y", "Z", "xs", "ys", "d1", "s1")] +
+                     [np.zeros(h * w, f32)], -1).astype(f32)
+    inl = ego_inliers(g, cflat, cam, thr).reshape(h, w)
+    with np.errstate(invalid="ignore"):
+        live = px["valid"] & (Zp > 0)
+    mask = np.where(live, np.where(inl, 0, 1), 2).astype(np.uint8)
+    X1, Y1, Z1 = ego_q(cam, px["xs"], px["ys"], px["s1"])
+    with np.errstate(all="ignore"):
+        om = np.stack([X1 - Xp, Y1 - Yp, Z1 - Zp], -1).astype(f32)
+    om = np.where(np.isnan(om), _QNAN, om)
+    objm = np.where(live[..., None], om, _QNAN).astype(f32)
+    return pose, st, mask, residual, objm
+
+
+def egomotion_params(params) -> dict:
+    return {k: params[k] for k in EGO_PARAM_FIELDS}
+
+
+def egomotion(F: np.ndarray, B: np.ndarray | None, disp0: np.ndarray, disp1: np.ndarray, camera, params):
+    """ofdis_egomotion_fullres bit for bit.  F: the forward flows (n, h, w, 2) exactly as ofdis_get_flow_fullres
+    returns them, B the partner flows of fb_check (else None); disp0, disp1 (n, h, w) float32 positive disparities
+    with NaN for unknown; camera a mapping with STEREO_CAMERA_FIELDS; params a mapping with EGO_PARAM_FIELDS.  Returns
+    (pose (n, 3, 4) float64, stats (n,) MOTION_STATS_DTYPE, mask (n, h, w) uint8, residual (n, h, w, 2) and
+    object_motion (n, h, w, 3) float32)."""
+    p = egomotion_params(params)
+    cam = _ego_cam(camera)
+    F = np.asarray(F, np.float32)
+    n, h, w = F.shape[:3]
+    D0 = np.asarray(disp0, np.float32).reshape(n, h, w)
+    D1 = np.asarray(disp1, np.float32).reshape(n, h, w)
+    out = [_ego_pair(F[k], None if B is None else np.asarray(B[k], np.float32), D0[k], D1[k], cam, p)
+           for k in range(n)]
+    pose = np.stack([o[0] for o in out]).reshape(n, 3, 4) if n else np.zeros((0, 3, 4))
+    stats = np.array([o[1] for o in out], MOTION_STATS_DTYPE).reshape(n)
+    return (pose, stats, np.stack([o[2] for o in out]), np.stack([o[3] for o in out]),
+            np.stack([o[4] for o in out]))
+
+
+# ---- poses (float64 host helpers, no bit contract) -------------------------------------------------------------------
+def _pose44(P) -> np.ndarray:
+    T = np.eye(4)
+    T[:3, :4] = np.asarray(P, np.float64).reshape(3, 4)
+    return T
+
+
+def chain_poses(rel) -> np.ndarray:
+    """Camera-to-world poses (n+1, 3, 4) of a clip in KITTI's odometry convention from its relative poses rel (n, 3, 4)
+    (camera t to camera t+1, as ofdis_egomotion_fullres returns them): T_0 = I, T_(k+1) = T_k inv([R | t]_k)."""
+    rel = np.asarray(rel, np.float64).reshape(-1, 3, 4)
+    T = np.eye(4)
+    out = [T[:3].copy()]
+    for P in rel:
+        T = T @ np.linalg.inv(_pose44(P))
+        out.append(T[:3].copy())
+    return np.stack(out)
+
+
+def write_kitti_poses(path: str, poses) -> None:
+    """KITTI's odometry poses file: one line of the 12 row-major numbers of [R | t] per frame (%.17g)."""
+    with open(path, "w") as f:
+        for P in np.asarray(poses, np.float64).reshape(-1, 12):
+            f.write(" ".join("%.17g" % v for v in P) + "\n")
+
+
+def read_kitti_poses(path: str) -> np.ndarray:
+    """A KITTI odometry poses file as (n, 3, 4) float64."""
+    rows = [list(map(float, line.split())) for line in open(path) if line.strip()]
+    if any(len(r) != 12 for r in rows):
+        raise ValueError("%s: every line of a KITTI poses file has 12 numbers" % path)
+    return np.array(rows, np.float64).reshape(-1, 3, 4)
+
+
+def pose_errors(rel, gt_abs):
+    """Per pair k the relative pose error of rel[k] (camera k to k+1) against ground-truth camera-to-world poses
+    gt_abs (n+1, 3, 4), formed as KITTI's devkit forms it: E = inv(inv(G_k) G_(k+1)) inv([R | t]_k), the translation
+    error |E_t| in metres and the rotation error acos((trace(E_R) - 1) / 2) in degrees.  Returns (t_err (n,),
+    r_err (n,))."""
+    rel = np.asarray(rel, np.float64).reshape(-1, 3, 4)
+    G = np.asarray(gt_abs, np.float64).reshape(-1, 3, 4)
+    t_err, r_err = [], []
+    for k, P in enumerate(rel):
+        d_gt = np.linalg.inv(_pose44(G[k])) @ _pose44(G[k + 1])
+        d_est = np.linalg.inv(_pose44(P))
+        E = np.linalg.inv(d_gt) @ d_est
+        t_err.append(float(np.linalg.norm(E[:3, 3])))
+        c = min(1.0, max(-1.0, 0.5 * (np.trace(E[:3, :3]) - 1.0)))
+        r_err.append(float(np.degrees(np.arccos(c))))
+    return np.array(t_err), np.array(r_err)
 
 
 # ---- video stabilisation (ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish) ---------------------------------

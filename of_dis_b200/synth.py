@@ -242,3 +242,112 @@ def shaky_clip(n: int, h: int, w: int, channels: int = 1, seed: int = 0, pan=(1.
     models = np.stack([poses[t + 1][0] @ np.linalg.inv(poses[t][0]) for t in range(n - 1)])
     smooth = np.stack([np.linalg.inv(J) for _, J in poses])
     return np.ascontiguousarray(np.stack(frames)), models, smooth
+
+
+def axis_angle(w) -> np.ndarray:
+    """The rotation matrix (3, 3) float64 of the rotation vector w (radians, Rodrigues' formula)."""
+    w = np.asarray(w, np.float64)
+    th = float(np.linalg.norm(w))
+    if th == 0.0:
+        return np.eye(3)
+    k = w / th
+    K = np.array([[0.0, -k[2], k[1]], [k[2], 0.0, -k[0]], [-k[1], k[0], 0.0]])
+    return np.eye(3) + np.sin(th) * K + (1.0 - np.cos(th)) * (K @ K)
+
+
+def _value_noise(table: np.ndarray, u: np.ndarray, v: np.ndarray) -> np.ndarray:
+    """Bilinear value noise of a periodic random table at lattice coordinates (u, v)."""
+    n = table.shape[0]
+    u0, v0 = np.floor(u), np.floor(v)
+    fu, fv = u - u0, v - v0
+    i0, j0 = u0.astype(np.int64) % n, v0.astype(np.int64) % n
+    i1, j1 = (i0 + 1) % n, (j0 + 1) % n
+    return ((table[j0, i0] * (1 - fu) + table[j0, i1] * fu) * (1 - fv) +
+            (table[j1, i0] * (1 - fu) + table[j1, i1] * fu) * fv)
+
+
+def rigid_stereo_clip(n: int, h: int, w: int, channels: int, seed: int, camera, motions, block=None):
+    """A stereo clip of a piecewise-planar textured scene seen by a moving rig: a ground plane 1.65 m below the first
+    camera and a back wall 40 m ahead, plus a box on the ground that moves on its own between frames.  camera: a
+    mapping with fx, fy, cx, cy, baseline, doffs; motions: n relative poses (3, 4) (or (R, t) pairs), each mapping a
+    point in camera-t coordinates to camera-t+1 coordinates.  block: None for the default box, or a mapping with
+    "centre" (world, metres, at frame 0), "half" (half sizes) and "velocity" (metres per frame).
+    Returns a dict: "left", "right" (n+1, h, w[, channels]) uint8 frames; "disp" (n+1, h, w) float32, the analytic
+    left disparity fb / Z - doffs of every frame; "flow" (n, h, w, 2) float32, the exact flow of every pair (a pixel's
+    surface point carried by the rig's motion, or by the box's); "poses" (n, 3, 4) float64, the true relative poses;
+    "abs" (n+1, 3, 4) camera-to-world poses; "box" (n, h, w) bool, the box's pixels in frame t."""
+    rng = np.random.default_rng(seed)
+    tables = [rng.uniform(0, 1, (256, 256)) for _ in range(3 * channels)]
+    fx, fy, cx, cy = (float(camera[k]) for k in ("fx", "fy", "cx", "cy"))
+    base, doffs = float(camera["baseline"]), float(camera["doffs"])
+    fb = float(np.float32(np.float32(fx) * np.float32(base)))
+    blk = {"centre": (-1.2, 0.85, 9.0), "half": (0.9, 0.8, 0.9), "velocity": (0.25, 0.0, -0.15)}
+    blk.update(block or {})
+    bc0, bh, bv = (np.asarray(blk[k], np.float64) for k in ("centre", "half", "velocity"))
+    ground, wall = 1.65, 40.0
+    rel = []
+    for mo in motions:
+        if isinstance(mo, (tuple, list)) and len(mo) == 2:
+            P = np.concatenate([np.asarray(mo[0], np.float64), np.asarray(mo[1], np.float64).reshape(3, 1)], 1)
+        else:
+            P = np.asarray(mo, np.float64).reshape(3, 4)
+        rel.append(P)
+    assert len(rel) == n
+    T = [np.eye(4)]
+    for P in rel:
+        M = np.eye(4)
+        M[:3] = P
+        T.append(T[-1] @ np.linalg.inv(M))
+    y, x = np.mgrid[0:h, 0:w].astype(np.float64)
+    dcam = np.stack([(x - cx) / fx, (y - cy) / fy, np.ones_like(x)], -1)
+
+    def cast(Tk, k, right):
+        Rc, tc = Tk[:3, :3], Tk[:3, 3]
+        d = dcam @ Rc.T
+        o = tc + (Rc @ np.array([base, 0.0, 0.0]) if right else 0.0)
+        inf = np.full((h, w), np.inf)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            tg = np.where(d[..., 1] > 0, (ground - o[1]) / d[..., 1], inf)
+            tw = np.where(d[..., 2] > 0, (wall - o[2]) / d[..., 2], inf)
+            lo, hi = bc0 + k * bv - bh, bc0 + k * bv + bh
+            t0 = (lo - o) / d
+            t1 = (hi - o) / d
+            tmin = np.max(np.minimum(t0, t1), -1)
+            tmax = np.min(np.maximum(t0, t1), -1)
+        tb = np.where((tmax >= tmin) & (tmin > 0), tmin, inf)
+        t = np.minimum(np.minimum(tg, tw), tb)
+        p = o + d * t[..., None]
+        return t, p, tb <= np.minimum(tg, tw), tg <= tw
+
+    def shade(p, isbox, isground, k):
+        loc = p - (bc0 + k * bv)
+        su = np.where(isbox, loc[..., 0] + 0.7 * loc[..., 2], p[..., 0])
+        sv = np.where(isbox, loc[..., 1] + 0.3 * loc[..., 2], np.where(isground, p[..., 2], p[..., 1]))
+        img = np.zeros((h, w, channels))
+        for c in range(channels):
+            acc = 0.0
+            for o, scale in enumerate((0.04, 0.15, 0.6)):
+                acc = acc + (0.5 ** o) * _value_noise(tables[3 * c + o], su / scale, sv / scale)
+            img[..., c] = 30.0 + 190.0 * acc / 1.75 + np.where(isbox, 20.0, 0.0)
+        img = np.clip(np.round(img), 0, 255).astype(np.uint8)
+        return img if channels > 1 else img[..., 0]
+
+    left, right, disp, pts, boxes = [], [], [], [], []
+    for k in range(n + 1):
+        t, p, isbox, isground = cast(T[k], k, False)
+        left.append(shade(p, isbox, isground, k))
+        tr, pr, isbox_r, isground_r = cast(T[k], k, True)
+        right.append(shade(pr, isbox_r, isground_r, k))
+        disp.append((fb / t - doffs).astype(np.float32))
+        pts.append(p)
+        boxes.append(isbox)
+    flows = []
+    for k in range(n):
+        p = pts[k] + np.where(boxes[k][..., None], bv, 0.0)
+        Ti = np.linalg.inv(T[k + 1])
+        q = p @ Ti[:3, :3].T + Ti[:3, 3]
+        flows.append(np.stack([fx * q[..., 0] / q[..., 2] + cx - x, fy * q[..., 1] / q[..., 2] + cy - y], -1))
+    return {"left": np.stack(left), "right": np.stack(right), "disp": np.stack(disp),
+            "flow": np.stack(flows).astype(np.float32) if n else np.zeros((0, h, w, 2), np.float32),
+            "poses": np.stack(rel) if n else np.zeros((0, 3, 4)), "abs": np.stack([Tk[:3] for Tk in T]),
+            "box": np.stack(boxes[:n]) if n else np.zeros((0, h, w), bool)}

@@ -6,7 +6,8 @@ kernel, stereo SOR), a 70-row level as three bands of the lane kernel and forced
 wave kernel with 1 and 2 rows per thread (st.async halo exchange), and the 8-bit frame path (pyramid and
 upsampling kernels), and a frame interpolation, a point tracking (advance, seed, block scan, scatter) and a filtered
 disparity (union-find speckles, fill, depth and xyz) and a global motion (correspondences, compaction, hypotheses,
-the bulk-copied score tiles with and without refills, refits, per-pixel outputs) and a Fisher encoding (projection,
+the bulk-copied score tiles with and without refills, refits, per-pixel outputs), a stereo ego-motion (the same
+stages on 32-byte correspondences, non-finite disparities, score tile refills) and a Fisher encoding (projection,
 posteriors, float64 statistics, the take) checked against their restatements.  Results are checked against the
 oracle so that a clean log means a correct run."""
 import os
@@ -147,6 +148,32 @@ exp = preprocess.global_motion(full, None, clip[1:], mp)
 ok = (stats["n_corr"] > 8192).all() and all(np.array_equal(np.asarray(g).view(np.uint8), np.asarray(e).view(np.uint8))
                                             for g, e in zip((models, stats, mask, res, reg), exp))
 print("%-22s %s" % ("global_motion_tiles", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# stereo ego-motion on the same two gray pairs at step 1 (more than two 2048-entry score tiles per pair), disparities
+# with NaN, +inf, -0 and negative entries, fb_check against the backward slots, every per-pixel output
+rng = np.random.default_rng(8)
+cam = dict(fx=200.0, fy=198.5, cx=79.75, cy=64.5, baseline=0.54, doffs=0.25)
+maps = rng.uniform(5.0, 20.0, (n + 1, h2, w2)).astype(np.float32)
+maps[rng.random(maps.shape) < 0.05] = np.nan
+maps[rng.random(maps.shape) < 0.02] = np.inf
+maps[rng.random(maps.shape) < 0.02] = -0.0
+maps[rng.random(maps.shape) < 0.02] = -3.0
+ctx = api.Context(prm, w2, h2, prm.p_samp_s, 2 * n)
+ctx.upload_sequence_bidir_u8(0, n, clip, w2, h2)
+ctx.run(2 * n)
+full = np.empty((2 * n, h2, w2, 2), np.float32)
+ctx.get_flow_fullres(0, 2 * n, full, w2, h2)
+ctx.sync()
+ep = dict(step=1, fb_check=1, alpha=0.01, beta=0.5, edge_diff=1.0, hypotheses=90, threshold=1.0, refine=3, seed=5)
+pose, stats, outs = ctx.egomotion_fullres(0, n, maps[:-1], maps[1:], ep, camera=cam, width_org=w2, height_org=h2,
+                                          b0=n, outputs=("mask", "residual", "object_motion"))
+ctx.close()
+exp = preprocess.egomotion(full[:n], full[n:], maps[:-1], maps[1:], cam, ep)
+ok = (stats["n_corr"] > 2 * 2048).all() and all(
+    np.array_equal(np.asarray(g).view(np.uint8), np.asarray(e).view(np.uint8))
+    for g, e in zip((pose, stats, outs["mask"], outs["residual"], outs["object_motion"]), exp))
+print("%-22s %s" % ("egomotion_tiles", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 # Fisher encoder (projection GEMM, posteriors, float64 statistics, the take): two chunks of descriptors with IDT's
