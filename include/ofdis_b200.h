@@ -148,7 +148,8 @@ size_t ofdis_packed_images_frame_floats(const ofdis_ctx* ctx);
 int ofdis_upload_packed_images(ofdis_ctx* ctx, int f0, int f1, const float* packed, int memkind);
 
 /* Read-back of one padded array of the device pyramid (which: 0 I0, 1 I0x, 2 I0y, 3 I1); the
- * inverse of ofdis_upload_level, used to check the device-built pyramids. */
+ * inverse of ofdis_upload_level, used to check the device-built pyramids.  With usefbcon, after
+ * ofdis_set_direction(ctx, 1), the arrays of the pair's backward frame: I1, its gradients, I0. */
 int ofdis_get_level(ofdis_ctx* ctx, int frame, int level, int which, float* dst, int memkind);
 
 /* Pyramid on the device (extension, SURVEY 8f rank 1 == ConstructImgPyramide, run_dense.cpp:130-178
@@ -1005,7 +1006,7 @@ int ofdis_profile_levels(ofdis_ctx* ctx, int nframes, int steps, double* ms_by_c
                          double* ms_by_level_class);
 /* usefbcon contexts only: address ONE grid of every pair (0 = forward, 1 = the grid on the swapped images)
  * in the following ofdis_patgrid_optimize / ofdis_patgrid_aggregate (one frame per call) / ofdis_set_flow /
- * ofdis_get_flow / ofdis_get_patches calls; -1 (default) restores "both grids; flows and patches of the
+ * ofdis_get_flow / ofdis_get_patches / ofdis_get_level calls; -1 (default) restores "both grids; flows and patches of the
  * forward one".  This is what two stand-alone PatGridClass objects joined by SetComplGrid
  * (patchgrid.h:36, oflow.cpp:162-170) are built on. */
 int ofdis_set_direction(ofdis_ctx* ctx, int dir);

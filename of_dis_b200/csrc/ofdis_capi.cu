@@ -587,7 +587,9 @@ int ofdis_get_level(ofdis_ctx* ctx, int frame, int level, int which, float* dst,
   if (!L || frame < 0 || frame >= ctx->max_frames || which < 0 || which > 3 || !dst) return fail(ctx, OFDIS_ERR_ARG, "get_level: bad argument");
   CK(cudaSetDevice(ctx->device));
   const size_t n = (size_t)L->tmp_w * L->tmp_h * L->noc;
-  CK(cudaMemcpyAsync(dst, L->img[which] + (size_t)frame * ctx->dirs * L->img_fs[which], sizeof(float) * n, kind_out(memkind), ctx->stream));
+  // the forward frame unless a direction is selected (usefbcon: the backward frame holds the swapped pair)
+  const size_t q = (size_t)frame * ctx->dirs + std::max(ctx->sel_dir, 0);
+  CK(cudaMemcpyAsync(dst, L->img[which] + q * L->img_fs[which], sizeof(float) * n, kind_out(memkind), ctx->stream));
   if (memkind != OFDIS_MEM_DEVICE) CK(cudaStreamSynchronize(ctx->stream));
   return OFDIS_OK;
 }

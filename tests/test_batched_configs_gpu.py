@@ -131,6 +131,13 @@ def batched_inputs(name):
     return prm, pairs, [preprocess.PairPyramids(a, b, prm.sc_f, prm.p_samp_s) for a, b in pairs]
 
 
+@functools.lru_cache(maxsize=None)
+def oracle_flows(name, oracle_port):
+    """the oracle's flows of the distinct pairs of configuration `name`"""
+    prm, _, pyrs = batched_inputs(name)
+    return [oracle_port.port_run(p, prm) for p in pyrs]
+
+
 def slot_pair(f):
     """distinct pair of slot f: neighbouring slots differ"""
     return f % N_DISTINCT
@@ -161,7 +168,7 @@ def test_batched_configuration_vs_oracle(name, api, oracle_port):
                 if k == "sor_max_cluster" and v == 16:
                     pytest.skip("device grants no 16-CTA clusters")
                 raise
-        exp = [oracle_port.port_run(p, prm) for p in pyrs]
+        exp = oracle_flows(name, oracle_port)
         if prm.usefbcon:
             for f in range(nfr):
                 ctx.upload_pyramids(f, pyrs[slot_pair(f)])

@@ -21,12 +21,14 @@ every patch size of SIZE_CASES; every upload path at a padding other than P, pyr
 than 16 frames with graph replay; the Python OFClass mirror.  tests/test_patch_geometry.py pins the oracle to the
 reference build on all of these inputs (golden/reference_digests.json)."""
 import dataclasses
+import types
 
 import numpy as np
 import pytest
 
 from of_dis_b200 import params, preprocess, synth
 from test_gpu_parity import _frames_u8, assert_bits
+from test_initflow_gpu import set_direction
 
 pytestmark = pytest.mark.gpu
 f32 = np.float32
@@ -105,6 +107,10 @@ UPLOAD_CASES = {
     "p12_gray_stereo_pad13": (1, 1, "3 1 12 4 0.05 0.95 0 12 0.75 0 1 1 1 10 10 5 1 3 1.6 0", 13, (96, 170)),
 }
 UPLOAD_PAIRS = 3
+# every route into the device pyramids: the host pyramids (upload_pyramids, upload_packed), host images with the
+# gradients (and usefbcon's swapped copies) derived on the device, float images of level sc_l, and 8-bit frames
+ROUTES = ("upload_pyramids", "upload_packed", "upload_packed_images", "upload_finest_level", "upload_frames_u8",
+          "upload_sequence_u8", "upload_sequence_bidir_u8")
 
 # a batch of more than 16 frames (4 lanes per patch, no dependent launch, the other SOR plans): BATCH_DISTINCT pairs
 # cycled over BATCH_FRAMES slots, padding 2P
@@ -249,15 +255,61 @@ def _levels(prm, pyr):
             yield lv, which, arr
 
 
-def _check_slots(ctx, prm, pyrs, exp, path, f0=0):
-    """every level and array of slots f0.. == their pyramids; after a run, every flow == exp (None: not checked)"""
+def swapped(pyr):
+    """the pyramids of the swapped pair: what a usefbcon context holds in the backward frame of a pair"""
+    return types.SimpleNamespace(i0=pyr.i1, i0x=pyr.i1x, i0y=pyr.i1y, i1=pyr.i0, i1x=pyr.i0x, i1y=pyr.i0y)
+
+
+def _check_slots(ctx, prm, pyrs, exp, path, f0=0, backward=False):
+    """every level and array of slots f0.. == their pyramids, with `backward` (usefbcon) also every array of their
+    backward frames == the swapped pair's; after a run, every flow == exp (None: not checked; exp None: no run)"""
     for f, p in enumerate(pyrs):
         for lv, which, arr in _levels(prm, p):
             assert_bits(ctx.get_level(f0 + f, lv, which), arr, "%s: slot %d level %d array %d" % (path, f0 + f, lv, which))
+    if backward:
+        from of_dis_b200 import api
+
+        set_direction(api, ctx, 1)
+        try:
+            for f, p in enumerate(pyrs):
+                for lv, which, arr in _levels(prm, swapped(p)):
+                    assert_bits(ctx.get_level(f0 + f, lv, which), arr,
+                                "%s: backward frame of slot %d level %d array %d" % (path, f0 + f, lv, which))
+        finally:
+            set_direction(api, ctx, -1)
+    if exp is None:
+        return
     ctx.run(ctx.max_frames)
     for f, e in enumerate(exp):
         if e is not None:
             assert_bits(ctx.get_flow(f0 + f, prm.sc_l), e, "%s: flow of slot %d" % (path, f0 + f))
+
+
+def upload_by_route(ctx, route, f0, pyrs, frames=None):
+    """Uploads pairs t < len(pyrs) into slots f0 + t by `route` (one of ROUTES); pyrs[t]: the pair's pyramids at the
+    context's padding, frames: the 8-bit clip whose frames t, t + 1 are pair t (the 8-bit routes only).
+    upload_sequence_bidir_u8 also uploads the swapped pairs into slots f0 + n + t."""
+    n, lv, pad = len(pyrs), ctx.prm.sc_l, ctx.pad
+    if route == "upload_pyramids":
+        for t, p in enumerate(pyrs):
+            ctx.upload_pyramids(f0 + t, p)
+    elif route == "upload_packed":
+        ctx.upload_packed(f0, f0 + n, np.stack([ctx.pack_frame(p) for p in pyrs]))
+    elif route == "upload_packed_images":
+        ctx.upload_packed_images(f0, f0 + n, np.ascontiguousarray(
+            np.stack([ctx.pack_frame(p)[:ctx.packed_images_frame_floats] for p in pyrs])))
+    elif route == "upload_finest_level":
+        ctx.upload_finest_level(f0, f0 + n, np.ascontiguousarray(
+            np.stack([np.stack([p.i0[lv][pad:-pad, pad:-pad], p.i1[lv][pad:-pad, pad:-pad]]) for p in pyrs])))
+    else:
+        h, w = frames.shape[1:3]
+        if route == "upload_frames_u8":
+            ctx.upload_frames_u8(f0, f0 + n, _frames_u8([(frames[t], frames[t + 1]) for t in range(n)]), w, h)
+        elif route == "upload_sequence_u8":
+            ctx.upload_sequence_u8(f0, f0 + n, np.ascontiguousarray(frames[:n + 1]), w, h)
+        else:
+            assert route == "upload_sequence_bidir_u8", route
+            ctx.upload_sequence_bidir_u8(f0, n, np.ascontiguousarray(frames[:n + 1]), w, h)
 
 
 @pytest.mark.parametrize("name", list(UPLOAD_CASES))
@@ -269,49 +321,21 @@ def test_every_upload_path_at_a_wider_padding(name, api, oracle_port):
 
     prm, pad, frames, fwd, bwd = upload_inputs(name)
     assert pad != prm.p_samp_s
-    n, l = UPLOAD_PAIRS, prm.sc_l
-    h, w = frames.shape[1:3]
+    n = UPLOAD_PAIRS
     exp = [oracle_port.port_run(p, prm) for p in fwd]
     # stereo: the backward slots run as the right camera (the oracle's level loop as the right camera, without usefbcon)
     exp_bwd = [oracle_port.port_run(p, prm) if prm.nop == 2 else
                (_right_camera_oracle(p, prm) if not prm.usefbcon else None) for p in bwd]
-    pairs = [(frames[t], frames[t + 1]) for t in range(n)]
-
-    def fresh(nfr=n):
-        return _context(api, prm, fwd[0], (), nfr)
-
-    ctx = fresh()
-    for f, p in enumerate(fwd):
-        ctx.upload_pyramids(f, p)
-    _check_slots(ctx, prm, fwd, exp, "upload_pyramids")
-    full = np.stack([ctx.pack_frame(p) for p in fwd])
-    ctx.close()
-    if not prm.usefbcon:
-        ctx = fresh()
-        ctx.upload_packed(0, n, full)
-        _check_slots(ctx, prm, fwd, exp, "upload_packed")
-        ctx.close()
-    ctx = fresh()
-    ctx.upload_packed_images(0, n, np.ascontiguousarray(full[:, :ctx.packed_images_frame_floats]))
-    _check_slots(ctx, prm, fwd, exp, "upload_packed_images")
-    ctx.close()
-    ctx = fresh()
-    ctx.upload_finest_level(0, n, np.ascontiguousarray(np.stack([np.stack([p.i0[l][pad:-pad, pad:-pad],
-                                                                           p.i1[l][pad:-pad, pad:-pad]]) for p in fwd])))
-    _check_slots(ctx, prm, fwd, exp, "upload_finest_level")
-    ctx.close()
-    ctx = fresh()
-    ctx.upload_frames_u8(0, n, _frames_u8(pairs), w, h)
-    _check_slots(ctx, prm, fwd, exp, "upload_frames_u8")
-    ctx.close()
-    ctx = fresh()
-    ctx.upload_sequence_u8(0, n, frames, w, h)
-    _check_slots(ctx, prm, fwd, exp, "upload_sequence_u8")
-    ctx.close()
-    ctx = fresh(2 * n)
-    ctx.upload_sequence_bidir_u8(0, n, frames, w, h)
-    _check_slots(ctx, prm, fwd + bwd, exp + exp_bwd, "upload_sequence_bidir_u8")
-    ctx.close()
+    for route in ROUTES:
+        if route == "upload_packed" and prm.usefbcon:
+            continue
+        bidir = route == "upload_sequence_bidir_u8"
+        ctx = _context(api, prm, fwd[0], (), 2 * n if bidir else n)
+        try:
+            upload_by_route(ctx, route, 0, fwd, frames)
+            _check_slots(ctx, prm, fwd + bwd if bidir else fwd, exp + exp_bwd if bidir else exp, route)
+        finally:
+            ctx.close()
 
 
 def test_batch_of_more_than_16_frames_at_twice_the_padding_eager_and_graph(api, oracle_port):
