@@ -627,6 +627,87 @@ int ofdis_egomotion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
                             unsigned char* mask, float* residual, float* object_motion,
                             int width_org, int height_org, int memkind);
 
+/* Volumetric fusion (extension): a truncated signed distance function (TSDF; Curless and Levoy, SIGGRAPH 1996;
+ * KinectFusion, Newcombe et al., ISMAR 2011) integrated from a clip's disparity maps and camera poses, its zero
+ * crossings as surface points and its depth rendered by ray casting.  The context owns one volume: T, W and, with
+ * colour, three bytes per voxel.  It persists across calls and across ofdis_run and the other extensions;
+ * ofdis_fuse_begin resets it and ofdis_destroy frees it.  It reads no flow: any context (flow or stereo) may own one.
+ * Float32 without contraction, with IEEE division and square root; the pose algebra on the host in float64;
+ * preprocess.fuse_integrate, fuse_extract and fuse_render restate it bit for bit.  qNaN = 0x7fc00000, known(d) =
+ * 0 <= d <= 1e9 (NaN fails, -0 passes), fb = fx * baseline rounded once, mu = trunc.
+ *   Volume.  Voxel (i, j, k), linear index (k*ny + j)*nx + i, sits at X = ox + (float)i * voxel, Y = oy + (float)j *
+ *   voxel, Z = oz + (float)k * voxel in the world: frame 0's camera, x right, y down, z forward.  Initially T = +0,
+ *   W = 0 and colour (0, 0, 0).
+ *   Push.  Frame k's pose P ([3][4] float64 row-major [R | t], camera-to-world, the convention of
+ *   preprocess.chain_poses and KITTI) gives the world-to-camera g ([3][4] float32): g_r0..g_r2 = R_0r, R_1r, R_2r and
+ *   g_r3 = -(((R_0r*t_0) + (R_1r*t_1)) + (R_2r*t_2)) in float64, each rounded to float32.  Per voxel, for k = 0 .. n-1
+ *   in order: Xc = ((g00*X + g01*Y) + g02*Z) + g03 (Yc with row 1, Zc with row 2); skip unless Zc > 0.
+ *   u = (fx*Xc)/Zc + cx, v = (fy*Yc)/Zc + cy; skip unless u + 0.5f and v + 0.5f lie in [0, W) and [0, H) (NaN fails);
+ *   px = (int)floorf(u + 0.5f), py likewise.  d = D_k(px, py); skip unless known(d) and s = d + doffs > 0.  z = fb / s;
+ *   skip when z > max_depth.  sdf = z - Zc; skip when sdf < -mu.  f = fminf(1.0f, sdf / mu); W' = W + 1.0f;
+ *   T = (T*W + f) / W'; with colour, per channel c = (unsigned char)floorf(((float)c*W + (float)obs) / W' + 0.5f)
+ *   with the W before the update and obs frame k's byte at (px, py) (gray replicated); then W = fminf(W', max_weight).
+ *   A push of n frames gives exactly the volume of n pushes of one frame each.
+ *   Extract.  For voxel a and axis e (x, y, z), in ascending voxel index and then axis order, with b = a + e inside
+ *   the volume: a crossing when W_a >= min_weight, W_b >= min_weight, fabsf(T_a) < 1, fabsf(T_b) < 1 and
+ *   (T_a > 0) != (T_b > 0).  Its point is a's (X, Y, Z) with the e component plus t * voxel, t = T_a / (T_a - T_b);
+ *   its normal the gradient G = (T(i+1, j, k) - T(i-1, j, k), T(i, j+1, k) - T(i, j-1, k), T(i, j, k+1) - T(i, j, k-1))
+ *   at a with indices clamped to the volume, divided per component by L = sqrtf((Gx*Gx + Gy*Gy) + Gz*Gz) when L > 0,
+ *   else (qNaN, qNaN, qNaN); its colour a's when t < 0.5f, else b's ((0, 0, 0) without colour); pad 0.
+ *   Render.  For pose k (rounded to float32 row-major, p) and pixel (x, y): the ray r = (((float)x - cx)/fx,
+ *   ((float)y - cy)/fy, 1); samples s = 0 .. 65536 with Z_s = z_near + (float)s*step while Z_s <= z_far; the sample's
+ *   world point Pw_r = ((p_r0*(r0*Z_s) + p_r1*(r1*Z_s)) + p_r2*Z_s) + p_r3 and voxel coordinates q = (Pw - origin) /
+ *   voxel per component.  fl = floorf(q) must satisfy 0 <= fl <= (float)(n - 2) on each axis (n = nx, ny, nz), i0 =
+ *   (int)fl, fr = q - fl; the sample is known when all 8 corners have W >= min_weight, and its T is trilinear, x first,
+ *   then y, then z, each step a*(1.0f - fr) + b*fr.  At the first s with samples s and s+1 both known and T_s > 0 >=
+ *   T_s+1: depth = Z_s + step * (T_s / (T_s - T_s+1)); none: qNaN.  The step is fixed: no adaptive skipping. */
+typedef struct ofdis_fuse_params {
+  int nx, ny, nz;       /* each >= 1, nx * ny * nz <= 2^30 */
+  float origin[3];      /* world position of voxel (0, 0, 0), metres; finite */
+  float voxel;          /* voxel size, metres; finite, > 0 */
+  float trunc;          /* truncation distance mu, metres; finite, > 0 */
+  float max_weight;     /* finite, >= 1 */
+  int color;            /* 0 | 1: keep three colour bytes per voxel */
+} ofdis_fuse_params;
+typedef struct ofdis_fuse_point {
+  float x, y, z;        /* the zero crossing, world metres */
+  float nx, ny, nz;     /* unit normal (towards T > 0, free space), qNaN where the gradient is 0 */
+  unsigned char r, g, b, pad;
+} ofdis_fuse_point;     /* 28 bytes */
+/* Resets the volume: every voxel to T = +0, W = 0, colour 0.  The volume -- 8 bytes per voxel, 11 with colour -- is
+ * allocated here, grows, never shrinks and is freed by ofdis_destroy.  A NULL or out-of-range p is OFDIS_ERR_ARG and
+ * leaves a live volume as it was.  One memset per array, no kernel. */
+int ofdis_fuse_begin(ofdis_ctx* ctx, const ofdis_fuse_params* p);
+/* Integrates frames k = 0 .. n-1 in order: disp + k*disp_stride ([H][W] positive disparities, NaN unknown, the maps of
+ * ofdis_scene_flow_fullres), poses [n][12] float64 on the host, and with colour frames + k*frame_stride ([H][W][noc]
+ * bytes, noc the context's channels; NULL without colour).  W = width_org, H = height_org; max_depth > 0 (+inf
+ * allowed).  disp and frames in memkind: host inputs go through the context's staging buffer.  One kernel plus the copy
+ * of the n float32 world-to-camera poses, whatever n.  OFDIS_ERR_ARG, with the volume unchanged: no live volume, NULL
+ * disp or poses, a NULL frames with colour, a NULL or bad cam (as ofdis_scene_flow_fullres checks it), max_depth NaN or
+ * not > 0, disp_stride < W*H, frame_stride below one frame (with colour), n outside 1 .. max_frames + 1, a non-finite
+ * pose entry, or a device disp that is not 4-byte aligned; frame sizes as ofdis_get_flow_fullres checks them. */
+int ofdis_fuse_push(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* poses,
+                    const ofdis_stereo_camera* cam, float max_depth, const unsigned char* frames, size_t frame_stride,
+                    int width_org, int height_org, int memkind);
+/* The volume's zero crossings in order: *count (host) gets the total, pts ([capacity] in memkind) the first
+ * min(capacity, total); capacity 0 counts only (pts may then be NULL).  Three kernels (count, scan, write), then one
+ * synchronise.  Host output goes through the context's full-resolution scratch.  OFDIS_ERR_ARG: no live volume, NULL
+ * count, capacity < 0, NULL pts with capacity > 0, min_weight NaN, or a device pts that is not 4-byte aligned. */
+int ofdis_fuse_extract(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, long capacity, long* count,
+                       int memkind);
+/* Ray-cast depth [n][H][W] float32 (memkind) for n poses ([n][12] float64 camera-to-world, host).  One kernel;
+ * host output goes through the full-resolution scratch and synchronises the stream.  OFDIS_ERR_ARG: no live volume,
+ * NULL poses or depth, a NULL or bad cam, z_near or step not finite and > 0, z_far not finite or below z_near,
+ * (z_far - z_near) / step > 65536 (float32), min_weight NaN, n outside 1 .. max_frames + 1, a non-finite pose entry, or
+ * a device depth that is not 4-byte aligned; frame sizes as ofdis_get_flow_fullres checks them. */
+int ofdis_fuse_render(ofdis_ctx* ctx, int n, const double* poses, const ofdis_stereo_camera* cam, float z_near,
+                      float z_far, float step, float min_weight, float* depth, int width_org, int height_org,
+                      int memkind);
+/* Copies the volume out in memkind: T and W [nz][ny][nx] float32 and color [nz][ny][nx][3] bytes, each may be NULL
+ * (color must be NULL for a volume without colour).  Synchronises the stream.  OFDIS_ERR_ARG: no live volume, a
+ * colour output without colour, or a device T or W that is not 4-byte aligned. */
+int ofdis_fuse_get_volume(ofdis_ctx* ctx, float* T, float* W, unsigned char* color, int memkind);
+
 /* Dense point trajectories (extension): the tracker of Sundaram, Brox and Keutzer ("Dense point trajectories by
  * GPU-accelerated large displacement optical flow", ECCV 2010) through consecutive pairs of bidirectional flows.
  * The context owns one tracker: the list of live tracks (sorted by id), the next id and the counters.  It persists

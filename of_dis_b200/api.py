@@ -14,7 +14,7 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import (DISP_FILTER_FIELDS, EGO_PARAM_FIELDS, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
+from .preprocess import (DISP_FILTER_FIELDS, EGO_PARAM_FIELDS, FUSE_PARAM_FIELDS, FUSE_POINT_DTYPE, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
                          STAB_FRAME_DTYPE, STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS,
                          TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
                          fisher_fit, fisher_pack, fisher_sizes, gaussian_weights, motion_params,
@@ -44,7 +44,8 @@ EXPORTS = [
     "ofdis_global_motion_fullres", "ofdis_stab_begin", "ofdis_stab_push", "ofdis_stab_finish",
     "ofdis_traj_begin", "ofdis_traj_advance", "ofdis_traj_stats_get", "ofdis_scene_flow_fullres",
     "ofdis_fisher_begin", "ofdis_fisher_push", "ofdis_fisher_take", "ofdis_traj_advance_fisher",
-    "ofdis_egomotion_fullres",
+    "ofdis_egomotion_fullres", "ofdis_fuse_begin", "ofdis_fuse_push", "ofdis_fuse_extract", "ofdis_fuse_render",
+    "ofdis_fuse_get_volume",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -125,6 +126,17 @@ class EgoParams(ctypes.Structure):
 
 
 assert tuple(k for k, _ in EgoParams._fields_) == EGO_PARAM_FIELDS
+
+
+class FuseParams(ctypes.Structure):
+    """ofdis_fuse_params (include/ofdis_b200.h)."""
+    _fields_ = [("nx", ctypes.c_int), ("ny", ctypes.c_int), ("nz", ctypes.c_int), ("origin", ctypes.c_float * 3),
+                ("voxel", ctypes.c_float), ("trunc", ctypes.c_float), ("max_weight", ctypes.c_float),
+                ("color", ctypes.c_int)]
+
+
+assert tuple(k for k, _ in FuseParams._fields_) == FUSE_PARAM_FIELDS
+assert FUSE_POINT_DTYPE.itemsize == 28
 
 
 class StabParams(ctypes.Structure):
@@ -257,6 +269,15 @@ def lib():
         L.ofdis_fisher_take.argtypes = [ctypes.c_void_p] + [ctypes.c_void_p] * 3 + [ctypes.c_int]
         L.ofdis_traj_advance_fisher.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
             [ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3
+        L.ofdis_fuse_begin.argtypes = [ctypes.c_void_p, ctypes.POINTER(FuseParams)]
+        L.ofdis_fuse_push.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p,
+                                      ctypes.POINTER(StereoCamera), ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t] + \
+            [ctypes.c_int] * 3
+        L.ofdis_fuse_extract.argtypes = [ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_long,
+                                         ctypes.POINTER(ctypes.c_long), ctypes.c_int]
+        L.ofdis_fuse_render.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.POINTER(StereoCamera)] + \
+            [ctypes.c_float] * 4 + [ctypes.c_void_p] + [ctypes.c_int] * 3
+        L.ofdis_fuse_get_volume.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int]
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -1042,6 +1063,93 @@ class Context:
             return self.fisher_take(with_fv=False)[1]
 
         return fisher_fit(x, blocks, dims, K, iters, seed, var_floor, estep=estep)
+
+    def fuse_begin(self, params):
+        """Resets the context's fusion volume (ofdis_fuse_begin; preprocess.fuse_new_volume is its restatement).
+        params: a mapping with preprocess.FUSE_PARAM_FIELDS (origin three numbers) or a FuseParams."""
+        if not isinstance(params, FuseParams):
+            params = FuseParams(int(params["nx"]), int(params["ny"]), int(params["nz"]),
+                                (ctypes.c_float * 3)(*[float(v) for v in params["origin"]]), float(params["voxel"]),
+                                float(params["trunc"]), float(params["max_weight"]), int(params["color"]))
+        self._ck(lib().ofdis_fuse_begin(self._h, ctypes.byref(params)))
+        self._fuse = (params.nx, params.ny, params.nz, params.color)
+
+    @staticmethod
+    def _fuse_cam(camera):
+        return None if camera is None else ctypes.byref(StereoCamera(*[camera[k] for k in STEREO_CAMERA_FIELDS]))
+
+    @staticmethod
+    def _fuse_poses(poses):
+        poses = np.ascontiguousarray(poses, np.float64)
+        if poses.size % 12:
+            raise ValueError("fuse: poses must be (n, 3, 4) float64")
+        return poses.reshape(-1, 12)
+
+    def fuse_push(self, disp, poses, camera, *, width_org, height_org, max_depth=float("inf"), frames=None,
+                  disp_stride=None, frame_stride=None, memkind=MEM_HOST):
+        """Integrates n frames into the volume (ofdis_fuse_push; preprocess.fuse_integrate restates it): disp (n, H, W)
+        positive disparities (NaN unknown), poses (n, 3, 4) camera-to-world float64 on the host, camera a mapping
+        with STEREO_CAMERA_FIELDS and, when the volume keeps colour, frames (n, H, W[, noc]) uint8.  Host arrays'
+        frames must be C-contiguous and equally spaced; with memkind=MEM_DEVICE disp and frames are device addresses
+        the caller owns and the strides count floats and bytes between frames (default one frame)."""
+        poses = self._fuse_poses(poses)
+        n = poses.shape[0]
+        pix = width_org * height_org
+        if memkind == MEM_HOST:
+            ok = isinstance(disp, np.ndarray) and disp.dtype == np.float32 and disp.shape == (n, height_org, width_org) \
+                and (n == 0 or disp[0].flags["C_CONTIGUOUS"]) and disp.strides[0] % 4 == 0
+            if not ok:
+                raise ValueError("fuse_push: disp must be a float32 array of shape %s whose frames are C-contiguous"
+                                 % ((n, height_org, width_org),))
+            disp_stride = disp.strides[0] // 4 if n > 1 else pix
+            if frames is not None:
+                frame_stride = self._frames_u8("fuse_push: frames", frames, n, width_org, height_org)
+                frames = frames.ctypes.data
+        else:
+            disp_stride = pix if disp_stride is None else disp_stride
+            frame_stride = pix * self.prm.noc if frame_stride is None else frame_stride
+        self._ck(lib().ofdis_fuse_push(self._h, n, _ptr(disp), disp_stride, _ptr(poses), self._fuse_cam(camera),
+                                       max_depth, _ptr(frames), frame_stride or 0, width_org, height_org, memkind))
+
+    def fuse_extract(self, min_weight=1.0, capacity=None, memkind=MEM_HOST, out=None):
+        """The volume's zero crossings (ofdis_fuse_extract; preprocess.fuse_extract restates it).  Host: returns
+        (points of FUSE_POINT_DTYPE, total); capacity None counts first and takes them all, else at most capacity.
+        With memkind=MEM_DEVICE out is a device address of capacity records the caller owns; returns (out, total)."""
+        total = ctypes.c_long(0)
+        if memkind != MEM_HOST:
+            self._ck(lib().ofdis_fuse_extract(self._h, min_weight, _ptr(out), capacity or 0, ctypes.byref(total),
+                                              memkind))
+            return out, total.value
+        if capacity is None:
+            self._ck(lib().ofdis_fuse_extract(self._h, min_weight, None, 0, ctypes.byref(total), memkind))
+            capacity = total.value
+        pts = np.zeros(capacity, FUSE_POINT_DTYPE)
+        self._ck(lib().ofdis_fuse_extract(self._h, min_weight, _ptr(pts) if capacity else None, capacity,
+                                          ctypes.byref(total), memkind))
+        return pts[:min(capacity, total.value)], total.value
+
+    def fuse_render(self, poses, camera, *, z_near, z_far, step, width_org, height_org, min_weight=1.0,
+                    memkind=MEM_HOST, out=None):
+        """Ray-cast depth of the volume from n camera-to-world poses (ofdis_fuse_render; preprocess.fuse_render
+        restates it): host (n, height_org, width_org) float32, qNaN where no ray meets the surface; with
+        memkind=MEM_DEVICE out is a device address the caller owns and is returned as given."""
+        poses = self._fuse_poses(poses)
+        n = poses.shape[0]
+        if memkind == MEM_HOST:
+            out = np.empty((n, height_org, width_org), np.float32)
+        self._ck(lib().ofdis_fuse_render(self._h, n, _ptr(poses), self._fuse_cam(camera), z_near, z_far, step,
+                                         min_weight, _ptr(out), width_org, height_org, memkind))
+        return out
+
+    def fuse_volume(self, memkind=MEM_HOST, T=None, W=None, color=None):
+        """The volume (ofdis_fuse_get_volume): host returns {"T", "W", "C"} as preprocess.fuse_new_volume lays them
+        out (C None without colour); with memkind=MEM_DEVICE T, W and color are device addresses (or None)."""
+        if memkind == MEM_HOST:
+            nx, ny, nz, col = getattr(self, "_fuse", (0, 0, 0, 0))
+            T, W = np.empty((nz, ny, nx), np.float32), np.empty((nz, ny, nx), np.float32)
+            color = np.empty((nz, ny, nx, 3), np.uint8) if col else None
+        self._ck(lib().ofdis_fuse_get_volume(self._h, _ptr(T), _ptr(W), _ptr(color), memkind))
+        return {"T": T, "W": W, "C": color}
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

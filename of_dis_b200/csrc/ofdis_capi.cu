@@ -128,6 +128,15 @@ struct ofdis_ctx {
   FisherGeom fgeom{};
   long long fisher_pushed = 0;
   bool fisher_on = false;
+  // the volume of ofdis_fuse_begin / ofdis_fuse_push / ofdis_fuse_extract / ofdis_fuse_render: T, W, the colour bytes,
+  // then FuseWork's poses and scan blocks; the geometry of the last begin; grows, never shrinks; never touched by
+  // ofdis_run
+  void* d_fuse = nullptr;
+  size_t fuse_bytes = 0;
+  FuseGeom fuse_geom{};
+  FuseVolume fuse_vol{};
+  FuseWork fuse_ws{};
+  bool fuse_on = false;
   std::vector<float*> d_flow;   // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -502,6 +511,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_traj);
   cudaFree(ctx->d_stab);
   cudaFree(ctx->d_fisher);
+  cudaFree(ctx->d_fuse);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -1438,6 +1448,218 @@ int ofdis_egomotion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
     std::memcpy(pose + 12 * (size_t)q, res[q].pose, sizeof(res[q].pose));
     stats[q] = res[q].st;
   }
+  return OFDIS_OK;
+}
+
+static bool fuse_cam_ok(const ofdis_stereo_camera* cam) {
+  return cam && finite_gt0(cam->fx) && finite_gt0(cam->fy) && finite_gt0(cam->baseline) && finite_f32(cam->cx) &&
+         finite_f32(cam->cy) && finite_f32(cam->doffs);
+}
+
+// n poses [n][12] float64 (camera-to-world) into ctx->fuse_ws.g as float32: world-to-camera (invert) or as given
+static int fuse_poses(ofdis_ctx* ctx, int n, const double* P, bool invert) {
+  std::vector<float> g((size_t)12 * n);
+  for (int k = 0; k < n; ++k) {
+    const double* p = P + (size_t)12 * k;
+    float* q = g.data() + (size_t)12 * k;
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 4; ++c) {
+        if (!(std::fabs(p[4 * r + c]) <= DBL_MAX)) return fail(ctx, OFDIS_ERR_ARG, "fuse: a pose entry is not finite");
+        if (!invert) q[4 * r + c] = (float)p[4 * r + c];
+      }
+      if (invert) {
+        for (int c = 0; c < 3; ++c) q[4 * r + c] = (float)p[4 * c + r];
+        q[4 * r + 3] = (float)(-(((p[r] * p[3]) + (p[4 + r] * p[7])) + (p[8 + r] * p[11])));
+      }
+    }
+  }
+  CK(cudaMemcpyAsync(ctx->fuse_ws.g, g.data(), sizeof(float) * g.size(), cudaMemcpyHostToDevice, ctx->stream));
+  // g is pageable host memory: the copy has left it when cudaMemcpyAsync returns
+  return OFDIS_OK;
+}
+
+int ofdis_fuse_begin(ofdis_ctx* ctx, const ofdis_fuse_params* p) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!p || p->nx < 1 || p->ny < 1 || p->nz < 1 || (long long)p->nx * p->ny * p->nz > (1ll << 30) ||
+      !finite_f32(p->origin[0]) || !finite_f32(p->origin[1]) || !finite_f32(p->origin[2]) || !finite_gt0(p->voxel) ||
+      !finite_gt0(p->trunc) || !(p->max_weight >= 1.0f && p->max_weight <= FLT_MAX) || (p->color != 0 && p->color != 1))
+    return fail(ctx, OFDIS_ERR_ARG, "fuse_begin: bad argument");
+  NvtxRange nvtx("fuse", -1);
+  CK(cudaSetDevice(ctx->device));
+  const size_t N = (size_t)p->nx * p->ny * p->nz, nb = (N + FUSE_BLOCK - 1) / FUSE_BLOCK;
+  const size_t b_t = align16(4 * N), b_c = p->color ? align16(3 * N) : 0;
+  const size_t b_g = align16(sizeof(float) * 12 * (size_t)(ctx->max_frames + 1)), b_s = 8 * (nb + 1);
+  const size_t bytes = 2 * b_t + b_c + b_g + b_s;
+  if (bytes > ctx->fuse_bytes) {
+    ctx->fuse_on = false;
+    CK(cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_fuse);
+    ctx->d_fuse = nullptr;
+    ctx->fuse_bytes = 0;
+    if (cudaMalloc(&ctx->d_fuse, bytes) != cudaSuccess) {
+      ctx->d_fuse = nullptr;
+      return fail(ctx, OFDIS_ERR_NOMEM, "fuse volume");
+    }
+    ctx->fuse_bytes = bytes;
+  }
+  char* b = static_cast<char*>(ctx->d_fuse);
+  FuseVolume& v = ctx->fuse_vol;
+  v.T = reinterpret_cast<float*>(b);
+  v.W = reinterpret_cast<float*>(b + b_t);
+  v.C = p->color ? reinterpret_cast<unsigned char*>(b + 2 * b_t) : nullptr;
+  ctx->fuse_ws.g = reinterpret_cast<float*>(b + 2 * b_t + b_c);
+  ctx->fuse_ws.bsum = reinterpret_cast<unsigned long long*>(b + 2 * b_t + b_c + b_g);
+  ctx->fuse_ws.total = ctx->fuse_ws.bsum + nb;
+  FuseGeom& g = ctx->fuse_geom;
+  g.count = (long long)N;
+  g.nx = p->nx, g.ny = p->ny, g.nz = p->nz;
+  g.ox = p->origin[0], g.oy = p->origin[1], g.oz = p->origin[2];
+  g.voxel = p->voxel, g.mu = p->trunc, g.max_weight = p->max_weight;
+  CK(cudaMemsetAsync(v.T, 0, 4 * N, ctx->stream));
+  CK(cudaMemsetAsync(v.W, 0, 4 * N, ctx->stream));
+  if (v.C) CK(cudaMemsetAsync(v.C, 0, 3 * N, ctx->stream));
+  ctx->fuse_on = true;
+  return OFDIS_OK;
+}
+
+int ofdis_fuse_push(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* poses,
+                    const ofdis_stereo_camera* cam, float max_depth, const unsigned char* frames, size_t frame_stride,
+                    int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_push: no live volume (ofdis_fuse_begin)");
+  const bool dev = memkind == OFDIS_MEM_DEVICE, color = ctx->fuse_vol.C != nullptr;
+  const size_t pix = (size_t)std::max(width_org, 0) * std::max(height_org, 0), hwc = pix * ctx->prm.noc;
+  if (n < 1 || n > ctx->max_frames + 1 || !disp || !poses || (color && !frames) || !fuse_cam_ok(cam) ||
+      !(max_depth > 0.0f) || disp_stride < pix || (color && frame_stride < hwc) ||
+      (dev && reinterpret_cast<uintptr_t>(disp) % sizeof(float)))
+    return fail(ctx, OFDIS_ERR_ARG, "fuse_push: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("fuse", -1);
+  CK(cudaSetDevice(ctx->device));
+  FusePush fp{};
+  fp.disp = disp, fp.disp_stride = disp_stride;
+  fp.frames = color ? frames : nullptr, fp.frame_stride = frame_stride;
+  fp.n = n, fp.w = width_org, fp.h = height_org, fp.noc = ctx->prm.noc, fp.max_depth = max_depth;
+  fp.cam = DispCamera{cam->fx * cam->baseline, cam->fx, cam->fy, cam->cx, cam->cy, cam->doffs};
+  fp.g = ctx->fuse_ws.g;
+  rc = fuse_poses(ctx, n, poses, true);
+  if (rc) return rc;
+  if (!dev) {
+    // the staging buffer: the disparity maps, then the frames, packed; sized for max_frames + 1 of each
+    const size_t b_d = align16(sizeof(float) * pix * (size_t)(ctx->max_frames + 1));
+    rc = ensure_stage(ctx, b_d + (color ? hwc * (size_t)(ctx->max_frames + 1) : 0));
+    if (rc) return rc;
+    char* st = static_cast<char*>(ctx->d_stage);
+    CK(cudaMemcpy2DAsync(st, sizeof(float) * pix, disp, sizeof(float) * disp_stride, sizeof(float) * pix, n,
+                         cudaMemcpyHostToDevice, ctx->stream));
+    fp.disp = reinterpret_cast<const float*>(st), fp.disp_stride = pix;
+    if (color) {
+      CK(cudaMemcpy2DAsync(st + b_d, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+      fp.frames = reinterpret_cast<const unsigned char*>(st + b_d), fp.frame_stride = hwc;
+    }
+  }
+  const int k = launch_fuse_push(ctx->fuse_geom, ctx->fuse_vol, fp, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_integrate_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  return OFDIS_OK;
+}
+
+int ofdis_fuse_extract(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, long capacity, long* count,
+                       int memkind) {
+  static_assert(sizeof(ofdis_fuse_point) == 28, "ofdis_fuse_point: 28 bytes, as preprocess.FUSE_POINT_DTYPE");
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_extract: no live volume (ofdis_fuse_begin)");
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  if (!count || capacity < 0 || (capacity > 0 && !pts) || std::isnan(min_weight) ||
+      (dev && reinterpret_cast<uintptr_t>(pts) % sizeof(float)))
+    return fail(ctx, OFDIS_ERR_ARG, "fuse_extract: bad argument");
+  NvtxRange nvtx("fuse", -1);
+  CK(cudaSetDevice(ctx->device));
+  int k = launch_fuse_count(ctx->fuse_geom, ctx->fuse_vol, min_weight, ctx->fuse_ws, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_count_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  unsigned long long total = 0;
+  ofdis_fuse_point* out = pts;
+  long long cap = capacity;
+  if (!dev) {
+    // the total decides how much of the full-resolution scratch the host output needs
+    CK(cudaMemcpyAsync(&total, ctx->fuse_ws.total, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    cap = (long long)std::min<unsigned long long>(total, (unsigned long long)capacity);
+    if (cap > 0) {
+      const int rc = ensure_full(ctx, (size_t)cap * sizeof(ofdis_fuse_point) / sizeof(float));
+      if (rc) return rc;
+    }
+    out = reinterpret_cast<ofdis_fuse_point*>(ctx->d_full);
+  }
+  k = launch_fuse_write(ctx->fuse_geom, ctx->fuse_vol, min_weight, ctx->fuse_ws, out, cap, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_write_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  if (!dev && cap > 0)
+    CK(cudaMemcpyAsync(pts, out, sizeof(ofdis_fuse_point) * (size_t)cap, cudaMemcpyDeviceToHost, ctx->stream));
+  if (dev) CK(cudaMemcpyAsync(&total, ctx->fuse_ws.total, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  *count = (long)total;
+  return OFDIS_OK;
+}
+
+int ofdis_fuse_render(ofdis_ctx* ctx, int n, const double* poses, const ofdis_stereo_camera* cam, float z_near,
+                      float z_far, float step, float min_weight, float* depth, int width_org, int height_org,
+                      int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_render: no live volume (ofdis_fuse_begin)");
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  if (n < 1 || n > ctx->max_frames + 1 || !poses || !depth || !fuse_cam_ok(cam) || !finite_gt0(z_near) ||
+      !finite_gt0(step) || !(z_far >= z_near && z_far <= FLT_MAX) || !((z_far - z_near) / step <= 65536.0f) ||
+      std::isnan(min_weight) || (dev && reinterpret_cast<uintptr_t>(depth) % sizeof(float)))
+    return fail(ctx, OFDIS_ERR_ARG, "fuse_render: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("fuse", -1);
+  CK(cudaSetDevice(ctx->device));
+  const size_t np = (size_t)width_org * height_org * n;
+  FuseRender fr{};
+  fr.depth = depth;
+  if (!dev) {
+    // the full-resolution scratch, sized for max_frames + 1 maps and at least what ofdis_get_flow_fullres asks for
+    const size_t pix = (size_t)width_org * height_org;
+    rc = ensure_full(ctx, std::max(pix * ctx->nop * (size_t)ctx->max_frames, pix * (size_t)(ctx->max_frames + 1)));
+    if (rc) return rc;
+    fr.depth = ctx->d_full;
+  }
+  rc = fuse_poses(ctx, n, poses, false);
+  if (rc) return rc;
+  fr.pose = ctx->fuse_ws.g;
+  fr.w = width_org, fr.h = height_org;
+  fr.z_near = z_near, fr.z_far = z_far, fr.step = step, fr.min_weight = min_weight;
+  fr.cam = DispCamera{cam->fx * cam->baseline, cam->fx, cam->fy, cam->cx, cam->cy, cam->doffs};
+  const int k = launch_fuse_render(ctx->fuse_geom, ctx->fuse_vol, fr, n, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_render_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  if (!dev) {
+    CK(cudaMemcpyAsync(depth, fr.depth, sizeof(float) * np, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  return OFDIS_OK;
+}
+
+int ofdis_fuse_get_volume(ofdis_ctx* ctx, float* T, float* W, unsigned char* color, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_get_volume: no live volume (ofdis_fuse_begin)");
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  const FuseVolume& v = ctx->fuse_vol;
+  if ((color && !v.C) || (dev && (reinterpret_cast<uintptr_t>(T) % 4 || reinterpret_cast<uintptr_t>(W) % 4)))
+    return fail(ctx, OFDIS_ERR_ARG, "fuse_get_volume: bad argument");
+  CK(cudaSetDevice(ctx->device));
+  const size_t N = (size_t)ctx->fuse_geom.count;
+  const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  if (T) CK(cudaMemcpyAsync(T, v.T, 4 * N, kind, ctx->stream));
+  if (W) CK(cudaMemcpyAsync(W, v.W, 4 * N, kind, ctx->stream));
+  if (color) CK(cudaMemcpyAsync(color, v.C, 3 * N, kind, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
   return OFDIS_OK;
 }
 

@@ -688,6 +688,18 @@ int main(int argc, char** argv) {
 // work: the stereo binaries, --warm-start, --odometry without --scene-flow or --camera, --gt-poses without
 // --odometry, a list that does not match the clips or a file with too few lines, and a DIR that cannot be written.
 // Every other output keeps its bytes.
+//
+// --fuse voxel,trunc,x0,y0,z0,nx,ny,nz (needs --odometry, whose poses place the disparities): one TSDF volume per clip
+// of --odometry (ofdis_fuse_begin / ofdis_fuse_push / ofdis_fuse_extract), nx x ny x nz voxels of `voxel` metres from
+// (x0, y0, z0) in the clip's first camera, truncation `trunc` metres, max_weight 64, max_depth +inf, with colour.  The
+// clip's first pair begins it; every pair pushes its image1 disparity (the first map of its DISPLIST line) with its
+// chained pose T_k of DIR/poses_<clip>.txt and image1's colours, and the clip's last pair also pushes image2's
+// disparity with T_n and image2's colours.  At the clip's end the zero crossings of weight >= 1 go to
+// DIR/fused_<clip %04d>.ply, a binary little-endian PLY of float x, y, z, nx, ny, nz and uchar red, green, blue, in
+// the volume's order (preprocess.fuse_extract, preprocess.write_fused_ply).  With verbosity > 0 every clip prints
+// `FUSE clip C frames F points P`.  Refused before any device work: --fuse without --odometry, the stereo binaries,
+// --warm-start and a spec that is not 8 numbers with voxel and trunc > 0, sizes >= 1 and at most 2^30 voxels.  Every
+// other output keeps its bytes.
 
 // Rigid poses as 12 doubles, row-major [R | t].  T <- T inv(P): the next camera-to-world pose of a clip (KITTI's
 // odometry convention) from the relative pose P, camera t to camera t+1.
@@ -1039,6 +1051,7 @@ int main(int argc, char** argv) {
             "       [--lr-check] [--speckle N R] [--fill] [--camera fx,fy,cx,cy,baseline,doffs]\n"
             "       [--global-motion similarity|affine|homography PATH [--stabilize RADIUS CROP DIR]]\n"
             "       [--scene-flow DISPLIST [--gt-scene-flow GTLIST]]\n"
+            "       [--odometry DIR [--gt-poses LIST] [--fuse voxel,trunc,x0,y0,z0,nx,ny,nz]]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -1078,7 +1091,10 @@ int main(int argc, char** argv) {
             "  --gt-scene-flow GTLIST: disp0, disp1 and flow ground truth per pair, SFEVAL lines; not with --warm-start\n"
             "  --odometry DIR (flow binaries, with --scene-flow and --camera): the rig's ego-motion of every pair to\n"
             "  DIR/odometry.txt, each clip's KITTI poses to DIR/poses_<clip>.txt, <stem>_objects.pgm and\n"
-            "  <stem>_objmotion.pfm; --gt-poses LIST: one KITTI poses file per clip, ODOEVAL lines; not with --warm-start\n",
+            "  <stem>_objmotion.pfm; --gt-poses LIST: one KITTI poses file per clip, ODOEVAL lines; not with --warm-start\n"
+            "  --fuse voxel,trunc,x0,y0,z0,nx,ny,nz (flow binaries, with --odometry): every clip's disparities fused\n"
+            "  into a TSDF volume of nx x ny x nz voxels from (x0, y0, z0), its surface points to DIR/fused_<clip>.ply;\n"
+            "  not with --warm-start\n",
             argv[0]);
     return 2;
   }
@@ -1101,6 +1117,7 @@ int main(int argc, char** argv) {
   const char* sf_gtlist = nullptr;  // --gt-scene-flow GTLIST
   const char* odo_dir = nullptr;     // --odometry DIR
   const char* odo_gtlist = nullptr;  // --gt-poses LIST
+  const char* fuse_arg = nullptr;    // --fuse voxel,trunc,x0,y0,z0,nx,ny,nz
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -1213,6 +1230,13 @@ int main(int argc, char** argv) {
       }
       odo_dir = argv[first_num + 1];
       first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--fuse")) {
+      if (argc < first_num + 2 || fuse_arg) {
+        fprintf(stderr, "error: --fuse takes voxel,trunc,x0,y0,z0,nx,ny,nz\n");
+        return 2;
+      }
+      fuse_arg = argv[first_num + 1];
+      first_num += 2;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt-poses")) {
       if (argc < first_num + 2 || odo_gtlist) {
         fprintf(stderr, "error: --gt-poses takes one list of KITTI poses files\n");
@@ -1274,6 +1298,48 @@ int main(int argc, char** argv) {
   if (odo_gtlist && !odo_dir) {
     fprintf(stderr, "error: --gt-poses evaluates the poses of --odometry; give --odometry too\n");
     return 2;
+  }
+  if (fuse_arg && SELECTMODE != 1) {
+    fprintf(stderr, "error: --fuse places disparities with the poses of --odometry; the stereo binaries take no --fuse\n");
+    return 2;
+  }
+  if (fuse_arg && warm) {
+    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --fuse\n");
+    return 2;
+  }
+  if (fuse_arg && !odo_dir) {
+    fprintf(stderr, "error: --fuse places disparities with the poses of --odometry; give --odometry too\n");
+    return 2;
+  }
+  ofdis_fuse_params fuse_p;
+  memset(&fuse_p, 0, sizeof(fuse_p));
+  if (fuse_arg) {
+    double v[8];
+    const char* q = fuse_arg;
+    bool ok = true;
+    for (int i = 0; i < 8 && ok; ++i) {
+      char* end = nullptr;
+      v[i] = strtod(q, &end);
+      ok = end != q && (i < 7 ? *end == ',' : *end == 0) && std::isfinite(v[i]);
+      q = end + (i < 7 ? 1 : 0);
+    }
+    for (int i = 5; i < 8 && ok; ++i) ok = v[i] >= 1.0 && v[i] <= (double)(1 << 30) && v[i] == std::floor(v[i]);
+    ok = ok && (float)v[0] > 0.0f && (float)v[1] > 0.0f && v[0] <= FLT_MAX && v[1] <= FLT_MAX &&
+         std::fabs(v[2]) <= FLT_MAX && std::fabs(v[3]) <= FLT_MAX && std::fabs(v[4]) <= FLT_MAX &&
+         v[5] * v[6] * v[7] <= (double)(1 << 30);
+    if (!ok) {
+      fprintf(stderr, "error: --fuse takes eight numbers voxel,trunc,x0,y0,z0,nx,ny,nz with voxel and trunc > 0, "
+                      "integer sizes >= 1 and at most 2^30 voxels, got %s\n", fuse_arg);
+      return 2;
+    }
+    fuse_p.voxel = (float)v[0];
+    fuse_p.trunc = (float)v[1];
+    for (int e = 0; e < 3; ++e) fuse_p.origin[e] = (float)v[2 + e];
+    fuse_p.nx = (int)v[5];
+    fuse_p.ny = (int)v[6];
+    fuse_p.nz = (int)v[7];
+    fuse_p.max_weight = 64.0f;
+    fuse_p.color = 1;
   }
   // --camera on a flow binary belongs to --scene-flow
   const bool disp_on = lr_check || disp_fill || speckle_arg[0] || (camera_arg && !sf_list);
@@ -1604,6 +1670,10 @@ int main(int argc, char** argv) {
   vector<ofdis_motion_stats> odo_stats;
   vector<uint8_t> odo_mask;
   vector<float> odo_om;
+  double fuse_T[12];              // --fuse: the chained pose of the clip's next image1
+  int fuse_frames = 0;            // frames pushed into the clip's volume
+  vector<double> fuse_poses;
+  vector<ofdis_fuse_point> fuse_pts;
   // --descriptors, --fisher: every pair's frames hold an N x N patch, checked before any device work
   for (size_t k = 0; k < jobs.size() && traj_stage; ++k) {
     int iw = 0, ih = 0;
@@ -2160,6 +2230,65 @@ int main(int argc, char** argv) {
           ++odo_eval;
           if (verbosity > 0) printf("ODOEVAL %d %d %.9g %.9g\n", c, fr, te, re);
         }
+      }
+      // --fuse: the runs of one clip within the batch; image1 of pair k at k * fs, its image2 one frame later
+      const size_t fs = seq ? hwc : 2 * hwc;
+      for (int k0 = 0, k1; k0 < n && rc == OFDIS_OK && fuse_arg; k0 = k1) {
+        const int c = odo_clip[j0 + k0];
+        for (k1 = k0 + 1; k1 < n && odo_clip[j0 + k1] == c;) ++k1;
+        if (odo_frame[j0 + k0] == 0) {
+          static const double kIdentity[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+          memcpy(fuse_T, kIdentity, sizeof(fuse_T));
+          fuse_frames = 0;
+          rc = ofdis_fuse_begin(ctx, &fuse_p);
+          if (rc != OFDIS_OK) break;
+        }
+        fuse_poses.resize((size_t)12 * (k1 - k0 + 1));
+        for (int k = k0; k < k1; ++k) {
+          memcpy(&fuse_poses[(size_t)12 * (k - k0)], fuse_T, sizeof(fuse_T));
+          chain_pose(fuse_T, odo_pose.data() + (size_t)12 * k);
+        }
+        memcpy(&fuse_poses[(size_t)12 * (k1 - k0)], fuse_T, sizeof(fuse_T));
+        rc = ofdis_fuse_push(ctx, k1 - k0, &sf_d0[k0 * pix], pix, fuse_poses.data(), &dcam, INFINITY,
+                             frames.data() + (size_t)k0 * fs, fs, w, h, OFDIS_MEM_HOST);
+        fuse_frames += k1 - k0;
+        if (rc != OFDIS_OK || (j0 + k1 < (int)jobs.size() && odo_clip[j0 + k1] == c)) continue;
+        // the clip ends with this run: its last image2, then the surface
+        rc = ofdis_fuse_push(ctx, 1, &sf_d1[(k1 - 1) * pix], pix, &fuse_poses[(size_t)12 * (k1 - k0)], &dcam, INFINITY,
+                             frames.data() + (size_t)(k1 - 1) * fs + hwc, fs, w, h, OFDIS_MEM_HOST);
+        ++fuse_frames;
+        long count = 0;
+        if (rc == OFDIS_OK) rc = ofdis_fuse_extract(ctx, 1.0f, nullptr, 0, &count, OFDIS_MEM_HOST);
+        if (rc != OFDIS_OK) break;
+        fuse_pts.resize(count);
+        rc = ofdis_fuse_extract(ctx, 1.0f, fuse_pts.data(), count, &count, OFDIS_MEM_HOST);
+        if (rc != OFDIS_OK) break;
+        char name[32];
+        snprintf(name, sizeof(name), "/fused_%04d.ply", c);
+        const string path = string(odo_dir) + name;
+        FILE* pf = fopen(path.c_str(), "wb");
+        bool wrote = pf != nullptr;
+        if (pf) {
+          fprintf(pf, "ply\nformat binary_little_endian 1.0\nelement vertex %ld\nproperty float x\nproperty float y\n"
+                      "property float z\nproperty float nx\nproperty float ny\nproperty float nz\nproperty uchar red\n"
+                      "property uchar green\nproperty uchar blue\nend_header\n", count);
+          vector<uint8_t> buf((size_t)27 * count);
+          for (long i = 0; i < count; ++i) {
+            const ofdis_fuse_point& q = fuse_pts[i];
+            memcpy(&buf[(size_t)27 * i], &q.x, 24);
+            // the decoder's BGR: channel 2 is red (gray: all three equal)
+            const uint8_t rgb[3] = {nochannels == 3 ? q.b : q.r, q.g, nochannels == 3 ? q.r : q.b};
+            memcpy(&buf[(size_t)27 * i + 24], rgb, 3);
+          }
+          wrote = fwrite(buf.data(), 1, buf.size(), pf) == buf.size();
+          wrote = fclose(pf) == 0 && wrote;
+        }
+        if (!wrote) {
+          fprintf(stderr, "error: cannot write %s\n", path.c_str());
+          ofdis_destroy(ctx);
+          return 1;
+        }
+        if (verbosity > 0) printf("FUSE clip %d frames %d points %ld\n", c, fuse_frames, count);
       }
     }
     if (rc != OFDIS_OK) {

@@ -1734,6 +1734,197 @@ def pose_errors(rel, gt_abs):
     return np.array(t_err), np.array(r_err)
 
 
+# ---- volumetric fusion (ofdis_fuse_begin / ofdis_fuse_push / ofdis_fuse_extract / ofdis_fuse_render) ----------------
+FUSE_PARAM_FIELDS = ("nx", "ny", "nz", "origin", "voxel", "trunc", "max_weight", "color")
+# ofdis_fuse_point, field for field (28 bytes)
+FUSE_POINT_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4"),
+                             ("r", "u1"), ("g", "u1"), ("b", "u1"), ("pad", "u1")])
+FUSE_MAX_SAMPLES = 65536
+f32 = np.float32
+
+
+def fuse_new_volume(params) -> dict:
+    """The volume of ofdis_fuse_begin: T and W float32 (nz, ny, nx) of +0 and, with colour, C uint8 (nz, ny, nx, 3)."""
+    shape = (int(params["nz"]), int(params["ny"]), int(params["nx"]))
+    return {"T": np.zeros(shape, f32), "W": np.zeros(shape, f32),
+            "C": np.zeros(shape + (3,), np.uint8) if params["color"] else None}
+
+
+def fuse_world_to_camera(P) -> np.ndarray:
+    """g of ofdis_fuse_push: [R^T | -R^T t] of a camera-to-world pose, formed in float64 and rounded to float32 (12,)."""
+    p = np.asarray(P, np.float64).reshape(12)
+    g = np.empty(12, np.float64)
+    for r in range(3):
+        g[4 * r:4 * r + 3] = p[r], p[4 + r], p[8 + r]
+        g[4 * r + 3] = -(((p[r] * p[3]) + (p[4 + r] * p[7])) + (p[8 + r] * p[11]))
+    return g.astype(f32)
+
+
+def _fuse_axes(params):
+    o = [f32(v) for v in params["origin"]]
+    vox = f32(params["voxel"])
+    return [o[e] + np.arange(int(params[k]), dtype=np.float64).astype(f32) * vox
+            for e, k in enumerate(("nx", "ny", "nz"))]
+
+
+def fuse_integrate(vol: dict, params, disp, poses, camera, max_depth=np.inf, frames=None) -> dict:
+    """Restates ofdis_fuse_push on vol (fuse_new_volume's dict), in place: disp (n, H, W) float32 positive disparities
+    (NaN unknown), poses (n, 3, 4) camera-to-world float64, frames (n, H, W[, 3]) uint8 when the volume keeps colour."""
+    disp = np.asarray(disp, f32).reshape((-1,) + np.shape(disp)[-2:])
+    n, H, W = disp.shape
+    poses = np.asarray(poses, np.float64).reshape(n, 12)
+    cam = {k: f32(camera[k]) for k in STEREO_CAMERA_FIELDS}
+    fb = f32(cam["fx"] * cam["baseline"])
+    mu, maxw, maxd = f32(params["trunc"]), f32(params["max_weight"]), f32(max_depth)
+    xa, ya, za = _fuse_axes(params)
+    Z, Y, X = np.meshgrid(za, ya, xa, indexing="ij")
+    T, Wt, C = vol["T"], vol["W"], vol["C"]
+    one, half = f32(1), f32(0.5)
+    for k in range(n):
+        q = fuse_world_to_camera(poses[k])
+        with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+            Zc = ((q[8] * X + q[9] * Y) + q[10] * Z) + q[11]
+            Xc = ((q[0] * X + q[1] * Y) + q[2] * Z) + q[3]
+            Yc = ((q[4] * X + q[5] * Y) + q[6] * Z) + q[7]
+            ok = Zc > 0
+            Zs = np.where(ok, Zc, one)
+            uu = ((cam["fx"] * Xc) / Zs + cam["cx"]) + half
+            vv = ((cam["fy"] * Yc) / Zs + cam["cy"]) + half
+            ok &= (uu >= 0) & (uu < f32(W)) & (vv >= 0) & (vv < f32(H))
+            px = np.where(ok, np.floor(np.where(ok, uu, 0)), 0).astype(np.int64)
+            py = np.where(ok, np.floor(np.where(ok, vv, 0)), 0).astype(np.int64)
+            d = disp[k][py, px]
+            s = d + cam["doffs"]
+            ok &= (d >= 0) & (d <= f32(1e9)) & (s > 0)
+            z = fb / np.where(ok, s, one)
+            ok &= ~(z > maxd)
+            sdf = z - Zc
+            ok &= ~(sdf < -mu)
+            f = np.minimum(one, sdf / mu)
+        W1 = Wt + one
+        Tn = (T * Wt + f) / W1
+        if C is not None:
+            fr = np.asarray(frames[k], np.uint8).reshape(H, W, -1)
+            obs = fr[py, px] if fr.shape[-1] == 3 else np.repeat(fr[py, px], 3, -1)
+            cn = np.floor((C.astype(f32) * Wt[..., None] + obs.astype(f32)) / W1[..., None] + half)
+            C[ok] = cn[ok].astype(np.uint8)
+        T[ok] = Tn[ok]
+        Wt[ok] = np.minimum(W1, maxw)[ok]
+    return vol
+
+
+def fuse_extract(vol: dict, params, min_weight) -> np.ndarray:
+    """Restates ofdis_fuse_extract: every zero crossing of vol as a FUSE_POINT_DTYPE array, in the header's order."""
+    T, Wt, C = vol["T"], vol["W"], vol["C"]
+    nz, ny, nx = T.shape
+    mw = f32(min_weight)
+    good = (Wt >= mw) & (np.abs(T) < f32(1))
+    pos = T > 0
+    parts = []
+    for e, ax in ((0, 2), (1, 1), (2, 0)):
+        m = np.zeros(T.shape, bool)
+        a = [slice(None)] * 3
+        b = [slice(None)] * 3
+        a[ax], b[ax] = slice(0, -1), slice(1, None)
+        m[tuple(a)] = good[tuple(a)] & good[tuple(b)] & (pos[tuple(a)] != pos[tuple(b)])
+        parts.append(np.flatnonzero(m) * 3 + e)
+    idx = np.sort(np.concatenate(parts))
+    a, e = idx // 3, idx % 3
+    i, j, k = a % nx, (a // nx) % ny, a // (nx * ny)
+    step = np.array([1, nx, nx * ny])[e]
+    Tf = T.ravel()
+    Ta, Tb = Tf[a], Tf[a + step]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        t = Ta / (Ta - Tb)
+        gx = T[k, j, np.minimum(i + 1, nx - 1)] - T[k, j, np.maximum(i - 1, 0)]
+        gy = T[k, np.minimum(j + 1, ny - 1), i] - T[k, np.maximum(j - 1, 0), i]
+        gz = T[np.minimum(k + 1, nz - 1), j, i] - T[np.maximum(k - 1, 0), j, i]
+        L = np.sqrt((gx * gx + gy * gy) + gz * gz)
+        nrm = [np.where(L > 0, g / np.where(L > 0, L, f32(1)), _QNAN).astype(f32) for g in (gx, gy, gz)]
+    xa, ya, za = _fuse_axes(params)
+    P = [xa[i], ya[j], za[k]]
+    dt = t * f32(params["voxel"])
+    out = np.zeros(len(idx), FUSE_POINT_DTYPE)
+    for c, name in enumerate(("x", "y", "z")):
+        out[name] = np.where(e == c, P[c] + dt, P[c])
+    for c, name in enumerate(("nx", "ny", "nz")):
+        out[name] = nrm[c]
+    if C is not None:
+        src = np.where(t < f32(0.5), a, a + step)
+        Cf = C.reshape(-1, 3)
+        out["r"], out["g"], out["b"] = Cf[src, 0], Cf[src, 1], Cf[src, 2]
+    return out
+
+
+def fuse_render(vol: dict, params, poses, camera, z_near, z_far, step, min_weight, width: int, height: int):
+    """Restates ofdis_fuse_render: depth (n, height, width) float32, qNaN where no ray crosses the surface."""
+    poses = np.asarray(poses, np.float64).reshape(-1, 12)
+    n = poses.shape[0]
+    cam = {k: f32(camera[k]) for k in STEREO_CAMERA_FIELDS}
+    T, Wt = vol["T"].ravel(), vol["W"].ravel()
+    nz, ny, nx = vol["T"].shape
+    o = [f32(v) for v in params["origin"]]
+    vox, mw = f32(params["voxel"]), f32(min_weight)
+    zn, zf, st = f32(z_near), f32(z_far), f32(step)
+    y, x = np.mgrid[0:height, 0:width]
+    r0 = (x.astype(f32) - cam["cx"]) / cam["fx"]
+    r1 = (y.astype(f32) - cam["cy"]) / cam["fy"]
+    p = poses.astype(f32)[:, :, None, None]
+    depth = np.full((n, height, width), _QNAN, f32)
+    done = np.zeros((n, height, width), bool)
+    prev = np.zeros((n, height, width), bool)
+    Tp = np.zeros((n, height, width), f32)
+    Zp, one = f32(0), f32(1)
+    for s in range(FUSE_MAX_SAMPLES + 1):
+        Zs = zn + f32(s) * st
+        if not Zs <= zf or done.all():
+            break
+        cx, cy = r0 * Zs, r1 * Zs
+        known = np.ones((n, height, width), bool)
+        i0, fr = [], []
+        with np.errstate(invalid="ignore", over="ignore"):
+            for e, dim in enumerate((nx, ny, nz)):
+                Pw = ((p[:, 4 * e] * cx + p[:, 4 * e + 1] * cy) + p[:, 4 * e + 2] * Zs) + p[:, 4 * e + 3]
+                q = (Pw - o[e]) / vox
+                fl = np.floor(q)
+                known &= (fl >= 0) & (fl <= f32(dim - 2))
+                i0.append(np.where(known, fl, 0).astype(np.int64))
+                fr.append((q - fl).astype(f32))
+        i0 = [np.where(known, v, 0) for v in i0]
+        base = (i0[2] * ny + i0[1]) * nx + i0[0]
+        offs = (0, 1, nx, nx + 1, nx * ny, nx * ny + 1, nx * ny + nx, nx * ny + nx + 1)
+        corner = [np.minimum(base + off, T.size - 1) for off in offs]  # clipped where the sample is unknown anyway
+        for ci in corner:
+            known &= Wt[ci] >= mw
+        c = [T[ci] for ci in corner]
+        gx, gy, gz = one - fr[0], one - fr[1], one - fr[2]
+        x00, x10 = c[0] * gx + c[1] * fr[0], c[2] * gx + c[3] * fr[0]
+        x01, x11 = c[4] * gx + c[5] * fr[0], c[6] * gx + c[7] * fr[0]
+        Ts = (x00 * gy + x10 * fr[1]) * gz + (x01 * gy + x11 * fr[1]) * fr[2]
+        hit = ~done & known & prev & (Tp > 0) & (Ts <= 0)
+        with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+            depth = np.where(hit, Zp + st * (Tp / (Tp - Ts)), depth).astype(f32)
+        done |= hit
+        prev = known
+        Tp = Ts
+        Zp = Zs
+    return depth
+
+
+def write_fused_ply(path: str, pts) -> None:
+    """The fused points (FUSE_POINT_DTYPE) as a binary little-endian PLY: x y z nx ny nz float, red green blue uchar --
+    the file of the batch command's --fuse."""
+    pts = np.asarray(pts, FUSE_POINT_DTYPE)
+    rec = np.empty(len(pts), [("p", "<f4", (6,)), ("c", "u1", (3,))])
+    rec["p"] = np.stack([pts[k] for k in ("x", "y", "z", "nx", "ny", "nz")], -1) if len(pts) else np.zeros((0, 6))
+    rec["c"] = np.stack([pts[k] for k in ("r", "g", "b")], -1) if len(pts) else np.zeros((0, 3))
+    with open(path, "wb") as f:
+        f.write(("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\n"
+                 "property float z\nproperty float nx\nproperty float ny\nproperty float nz\nproperty uchar red\n"
+                 "property uchar green\nproperty uchar blue\nend_header\n" % len(pts)).encode())
+        f.write(rec.tobytes())
+
+
 # ---- video stabilisation (ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish) ---------------------------------
 STAB_PARAM_FIELDS = ("radius", "crop", "limit")
 # ofdis_stab_frame, field for field (96 bytes)

@@ -7,8 +7,9 @@ wave kernel with 1 and 2 rows per thread (st.async halo exchange), and the 8-bit
 upsampling kernels), and a frame interpolation, a point tracking (advance, seed, block scan, scatter) and a filtered
 disparity (union-find speckles, fill, depth and xyz) and a global motion (correspondences, compaction, hypotheses,
 the bulk-copied score tiles with and without refills, refits, per-pixel outputs), a stereo ego-motion (the same
-stages on 32-byte correspondences, non-finite disparities, score tile refills) and a Fisher encoding (projection,
-posteriors, float64 statistics, the take) checked against their restatements.  Results are checked against the
+stages on 32-byte correspondences, non-finite disparities, score tile refills), a Fisher encoding (projection,
+posteriors, float64 statistics, the take) and a TSDF fusion (integration, crossing count, scan and write, ray casting)
+checked against their restatements.  Results are checked against the
 oracle so that a clean log means a correct run."""
 import os
 import sys
@@ -203,6 +204,33 @@ exp = preprocess.fisher_encode(x, cb)
 ok = all(np.array_equal(g.view(np.uint8), e.view(np.uint8)) for g, e in zip(got[:2], exp[:2])) and \
     np.array_equal(got[2]["n"], exp[2]["n"]) and np.array_equal(got[2]["skipped"], exp[2]["skipped"])
 print("%-22s %s" % ("fisher_idt_k24", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# volumetric fusion: a 29 x 17 x 33 volume straddling the frustum (beside and behind the cameras), disparities with
+# NaN, -0, +inf and 3e9, RGB colour, then the volume, every point and a render checked bitwise
+rng = np.random.default_rng(9)
+cam = dict(fx=80.0, fy=77.0, cx=31.25, cy=23.5, baseline=0.5, doffs=0.25)
+h3, w3 = 48, 64
+maps = (np.float32(40.0) / rng.uniform(1.1, 1.6, (3, h3, w3)) - np.float32(0.25)).astype(np.float32)
+for v, share in ((np.nan, 0.05), (-0.0, 0.03), (np.inf, 0.02), (3e9, 0.02)):
+    maps[rng.random(maps.shape) < share] = v
+poses = np.stack([np.concatenate([synth.axis_angle(rng.uniform(-0.1, 0.1, 3)),
+                                  rng.uniform(-0.2, 0.2, (3, 1))], 1) for _ in range(3)])
+rgb = rng.integers(0, 256, (3, h3, w3, 3)).astype(np.uint8)
+fp = dict(nx=29, ny=17, nz=33, origin=(-1.5, -0.8, 0.2), voxel=0.07, trunc=0.2, max_weight=5.0, color=1)
+prm = params.from_cli_numbers("3 1 8 8 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=3, nop=2)
+ctx = api.Context(prm, w3, h3, prm.p_samp_s, 2)
+ctx.fuse_begin(fp)
+ctx.fuse_push(maps, poses, cam, width_org=w3, height_org=h3, frames=rgb)
+gv = ctx.fuse_volume()
+gp, _ = ctx.fuse_extract(1.0)
+gd = ctx.fuse_render(poses, cam, z_near=0.3, z_far=2.5, step=0.03, width_org=w3, height_org=h3)
+ctx.close()
+ev = preprocess.fuse_integrate(preprocess.fuse_new_volume(fp), fp, maps, poses, cam, frames=rgb)
+ok = all(np.array_equal(gv[k].view(np.uint8), ev[k].view(np.uint8)) for k in ("T", "W", "C")) and \
+    np.array_equal(gp.view(np.uint8), preprocess.fuse_extract(ev, fp, 1.0).view(np.uint8)) and \
+    np.array_equal(gd.view(np.uint8), preprocess.fuse_render(ev, fp, poses, cam, 0.3, 2.5, 0.03, 1.0, w3, h3).view(np.uint8))
+print("%-22s %s" % ("fuse", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
