@@ -707,6 +707,51 @@ int ofdis_fuse_render(ofdis_ctx* ctx, int n, const double* poses, const ofdis_st
  * (color must be NULL for a volume without colour).  Synchronises the stream.  OFDIS_ERR_ARG: no live volume, a
  * colour output without colour, or a device T or W that is not 4-byte aligned. */
 int ofdis_fuse_get_volume(ofdis_ctx* ctx, float* T, float* W, unsigned char* color, int memkind);
+/* The inverse of ofdis_fuse_get_volume: T, W and color (as it lays them out, in memkind) into the volume; a NULL
+ * array leaves that array as it was.  Any float bits are accepted: the comparisons of the contract then apply as
+ * written (NaN fails every test).  One copy per array, no kernel; synchronises the stream.  OFDIS_ERR_ARG, with the
+ * volume unchanged: no live volume, a colour input for a volume without colour, or a device T or W that is not 4-byte
+ * aligned. */
+int ofdis_fuse_set_volume(ofdis_ctx* ctx, const float* T, const float* W, const unsigned char* color, int memkind);
+/* Marching cubes (extension): the volume's surface as a closed, oriented triangle mesh over the crossings of
+ * ofdis_fuse_extract.  preprocess.fuse_mesh restates it bit for bit and preprocess.fuse_mc_table generates its table.
+ *   Vertices.  Exactly ofdis_fuse_extract(min_weight)'s points, in its order and bit for bit: the crossing of voxel a
+ *   along axis e has vertex index = its position in that list (uint32: a volume has at most 3 * 2^30 crossings).
+ *   Cubes.  Cube (i, j, k) exists for i < nx-1, j < ny-1, k < nz-1.  Its corner q = 0 .. 7 is voxel (i + (q&1),
+ *   j + ((q>>1)&1), k + (q>>2)).  A cube is meshed when all 8 corners satisfy W >= min_weight && fabsf(T) < 1, the
+ *   extraction's per-voxel test; its case is the sum over q of (T_q > 0) << q (-0 and NaN count as solid, but NaN
+ *   fails the test).  Every sign-changing edge of a meshed cube therefore joins two voxels that pass the test: it is
+ *   an extraction crossing, and every face index refers to an existing vertex.  Edge n = 4*e + r (e the axis) runs
+ *   from corner q -- r with a 0 bit inserted at bit e -- to q | (1 << e): edges 0..3 join corners 0-1, 2-3, 4-5, 6-7,
+ *   edges 4..7 join 0-2, 1-3, 4-6, 5-7, edges 8..11 join 0-4, 1-5, 2-6, 3-7.  Its vertex is the crossing of corner q's
+ *   voxel along e.
+ *   Table (preprocess.fuse_mc_table; 820 triangles over the 256 cases, at most 5 per case), from three rules:
+ *     face rule: on each cube face the crossing edges are joined by segments; on an ambiguous face (diagonal corners
+ *     of equal sign) the segments cut off the two T > 0 corners, so that the solid side stays connected across the
+ *     face.  The rule depends only on the face's four signs, so two cubes sharing a face make the same segments and
+ *     the mesh has no cracks (the classic 15-case table does not have this property);
+ *     loops: the segments link into closed loops (every crossing edge lies on exactly two faces, so the loops are
+ *     unique), oriented so that each triangle's normal (p1 - p0) x (p2 - p0) points towards T > 0 -- free space, the
+ *     direction of the extraction's normals.  A cube's loops go in the order of their lowest edge numbers, and each
+ *     loop v_0 .. v_L-1 starts at its lowest edge;
+ *     triangulation: each loop takes the first triangulation, in this enumeration, in which no diagonal joins two
+ *     edges on the same cube face.  The triangulations of v_lo .. v_hi: for the apex k = lo+1 .. hi-1 in ascending
+ *     order, the triangle (v_lo, v_k, v_hi), then each triangulation of v_lo .. v_k and, within it, of v_k .. v_hi;
+ *     that is also the order of the triangles.
+ *   Faces.  Meshed cubes in ascending voxel index of corner 0, each cube's triangles in table order, as [3] uint32
+ *   vertex indices.
+ * *pt_count and *face_count (host) get the totals; pts ([pt_capacity] records) and faces ([face_capacity][3]) in
+ * memkind the first min(capacity, total) entries; capacity 0 counts only (the array may then be NULL).  Faces keep
+ * their global indices when pt_capacity is below the vertex total.  Six kernels whatever the volume (the extraction's
+ * count and scan, a cube count and the same scan, the extraction's write with each crossing voxel's first vertex
+ * index, a face write), one synchronise, and with host output one readback of the two totals before the writes; host
+ * output goes through the full-resolution scratch.  The workspace (4 bytes per voxel plus 8 per scan block of 1024
+ * voxels, and 8 for the total) is allocated at the first call, grows, never shrinks and is freed by ofdis_destroy;
+ * OFDIS_ERR_NOMEM when that fails, with the volume intact.  OFDIS_ERR_ARG, with the volume and the outputs untouched:
+ * no live volume, NULL pt_count or face_count, a capacity < 0, a NULL array with capacity > 0, min_weight NaN, or a
+ * device pts or faces that is not 4-byte aligned. */
+int ofdis_fuse_mesh(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, long pt_capacity, long* pt_count,
+                    unsigned int* faces, long face_capacity, long* face_count, int memkind);
 
 /* Dense point trajectories (extension): the tracker of Sundaram, Brox and Keutzer ("Dense point trajectories by
  * GPU-accelerated large displacement optical flow", ECCV 2010) through consecutive pairs of bidirectional flows.

@@ -45,7 +45,7 @@ EXPORTS = [
     "ofdis_traj_begin", "ofdis_traj_advance", "ofdis_traj_stats_get", "ofdis_scene_flow_fullres",
     "ofdis_fisher_begin", "ofdis_fisher_push", "ofdis_fisher_take", "ofdis_traj_advance_fisher",
     "ofdis_egomotion_fullres", "ofdis_fuse_begin", "ofdis_fuse_push", "ofdis_fuse_extract", "ofdis_fuse_render",
-    "ofdis_fuse_get_volume",
+    "ofdis_fuse_get_volume", "ofdis_fuse_set_volume", "ofdis_fuse_mesh",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -278,6 +278,9 @@ def lib():
         L.ofdis_fuse_render.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.POINTER(StereoCamera)] + \
             [ctypes.c_float] * 4 + [ctypes.c_void_p] + [ctypes.c_int] * 3
         L.ofdis_fuse_get_volume.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int]
+        L.ofdis_fuse_set_volume.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int]
+        L.ofdis_fuse_mesh.argtypes = [ctypes.c_void_p, ctypes.c_float] + \
+            [ctypes.c_void_p, ctypes.c_long, ctypes.POINTER(ctypes.c_long)] * 2 + [ctypes.c_int]
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -1150,6 +1153,47 @@ class Context:
             color = np.empty((nz, ny, nx, 3), np.uint8) if col else None
         self._ck(lib().ofdis_fuse_get_volume(self._h, _ptr(T), _ptr(W), _ptr(color), memkind))
         return {"T": T, "W": W, "C": color}
+
+    def fuse_set_volume(self, T=None, W=None, color=None, memkind=MEM_HOST):
+        """Loads the volume (ofdis_fuse_set_volume, the inverse of fuse_volume): host T and W float32 and color uint8
+        as preprocess.fuse_new_volume lays them out, or device addresses with memkind=MEM_DEVICE; None leaves that
+        array as it was."""
+        if memkind == MEM_HOST:
+            nx, ny, nz, _ = getattr(self, "_fuse", (0, 0, 0, 0))
+            arrs = []
+            for a, dt, shape in ((T, np.float32, (nz, ny, nx)), (W, np.float32, (nz, ny, nx)),
+                                 (color, np.uint8, (nz, ny, nx, 3))):
+                if a is not None:
+                    a = np.ascontiguousarray(a, dt)
+                    if a.shape != shape:
+                        raise ValueError("fuse_set_volume: an array of shape %s, expected %s" % (a.shape, shape))
+                arrs.append(a)
+            T, W, color = arrs
+        self._ck(lib().ofdis_fuse_set_volume(self._h, _ptr(T), _ptr(W), _ptr(color), memkind))
+
+    def fuse_mesh(self, min_weight=1.0, pt_capacity=None, face_capacity=None, memkind=MEM_HOST, pts_out=None,
+                  faces_out=None):
+        """The volume's triangle mesh (ofdis_fuse_mesh; preprocess.fuse_mesh restates it): returns (points, faces,
+        n_points, n_faces).  Host: points of FUSE_POINT_DTYPE (the points of fuse_extract) and faces (F, 3) uint32; a
+        capacity None counts first and takes them all, else at most that many.  With memkind=MEM_DEVICE pts_out and
+        faces_out are device addresses of the capacities' records the caller owns and are returned as given."""
+        n_pts, n_faces = ctypes.c_long(0), ctypes.c_long(0)
+        if memkind != MEM_HOST:
+            self._ck(lib().ofdis_fuse_mesh(self._h, min_weight, _ptr(pts_out), pt_capacity or 0, ctypes.byref(n_pts),
+                                           _ptr(faces_out), face_capacity or 0, ctypes.byref(n_faces), memkind))
+            return pts_out, faces_out, n_pts.value, n_faces.value
+        if pt_capacity is None or face_capacity is None:
+            self._ck(lib().ofdis_fuse_mesh(self._h, min_weight, None, 0, ctypes.byref(n_pts), None, 0,
+                                           ctypes.byref(n_faces), memkind))
+            pt_capacity = n_pts.value if pt_capacity is None else pt_capacity
+            face_capacity = n_faces.value if face_capacity is None else face_capacity
+        pts = np.zeros(pt_capacity, FUSE_POINT_DTYPE)
+        faces = np.zeros((face_capacity, 3), np.uint32)
+        self._ck(lib().ofdis_fuse_mesh(self._h, min_weight, _ptr(pts) if pt_capacity else None, pt_capacity,
+                                       ctypes.byref(n_pts), _ptr(faces) if face_capacity else None, face_capacity,
+                                       ctypes.byref(n_faces), memkind))
+        return pts[:min(pt_capacity, n_pts.value)], faces[:min(face_capacity, n_faces.value)], n_pts.value, \
+            n_faces.value
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

@@ -9,6 +9,11 @@
 //   fuse_write_kernel      the block's crossings again, scanned within the CTA, written at their global index while it
 //                          is below the capacity: the order of the header, whatever the grid.
 //   fuse_render_kernel     one thread per (pose, pixel), fixed-step ray march to the first sign change.
+// Marching cubes (ofdis_fuse_mesh; preprocess.fuse_mesh restates it): the count, scan and write kernels above give the
+// vertices, the write kernel also each crossing voxel's first vertex index, then
+//   fuse_cube_count_kernel triangles per scan block of FUSE_BLOCK cubes (cube = the voxel of its corner 0), scanned by
+//                          fuse_scan_kernel into a second offset array;
+//   fuse_face_kernel       the block's triangles again, written at their global index while it is below the capacity.
 #include <cuda_runtime.h>
 
 #include "ofdis_internal.cuh"
@@ -23,6 +28,267 @@ constexpr int FUSE_SCAN_THREADS = 1024;
 constexpr int FUSE_RENDER_ROWS = 8;                 // a render CTA is 32 x 8 pixels of one pose
 
 __device__ __forceinline__ float qnan() { return __int_as_float(0x7fc00000); }
+
+// The marching-cubes table of ofdis_fuse_mesh, as preprocess.fuse_mc_table generates it from the header's rules: row =
+// case, [0] the triangles, [1 + 3t + s] the cube edge of triangle t's vertex s, 255 past the last.
+__constant__ unsigned char FUSE_MC[256][16] = {
+    {0, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 0, 8, 4, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 0, 5, 9, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 4, 5, 8, 5, 9, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 1, 4, 10, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 8, 1, 8, 10, 1, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 5, 9, 1, 4, 10, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 1, 5, 10, 5, 9, 10, 9, 8, 10, 255, 255, 255, 255, 255, 255},
+    {1, 1, 11, 5, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 8, 4, 1, 11, 5, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 1, 9, 1, 11, 9, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 1, 11, 4, 11, 9, 4, 9, 8, 4, 255, 255, 255, 255, 255, 255},
+    {2, 4, 10, 5, 10, 11, 5, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 5, 8, 10, 5, 10, 11, 5, 255, 255, 255, 255, 255, 255},
+    {3, 0, 4, 9, 4, 10, 9, 10, 11, 9, 255, 255, 255, 255, 255, 255},
+    {2, 8, 10, 9, 10, 11, 9, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 2, 6, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 2, 4, 2, 6, 4, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 5, 9, 2, 6, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 2, 6, 9, 6, 4, 9, 4, 5, 9, 255, 255, 255, 255, 255, 255},
+    {2, 1, 4, 10, 2, 6, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 2, 1, 2, 6, 1, 6, 10, 1, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 9, 1, 4, 10, 2, 6, 8, 255, 255, 255, 255, 255, 255},
+    {4, 1, 5, 10, 5, 9, 10, 9, 2, 10, 2, 6, 10, 255, 255, 255},
+    {2, 1, 11, 5, 2, 6, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 2, 4, 2, 6, 4, 1, 11, 5, 255, 255, 255, 255, 255, 255},
+    {3, 0, 1, 9, 1, 11, 9, 2, 6, 8, 255, 255, 255, 255, 255, 255},
+    {4, 1, 11, 4, 11, 9, 4, 9, 2, 4, 2, 6, 4, 255, 255, 255},
+    {3, 2, 6, 8, 4, 10, 5, 10, 11, 5, 255, 255, 255, 255, 255, 255},
+    {4, 0, 2, 5, 2, 6, 5, 6, 10, 5, 10, 11, 5, 255, 255, 255},
+    {4, 0, 4, 9, 4, 10, 9, 10, 11, 9, 2, 6, 8, 255, 255, 255},
+    {3, 2, 6, 9, 6, 10, 9, 10, 11, 9, 255, 255, 255, 255, 255, 255},
+    {1, 2, 9, 7, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 8, 4, 2, 9, 7, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 5, 2, 5, 7, 2, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 2, 8, 7, 8, 4, 7, 4, 5, 7, 255, 255, 255, 255, 255, 255},
+    {2, 1, 4, 10, 2, 9, 7, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 1, 8, 10, 1, 2, 9, 7, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 2, 5, 7, 2, 1, 4, 10, 255, 255, 255, 255, 255, 255},
+    {4, 1, 5, 10, 5, 7, 10, 7, 2, 10, 2, 8, 10, 255, 255, 255},
+    {2, 1, 11, 5, 2, 9, 7, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 4, 1, 11, 5, 2, 9, 7, 255, 255, 255, 255, 255, 255},
+    {3, 0, 1, 2, 1, 11, 2, 11, 7, 2, 255, 255, 255, 255, 255, 255},
+    {4, 1, 11, 4, 11, 7, 4, 7, 2, 4, 2, 8, 4, 255, 255, 255},
+    {3, 2, 9, 7, 4, 10, 5, 10, 11, 5, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 5, 8, 10, 5, 10, 11, 5, 2, 9, 7, 255, 255, 255},
+    {4, 0, 4, 2, 4, 10, 2, 10, 11, 2, 11, 7, 2, 255, 255, 255},
+    {3, 2, 8, 7, 8, 10, 7, 10, 11, 7, 255, 255, 255, 255, 255, 255},
+    {2, 6, 8, 7, 8, 9, 7, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 9, 4, 9, 7, 4, 7, 6, 4, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 8, 5, 7, 8, 7, 6, 8, 255, 255, 255, 255, 255, 255},
+    {2, 4, 5, 6, 5, 7, 6, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 1, 4, 10, 6, 8, 7, 8, 9, 7, 255, 255, 255, 255, 255, 255},
+    {4, 0, 9, 1, 9, 7, 1, 7, 6, 1, 6, 10, 1, 255, 255, 255},
+    {4, 0, 5, 8, 5, 7, 8, 7, 6, 8, 1, 4, 10, 255, 255, 255},
+    {3, 1, 5, 10, 5, 7, 10, 7, 6, 10, 255, 255, 255, 255, 255, 255},
+    {3, 1, 11, 5, 6, 8, 7, 8, 9, 7, 255, 255, 255, 255, 255, 255},
+    {4, 0, 9, 4, 9, 7, 4, 7, 6, 4, 1, 11, 5, 255, 255, 255},
+    {4, 0, 1, 8, 1, 11, 8, 11, 7, 8, 7, 6, 8, 255, 255, 255},
+    {3, 1, 11, 4, 11, 7, 4, 7, 6, 4, 255, 255, 255, 255, 255, 255},
+    {4, 4, 10, 5, 10, 11, 5, 6, 8, 7, 8, 9, 7, 255, 255, 255},
+    {5, 0, 6, 5, 0, 9, 6, 9, 7, 6, 6, 10, 5, 10, 11, 5},
+    {5, 0, 11, 8, 0, 4, 11, 4, 10, 11, 11, 7, 8, 7, 6, 8},
+    {2, 6, 10, 7, 10, 11, 7, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 3, 10, 6, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 8, 4, 3, 10, 6, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 5, 9, 3, 10, 6, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 3, 10, 6, 4, 5, 8, 5, 9, 8, 255, 255, 255, 255, 255, 255},
+    {2, 1, 4, 3, 4, 6, 3, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 1, 8, 6, 1, 6, 3, 1, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 9, 1, 4, 3, 4, 6, 3, 255, 255, 255, 255, 255, 255},
+    {4, 1, 5, 3, 5, 9, 3, 9, 8, 3, 8, 6, 3, 255, 255, 255},
+    {2, 1, 11, 5, 3, 10, 6, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 4, 1, 11, 5, 3, 10, 6, 255, 255, 255, 255, 255, 255},
+    {3, 0, 1, 9, 1, 11, 9, 3, 10, 6, 255, 255, 255, 255, 255, 255},
+    {4, 1, 11, 4, 11, 9, 4, 9, 8, 4, 3, 10, 6, 255, 255, 255},
+    {3, 3, 11, 6, 11, 5, 6, 5, 4, 6, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 5, 8, 6, 5, 6, 3, 5, 3, 11, 5, 255, 255, 255},
+    {4, 0, 4, 9, 4, 6, 9, 6, 3, 9, 3, 11, 9, 255, 255, 255},
+    {3, 3, 11, 6, 11, 9, 6, 9, 8, 6, 255, 255, 255, 255, 255, 255},
+    {2, 2, 3, 8, 3, 10, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 2, 4, 2, 3, 4, 3, 10, 4, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 9, 2, 3, 8, 3, 10, 8, 255, 255, 255, 255, 255, 255},
+    {4, 2, 3, 9, 3, 10, 9, 10, 4, 9, 4, 5, 9, 255, 255, 255},
+    {3, 1, 4, 3, 4, 8, 3, 8, 2, 3, 255, 255, 255, 255, 255, 255},
+    {2, 0, 2, 1, 2, 3, 1, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {4, 0, 5, 9, 1, 4, 3, 4, 8, 3, 8, 2, 3, 255, 255, 255},
+    {3, 1, 5, 3, 5, 9, 3, 9, 2, 3, 255, 255, 255, 255, 255, 255},
+    {3, 1, 11, 5, 2, 3, 8, 3, 10, 8, 255, 255, 255, 255, 255, 255},
+    {4, 0, 2, 4, 2, 3, 4, 3, 10, 4, 1, 11, 5, 255, 255, 255},
+    {4, 0, 1, 9, 1, 11, 9, 2, 3, 8, 3, 10, 8, 255, 255, 255},
+    {5, 1, 11, 4, 11, 9, 4, 9, 2, 4, 2, 3, 4, 3, 10, 4},
+    {4, 2, 3, 8, 3, 11, 8, 11, 5, 8, 5, 4, 8, 255, 255, 255},
+    {3, 0, 2, 5, 2, 3, 5, 3, 11, 5, 255, 255, 255, 255, 255, 255},
+    {5, 0, 4, 9, 4, 3, 9, 4, 8, 3, 8, 2, 3, 3, 11, 9},
+    {2, 2, 3, 9, 3, 11, 9, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 2, 9, 7, 3, 10, 6, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 4, 2, 9, 7, 3, 10, 6, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 2, 5, 7, 2, 3, 10, 6, 255, 255, 255, 255, 255, 255},
+    {4, 2, 8, 7, 8, 4, 7, 4, 5, 7, 3, 10, 6, 255, 255, 255},
+    {3, 1, 4, 3, 4, 6, 3, 2, 9, 7, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 1, 8, 6, 1, 6, 3, 1, 2, 9, 7, 255, 255, 255},
+    {4, 0, 5, 2, 5, 7, 2, 1, 4, 3, 4, 6, 3, 255, 255, 255},
+    {5, 1, 5, 3, 5, 8, 3, 5, 7, 8, 7, 2, 8, 8, 6, 3},
+    {3, 1, 11, 5, 2, 9, 7, 3, 10, 6, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 4, 1, 11, 5, 2, 9, 7, 3, 10, 6, 255, 255, 255},
+    {4, 0, 1, 2, 1, 11, 2, 11, 7, 2, 3, 10, 6, 255, 255, 255},
+    {5, 1, 11, 4, 11, 7, 4, 7, 2, 4, 2, 8, 4, 3, 10, 6},
+    {4, 2, 9, 7, 3, 11, 6, 11, 5, 6, 5, 4, 6, 255, 255, 255},
+    {5, 0, 8, 5, 8, 6, 5, 6, 3, 5, 3, 11, 5, 2, 9, 7},
+    {5, 0, 4, 2, 4, 11, 2, 4, 6, 11, 6, 3, 11, 11, 7, 2},
+    {4, 2, 8, 7, 8, 11, 7, 8, 6, 11, 6, 3, 11, 255, 255, 255},
+    {3, 3, 10, 7, 10, 8, 7, 8, 9, 7, 255, 255, 255, 255, 255, 255},
+    {4, 0, 9, 4, 9, 7, 4, 7, 3, 4, 3, 10, 4, 255, 255, 255},
+    {4, 0, 5, 8, 5, 7, 8, 7, 3, 8, 3, 10, 8, 255, 255, 255},
+    {3, 3, 10, 7, 10, 4, 7, 4, 5, 7, 255, 255, 255, 255, 255, 255},
+    {4, 1, 4, 3, 4, 8, 3, 8, 9, 3, 9, 7, 3, 255, 255, 255},
+    {3, 0, 9, 1, 9, 7, 1, 7, 3, 1, 255, 255, 255, 255, 255, 255},
+    {5, 0, 5, 8, 5, 7, 8, 7, 3, 8, 3, 1, 8, 1, 4, 8},
+    {2, 1, 5, 3, 5, 7, 3, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {4, 1, 11, 5, 3, 10, 7, 10, 8, 7, 8, 9, 7, 255, 255, 255},
+    {5, 0, 9, 4, 9, 7, 4, 7, 3, 4, 3, 10, 4, 1, 11, 5},
+    {5, 0, 1, 8, 1, 11, 8, 11, 7, 8, 7, 3, 8, 3, 10, 8},
+    {4, 1, 11, 4, 11, 7, 4, 7, 3, 4, 3, 10, 4, 255, 255, 255},
+    {5, 3, 4, 7, 3, 11, 4, 11, 5, 4, 4, 8, 7, 8, 9, 7},
+    {4, 0, 3, 5, 0, 9, 3, 9, 7, 3, 3, 11, 5, 255, 255, 255},
+    {2, 0, 4, 8, 3, 11, 7, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 3, 11, 7, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 3, 7, 11, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 8, 4, 3, 7, 11, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 0, 5, 9, 3, 7, 11, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 3, 7, 11, 4, 5, 8, 5, 9, 8, 255, 255, 255, 255, 255, 255},
+    {2, 1, 4, 10, 3, 7, 11, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 1, 8, 10, 1, 3, 7, 11, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 9, 1, 4, 10, 3, 7, 11, 255, 255, 255, 255, 255, 255},
+    {4, 1, 5, 10, 5, 9, 10, 9, 8, 10, 3, 7, 11, 255, 255, 255},
+    {2, 1, 3, 5, 3, 7, 5, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 4, 1, 3, 5, 3, 7, 5, 255, 255, 255, 255, 255, 255},
+    {3, 0, 1, 9, 1, 3, 9, 3, 7, 9, 255, 255, 255, 255, 255, 255},
+    {4, 1, 3, 4, 3, 7, 4, 7, 9, 4, 9, 8, 4, 255, 255, 255},
+    {3, 3, 7, 10, 7, 5, 10, 5, 4, 10, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 5, 8, 10, 5, 10, 3, 5, 3, 7, 5, 255, 255, 255},
+    {4, 0, 4, 9, 4, 10, 9, 10, 3, 9, 3, 7, 9, 255, 255, 255},
+    {3, 3, 7, 10, 7, 9, 10, 9, 8, 10, 255, 255, 255, 255, 255, 255},
+    {2, 2, 6, 8, 3, 7, 11, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 2, 4, 2, 6, 4, 3, 7, 11, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 9, 2, 6, 8, 3, 7, 11, 255, 255, 255, 255, 255, 255},
+    {4, 2, 6, 9, 6, 4, 9, 4, 5, 9, 3, 7, 11, 255, 255, 255},
+    {3, 1, 4, 10, 2, 6, 8, 3, 7, 11, 255, 255, 255, 255, 255, 255},
+    {4, 0, 2, 1, 2, 6, 1, 6, 10, 1, 3, 7, 11, 255, 255, 255},
+    {4, 0, 5, 9, 1, 4, 10, 2, 6, 8, 3, 7, 11, 255, 255, 255},
+    {5, 1, 5, 10, 5, 9, 10, 9, 2, 10, 2, 6, 10, 3, 7, 11},
+    {3, 1, 3, 5, 3, 7, 5, 2, 6, 8, 255, 255, 255, 255, 255, 255},
+    {4, 0, 2, 4, 2, 6, 4, 1, 3, 5, 3, 7, 5, 255, 255, 255},
+    {4, 0, 1, 9, 1, 3, 9, 3, 7, 9, 2, 6, 8, 255, 255, 255},
+    {5, 1, 3, 4, 3, 7, 4, 7, 9, 4, 9, 2, 4, 2, 6, 4},
+    {4, 2, 6, 8, 3, 7, 10, 7, 5, 10, 5, 4, 10, 255, 255, 255},
+    {5, 0, 2, 5, 2, 6, 5, 6, 10, 5, 10, 3, 5, 3, 7, 5},
+    {5, 0, 4, 9, 4, 10, 9, 10, 3, 9, 3, 7, 9, 2, 6, 8},
+    {4, 2, 6, 9, 6, 10, 9, 10, 3, 9, 3, 7, 9, 255, 255, 255},
+    {2, 2, 9, 3, 9, 11, 3, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 4, 2, 9, 3, 9, 11, 3, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 2, 5, 11, 2, 11, 3, 2, 255, 255, 255, 255, 255, 255},
+    {4, 2, 8, 3, 8, 4, 3, 4, 5, 3, 5, 11, 3, 255, 255, 255},
+    {3, 1, 4, 10, 2, 9, 3, 9, 11, 3, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 1, 8, 10, 1, 2, 9, 3, 9, 11, 3, 255, 255, 255},
+    {4, 0, 5, 2, 5, 11, 2, 11, 3, 2, 1, 4, 10, 255, 255, 255},
+    {5, 1, 5, 10, 5, 2, 10, 5, 11, 2, 11, 3, 2, 2, 8, 10},
+    {3, 1, 3, 5, 3, 2, 5, 2, 9, 5, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 4, 1, 3, 5, 3, 2, 5, 2, 9, 5, 255, 255, 255},
+    {2, 0, 1, 2, 1, 3, 2, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 1, 3, 4, 3, 2, 4, 2, 8, 4, 255, 255, 255, 255, 255, 255},
+    {4, 2, 9, 3, 9, 5, 3, 5, 4, 3, 4, 10, 3, 255, 255, 255},
+    {5, 0, 8, 5, 8, 10, 5, 10, 3, 5, 3, 2, 5, 2, 9, 5},
+    {3, 0, 4, 2, 4, 10, 2, 10, 3, 2, 255, 255, 255, 255, 255, 255},
+    {2, 2, 8, 3, 8, 10, 3, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 3, 6, 11, 6, 8, 11, 8, 9, 11, 255, 255, 255, 255, 255, 255},
+    {4, 0, 9, 4, 9, 11, 4, 11, 3, 4, 3, 6, 4, 255, 255, 255},
+    {4, 0, 5, 8, 5, 11, 8, 11, 3, 8, 3, 6, 8, 255, 255, 255},
+    {3, 3, 6, 11, 6, 4, 11, 4, 5, 11, 255, 255, 255, 255, 255, 255},
+    {4, 1, 4, 10, 3, 6, 11, 6, 8, 11, 8, 9, 11, 255, 255, 255},
+    {5, 0, 9, 1, 9, 6, 1, 9, 11, 6, 11, 3, 6, 6, 10, 1},
+    {5, 0, 5, 8, 5, 11, 8, 11, 3, 8, 3, 6, 8, 1, 4, 10},
+    {4, 1, 5, 10, 5, 6, 10, 5, 11, 6, 11, 3, 6, 255, 255, 255},
+    {4, 1, 3, 5, 3, 6, 5, 6, 8, 5, 8, 9, 5, 255, 255, 255},
+    {5, 0, 9, 4, 9, 3, 4, 9, 5, 3, 5, 1, 3, 3, 6, 4},
+    {3, 0, 1, 8, 1, 3, 8, 3, 6, 8, 255, 255, 255, 255, 255, 255},
+    {2, 1, 3, 4, 3, 6, 4, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {5, 3, 9, 10, 3, 6, 9, 6, 8, 9, 9, 5, 10, 5, 4, 10},
+    {2, 0, 9, 5, 3, 6, 10, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {4, 0, 3, 8, 0, 4, 3, 4, 10, 3, 3, 6, 8, 255, 255, 255},
+    {1, 3, 6, 10, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 6, 7, 10, 7, 11, 10, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 4, 6, 7, 10, 7, 11, 10, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 9, 6, 7, 10, 7, 11, 10, 255, 255, 255, 255, 255, 255},
+    {4, 4, 5, 8, 5, 9, 8, 6, 7, 10, 7, 11, 10, 255, 255, 255},
+    {3, 1, 4, 11, 4, 6, 11, 6, 7, 11, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 1, 8, 6, 1, 6, 7, 1, 7, 11, 1, 255, 255, 255},
+    {4, 0, 5, 9, 1, 4, 11, 4, 6, 11, 6, 7, 11, 255, 255, 255},
+    {5, 1, 8, 11, 1, 5, 8, 5, 9, 8, 8, 6, 11, 6, 7, 11},
+    {3, 1, 10, 5, 10, 6, 5, 6, 7, 5, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 4, 1, 10, 5, 10, 6, 5, 6, 7, 5, 255, 255, 255},
+    {4, 0, 1, 9, 1, 10, 9, 10, 6, 9, 6, 7, 9, 255, 255, 255},
+    {5, 1, 7, 4, 1, 10, 7, 10, 6, 7, 7, 9, 4, 9, 8, 4},
+    {2, 4, 6, 5, 6, 7, 5, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 8, 5, 8, 6, 5, 6, 7, 5, 255, 255, 255, 255, 255, 255},
+    {3, 0, 4, 9, 4, 6, 9, 6, 7, 9, 255, 255, 255, 255, 255, 255},
+    {2, 6, 7, 8, 7, 9, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 2, 7, 8, 7, 11, 8, 11, 10, 8, 255, 255, 255, 255, 255, 255},
+    {4, 0, 2, 4, 2, 7, 4, 7, 11, 4, 11, 10, 4, 255, 255, 255},
+    {4, 0, 5, 9, 2, 7, 8, 7, 11, 8, 11, 10, 8, 255, 255, 255},
+    {5, 2, 10, 9, 2, 7, 10, 7, 11, 10, 10, 4, 9, 4, 5, 9},
+    {4, 1, 4, 11, 4, 8, 11, 8, 2, 11, 2, 7, 11, 255, 255, 255},
+    {3, 0, 2, 1, 2, 7, 1, 7, 11, 1, 255, 255, 255, 255, 255, 255},
+    {5, 0, 5, 9, 1, 4, 11, 4, 8, 11, 8, 2, 11, 2, 7, 11},
+    {4, 1, 2, 11, 1, 5, 2, 5, 9, 2, 2, 7, 11, 255, 255, 255},
+    {4, 1, 10, 5, 10, 8, 5, 8, 2, 5, 2, 7, 5, 255, 255, 255},
+    {5, 0, 2, 4, 2, 7, 4, 7, 10, 4, 7, 5, 10, 5, 1, 10},
+    {5, 0, 1, 9, 1, 10, 9, 10, 7, 9, 10, 8, 7, 8, 2, 7},
+    {2, 1, 10, 4, 2, 7, 9, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 2, 7, 8, 7, 5, 8, 5, 4, 8, 255, 255, 255, 255, 255, 255},
+    {2, 0, 2, 5, 2, 7, 5, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {4, 0, 4, 9, 4, 7, 9, 4, 8, 7, 8, 2, 7, 255, 255, 255},
+    {1, 2, 7, 9, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 2, 9, 6, 9, 11, 6, 11, 10, 6, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 4, 2, 9, 6, 9, 11, 6, 11, 10, 6, 255, 255, 255},
+    {4, 0, 5, 2, 5, 11, 2, 11, 10, 2, 10, 6, 2, 255, 255, 255},
+    {5, 2, 5, 6, 2, 8, 5, 8, 4, 5, 5, 11, 6, 11, 10, 6},
+    {4, 1, 4, 11, 4, 6, 11, 6, 2, 11, 2, 9, 11, 255, 255, 255},
+    {5, 0, 8, 1, 8, 6, 1, 6, 2, 1, 2, 9, 1, 9, 11, 1},
+    {5, 0, 5, 2, 5, 11, 2, 11, 1, 2, 1, 4, 2, 4, 6, 2},
+    {2, 1, 5, 11, 2, 8, 6, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {4, 1, 10, 5, 10, 6, 5, 6, 2, 5, 2, 9, 5, 255, 255, 255},
+    {5, 0, 8, 4, 1, 10, 5, 10, 6, 5, 6, 2, 5, 2, 9, 5},
+    {3, 0, 1, 2, 1, 10, 2, 10, 6, 2, 255, 255, 255, 255, 255, 255},
+    {4, 1, 2, 4, 1, 10, 2, 10, 6, 2, 2, 8, 4, 255, 255, 255},
+    {3, 2, 9, 6, 9, 5, 6, 5, 4, 6, 255, 255, 255, 255, 255, 255},
+    {4, 0, 8, 5, 8, 6, 5, 6, 2, 5, 2, 9, 5, 255, 255, 255},
+    {2, 0, 4, 2, 4, 6, 2, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 2, 8, 6, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 8, 9, 10, 9, 11, 10, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 0, 9, 4, 9, 11, 4, 11, 10, 4, 255, 255, 255, 255, 255, 255},
+    {3, 0, 5, 8, 5, 11, 8, 11, 10, 8, 255, 255, 255, 255, 255, 255},
+    {2, 4, 5, 10, 5, 11, 10, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 1, 4, 11, 4, 8, 11, 8, 9, 11, 255, 255, 255, 255, 255, 255},
+    {2, 0, 9, 1, 9, 11, 1, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {4, 0, 5, 8, 5, 11, 8, 11, 1, 8, 1, 4, 8, 255, 255, 255},
+    {1, 1, 5, 11, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {3, 1, 10, 5, 10, 8, 5, 8, 9, 5, 255, 255, 255, 255, 255, 255},
+    {4, 0, 9, 4, 9, 10, 4, 9, 5, 10, 5, 1, 10, 255, 255, 255},
+    {2, 0, 1, 8, 1, 10, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 1, 10, 4, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {2, 4, 8, 5, 8, 9, 5, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 0, 9, 5, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {1, 0, 4, 8, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+    {0, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
+};
 
 __global__ void __launch_bounds__(FUSE_THREADS) fuse_integrate_kernel(FuseGeom g, FuseVolume v, FusePush p) {
   const long long a = (long long)blockIdx.x * FUSE_THREADS + threadIdx.x;
@@ -144,9 +410,12 @@ __global__ void __launch_bounds__(FUSE_SCAN_THREADS) fuse_scan_kernel(unsigned l
   if (threadIdx.x == 0) *total = carry;
 }
 
+// BASES: also vbase[a] = the index of voxel a's first crossing, for every voxel with a crossing, whatever the capacity
+template <bool BASES>
 __global__ void __launch_bounds__(FUSE_THREADS) fuse_write_kernel(FuseGeom g, FuseVolume v, float minw,
                                                                   const unsigned long long* bsum,
-                                                                  ofdis_fuse_point* out, long long cap) {
+                                                                  ofdis_fuse_point* out, long long cap,
+                                                                  unsigned int* vbase) {
   __shared__ unsigned int sw[FUSE_THREADS / 32];
   const long long a0 = (long long)blockIdx.x * FUSE_BLOCK + (long long)threadIdx.x * FUSE_VPT;
   unsigned m[FUSE_VPT], cnt = 0;
@@ -158,6 +427,14 @@ __global__ void __launch_bounds__(FUSE_THREADS) fuse_write_kernel(FuseGeom g, Fu
   unsigned int total;
   const unsigned int ex = block_exclusive_scan<FUSE_THREADS>(cnt, sw, total);
   unsigned long long o = bsum[blockIdx.x] + ex;
+  if (BASES) {
+    unsigned long long ob = o;
+#pragma unroll
+    for (int q = 0; q < FUSE_VPT; ++q) {
+      if (m[q]) vbase[a0 + q] = (unsigned int)ob;
+      ob += __popc(m[q]);
+    }
+  }
   if (!cnt || o >= (unsigned long long)cap) return;
 #pragma unroll
   for (int q = 0; q < FUSE_VPT; ++q) {
@@ -197,6 +474,82 @@ __global__ void __launch_bounds__(FUSE_THREADS) fuse_write_kernel(FuseGeom g, Fu
       rec.b = v.C ? v.C[3 * src + 2] : 0;
       rec.pad = 0;
       out[o++] = rec;
+    }
+  }
+}
+
+// the case of the cube whose corner 0 is voxel a, or -1 where the cube does not exist or is not meshed (a corner fails
+// W >= minw && fabsf(T) < 1)
+__device__ __forceinline__ int cube_case(const FuseGeom& g, const FuseVolume& v, float minw, long long a) {
+  if (a >= g.count) return -1;
+  const int i = (int)(a % g.nx);
+  const long long r = a / g.nx;
+  const int j = (int)(r % g.ny), k = (int)(r / g.ny);
+  if (i + 1 >= g.nx || j + 1 >= g.ny || k + 1 >= g.nz) return -1;
+  const long long sy = g.nx, sz = (long long)g.nx * g.ny;
+  int c = 0;
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const long long b = a + (q & 1) + ((q >> 1) & 1) * sy + (q >> 2) * sz;
+    const float T = __ldg(v.T + b), W = __ldg(v.W + b);
+    if (!(W >= minw && fabsf(T) < 1.0f)) return -1;
+    c |= (T > 0.0f ? 1 : 0) << q;
+  }
+  return c;
+}
+
+__global__ void __launch_bounds__(FUSE_THREADS) fuse_cube_count_kernel(FuseGeom g, FuseVolume v, float minw,
+                                                                       unsigned long long* bsum) {
+  __shared__ unsigned int sw[FUSE_THREADS / 32];
+  const long long a0 = (long long)blockIdx.x * FUSE_BLOCK + (long long)threadIdx.x * FUSE_VPT;
+  unsigned cnt = 0;
+#pragma unroll
+  for (int q = 0; q < FUSE_VPT; ++q) {
+    const int c = cube_case(g, v, minw, a0 + q);
+    if (c >= 0) cnt += FUSE_MC[c][0];
+  }
+  unsigned int total;
+  block_exclusive_scan<FUSE_THREADS>(cnt, sw, total);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = total;
+}
+
+// the vertex of cube edge n (lower corner q, axis e) of the cube at voxel a: the first vertex of corner q's voxel plus
+// that voxel's crossings along the axes before e
+__device__ __forceinline__ unsigned int edge_vertex(const FuseGeom& g, const FuseVolume& v, float minw,
+                                                    const unsigned int* vbase, long long a, int n) {
+  const int e = n >> 2, r = n & 3;
+  const int q = (r & ((1 << e) - 1)) | ((r >> e) << (e + 1));
+  const long long b = a + (q & 1) + ((q >> 1) & 1) * (long long)g.nx + (q >> 2) * ((long long)g.nx * g.ny);
+  return vbase[b] + (unsigned int)__popc(crossings(g, v, minw, b) & ((1u << e) - 1u));
+}
+
+__global__ void __launch_bounds__(FUSE_THREADS) fuse_face_kernel(FuseGeom g, FuseVolume v, float minw,
+                                                                 const unsigned long long* bsum,
+                                                                 const unsigned int* vbase, unsigned int* faces,
+                                                                 long long cap) {
+  __shared__ unsigned int sw[FUSE_THREADS / 32];
+  const long long a0 = (long long)blockIdx.x * FUSE_BLOCK + (long long)threadIdx.x * FUSE_VPT;
+  int c[FUSE_VPT];
+  unsigned cnt = 0;
+#pragma unroll
+  for (int q = 0; q < FUSE_VPT; ++q) {
+    c[q] = cube_case(g, v, minw, a0 + q);
+    if (c[q] >= 0) cnt += FUSE_MC[c[q]][0];
+  }
+  unsigned int total;
+  const unsigned int ex = block_exclusive_scan<FUSE_THREADS>(cnt, sw, total);
+  unsigned long long o = bsum[blockIdx.x] + ex;
+  if (!cnt || o >= (unsigned long long)cap) return;
+#pragma unroll
+  for (int q = 0; q < FUSE_VPT; ++q) {
+    if (c[q] < 0) continue;
+    const int nt = FUSE_MC[c[q]][0];
+    for (int t = 0; t < nt; ++t) {
+      if (o >= (unsigned long long)cap) return;
+      unsigned int* f = faces + 3 * o;
+#pragma unroll
+      for (int s = 0; s < 3; ++s) f[s] = edge_vertex(g, v, minw, vbase, a0 + q, FUSE_MC[c[q]][1 + 3 * t + s]);
+      ++o;
     }
   }
 }
@@ -277,9 +630,27 @@ int launch_fuse_count(const FuseGeom& g, const FuseVolume& v, float min_weight, 
 }
 
 int launch_fuse_write(const FuseGeom& g, const FuseVolume& v, float min_weight, const FuseWork& ws,
-                      ofdis_fuse_point* out, long long cap, cudaStream_t st) {
+                      ofdis_fuse_point* out, long long cap, cudaStream_t st, unsigned int* vbase) {
   const int nb = (int)((g.count + FUSE_BLOCK - 1) / FUSE_BLOCK);
-  fuse_write_kernel<<<nb, FUSE_THREADS, 0, st>>>(g, v, min_weight, ws.bsum, out, cap);
+  if (vbase)
+    fuse_write_kernel<true><<<nb, FUSE_THREADS, 0, st>>>(g, v, min_weight, ws.bsum, out, cap, vbase);
+  else
+    fuse_write_kernel<false><<<nb, FUSE_THREADS, 0, st>>>(g, v, min_weight, ws.bsum, out, cap, nullptr);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_fuse_cube_count(const FuseGeom& g, const FuseVolume& v, float min_weight, const FuseMeshWork& mw,
+                           cudaStream_t st) {
+  const int nb = (int)((g.count + FUSE_BLOCK - 1) / FUSE_BLOCK);
+  fuse_cube_count_kernel<<<nb, FUSE_THREADS, 0, st>>>(g, v, min_weight, mw.bsum);
+  fuse_scan_kernel<<<1, FUSE_SCAN_THREADS, 0, st>>>(mw.bsum, nb, mw.total);
+  return cudaGetLastError() == cudaSuccess ? 2 : -1;
+}
+
+int launch_fuse_faces(const FuseGeom& g, const FuseVolume& v, float min_weight, const FuseMeshWork& mw,
+                      unsigned int* faces, long long cap, cudaStream_t st) {
+  const int nb = (int)((g.count + FUSE_BLOCK - 1) / FUSE_BLOCK);
+  fuse_face_kernel<<<nb, FUSE_THREADS, 0, st>>>(g, v, min_weight, mw.bsum, mw.vbase, faces, cap);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -137,6 +137,10 @@ struct ofdis_ctx {
   FuseVolume fuse_vol{};
   FuseWork fuse_ws{};
   bool fuse_on = false;
+  // lazily allocated workspace of ofdis_fuse_mesh (FuseMeshWork: the per-voxel first vertex indices, the second scan
+  // blocks and their total); grows, never shrinks; never touched by ofdis_run
+  void* d_mesh = nullptr;
+  size_t mesh_bytes = 0;
   std::vector<float*> d_flow;   // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -512,6 +516,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_stab);
   cudaFree(ctx->d_fisher);
   cudaFree(ctx->d_fuse);
+  cudaFree(ctx->d_mesh);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -1659,6 +1664,97 @@ int ofdis_fuse_get_volume(ofdis_ctx* ctx, float* T, float* W, unsigned char* col
   if (T) CK(cudaMemcpyAsync(T, v.T, 4 * N, kind, ctx->stream));
   if (W) CK(cudaMemcpyAsync(W, v.W, 4 * N, kind, ctx->stream));
   if (color) CK(cudaMemcpyAsync(color, v.C, 3 * N, kind, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return OFDIS_OK;
+}
+
+int ofdis_fuse_mesh(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, long pt_capacity, long* pt_count,
+                    unsigned int* faces, long face_capacity, long* face_count, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_mesh: no live volume (ofdis_fuse_begin)");
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  if (!pt_count || !face_count || pt_capacity < 0 || face_capacity < 0 || (pt_capacity > 0 && !pts) ||
+      (face_capacity > 0 && !faces) || std::isnan(min_weight) ||
+      (dev && (reinterpret_cast<uintptr_t>(pts) % sizeof(float) || reinterpret_cast<uintptr_t>(faces) % 4)))
+    return fail(ctx, OFDIS_ERR_ARG, "fuse_mesh: bad argument");
+  NvtxRange nvtx("fuse", -1);
+  CK(cudaSetDevice(ctx->device));
+  const FuseGeom& g = ctx->fuse_geom;
+  const size_t N = (size_t)g.count, nb = (N + FUSE_BLOCK - 1) / FUSE_BLOCK, b_v = align16(4 * N);
+  const size_t bytes = b_v + 8 * (nb + 1);
+  if (bytes > ctx->mesh_bytes) {
+    CK(cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_mesh);
+    ctx->d_mesh = nullptr;
+    ctx->mesh_bytes = 0;
+    if (cudaMalloc(&ctx->d_mesh, bytes) != cudaSuccess) {
+      ctx->d_mesh = nullptr;
+      return fail(ctx, OFDIS_ERR_NOMEM, "fuse_mesh workspace");
+    }
+    ctx->mesh_bytes = bytes;
+  }
+  FuseMeshWork mw;
+  mw.vbase = static_cast<unsigned int*>(ctx->d_mesh);
+  mw.bsum = reinterpret_cast<unsigned long long*>(static_cast<char*>(ctx->d_mesh) + b_v);
+  mw.total = mw.bsum + nb;
+  int k = launch_fuse_count(g, ctx->fuse_vol, min_weight, ctx->fuse_ws, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_count_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  k = launch_fuse_cube_count(g, ctx->fuse_vol, min_weight, mw, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_cube_count_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  unsigned long long total[2] = {0, 0};  // vertices, triangles
+  ofdis_fuse_point* out = pts;
+  unsigned int* fout = faces;
+  long long pcap = pt_capacity, fcap = face_capacity;
+  if (!dev) {
+    // the totals decide how much of the full-resolution scratch the host outputs need: the points, then the faces
+    CK(cudaMemcpyAsync(&total[0], ctx->fuse_ws.total, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(&total[1], mw.total, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    pcap = (long long)std::min<unsigned long long>(total[0], (unsigned long long)pt_capacity);
+    fcap = (long long)std::min<unsigned long long>(total[1], (unsigned long long)face_capacity);
+    const size_t b_p = align16(sizeof(ofdis_fuse_point) * (size_t)pcap);
+    if (pcap > 0 || fcap > 0) {
+      const int rc = ensure_full(ctx, (b_p + 12 * (size_t)fcap + 3) / sizeof(float));
+      if (rc) return rc;
+    }
+    out = reinterpret_cast<ofdis_fuse_point*>(ctx->d_full);
+    fout = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(ctx->d_full) + b_p);
+  }
+  k = launch_fuse_write(g, ctx->fuse_vol, min_weight, ctx->fuse_ws, out, pcap, ctx->stream, mw.vbase);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_write_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  k = launch_fuse_faces(g, ctx->fuse_vol, min_weight, mw, fout, fcap, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_face_kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  if (!dev && pcap > 0)
+    CK(cudaMemcpyAsync(pts, out, sizeof(ofdis_fuse_point) * (size_t)pcap, cudaMemcpyDeviceToHost, ctx->stream));
+  if (!dev && fcap > 0)
+    CK(cudaMemcpyAsync(faces, fout, 12 * (size_t)fcap, cudaMemcpyDeviceToHost, ctx->stream));
+  if (dev) {
+    CK(cudaMemcpyAsync(&total[0], ctx->fuse_ws.total, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(&total[1], mw.total, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  CK(cudaStreamSynchronize(ctx->stream));
+  *pt_count = (long)total[0];
+  *face_count = (long)total[1];
+  return OFDIS_OK;
+}
+
+int ofdis_fuse_set_volume(ofdis_ctx* ctx, const float* T, const float* W, const unsigned char* color, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_set_volume: no live volume (ofdis_fuse_begin)");
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  const FuseVolume& v = ctx->fuse_vol;
+  if ((color && !v.C) || (dev && (reinterpret_cast<uintptr_t>(T) % 4 || reinterpret_cast<uintptr_t>(W) % 4)))
+    return fail(ctx, OFDIS_ERR_ARG, "fuse_set_volume: bad argument");
+  CK(cudaSetDevice(ctx->device));
+  const size_t N = (size_t)ctx->fuse_geom.count;
+  const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  if (T) CK(cudaMemcpyAsync(v.T, T, 4 * N, kind, ctx->stream));
+  if (W) CK(cudaMemcpyAsync(v.W, W, 4 * N, kind, ctx->stream));
+  if (color) CK(cudaMemcpyAsync(v.C, color, 3 * N, kind, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   return OFDIS_OK;
 }

@@ -700,6 +700,41 @@ int main(int argc, char** argv) {
 // `FUSE clip C frames F points P`.  Refused before any device work: --fuse without --odometry, the stereo binaries,
 // --warm-start and a spec that is not 8 numbers with voxel and trunc > 0, sizes >= 1 and at most 2^30 voxels.  Every
 // other output keeps its bytes.
+//
+// --mesh (with --fuse): at each clip's end also DIR/fused_<clip %04d>_mesh.ply, the same volume's triangle mesh of
+// weight >= 1 (ofdis_fuse_mesh): the vertices of fused_<clip>.ply, then `element face F` with `property list uchar uint
+// vertex_indices` (preprocess.fuse_mesh, preprocess.write_fused_mesh_ply).  With verbosity > 0 every clip prints
+// `MESH clip C vertices V faces F`.  Refused before any device work: --mesh without --fuse, and whatever --fuse
+// refuses.  Every other output keeps its bytes.
+
+// The fused points (with mesh, the mesh) as a binary little-endian PLY: float x, y, z, nx, ny, nz and uchar red,
+// green, blue per vertex, then with mesh nf faces of uchar 3 and three uint vertex indices.  False when it cannot be
+// written.
+static bool write_fused_ply(const string& path, const ofdis_fuse_point* pts, long count, int nochannels, bool mesh,
+                            const unsigned int* faces, long nf) {
+  FILE* pf = fopen(path.c_str(), "wb");
+  if (!pf) return false;
+  fprintf(pf, "ply\nformat binary_little_endian 1.0\nelement vertex %ld\nproperty float x\nproperty float y\n"
+              "property float z\nproperty float nx\nproperty float ny\nproperty float nz\nproperty uchar red\n"
+              "property uchar green\nproperty uchar blue\n", count);
+  if (mesh) fprintf(pf, "element face %ld\nproperty list uchar uint vertex_indices\n", nf);
+  fprintf(pf, "end_header\n");
+  vector<uint8_t> buf((size_t)27 * count + (mesh ? (size_t)13 * nf : 0));
+  for (long i = 0; i < count; ++i) {
+    const ofdis_fuse_point& q = pts[i];
+    memcpy(&buf[(size_t)27 * i], &q.x, 24);
+    // the decoder's BGR: channel 2 is red (gray: all three equal)
+    const uint8_t rgb[3] = {nochannels == 3 ? q.b : q.r, q.g, nochannels == 3 ? q.r : q.b};
+    memcpy(&buf[(size_t)27 * i + 24], rgb, 3);
+  }
+  for (long i = 0; mesh && i < nf; ++i) {
+    uint8_t* f = &buf[(size_t)27 * count + (size_t)13 * i];
+    f[0] = 3;
+    memcpy(f + 1, faces + (size_t)3 * i, 12);
+  }
+  bool wrote = fwrite(buf.data(), 1, buf.size(), pf) == buf.size();
+  return fclose(pf) == 0 && wrote;
+}
 
 // Rigid poses as 12 doubles, row-major [R | t].  T <- T inv(P): the next camera-to-world pose of a clip (KITTI's
 // odometry convention) from the relative pose P, camera t to camera t+1.
@@ -1051,7 +1086,7 @@ int main(int argc, char** argv) {
             "       [--lr-check] [--speckle N R] [--fill] [--camera fx,fy,cx,cy,baseline,doffs]\n"
             "       [--global-motion similarity|affine|homography PATH [--stabilize RADIUS CROP DIR]]\n"
             "       [--scene-flow DISPLIST [--gt-scene-flow GTLIST]]\n"
-            "       [--odometry DIR [--gt-poses LIST] [--fuse voxel,trunc,x0,y0,z0,nx,ny,nz]]\n"
+            "       [--odometry DIR [--gt-poses LIST] [--fuse voxel,trunc,x0,y0,z0,nx,ny,nz [--mesh]]]\n"
             "       [oppoint | 20 parameters (README.md:66-88)]\n"
             "  --warm-start: latency mode for video, one pair per launch; a pair whose image1 is the previous pair's\n"
             "  image2 starts from that pair's flow (the reference's init flow); a clip then runs serially\n"
@@ -1094,7 +1129,8 @@ int main(int argc, char** argv) {
             "  <stem>_objmotion.pfm; --gt-poses LIST: one KITTI poses file per clip, ODOEVAL lines; not with --warm-start\n"
             "  --fuse voxel,trunc,x0,y0,z0,nx,ny,nz (flow binaries, with --odometry): every clip's disparities fused\n"
             "  into a TSDF volume of nx x ny x nz voxels from (x0, y0, z0), its surface points to DIR/fused_<clip>.ply;\n"
-            "  not with --warm-start\n",
+            "  not with --warm-start\n"
+            "  --mesh (with --fuse): also the volume's triangle mesh to DIR/fused_<clip>_mesh.ply\n",
             argv[0]);
     return 2;
   }
@@ -1118,6 +1154,7 @@ int main(int argc, char** argv) {
   const char* odo_dir = nullptr;     // --odometry DIR
   const char* odo_gtlist = nullptr;  // --gt-poses LIST
   const char* fuse_arg = nullptr;    // --fuse voxel,trunc,x0,y0,z0,nx,ny,nz
+  bool fuse_mesh = false;            // --mesh
   for (;;) {
     if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
       maxb = atoi(argv[first_num + 1]);
@@ -1237,6 +1274,9 @@ int main(int argc, char** argv) {
       }
       fuse_arg = argv[first_num + 1];
       first_num += 2;
+    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--mesh")) {
+      fuse_mesh = true;
+      first_num += 1;
     } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt-poses")) {
       if (argc < first_num + 2 || odo_gtlist) {
         fprintf(stderr, "error: --gt-poses takes one list of KITTI poses files\n");
@@ -1309,6 +1349,10 @@ int main(int argc, char** argv) {
   }
   if (fuse_arg && !odo_dir) {
     fprintf(stderr, "error: --fuse places disparities with the poses of --odometry; give --odometry too\n");
+    return 2;
+  }
+  if (fuse_mesh && !fuse_arg) {
+    fprintf(stderr, "error: --mesh meshes the volume of --fuse; give --fuse too\n");
     return 2;
   }
   ofdis_fuse_params fuse_p;
@@ -1674,6 +1718,7 @@ int main(int argc, char** argv) {
   int fuse_frames = 0;            // frames pushed into the clip's volume
   vector<double> fuse_poses;
   vector<ofdis_fuse_point> fuse_pts;
+  vector<unsigned int> fuse_faces;  // --mesh
   // --descriptors, --fisher: every pair's frames hold an N x N patch, checked before any device work
   for (size_t k = 0; k < jobs.size() && traj_stage; ++k) {
     int iw = 0, ih = 0;
@@ -2265,30 +2310,29 @@ int main(int argc, char** argv) {
         if (rc != OFDIS_OK) break;
         char name[32];
         snprintf(name, sizeof(name), "/fused_%04d.ply", c);
-        const string path = string(odo_dir) + name;
-        FILE* pf = fopen(path.c_str(), "wb");
-        bool wrote = pf != nullptr;
-        if (pf) {
-          fprintf(pf, "ply\nformat binary_little_endian 1.0\nelement vertex %ld\nproperty float x\nproperty float y\n"
-                      "property float z\nproperty float nx\nproperty float ny\nproperty float nz\nproperty uchar red\n"
-                      "property uchar green\nproperty uchar blue\nend_header\n", count);
-          vector<uint8_t> buf((size_t)27 * count);
-          for (long i = 0; i < count; ++i) {
-            const ofdis_fuse_point& q = fuse_pts[i];
-            memcpy(&buf[(size_t)27 * i], &q.x, 24);
-            // the decoder's BGR: channel 2 is red (gray: all three equal)
-            const uint8_t rgb[3] = {nochannels == 3 ? q.b : q.r, q.g, nochannels == 3 ? q.r : q.b};
-            memcpy(&buf[(size_t)27 * i + 24], rgb, 3);
-          }
-          wrote = fwrite(buf.data(), 1, buf.size(), pf) == buf.size();
-          wrote = fclose(pf) == 0 && wrote;
-        }
-        if (!wrote) {
+        string path = string(odo_dir) + name;
+        if (!write_fused_ply(path, fuse_pts.data(), count, nochannels, false, nullptr, 0)) {
           fprintf(stderr, "error: cannot write %s\n", path.c_str());
           ofdis_destroy(ctx);
           return 1;
         }
         if (verbosity > 0) printf("FUSE clip %d frames %d points %ld\n", c, fuse_frames, count);
+        if (!fuse_mesh) continue;
+        // the mesh's vertices are the points just extracted: only the faces come back
+        long nv = 0, nf = 0;
+        rc = ofdis_fuse_mesh(ctx, 1.0f, nullptr, 0, &nv, nullptr, 0, &nf, OFDIS_MEM_HOST);
+        if (rc != OFDIS_OK) break;
+        fuse_faces.resize((size_t)3 * nf);
+        rc = ofdis_fuse_mesh(ctx, 1.0f, nullptr, 0, &nv, fuse_faces.data(), nf, &nf, OFDIS_MEM_HOST);
+        if (rc != OFDIS_OK) break;
+        snprintf(name, sizeof(name), "/fused_%04d_mesh.ply", c);
+        path = string(odo_dir) + name;
+        if (!write_fused_ply(path, fuse_pts.data(), count, nochannels, true, fuse_faces.data(), nf)) {
+          fprintf(stderr, "error: cannot write %s\n", path.c_str());
+          ofdis_destroy(ctx);
+          return 1;
+        }
+        if (verbosity > 0) printf("MESH clip %d vertices %ld faces %ld\n", c, nv, nf);
       }
     }
     if (rc != OFDIS_OK) {

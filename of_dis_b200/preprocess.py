@@ -13,6 +13,7 @@ when it is importable.
 """
 from __future__ import annotations
 
+import functools
 import math
 
 import numpy as np
@@ -1813,12 +1814,9 @@ def fuse_integrate(vol: dict, params, disp, poses, camera, max_depth=np.inf, fra
     return vol
 
 
-def fuse_extract(vol: dict, params, min_weight) -> np.ndarray:
-    """Restates ofdis_fuse_extract: every zero crossing of vol as a FUSE_POINT_DTYPE array, in the header's order."""
-    T, Wt, C = vol["T"], vol["W"], vol["C"]
-    nz, ny, nx = T.shape
-    mw = f32(min_weight)
-    good = (Wt >= mw) & (np.abs(T) < f32(1))
+def _fuse_crossings(T, Wt, min_weight):
+    """The crossings of ofdis_fuse_extract in its order, as keys voxel * 3 + axis, and the per-voxel test."""
+    good = (Wt >= f32(min_weight)) & (np.abs(T) < f32(1))
     pos = T > 0
     parts = []
     for e, ax in ((0, 2), (1, 1), (2, 0)):
@@ -1828,7 +1826,14 @@ def fuse_extract(vol: dict, params, min_weight) -> np.ndarray:
         a[ax], b[ax] = slice(0, -1), slice(1, None)
         m[tuple(a)] = good[tuple(a)] & good[tuple(b)] & (pos[tuple(a)] != pos[tuple(b)])
         parts.append(np.flatnonzero(m) * 3 + e)
-    idx = np.sort(np.concatenate(parts))
+    return np.sort(np.concatenate(parts)), good
+
+
+def fuse_extract(vol: dict, params, min_weight) -> np.ndarray:
+    """Restates ofdis_fuse_extract: every zero crossing of vol as a FUSE_POINT_DTYPE array, in the header's order."""
+    T, Wt, C = vol["T"], vol["W"], vol["C"]
+    nz, ny, nx = T.shape
+    idx, _ = _fuse_crossings(T, Wt, min_weight)
     a, e = idx // 3, idx % 3
     i, j, k = a % nx, (a // nx) % ny, a // (nx * ny)
     step = np.array([1, nx, nx * ny])[e]
@@ -1923,6 +1928,160 @@ def write_fused_ply(path: str, pts) -> None:
                  "property float z\nproperty float nx\nproperty float ny\nproperty float nz\nproperty uchar red\n"
                  "property uchar green\nproperty uchar blue\nend_header\n" % len(pts)).encode())
         f.write(rec.tobytes())
+
+
+# ---- marching cubes of the fused volume (ofdis_fuse_mesh) -------------------------------------------------------------
+def fuse_mc_edge(n: int):
+    """Cube edge n = 4*axis + r of the header: (lower corner q, axis); q is r with a 0 bit inserted at bit `axis`."""
+    axis, r = n >> 2, n & 3
+    return (r & ((1 << axis) - 1)) | ((r >> axis) << (axis + 1)), axis
+
+
+def _mc_loops(case: int):
+    """The oriented loops of one case: lists of edge numbers, each starting at its lowest edge."""
+    pos = [(case >> q) & 1 for q in range(8)]
+    xyz = [np.array([q & 1, (q >> 1) & 1, q >> 2], float) for q in range(8)]
+    edges = [fuse_mc_edge(n) for n in range(12)]
+    mid = [(xyz[q] + xyz[q | (1 << ax)]) / 2 for q, ax in edges]
+    nxt = {}
+    for f in range(3):
+        u, v = [a for a in range(3) if a != f]
+        for side in (0, 1):
+            nf = np.zeros(3)
+            nf[f] = 1.0 if side else -1.0
+            ring = [(side << f) | (a << u) | (b << v) for a, b in ((0, 0), (1, 0), (1, 1), (0, 1))]
+            # the face edge between ring[m] and ring[m + 1]
+            fe = []
+            for m in range(4):
+                a, b = ring[m], ring[(m + 1) % 4]
+                fe.append(next(n for n, (q, ax) in enumerate(edges) if {q, q | (1 << ax)} == {a, b}))
+            s = [pos[c] for c in ring]
+            cross = [m for m in range(4) if s[m] != s[(m + 1) % 4]]
+            if not cross:
+                continue
+            if len(cross) == 4:
+                # ambiguous: a segment cuts off each T > 0 corner (its two face edges: m - 1 and m)
+                segs = [((m - 1) % 4, m, xyz[ring[m]] - (xyz[ring[0]] + xyz[ring[2]]) / 2) for m in range(4) if s[m]]
+            else:
+                p = np.mean([xyz[c] for c in ring if pos[c]], 0) - np.mean([xyz[c] for c in ring if not pos[c]], 0)
+                segs = [(cross[0], cross[1], p)]
+            for ma, mb, p in segs:
+                a, b = fe[ma], fe[mb]
+                # with the patch's normal towards T > 0, its boundary runs along p x nf on this face
+                if np.dot(mid[b] - mid[a], np.cross(p, nf)) < 0:
+                    a, b = b, a
+                assert a not in nxt
+                nxt[a] = b
+    loops, seen = [], set()
+    for n in sorted(nxt):
+        if n in seen:
+            continue
+        loop = [n]
+        while nxt[loop[-1]] != n:
+            loop.append(nxt[loop[-1]])
+        seen.update(loop)
+        loops.append(loop)
+    return loops
+
+
+def _mc_triangulations(lo: int, hi: int):
+    """Triangulations of the polygon lo..hi (loop positions) in the header's enumeration: the triangle on side
+    (lo, hi) with apex k ascending, then the polygon lo..k, then k..hi."""
+    if hi - lo < 2:
+        yield []
+        return
+    for k in range(lo + 1, hi):
+        for left in _mc_triangulations(lo, k):
+            for right in _mc_triangulations(k, hi):
+                yield [(lo, k, hi)] + left + right
+
+
+def _mc_faces(n: int):
+    q, ax = fuse_mc_edge(n)
+    return {(f, (q >> f) & 1) for f in range(3) if f != ax}
+
+
+@functools.lru_cache(maxsize=None)
+def _mc_table_cached() -> bytes:
+    tab = np.full((256, 16), 255, np.uint8)
+    for case in range(256):
+        tris = []
+        for loop in _mc_loops(case):
+            L = len(loop)
+            for tri in _mc_triangulations(0, L - 1):
+                sides = {tuple(sorted((t[a], t[b]))) for t in tri for a, b in ((0, 1), (1, 2), (0, 2))}
+                diag = [(a, b) for a, b in sides if b - a not in (1, L - 1)]
+                if all(not (_mc_faces(loop[a]) & _mc_faces(loop[b])) for a, b in diag):
+                    tris += [[loop[a] for a in t] for t in tri]
+                    break
+            else:
+                raise AssertionError("case %d: a loop without a valid triangulation" % case)
+        tab[case, 0] = len(tris)
+        tab[case, 1:1 + 3 * len(tris)] = np.asarray(tris, np.uint8).ravel()
+    return tab.tobytes()
+
+
+def fuse_mc_table() -> np.ndarray:
+    """The marching-cubes table of ofdis_fuse_mesh, generated from the header's rules: (256, 16) uint8, row = case,
+    [0] the triangles, [1 + 3t + s] the edge of triangle t's vertex s, 255 past the last."""
+    return np.frombuffer(_mc_table_cached(), np.uint8).reshape(256, 16).copy()
+
+
+def fuse_mesh(vol: dict, params, min_weight):
+    """Restates ofdis_fuse_mesh: (points, faces) with points = fuse_extract(vol, params, min_weight) and faces (F, 3)
+    uint32 vertex indices, meshed cubes in ascending voxel index of corner 0 and each cube's triangles in table order."""
+    pts = fuse_extract(vol, params, min_weight)
+    T = vol["T"]
+    nz, ny, nx = T.shape
+    idx, good = _fuse_crossings(T, vol["W"], min_weight)
+    pos = T > 0
+    # the vertex of crossing (voxel a, axis e) is its position in fuse_extract's order
+    key = np.full(T.size * 3, -1, np.int64)
+    key[idx] = np.arange(len(idx))
+    if nx < 2 or ny < 2 or nz < 2:
+        return pts, np.zeros((0, 3), np.uint32)
+    sl = [(slice(dk, nz - 1 + dk), slice(dj, ny - 1 + dj), slice(di, nx - 1 + di))
+          for q in range(8) for di, dj, dk in [(q & 1, (q >> 1) & 1, q >> 2)]]
+    meshed = np.ones((nz - 1, ny - 1, nx - 1), bool)
+    case = np.zeros((nz - 1, ny - 1, nx - 1), np.int64)
+    for q in range(8):
+        meshed &= good[sl[q]]
+        case |= pos[sl[q]].astype(np.int64) << q
+    kk, jj, ii = np.nonzero(meshed)  # C order: ascending voxel index
+    case = case[kk, jj, ii]
+    tab = fuse_mc_table().astype(np.int64)
+    ntri = tab[case, 0]
+    cube = np.repeat(np.arange(len(case)), ntri)
+    t = np.arange(len(cube)) - np.repeat(np.cumsum(ntri) - ntri, ntri)
+    a0 = ((kk * ny + jj) * nx + ii)[cube]
+    faces = np.empty((len(cube), 3), np.int64)
+    for s in range(3):
+        edge = tab[case[cube], 1 + 3 * t + s]
+        q, e = (edge & 3), edge >> 2
+        q = (q & ((1 << e) - 1)) | ((q >> e) << (e + 1))
+        aq = a0 + (q & 1) + ((q >> 1) & 1) * nx + (q >> 2) * (nx * ny)
+        faces[:, s] = key[aq * 3 + e]
+    assert (faces >= 0).all()
+    return pts, faces.astype(np.uint32)
+
+
+def write_fused_mesh_ply(path: str, pts, faces) -> None:
+    """The mesh as a binary little-endian PLY: the vertices of write_fused_ply, then `element face F` with
+    `property list uchar uint vertex_indices` -- the file of the batch command's --mesh."""
+    pts = np.asarray(pts, FUSE_POINT_DTYPE)
+    faces = np.asarray(faces, np.uint32).reshape(-1, 3)
+    rec = np.empty(len(pts), [("p", "<f4", (6,)), ("c", "u1", (3,))])
+    rec["p"] = np.stack([pts[k] for k in ("x", "y", "z", "nx", "ny", "nz")], -1) if len(pts) else np.zeros((0, 6))
+    rec["c"] = np.stack([pts[k] for k in ("r", "g", "b")], -1) if len(pts) else np.zeros((0, 3))
+    frec = np.empty(len(faces), [("n", "u1"), ("v", "<u4", (3,))])
+    frec["n"], frec["v"] = 3, faces
+    with open(path, "wb") as f:
+        f.write(("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\n"
+                 "property float z\nproperty float nx\nproperty float ny\nproperty float nz\nproperty uchar red\n"
+                 "property uchar green\nproperty uchar blue\nelement face %d\nproperty list uchar uint vertex_indices\n"
+                 "end_header\n" % (len(pts), len(faces))).encode())
+        f.write(rec.tobytes())
+        f.write(frec.tobytes())
 
 
 # ---- video stabilisation (ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish) ---------------------------------

@@ -9,13 +9,15 @@ disparity (union-find speckles, fill, depth and xyz) and a global motion (corres
 the bulk-copied score tiles with and without refills, refits, per-pixel outputs), a stereo ego-motion (the same
 stages on 32-byte correspondences, non-finite disparities, score tile refills), a Fisher encoding (projection,
 posteriors, float64 statistics, the take) and a TSDF fusion (integration, crossing count, scan and write, ray casting)
-checked against their restatements.  Results are checked against the
+and its marching cubes (set_volume, the write with vertex bases, cube count, scan, faces) checked against their
+restatements.  Results are checked against the
 oracle so that a clean log means a correct run."""
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
+import torch
 
 from of_dis_b200 import api, params, preprocess, synth
 from oracle import port_driver
@@ -231,6 +233,36 @@ ok = all(np.array_equal(gv[k].view(np.uint8), ev[k].view(np.uint8)) for k in ("T
     np.array_equal(gp.view(np.uint8), preprocess.fuse_extract(ev, fp, 1.0).view(np.uint8)) and \
     np.array_equal(gd.view(np.uint8), preprocess.fuse_render(ev, fp, poses, cam, 0.3, 2.5, 0.03, 1.0, w3, h3).view(np.uint8))
 print("%-22s %s" % ("fuse", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# marching cubes: a 23 x 29 x 41 volume (cubes straddling scan blocks) loaded with fuse_set_volume, T uniform with
+# planted +0, -0, +-1, nextafter(1, 0) and NaN, W at, just below and above min_weight and NaN; host output at full
+# capacity and device output at capacities one short of the totals
+mp = dict(nx=23, ny=29, nz=41, origin=(-0.5, -0.5, 0.5), voxel=0.05, trunc=0.15, max_weight=8.0, color=1)
+shape = (mp["nz"], mp["ny"], mp["nx"])
+below1 = np.nextafter(np.float32(1), np.float32(0))
+mv = preprocess.fuse_new_volume(mp)
+mv["T"][:] = rng.uniform(-1.2, 1.2, shape).astype(np.float32)
+mv["W"][:] = rng.choice(np.array([1.0, 2.0, 3.0], np.float32), shape)
+for v, share in ((0.0, 0.05), (-0.0, 0.05), (1.0, 0.02), (-1.0, 0.02), (below1, 0.02), (np.nan, 0.01)):
+    mv["T"][rng.random(shape) < share] = np.float32(v)
+for v, share in ((0.0, 0.02), (below1, 0.02), (np.nan, 0.01)):
+    mv["W"][rng.random(shape) < share] = np.float32(v)
+mv["C"][:] = rng.integers(0, 256, shape + (3,))
+ctx = api.Context(prm, w3, h3, prm.p_samp_s, 2)
+ctx.fuse_begin(mp)
+ctx.fuse_set_volume(mv["T"], mv["W"], mv["C"])
+hp, hf, nv, nf = ctx.fuse_mesh(1.0)
+dp = torch.zeros(28 * nv, dtype=torch.uint8, device="cuda")
+df = torch.zeros(3 * nf, dtype=torch.int32, device="cuda")
+ctx.fuse_mesh(1.0, pt_capacity=nv - 1, face_capacity=nf - 1, memkind=api.MEM_DEVICE, pts_out=dp.data_ptr(),
+              faces_out=df.data_ptr())
+ctx.close()
+ep, ef = preprocess.fuse_mesh(mv, mp, 1.0)
+ok = nf > 100 and np.array_equal(hp.view(np.uint8), ep.view(np.uint8)) and np.array_equal(hf, ef) and \
+    np.array_equal(dp.cpu().numpy()[:28 * (nv - 1)], ep[:nv - 1].view(np.uint8)) and \
+    np.array_equal(df.cpu().numpy()[:3 * (nf - 1)].view(np.uint32), ef[:nf - 1].ravel())
+print("%-22s %s" % ("fuse_mesh", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
