@@ -14,6 +14,7 @@
 #include <zlib.h>
 
 #include <cfloat>
+#include <cstdarg>
 #include <climits>
 #include <cmath>
 #include <cstdint>
@@ -22,6 +23,7 @@
 #include <cstring>
 #include <iostream>
 #include <limits>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -1077,6 +1079,1322 @@ static bool read_fisher_book(const char* path, FisherBook& fb, string& err) {
   return true;
 }
 
+// One refusal line on stderr, "error: " and the formatted message; returns `code`, the exit code.
+static __attribute__((format(printf, 2, 3))) int refuse(int code, const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  fputs("error: ", stderr);
+  vfprintf(stderr, fmt, ap);
+  fputc('\n', stderr);
+  va_end(ap);
+  return code;
+}
+
+// A whitespace-separated list file (the list file, --gt, --scene-flow, --gt-scene-flow, --gt-poses): its words
+static bool read_words(const char* path, vector<string>& words) {
+  FILE* f = fopen(path, "r");
+  if (!f) return false;
+  char g[4096];
+  while (fscanf(f, "%4095s", g) == 1) words.push_back(g);
+  fclose(f);
+  return true;
+}
+
+// The decoder's BGR order as RGB: `im` itself for gray, else `buf` holding the converted copy
+static const uint8_t* as_rgb(const uint8_t* im, size_t hwc, int nochannels, vector<uint8_t>& buf) {
+  if (nochannels != 3) return im;
+  buf.resize(hwc);
+  for (size_t q = 0; q < hwc; q += 3) {
+    buf[q] = im[q + 2];
+    buf[q + 1] = im[q + 1];
+    buf[q + 2] = im[q];
+  }
+  return buf.data();
+}
+
+// KITTI's 16-bit disparity PNG of positive disparities: d * 256 clamped to [1, 65535], 0 where d is negative or NaN
+static void save_kitti_disp(const float* d, int w, int h, const string& path) {
+  vector<uint16_t> enc((size_t)w * h);
+  for (size_t i = 0; i < enc.size(); ++i)  // NaN fails d >= 0 and is written as 0
+    enc[i] = d[i] >= 0.0f ? (uint16_t)fminf(fmaxf(d[i] * 256.0f, 1.0f), 65535.0f) : (uint16_t)0;
+  save_png(enc.data(), w, h, 1, 16, path.c_str());
+}
+
+// KITTI's 16-bit flow PNG, the encoding of OFDIS_ENC_KITTI: (u * 64 + 2^15, v * 64 + 2^15, 1), (0, 0, 0) where NaN
+static void save_kitti_flow(const float* f, int w, int h, const string& path) {
+  vector<uint16_t> enc((size_t)3 * w * h);
+  for (size_t i = 0; i < (size_t)w * h; ++i) {
+    const float u = f[2 * i], v = f[2 * i + 1];
+    const bool valid = !std::isnan(u) && !std::isnan(v);
+    enc[3 * i] = valid ? (uint16_t)fminf(fmaxf(u * 64.0f + 32768.0f, 0.0f), 65535.0f) : (uint16_t)0;
+    enc[3 * i + 1] = valid ? (uint16_t)fminf(fmaxf(v * 64.0f + 32768.0f, 0.0f), 65535.0f) : (uint16_t)0;
+    enc[3 * i + 2] = valid ? 1 : 0;
+  }
+  save_png(enc.data(), w, h, 3, 16, path.c_str());
+}
+
+// A 1-channel PFM holding v as it is (a positive disparity, a depth): SavePFMFile writes -value, so v goes in negated
+static void save_pfm1(const float* v, int w, int h, const string& path) {
+  ImageF f;
+  f.w = w;
+  f.h = h;
+  f.c = 1;
+  f.px.resize((size_t)w * h);
+  for (size_t i = 0; i < f.px.size(); ++i) f.px[i] = -v[i];
+  SavePFMFile(f, path.c_str());
+}
+
+// Wang and Schmid's trajectory settings (--descriptors, --fisher)
+static ofdis_traj_params traj_settings() {
+  ofdis_traj_params trp;
+  memset(&trp, 0, sizeof(trp));
+  trp.L = 15;
+  trp.nt = 3;
+  trp.N = 32;
+  trp.ns = 2;
+  trp.min_flow = 0.4f;
+  trp.eps = 0.05f;
+  trp.min_disp = 1.0f;
+  trp.min_var = (float)std::sqrt(3.0);
+  trp.max_var = 50.0f;
+  trp.max_dis = 20.0f;
+  return trp;
+}
+
+// Every flag's value as given, then what the checks read from them
+struct Options {
+  const char* batch = nullptr;  // --batch N: the last one given
+  bool warm = false, bidir = false, kitti = false, color = false, lr_check = false, fill = false, mesh = false;
+  const char* color_max_arg = nullptr;                // --color-max M
+  const char* interp_arg = nullptr;                   // --interpolate T
+  const char* gtlist = nullptr;                       // --gt gtlist
+  const char* tracks = nullptr;                       // --tracks PATH
+  const char* desc = nullptr;                         // --descriptors PATH
+  const char* fisher[2] = {nullptr, nullptr};         // --fisher CODEBOOK PATH
+  const char* speckle[2] = {nullptr, nullptr};        // --speckle N R
+  const char* camera = nullptr;                       // --camera fx,fy,cx,cy,baseline,doffs
+  const char* gm[2] = {nullptr, nullptr};             // --global-motion MODEL PATH
+  const char* stab[3] = {nullptr, nullptr, nullptr};  // --stabilize RADIUS CROP DIR
+  const char* sf_list = nullptr;                      // --scene-flow DISPLIST
+  const char* sf_gtlist = nullptr;                    // --gt-scene-flow GTLIST
+  const char* odo_dir = nullptr;                      // --odometry DIR
+  const char* odo_gtlist = nullptr;                   // --gt-poses LIST
+  const char* fuse = nullptr;                         // --fuse voxel,trunc,x0,y0,z0,nx,ny,nz
+  int nnum = 0;                                       // the operating point or the 20 parameters after the flags
+  char** nums = nullptr;
+
+  int maxb = 64;
+  float color_max = 0.0f;   // 0: every pair's own maximum
+  float interp_t = 0.0f;
+  int gm_model = 0;         // OFDIS_MOTION_*
+  bool disp_on = false;     // filtered disparities (stereo binaries)
+  bool traj_stage = false;  // the descriptor stage runs in place of the tracker's calls
+  bool two_way = false;     // the backward slots run
+  ofdis_fuse_params fuse_p{};
+  ofdis_traj_params trp = traj_settings();
+  int tdim = 2 * trp.L + trp.ns * trp.ns * trp.nt * 33;  // floats per descriptor
+  FisherBook fbook;  // --fisher: the codebook, whose blocks must be the descriptors' (shape, HOG, HOF, MBHx, MBHy)
+  int fv_floats = 0;
+  ofdis_stab_params stp{};
+  vector<double> stab_wts;
+  ofdis_disp_filter dfilt{};
+  ofdis_stereo_camera dcam{};
+};
+
+// The flags, read from argv[2] on until the first word that is none of them.  An argument-taking flag without its
+// arguments, or given twice, is refused with what it takes; a switch may repeat.  --batch is the exception: a repeat
+// keeps the last value, and a trailing --batch without one ends the flags (it is then read as the operating point).
+static int parse_flags(int argc, char** argv, Options& o) {
+  struct Flag {
+    const char* name;
+    int nargs;
+    const char** dest;  // its nargs values
+    bool* on;           // a switch
+    const char* takes;  // nullptr: --batch
+  };
+  const Flag flags[] = {
+      {"--batch", 1, &o.batch, nullptr, nullptr},
+      {"--warm-start", 0, nullptr, &o.warm, nullptr},
+      {"--bidirectional", 0, nullptr, &o.bidir, nullptr},
+      {"--kitti", 0, nullptr, &o.kitti, nullptr},
+      {"--color", 0, nullptr, &o.color, nullptr},
+      {"--color-max", 1, &o.color_max_arg, nullptr, "one positive number"},
+      {"--interpolate", 1, &o.interp_arg, nullptr, "one time between 0 and 1"},
+      {"--tracks", 1, &o.tracks, nullptr, "one output path"},
+      {"--descriptors", 1, &o.desc, nullptr, "one output path"},
+      {"--fisher", 2, o.fisher, nullptr, "a codebook file and an output path"},
+      {"--lr-check", 0, nullptr, &o.lr_check, nullptr},
+      {"--fill", 0, nullptr, &o.fill, nullptr},
+      {"--speckle", 2, o.speckle, nullptr, "a size N and a difference R"},
+      {"--camera", 1, &o.camera, nullptr, "fx,fy,cx,cy,baseline,doffs"},
+      {"--global-motion", 2, o.gm, nullptr, "a model (similarity, affine or homography) and an output path"},
+      {"--stabilize", 3, o.stab, nullptr, "a radius, a crop and an output directory"},
+      {"--scene-flow", 1, &o.sf_list, nullptr, "one disparity list file"},
+      {"--gt-scene-flow", 1, &o.sf_gtlist, nullptr, "one ground-truth list file"},
+      {"--odometry", 1, &o.odo_dir, nullptr, "one output directory"},
+      {"--fuse", 1, &o.fuse, nullptr, "voxel,trunc,x0,y0,z0,nx,ny,nz"},
+      {"--mesh", 0, nullptr, &o.mesh, nullptr},
+      {"--gt-poses", 1, &o.odo_gtlist, nullptr, "one list of KITTI poses files"},
+      {"--gt", 1, &o.gtlist, nullptr, "one ground-truth list file"},
+  };
+  int i = 2;
+  while (i < argc) {
+    const Flag* f = nullptr;
+    for (const Flag& g : flags)
+      if (!strcmp(argv[i], g.name)) f = &g;
+    if (!f) break;
+    const bool missing = i + f->nargs >= argc;
+    if (!f->takes && missing) break;
+    if (f->takes && (missing || f->dest[0])) return refuse(2, "%s takes %s", f->name, f->takes);
+    if (f->on) *f->on = true;
+    for (int a = 0; a < f->nargs; ++a) f->dest[a] = argv[i + 1 + a];
+    i += 1 + f->nargs;
+  }
+  o.nnum = argc - i;
+  o.nums = argv + i;
+  return 0;
+}
+
+// The value readers of the flags that take numbers, a model or a codebook: each refuses a bad value
+static int read_fuse(Options& o) {
+  double v[8];
+  const char* q = o.fuse;
+  bool ok = true;
+  for (int i = 0; i < 8 && ok; ++i) {
+    char* end = nullptr;
+    v[i] = strtod(q, &end);
+    ok = end != q && (i < 7 ? *end == ',' : *end == 0) && std::isfinite(v[i]);
+    q = end + (i < 7 ? 1 : 0);
+  }
+  for (int i = 5; i < 8 && ok; ++i) ok = v[i] >= 1.0 && v[i] <= (double)(1 << 30) && v[i] == std::floor(v[i]);
+  ok = ok && (float)v[0] > 0.0f && (float)v[1] > 0.0f && v[0] <= FLT_MAX && v[1] <= FLT_MAX &&
+       std::fabs(v[2]) <= FLT_MAX && std::fabs(v[3]) <= FLT_MAX && std::fabs(v[4]) <= FLT_MAX &&
+       v[5] * v[6] * v[7] <= (double)(1 << 30);
+  if (!ok)
+    return refuse(2, "--fuse takes eight numbers voxel,trunc,x0,y0,z0,nx,ny,nz with voxel and trunc > 0, integer sizes "
+                     ">= 1 and at most 2^30 voxels, got %s", o.fuse);
+  o.fuse_p.voxel = (float)v[0];
+  o.fuse_p.trunc = (float)v[1];
+  for (int e = 0; e < 3; ++e) o.fuse_p.origin[e] = (float)v[2 + e];
+  o.fuse_p.nx = (int)v[5];
+  o.fuse_p.ny = (int)v[6];
+  o.fuse_p.nz = (int)v[7];
+  o.fuse_p.max_weight = 64.0f;
+  o.fuse_p.color = 1;
+  return 0;
+}
+
+static int read_global_motion(Options& o) {
+  o.gm_model = !strcmp(o.gm[0], "similarity")   ? OFDIS_MOTION_SIMILARITY
+               : !strcmp(o.gm[0], "affine")     ? OFDIS_MOTION_AFFINE
+               : !strcmp(o.gm[0], "homography") ? OFDIS_MOTION_HOMOGRAPHY : 0;
+  if (!o.gm_model) return refuse(2, "--global-motion takes the model similarity, affine or homography, got %s", o.gm[0]);
+  return 0;
+}
+
+static int read_codebook(Options& o) {
+  string err;
+  if (!read_fisher_book(o.fisher[0], o.fbook, err)) return refuse(2, "%s: %s", o.fisher[0], err.c_str());
+  const ofdis_traj_params& t = o.trp;
+  const int c = t.nt * t.ns * t.ns, din[5] = {2 * t.L, 8 * c, 9 * c, 8 * c, 8 * c};
+  const ofdis_fisher_codebook& cb = o.fbook.cb;
+  bool match = cb.desc_dim == o.tdim && cb.nblocks == 5;
+  for (int b = 0, off = 0; match && b < 5; off += din[b++])
+    match = cb.blocks[b].offset == off && cb.blocks[b].dim_in == din[b];
+  if (!match)
+    return refuse(2, "%s: the codebook's blocks are not the descriptors' (desc_dim %d, blocks 0+%d, %d+%d, %d+%d, %d+%d, "
+                     "%d+%d)", o.fisher[0], o.tdim, din[0], din[0], din[1], din[0] + din[1], din[2],
+                  din[0] + din[1] + din[2], din[3], o.tdim - din[4], din[4]);
+  for (int b = 0; b < cb.nblocks; ++b) o.fv_floats += 2 * cb.K * cb.blocks[b].dim;
+  return 0;
+}
+
+static int read_stabilize(Options& o) {
+  char *e0 = nullptr, *e1 = nullptr;
+  const long r = strtol(o.stab[0], &e0, 10);
+  const float crop = strtof(o.stab[1], &e1);
+  if (e0 == o.stab[0] || *e0 || r < 1 || r > 64 || e1 == o.stab[1] || *e1 || !(crop >= 0.0f && crop < 0.5f))
+    return refuse(2, "--stabilize takes a radius 1..64 and a crop 0 <= CROP < 0.5, got %s %s", o.stab[0], o.stab[1]);
+  o.stp.radius = (int)r;
+  o.stp.crop = crop;
+  o.stp.limit = crop > 0.0f ? 1 : 0;
+  for (int d = 0; d <= o.stp.radius; ++d) o.stab_wts.push_back(exp(-(double)(d * d) / (2.0 * o.stp.radius)));
+  return 0;
+}
+
+static int read_speckle(Options& o) {
+  char *e0 = nullptr, *e1 = nullptr;
+  const long sz = strtol(o.speckle[0], &e0, 10);
+  const float diff = strtof(o.speckle[1], &e1);
+  if (e0 == o.speckle[0] || *e0 || sz < 1 || sz > INT_MAX || e1 == o.speckle[1] || *e1 ||
+      !(diff >= 0.0f && diff <= FLT_MAX))
+    return refuse(2, "--speckle takes a size N >= 1 and a finite difference R >= 0, got %s %s", o.speckle[0],
+                  o.speckle[1]);
+  o.dfilt.speckle_size = (int)sz;
+  o.dfilt.speckle_diff = diff;
+  return 0;
+}
+
+static int read_camera(Options& o) {
+  float v[6];
+  const char* q = o.camera;
+  bool ok = true;
+  for (int i = 0; i < 6 && ok; ++i) {
+    char* end = nullptr;
+    v[i] = strtof(q, &end);
+    ok = end != q && (i < 5 ? *end == ',' : *end == 0) && v[i] >= -FLT_MAX && v[i] <= FLT_MAX;
+    q = end + (i < 5 ? 1 : 0);
+  }
+  if (!ok || !(v[0] > 0.0f) || !(v[1] > 0.0f) || !(v[4] > 0.0f))
+    return refuse(2, "--camera takes six finite numbers fx,fy,cx,cy,baseline,doffs with fx, fy and baseline > 0, got %s",
+                  o.camera);
+  o.dcam = ofdis_stereo_camera{v[0], v[1], v[2], v[3], v[4], v[5]};
+  return 0;
+}
+
+static int read_interpolate(Options& o) {
+  char* end = nullptr;
+  o.interp_t = strtof(o.interp_arg, &end);
+  if (end == o.interp_arg || *end || !(o.interp_t > 0.0f && o.interp_t < 1.0f))
+    return refuse(2, "--interpolate takes a time T with 0 < T < 1, got %s", o.interp_arg);
+  return 0;
+}
+
+static int read_color_max(Options& o) {
+  char* end = nullptr;
+  o.color_max = strtof(o.color_max_arg, &end);
+  if (end == o.color_max_arg || *end || !(o.color_max > 0.0f && o.color_max <= FLT_MAX))
+    return refuse(2, "--color-max takes a positive finite number, got %s", o.color_max_arg);
+  return 0;
+}
+
+// The option refusals, before any file is read: the rules in order, the first that fails refuses the run (exit 2).
+// Each rule is one given flag: the binaries of the other kind refuse it, saying what it does; --warm-start, which
+// runs one pair per launch, refuses it; it needs another flag; then its value is read.
+static int check_options(Options& o) {
+  enum { kAny, kFlow, kStereo };
+  struct Rule {
+    bool given;
+    const char* flag;  // as the refusals name it
+    int only;          // kFlow, kStereo: what it does, which the other binaries are told
+    const char* does;
+    bool no_warm;
+    bool has_needed;  // false: refused with `needs`
+    const char* needs;
+    int (*value)(Options&);
+  };
+  o.disp_on = o.lr_check || o.fill || o.speckle[0] || (o.camera && !o.sf_list);  // --camera with --scene-flow is its own
+  o.dfilt.lr_check = o.lr_check ? 1 : 0;
+  o.dfilt.alpha = 0.0f;
+  o.dfilt.beta = 1.0f;
+  o.dfilt.speckle_diff = 1.0f;
+  o.dfilt.fill = o.fill ? 1 : 0;
+  const Rule rules[] = {
+      {o.batch != nullptr, "--batch", kAny, nullptr, true, true, nullptr, nullptr},
+      {o.bidir, "--bidirectional", kAny, nullptr, true, true, nullptr, nullptr},
+      {o.interp_arg != nullptr, "--interpolate", kAny, nullptr, true, true, nullptr, nullptr},
+      {o.tracks != nullptr, "--tracks", kAny, nullptr, true, true, nullptr, nullptr},
+      {o.sf_list != nullptr, "--scene-flow", kFlow, "--scene-flow joins flows with disparities", true, true, nullptr,
+       nullptr},
+      {o.sf_gtlist != nullptr, "--gt-scene-flow", kAny, nullptr, false, o.sf_list != nullptr,
+       "--gt-scene-flow evaluates the scene flow of --scene-flow; give --scene-flow too", nullptr},
+      {o.odo_dir != nullptr, "--odometry", kFlow, "--odometry fits the rig's motion from flows", true,
+       o.sf_list && o.camera, "--odometry needs the disparities of --scene-flow and the stereo camera of --camera",
+       nullptr},
+      {o.odo_gtlist != nullptr, "--gt-poses", kAny, nullptr, false, o.odo_dir != nullptr,
+       "--gt-poses evaluates the poses of --odometry; give --odometry too", nullptr},
+      {o.fuse != nullptr, "--fuse", kFlow, "--fuse places disparities with the poses of --odometry", true,
+       o.odo_dir != nullptr, "--fuse places disparities with the poses of --odometry; give --odometry too", read_fuse},
+      {o.mesh, "--mesh", kAny, nullptr, false, o.fuse != nullptr, "--mesh meshes the volume of --fuse; give --fuse too",
+       nullptr},
+      {o.disp_on, "--lr-check, --speckle, --fill or --camera", kStereo,
+       "--lr-check, --speckle, --fill and --camera filter stereo disparities", true, true, nullptr, nullptr},
+      {o.gm[0] != nullptr, "--global-motion", kFlow, "--global-motion fits the camera motion of flows", true, true,
+       nullptr, read_global_motion},
+      {o.desc != nullptr, "--descriptors", kFlow, "--descriptors describes the tracks of flows", true,
+       o.tracks != nullptr, "--descriptors describes the clips of --tracks; give --tracks too", nullptr},
+      {o.fisher[0] != nullptr, "--fisher", kFlow, "--fisher encodes the descriptors of flows", true,
+       o.tracks != nullptr, "--fisher encodes the clips of --tracks; give --tracks too", read_codebook},
+      {o.stab[0] != nullptr, "--stabilize", kFlow, "--stabilize smooths the camera motion of flows", true,
+       o.gm[0] != nullptr, "--stabilize smooths the models of --global-motion; give --global-motion too",
+       read_stabilize},
+      {o.speckle[0] != nullptr, "--speckle", kAny, nullptr, false, true, nullptr, read_speckle},
+      {o.camera != nullptr, "--camera", kAny, nullptr, false, true, nullptr, read_camera},
+      {o.interp_arg != nullptr, "--interpolate", kAny, nullptr, false, true, nullptr, read_interpolate},
+      {o.color_max_arg != nullptr, "--color-max", kAny, nullptr, false, o.color, "--color-max needs --color",
+       read_color_max},
+  };
+  for (const Rule& r : rules) {
+    if (!r.given) continue;
+    if (r.only == kFlow && SELECTMODE != 1) return refuse(2, "%s; the stereo binaries take no %s", r.does, r.flag);
+    if (r.only == kStereo && SELECTMODE == 1) return refuse(2, "%s; the flow binaries take none of them", r.does);
+    if (r.no_warm && o.warm) return refuse(2, "--warm-start runs one pair per launch; it takes no %s", r.flag);
+    if (!r.has_needed) return refuse(2, "%s", r.needs);
+    if (r.value)
+      if (int rc = r.value(o)) return rc;
+  }
+  o.traj_stage = o.desc || o.fisher[0];
+  // --interpolate and --tracks need the backward flows: the backward slots run whenever one of them is given
+  o.two_way = o.bidir || o.interp_arg || o.tracks || o.lr_check;
+  o.maxb = o.warm ? 1 : o.batch ? atoi(o.batch) : 64;
+  if (o.maxb < 1 || (o.nnum > 1 && o.nnum != 20))
+    return refuse(2, "expected 0, 1 or exactly 20 numbers, got %d", o.nnum);
+  return 0;
+}
+
+struct Job {
+  string a, b, out;
+};
+
+static int refuse_pair(const Job& jb) {
+  return refuse(1, "cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)", jb.a.c_str(),
+                jb.b.c_str());
+}
+
+// The clip index: pair k continues pair k - 1 when its image1 path is pair k - 1's image2 path (string equality).
+// clip[k] and frame[k] count from 0; a pair of frame 0 begins its clip.
+struct ClipIndex {
+  vector<int> clip, frame;
+  int count = 0;
+};
+
+static ClipIndex index_clips(const vector<Job>& jobs) {
+  ClipIndex ci;
+  for (size_t k = 0; k < jobs.size(); ++k) {
+    const bool cont = k > 0 && jobs[k].a == jobs[k - 1].b;
+    ci.clip.push_back(cont ? ci.clip[k - 1] : ci.count++);
+    ci.frame.push_back(cont ? ci.frame[k - 1] + 1 : 0);
+  }
+  return ci;
+}
+
+// A batch's pairs [k0, k1) of one clip, whether they begin it and whether they end it
+struct ClipRun {
+  int k0, k1;
+  bool starts, ends;
+};
+
+static vector<ClipRun> clip_runs(const ClipIndex& ci, size_t j0, int n) {
+  vector<ClipRun> runs;
+  for (int k0 = 0, k1; k0 < n; k0 = k1) {
+    for (k1 = k0 + 1; k1 < n && ci.frame[j0 + k1] > 0;) ++k1;
+    runs.push_back({k0, k1, ci.frame[j0 + k0] == 0, j0 + k1 == ci.frame.size() || ci.frame[j0 + k1] == 0});
+  }
+  return runs;
+}
+
+// The per-pair input lists, every file checked against its pair's image size before any device work
+struct Inputs {
+  vector<string> gts;               // --gt: one per pair
+  vector<string> sf_files, sf_gts;  // --scene-flow: two per pair; --gt-scene-flow: three
+  vector<vector<double>> odo_gt;    // --gt-poses: per clip, 12 numbers per line
+};
+
+static int read_inputs(const Options& o, const vector<Job>& jobs, const ClipIndex& clips, Inputs& in) {
+  const int nop = SELECTMODE == 1 ? 2 : 1;
+  vector<float> tmp;
+  string err;
+  int iw = 0, ih = 0;
+  if (o.gtlist) {
+    if (!read_words(o.gtlist, in.gts)) return refuse(1, "cannot read %s", o.gtlist);
+    if (in.gts.size() != jobs.size())
+      return refuse(2, "--gt: %s lists %zu ground-truth files for %zu pairs", o.gtlist, in.gts.size(), jobs.size());
+    for (size_t k = 0; k < jobs.size(); ++k) {
+      if (!image_size(jobs[k].a.c_str(), iw, ih)) return refuse_pair(jobs[k]);
+      if (!read_gt_file(in.gts[k].c_str(), iw, ih, nop, tmp, err))
+        return refuse(1, "%s: %s", in.gts[k].c_str(), err.c_str());
+    }
+  }
+  for (int li = 0; li < 2; ++li) {  // --scene-flow, --gt-scene-flow
+    const char* list = li ? o.sf_gtlist : o.sf_list;
+    vector<string>& files = li ? in.sf_gts : in.sf_files;
+    const size_t per = li ? 3 : 2;
+    if (!list) continue;
+    if (!read_words(list, files)) return refuse(1, "cannot read %s", list);
+    if (files.size() != per * jobs.size())
+      return refuse(2, "%s: %s lists %zu files for %zu pairs (%zu per pair)", li ? "--gt-scene-flow" : "--scene-flow",
+                    list, files.size(), jobs.size(), per);
+    for (size_t k = 0; k < files.size(); ++k) {
+      if (!image_size(jobs[k / per].a.c_str(), iw, ih)) return refuse_pair(jobs[k / per]);
+      if (!read_gt_file(files[k].c_str(), iw, ih, li && k % 3 == 2 ? 2 : 1, tmp, err))
+        return refuse(2, "%s: %s", files[k].c_str(), err.c_str());
+    }
+  }
+  if (o.odo_gtlist) {  // a poses file per clip, with a line for each of its frames
+    vector<string> files;
+    if (!read_words(o.odo_gtlist, files)) return refuse(2, "cannot read %s", o.odo_gtlist);
+    if ((int)files.size() != clips.count)
+      return refuse(2, "--gt-poses: %s lists %zu poses files for %d clips", o.odo_gtlist, files.size(), clips.count);
+    vector<int> need(clips.count, 0);
+    for (size_t k = 0; k < jobs.size(); ++k) need[clips.clip[k]] = clips.frame[k] + 2;
+    for (int c = 0; c < clips.count; ++c) {
+      FILE* pf = fopen(files[c].c_str(), "r");
+      if (!pf) return refuse(2, "cannot read %s", files[c].c_str());
+      vector<double> v;
+      double x;
+      while (fscanf(pf, "%lf", &x) == 1) v.push_back(x);
+      const bool eof = feof(pf);
+      fclose(pf);
+      if (!eof || v.size() % 12 || (int)(v.size() / 12) < need[c])
+        return refuse(2, "%s: a KITTI poses file of at least %d lines of 12 numbers, got %zu numbers",
+                      files[c].c_str(), need[c], v.size());
+      in.odo_gt.push_back(v);
+    }
+  }
+  return 0;
+}
+
+// The list outputs, one file each for the whole run
+struct ListOutputs {
+  struct File {
+    FILE* f = nullptr;
+    string path;
+  };
+  File odo, desc, fisher, tracks, stab, gm;
+
+  bool open(File& x, const string& path) {
+    x.path = path;
+    x.f = fopen(path.c_str(), "w");
+    return x.f != nullptr;
+  }
+  // The end of a run: stab.txt, tracks, descriptors, fisher, global motion and odometry.txt are closed in this order,
+  // and the first that cannot be written is refused
+  int close() {
+    for (File* x : {&stab, &tracks, &desc, &fisher, &gm, &odo}) {
+      if (!x->f) continue;
+      const bool ok = fclose(x->f) == 0;
+      x->f = nullptr;
+      if (!ok) return refuse(1, "cannot write %s", x->path.c_str());
+    }
+    return 0;
+  }
+  ~ListOutputs() {  // a refused run
+    for (File* x : {&stab, &tracks, &desc, &fisher, &gm, &odo})
+      if (x->f) fclose(x->f);
+  }
+};
+
+// Opened before any device work in this order, which decides the files a refused run leaves behind: odometry.txt,
+// descriptors, fisher, tracks, stab.txt, global motion.  The descriptor stage's frame sizes are checked after
+// odometry.txt is opened.
+static int open_outputs(const Options& o, const vector<Job>& jobs, ListOutputs& out) {
+  if (o.odo_dir && !out.open(out.odo, string(o.odo_dir) + "/odometry.txt"))
+    return refuse(2, "--odometry: cannot write %s", out.odo.path.c_str());
+  for (size_t k = 0; k < jobs.size() && o.traj_stage; ++k) {  // an N x N patch in every frame
+    int iw = 0, ih = 0;
+    if (!image_size(jobs[k].a.c_str(), iw, ih)) return refuse_pair(jobs[k]);
+    if (iw < o.trp.N || ih < o.trp.N)
+      return refuse(2, "--%s needs frames of at least %d x %d, %s is %d x %d", o.desc ? "descriptors" : "fisher",
+                    o.trp.N, o.trp.N, jobs[k].a.c_str(), iw, ih);
+  }
+  if (o.desc) {
+    if (!out.open(out.desc, o.desc)) return refuse(1, "cannot write %s", o.desc);
+    fprintf(out.desc.f, "# clip id start mean_x mean_y sd_x sd_y length d0 .. d%d\n", o.tdim - 1);
+  }
+  if (o.fisher[0]) {
+    if (!out.open(out.fisher, o.fisher[1])) return refuse(1, "cannot write %s", o.fisher[1]);
+    fprintf(out.fisher.f, "# clip n_desc n_0 .. n_%d fv0 .. fv%d\n", o.fbook.cb.nblocks - 1, o.fv_floats - 1);
+  }
+  if (o.tracks) {
+    if (!out.open(out.tracks, o.tracks)) return refuse(1, "cannot write %s", o.tracks);
+    fprintf(out.tracks.f, "# clip frame id x y\n");
+  }
+  if (o.stab[0] && !out.open(out.stab, string(o.stab[2]) + "/stab.txt"))
+    return refuse(1, "cannot write %s", out.stab.path.c_str());
+  if (o.gm_model && !out.open(out.gm, o.gm[1])) return refuse(1, "cannot write %s", o.gm[1]);
+  return 0;
+}
+
+struct CtxDeleter {
+  void operator()(ofdis_ctx* c) const { ofdis_destroy(c); }
+};
+
+// One batch: pairs j0 .. j0 + n - 1 of one size, their frames, and what the device stages return for them
+struct Batch {
+  size_t j0 = 0;
+  int n = 0, w = 0, h = 0, slots = 0;
+  bool seq = false;  // a clip: frame k is image1 of pair k, frame k + 1 its image2
+  size_t hwc = 0;    // bytes per frame
+  size_t fs = 0;     // image1 of pair k at k * fs, its image2 one frame (hwc) later
+  vector<uint8_t> frames;
+  vector<float> flows;
+  vector<uint16_t> kflows;  // --kitti: the encoded slots
+  vector<uint8_t> masks;
+  vector<uint8_t> colors;  // --color: the color images of the slots
+  vector<uint8_t> interp;  // --interpolate: the frames at time T
+  vector<float> ddisp, ddepth, dxyz;  // --lr-check / --speckle / --fill / --camera: the filtered outputs
+  vector<uint8_t> dstatus;
+  size_t dcount[6];  // statuses 0..4, filled
+  vector<double> gm_models;  // --global-motion: the models, stats and per-pixel outputs
+  vector<ofdis_motion_stats> gm_stats;
+  vector<uint8_t> gm_mask, gm_reg;
+  vector<float> gm_res;
+  vector<float> sf_d0, sf_d1, sf_w, sf_m;  // --scene-flow: the disparities of image1 and image2, outputs
+  vector<double> odo_pose;                 // --odometry: the relative poses
+};
+
+// The run's state across batches: the context and what clips and the end-of-run summary carry over
+struct State {
+  State(const Options& o_, const vector<Job>& jobs_, const ClipIndex& clips_, const Inputs& in_, ListOutputs& out_)
+      : o(o_), jobs(jobs_), clips(clips_), in(in_), out(out_), nclasses(o_.bidir ? 3 : 1), eval_total(nclasses + 1),
+        sf_total(nclasses + 1), fvec(o_.fv_floats) {
+    memset(eval_total.data(), 0, sizeof(ofdis_error_stats) * eval_total.size());
+    memset(sf_total.data(), 0, sizeof(ofdis_sf_stats) * sf_total.size());
+    if (o.odo_dir) odo_rel.resize(clips.count);
+  }
+  const Options& o;
+  const vector<Job>& jobs;
+  const ClipIndex& clips;
+  const Inputs& in;
+  ListOutputs& out;
+  const int nochannels = SELECTCHANNEL == 3 ? 3 : 1, nop = SELECTMODE == 1 ? 2 : 1;
+  const int nclasses;  // with --bidirectional the forward consistency mask's classes
+  std::unique_ptr<ofdis_ctx, CtxDeleter> ctx;
+  int ctx_w = -1, ctx_h = -1, verbosity = 0;
+  Image8 last;  // image2 of the previous batch's last pair
+  size_t done = 0, seq_pairs = 0, seq_decoded = 0, warm_pairs = 0;
+  vector<ofdis_error_stats> eval_total;  // --gt: [0] all pixels, [1 + c] class c
+  vector<ofdis_sf_stats> sf_total;       // --gt-scene-flow, as eval_total
+  // --tracks: the clip being tracked (-1 none) and its next frame; the totals of the finished clips (with
+  // --descriptors and --fisher theirs too)
+  int tclip = -1, tframe = 0;
+  size_t tframes = 0;
+  ofdis_track_stats ttotal{};
+  ofdis_traj_stats dtotal{};
+  vector<float> fvec;
+  int fclips = 0;
+  long long fpushed = 0, fskipped[OFDIS_FISHER_MAX_BLOCKS] = {0};
+  int sclip = -1;  // --stabilize: the clip being stabilised (-1 none)
+  vector<vector<double>> odo_rel;  // --odometry: per clip, 12 numbers per pair
+  double odo_terr = 0.0, odo_rerr = 0.0;
+  size_t odo_eval = 0;
+  double fuse_T[12];    // --fuse: the chained pose of the clip's next image1
+  int fuse_frames = 0;  // frames pushed into the clip's volume
+  // scratch of the stages, kept across batches
+  vector<uint8_t> png;
+  vector<float> gt_batch, gt_one;
+  vector<ofdis_error_stats> eval_pairs;
+  vector<float> sf_g0, sf_g1, sf_gf;
+  vector<ofdis_sf_stats> sf_pairs;
+  vector<ofdis_motion_stats> odo_stats;
+  vector<uint8_t> odo_mask;
+  vector<float> odo_om;
+  vector<ofdis_track_point> tpoints;
+  vector<int> tcounts, tndesc;
+  vector<ofdis_traj_record> trec;
+  vector<float> tdesc;
+  vector<uint8_t> sbuf;
+  vector<ofdis_stab_frame> sinfo;
+  vector<double> fuse_poses;
+  vector<ofdis_fuse_point> fuse_pts;
+  vector<unsigned int> fuse_faces;
+};
+
+// Up to maxb pairs of one size from pair j0 on; a frame that continues the previous pair is not decoded again.  A
+// batch of two or more pairs that all continue each other is a clip and goes up frame by frame; any other batch goes
+// as its pairs, followed with two_way by their swapped copies.
+static int load_batch(State& s, Batch& b, size_t j0) {
+  const vector<Job>& jobs = s.jobs;
+  vector<Image8> imgs;  // decoded frames of this batch
+  vector<int> ia, ib;   // per pair: indices of image1, image2 in imgs
+  int w = 0, h = 0, n = 0, decoded = 0;
+  while (j0 + n < jobs.size() && n < s.o.maxb) {
+    const Job& jb = jobs[j0 + n];
+    const bool in_batch = n > 0 && jb.a == jobs[j0 + n - 1].b;          // image1 = this batch's last frame
+    const bool from_last = n == 0 && j0 > 0 && jb.a == jobs[j0 - 1].b;  // image1 = the previous batch's last frame
+    Image8 a8, b8;
+    if (from_last) a8 = s.last;
+    const bool ok = in_batch || from_last || load_image(jb.a.c_str(), s.nochannels, a8);
+    const Image8& ra = in_batch ? imgs[ib.back()] : a8;
+    if (!ok || !load_image(jb.b.c_str(), s.nochannels, b8) || ra.w != b8.w || ra.h != b8.h) return refuse_pair(jb);
+    if (n == 0) {
+      w = b8.w;
+      h = b8.h;
+    } else if (b8.w != w || b8.h != h) {
+      break;  // next group
+    }
+    if (in_batch) {
+      ia.push_back(ib.back());
+    } else {
+      decoded += from_last ? 0 : 1;
+      ia.push_back((int)imgs.size());
+      imgs.push_back(std::move(a8));
+    }
+    ib.push_back((int)imgs.size());
+    imgs.push_back(std::move(b8));
+    ++decoded;
+    ++n;
+  }
+  b.j0 = j0;
+  b.n = n;
+  b.w = w;
+  b.h = h;
+  b.hwc = (size_t)w * h * s.nochannels;
+  b.seq = n >= 2;
+  for (int k = 1; k < n && b.seq; ++k) b.seq = ia[k] == ib[k - 1];
+  b.fs = b.seq ? b.hwc : 2 * b.hwc;
+  b.slots = s.o.two_way ? 2 * n : n;  // two-way: forward slots [0, n), backward slots [n, 2n)
+  auto put = [&b, &imgs](int i) { b.frames.insert(b.frames.end(), imgs[i].px.begin(), imgs[i].px.end()); };
+  b.frames.clear();
+  if (b.seq) {
+    put(ia[0]);
+    for (int k = 0; k < n; ++k) put(ib[k]);
+    s.seq_pairs += n;
+    s.seq_decoded += decoded;
+  } else {
+    for (int k = 0; k < n; ++k) {
+      put(ia[k]);
+      put(ib[k]);
+    }
+    for (int k = 0; k < n && s.o.two_way; ++k) {  // the swapped copies
+      put(ib[k]);
+      put(ia[k]);
+    }
+  }
+  s.last = std::move(imgs[ib.back()]);
+  return 0;
+}
+
+// A context per frame size.  The clip-scoped stages (the tracker or the descriptor stage, the Fisher encoder, the
+// stabiliser, the fusion volume) keep a clip's state in the context, so every clip must end before its context is
+// destroyed.  It does: a size change always begins a clip (a pair that continues the previous one shares its frame),
+// and each of these stages ends a clip with the run of pairs that ends it, in the batch that holds that run.
+static int ensure_context(State& s, const Batch& b, const CliParams& P) {
+  if (b.w == s.ctx_w && b.h == s.ctx_h) return 0;
+  s.ctx.reset();
+  ofdis_params p;
+  memset(&p, 0, sizeof(p));
+  p.sc_f = P.lv_f; p.sc_l = P.lv_l; p.max_iter = P.maxiter; p.min_iter = P.miniter;
+  p.dp_thresh = P.mindprate; p.dr_thresh = P.mindrrate; p.res_thresh = P.minimgerr;
+  p.p_samp_s = P.patchsz; p.patove = P.poverl; p.usefbcon = P.usefbcon ? 1 : 0; p.costfct = P.costfct;
+  p.noc = s.nochannels; p.patnorm = P.patnorm; p.usetvref = P.usetvref ? 1 : 0;
+  p.tv_alpha = P.tv_alpha; p.tv_gamma = P.tv_gamma; p.tv_delta = P.tv_delta;
+  p.tv_innerit = P.tv_innerit; p.tv_solverit = P.tv_solverit; p.tv_sor = P.tv_sor; p.verbosity = P.verbosity;
+  const int scf = 1 << (s.o.warm ? P.lv_f + 1 : P.lv_f);
+  ofdis_ctx* ctx = nullptr;
+  const int rc = ofdis_create(&ctx, 0, nullptr, &p, s.nop, (b.w + scf - 1) / scf * scf, (b.h + scf - 1) / scf * scf,
+                              P.patchsz, s.o.two_way ? 2 * s.o.maxb : s.o.maxb);
+  if (rc != OFDIS_OK) return refuse(1, "ofdis_create failed with status %d for %dx%d frames", rc, b.w, b.h);
+  s.ctx.reset(ctx);
+  ofdis_set_graph_mode(ctx, 1);
+  s.ctx_w = b.w;
+  s.ctx_h = b.h;
+  return 0;
+}
+
+// The flows of the batch's slots, with --color their colors and with --bidirectional the consistency masks
+static int run_flows(State& s, Batch& b) {
+  const Options& o = s.o;
+  ofdis_ctx* ctx = s.ctx.get();
+  const int n = b.n, w = b.w, h = b.h;
+  if (o.kitti) b.kflows.resize((size_t)b.slots * w * h * (s.nop == 2 ? 3 : 1));
+  else b.flows.resize((size_t)b.slots * w * h * s.nop);
+  int rc;
+  if (o.two_way && b.seq) {
+    rc = ofdis_upload_sequence_bidir_u8(ctx, 0, n, b.frames.data(), w, h, OFDIS_MEM_HOST);
+  } else if (o.two_way) {
+    rc = ofdis_upload_frames_u8(ctx, 0, 2 * n, b.frames.data(), w, h, OFDIS_MEM_HOST);
+    if (rc == OFDIS_OK) rc = ofdis_set_swapped_slots(ctx, 0, n, 0);
+    if (rc == OFDIS_OK) rc = ofdis_set_swapped_slots(ctx, n, 2 * n, 1);
+  } else {
+    rc = b.seq ? ofdis_upload_sequence_u8(ctx, 0, n, b.frames.data(), w, h, OFDIS_MEM_HOST)
+               : ofdis_upload_frames_u8(ctx, 0, n, b.frames.data(), w, h, OFDIS_MEM_HOST);
+  }
+  // warm start: the context still holds the previous pair's flow (same size, so it was not recreated)
+  const bool from_prev = o.warm && s.clips.frame[b.j0] > 0;
+  if (rc == OFDIS_OK && from_prev) rc = ofdis_set_initflow_from_result(ctx, 0, 1, 0, w, h);
+  s.warm_pairs += from_prev ? 1 : 0;
+  if (rc == OFDIS_OK) rc = ofdis_run(ctx, b.slots, from_prev ? 1 : 0);
+  if (rc == OFDIS_OK)
+    rc = o.kitti ? ofdis_get_flow_fullres_encoded(ctx, 0, b.slots, OFDIS_ENC_KITTI, b.kflows.data(), w, h, OFDIS_MEM_HOST)
+                 : ofdis_get_flow_fullres(ctx, 0, b.slots, b.flows.data(), w, h, OFDIS_MEM_HOST);
+  if (rc == OFDIS_OK && o.color) {
+    b.colors.resize((size_t)b.slots * w * h * 3);
+    rc = ofdis_flow_color_fullres(ctx, 0, b.slots, b.colors.data(), nullptr, o.color_max, w, h, OFDIS_MEM_HOST);
+  }
+  if (rc == OFDIS_OK && o.bidir) {
+    b.masks.resize((size_t)n * w * h);
+    rc = ofdis_consistency_fullres(ctx, 0, n, n, b.masks.data(), nullptr, s.nop == 2 ? 0.01f : 0.0f,
+                                   s.nop == 2 ? 0.5f : 1.0f, w, h, OFDIS_MEM_HOST);
+  }
+  return rc;
+}
+
+// --interpolate: image1 / image2 of pair k are frames k and k + 1 of a clip, or the k-th pair of the pairs layout
+static int run_interpolate(State& s, Batch& b) {
+  b.interp.resize((size_t)b.n * b.hwc);
+  return ofdis_interpolate_fullres(s.ctx.get(), 0, b.n, b.n, b.frames.data(), b.frames.data() + b.hwc, b.fs,
+                                   s.o.interp_t, s.nop == 2 ? 0.01f : 0.0f, s.nop == 2 ? 0.5f : 1.0f, b.interp.data(),
+                                   nullptr, b.w, b.h, OFDIS_MEM_HOST);
+}
+
+static int run_global_motion(State& s, Batch& b) {
+  const size_t np = (size_t)b.n * b.w * b.h;
+  b.gm_models.resize((size_t)9 * b.n);
+  b.gm_stats.resize(b.n);
+  b.gm_mask.resize(np);
+  b.gm_res.resize(2 * np);
+  b.gm_reg.resize((size_t)b.n * b.hwc);
+  ofdis_motion_params mp;
+  memset(&mp, 0, sizeof(mp));
+  mp.model = s.o.gm_model;
+  mp.step = 8;
+  mp.fb_check = s.o.bidir ? 1 : 0;
+  mp.alpha = 0.01f;
+  mp.beta = 0.5f;
+  mp.hypotheses = 1024;
+  mp.threshold = 1.0f;
+  mp.refine = 3;
+  mp.seed = 0;
+  return ofdis_global_motion_fullres(s.ctx.get(), 0, b.n, b.n, &mp, b.frames.data() + b.hwc, b.fs, b.gm_models.data(),
+                                     b.gm_stats.data(), b.gm_mask.data(), b.gm_res.data(), b.gm_reg.data(), b.w, b.h,
+                                     OFDIS_MEM_HOST);
+}
+
+static int run_disparity(State& s, Batch& b) {
+  const Options& o = s.o;
+  const size_t np = (size_t)b.n * b.w * b.h;
+  b.ddisp.resize(np);
+  b.dstatus.resize(np);
+  b.ddepth.resize(o.camera ? np : 0);
+  b.dxyz.resize(o.camera ? 3 * np : 0);
+  const int rc = ofdis_disparity_fullres(s.ctx.get(), 0, b.n, b.n, &o.dfilt, o.camera ? &o.dcam : nullptr,
+                                         b.ddisp.data(), b.dstatus.data(), o.camera ? b.ddepth.data() : nullptr,
+                                         o.camera ? b.dxyz.data() : nullptr, b.w, b.h, OFDIS_MEM_HOST);
+  memset(b.dcount, 0, sizeof(b.dcount));
+  for (size_t i = 0; i < np && rc == OFDIS_OK; ++i) {
+    b.dcount[b.dstatus[i] < 5 ? b.dstatus[i] : 0] += 1;
+    b.dcount[5] += b.dstatus[i] != 0 && !std::isnan(b.ddisp[i]);
+  }
+  return rc;
+}
+
+static void write_tracks(State& s, const ofdis_track_point* p, int count) {
+  for (int i = 0; i < count; ++i)
+    fprintf(s.out.tracks.f, "%d %d %d %.9g %.9g\n", s.tclip, s.tframe, p[i].id, (double)p[i].x, (double)p[i].y);
+  ++s.tframe;
+  ++s.tframes;
+}
+
+static void write_desc(State& s, int count) {
+  const int tdim = s.o.tdim;
+  for (int i = 0; i < count; ++i) {
+    const ofdis_traj_record& r = s.trec[i];
+    fprintf(s.out.desc.f, "%d %d %d %.9g %.9g %.9g %.9g %.9g", s.tclip, r.id, r.start, (double)r.mean_x,
+            (double)r.mean_y, (double)r.sd_x, (double)r.sd_y, (double)r.length);
+    const float* d = s.tdesc.data() + (size_t)i * tdim;
+    for (int e = 0; e < tdim; ++e) fprintf(s.out.desc.f, " %.9g", (double)d[e]);
+    fprintf(s.out.desc.f, "\n");
+  }
+}
+
+// The tracked clip's end: --fisher takes its vector; the tracker's (and the descriptor stage's) counters go to the
+// totals
+static int end_track_clip(State& s) {
+  ofdis_ctx* ctx = s.ctx.get();
+  const ofdis_fisher_codebook& cb = s.o.fbook.cb;
+  if (s.out.fisher.f) {
+    ofdis_fisher_stats fs;
+    const int rc = ofdis_fisher_take(ctx, s.fvec.data(), nullptr, &fs, OFDIS_MEM_HOST);
+    if (rc != OFDIS_OK) return rc;
+    fprintf(s.out.fisher.f, "%d %lld", s.tclip, fs.pushed);
+    for (int b = 0; b < cb.nblocks; ++b) fprintf(s.out.fisher.f, " %lld", fs.n[b]);
+    for (float v : s.fvec) fprintf(s.out.fisher.f, " %.9g", (double)v);
+    fprintf(s.out.fisher.f, "\n");
+    ++s.fclips;
+    s.fpushed += fs.pushed;
+    for (int b = 0; b < cb.nblocks; ++b) s.fskipped[b] += fs.skipped[b];
+  }
+  ofdis_track_stats st;
+  if (ofdis_track_stats_get(ctx, &st) != OFDIS_OK) return OFDIS_OK;
+  s.ttotal.seeded += st.seeded;
+  s.ttotal.ended_leaves += st.ended_leaves;
+  s.ttotal.ended_inconsistent += st.ended_inconsistent;
+  s.ttotal.ended_boundary += st.ended_boundary;
+  s.ttotal.dropped += st.dropped;
+  ofdis_traj_stats ds;
+  if (!s.o.traj_stage || ofdis_traj_stats_get(ctx, &ds) != OFDIS_OK) return OFDIS_OK;
+  s.dtotal.emitted += ds.emitted;
+  s.dtotal.rejected_static += ds.rejected_static;
+  s.dtotal.rejected_erratic += ds.rejected_erratic;
+  s.dtotal.rejected_jump += ds.rejected_jump;
+  s.dtotal.rejected_camera += ds.rejected_camera;
+  return OFDIS_OK;
+}
+
+// --tracks, with --descriptors / --fisher through the descriptor stage: a run that begins a clip begins the tracker on
+// its first image1 (and the Fisher encoder), every run advances it through its image2 frames, and a run that ends the
+// clip ends it
+static int run_tracks(State& s, Batch& b) {
+  const Options& o = s.o;
+  ofdis_ctx* ctx = s.ctx.get();
+  const int n = b.n, w = b.w, h = b.h;
+  const double* models = o.gm_model ? b.gm_models.data() : nullptr;
+  ofdis_track_params tp;
+  tp.spacing = 8;
+  tp.capacity = 4 * ((w + 7) / 8) * ((h + 7) / 8);
+  tp.alpha = s.nop == 2 ? 0.01f : 0.0f;
+  tp.beta = s.nop == 2 ? 0.5f : 1.0f;
+  tp.mb_alpha = 0.01f;
+  tp.mb_beta = 0.002f;
+  tp.min_eig = 25.0f;
+  s.tpoints.resize((size_t)n * tp.capacity);
+  s.tcounts.resize(n);
+  int rc = OFDIS_OK;
+  for (const ClipRun& r : clip_runs(s.clips, b.j0, n)) {
+    const int k0 = r.k0, k1 = r.k1;
+    const uint8_t* im1 = b.frames.data() + (size_t)k0 * b.fs;
+    const uint8_t* im2 = im1 + b.hwc;
+    if (r.starts) {
+      ++s.tclip;
+      s.tframe = 0;
+      rc = o.traj_stage ? ofdis_traj_begin(ctx, &tp, &o.trp, im1, s.tpoints.data(), s.tcounts.data(), w, h,
+                                           OFDIS_MEM_HOST)
+                        : ofdis_track_begin(ctx, &tp, im1, s.tpoints.data(), s.tcounts.data(), w, h, OFDIS_MEM_HOST);
+      if (rc == OFDIS_OK && s.out.fisher.f) rc = ofdis_fisher_begin(ctx, &o.fbook.cb);
+      if (rc == OFDIS_OK) write_tracks(s, s.tpoints.data(), s.tcounts[0]);
+    }
+    s.tndesc.resize(k1 - k0);
+    if (rc == OFDIS_OK && o.traj_stage && !o.desc) {  // --fisher alone: the descriptors stay on the device
+      rc = ofdis_traj_advance_fisher(ctx, k0, k1, n + k0, im2, b.fs, models ? models + (size_t)9 * k0 : nullptr,
+                                     s.tpoints.data(), s.tcounts.data(), s.tndesc.data(), w, h, OFDIS_MEM_HOST);
+    } else if (rc == OFDIS_OK && o.desc) {
+      const size_t bound = (size_t)tp.capacity * ((k1 - k0 + 2 * o.trp.L - 2) / o.trp.L);
+      s.trec.resize(bound);
+      s.tdesc.resize(bound * o.tdim);
+      rc = ofdis_traj_advance(ctx, k0, k1, n + k0, im2, b.fs, models ? models + (size_t)9 * k0 : nullptr,
+                              s.tpoints.data(), s.tcounts.data(), s.trec.data(), s.tdesc.data(), s.tndesc.data(), w, h,
+                              OFDIS_MEM_HOST);
+      int total = 0;
+      for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k) total += s.tndesc[k];
+      if (rc == OFDIS_OK) write_desc(s, total);
+      if (rc == OFDIS_OK && s.out.fisher.f) rc = ofdis_fisher_push(ctx, s.tdesc.data(), total, OFDIS_MEM_HOST);
+    } else if (rc == OFDIS_OK) {
+      rc = ofdis_track_advance(ctx, k0, k1, n + k0, im2, b.fs, s.tpoints.data(), s.tcounts.data(), w, h,
+                               OFDIS_MEM_HOST);
+    }
+    for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k)
+      write_tracks(s, s.tpoints.data() + (size_t)k * tp.capacity, s.tcounts[k]);
+    if (rc == OFDIS_OK && r.ends) rc = end_track_clip(s);
+    if (rc != OFDIS_OK) break;
+  }
+  return rc;
+}
+
+// --stabilize: `count` emitted frames of the clip being stabilised to DIR/stab_<clip>_<frame>.png and stab.txt
+static void write_stab(State& s, const Batch& b, int count) {
+  for (int i = 0; i < count; ++i) {
+    const ofdis_stab_frame& f = s.sinfo[i];
+    fprintf(s.out.stab.f, "%d %lld", s.sclip, f.frame);
+    for (int e = 0; e < 9; ++e) fprintf(s.out.stab.f, " %.17g", f.correction[e]);
+    fprintf(s.out.stab.f, " %.17g %d\n", f.lambda, f.status);
+    char name[64];
+    snprintf(name, sizeof(name), "/stab_%04d_%06lld.png", s.sclip, f.frame);
+    save_png(as_rgb(s.sbuf.data() + (size_t)i * b.hwc, b.hwc, s.nochannels, s.png), b.w, b.h, s.nochannels, 8,
+             (string(s.o.stab[2]) + name).c_str());
+  }
+}
+
+// --stabilize: a run that begins a clip begins the stabiliser on its first image1, every run pushes its image2 frames
+// with their --global-motion models, and a run that ends the clip emits the rest
+static int run_stabilize(State& s, Batch& b) {
+  ofdis_ctx* ctx = s.ctx.get();
+  int rc = OFDIS_OK;
+  for (const ClipRun& r : clip_runs(s.clips, b.j0, b.n)) {
+    const uint8_t* im1 = b.frames.data() + (size_t)r.k0 * b.fs;
+    if (r.starts) {
+      rc = ofdis_stab_begin(ctx, &s.o.stp, s.o.stab_wts.data(), im1, b.w, b.h, OFDIS_MEM_HOST);
+      if (rc != OFDIS_OK) break;
+      ++s.sclip;
+    }
+    s.sbuf.resize((size_t)(r.k1 - r.k0) * b.hwc);
+    s.sinfo.resize(r.k1 - r.k0);
+    int count = 0;
+    rc = ofdis_stab_push(ctx, r.k1 - r.k0, b.gm_models.data() + (size_t)9 * r.k0, im1 + b.hwc, b.fs, s.sbuf.data(),
+                         s.sinfo.data(), &count, OFDIS_MEM_HOST);
+    if (rc == OFDIS_OK) write_stab(s, b, count);
+    if (rc == OFDIS_OK && r.ends) {
+      s.sbuf.resize((size_t)s.o.stp.radius * b.hwc);
+      s.sinfo.resize(s.o.stp.radius);
+      rc = ofdis_stab_finish(ctx, s.sbuf.data(), s.sinfo.data(), &count, OFDIS_MEM_HOST);
+      if (rc == OFDIS_OK) write_stab(s, b, count);
+    }
+    if (rc != OFDIS_OK) break;
+  }
+  return rc;
+}
+
+// A host-side failure whose refusal is printed already (every OFDIS_* status is <= 0)
+static const int kRefused = 1;
+
+// --gt: the forward slots against the batch's ground truth
+static int run_eval(State& s, Batch& b) {
+  const int n = b.n, w = b.w, h = b.h, nop = s.nop, nclasses = s.nclasses;
+  s.gt_batch.resize((size_t)n * w * h * nop);
+  for (int k = 0; k < n; ++k) {
+    string err;
+    const string& gt = s.in.gts[b.j0 + k];
+    if (!read_gt_file(gt.c_str(), w, h, nop, s.gt_one, err)) return refuse(kRefused, "%s: %s", gt.c_str(), err.c_str());
+    memcpy(s.gt_batch.data() + (size_t)k * w * h * nop, s.gt_one.data(), sizeof(float) * s.gt_one.size());
+  }
+  s.eval_pairs.resize((size_t)n * nclasses);
+  const int rc = ofdis_flow_error_fullres(s.ctx.get(), 0, n, s.gt_batch.data(), s.o.bidir ? b.masks.data() : nullptr,
+                                          nclasses, s.eval_pairs.data(), nullptr, w, h, OFDIS_MEM_HOST);
+  for (int k = 0; k < n && rc == OFDIS_OK; ++k)
+    for (int c = 0; c < nclasses; ++c) {
+      add_stats(s.eval_total[0], s.eval_pairs[(size_t)k * nclasses + c]);
+      if (s.o.bidir) add_stats(s.eval_total[1 + c], s.eval_pairs[(size_t)k * nclasses + c]);
+    }
+  return rc;
+}
+
+// --scene-flow: the pairs' disparities in, the scene flow and its evaluation, <stem>_disp1 and <stem>_sceneflow.pfm out
+static int run_scene_flow(State& s, Batch& b) {
+  const Options& o = s.o;
+  const int n = b.n, w = b.w, h = b.h, nclasses = s.nclasses;
+  const size_t pix = (size_t)w * h, j0 = b.j0;
+  // positive disparities: the readers return this library's stereo convention, -d
+  auto load = [&](const string& path, int fnop, float sign, float* dst) {
+    string err;
+    if (!read_gt_file(path.c_str(), w, h, fnop, s.gt_one, err)) {
+      refuse(kRefused, "%s: %s", path.c_str(), err.c_str());
+      return false;
+    }
+    for (size_t i = 0; i < s.gt_one.size(); ++i) dst[i] = sign * s.gt_one[i];
+    return true;
+  };
+  const vector<string>& df = s.in.sf_files;
+  const vector<string>& gf = s.in.sf_gts;
+  b.sf_d0.resize(n * pix);
+  b.sf_d1.resize(n * pix);
+  b.sf_w.resize(n * pix);
+  b.sf_m.resize(o.camera ? 3 * n * pix : 0);
+  bool ok = true;
+  for (int k = 0; k < n && ok; ++k)
+    ok = load(df[2 * (j0 + k)], 1, -1.0f, &b.sf_d0[k * pix]) && load(df[2 * (j0 + k) + 1], 1, -1.0f, &b.sf_d1[k * pix]);
+  if (o.sf_gtlist) {
+    s.sf_g0.resize(n * pix);
+    s.sf_g1.resize(n * pix);
+    s.sf_gf.resize(2 * n * pix);
+    for (int k = 0; k < n && ok; ++k)
+      ok = load(gf[3 * (j0 + k)], 1, -1.0f, &s.sf_g0[k * pix]) && load(gf[3 * (j0 + k) + 1], 1, -1.0f, &s.sf_g1[k * pix]) &&
+           load(gf[3 * (j0 + k) + 2], 2, 1.0f, &s.sf_gf[2 * k * pix]);
+    s.sf_pairs.resize((size_t)n * nclasses);
+  }
+  if (!ok) return kRefused;
+  const ofdis_sf_gt sgt{s.sf_g0.data(), s.sf_g1.data(), s.sf_gf.data()};
+  const int rc = ofdis_scene_flow_fullres(s.ctx.get(), 0, n, b.sf_d0.data(), b.sf_d1.data(), pix, 1.0f,
+                                          o.camera ? &o.dcam : nullptr, b.sf_w.data(), nullptr,
+                                          o.camera ? b.sf_m.data() : nullptr, o.sf_gtlist ? &sgt : nullptr,
+                                          o.bidir ? b.masks.data() : nullptr, nclasses,
+                                          o.sf_gtlist ? s.sf_pairs.data() : nullptr, w, h, OFDIS_MEM_HOST);
+  for (int k = 0; k < n && rc == OFDIS_OK && o.sf_gtlist; ++k) {
+    ofdis_sf_stats all;
+    memset(&all, 0, sizeof(all));
+    for (int c = 0; c < nclasses; ++c) {
+      add_sf_stats(all, s.sf_pairs[(size_t)k * nclasses + c]);
+      add_sf_stats(s.sf_total[1 + c], s.sf_pairs[(size_t)k * nclasses + c]);
+    }
+    add_sf_stats(s.sf_total[0], all);
+    if (s.verbosity > 0) print_sfeval(s.jobs[j0 + k].out.c_str(), 0, all);
+  }
+  for (int k = 0; k < n && rc == OFDIS_OK; ++k) {
+    const string& out = s.jobs[j0 + k].out;
+    if (o.kitti) save_kitti_disp(&b.sf_w[k * pix], w, h, with_suffix(out, "_disp1"));
+    else save_pfm1(&b.sf_w[k * pix], w, h, with_suffix(out, "_disp1", ".pfm"));
+    if (o.camera) save_pfm3(&b.sf_m[3 * k * pix], w, h, with_suffix(out, "_sceneflow", ".pfm").c_str());
+  }
+  return rc;
+}
+
+// --odometry: the rig's motion of every pair to odometry.txt, <stem>_objects.pgm and <stem>_objmotion.pfm; --gt-poses
+// its error
+static int run_odometry(State& s, Batch& b) {
+  const int n = b.n, w = b.w, h = b.h;
+  const size_t pix = (size_t)w * h;
+  FILE* f = s.out.odo.f;
+  ofdis_egomotion_params ep;
+  memset(&ep, 0, sizeof(ep));
+  ep.step = 8;
+  ep.fb_check = s.o.bidir ? 1 : 0;
+  ep.alpha = 0.01f;
+  ep.beta = 0.5f;
+  ep.edge_diff = 1.0f;
+  ep.hypotheses = 1024;
+  ep.threshold = 1.0f;
+  ep.refine = 5;
+  ep.seed = 0;
+  b.odo_pose.resize((size_t)12 * n);
+  s.odo_stats.resize(n);
+  s.odo_mask.resize(n * pix);
+  s.odo_om.resize(3 * n * pix);
+  const int rc = ofdis_egomotion_fullres(s.ctx.get(), 0, n, n, &ep, b.sf_d0.data(), b.sf_d1.data(), pix, &s.o.dcam,
+                                         b.odo_pose.data(), s.odo_stats.data(), s.odo_mask.data(), nullptr,
+                                         s.odo_om.data(), w, h, OFDIS_MEM_HOST);
+  for (int k = 0; k < n && rc == OFDIS_OK; ++k) {
+    const int c = s.clips.clip[b.j0 + k], fr = s.clips.frame[b.j0 + k];
+    const ofdis_motion_stats& st = s.odo_stats[k];
+    const double* P = b.odo_pose.data() + (size_t)12 * k;
+    const string& out = s.jobs[b.j0 + k].out;
+    fprintf(f, "%d %d %d %d %d %d", c, fr, st.status, st.n_corr, st.ransac_inliers, st.n_inliers);
+    for (int i = 0; i < 12; ++i) fprintf(f, " %.17g", P[i]);
+    fprintf(f, "\n");
+    s.odo_rel[c].insert(s.odo_rel[c].end(), P, P + 12);
+    save_mask_pgm(s.odo_mask.data() + k * pix, w, h, with_suffix(out, "_objects", ".pgm").c_str());
+    save_pfm3(&s.odo_om[3 * k * pix], w, h, with_suffix(out, "_objmotion", ".pfm").c_str());
+    if (!s.o.odo_gtlist) continue;
+    double te, re;
+    const vector<double>& gt = s.in.odo_gt[c];
+    pose_error(&gt[(size_t)12 * fr], &gt[(size_t)12 * (fr + 1)], P, &te, &re);
+    s.odo_terr += te;
+    s.odo_rerr += re;
+    ++s.odo_eval;
+    if (s.verbosity > 0) printf("ODOEVAL %d %d %.9g %.9g\n", c, fr, te, re);
+  }
+  return rc;
+}
+
+// --fuse: the end of a clip's volume, pushed with its last image2: the surface to DIR/fused_<clip>.ply, with --mesh
+// the triangle mesh to DIR/fused_<clip>_mesh.ply
+static int end_fuse_clip(State& s, const Batch& b, const ClipRun& r) {
+  ofdis_ctx* ctx = s.ctx.get();
+  const int c = s.clips.clip[b.j0 + r.k0], w = b.w, h = b.h;
+  const size_t pix = (size_t)w * h;
+  int rc = ofdis_fuse_push(ctx, 1, &b.sf_d1[(r.k1 - 1) * pix], pix, &s.fuse_poses[(size_t)12 * (r.k1 - r.k0)],
+                           &s.o.dcam, INFINITY, b.frames.data() + (size_t)(r.k1 - 1) * b.fs + b.hwc, b.fs, w, h,
+                           OFDIS_MEM_HOST);
+  ++s.fuse_frames;
+  long count = 0;
+  if (rc == OFDIS_OK) rc = ofdis_fuse_extract(ctx, 1.0f, nullptr, 0, &count, OFDIS_MEM_HOST);
+  if (rc != OFDIS_OK) return rc;
+  s.fuse_pts.resize(count);
+  rc = ofdis_fuse_extract(ctx, 1.0f, s.fuse_pts.data(), count, &count, OFDIS_MEM_HOST);
+  if (rc != OFDIS_OK) return rc;
+  char name[32];
+  snprintf(name, sizeof(name), "/fused_%04d.ply", c);
+  string path = string(s.o.odo_dir) + name;
+  if (!write_fused_ply(path, s.fuse_pts.data(), count, s.nochannels, false, nullptr, 0))
+    return refuse(kRefused, "cannot write %s", path.c_str());
+  if (s.verbosity > 0) printf("FUSE clip %d frames %d points %ld\n", c, s.fuse_frames, count);
+  if (!s.o.mesh) return OFDIS_OK;
+  // the mesh's vertices are the points just extracted: only the faces come back
+  long nv = 0, nf = 0;
+  rc = ofdis_fuse_mesh(ctx, 1.0f, nullptr, 0, &nv, nullptr, 0, &nf, OFDIS_MEM_HOST);
+  if (rc != OFDIS_OK) return rc;
+  s.fuse_faces.resize((size_t)3 * nf);
+  rc = ofdis_fuse_mesh(ctx, 1.0f, nullptr, 0, &nv, s.fuse_faces.data(), nf, &nf, OFDIS_MEM_HOST);
+  if (rc != OFDIS_OK) return rc;
+  snprintf(name, sizeof(name), "/fused_%04d_mesh.ply", c);
+  path = string(s.o.odo_dir) + name;
+  if (!write_fused_ply(path, s.fuse_pts.data(), count, s.nochannels, true, s.fuse_faces.data(), nf))
+    return refuse(kRefused, "cannot write %s", path.c_str());
+  if (s.verbosity > 0) printf("MESH clip %d vertices %ld faces %ld\n", c, nv, nf);
+  return OFDIS_OK;
+}
+
+// --fuse: a run that begins a clip begins its volume; every run pushes its image1 disparities with their chained poses,
+// and a run that ends the clip ends the volume
+static int run_fuse(State& s, Batch& b) {
+  static const double kIdentity[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+  const size_t pix = (size_t)b.w * b.h;
+  int rc = OFDIS_OK;
+  for (const ClipRun& r : clip_runs(s.clips, b.j0, b.n)) {
+    if (r.starts) {
+      memcpy(s.fuse_T, kIdentity, sizeof(s.fuse_T));
+      s.fuse_frames = 0;
+      rc = ofdis_fuse_begin(s.ctx.get(), &s.o.fuse_p);
+      if (rc != OFDIS_OK) break;
+    }
+    s.fuse_poses.resize((size_t)12 * (r.k1 - r.k0 + 1));
+    for (int k = r.k0; k < r.k1; ++k) {
+      memcpy(&s.fuse_poses[(size_t)12 * (k - r.k0)], s.fuse_T, sizeof(s.fuse_T));
+      chain_pose(s.fuse_T, b.odo_pose.data() + (size_t)12 * k);
+    }
+    memcpy(&s.fuse_poses[(size_t)12 * (r.k1 - r.k0)], s.fuse_T, sizeof(s.fuse_T));
+    rc = ofdis_fuse_push(s.ctx.get(), r.k1 - r.k0, &b.sf_d0[r.k0 * pix], pix, s.fuse_poses.data(), &s.o.dcam, INFINITY,
+                         b.frames.data() + (size_t)r.k0 * b.fs, b.fs, b.w, b.h, OFDIS_MEM_HOST);
+    s.fuse_frames += r.k1 - r.k0;
+    if (rc == OFDIS_OK && r.ends) rc = end_fuse_clip(s, b, r);
+    if (rc != OFDIS_OK) break;
+  }
+  return rc;
+}
+
+// The device stages of a batch, in order; the first failure ends them
+static int run_stages(State& s, Batch& b) {
+  const Options& o = s.o;
+  int rc = run_flows(s, b);
+  if (rc == OFDIS_OK && o.interp_arg) rc = run_interpolate(s, b);
+  if (rc == OFDIS_OK && o.gm_model) rc = run_global_motion(s, b);
+  if (rc == OFDIS_OK && o.disp_on) rc = run_disparity(s, b);
+  if (rc == OFDIS_OK && o.tracks) rc = run_tracks(s, b);
+  if (rc == OFDIS_OK && o.stab[0]) rc = run_stabilize(s, b);
+  if (rc == OFDIS_OK) rc = ofdis_sync(s.ctx.get());
+  if (rc == OFDIS_OK && o.gtlist) rc = run_eval(s, b);
+  if (rc == OFDIS_OK && o.sf_list) rc = run_scene_flow(s, b);
+  if (rc == OFDIS_OK && o.odo_dir) rc = run_odometry(s, b);
+  if (rc == OFDIS_OK && o.fuse) rc = run_fuse(s, b);
+  return rc;
+}
+
+// Every pair's <stem><ext> (KITTI's PNG with --kitti), with --bidirectional <stem>_bw<ext> and <stem>_occ.pgm
+static void write_flows(State& s, const Batch& b) {
+  const int w = b.w, h = b.h, nop = s.nop, kch = nop == 2 ? 3 : 1;
+  ImageF img;
+  img.w = w;
+  img.h = h;
+  img.c = nop;
+  auto save = [&](int slot, const string& path) {
+    if (s.o.kitti) {
+      save_png(b.kflows.data() + (size_t)slot * w * h * kch, w, h, kch, 16, path.c_str());
+      return;
+    }
+    img.px.assign(b.flows.begin() + (size_t)slot * w * h * nop, b.flows.begin() + (size_t)(slot + 1) * w * h * nop);
+    if (SELECTMODE == 1) SaveFlowFile(img, path.c_str());
+    else SavePFMFile(img, path.c_str());
+  };
+  for (int k = 0; k < b.n; ++k) {
+    const string& out = s.jobs[b.j0 + k].out;
+    save(k, out);
+    if (!s.o.bidir) continue;
+    save(b.n + k, with_suffix(out, "_bw"));
+    save_mask_pgm(b.masks.data() + (size_t)k * w * h, w, h, with_suffix(out, "_occ", ".pgm").c_str());
+  }
+}
+
+// --global-motion: every pair's line, <stem>_residual<ext>, <stem>_moving.pgm and <stem>_registered.png
+static void write_global_motion(State& s, const Batch& b) {
+  const int w = b.w, h = b.h;
+  for (int k = 0; k < b.n; ++k) {
+    const string& o = s.jobs[b.j0 + k].out;
+    fprintf(s.out.gm.f, "%s", with_suffix(o, "", "").c_str());
+    for (int i = 0; i < 9; ++i) fprintf(s.out.gm.f, " %.17g", b.gm_models[(size_t)9 * k + i]);
+    fprintf(s.out.gm.f, " %d %d %d\n", b.gm_stats[k].status, b.gm_stats[k].n_corr, b.gm_stats[k].n_inliers);
+    const float* r = b.gm_res.data() + (size_t)2 * k * w * h;
+    if (s.o.kitti) {
+      save_kitti_flow(r, w, h, with_suffix(o, "_residual"));
+    } else {
+      ImageF f;
+      f.w = w;
+      f.h = h;
+      f.c = 2;
+      f.px.assign(r, r + (size_t)2 * w * h);
+      SaveFlowFile(f, with_suffix(o, "_residual").c_str());
+    }
+    save_mask_pgm(b.gm_mask.data() + (size_t)k * w * h, w, h, with_suffix(o, "_moving", ".pgm").c_str());
+    save_png(as_rgb(b.gm_reg.data() + (size_t)k * b.hwc, b.hwc, s.nochannels, s.png), w, h, s.nochannels, 8,
+             with_suffix(o, "_registered", ".png").c_str());
+  }
+}
+
+// The filtered disparities: every pair's <stem>_filtered<ext>, with --camera <stem>_depth.pfm and <stem>.ply
+static void write_disparities(State& s, const Batch& b) {
+  const int w = b.w, h = b.h, ch = s.nochannels;
+  vector<uint8_t> ply;
+  for (int k = 0; k < b.n; ++k) {
+    const size_t o = (size_t)k * w * h;
+    const string& out = s.jobs[b.j0 + k].out;
+    if (s.o.kitti) save_kitti_disp(&b.ddisp[o], w, h, with_suffix(out, "_filtered"));
+    else save_pfm1(&b.ddisp[o], w, h, with_suffix(out, "_filtered"));  // the sign of <stem><ext>
+    if (!s.o.camera) continue;
+    save_pfm1(&b.ddepth[o], w, h, with_suffix(out, "_depth", ".pfm"));
+    const uint8_t* im1 = b.frames.data() + (size_t)k * b.fs;
+    size_t npts = 0;
+    ply.clear();
+    for (size_t i = 0; i < (size_t)w * h; ++i) {
+      if (!std::isfinite(b.ddepth[o + i])) continue;
+      const uint8_t* qb = reinterpret_cast<const uint8_t*>(b.dxyz.data() + (o + i) * 3);
+      const uint8_t* c = im1 + i * ch;
+      const uint8_t rgb[3] = {ch == 3 ? c[2] : c[0], c[ch == 3 ? 1 : 0], c[0]};  // the decoder's BGR
+      ply.insert(ply.end(), qb, qb + 12);
+      ply.insert(ply.end(), rgb, rgb + 3);
+      ++npts;
+    }
+    FILE* pf = fopen(with_suffix(out, "", ".ply").c_str(), "wb");
+    if (!pf) {
+      cout << "WriteFile: could not open file" << endl;
+      continue;
+    }
+    fprintf(pf, "ply\nformat binary_little_endian 1.0\nelement vertex %zu\nproperty float x\nproperty float y\n"
+                "property float z\nproperty uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n", npts);
+    if (fwrite(ply.data(), 1, ply.size(), pf) != ply.size()) cout << "WriteFile: problem writing data" << endl;
+    fclose(pf);
+  }
+  if (s.verbosity > 0)
+    printf("DISP pairs %d valid %zu inconsistent %zu leaves %zu range %zu speckle %zu filled %zu\n", b.n, b.dcount[0],
+           b.dcount[1], b.dcount[2], b.dcount[3], b.dcount[4], b.dcount[5]);
+}
+
+// The batch's per-pair files (KITTI's PNGs first and the .flo / .pfm files last, as they have always gone)
+static void write_outputs(State& s, const Batch& b) {
+  const Options& o = s.o;
+  const int w = b.w, h = b.h;
+  if (o.kitti) write_flows(s, b);
+  for (int k = 0; k < b.n && o.color; ++k) {
+    const string& out = s.jobs[b.j0 + k].out;
+    save_png(b.colors.data() + (size_t)k * w * h * 3, w, h, 3, 8, with_suffix(out, "_color", ".png").c_str());
+    if (o.bidir)
+      save_png(b.colors.data() + (size_t)(b.n + k) * w * h * 3, w, h, 3, 8, with_suffix(out, "_bw_color", ".png").c_str());
+  }
+  for (int k = 0; k < b.n && o.interp_arg; ++k)
+    save_png(as_rgb(b.interp.data() + (size_t)k * b.hwc, b.hwc, s.nochannels, s.png), w, h, s.nochannels, 8,
+             with_suffix(s.jobs[b.j0 + k].out, "_interp", ".png").c_str());
+  if (o.gm_model) write_global_motion(s, b);
+  if (o.disp_on) write_disparities(s, b);
+  if (!o.kitti) write_flows(s, b);
+}
+
+// --odometry: every clip's camera-to-world poses to DIR/poses_<clip>.txt
+static int write_poses(const State& s) {
+  for (size_t c = 0; c < s.odo_rel.size(); ++c) {
+    char name[32];
+    snprintf(name, sizeof(name), "/poses_%04zu.txt", c);
+    const string path = string(s.o.odo_dir) + name;
+    FILE* f = fopen(path.c_str(), "w");
+    double T[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+    for (size_t k = 0; f && k <= s.odo_rel[c].size() / 12; ++k) {
+      if (k > 0) chain_pose(T, &s.odo_rel[c][12 * (k - 1)]);
+      for (int i = 0; i < 12; ++i) fprintf(f, i ? " %.17g" : "%.17g", T[i]);
+      fprintf(f, "\n");
+    }
+    if (!f || fclose(f) != 0) return refuse(1, "cannot write %s", path.c_str());
+  }
+  return 0;
+}
+
+static void print_summary(const State& s, timeval& tv) {
+  if (s.verbosity <= 0) return;
+  const Options& o = s.o;
+  static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
+  printf("TIME (%zu pairs, load + flow + save) (ms): %3g\n", s.done, elapsed_ms(tv));
+  if (s.seq_pairs) printf("SEQUENCE (%zu of %zu pairs from %zu decoded frames)\n", s.seq_pairs, s.done, s.seq_decoded);
+  if (o.warm) printf("WARM START (%zu of %zu pairs from the previous pair's flow)\n", s.warm_pairs, s.done);
+  if (o.tracks)
+    printf("TRACKS clips %d frames %zu seeded %lld leaves %lld inconsistent %lld boundary %lld dropped %lld\n",
+           s.tclip + 1, s.tframes, s.ttotal.seeded, s.ttotal.ended_leaves, s.ttotal.ended_inconsistent,
+           s.ttotal.ended_boundary, s.ttotal.dropped);
+  if (o.desc)
+    printf("DESCRIPTORS clips %d emitted %lld static %lld erratic %lld jump %lld camera %lld\n", s.tclip + 1,
+           s.dtotal.emitted, s.dtotal.rejected_static, s.dtotal.rejected_erratic, s.dtotal.rejected_jump,
+           s.dtotal.rejected_camera);
+  if (o.fisher[0]) {
+    printf("FISHER clips %d descriptors %lld skipped", s.fclips, s.fpushed);
+    for (int b = 0; b < o.fbook.cb.nblocks; ++b) printf(" %lld", s.fskipped[b]);
+    printf("\n");
+  }
+  if (o.gtlist) {
+    print_eval("", s.done, s.eval_total[0]);
+    for (int c = 0; c < s.nclasses && o.bidir; ++c) print_eval(kClassNames[c], s.done, s.eval_total[1 + c]);
+  }
+  if (o.odo_gtlist)
+    printf("ODOEVAL (%zu pairs) t_err %.9g r_err %.9g\n", s.odo_eval, s.odo_eval ? s.odo_terr / s.odo_eval : 0.0,
+           s.odo_eval ? s.odo_rerr / s.odo_eval : 0.0);
+  if (o.sf_gtlist) {
+    print_sfeval("", s.done, s.sf_total[0]);
+    for (int c = 0; c < s.nclasses && o.bidir; ++c) print_sfeval(kClassNames[c], s.done, s.sf_total[1 + c]);
+  }
+}
+
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr,
@@ -1134,1414 +2452,38 @@ int main(int argc, char** argv) {
             argv[0]);
     return 2;
   }
-  int maxb = 64, first_num = 2;
-  bool warm = false, batch_set = false, bidir = false, kitti = false, color = false;
-  float color_max = 0.0f;  // --color-max; 0: every pair's own maximum
-  const char* color_max_arg = nullptr;
-  const char* interp_arg = nullptr;  // --interpolate T
-  float interp_t = 0.0f;
-  const char* gtlist = nullptr;
-  const char* tracks_path = nullptr;  // --tracks PATH
-  const char* desc_path = nullptr;    // --descriptors PATH
-  const char* fisher_arg[2] = {nullptr, nullptr};  // --fisher CODEBOOK PATH
-  bool lr_check = false, disp_fill = false;  // --lr-check, --fill
-  const char* speckle_arg[2] = {nullptr, nullptr};  // --speckle N R
-  const char* camera_arg = nullptr;  // --camera fx,fy,cx,cy,baseline,doffs
-  const char* gm_arg[2] = {nullptr, nullptr};  // --global-motion MODEL PATH
-  const char* stab_arg[3] = {nullptr, nullptr, nullptr};  // --stabilize RADIUS CROP DIR
-  const char* sf_list = nullptr;    // --scene-flow DISPLIST
-  const char* sf_gtlist = nullptr;  // --gt-scene-flow GTLIST
-  const char* odo_dir = nullptr;     // --odometry DIR
-  const char* odo_gtlist = nullptr;  // --gt-poses LIST
-  const char* fuse_arg = nullptr;    // --fuse voxel,trunc,x0,y0,z0,nx,ny,nz
-  bool fuse_mesh = false;            // --mesh
-  for (;;) {
-    if (argc >= first_num + 2 && !strcmp(argv[first_num], "--batch")) {
-      maxb = atoi(argv[first_num + 1]);
-      first_num += 2;
-      batch_set = true;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--warm-start")) {
-      warm = true;
-      first_num += 1;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--bidirectional")) {
-      bidir = true;
-      first_num += 1;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--kitti")) {
-      kitti = true;
-      first_num += 1;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--color")) {
-      color = true;
-      first_num += 1;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--color-max")) {
-      if (argc < first_num + 2 || color_max_arg) {
-        fprintf(stderr, "error: --color-max takes one positive number\n");
-        return 2;
-      }
-      color_max_arg = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--interpolate")) {
-      if (argc < first_num + 2 || interp_arg) {
-        fprintf(stderr, "error: --interpolate takes one time between 0 and 1\n");
-        return 2;
-      }
-      interp_arg = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--tracks")) {
-      if (argc < first_num + 2 || tracks_path) {
-        fprintf(stderr, "error: --tracks takes one output path\n");
-        return 2;
-      }
-      tracks_path = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--descriptors")) {
-      if (argc < first_num + 2 || desc_path) {
-        fprintf(stderr, "error: --descriptors takes one output path\n");
-        return 2;
-      }
-      desc_path = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--fisher")) {
-      if (argc < first_num + 3 || fisher_arg[0]) {
-        fprintf(stderr, "error: --fisher takes a codebook file and an output path\n");
-        return 2;
-      }
-      fisher_arg[0] = argv[first_num + 1];
-      fisher_arg[1] = argv[first_num + 2];
-      first_num += 3;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--lr-check")) {
-      lr_check = true;
-      first_num += 1;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--fill")) {
-      disp_fill = true;
-      first_num += 1;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--speckle")) {
-      if (argc < first_num + 3 || speckle_arg[0]) {
-        fprintf(stderr, "error: --speckle takes a size N and a difference R\n");
-        return 2;
-      }
-      speckle_arg[0] = argv[first_num + 1];
-      speckle_arg[1] = argv[first_num + 2];
-      first_num += 3;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--camera")) {
-      if (argc < first_num + 2 || camera_arg) {
-        fprintf(stderr, "error: --camera takes fx,fy,cx,cy,baseline,doffs\n");
-        return 2;
-      }
-      camera_arg = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--global-motion")) {
-      if (argc < first_num + 3 || gm_arg[0]) {
-        fprintf(stderr, "error: --global-motion takes a model (similarity, affine or homography) and an output path\n");
-        return 2;
-      }
-      gm_arg[0] = argv[first_num + 1];
-      gm_arg[1] = argv[first_num + 2];
-      first_num += 3;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--stabilize")) {
-      if (argc < first_num + 4 || stab_arg[0]) {
-        fprintf(stderr, "error: --stabilize takes a radius, a crop and an output directory\n");
-        return 2;
-      }
-      stab_arg[0] = argv[first_num + 1];
-      stab_arg[1] = argv[first_num + 2];
-      stab_arg[2] = argv[first_num + 3];
-      first_num += 4;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--scene-flow")) {
-      if (argc < first_num + 2 || sf_list) {
-        fprintf(stderr, "error: --scene-flow takes one disparity list file\n");
-        return 2;
-      }
-      sf_list = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt-scene-flow")) {
-      if (argc < first_num + 2 || sf_gtlist) {
-        fprintf(stderr, "error: --gt-scene-flow takes one ground-truth list file\n");
-        return 2;
-      }
-      sf_gtlist = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--odometry")) {
-      if (argc < first_num + 2 || odo_dir) {
-        fprintf(stderr, "error: --odometry takes one output directory\n");
-        return 2;
-      }
-      odo_dir = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--fuse")) {
-      if (argc < first_num + 2 || fuse_arg) {
-        fprintf(stderr, "error: --fuse takes voxel,trunc,x0,y0,z0,nx,ny,nz\n");
-        return 2;
-      }
-      fuse_arg = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--mesh")) {
-      fuse_mesh = true;
-      first_num += 1;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt-poses")) {
-      if (argc < first_num + 2 || odo_gtlist) {
-        fprintf(stderr, "error: --gt-poses takes one list of KITTI poses files\n");
-        return 2;
-      }
-      odo_gtlist = argv[first_num + 1];
-      first_num += 2;
-    } else if (argc >= first_num + 1 && !strcmp(argv[first_num], "--gt")) {
-      if (argc < first_num + 2 || gtlist) {
-        fprintf(stderr, "error: --gt takes one ground-truth list file\n");
-        return 2;
-      }
-      gtlist = argv[first_num + 1];
-      first_num += 2;
-    } else {
-      break;
-    }
-  }
-  if (warm && batch_set) {
-    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --batch\n");
-    return 2;
-  }
-  if (warm && bidir) {
-    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --bidirectional\n");
-    return 2;
-  }
-  if (warm && interp_arg) {
-    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --interpolate\n");
-    return 2;
-  }
-  if (warm && tracks_path) {
-    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --tracks\n");
-    return 2;
-  }
-  if (sf_list && SELECTMODE != 1) {
-    fprintf(stderr, "error: --scene-flow joins flows with disparities; the stereo binaries take no --scene-flow\n");
-    return 2;
-  }
-  if (sf_list && warm) {
-    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --scene-flow\n");
-    return 2;
-  }
-  if (sf_gtlist && !sf_list) {
-    fprintf(stderr, "error: --gt-scene-flow evaluates the scene flow of --scene-flow; give --scene-flow too\n");
-    return 2;
-  }
-  if (odo_dir && SELECTMODE != 1) {
-    fprintf(stderr, "error: --odometry fits the rig's motion from flows; the stereo binaries take no --odometry\n");
-    return 2;
-  }
-  if (odo_dir && warm) {
-    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --odometry\n");
-    return 2;
-  }
-  if (odo_dir && (!sf_list || !camera_arg)) {
-    fprintf(stderr, "error: --odometry needs the disparities of --scene-flow and the stereo camera of --camera\n");
-    return 2;
-  }
-  if (odo_gtlist && !odo_dir) {
-    fprintf(stderr, "error: --gt-poses evaluates the poses of --odometry; give --odometry too\n");
-    return 2;
-  }
-  if (fuse_arg && SELECTMODE != 1) {
-    fprintf(stderr, "error: --fuse places disparities with the poses of --odometry; the stereo binaries take no --fuse\n");
-    return 2;
-  }
-  if (fuse_arg && warm) {
-    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --fuse\n");
-    return 2;
-  }
-  if (fuse_arg && !odo_dir) {
-    fprintf(stderr, "error: --fuse places disparities with the poses of --odometry; give --odometry too\n");
-    return 2;
-  }
-  if (fuse_mesh && !fuse_arg) {
-    fprintf(stderr, "error: --mesh meshes the volume of --fuse; give --fuse too\n");
-    return 2;
-  }
-  ofdis_fuse_params fuse_p;
-  memset(&fuse_p, 0, sizeof(fuse_p));
-  if (fuse_arg) {
-    double v[8];
-    const char* q = fuse_arg;
-    bool ok = true;
-    for (int i = 0; i < 8 && ok; ++i) {
-      char* end = nullptr;
-      v[i] = strtod(q, &end);
-      ok = end != q && (i < 7 ? *end == ',' : *end == 0) && std::isfinite(v[i]);
-      q = end + (i < 7 ? 1 : 0);
-    }
-    for (int i = 5; i < 8 && ok; ++i) ok = v[i] >= 1.0 && v[i] <= (double)(1 << 30) && v[i] == std::floor(v[i]);
-    ok = ok && (float)v[0] > 0.0f && (float)v[1] > 0.0f && v[0] <= FLT_MAX && v[1] <= FLT_MAX &&
-         std::fabs(v[2]) <= FLT_MAX && std::fabs(v[3]) <= FLT_MAX && std::fabs(v[4]) <= FLT_MAX &&
-         v[5] * v[6] * v[7] <= (double)(1 << 30);
-    if (!ok) {
-      fprintf(stderr, "error: --fuse takes eight numbers voxel,trunc,x0,y0,z0,nx,ny,nz with voxel and trunc > 0, "
-                      "integer sizes >= 1 and at most 2^30 voxels, got %s\n", fuse_arg);
-      return 2;
-    }
-    fuse_p.voxel = (float)v[0];
-    fuse_p.trunc = (float)v[1];
-    for (int e = 0; e < 3; ++e) fuse_p.origin[e] = (float)v[2 + e];
-    fuse_p.nx = (int)v[5];
-    fuse_p.ny = (int)v[6];
-    fuse_p.nz = (int)v[7];
-    fuse_p.max_weight = 64.0f;
-    fuse_p.color = 1;
-  }
-  // --camera on a flow binary belongs to --scene-flow
-  const bool disp_on = lr_check || disp_fill || speckle_arg[0] || (camera_arg && !sf_list);
-  if (disp_on && SELECTMODE == 1) {
-    fprintf(stderr, "error: --lr-check, --speckle, --fill and --camera filter stereo disparities; the flow binaries "
-                    "take none of them\n");
-    return 2;
-  }
-  if (warm && disp_on) {
-    fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --lr-check, --speckle, --fill or --camera\n");
-    return 2;
-  }
-  int gm_model = 0;  // --global-motion: OFDIS_MOTION_*
-  if (gm_arg[0]) {
-    if (SELECTMODE != 1) {
-      fprintf(stderr, "error: --global-motion fits the camera motion of flows; the stereo binaries take no "
-                      "--global-motion\n");
-      return 2;
-    }
-    if (warm) {
-      fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --global-motion\n");
-      return 2;
-    }
-    gm_model = !strcmp(gm_arg[0], "similarity") ? OFDIS_MOTION_SIMILARITY
-               : !strcmp(gm_arg[0], "affine")   ? OFDIS_MOTION_AFFINE
-               : !strcmp(gm_arg[0], "homography") ? OFDIS_MOTION_HOMOGRAPHY : 0;
-    if (!gm_model) {
-      fprintf(stderr, "error: --global-motion takes the model similarity, affine or homography, got %s\n", gm_arg[0]);
-      return 2;
-    }
-  }
-  if (desc_path) {
-    if (SELECTMODE != 1) {
-      fprintf(stderr, "error: --descriptors describes the tracks of flows; the stereo binaries take no --descriptors\n");
-      return 2;
-    }
-    if (warm) {
-      fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --descriptors\n");
-      return 2;
-    }
-    if (!tracks_path) {
-      fprintf(stderr, "error: --descriptors describes the clips of --tracks; give --tracks too\n");
-      return 2;
-    }
-  }
-  if (fisher_arg[0]) {
-    if (SELECTMODE != 1) {
-      fprintf(stderr, "error: --fisher encodes the descriptors of flows; the stereo binaries take no --fisher\n");
-      return 2;
-    }
-    if (warm) {
-      fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --fisher\n");
-      return 2;
-    }
-    if (!tracks_path) {
-      fprintf(stderr, "error: --fisher encodes the clips of --tracks; give --tracks too\n");
-      return 2;
-    }
-  }
-  ofdis_traj_params trp;  // --descriptors, --fisher: Wang and Schmid's settings
-  memset(&trp, 0, sizeof(trp));
-  trp.L = 15;
-  trp.nt = 3;
-  trp.N = 32;
-  trp.ns = 2;
-  trp.min_flow = 0.4f;
-  trp.eps = 0.05f;
-  trp.min_disp = 1.0f;
-  trp.min_var = (float)std::sqrt(3.0);
-  trp.max_var = 50.0f;
-  trp.max_dis = 20.0f;
-  const int tdim = 2 * trp.L + trp.ns * trp.ns * trp.nt * 33;
-  FisherBook fbook;  // --fisher: the codebook, whose blocks must be the descriptors' (shape, HOG, HOF, MBHx, MBHy)
-  if (fisher_arg[0]) {
-    string err;
-    if (!read_fisher_book(fisher_arg[0], fbook, err)) {
-      fprintf(stderr, "error: %s: %s\n", fisher_arg[0], err.c_str());
-      return 2;
-    }
-    const int c = trp.nt * trp.ns * trp.ns, din[5] = {2 * trp.L, 8 * c, 9 * c, 8 * c, 8 * c};
-    bool match = fbook.cb.desc_dim == tdim && fbook.cb.nblocks == 5;
-    for (int b = 0, off = 0; match && b < 5; off += din[b++])
-      match = fbook.cb.blocks[b].offset == off && fbook.cb.blocks[b].dim_in == din[b];
-    if (!match) {
-      fprintf(stderr, "error: %s: the codebook's blocks are not the descriptors' (desc_dim %d, blocks 0+%d, %d+%d, "
-                      "%d+%d, %d+%d, %d+%d)\n", fisher_arg[0], tdim, din[0], din[0], din[1], din[0] + din[1], din[2],
-              din[0] + din[1] + din[2], din[3], tdim - din[4], din[4]);
-      return 2;
-    }
-  }
-  const bool traj_stage = desc_path || fisher_arg[0];  // the descriptor stage runs in place of the tracker's calls
-  ofdis_stab_params stp;  // --stabilize
-  memset(&stp, 0, sizeof(stp));
-  vector<double> stab_wts;
-  if (stab_arg[0]) {
-    if (SELECTMODE != 1) {
-      fprintf(stderr, "error: --stabilize smooths the camera motion of flows; the stereo binaries take no --stabilize\n");
-      return 2;
-    }
-    if (warm) {
-      fprintf(stderr, "error: --warm-start runs one pair per launch; it takes no --stabilize\n");
-      return 2;
-    }
-    if (!gm_arg[0]) {
-      fprintf(stderr, "error: --stabilize smooths the models of --global-motion; give --global-motion too\n");
-      return 2;
-    }
-    char *e0 = nullptr, *e1 = nullptr;
-    const long r = strtol(stab_arg[0], &e0, 10);
-    const float crop = strtof(stab_arg[1], &e1);
-    if (e0 == stab_arg[0] || *e0 || r < 1 || r > 64 || e1 == stab_arg[1] || *e1 || !(crop >= 0.0f && crop < 0.5f)) {
-      fprintf(stderr, "error: --stabilize takes a radius 1..64 and a crop 0 <= CROP < 0.5, got %s %s\n", stab_arg[0],
-              stab_arg[1]);
-      return 2;
-    }
-    stp.radius = (int)r;
-    stp.crop = crop;
-    stp.limit = crop > 0.0f ? 1 : 0;
-    for (int d = 0; d <= stp.radius; ++d) stab_wts.push_back(exp(-(double)(d * d) / (2.0 * stp.radius)));
-  }
-  ofdis_disp_filter dfilt;
-  memset(&dfilt, 0, sizeof(dfilt));
-  dfilt.lr_check = lr_check ? 1 : 0;
-  dfilt.alpha = 0.0f;
-  dfilt.beta = 1.0f;
-  dfilt.speckle_diff = 1.0f;
-  dfilt.fill = disp_fill ? 1 : 0;
-  if (speckle_arg[0]) {
-    char *e0 = nullptr, *e1 = nullptr;
-    const long sz = strtol(speckle_arg[0], &e0, 10);
-    const float diff = strtof(speckle_arg[1], &e1);
-    if (e0 == speckle_arg[0] || *e0 || sz < 1 || sz > INT_MAX || e1 == speckle_arg[1] || *e1 ||
-        !(diff >= 0.0f && diff <= FLT_MAX)) {
-      fprintf(stderr, "error: --speckle takes a size N >= 1 and a finite difference R >= 0, got %s %s\n", speckle_arg[0],
-              speckle_arg[1]);
-      return 2;
-    }
-    dfilt.speckle_size = (int)sz;
-    dfilt.speckle_diff = diff;
-  }
-  ofdis_stereo_camera dcam;
-  memset(&dcam, 0, sizeof(dcam));
-  if (camera_arg) {
-    float v[6];
-    const char* q = camera_arg;
-    bool ok = true;
-    for (int i = 0; i < 6 && ok; ++i) {
-      char* end = nullptr;
-      v[i] = strtof(q, &end);
-      ok = end != q && (i < 5 ? *end == ',' : *end == 0) && v[i] >= -FLT_MAX && v[i] <= FLT_MAX;
-      q = end + (i < 5 ? 1 : 0);
-    }
-    if (!ok || !(v[0] > 0.0f) || !(v[1] > 0.0f) || !(v[4] > 0.0f)) {
-      fprintf(stderr, "error: --camera takes six finite numbers fx,fy,cx,cy,baseline,doffs with fx, fy and baseline "
-                      "> 0, got %s\n", camera_arg);
-      return 2;
-    }
-    dcam = ofdis_stereo_camera{v[0], v[1], v[2], v[3], v[4], v[5]};
-  }
-  if (interp_arg) {
-    char* end = nullptr;
-    interp_t = strtof(interp_arg, &end);
-    if (end == interp_arg || *end || !(interp_t > 0.0f && interp_t < 1.0f)) {
-      fprintf(stderr, "error: --interpolate takes a time T with 0 < T < 1, got %s\n", interp_arg);
-      return 2;
-    }
-  }
-  // --interpolate and --tracks need the backward flows: the backward slots run whenever one of them is given
-  const bool two_way = bidir || interp_arg || tracks_path || lr_check;
-  if (color_max_arg) {
-    char* end = nullptr;
-    color_max = strtof(color_max_arg, &end);
-    if (!color) {
-      fprintf(stderr, "error: --color-max needs --color\n");
-      return 2;
-    }
-    if (end == color_max_arg || *end || !(color_max > 0.0f && color_max <= FLT_MAX)) {
-      fprintf(stderr, "error: --color-max takes a positive finite number, got %s\n", color_max_arg);
-      return 2;
-    }
-  }
-  if (warm) maxb = 1;
-  const int nnum = argc - first_num;
-  if (maxb < 1 || (nnum > 1 && nnum != 20)) {
-    fprintf(stderr, "error: expected 0, 1 or exactly 20 numbers, got %d\n", nnum);
-    return 2;
-  }
-  struct Job { string a, b, out; };
+  Options o;
+  if (int rc = parse_flags(argc, argv, o)) return rc;
+  if (int rc = check_options(o)) return rc;
+  vector<string> words;
+  if (!read_words(argv[1], words)) return refuse(1, "cannot read %s", argv[1]);
   vector<Job> jobs;
-  {
-    FILE* f = fopen(argv[1], "r");
-    if (!f) {
-      fprintf(stderr, "error: cannot read %s\n", argv[1]);
-      return 1;
-    }
-    char a[4096], b[4096], o[4096];
-    while (fscanf(f, "%4095s %4095s %4095s", a, b, o) == 3) jobs.push_back({a, b, o});
-    fclose(f);
-  }
-  const int nochannels = (SELECTCHANNEL == 3) ? 3 : 1;
-  const int nop = (SELECTMODE == 1) ? 2 : 1;
-  // --gt: the list, then every file against its pair's image size, before any device work
-  vector<string> gts;
-  if (gtlist) {
-    FILE* f = fopen(gtlist, "r");
-    if (!f) {
-      fprintf(stderr, "error: cannot read %s\n", gtlist);
-      return 1;
-    }
-    char g[4096];
-    while (fscanf(f, "%4095s", g) == 1) gts.push_back(g);
-    fclose(f);
-    if (gts.size() != jobs.size()) {
-      fprintf(stderr, "error: --gt: %s lists %zu ground-truth files for %zu pairs\n", gtlist, gts.size(), jobs.size());
-      return 2;
-    }
-    vector<float> gtf;
-    for (size_t k = 0; k < jobs.size(); ++k) {
-      int iw = 0, ih = 0;
-      string err;
-      if (!image_size(jobs[k].a.c_str(), iw, ih)) {
-        fprintf(stderr, "error: cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)\n",
-                jobs[k].a.c_str(), jobs[k].b.c_str());
-        return 1;
-      }
-      if (!read_gt_file(gts[k].c_str(), iw, ih, nop, gtf, err)) {
-        fprintf(stderr, "error: %s: %s\n", gts[k].c_str(), err.c_str());
-        return 1;
-      }
-    }
-  }
-  // --scene-flow / --gt-scene-flow: two and three files per pair, each checked against its pair's image size before
-  // any device work
-  vector<string> sf_files, sf_gts;
-  for (int li = 0; li < 2; ++li) {
-    const char* list = li ? sf_gtlist : sf_list;
-    vector<string>& files = li ? sf_gts : sf_files;
-    const size_t per = li ? 3 : 2;
-    if (!list) continue;
-    FILE* f = fopen(list, "r");
-    if (!f) {
-      fprintf(stderr, "error: cannot read %s\n", list);
-      return 1;
-    }
-    char g[4096];
-    while (fscanf(f, "%4095s", g) == 1) files.push_back(g);
-    fclose(f);
-    if (files.size() != per * jobs.size()) {
-      fprintf(stderr, "error: %s: %s lists %zu files for %zu pairs (%zu per pair)\n",
-              li ? "--gt-scene-flow" : "--scene-flow", list, files.size(), jobs.size(), per);
-      return 2;
-    }
-    vector<float> tmp;
-    for (size_t k = 0; k < files.size(); ++k) {
-      int iw = 0, ih = 0;
-      string err;
-      const Job& jb = jobs[k / per];
-      if (!image_size(jb.a.c_str(), iw, ih)) {
-        fprintf(stderr, "error: cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)\n", jb.a.c_str(),
-                jb.b.c_str());
-        return 1;
-      }
-      if (!read_gt_file(files[k].c_str(), iw, ih, li && k % 3 == 2 ? 2 : 1, tmp, err)) {
-        fprintf(stderr, "error: %s: %s\n", files[k].c_str(), err.c_str());
-        return 2;
-      }
-    }
-  }
-  // --odometry: the clip and frame of every pair, the ground-truth poses of every clip and the output files, before
-  // any device work
-  vector<int> odo_clip(jobs.size(), 0), odo_frame(jobs.size(), 0);
-  vector<vector<double>> odo_gt;  // per clip, 12 numbers per line
-  vector<vector<double>> odo_rel;  // per clip, 12 numbers per pair (filled as the pairs are computed)
-  FILE* odo_file = nullptr;
-  if (odo_dir) {
-    int nclips = 0;
-    for (size_t k = 0; k < jobs.size(); ++k) {
-      const bool cont = k > 0 && jobs[k].a == jobs[k - 1].b;
-      odo_clip[k] = cont ? odo_clip[k - 1] : nclips++;
-      odo_frame[k] = cont ? odo_frame[k - 1] + 1 : 0;
-    }
-    odo_rel.resize(nclips);
-    if (odo_gtlist) {
-      FILE* f = fopen(odo_gtlist, "r");
-      if (!f) {
-        fprintf(stderr, "error: cannot read %s\n", odo_gtlist);
-        return 2;
-      }
-      vector<string> files;
-      char g[4096];
-      while (fscanf(f, "%4095s", g) == 1) files.push_back(g);
-      fclose(f);
-      if ((int)files.size() != nclips) {
-        fprintf(stderr, "error: --gt-poses: %s lists %zu poses files for %d clips\n", odo_gtlist, files.size(), nclips);
-        return 2;
-      }
-      vector<int> need(nclips, 0);
-      for (size_t k = 0; k < jobs.size(); ++k) need[odo_clip[k]] = odo_frame[k] + 2;
-      for (int c = 0; c < nclips; ++c) {
-        FILE* pf = fopen(files[c].c_str(), "r");
-        if (!pf) {
-          fprintf(stderr, "error: cannot read %s\n", files[c].c_str());
-          return 2;
-        }
-        vector<double> v;
-        double x;
-        while (fscanf(pf, "%lf", &x) == 1) v.push_back(x);
-        const bool eof = feof(pf);
-        fclose(pf);
-        if (!eof || v.size() % 12 || (int)(v.size() / 12) < need[c]) {
-          fprintf(stderr, "error: %s: a KITTI poses file of at least %d lines of 12 numbers, got %zu numbers\n",
-                  files[c].c_str(), need[c], v.size());
-          return 2;
-        }
-        odo_gt.push_back(v);
-      }
-    }
-    const string path = string(odo_dir) + "/odometry.txt";
-    odo_file = fopen(path.c_str(), "w");
-    if (!odo_file) {
-      fprintf(stderr, "error: --odometry: cannot write %s\n", path.c_str());
-      return 2;
-    }
-  }
-  double odo_terr = 0.0, odo_rerr = 0.0;
-  size_t odo_eval = 0;
-  vector<double> odo_pose;
-  vector<ofdis_motion_stats> odo_stats;
-  vector<uint8_t> odo_mask;
-  vector<float> odo_om;
-  double fuse_T[12];              // --fuse: the chained pose of the clip's next image1
-  int fuse_frames = 0;            // frames pushed into the clip's volume
-  vector<double> fuse_poses;
-  vector<ofdis_fuse_point> fuse_pts;
-  vector<unsigned int> fuse_faces;  // --mesh
-  // --descriptors, --fisher: every pair's frames hold an N x N patch, checked before any device work
-  for (size_t k = 0; k < jobs.size() && traj_stage; ++k) {
-    int iw = 0, ih = 0;
-    if (!image_size(jobs[k].a.c_str(), iw, ih)) {
-      fprintf(stderr, "error: cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)\n",
-              jobs[k].a.c_str(), jobs[k].b.c_str());
-      return 1;
-    }
-    if (iw < trp.N || ih < trp.N) {
-      fprintf(stderr, "error: --%s needs frames of at least %d x %d, %s is %d x %d\n",
-              desc_path ? "descriptors" : "fisher", trp.N, trp.N, jobs[k].a.c_str(), iw, ih);
-      return 2;
-    }
-  }
-  FILE* desc_file = nullptr;
-  if (desc_path) {
-    desc_file = fopen(desc_path, "w");
-    if (!desc_file) {
-      fprintf(stderr, "error: cannot write %s\n", desc_path);
-      return 1;
-    }
-    fprintf(desc_file, "# clip id start mean_x mean_y sd_x sd_y length d0 .. d%d\n", tdim - 1);
-  }
-  FILE* fisher_file = nullptr;
-  int fv_floats = 0;
-  if (fisher_arg[0]) {
-    fisher_file = fopen(fisher_arg[1], "w");
-    if (!fisher_file) {
-      fprintf(stderr, "error: cannot write %s\n", fisher_arg[1]);
-      if (desc_file) fclose(desc_file);
-      return 1;
-    }
-    for (int b = 0; b < fbook.cb.nblocks; ++b) fv_floats += 2 * fbook.cb.K * fbook.cb.blocks[b].dim;
-    fprintf(fisher_file, "# clip n_desc n_0 .. n_%d fv0 .. fv%d\n", fbook.cb.nblocks - 1, fv_floats - 1);
-  }
-  FILE* tracks_file = nullptr;
-  if (tracks_path) {
-    tracks_file = fopen(tracks_path, "w");
-    if (!tracks_file) {
-      fprintf(stderr, "error: cannot write %s\n", tracks_path);
-      if (desc_file) fclose(desc_file);
-      if (fisher_file) fclose(fisher_file);
-      return 1;
-    }
-    fprintf(tracks_file, "# clip frame id x y\n");
-  }
-  FILE* stab_file = nullptr;
-  const string stab_txt = stab_arg[0] ? string(stab_arg[2]) + "/stab.txt" : string();
-  if (stab_arg[0]) {
-    stab_file = fopen(stab_txt.c_str(), "w");
-    if (!stab_file) {
-      fprintf(stderr, "error: cannot write %s\n", stab_txt.c_str());
-      if (tracks_file) fclose(tracks_file);
-      if (desc_file) fclose(desc_file);
-      if (fisher_file) fclose(fisher_file);
-      return 1;
-    }
-  }
-  FILE* gm_file = nullptr;
-  if (gm_model) {
-    gm_file = fopen(gm_arg[1], "w");
-    if (!gm_file) {
-      fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
-      if (tracks_file) fclose(tracks_file);
-      if (desc_file) fclose(desc_file);
-      if (fisher_file) fclose(fisher_file);
-      if (stab_file) fclose(stab_file);
-      return 1;
-    }
-  }
-  const int nclasses = bidir ? 3 : 1;  // with --bidirectional the forward consistency mask's classes
-  vector<ofdis_error_stats> eval_total(nclasses + 1), eval_pairs;  // [0]: all pixels, [1 + c]: class c
-  memset(eval_total.data(), 0, sizeof(ofdis_error_stats) * eval_total.size());
-  vector<float> gt_batch, gt_one;
-  // --scene-flow: the batch's disparities, ground truth and outputs; the totals ([0]: all pixels, [1 + c]: class c)
-  vector<float> sf_d0, sf_d1, sf_g0, sf_g1, sf_gf, sf_w, sf_m;
-  vector<ofdis_sf_stats> sf_pairs, sf_total(nclasses + 1);
-  memset(sf_total.data(), 0, sizeof(ofdis_sf_stats) * sf_total.size());
+  for (size_t i = 0; i + 3 <= words.size(); i += 3) jobs.push_back({words[i], words[i + 1], words[i + 2]});
+  const ClipIndex clips = index_clips(jobs);
+  Inputs in;
+  if (int rc = read_inputs(o, jobs, clips, in)) return rc;
+  ListOutputs out;
+  if (int rc = open_outputs(o, jobs, out)) return rc;
   timeval tv;
   gettimeofday(&tv, NULL);
-  size_t done = 0, seq_pairs = 0, seq_decoded = 0, warm_pairs = 0;
-  ofdis_ctx* ctx = nullptr;
-  int ctx_w = -1, ctx_h = -1, verbosity = 0;
-  vector<uint8_t> frames;
-  vector<float> flows;
-  vector<uint16_t> kflows;  // --kitti: the encoded slots
-  vector<uint8_t> masks;
-  vector<uint8_t> colors;  // --color: the color images of the slots
-  vector<uint8_t> interp, interp_png;  // --interpolate: the frames at time T, one written as RGB
-  vector<float> ddisp, ddepth, dxyz;  // --lr-check / --speckle / --fill / --camera: the filtered outputs
-  vector<uint8_t> dstatus, dply;
-  vector<double> gm_models;  // --global-motion: the models, stats and per-pixel outputs of the batch
-  vector<ofdis_motion_stats> gm_stats;
-  vector<uint8_t> gm_mask, gm_reg, gm_png;
-  vector<float> gm_res;
-  Image8 last;  // image2 of the previous batch's last pair
-  // --tracks: the tracker's points and counts, the clip being tracked (-1 none) and its next frame, the totals of the
-  // finished clips
-  vector<ofdis_track_point> tpoints;
-  vector<int> tcounts;
-  int tclip = -1, tframe = 0;
-  size_t tframes = 0;
-  ofdis_track_stats ttotal;
-  memset(&ttotal, 0, sizeof(ttotal));
-  // --descriptors: the segments of a call and the totals of the finished clips
-  vector<ofdis_traj_record> trec;
-  vector<float> tdesc;
-  vector<int> tndesc;
-  ofdis_traj_stats dtotal;
-  memset(&dtotal, 0, sizeof(dtotal));
-  // --fisher: whether the clip's encoder is live, the vector of a take, the totals, the status of the last take
-  bool fisher_live = false;
-  vector<float> fvec(fv_floats);
-  long long fpushed = 0, fskipped[OFDIS_FISHER_MAX_BLOCKS] = {0};
-  int fclips = 0, fisher_rc = OFDIS_OK;
-  auto end_clip = [&]() {  // adds the tracked clip's counters to the totals; --fisher: takes the clip's vector
-    if (fisher_live) {
-      fisher_live = false;
-      ofdis_fisher_stats fs;
-      fisher_rc = ofdis_fisher_take(ctx, fvec.data(), nullptr, &fs, OFDIS_MEM_HOST);
-      if (fisher_rc == OFDIS_OK) {
-        fprintf(fisher_file, "%d %lld", tclip, fs.pushed);
-        for (int b = 0; b < fbook.cb.nblocks; ++b) fprintf(fisher_file, " %lld", fs.n[b]);
-        for (int i = 0; i < fv_floats; ++i) fprintf(fisher_file, " %.9g", (double)fvec[i]);
-        fprintf(fisher_file, "\n");
-        ++fclips;
-        fpushed += fs.pushed;
-        for (int b = 0; b < fbook.cb.nblocks; ++b) fskipped[b] += fs.skipped[b];
-      }
-    }
-    ofdis_track_stats st;
-    if (tclip < 0 || ofdis_track_stats_get(ctx, &st) != OFDIS_OK) return;
-    ttotal.seeded += st.seeded;
-    ttotal.ended_leaves += st.ended_leaves;
-    ttotal.ended_inconsistent += st.ended_inconsistent;
-    ttotal.ended_boundary += st.ended_boundary;
-    ttotal.dropped += st.dropped;
-    ofdis_traj_stats ds;
-    if (!traj_stage || ofdis_traj_stats_get(ctx, &ds) != OFDIS_OK) return;
-    dtotal.emitted += ds.emitted;
-    dtotal.rejected_static += ds.rejected_static;
-    dtotal.rejected_erratic += ds.rejected_erratic;
-    dtotal.rejected_jump += ds.rejected_jump;
-    dtotal.rejected_camera += ds.rejected_camera;
-  };
-  auto write_desc = [&](int count) {
-    for (int i = 0; i < count; ++i) {
-      const ofdis_traj_record& r = trec[i];
-      fprintf(desc_file, "%d %d %d %.9g %.9g %.9g %.9g %.9g", tclip, r.id, r.start, (double)r.mean_x, (double)r.mean_y,
-              (double)r.sd_x, (double)r.sd_y, (double)r.length);
-      const float* d = tdesc.data() + (size_t)i * tdim;
-      for (int e = 0; e < tdim; ++e) fprintf(desc_file, " %.9g", (double)d[e]);
-      fprintf(desc_file, "\n");
-    }
-  };
-  // --stabilize: the emitted frames and records, the clip being stabilised (-1 none), whether its stabiliser is live
-  // and its frame size
-  vector<uint8_t> sbuf, spng;
-  vector<ofdis_stab_frame> sinfo;
-  int sclip = -1, sw = 0, sh = 0;
-  bool stab_live = false;
-  auto write_stab = [&](int count) {
-    const size_t shwc = (size_t)sw * sh * nochannels;
-    for (int i = 0; i < count; ++i) {
-      const ofdis_stab_frame& f = sinfo[i];
-      fprintf(stab_file, "%d %lld", sclip, f.frame);
-      for (int e = 0; e < 9; ++e) fprintf(stab_file, " %.17g", f.correction[e]);
-      fprintf(stab_file, " %.17g %d\n", f.lambda, f.status);
-      const uint8_t* im = sbuf.data() + (size_t)i * shwc;
-      if (nochannels == 3) {  // the decoder's BGR -> RGB
-        spng.resize(shwc);
-        for (size_t q = 0; q < shwc; q += 3) {
-          spng[q] = im[q + 2];
-          spng[q + 1] = im[q + 1];
-          spng[q + 2] = im[q];
-        }
-        im = spng.data();
-      }
-      char name[64];
-      snprintf(name, sizeof(name), "/stab_%04d_%06lld.png", sclip, f.frame);
-      save_png(im, sw, sh, nochannels, 8, (string(stab_arg[2]) + name).c_str());
-    }
-  };
-  auto stab_end = [&]() -> int {  // emits the rest of the clip being stabilised
-    if (!stab_live) return OFDIS_OK;
-    stab_live = false;
-    sbuf.resize((size_t)stp.radius * sw * sh * nochannels);
-    sinfo.resize(stp.radius);
-    int count = 0;
-    const int rc = ofdis_stab_finish(ctx, sbuf.data(), sinfo.data(), &count, OFDIS_MEM_HOST);
-    if (rc == OFDIS_OK) write_stab(count);
-    return rc;
-  };
-  auto write_tracks = [&](const ofdis_track_point* p, int count) {
-    for (int i = 0; i < count; ++i)
-      fprintf(tracks_file, "%d %d %d %.9g %.9g\n", tclip, tframe, p[i].id, (double)p[i].x, (double)p[i].y);
-    ++tframe;
-    ++tframes;
-  };
-  size_t j0 = 0;
-  while (j0 < jobs.size()) {
-    // load up to maxb pairs of one size; a frame that continues the previous pair is not decoded again
-    vector<Image8> imgs;  // decoded frames of this batch
-    vector<int> ia, ib;   // per pair: indices of image1, image2 in imgs
-    int w = 0, h = 0, n = 0, decoded = 0;
-    while (j0 + n < jobs.size() && n < maxb) {
-      const Job& jb = jobs[j0 + n];
-      const bool in_batch = n > 0 && jb.a == jobs[j0 + n - 1].b;          // image1 = this batch's last frame
-      const bool from_last = n == 0 && j0 > 0 && jb.a == jobs[j0 - 1].b;  // image1 = the previous batch's last frame
-      Image8 a8, b8;
-      if (from_last) a8 = last;
-      const bool ok = in_batch || from_last || load_image(jb.a.c_str(), nochannels, a8);
-      const Image8& ra = in_batch ? imgs[ib.back()] : a8;
-      if (!ok || !load_image(jb.b.c_str(), nochannels, b8) || ra.w != b8.w || ra.h != b8.h) {
-        fprintf(stderr, "error: cannot read the pair %s %s (binary PGM/PPM or 8-bit PNG of equal size)\n",
-                jb.a.c_str(), jb.b.c_str());
-        if (ctx) ofdis_destroy(ctx);
-        return 1;
-      }
-      if (n == 0) { w = b8.w; h = b8.h; }
-      else if (b8.w != w || b8.h != h) break;  // next group
-      if (in_batch) ia.push_back(ib.back());
-      else {
-        decoded += from_last ? 0 : 1;
-        ia.push_back((int)imgs.size());
-        imgs.push_back(std::move(a8));
-      }
-      ib.push_back((int)imgs.size());
-      imgs.push_back(std::move(b8));
-      ++decoded;
-      ++n;
-    }
-    bool seq = n >= 2;
-    for (int k = 1; k < n && seq; ++k) seq = ia[k] == ib[k - 1];
-    frames.clear();
-    if (seq) {
-      frames.insert(frames.end(), imgs[ia[0]].px.begin(), imgs[ia[0]].px.end());
-      for (int k = 0; k < n; ++k) frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
-      seq_pairs += n;
-      seq_decoded += decoded;
-    } else {
-      for (int k = 0; k < n; ++k) {
-        frames.insert(frames.end(), imgs[ia[k]].px.begin(), imgs[ia[k]].px.end());
-        frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
-      }
-      for (int k = 0; k < n && two_way; ++k) {  // the swapped copies
-        frames.insert(frames.end(), imgs[ib[k]].px.begin(), imgs[ib[k]].px.end());
-        frames.insert(frames.end(), imgs[ia[k]].px.begin(), imgs[ia[k]].px.end());
-      }
-    }
-    last = std::move(imgs[ib.back()]);
+  State s(o, jobs, clips, in, out);
+  Batch b;
+  for (size_t j0 = 0; j0 < jobs.size(); j0 += b.n) {
+    if (int rc = load_batch(s, b, j0)) return rc;
     CliParams P;
-    parse_cli_params(nnum, argv + first_num, w, P);
-    verbosity = P.verbosity;
-    if (w != ctx_w || h != ctx_h) {
-      end_clip();  // a pair of another size never continues the previous one
-      if (fisher_rc != OFDIS_OK || stab_end() != OFDIS_OK) {
-        fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
-        ofdis_destroy(ctx);
-        return 1;
-      }
-      if (ctx) ofdis_destroy(ctx);
-      ctx = nullptr;
-      ofdis_params p;
-      memset(&p, 0, sizeof(p));
-      p.sc_f = P.lv_f; p.sc_l = P.lv_l; p.max_iter = P.maxiter; p.min_iter = P.miniter;
-      p.dp_thresh = P.mindprate; p.dr_thresh = P.mindrrate; p.res_thresh = P.minimgerr;
-      p.p_samp_s = P.patchsz; p.patove = P.poverl; p.usefbcon = P.usefbcon ? 1 : 0; p.costfct = P.costfct;
-      p.noc = nochannels; p.patnorm = P.patnorm; p.usetvref = P.usetvref ? 1 : 0;
-      p.tv_alpha = P.tv_alpha; p.tv_gamma = P.tv_gamma; p.tv_delta = P.tv_delta;
-      p.tv_innerit = P.tv_innerit; p.tv_solverit = P.tv_solverit; p.tv_sor = P.tv_sor; p.verbosity = P.verbosity;
-      const int scf = 1 << (warm ? P.lv_f + 1 : P.lv_f);
-      const int rc = ofdis_create(&ctx, 0, nullptr, &p, nop, (w + scf - 1) / scf * scf, (h + scf - 1) / scf * scf,
-                                  P.patchsz, two_way ? 2 * maxb : maxb);
-      if (rc != OFDIS_OK) {
-        fprintf(stderr, "error: ofdis_create failed with status %d for %dx%d frames\n", rc, w, h);
-        return 1;
-      }
-      ofdis_set_graph_mode(ctx, 1);
-      ctx_w = w;
-      ctx_h = h;
-    }
-    const int slots = two_way ? 2 * n : n;  // two-way: forward slots [0, n), backward slots [n, 2n)
-    const int kch = nop == 2 ? 3 : 1;     // --kitti: uint16 values per pixel
-    if (kitti) kflows.resize((size_t)slots * w * h * kch);
-    else flows.resize((size_t)slots * w * h * nop);
-    int rc;
-    if (two_way && seq) {
-      rc = ofdis_upload_sequence_bidir_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
-    } else if (two_way) {
-      rc = ofdis_upload_frames_u8(ctx, 0, 2 * n, frames.data(), w, h, OFDIS_MEM_HOST);
-      if (rc == OFDIS_OK) rc = ofdis_set_swapped_slots(ctx, 0, n, 0);
-      if (rc == OFDIS_OK) rc = ofdis_set_swapped_slots(ctx, n, 2 * n, 1);
-    } else {
-      rc = seq ? ofdis_upload_sequence_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST)
-               : ofdis_upload_frames_u8(ctx, 0, n, frames.data(), w, h, OFDIS_MEM_HOST);
-    }
-    // warm start: the context still holds the previous pair's flow (same size, so it was not recreated)
-    const bool from_prev = warm && j0 > 0 && jobs[j0].a == jobs[j0 - 1].b;
-    if (rc == OFDIS_OK && from_prev) rc = ofdis_set_initflow_from_result(ctx, 0, 1, 0, w, h);
-    warm_pairs += from_prev ? 1 : 0;
-    if (rc == OFDIS_OK) rc = ofdis_run(ctx, slots, from_prev ? 1 : 0);
-    if (rc == OFDIS_OK)
-      rc = kitti ? ofdis_get_flow_fullres_encoded(ctx, 0, slots, OFDIS_ENC_KITTI, kflows.data(), w, h, OFDIS_MEM_HOST)
-                 : ofdis_get_flow_fullres(ctx, 0, slots, flows.data(), w, h, OFDIS_MEM_HOST);
-    if (rc == OFDIS_OK && color) {
-      colors.resize((size_t)slots * w * h * 3);
-      rc = ofdis_flow_color_fullres(ctx, 0, slots, colors.data(), nullptr, color_max, w, h, OFDIS_MEM_HOST);
-    }
-    if (rc == OFDIS_OK && bidir) {
-      masks.resize((size_t)n * w * h);
-      rc = ofdis_consistency_fullres(ctx, 0, n, n, masks.data(), nullptr, nop == 2 ? 0.01f : 0.0f,
-                                     nop == 2 ? 0.5f : 1.0f, w, h, OFDIS_MEM_HOST);
-    }
-    const size_t hwc = (size_t)w * h * nochannels;
-    if (rc == OFDIS_OK && interp_arg) {
-      // image1 / image2 of pair k: frames k and k + 1 of a clip, or the k-th pair of the pairs layout
-      interp.resize((size_t)n * hwc);
-      rc = ofdis_interpolate_fullres(ctx, 0, n, n, frames.data(), frames.data() + hwc, seq ? hwc : 2 * hwc, interp_t,
-                                     nop == 2 ? 0.01f : 0.0f, nop == 2 ? 0.5f : 1.0f, interp.data(), nullptr, w, h,
-                                     OFDIS_MEM_HOST);
-    }
-    if (rc == OFDIS_OK && gm_model) {
-      // image2 of pair k: frame k + 1 of a clip, or the second image of the k-th pair
-      const size_t np = (size_t)n * w * h;
-      gm_models.resize((size_t)9 * n);
-      gm_stats.resize(n);
-      gm_mask.resize(np);
-      gm_res.resize(2 * np);
-      gm_reg.resize((size_t)n * hwc);
-      ofdis_motion_params mp;
-      memset(&mp, 0, sizeof(mp));
-      mp.model = gm_model;
-      mp.step = 8;
-      mp.fb_check = bidir ? 1 : 0;
-      mp.alpha = 0.01f;
-      mp.beta = 0.5f;
-      mp.hypotheses = 1024;
-      mp.threshold = 1.0f;
-      mp.refine = 3;
-      mp.seed = 0;
-      rc = ofdis_global_motion_fullres(ctx, 0, n, n, &mp, frames.data() + hwc, seq ? hwc : 2 * hwc, gm_models.data(),
-                                       gm_stats.data(), gm_mask.data(), gm_res.data(), gm_reg.data(), w, h,
-                                       OFDIS_MEM_HOST);
-    }
-    size_t dcount[6] = {0, 0, 0, 0, 0, 0};  // statuses 0..4, filled
-    if (rc == OFDIS_OK && disp_on) {
-      const size_t np = (size_t)n * w * h;
-      ddisp.resize(np);
-      dstatus.resize(np);
-      ddepth.resize(camera_arg ? np : 0);
-      dxyz.resize(camera_arg ? 3 * np : 0);
-      rc = ofdis_disparity_fullres(ctx, 0, n, n, &dfilt, camera_arg ? &dcam : nullptr, ddisp.data(), dstatus.data(),
-                                   camera_arg ? ddepth.data() : nullptr, camera_arg ? dxyz.data() : nullptr, w, h,
-                                   OFDIS_MEM_HOST);
-      for (size_t i = 0; i < np && rc == OFDIS_OK; ++i) {
-        dcount[dstatus[i] < 5 ? dstatus[i] : 0] += 1;
-        dcount[5] += dstatus[i] != 0 && !std::isnan(ddisp[i]);
-      }
-    }
-    // --tracks: runs of pairs that continue each other; a run that does not continue the previous pair begins a clip
-    for (int k0 = 0, k1; k0 < n && tracks_file && rc == OFDIS_OK; k0 = k1) {
-      for (k1 = k0 + 1; k1 < n && jobs[j0 + k1].a == jobs[j0 + k1 - 1].b;) ++k1;
-      const size_t fs = seq ? hwc : 2 * hwc;  // image1 of pair k at k * fs, its image2 one frame later
-      const uint8_t* im1 = frames.data() + (size_t)k0 * fs;
-      const uint8_t* im2 = im1 + hwc;
-      ofdis_track_params tp;
-      tp.spacing = 8;
-      tp.capacity = 4 * ((w + 7) / 8) * ((h + 7) / 8);
-      tp.alpha = nop == 2 ? 0.01f : 0.0f;
-      tp.beta = nop == 2 ? 0.5f : 1.0f;
-      tp.mb_alpha = 0.01f;
-      tp.mb_beta = 0.002f;
-      tp.min_eig = 25.0f;
-      tpoints.resize((size_t)n * tp.capacity);
-      tcounts.resize(n);
-      if (j0 + k0 == 0 || jobs[j0 + k0].a != jobs[j0 + k0 - 1].b) {
-        end_clip();
-        rc = fisher_rc;
-        ++tclip;
-        tframe = 0;
-        if (rc == OFDIS_OK)
-          rc = traj_stage ? ofdis_traj_begin(ctx, &tp, &trp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST)
-                          : ofdis_track_begin(ctx, &tp, im1, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
-        if (rc == OFDIS_OK && fisher_file) {
-          rc = ofdis_fisher_begin(ctx, &fbook.cb);
-          fisher_live = rc == OFDIS_OK;
-        }
-        if (rc == OFDIS_OK) write_tracks(tpoints.data(), tcounts[0]);
-      }
-      if (rc == OFDIS_OK && traj_stage && !desc_file) {  // --fisher alone: the descriptors stay on the device
-        tndesc.resize(k1 - k0);
-        rc = ofdis_traj_advance_fisher(ctx, k0, k1, n + k0, im2, fs,
-                                       gm_model ? gm_models.data() + (size_t)9 * k0 : nullptr, tpoints.data(),
-                                       tcounts.data(), tndesc.data(), w, h, OFDIS_MEM_HOST);
-      } else if (rc == OFDIS_OK && desc_file) {
-        const size_t bound = (size_t)tp.capacity * ((k1 - k0 + 2 * trp.L - 2) / trp.L);
-        trec.resize(bound);
-        tdesc.resize(bound * tdim);
-        tndesc.resize(k1 - k0);
-        rc = ofdis_traj_advance(ctx, k0, k1, n + k0, im2, fs, gm_model ? gm_models.data() + (size_t)9 * k0 : nullptr,
-                                tpoints.data(), tcounts.data(), trec.data(), tdesc.data(), tndesc.data(), w, h,
-                                OFDIS_MEM_HOST);
-        int total = 0;
-        for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k) total += tndesc[k];
-        if (rc == OFDIS_OK) write_desc(total);
-        if (rc == OFDIS_OK && fisher_file) rc = ofdis_fisher_push(ctx, tdesc.data(), total, OFDIS_MEM_HOST);
-      } else if (rc == OFDIS_OK) {
-        rc = ofdis_track_advance(ctx, k0, k1, n + k0, im2, fs, tpoints.data(), tcounts.data(), w, h, OFDIS_MEM_HOST);
-      }
-      for (int k = 0; k < k1 - k0 && rc == OFDIS_OK; ++k) write_tracks(tpoints.data() + (size_t)k * tp.capacity, tcounts[k]);
-    }
-    // --stabilize: the runs of --tracks; a clip begins on its first image1, every run pushes its image2 frames with
-    // their --global-motion models
-    for (int k0 = 0, k1; k0 < n && stab_file && rc == OFDIS_OK; k0 = k1) {
-      for (k1 = k0 + 1; k1 < n && jobs[j0 + k1].a == jobs[j0 + k1 - 1].b;) ++k1;
-      const size_t fs = seq ? hwc : 2 * hwc;  // image1 of pair k at k * fs, its image2 one frame later
-      const uint8_t* im1 = frames.data() + (size_t)k0 * fs;
-      if (j0 + k0 == 0 || jobs[j0 + k0].a != jobs[j0 + k0 - 1].b) {
-        rc = stab_end();
-        if (rc == OFDIS_OK) rc = ofdis_stab_begin(ctx, &stp, stab_wts.data(), im1, w, h, OFDIS_MEM_HOST);
-        if (rc == OFDIS_OK) {
-          stab_live = true;
-          ++sclip;
-          sw = w;
-          sh = h;
-        }
-      }
-      if (rc != OFDIS_OK) break;
-      sbuf.resize((size_t)(k1 - k0) * hwc);
-      sinfo.resize(k1 - k0);
-      int count = 0;
-      rc = ofdis_stab_push(ctx, k1 - k0, gm_models.data() + (size_t)9 * k0, im1 + hwc, fs, sbuf.data(), sinfo.data(),
-                           &count, OFDIS_MEM_HOST);
-      if (rc == OFDIS_OK) write_stab(count);
-    }
-    if (rc == OFDIS_OK) rc = ofdis_sync(ctx);
-    if (rc == OFDIS_OK && gtlist) {
-      gt_batch.resize((size_t)n * w * h * nop);
-      for (int k = 0; k < n; ++k) {
-        string err;
-        if (!read_gt_file(gts[j0 + k].c_str(), w, h, nop, gt_one, err)) {
-          fprintf(stderr, "error: %s: %s\n", gts[j0 + k].c_str(), err.c_str());
-          ofdis_destroy(ctx);
-          return 1;
-        }
-        memcpy(gt_batch.data() + (size_t)k * w * h * nop, gt_one.data(), sizeof(float) * gt_one.size());
-      }
-      eval_pairs.resize((size_t)n * nclasses);
-      rc = ofdis_flow_error_fullres(ctx, 0, n, gt_batch.data(), bidir ? masks.data() : nullptr, nclasses,
-                                    eval_pairs.data(), nullptr, w, h, OFDIS_MEM_HOST);
-      for (int k = 0; k < n && rc == OFDIS_OK; ++k)
-        for (int c = 0; c < nclasses; ++c) {
-          add_stats(eval_total[0], eval_pairs[(size_t)k * nclasses + c]);
-          if (bidir) add_stats(eval_total[1 + c], eval_pairs[(size_t)k * nclasses + c]);
-        }
-    }
-    if (rc == OFDIS_OK && sf_list) {
-      const size_t pix = (size_t)w * h;
-      // positive disparities: the readers return this library's stereo convention, -d
-      auto load = [&](const string& path, int fnop, float sign, float* dst) {
-        string err;
-        if (!read_gt_file(path.c_str(), w, h, fnop, gt_one, err)) {
-          fprintf(stderr, "error: %s: %s\n", path.c_str(), err.c_str());
-          return false;
-        }
-        for (size_t i = 0; i < gt_one.size(); ++i) dst[i] = sign * gt_one[i];
-        return true;
-      };
-      sf_d0.resize(n * pix);
-      sf_d1.resize(n * pix);
-      sf_w.resize(n * pix);
-      sf_m.resize(camera_arg ? 3 * n * pix : 0);
-      bool ok = true;
-      for (int k = 0; k < n && ok; ++k)
-        ok = load(sf_files[2 * (j0 + k)], 1, -1.0f, &sf_d0[k * pix]) && load(sf_files[2 * (j0 + k) + 1], 1, -1.0f, &sf_d1[k * pix]);
-      if (sf_gtlist) {
-        sf_g0.resize(n * pix);
-        sf_g1.resize(n * pix);
-        sf_gf.resize(2 * n * pix);
-        for (int k = 0; k < n && ok; ++k)
-          ok = load(sf_gts[3 * (j0 + k)], 1, -1.0f, &sf_g0[k * pix]) && load(sf_gts[3 * (j0 + k) + 1], 1, -1.0f, &sf_g1[k * pix]) &&
-               load(sf_gts[3 * (j0 + k) + 2], 2, 1.0f, &sf_gf[2 * k * pix]);
-        sf_pairs.resize((size_t)n * nclasses);
-      }
-      if (!ok) {
-        ofdis_destroy(ctx);
-        return 1;
-      }
-      const ofdis_sf_gt sgt{sf_g0.data(), sf_g1.data(), sf_gf.data()};
-      rc = ofdis_scene_flow_fullres(ctx, 0, n, sf_d0.data(), sf_d1.data(), pix, 1.0f, camera_arg ? &dcam : nullptr,
-                                    sf_w.data(), nullptr, camera_arg ? sf_m.data() : nullptr, sf_gtlist ? &sgt : nullptr,
-                                    bidir ? masks.data() : nullptr, nclasses, sf_gtlist ? sf_pairs.data() : nullptr, w, h,
-                                    OFDIS_MEM_HOST);
-      for (int k = 0; k < n && rc == OFDIS_OK && sf_gtlist; ++k) {
-        ofdis_sf_stats all;
-        memset(&all, 0, sizeof(all));
-        for (int c = 0; c < nclasses; ++c) {
-          add_sf_stats(all, sf_pairs[(size_t)k * nclasses + c]);
-          add_sf_stats(sf_total[1 + c], sf_pairs[(size_t)k * nclasses + c]);
-        }
-        add_sf_stats(sf_total[0], all);
-        if (verbosity > 0) print_sfeval(jobs[j0 + k].out.c_str(), 0, all);
-      }
-      for (int k = 0; k < n && rc == OFDIS_OK; ++k) {
-        const float* d = &sf_w[k * pix];
-        if (kitti) {
-          vector<uint16_t> enc(pix);
-          for (size_t i = 0; i < pix; ++i)  // NaN fails d >= 0 and is written as 0
-            enc[i] = d[i] >= 0.0f ? (uint16_t)fminf(fmaxf(d[i] * 256.0f, 1.0f), 65535.0f) : (uint16_t)0;
-          save_png(enc.data(), w, h, 1, 16, with_suffix(jobs[j0 + k].out, "_disp1").c_str());
-        } else {
-          ImageF f;  // SavePFMFile writes -value: the positive disparity goes in as -d
-          f.w = w; f.h = h; f.c = 1;
-          f.px.resize(pix);
-          for (size_t i = 0; i < pix; ++i) f.px[i] = -d[i];
-          SavePFMFile(f, with_suffix(jobs[j0 + k].out, "_disp1", ".pfm").c_str());
-        }
-        if (camera_arg) save_pfm3(&sf_m[3 * k * pix], w, h, with_suffix(jobs[j0 + k].out, "_sceneflow", ".pfm").c_str());
-      }
-      if (rc == OFDIS_OK && odo_dir) {
-        ofdis_egomotion_params ep;
-        memset(&ep, 0, sizeof(ep));
-        ep.step = 8;
-        ep.fb_check = bidir ? 1 : 0;
-        ep.alpha = 0.01f;
-        ep.beta = 0.5f;
-        ep.edge_diff = 1.0f;
-        ep.hypotheses = 1024;
-        ep.threshold = 1.0f;
-        ep.refine = 5;
-        ep.seed = 0;
-        odo_pose.resize((size_t)12 * n);
-        odo_stats.resize(n);
-        odo_mask.resize(n * pix);
-        odo_om.resize(3 * n * pix);
-        rc = ofdis_egomotion_fullres(ctx, 0, n, n, &ep, sf_d0.data(), sf_d1.data(), pix, &dcam, odo_pose.data(),
-                                     odo_stats.data(), odo_mask.data(), nullptr, odo_om.data(), w, h, OFDIS_MEM_HOST);
-        for (int k = 0; k < n && rc == OFDIS_OK; ++k) {
-          const int c = odo_clip[j0 + k], fr = odo_frame[j0 + k];
-          const ofdis_motion_stats& st = odo_stats[k];
-          const double* P = odo_pose.data() + (size_t)12 * k;
-          fprintf(odo_file, "%d %d %d %d %d %d", c, fr, st.status, st.n_corr, st.ransac_inliers, st.n_inliers);
-          for (int i = 0; i < 12; ++i) fprintf(odo_file, " %.17g", P[i]);
-          fprintf(odo_file, "\n");
-          odo_rel[c].insert(odo_rel[c].end(), P, P + 12);
-          save_mask_pgm(odo_mask.data() + k * pix, w, h, with_suffix(jobs[j0 + k].out, "_objects", ".pgm").c_str());
-          save_pfm3(&odo_om[3 * k * pix], w, h, with_suffix(jobs[j0 + k].out, "_objmotion", ".pfm").c_str());
-          if (!odo_gtlist) continue;
-          double te, re;
-          pose_error(&odo_gt[c][(size_t)12 * fr], &odo_gt[c][(size_t)12 * (fr + 1)], P, &te, &re);
-          odo_terr += te;
-          odo_rerr += re;
-          ++odo_eval;
-          if (verbosity > 0) printf("ODOEVAL %d %d %.9g %.9g\n", c, fr, te, re);
-        }
-      }
-      // --fuse: the runs of one clip within the batch; image1 of pair k at k * fs, its image2 one frame later
-      const size_t fs = seq ? hwc : 2 * hwc;
-      for (int k0 = 0, k1; k0 < n && rc == OFDIS_OK && fuse_arg; k0 = k1) {
-        const int c = odo_clip[j0 + k0];
-        for (k1 = k0 + 1; k1 < n && odo_clip[j0 + k1] == c;) ++k1;
-        if (odo_frame[j0 + k0] == 0) {
-          static const double kIdentity[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
-          memcpy(fuse_T, kIdentity, sizeof(fuse_T));
-          fuse_frames = 0;
-          rc = ofdis_fuse_begin(ctx, &fuse_p);
-          if (rc != OFDIS_OK) break;
-        }
-        fuse_poses.resize((size_t)12 * (k1 - k0 + 1));
-        for (int k = k0; k < k1; ++k) {
-          memcpy(&fuse_poses[(size_t)12 * (k - k0)], fuse_T, sizeof(fuse_T));
-          chain_pose(fuse_T, odo_pose.data() + (size_t)12 * k);
-        }
-        memcpy(&fuse_poses[(size_t)12 * (k1 - k0)], fuse_T, sizeof(fuse_T));
-        rc = ofdis_fuse_push(ctx, k1 - k0, &sf_d0[k0 * pix], pix, fuse_poses.data(), &dcam, INFINITY,
-                             frames.data() + (size_t)k0 * fs, fs, w, h, OFDIS_MEM_HOST);
-        fuse_frames += k1 - k0;
-        if (rc != OFDIS_OK || (j0 + k1 < (int)jobs.size() && odo_clip[j0 + k1] == c)) continue;
-        // the clip ends with this run: its last image2, then the surface
-        rc = ofdis_fuse_push(ctx, 1, &sf_d1[(k1 - 1) * pix], pix, &fuse_poses[(size_t)12 * (k1 - k0)], &dcam, INFINITY,
-                             frames.data() + (size_t)(k1 - 1) * fs + hwc, fs, w, h, OFDIS_MEM_HOST);
-        ++fuse_frames;
-        long count = 0;
-        if (rc == OFDIS_OK) rc = ofdis_fuse_extract(ctx, 1.0f, nullptr, 0, &count, OFDIS_MEM_HOST);
-        if (rc != OFDIS_OK) break;
-        fuse_pts.resize(count);
-        rc = ofdis_fuse_extract(ctx, 1.0f, fuse_pts.data(), count, &count, OFDIS_MEM_HOST);
-        if (rc != OFDIS_OK) break;
-        char name[32];
-        snprintf(name, sizeof(name), "/fused_%04d.ply", c);
-        string path = string(odo_dir) + name;
-        if (!write_fused_ply(path, fuse_pts.data(), count, nochannels, false, nullptr, 0)) {
-          fprintf(stderr, "error: cannot write %s\n", path.c_str());
-          ofdis_destroy(ctx);
-          return 1;
-        }
-        if (verbosity > 0) printf("FUSE clip %d frames %d points %ld\n", c, fuse_frames, count);
-        if (!fuse_mesh) continue;
-        // the mesh's vertices are the points just extracted: only the faces come back
-        long nv = 0, nf = 0;
-        rc = ofdis_fuse_mesh(ctx, 1.0f, nullptr, 0, &nv, nullptr, 0, &nf, OFDIS_MEM_HOST);
-        if (rc != OFDIS_OK) break;
-        fuse_faces.resize((size_t)3 * nf);
-        rc = ofdis_fuse_mesh(ctx, 1.0f, nullptr, 0, &nv, fuse_faces.data(), nf, &nf, OFDIS_MEM_HOST);
-        if (rc != OFDIS_OK) break;
-        snprintf(name, sizeof(name), "/fused_%04d_mesh.ply", c);
-        path = string(odo_dir) + name;
-        if (!write_fused_ply(path, fuse_pts.data(), count, nochannels, true, fuse_faces.data(), nf)) {
-          fprintf(stderr, "error: cannot write %s\n", path.c_str());
-          ofdis_destroy(ctx);
-          return 1;
-        }
-        if (verbosity > 0) printf("MESH clip %d vertices %ld faces %ld\n", c, nv, nf);
-      }
-    }
-    if (rc != OFDIS_OK) {
-      fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
-      ofdis_destroy(ctx);
-      return 1;
-    }
-    for (int k = 0; k < n && kitti; ++k) {
-      save_png(kflows.data() + (size_t)k * w * h * kch, w, h, kch, 16, jobs[j0 + k].out.c_str());
-      if (bidir) {
-        save_png(kflows.data() + (size_t)(n + k) * w * h * kch, w, h, kch, 16,
-                 with_suffix(jobs[j0 + k].out, "_bw").c_str());
-        save_mask_pgm(masks.data() + (size_t)k * w * h, w, h, with_suffix(jobs[j0 + k].out, "_occ", ".pgm").c_str());
-      }
-    }
-    for (int k = 0; k < n && color; ++k) {
-      save_png(colors.data() + (size_t)k * w * h * 3, w, h, 3, 8, with_suffix(jobs[j0 + k].out, "_color", ".png").c_str());
-      if (bidir)
-        save_png(colors.data() + (size_t)(n + k) * w * h * 3, w, h, 3, 8,
-                 with_suffix(jobs[j0 + k].out, "_bw_color", ".png").c_str());
-    }
-    for (int k = 0; k < n && interp_arg; ++k) {
-      const uint8_t* im = interp.data() + (size_t)k * hwc;
-      if (nochannels == 3) {  // the decoder's BGR -> RGB
-        interp_png.resize(hwc);
-        for (size_t p = 0; p < hwc; p += 3) {
-          interp_png[p] = im[p + 2];
-          interp_png[p + 1] = im[p + 1];
-          interp_png[p + 2] = im[p];
-        }
-        im = interp_png.data();
-      }
-      save_png(im, w, h, nochannels, 8, with_suffix(jobs[j0 + k].out, "_interp", ".png").c_str());
-    }
-    for (int k = 0; k < n && gm_model; ++k) {
-      const string& o = jobs[j0 + k].out;
-      fprintf(gm_file, "%s", with_suffix(o, "", "").c_str());
-      for (int i = 0; i < 9; ++i) fprintf(gm_file, " %.17g", gm_models[(size_t)9 * k + i]);
-      fprintf(gm_file, " %d %d %d\n", gm_stats[k].status, gm_stats[k].n_corr, gm_stats[k].n_inliers);
-      const float* r = gm_res.data() + (size_t)2 * k * w * h;
-      if (kitti) {  // the encoding of OFDIS_ENC_KITTI (flow)
-        vector<uint16_t> enc((size_t)3 * w * h);
-        for (size_t i = 0; i < (size_t)w * h; ++i) {
-          const float u = r[2 * i], v = r[2 * i + 1];
-          const bool valid = !std::isnan(u) && !std::isnan(v);
-          enc[3 * i] = valid ? (uint16_t)fminf(fmaxf(u * 64.0f + 32768.0f, 0.0f), 65535.0f) : (uint16_t)0;
-          enc[3 * i + 1] = valid ? (uint16_t)fminf(fmaxf(v * 64.0f + 32768.0f, 0.0f), 65535.0f) : (uint16_t)0;
-          enc[3 * i + 2] = valid ? 1 : 0;
-        }
-        save_png(enc.data(), w, h, 3, 16, with_suffix(o, "_residual").c_str());
-      } else {
-        ImageF f;
-        f.w = w; f.h = h; f.c = 2;
-        f.px.assign(r, r + (size_t)2 * w * h);
-        SaveFlowFile(f, with_suffix(o, "_residual").c_str());
-      }
-      save_mask_pgm(gm_mask.data() + (size_t)k * w * h, w, h, with_suffix(o, "_moving", ".pgm").c_str());
-      const uint8_t* im = gm_reg.data() + (size_t)k * hwc;
-      if (nochannels == 3) {  // the decoder's BGR -> RGB
-        gm_png.resize(hwc);
-        for (size_t q = 0; q < hwc; q += 3) {
-          gm_png[q] = im[q + 2];
-          gm_png[q + 1] = im[q + 1];
-          gm_png[q + 2] = im[q];
-        }
-        im = gm_png.data();
-      }
-      save_png(im, w, h, nochannels, 8, with_suffix(o, "_registered", ".png").c_str());
-    }
-    for (int k = 0; k < n && disp_on; ++k) {
-      const size_t o = (size_t)k * w * h;
-      if (kitti) {
-        vector<uint16_t> enc((size_t)w * h);
-        for (size_t i = 0; i < enc.size(); ++i) {
-          const float d = ddisp[o + i];  // NaN fails d >= 0 and is written as 0
-          enc[i] = d >= 0.0f ? (uint16_t)fminf(fmaxf(d * 256.0f, 1.0f), 65535.0f) : (uint16_t)0;
-        }
-        save_png(enc.data(), w, h, 1, 16, with_suffix(jobs[j0 + k].out, "_filtered").c_str());
-      } else {
-        ImageF f;  // SavePFMFile writes -value: the positive disparity goes in as -d, the sign of <stem><ext>
-        f.w = w; f.h = h; f.c = 1;
-        f.px.resize((size_t)w * h);
-        for (size_t i = 0; i < f.px.size(); ++i) f.px[i] = -ddisp[o + i];
-        SavePFMFile(f, with_suffix(jobs[j0 + k].out, "_filtered").c_str());
-      }
-      if (!camera_arg) continue;
-      ImageF z;
-      z.w = w; z.h = h; z.c = 1;
-      z.px.resize((size_t)w * h);
-      for (size_t i = 0; i < z.px.size(); ++i) z.px[i] = -ddepth[o + i];
-      SavePFMFile(z, with_suffix(jobs[j0 + k].out, "_depth", ".pfm").c_str());
-      // image1 of pair k: frame k of a clip, or the first image of the k-th pair
-      const uint8_t* im1 = frames.data() + (size_t)k * (seq ? hwc : 2 * hwc);
-      size_t npts = 0;
-      dply.clear();
-      for (size_t i = 0; i < (size_t)w * h; ++i) {
-        if (!std::isfinite(ddepth[o + i])) continue;
-        const float* q = dxyz.data() + (o + i) * 3;
-        const uint8_t* c = im1 + i * nochannels;
-        const uint8_t rgb[3] = {nochannels == 3 ? c[2] : c[0], c[nochannels == 3 ? 1 : 0], c[0]};  // the decoder's BGR
-        const uint8_t* qb = reinterpret_cast<const uint8_t*>(q);
-        dply.insert(dply.end(), qb, qb + 12);
-        dply.insert(dply.end(), rgb, rgb + 3);
-        ++npts;
-      }
-      const string ply = with_suffix(jobs[j0 + k].out, "", ".ply");
-      FILE* pf = fopen(ply.c_str(), "wb");
-      if (!pf) {
-        cout << "WriteFile: could not open file" << endl;
-        continue;
-      }
-      fprintf(pf, "ply\nformat binary_little_endian 1.0\nelement vertex %zu\nproperty float x\nproperty float y\n"
-                  "property float z\nproperty uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n", npts);
-      if (fwrite(dply.data(), 1, dply.size(), pf) != dply.size()) cout << "WriteFile: problem writing data" << endl;
-      fclose(pf);
-    }
-    if (verbosity > 0 && disp_on)
-      printf("DISP pairs %d valid %zu inconsistent %zu leaves %zu range %zu speckle %zu filled %zu\n", n, dcount[0],
-             dcount[1], dcount[2], dcount[3], dcount[4], dcount[5]);
-    ImageF out;
-    out.w = w; out.h = h; out.c = nop;
-    for (int k = 0; k < n && !kitti; ++k) {
-      out.px.assign(flows.begin() + (size_t)k * w * h * nop, flows.begin() + (size_t)(k + 1) * w * h * nop);
-      if (SELECTMODE == 1) SaveFlowFile(out, jobs[j0 + k].out.c_str());
-      else SavePFMFile(out, jobs[j0 + k].out.c_str());
-      if (!bidir) continue;
-      out.px.assign(flows.begin() + (size_t)(n + k) * w * h * nop, flows.begin() + (size_t)(n + k + 1) * w * h * nop);
-      const string bw = with_suffix(jobs[j0 + k].out, "_bw");
-      if (SELECTMODE == 1) SaveFlowFile(out, bw.c_str());
-      else SavePFMFile(out, bw.c_str());
-      save_mask_pgm(masks.data() + (size_t)k * w * h, w, h, with_suffix(jobs[j0 + k].out, "_occ", ".pgm").c_str());
-    }
-    j0 += n;
-    done += n;
+    parse_cli_params(o.nnum, o.nums, b.w, P);
+    s.verbosity = P.verbosity;
+    if (int rc = ensure_context(s, b, P)) return rc;
+    const int rc = run_stages(s, b);
+    if (rc == kRefused) return 1;
+    if (rc != OFDIS_OK) return refuse(1, "%s", ofdis_last_error(s.ctx.get()));
+    write_outputs(s, b);
+    s.done += b.n;
   }
-  end_clip();
-  if (fisher_rc != OFDIS_OK || stab_end() != OFDIS_OK) {
-    fprintf(stderr, "error: %s\n", ofdis_last_error(ctx));
-    ofdis_destroy(ctx);
-    return 1;
-  }
-  if (ctx) ofdis_destroy(ctx);
-  if (stab_file && fclose(stab_file) != 0) {
-    fprintf(stderr, "error: cannot write %s\n", stab_txt.c_str());
-    return 1;
-  }
-  if (tracks_file && fclose(tracks_file) != 0) {
-    fprintf(stderr, "error: cannot write %s\n", tracks_path);
-    return 1;
-  }
-  if (desc_file && fclose(desc_file) != 0) {
-    fprintf(stderr, "error: cannot write %s\n", desc_path);
-    return 1;
-  }
-  if (fisher_file && fclose(fisher_file) != 0) {
-    fprintf(stderr, "error: cannot write %s\n", fisher_arg[1]);
-    return 1;
-  }
-  if (gm_file && fclose(gm_file) != 0) {
-    fprintf(stderr, "error: cannot write %s\n", gm_arg[1]);
-    return 1;
-  }
-  if (odo_file && fclose(odo_file) != 0) {
-    fprintf(stderr, "error: cannot write %s/odometry.txt\n", odo_dir);
-    return 1;
-  }
-  for (size_t c = 0; c < odo_rel.size(); ++c) {
-    char name[32];
-    snprintf(name, sizeof(name), "/poses_%04zu.txt", c);
-    const string path = string(odo_dir) + name;
-    FILE* f = fopen(path.c_str(), "w");
-    double T[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
-    for (size_t k = 0; f && k <= odo_rel[c].size() / 12; ++k) {
-      if (k > 0) chain_pose(T, &odo_rel[c][12 * (k - 1)]);
-      for (int i = 0; i < 12; ++i) fprintf(f, i ? " %.17g" : "%.17g", T[i]);
-      fprintf(f, "\n");
-    }
-    if (!f || fclose(f) != 0) {
-      fprintf(stderr, "error: cannot write %s\n", path.c_str());
-      return 1;
-    }
-  }
-  if (verbosity > 0) printf("TIME (%zu pairs, load + flow + save) (ms): %3g\n", done, elapsed_ms(tv));
-  if (verbosity > 0 && seq_pairs) printf("SEQUENCE (%zu of %zu pairs from %zu decoded frames)\n", seq_pairs, done, seq_decoded);
-  if (verbosity > 0 && warm) printf("WARM START (%zu of %zu pairs from the previous pair's flow)\n", warm_pairs, done);
-  if (verbosity > 0 && tracks_path)
-    printf("TRACKS clips %d frames %zu seeded %lld leaves %lld inconsistent %lld boundary %lld dropped %lld\n", tclip + 1,
-           tframes, ttotal.seeded, ttotal.ended_leaves, ttotal.ended_inconsistent, ttotal.ended_boundary, ttotal.dropped);
-  if (verbosity > 0 && desc_path)
-    printf("DESCRIPTORS clips %d emitted %lld static %lld erratic %lld jump %lld camera %lld\n", tclip + 1,
-           dtotal.emitted, dtotal.rejected_static, dtotal.rejected_erratic, dtotal.rejected_jump, dtotal.rejected_camera);
-  if (verbosity > 0 && fisher_arg[0]) {
-    printf("FISHER clips %d descriptors %lld skipped", fclips, fpushed);
-    for (int b = 0; b < fbook.cb.nblocks; ++b) printf(" %lld", fskipped[b]);
-    printf("\n");
-  }
-  if (verbosity > 0 && gtlist) {
-    static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
-    print_eval("", done, eval_total[0]);
-    for (int c = 0; c < nclasses && bidir; ++c) print_eval(kClassNames[c], done, eval_total[1 + c]);
-  }
-  if (verbosity > 0 && odo_gtlist)
-    printf("ODOEVAL (%zu pairs) t_err %.9g r_err %.9g\n", odo_eval, odo_eval ? odo_terr / odo_eval : 0.0,
-           odo_eval ? odo_rerr / odo_eval : 0.0);
-  if (verbosity > 0 && sf_gtlist) {
-    static const char* const kClassNames[3] = {"consistent", "inconsistent", "leaves"};
-    print_sfeval("", done, sf_total[0]);
-    for (int c = 0; c < nclasses && bidir; ++c) print_sfeval(kClassNames[c], done, sf_total[1 + c]);
-  }
+  s.ctx.reset();
+  if (int rc = out.close()) return rc;
+  if (int rc = write_poses(s)) return rc;
+  print_summary(s, tv);
   return 0;
 }
 #else
