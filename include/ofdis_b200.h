@@ -752,6 +752,84 @@ int ofdis_fuse_set_volume(ofdis_ctx* ctx, const float* T, const float* W, const 
  * device pts or faces that is not 4-byte aligned. */
 int ofdis_fuse_mesh(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, long pt_capacity, long* pt_count,
                     unsigned int* faces, long face_capacity, long* face_count, int memkind);
+/* Camera tracking against the volume (extension): each frame aligned to the TSDF before it is pushed, the SDF
+ * formulation of Bylow et al. (RSS 2013): the frame's points, moved into the volume by the camera-to-world pose, should
+ * land on T = 0.  preprocess.fuse_track restates it bit for bit.  float32 where marked, float64 in the sums and the
+ * pose algebra, everything without contraction and with IEEE division and square root; the terms of the fusion header
+ * above (known(d), fb, the volume's layout).  W = width_org, H = height_org.  For k = 0 .. n-1:
+ *   1. Prediction (float64).  T(-1) = prev ([12], camera-to-world); P = T(k-1) and M = motions[k] (camera k-1 to
+ *      camera k, as ofdis_egomotion_fullres returns it): inv(M) = [Ri | ti] with Ri_rc = M_cr and ti_r =
+ *      -(((M_0r*M_03) + (M_1r*M_13)) + (M_2r*M_23)), and T_pred_rc = ((P_r0*Ri_0c) + (P_r1*Ri_1c)) + (P_r2*Ri_2c) for
+ *      c < 3, T_pred_r3 = (((P_r0*ti_0) + (P_r1*ti_1)) + (P_r2*ti_2)) + P_r3.  motions NULL: T_pred = T(k-1) as it is.
+ *      This can differ in the last bits from preprocess.chain_poses, which inverts with np.linalg.inv.  T(k-1) is frame
+ *      k-1's final pose from step 4, so the chain runs through the tracked poses.
+ *   2. Evaluation of a pose M (float64 [12]) of frame k: g = M rounded to float32.  The cells of
+ *      ofdis_global_motion_fullres at step s, in cell order, cell (i, j) at its pixel (px, py): d = D_k(px, py),
+ *      sd = d + doffs, Z = fb / sd, X = (((float)px - cx) * Z) / fx, Y = (((float)py - cy) * Z) / fy (ofdis_scene_flow's
+ *      xyz), Pw_r = ((g_r0*X + g_r1*Y) + g_r2*Z) + g_r3 (the push's order), q_e = (Pw_e - origin_e) / voxel (the
+ *      render's).  The cell is valid when known(d), sd > 0, Z <= max_depth, fl = floorf(q) satisfies 0 <= fl <= (float)
+ *      (n - 2) on each axis (NaN fails), and all 8 corners of the cube at i0 = (int)fl have W >= min_weight and
+ *      fabsf(T) < 1.  With fr = q - fl, gx = 1.0f - fr_0 (gy, gz likewise) and the corners c0..c7 in the render's
+ *      order: x00 = c0*gx + c1*fr_0, x10 = c2*gx + c3*fr_0, x01 = c4*gx + c5*fr_0, x11 = c6*gx + c7*fr_0,
+ *      y0 = x00*gy + x10*fr_1, y1 = x01*gy + x11*fr_1, the residual r = y0*gz + y1*fr_2 (the render's T); the gradient
+ *      G_0 = (((c1 - c0)*gy + (c3 - c2)*fr_1)*gz + ((c5 - c4)*gy + (c7 - c6)*fr_1)*fr_2) / voxel,
+ *      G_1 = ((x10 - x00)*gz + (x11 - x01)*fr_2) / voxel, G_2 = (y1 - y0) / voxel (float32, the exact partial
+ *      derivatives of the trilinear T in metres).  Huber weight wt = 1.0f when fabsf(r) <= huber, else
+ *      huber / fabsf(r).  In float64 of those values, a = G and w = 2 Pw per component: the Jacobian row of the left
+ *      update J = ((a1*-w2) + (a2*w1), (a0*w2) + (a2*-w0), (a0*-w1) + (a1*w0), a0, a1, a2) (ofdis_egomotion_fullres's
+ *      row), v = wt * J per component, N_ij = v_i * J_j for i <= j (21, row-major), b_i = -(v_i * r) (6) and
+ *      e = (wt * r) * r (1).  These 28 sums and the count of valid cells run over the cells as the refits of
+ *      ofdis_global_motion_fullres sum: chunks of 32 consecutive cells from +0.0 in cell order (an invalid cell or one
+ *      past the last adds nothing), then the pairwise tree over the chunk sums padded with +0.0 to a power of two.
+ *   3. Rounds r = 0, 1, ...: M = T_pred at r = 0.  Evaluate M (step 2): n_corr = the count, cost = e, and at r = 0
+ *      cost0 = e.  Stop when n_corr < min_corr (status 1 when r = 0), when r = rounds, or when N with damping added to
+ *      each diagonal entry (N_ii + damping) fails the elimination of ofdis_global_motion_fullres.  Otherwise x = its
+ *      solution (omega, tau); stop when max_i fabs(x_i) <= eps (the update is not applied), else M = the Cayley update
+ *      of ofdis_egomotion_fullres's step 4 applied to M (R <- C R, t <- C t + tau), rounds = r + 1, next r.  So a frame
+ *      takes at most rounds + 1 evaluations and the stats describe the last evaluated pose.
+ *   4. Guard.  Unless status 1, with M_f the last evaluated pose and M_p = T_pred: dt = t_f - t_p, the shift
+ *      sqrt((dt0*dt0 + dt1*dt1) + dt2*dt2) <= max_shift and, with s_i = ((Rf_i0*Rp_i0) + (Rf_i1*Rp_i1)) +
+ *      (Rf_i2*Rp_i2), (((s0 + s1) + s2) - 1.0) / 2.0 >= min_cos (the cosine of the rotation between them): status 0
+ *      and T(k) = M_f; else status 2 (NaN fails).  Status 1 or 2: T(k) = T_pred.  poses[k] = T(k).
+ *   5. Integration (integrate 1): frame k is pushed at T(k) before frame k+1 is predicted, by exactly ofdis_fuse_push's
+ *      rule (its world-to-camera g formed in float64 and rounded once, max_depth, colour from frames + k*frame_stride
+ *      when the volume keeps it).  So one call of n frames equals n calls of one frame with prev = the last pose
+ *      returned, and equals, frame by frame, a call with integrate 0 followed by ofdis_fuse_push at the returned pose.
+ * disp + k*disp_stride ([H][W], the maps of ofdis_fuse_push) and frames are in memkind; host inputs go through the
+ * staging buffer.  prev ([12]), motions ([n][12] or NULL), poses ([n][12] float64) and stats ([n]) are host memory.
+ * OFDIS_ERR_ARG, with the volume and the outputs untouched: no live volume, n outside 1 .. max_frames + 1, NULL disp,
+ * prev, p, poses or stats, a NULL or bad cam (as ofdis_fuse_push checks it), p out of range (see the fields), a NULL
+ * frames when integrating into a volume with colour, a non-finite entry of prev or motions, disp_stride < W*H,
+ * frame_stride below one frame (when frames are read), or a device disp or frames that is not aligned to its element;
+ * frame sizes as ofdis_get_flow_fullres checks them.  The workspace -- 28 doubles of chunk sums per 32 cells, the pose
+ * chain (the motions, poses and stats of max_frames + 1 frames and the current frame's poses) and one arrival
+ * counter -- is allocated at the first call, grows, never shrinks and is freed by ofdis_destroy; OFDIS_ERR_NOMEM when
+ * that fails, with the volume intact.  Enqueued on the context's stream as rounds + 1 evaluation kernels per frame
+ * (a frame that stops early makes its later ones return at once) plus, with integrate, one integration kernel per
+ * frame: n * (rounds + 1 + integrate) kernels whatever the data.  The call synchronises the stream once, at the end. */
+typedef struct ofdis_fuse_track_params {
+  int step;             /* >= 1: the correspondence cells of ofdis_global_motion_fullres at this step */
+  int rounds;           /* 0 .. 32 Gauss-Newton rounds per frame */
+  float min_weight;     /* every one of the 8 corners needs W >= min_weight; not NaN */
+  float max_depth;      /* > 0, +inf allowed: used by the alignment and, when integrating, by the push */
+  float huber;          /* finite, > 0: Huber threshold on the residual r (units of T) */
+  double damping;       /* finite, >= 0: added to the normal matrix's diagonal */
+  int min_corr;         /* >= 6 */
+  double max_shift;     /* finite, > 0, metres: the guard on translation */
+  double min_cos;       /* [-1, 1]: the guard on rotation, (trace(R_f R_p^T) - 1) / 2 >= min_cos */
+  double eps;           /* finite, >= 0: an update with max_i |x_i| <= eps ends the frame's rounds */
+  int integrate;        /* 0 | 1: push each frame at its final pose before aligning the next */
+} ofdis_fuse_track_params;
+typedef struct ofdis_fuse_track_stats {
+  int status;           /* 0 aligned; 1 fewer than min_corr at the prediction; 2 rejected by the guard */
+  int n_corr;           /* valid cells at the last evaluated pose */
+  int rounds;           /* updates applied */
+  double cost0, cost;   /* sum of wt*r*r at the prediction and at the last evaluated pose */
+} ofdis_fuse_track_stats;  /* 32 bytes */
+int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* motions,
+                     const double* prev, const ofdis_stereo_camera* cam, const ofdis_fuse_track_params* p,
+                     const unsigned char* frames, size_t frame_stride, double* poses, ofdis_fuse_track_stats* stats,
+                     int width_org, int height_org, int memkind);
 
 /* Dense point trajectories (extension): the tracker of Sundaram, Brox and Keutzer ("Dense point trajectories by
  * GPU-accelerated large displacement optical flow", ECCV 2010) through consecutive pairs of bidirectional flows.

@@ -14,7 +14,8 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import (DISP_FILTER_FIELDS, EGO_PARAM_FIELDS, FUSE_PARAM_FIELDS, FUSE_POINT_DTYPE, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
+from .preprocess import (DISP_FILTER_FIELDS, EGO_PARAM_FIELDS, FUSE_PARAM_FIELDS, FUSE_POINT_DTYPE,
+                         FUSE_TRACK_PARAM_FIELDS, FUSE_TRACK_STATS_DTYPE, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
                          STAB_FRAME_DTYPE, STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS,
                          TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
                          fisher_fit, fisher_pack, fisher_sizes, gaussian_weights, motion_params,
@@ -45,7 +46,7 @@ EXPORTS = [
     "ofdis_traj_begin", "ofdis_traj_advance", "ofdis_traj_stats_get", "ofdis_scene_flow_fullres",
     "ofdis_fisher_begin", "ofdis_fisher_push", "ofdis_fisher_take", "ofdis_traj_advance_fisher",
     "ofdis_egomotion_fullres", "ofdis_fuse_begin", "ofdis_fuse_push", "ofdis_fuse_extract", "ofdis_fuse_render",
-    "ofdis_fuse_get_volume", "ofdis_fuse_set_volume", "ofdis_fuse_mesh",
+    "ofdis_fuse_get_volume", "ofdis_fuse_set_volume", "ofdis_fuse_mesh", "ofdis_fuse_track",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -137,6 +138,24 @@ class FuseParams(ctypes.Structure):
 
 assert tuple(k for k, _ in FuseParams._fields_) == FUSE_PARAM_FIELDS
 assert FUSE_POINT_DTYPE.itemsize == 28
+
+
+class FuseTrackParams(ctypes.Structure):
+    """ofdis_fuse_track_params (include/ofdis_b200.h)."""
+    _fields_ = [("step", ctypes.c_int), ("rounds", ctypes.c_int), ("min_weight", ctypes.c_float),
+                ("max_depth", ctypes.c_float), ("huber", ctypes.c_float), ("damping", ctypes.c_double),
+                ("min_corr", ctypes.c_int), ("max_shift", ctypes.c_double), ("min_cos", ctypes.c_double),
+                ("eps", ctypes.c_double), ("integrate", ctypes.c_int)]
+
+
+class FuseTrackStats(ctypes.Structure):
+    """ofdis_fuse_track_stats (include/ofdis_b200.h); FUSE_TRACK_STATS_DTYPE is the same record as numpy sees it."""
+    _fields_ = [("status", ctypes.c_int), ("n_corr", ctypes.c_int), ("rounds", ctypes.c_int),
+                ("cost0", ctypes.c_double), ("cost", ctypes.c_double)]
+
+
+assert tuple(k for k, _ in FuseTrackParams._fields_) == FUSE_TRACK_PARAM_FIELDS
+assert ctypes.sizeof(FuseTrackStats) == FUSE_TRACK_STATS_DTYPE.itemsize == 32
 
 
 class StabParams(ctypes.Structure):
@@ -281,6 +300,9 @@ def lib():
         L.ofdis_fuse_set_volume.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int]
         L.ofdis_fuse_mesh.argtypes = [ctypes.c_void_p, ctypes.c_float] + \
             [ctypes.c_void_p, ctypes.c_long, ctypes.POINTER(ctypes.c_long)] * 2 + [ctypes.c_int]
+        L.ofdis_fuse_track.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t] + \
+            [ctypes.c_void_p] * 2 + [ctypes.POINTER(StereoCamera), ctypes.POINTER(FuseTrackParams), ctypes.c_void_p,
+                                     ctypes.c_size_t] + [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -1194,6 +1216,52 @@ class Context:
                                        ctypes.byref(n_faces), memkind))
         return pts[:min(pt_capacity, n_pts.value)], faces[:min(face_capacity, n_faces.value)], n_pts.value, \
             n_faces.value
+
+    def fuse_track(self, disp, motions, prev, camera, params, *, width_org, height_org, frames=None, disp_stride=None,
+                   frame_stride=None, n=None, memkind=MEM_HOST):
+        """Aligns n frames to the volume, each before the next, and with params["integrate"] pushes each at its final
+        pose (ofdis_fuse_track; preprocess.fuse_track restates it).  disp (n, H, W) float32 positive disparities (NaN
+        unknown), motions (n, 3, 4) float64 camera k-1 to camera k or None (the identity), prev (3, 4) the
+        camera-to-world pose before frame 0, params a mapping with preprocess.FUSE_TRACK_PARAM_FIELDS or a
+        FuseTrackParams, frames (n, H, W[, noc]) uint8 when integrating into a volume with colour.  With
+        memkind=MEM_DEVICE disp and frames are device addresses the caller owns, n is required and the strides count
+        floats and bytes between frames (default one frame).  Returns (poses (n, 3, 4) float64, stats (n,)
+        FUSE_TRACK_STATS_DTYPE)."""
+        if not isinstance(params, FuseTrackParams):
+            params = FuseTrackParams(*[params[k] for k in FUSE_TRACK_PARAM_FIELDS])
+        pix = width_org * height_org
+        if memkind == MEM_HOST:
+            n = disp.shape[0] if isinstance(disp, np.ndarray) and disp.ndim == 3 else -1
+            ok = isinstance(disp, np.ndarray) and disp.dtype == np.float32 and disp.shape == (n, height_org, width_org) \
+                and (n == 0 or disp[0].flags["C_CONTIGUOUS"]) and disp.strides[0] % 4 == 0
+            if not ok:
+                raise ValueError("fuse_track: disp must be a float32 array (n, %d, %d) whose frames are C-contiguous"
+                                 % (height_org, width_org))
+            disp_stride = disp.strides[0] // 4 if n > 1 else pix
+            if frames is not None:
+                frame_stride = self._frames_u8("fuse_track: frames", frames, n, width_org, height_org)
+                frames = frames.ctypes.data
+        else:
+            if n is None:
+                raise ValueError("fuse_track: device input needs n, the number of frames at the address")
+            disp_stride = pix if disp_stride is None else disp_stride
+            frame_stride = pix * self.prm.noc if frame_stride is None else frame_stride
+        if motions is not None:
+            motions = np.ascontiguousarray(motions, np.float64)
+            if motions.size != 12 * n:
+                raise ValueError("fuse_track: motions must be (n, 3, 4) float64")
+        prev = np.ascontiguousarray(prev, np.float64)
+        if prev.size != 12:
+            raise ValueError("fuse_track: prev must be (3, 4) float64")
+        poses = np.zeros((max(n, 1), 3, 4))
+        stats = np.zeros(max(n, 1), FUSE_TRACK_STATS_DTYPE)
+        st = (FuseTrackStats * max(n, 1))()
+        self._ck(lib().ofdis_fuse_track(self._h, n, _ptr(disp), disp_stride, _ptr(motions), _ptr(prev),
+                                        self._fuse_cam(camera), ctypes.byref(params), _ptr(frames), frame_stride or 0,
+                                        _ptr(poses), st, width_org, height_org, memkind))
+        for k in range(n):
+            stats[k] = (st[k].status, st[k].n_corr, st[k].rounds, st[k].cost0, st[k].cost)
+        return poses[:n], stats[:n]
 
     def set_initflow_fullres(self, f0, f1, flow, width_org, height_org, memkind=MEM_HOST):
         """[f1-f0][height_org][width_org][nop] flows of the original frame size -> the init flow of pairs [f0, f1)

@@ -141,6 +141,10 @@ struct ofdis_ctx {
   // blocks and their total); grows, never shrinks; never touched by ofdis_run
   void* d_mesh = nullptr;
   size_t mesh_bytes = 0;
+  // lazily allocated workspace of ofdis_fuse_track (the pose chain's state, motions, poses and stats, the push pose,
+  // then the chunk sums); grows, never shrinks; never touched by ofdis_run
+  void* d_ftrack = nullptr;
+  size_t ftrack_bytes = 0;
   std::vector<float*> d_flow;   // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -517,6 +521,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   cudaFree(ctx->d_fisher);
   cudaFree(ctx->d_fuse);
   cudaFree(ctx->d_mesh);
+  cudaFree(ctx->d_ftrack);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -1756,6 +1761,116 @@ int ofdis_fuse_set_volume(ofdis_ctx* ctx, const float* T, const float* W, const 
   if (W) CK(cudaMemcpyAsync(v.W, W, 4 * N, kind, ctx->stream));
   if (color) CK(cudaMemcpyAsync(v.C, color, 3 * N, kind, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
+  return OFDIS_OK;
+}
+
+static bool finite_f64(double v) { return std::fabs(v) <= DBL_MAX; }
+
+int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* motions,
+                     const double* prev, const ofdis_stereo_camera* cam, const ofdis_fuse_track_params* p,
+                     const unsigned char* frames, size_t frame_stride, double* poses, ofdis_fuse_track_stats* stats,
+                     int width_org, int height_org, int memkind) {
+  static_assert(sizeof(ofdis_fuse_track_stats) == 32, "ofdis_fuse_track_stats: 32 bytes, as FUSE_TRACK_STATS_DTYPE");
+  if (!ctx) return OFDIS_ERR_ARG;
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_track: no live volume (ofdis_fuse_begin)");
+  const bool dev = memkind == OFDIS_MEM_DEVICE, color = ctx->fuse_vol.C != nullptr;
+  const size_t pix = (size_t)std::max(width_org, 0) * std::max(height_org, 0), hwc = pix * ctx->prm.noc;
+  bool ok = n >= 1 && n <= ctx->max_frames + 1 && disp && prev && poses && stats && fuse_cam_ok(cam) && p &&
+            disp_stride >= pix && !(dev && reinterpret_cast<uintptr_t>(disp) % sizeof(float));
+  ok = ok && p->step >= 1 && p->rounds >= 0 && p->rounds <= 32 && !std::isnan(p->min_weight) &&
+       p->max_depth > 0.0f && finite_gt0(p->huber) && finite_f64(p->damping) && p->damping >= 0.0 &&
+       p->min_corr >= 6 && finite_f64(p->max_shift) && p->max_shift > 0.0 && p->min_cos >= -1.0 && p->min_cos <= 1.0 &&
+       finite_f64(p->eps) && p->eps >= 0.0 && (p->integrate == 0 || p->integrate == 1);
+  const bool use_frames = ok && p->integrate && color;
+  ok = ok && (!use_frames || (frames && frame_stride >= hwc));
+  for (int i = 0; ok && i < 12; ++i) ok = finite_f64(prev[i]);
+  for (size_t i = 0; ok && motions && i < (size_t)12 * n; ++i) ok = finite_f64(motions[i]);
+  if (!ok) return fail(ctx, OFDIS_ERR_ARG, "fuse_track: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  NvtxRange nvtx("fuse", -1);
+  CK(cudaSetDevice(ctx->device));
+  FuseTrack t{};
+  t.w = width_org, t.h = height_org, t.s = p->step;
+  t.ncx = (width_org - 1) / p->step + 1;
+  t.cells = t.ncx * ((height_org - 1) / p->step + 1);
+  t.nchunks = (t.cells + 31) / 32;
+  t.rounds = p->rounds, t.min_corr = p->min_corr, t.has_motion = motions != nullptr;
+  t.min_weight = p->min_weight, t.max_depth = p->max_depth, t.huber = p->huber;
+  t.damping = p->damping, t.max_shift = p->max_shift, t.min_cos = p->min_cos, t.eps = p->eps;
+  t.cam = DispCamera{cam->fx * cam->baseline, cam->fx, cam->fy, cam->cx, cam->cy, cam->doffs};
+  // the workspace: the state, the motions, poses and stats of max_frames + 1 frames, the push pose, the chunk sums
+  const size_t F = (size_t)ctx->max_frames + 1;
+  const size_t b_s = align16(sizeof(FuseTrackState)), b_m = align16(sizeof(double) * 12 * F);
+  const size_t b_st = align16(sizeof(ofdis_fuse_track_stats) * F), b_g = align16(sizeof(float) * 12);
+  const size_t bytes = b_s + 2 * b_m + b_st + b_g + sizeof(double) * FTRACK_NE * (size_t)t.nchunks;
+  if (bytes > ctx->ftrack_bytes) {
+    CK(cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_ftrack);
+    ctx->d_ftrack = nullptr;
+    ctx->ftrack_bytes = 0;
+    if (cudaMalloc(&ctx->d_ftrack, bytes) != cudaSuccess) {
+      ctx->d_ftrack = nullptr;
+      return fail(ctx, OFDIS_ERR_NOMEM, "fuse_track workspace");
+    }
+    ctx->ftrack_bytes = bytes;
+  }
+  char* b = static_cast<char*>(ctx->d_ftrack);
+  t.state = reinterpret_cast<FuseTrackState*>(b);
+  t.motion = reinterpret_cast<const double*>(b + b_s);
+  t.pose = reinterpret_cast<double*>(b + b_s + b_m);
+  t.stats = reinterpret_cast<ofdis_fuse_track_stats*>(b + b_s + 2 * b_m);
+  t.g = reinterpret_cast<float*>(b + b_s + 2 * b_m + b_st);
+  t.chunk = reinterpret_cast<double*>(b + b_s + 2 * b_m + b_st + b_g);
+  t.disp = disp, t.disp_stride = disp_stride;
+  const unsigned char* fr = use_frames ? frames : nullptr;
+  size_t fstride = frame_stride;
+  if (!dev) {
+    // the staging buffer: the disparity maps, then the frames, packed; sized for max_frames + 1 of each, as the push
+    const size_t b_d = align16(sizeof(float) * pix * F);
+    rc = ensure_stage(ctx, b_d + (color ? hwc * F : 0));
+    if (rc) return rc;
+    char* st = static_cast<char*>(ctx->d_stage);
+    CK(cudaMemcpy2DAsync(st, sizeof(float) * pix, disp, sizeof(float) * disp_stride, sizeof(float) * pix, n,
+                         cudaMemcpyHostToDevice, ctx->stream));
+    t.disp = reinterpret_cast<const float*>(st), t.disp_stride = pix;
+    if (use_frames) {
+      CK(cudaMemcpy2DAsync(st + b_d, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+      fr = reinterpret_cast<const unsigned char*>(st + b_d), fstride = hwc;
+    }
+  }
+  FuseTrackState init{};
+  std::memcpy(init.prev, prev, sizeof(init.prev));
+  CK(cudaMemcpyAsync(t.state, &init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+  if (motions)
+    CK(cudaMemcpyAsync(const_cast<double*>(t.motion), motions, sizeof(double) * 12 * n, cudaMemcpyHostToDevice,
+                       ctx->stream));
+  // init and motions are pageable host memory: the copies have left them when cudaMemcpyAsync returns
+  FusePush fp{};
+  fp.g = t.g;
+  fp.n = 1, fp.w = width_org, fp.h = height_org, fp.noc = ctx->prm.noc, fp.max_depth = p->max_depth;
+  fp.cam = t.cam;
+  for (int k = 0; k < n; ++k) {
+    for (int r = 0; r <= p->rounds; ++r) {
+      const int kk = launch_fuse_track_eval(ctx->fuse_geom, ctx->fuse_vol, t, k, r, ctx->stream);
+      if (kk < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_track_kernel launch", cudaGetLastError());
+      ctx->launches += kk;
+    }
+    if (!p->integrate) continue;
+    fp.disp = t.disp + (size_t)k * t.disp_stride, fp.disp_stride = t.disp_stride;
+    fp.frames = fr ? fr + (size_t)k * fstride : nullptr, fp.frame_stride = fstride;
+    const int kk = launch_fuse_push(ctx->fuse_geom, ctx->fuse_vol, fp, ctx->stream);
+    if (kk < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_integrate_kernel launch", cudaGetLastError());
+    ctx->launches += kk;
+  }
+  std::vector<double> P((size_t)12 * n);
+  std::vector<ofdis_fuse_track_stats> S(n);
+  CK(cudaMemcpyAsync(P.data(), t.pose, sizeof(double) * P.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(S.data(), t.stats, sizeof(ofdis_fuse_track_stats) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  std::memcpy(poses, P.data(), sizeof(double) * P.size());
+  std::memcpy(stats, S.data(), sizeof(ofdis_fuse_track_stats) * n);
   return OFDIS_OK;
 }
 

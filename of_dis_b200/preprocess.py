@@ -1810,7 +1810,7 @@ def fuse_integrate(vol: dict, params, disp, poses, camera, max_depth=np.inf, fra
             cn = np.floor((C.astype(f32) * Wt[..., None] + obs.astype(f32)) / W1[..., None] + half)
             C[ok] = cn[ok].astype(np.uint8)
         T[ok] = Tn[ok]
-        Wt[ok] = np.minimum(W1, maxw)[ok]
+        Wt[ok] = np.fmin(W1, maxw)[ok]  # fminf: a NaN W becomes max_weight
     return vol
 
 
@@ -2082,6 +2082,178 @@ def write_fused_mesh_ply(path: str, pts, faces) -> None:
                  "end_header\n" % (len(pts), len(faces))).encode())
         f.write(rec.tobytes())
         f.write(frec.tobytes())
+
+
+# ---- camera tracking against the volume (ofdis_fuse_track) ------------------------------------------------------------
+FUSE_TRACK_PARAM_FIELDS = ("step", "rounds", "min_weight", "max_depth", "huber", "damping", "min_corr", "max_shift",
+                           "min_cos", "eps", "integrate")
+# ofdis_fuse_track_stats, field for field (32 bytes, 4 of padding after rounds)
+FUSE_TRACK_STATS_DTYPE = np.dtype({"names": ["status", "n_corr", "rounds", "cost0", "cost"],
+                                   "formats": ["<i4", "<i4", "<i4", "<f8", "<f8"], "offsets": [0, 4, 8, 16, 24],
+                                   "itemsize": 32})
+
+
+def fuse_track_predict(prev, motion) -> np.ndarray:
+    """Step 1 of ofdis_fuse_track: T(k-1) inv(M) in the header's float64 order (12,), or T(k-1) when motion is None."""
+    P = np.asarray(prev, np.float64).reshape(12)
+    if motion is None:
+        return P.copy()
+    m = np.asarray(motion, np.float64).reshape(12)
+    Ri = [[m[4 * c + r] for c in range(3)] for r in range(3)]
+    ti = [-(((m[r] * m[3]) + (m[4 + r] * m[7])) + (m[8 + r] * m[11])) for r in range(3)]
+    M = np.empty(12)
+    for r in range(3):
+        for c in range(3):
+            M[4 * r + c] = ((P[4 * r] * Ri[0][c]) + (P[4 * r + 1] * Ri[1][c])) + (P[4 * r + 2] * Ri[2][c])
+        M[4 * r + 3] = (((P[4 * r] * ti[0]) + (P[4 * r + 1] * ti[1])) + (P[4 * r + 2] * ti[2])) + P[4 * r + 3]
+    return M
+
+
+def fuse_track_cells(vol: dict, params, D: np.ndarray, cam: dict, step: int, min_weight, max_depth, M):
+    """Step 2 of ofdis_fuse_track at every cell of the map D (H, W) float32 for the float64 pose M (12,): returns
+    (valid (cells,) bool, r (cells,), G (cells, 3) and Pw (cells, 3) float32, meaningful where valid)."""
+    g = np.asarray(M, np.float64).reshape(12).astype(f32)
+    H, W = D.shape
+    s = int(step)
+    ncx, ncy = (W - 1) // s + 1, (H - 1) // s + 1
+    cell = np.arange(ncx * ncy)
+    px = np.minimum((cell % ncx) * s + s // 2, W - 1)
+    py = np.minimum((cell // ncx) * s + s // 2, H - 1)
+    T, Wt = vol["T"].ravel(), vol["W"].ravel()
+    nz, ny, nx = vol["T"].shape
+    o = [f32(v) for v in params["origin"]]
+    vox = f32(params["voxel"])
+    d = D[py, px]
+    with np.errstate(all="ignore"):
+        sd = d + cam["doffs"]
+        ok = (d >= 0) & (d <= f32(1e9)) & (sd > 0)
+        Z = cam["fb"] / sd
+        ok &= Z <= f32(max_depth)
+        X = ((px.astype(f32) - cam["cx"]) * Z) / cam["fx"]
+        Y = ((py.astype(f32) - cam["cy"]) * Z) / cam["fy"]
+        Pw, i0, fr = [], [], []
+        for e, n in enumerate((nx, ny, nz)):
+            Pw.append(((g[4 * e] * X + g[4 * e + 1] * Y) + g[4 * e + 2] * Z) + g[4 * e + 3])
+            q = (Pw[e] - o[e]) / vox
+            fl = np.floor(q)
+            ok &= (fl >= 0) & (fl <= f32(n - 2))
+            i0.append(fl)
+            fr.append((q - fl).astype(f32))
+    i0 = [np.where(ok, v, 0).astype(np.int64) for v in i0]
+    base = (i0[2] * ny + i0[1]) * nx + i0[0]
+    c = []
+    for off in (0, 1, nx, nx + 1, nx * ny, nx * ny + 1, nx * ny + nx, nx * ny + nx + 1):
+        ci = np.minimum(base + off, T.size - 1)  # clipped where the cell is invalid anyway
+        with np.errstate(invalid="ignore"):
+            ok &= (Wt[ci] >= f32(min_weight)) & (np.abs(T[ci]) < f32(1))
+        c.append(T[ci])
+    one = f32(1)
+    with np.errstate(all="ignore"):
+        gx, gy, gz = one - fr[0], one - fr[1], one - fr[2]
+        x00, x10 = c[0] * gx + c[1] * fr[0], c[2] * gx + c[3] * fr[0]
+        x01, x11 = c[4] * gx + c[5] * fr[0], c[6] * gx + c[7] * fr[0]
+        y0, y1 = x00 * gy + x10 * fr[1], x01 * gy + x11 * fr[1]
+        r = y0 * gz + y1 * fr[2]
+        G0 = (((c[1] - c[0]) * gy + (c[3] - c[2]) * fr[1]) * gz + ((c[5] - c[4]) * gy + (c[7] - c[6]) * fr[1]) * fr[2]) / vox
+        G1 = ((x10 - x00) * gz + (x11 - x01) * fr[2]) / vox
+        G2 = (y1 - y0) / vox
+    return ok, r.astype(f32), np.stack([G0, G1, G2], -1).astype(f32), np.stack(Pw, -1).astype(f32)
+
+
+def fuse_track_terms(r, G, Pw, huber) -> np.ndarray:
+    """The 28 float64 terms of cells (m, 28): N (21, upper triangle row-major), b (6) and the cost, step 2's order."""
+    a = [G[:, e].astype(np.float64) for e in range(3)]
+    w0, w1, w2 = (2.0 * Pw[:, e].astype(np.float64) for e in range(3))
+    J = [(a[1] * -w2) + (a[2] * w1), (a[0] * w2) + (a[2] * -w0), (a[0] * -w1) + (a[1] * w0), a[0], a[1], a[2]]
+    ar = np.abs(r)
+    with np.errstate(all="ignore"):
+        wt = np.where(ar <= f32(huber), f32(1), f32(huber) / ar).astype(np.float64)
+    rd = r.astype(np.float64)
+    terms = [(wt * J[i]) * J[j] for i in range(6) for j in range(i, 6)]
+    terms += [-((wt * J[i]) * rd) for i in range(6)]
+    terms.append((wt * rd) * rd)
+    return np.stack(terms, -1)
+
+
+def fuse_track_eval(vol: dict, params, D, cam: dict, p: dict, M):
+    """One evaluation of ofdis_fuse_track: (N (6, 6) mirrored, b (6,), cost, n_corr) at the pose M."""
+    ok, r, G, Pw = fuse_track_cells(vol, params, D, cam, p["step"], p["min_weight"], p["max_depth"], M)
+    with np.errstate(all="ignore"):
+        T = np.where(ok[:, None], fuse_track_terms(r, G, Pw, p["huber"]), 0.0)
+    v = _chunk_tree(T)
+    A = np.zeros((6, 6))
+    e = 0
+    for a in range(6):
+        for b in range(a, 6):
+            A[a, b] = A[b, a] = v[e]
+            e += 1
+    return A, v[21:27], v[27], int(ok.sum())
+
+
+def fuse_track_guard(M, pred, max_shift, min_cos) -> bool:
+    """Step 4's test of ofdis_fuse_track: the last evaluated pose M against the prediction."""
+    dt = [M[3] - pred[3], M[7] - pred[7], M[11] - pred[11]]
+    shift = np.sqrt((dt[0] * dt[0] + dt[1] * dt[1]) + dt[2] * dt[2])
+    s = [((M[4 * i] * pred[4 * i]) + (M[4 * i + 1] * pred[4 * i + 1])) + (M[4 * i + 2] * pred[4 * i + 2])
+         for i in range(3)]
+    return bool(shift <= max_shift) and bool((((s[0] + s[1]) + s[2]) - 1.0) / 2.0 >= min_cos)
+
+
+def fuse_track_params(params) -> dict:
+    return {k: params[k] for k in FUSE_TRACK_PARAM_FIELDS}
+
+
+def fuse_track(vol: dict, fuse_params, track_params, disp, motions, prev, camera, frames=None):
+    """Restates ofdis_fuse_track: disp (n, H, W) float32, motions (n, 3, 4) float64 or None (the identity), prev (3, 4)
+    camera-to-world, frames (n, H, W[, 3]) uint8 when integrating into a volume with colour.  With integrate, vol is
+    updated in place by fuse_integrate.  Returns (poses (n, 3, 4) float64, stats (n,) FUSE_TRACK_STATS_DTYPE)."""
+    p = fuse_track_params(track_params)
+    cam = _ego_cam(camera)
+    disp = np.asarray(disp, f32).reshape((-1,) + np.shape(disp)[-2:])
+    n = disp.shape[0]
+    mot = None if motions is None else np.asarray(motions, np.float64).reshape(n, 12)
+    P = np.asarray(prev, np.float64).reshape(12)
+    poses = np.zeros((n, 12))
+    stats = np.zeros(n, FUSE_TRACK_STATS_DTYPE)
+    for k in range(n):
+        pred = fuse_track_predict(P, None if mot is None else mot[k])
+        M, applied, status = pred, 0, 0
+        for r in range(int(p["rounds"]) + 1):
+            A, b, cost, cnt = fuse_track_eval(vol, fuse_params, disp[k], cam, p, M)
+            if r == 0:
+                cost0 = cost
+            if cnt < int(p["min_corr"]):
+                status = 1 if r == 0 else 0
+                break
+            if r == int(p["rounds"]):
+                break
+            for i in range(6):
+                A[i, i] = A[i, i] + float(p["damping"])
+            x, ok = motion_solve(A[None], b[None])
+            if not ok[0] or np.max(np.abs(x[0])) <= float(p["eps"]):
+                break
+            M, applied = ego_update(M, x[0]), r + 1
+        if status == 0 and not fuse_track_guard(M, pred, float(p["max_shift"]), float(p["min_cos"])):
+            status = 2
+        F = pred if status else M
+        poses[k] = F
+        stats[k] = (status, cnt, applied, cost0, cost)
+        if p["integrate"]:
+            fuse_integrate(vol, fuse_params, disp[k:k + 1], F.reshape(1, 3, 4), camera, p["max_depth"],
+                           None if vol["C"] is None else np.asarray(frames)[k:k + 1])
+        P = F
+    return poses.reshape(n, 3, 4), stats
+
+
+def trajectory_errors(abs_poses, gt_abs):
+    """Per frame the absolute error of camera-to-world poses abs_poses against gt_abs (both (n, 3, 4), expressed in
+    the same world, e.g. sharing frame 0): the translation error |t - t_gt| in metres and the rotation error
+    acos((trace(R_gt^T R) - 1) / 2) in degrees.  Returns (t_err (n,), r_err (n,))."""
+    A = np.asarray(abs_poses, np.float64).reshape(-1, 3, 4)
+    G = np.asarray(gt_abs, np.float64).reshape(-1, 3, 4)
+    t_err = np.linalg.norm(A[:, :, 3] - G[:, :, 3], axis=1)
+    c = np.clip(0.5 * (np.einsum("kij,kij->k", A[:, :, :3], G[:, :, :3]) - 1.0), -1.0, 1.0)
+    return t_err, np.degrees(np.arccos(c))
 
 
 # ---- video stabilisation (ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish) ---------------------------------

@@ -9,8 +9,9 @@ disparity (union-find speckles, fill, depth and xyz) and a global motion (corres
 the bulk-copied score tiles with and without refills, refits, per-pixel outputs), a stereo ego-motion (the same
 stages on 32-byte correspondences, non-finite disparities, score tile refills), a Fisher encoding (projection,
 posteriors, float64 statistics, the take) and a TSDF fusion (integration, crossing count, scan and write, ray casting)
-and its marching cubes (set_volume, the write with vertex bases, cube count, scan, faces) checked against their
-restatements.  Results are checked against the
+and its marching cubes (set_volume, the write with vertex bases, cube count, scan, faces) and a camera tracking
+against it (the evaluation kernel's chunk sums, arrival counter and tree, with and without the push) checked against
+their restatements.  Results are checked against the
 oracle so that a clean log means a correct run."""
 import os
 import sys
@@ -263,6 +264,45 @@ ok = nf > 100 and np.array_equal(hp.view(np.uint8), ep.view(np.uint8)) and np.ar
     np.array_equal(dp.cpu().numpy()[:28 * (nv - 1)], ep[:nv - 1].view(np.uint8)) and \
     np.array_equal(df.cpu().numpy()[:3 * (nf - 1)].view(np.uint32), ef[:nf - 1].ravel())
 print("%-22s %s" % ("fuse_mesh", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# camera tracking: a 29 x 17 x 33 volume loaded with fuse_set_volume (a tilted plane's TSDF with planted NaN, +-0 and
+# +-1 T, W at, just below and above min_weight and NaN), disparities with NaN, -0, +inf and 3e9, three frames of 4
+# rounds, without and with integration, the poses, stats and volume checked bitwise
+tp_ = dict(nx=29, ny=17, nz=33, origin=(-1.0, -0.6, 0.4), voxel=0.05, trunc=0.15, max_weight=5.0, color=1)
+tv = preprocess.fuse_new_volume(tp_)
+zz = tp_["origin"][2] + np.arange(tp_["nz"])[:, None, None] * tp_["voxel"]
+yy = tp_["origin"][1] + np.arange(tp_["ny"])[None, :, None] * tp_["voxel"]
+tv["T"][:] = np.clip((1.2 + 0.1 * yy - zz) / tp_["trunc"], -1, 1).astype(np.float32)
+tv["W"][:] = rng.choice(np.array([1.0, 2.0, 3.0], np.float32), tv["W"].shape)
+for v, share in ((0.0, 0.02), (-0.0, 0.02), (1.0, 0.01), (-1.0, 0.01), (np.nan, 0.01)):
+    tv["T"][rng.random(tv["T"].shape) < share] = np.float32(v)
+for v, share in ((0.0, 0.02), (below1, 0.02), (np.nan, 0.01)):
+    tv["W"][rng.random(tv["W"].shape) < share] = np.float32(v)
+tv["C"][:] = rng.integers(0, 256, tv["C"].shape)
+tmaps = (np.float32(40.0) / rng.uniform(1.15, 1.25, (3, h3, w3)) - np.float32(0.25)).astype(np.float32)
+for v, share in ((np.nan, 0.05), (-0.0, 0.03), (np.inf, 0.02), (3e9, 0.02)):
+    tmaps[rng.random(tmaps.shape) < share] = v
+tmot = np.stack([np.concatenate([synth.axis_angle(rng.uniform(-0.005, 0.005, 3)),
+                                 rng.uniform(-0.02, 0.02, (3, 1))], 1) for _ in range(3)])
+tprev = np.concatenate([np.eye(3), [[0.01], [0.0], [0.02]]], 1)
+ok = True
+for integrate in (0, 1):
+    trk = dict(step=1, rounds=4, min_weight=1.0, max_depth=float("inf"), huber=0.2, damping=0.1, min_corr=6,
+               max_shift=0.5, min_cos=0.99, eps=0.0, integrate=integrate)
+    ctx = api.Context(prm, w3, h3, prm.p_samp_s, 2)
+    ctx.fuse_begin(tp_)
+    ctx.fuse_set_volume(tv["T"], tv["W"], tv["C"])
+    gpo, gst = ctx.fuse_track(tmaps, tmot, tprev, cam, trk, width_org=w3, height_org=h3, frames=rgb)
+    gv = ctx.fuse_volume()
+    ctx.close()
+    ev = {k: v.copy() for k, v in tv.items()}
+    epo, est = preprocess.fuse_track(ev, tp_, trk, tmaps, tmot, tprev, cam, rgb)
+    ok = ok and np.array_equal(gpo.view(np.uint64), epo.view(np.uint64)) and \
+        all(np.array_equal(gst[k], est[k]) for k in est.dtype.names) and (est["rounds"] > 0).any() and \
+        all(np.array_equal(*(np.where(np.isnan(a), np.float32(np.nan), a).view(np.uint8) if a.dtype == np.float32
+                             else a for a in (gv[k], ev[k]))) for k in ("T", "W", "C"))
+print("%-22s %s" % ("fuse_track", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
