@@ -198,6 +198,50 @@ int ofdis_set_swapped_slots(ofdis_ctx* ctx, int f0, int f1, int swapped);
  * host output goes through the context's full-resolution scratch.  The flows are not changed. */
 int ofdis_consistency_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, unsigned char* mask, float* err, float alpha,
                               float beta, int width_org, int height_org, int memkind);
+/* Per-pixel confidence of the last run's slots [f0, f1) (extension): a number in [0, 1] per pixel that ranks how far
+ * the flow or disparity there can be trusted, from three terms (the measures surveyed by Hu and Mordohai, PAMI 2012).
+ * Flow (nop 2) and stereo (nop 1, v = 0) contexts.  For pair k, F is slot a = f0+k's full-resolution flow, exactly
+ * what ofdis_get_flow_fullres returns (computed from the level flows, without a full-resolution copy).  I0 and I1 are
+ * frames0 + k*frame_stride and frames1 + k*frame_stride, [H][W][noc] bytes in the context's channel count
+ * (frame_stride >= H*W*noc; a clip passes frames1 = frames0 + frame_stride, as ofdis_interpolate_fullres).
+ * W = width_org, H = height_org.  Everything is float32 with +, -, *, IEEE / and sqrtf only, without contraction; every
+ * sum starts from +0.0f and runs dy = -r .. r outer, dx = -r .. r inner.
+ *   Brightness g(I, x, y): the byte, or ((float)b0 + (float)b1 + (float)b2) / 3.0f in memory order (the tracker's).
+ *   Window: r = p->radius; window pixel (dx, dy) of (X, Y) is q = (clamp(X + dx), clamp(Y + dy)), clamped to the frame
+ *     as the tracker's seeding clamps (border pixels repeat).
+ *   Warp: for a window pixel q with flow F(q) = (u, v): (xs, ys) = ((float)qx + u, (float)qy + v); when 0 <= xs <= W-1
+ *     and 0 <= ys <= H-1 (NaN fails), Iw(q) = the bilinear rule of ofdis_consistency_fullres on the brightness of I1's
+ *     four corners (x0 = floor(xs), x1 = min(x0 + 1, W - 1), fx = xs - x0, the same in y; r0 = g00*(1-fx) + g10*fx,
+ *     r1 = g01*(1-fx) + g11*fx, Iw = r0*(1-fy) + r1*fy); else q is not a sample.
+ *   z (photometric): over the samples of the window, n their count (int), s0 += g(I0, q), s1 += Iw(q); with
+ *     n >= min_count, m0 = s0 / (float)n, m1 = s1 / (float)n, then over the samples again c00 += (g0 - m0)*(g0 - m0),
+ *     c11 += (Iw - m1)*(Iw - m1), c01 += (g0 - m0)*(Iw - m1); den = c00 * c11; z = c01 / sqrtf(den) when den > 0.
+ *     Otherwise (n < min_count, or zero variance) z = qNaN.
+ *   e (forward-backward / left-right): with b0 >= 0, err of ofdis_consistency_fullres of slot a against slot b0+k at
+ *     (X, Y), bit for bit (+inf where the target leaves the frame, a NaN of any payload where the partner's flow there is
+ *     NaN); with b0 < 0, e = qNaN and it is not used.
+ *   lambda (texture): over every window pixel, ix = (g(I0, min(qx+1, W-1), qy) - g(I0, max(qx-1, 0), qy)) * 0.5f,
+ *     iy likewise in y, a += ix*ix, b += ix*iy, c += iy*iy; d = a - c; lambda = (a + c)*0.5f - sqrtf(d*d*0.25f + b*b):
+ *     the smaller eigenvalue of the structure tensor, at r = 2 the tracker's seeding value bit for bit.
+ *   conf = (cz * ce) * cl with cz = z > 0 ? z : 0 (NaN gives 0; rounding may leave z a few ulp above 1),
+ *     ce = e >= 0 ? s_fb / (s_fb + e) : 0 (so +inf gives 0 and NaN gives 0), and ce = 1 with b0 < 0,
+ *     cl = lambda > 0 ? lambda / (lambda + s_tex) : 0.
+ * conf = [f1-f0][H][W] float32, terms = [f1-f0][H][W][3] float32 (z, e, lambda); either may be NULL, not both.
+ * frames, conf and terms are in memkind: host frames go through the context's staging buffer (two 2-D copies), host
+ * outputs through its full-resolution scratch, and the call then synchronises the stream once.  One kernel for all
+ * pairs.  OFDIS_ERR_ARG, with the outputs untouched: slots outside the context, b0 >= 0 with [b0, b0 + f1 - f0)
+ * outside it, a NULL p, radius outside 1 .. 7, s_fb or s_tex not finite and > 0, min_count outside 1 .. (2r+1)^2,
+ * NULL frames0 or frames1, frame_stride below one frame, both outputs NULL, a device output not 4-byte aligned; frame
+ * sizes as ofdis_get_flow_fullres checks them.  Not part of ofdis_run's graph; the flows are not changed. */
+typedef struct ofdis_conf_params {
+  int radius;           /* window (2r+1)^2, r in 1 .. 7 */
+  float s_fb;           /* > 0, finite: scale of the forward-backward term (px^2) */
+  float s_tex;          /* > 0, finite: scale of the texture term */
+  int min_count;        /* 1 .. (2r+1)^2: in-frame warped samples a window needs */
+} ofdis_conf_params;
+int ofdis_confidence_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_conf_params* p,
+                             const unsigned char* frames0, const unsigned char* frames1, size_t frame_stride,
+                             float* conf, float* terms, int width_org, int height_org, int memkind);
 /* Error statistics of one (pair, class) of ofdis_flow_error_fullres (48 bytes). */
 typedef struct ofdis_error_stats {
   long long n;          /* pixels counted */
@@ -689,6 +733,18 @@ int ofdis_fuse_begin(ofdis_ctx* ctx, const ofdis_fuse_params* p);
 int ofdis_fuse_push(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* poses,
                     const ofdis_stereo_camera* cam, float max_depth, const unsigned char* frames, size_t frame_stride,
                     int width_org, int height_org, int memkind);
+/* Confidence-weighted integration: ofdis_fuse_push with weight + k*weight_stride ([H][W] float32 in memkind, for
+ * example ofdis_confidence_fullres's conf) for frame k.  An observation at pixel (px, py) with c = weight there is
+ * skipped unless 0 < c <= FLT_MAX (NaN, +-0, negative values and +-inf skip); otherwise, in float32, W' = W + c, T = (T*W + f*c) / W',
+ * each colour byte floor(((float)col*W + (float)obs*c) / W' + 0.5f) and W = fminf(W', max_weight).  With c = 1.0f
+ * everywhere this is ofdis_fuse_push bit for bit (f*1 = f).  W is then a sum of confidences, and min_weight in
+ * ofdis_fuse_extract, ofdis_fuse_render, ofdis_fuse_mesh and ofdis_fuse_track compares against that sum.  Host weights go
+ * through the staging buffer after the maps and frames.  One kernel, as the push; OFDIS_ERR_ARG as the push, and for a
+ * NULL weight, weight_stride < W*H or a device weight that is not 4-byte aligned. */
+int ofdis_fuse_push_weighted(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* poses,
+                             const ofdis_stereo_camera* cam, float max_depth, const unsigned char* frames,
+                             size_t frame_stride, const float* weight, size_t weight_stride, int width_org,
+                             int height_org, int memkind);
 /* The volume's zero crossings in order: *count (host) gets the total, pts ([capacity] in memkind) the first
  * min(capacity, total); capacity 0 counts only (pts may then be NULL).  Three kernels (count, scan, write), then one
  * synchronise.  Host output goes through the context's full-resolution scratch.  OFDIS_ERR_ARG: no live volume, NULL
@@ -830,6 +886,19 @@ int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_strid
                      const double* prev, const ofdis_stereo_camera* cam, const ofdis_fuse_track_params* p,
                      const unsigned char* frames, size_t frame_stride, double* poses, ofdis_fuse_track_stats* stats,
                      int width_org, int height_org, int memkind);
+/* Confidence-weighted tracking: ofdis_fuse_track with weight + k*weight_stride ([H][W] float32 in memkind) for frame
+ * k.  A cell at pixel (px, py) is valid only when, in addition, 0 < c <= FLT_MAX for c = weight there (NaN and +-inf
+ * fail); its weight in N,
+ * b and the cost becomes (double)(wt * c), the float32 product of the Huber weight and c.  With integrate, the push is
+ * ofdis_fuse_push_weighted's.  With c = 1.0f everywhere this is ofdis_fuse_track bit for bit: poses, stats and volume.
+ * Host weights go through the staging buffer after the maps and frames.  The same launches as ofdis_fuse_track;
+ * OFDIS_ERR_ARG as ofdis_fuse_track, and for a NULL weight, weight_stride < W*H or a device weight that is not 4-byte
+ * aligned. */
+int ofdis_fuse_track_weighted(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* motions,
+                              const double* prev, const ofdis_stereo_camera* cam, const ofdis_fuse_track_params* p,
+                              const unsigned char* frames, size_t frame_stride, const float* weight,
+                              size_t weight_stride, double* poses, ofdis_fuse_track_stats* stats, int width_org,
+                              int height_org, int memkind);
 
 /* Dense point trajectories (extension): the tracker of Sundaram, Brox and Keutzer ("Dense point trajectories by
  * GPU-accelerated large displacement optical flow", ECCV 2010) through consecutive pairs of bidirectional flows.

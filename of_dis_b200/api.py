@@ -14,7 +14,7 @@ import os
 import numpy as np
 
 from .params import CParams, DisParams
-from .preprocess import (DISP_FILTER_FIELDS, EGO_PARAM_FIELDS, FUSE_PARAM_FIELDS, FUSE_POINT_DTYPE,
+from .preprocess import (CONF_PARAM_FIELDS, DISP_FILTER_FIELDS, EGO_PARAM_FIELDS, FUSE_PARAM_FIELDS, FUSE_POINT_DTYPE,
                          FUSE_TRACK_PARAM_FIELDS, FUSE_TRACK_STATS_DTYPE, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
                          STAB_FRAME_DTYPE, STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS,
                          TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
@@ -47,6 +47,7 @@ EXPORTS = [
     "ofdis_fisher_begin", "ofdis_fisher_push", "ofdis_fisher_take", "ofdis_traj_advance_fisher",
     "ofdis_egomotion_fullres", "ofdis_fuse_begin", "ofdis_fuse_push", "ofdis_fuse_extract", "ofdis_fuse_render",
     "ofdis_fuse_get_volume", "ofdis_fuse_set_volume", "ofdis_fuse_mesh", "ofdis_fuse_track",
+    "ofdis_confidence_fullres", "ofdis_fuse_push_weighted", "ofdis_fuse_track_weighted",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -146,6 +147,15 @@ class FuseTrackParams(ctypes.Structure):
                 ("max_depth", ctypes.c_float), ("huber", ctypes.c_float), ("damping", ctypes.c_double),
                 ("min_corr", ctypes.c_int), ("max_shift", ctypes.c_double), ("min_cos", ctypes.c_double),
                 ("eps", ctypes.c_double), ("integrate", ctypes.c_int)]
+
+
+class ConfParams(ctypes.Structure):
+    """ofdis_conf_params (include/ofdis_b200.h)."""
+    _fields_ = [("radius", ctypes.c_int), ("s_fb", ctypes.c_float), ("s_tex", ctypes.c_float),
+                ("min_count", ctypes.c_int)]
+
+
+assert tuple(k for k, _ in ConfParams._fields_) == CONF_PARAM_FIELDS
 
 
 class FuseTrackStats(ctypes.Structure):
@@ -303,6 +313,15 @@ def lib():
         L.ofdis_fuse_track.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t] + \
             [ctypes.c_void_p] * 2 + [ctypes.POINTER(StereoCamera), ctypes.POINTER(FuseTrackParams), ctypes.c_void_p,
                                      ctypes.c_size_t] + [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
+        L.ofdis_fuse_track_weighted.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t] + \
+            [ctypes.c_void_p] * 2 + [ctypes.POINTER(StereoCamera), ctypes.POINTER(FuseTrackParams)] + \
+            [ctypes.c_void_p, ctypes.c_size_t] * 2 + [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3
+        L.ofdis_fuse_push_weighted.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
+                                               ctypes.c_void_p, ctypes.POINTER(StereoCamera), ctypes.c_float] + \
+            [ctypes.c_void_p, ctypes.c_size_t] * 2 + [ctypes.c_int] * 3
+        L.ofdis_confidence_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
+            [ctypes.POINTER(ConfParams), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 2 + \
+            [ctypes.c_int] * 3
         L.ofdis_set_initflow_fullres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.ofdis_set_initflow_from_result.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5
@@ -495,6 +514,44 @@ class Context:
         if memkind == MEM_HOST:
             self.sync()
         return mask, err
+
+    def confidence_fullres(self, f0, f1, b0, frames0, frames1, params, width_org, height_org, with_conf=True,
+                           with_terms=False, memkind=MEM_HOST, conf=None, terms=None, frame_stride=None):
+        """Per-pixel confidence of the last run's slots [f0, f1) (ofdis_confidence_fullres; preprocess.confidence
+        restates it), with the forward-backward term against slots [b0, b0 + f1 - f0), or without it for b0 < 0.
+        params: a mapping with preprocess.CONF_PARAM_FIELDS or a ConfParams.  Returns (conf, terms): [f1-f0][H][W]
+        and [f1-f0][H][W][3] (z, e, lambda) float32, each None unless asked for.  Host: frames0 and frames1 as
+        interpolate_fullres takes them (frames[:-1] / frames[1:] of a clip qualify), outputs new or given as numpy
+        arrays of exactly that shape; the call synchronises the stream.  With memkind=MEM_DEVICE frames0, frames1,
+        conf and terms are device addresses (conf or terms may be None) and frame_stride the bytes between frames
+        (default one frame)."""
+        if not isinstance(params, ConfParams):
+            params = ConfParams(int(params["radius"]), float(params["s_fb"]), float(params["s_tex"]),
+                                int(params["min_count"]))
+        n = max(f1 - f0, 0)
+        hwc = height_org * width_org * self.prm.noc
+        if memkind == MEM_HOST:
+            strides = [self._frames_u8("confidence_fullres: %s" % name, arr, n, width_org, height_org)
+                       for name, arr in (("frames0", frames0), ("frames1", frames1))]
+            if strides[0] != strides[1]:
+                raise ValueError("confidence_fullres: frames0 and frames1 must have the same strides[0]")
+            frame_stride = strides[0]
+            frames0, frames1 = frames0.ctypes.data, frames1.ctypes.data
+            shapes = {"conf": (n, height_org, width_org), "terms": (n, height_org, width_org, 3)}
+            conf = (np.empty(shapes["conf"], np.float32) if conf is None else conf) if with_conf else None
+            terms = (np.empty(shapes["terms"], np.float32) if terms is None else terms) if with_terms else None
+            for name, arr in (("conf", conf), ("terms", terms)):
+                if arr is not None and not (isinstance(arr, np.ndarray) and arr.dtype == np.float32 and
+                                            arr.shape == shapes[name] and arr.flags["C_CONTIGUOUS"] and
+                                            arr.flags["WRITEABLE"]):
+                    raise ValueError("confidence_fullres: %s must be a writeable C-contiguous float32 array of shape %s"
+                                     % (name, shapes[name]))
+        else:
+            frame_stride = hwc if frame_stride is None else frame_stride
+        self._ck(lib().ofdis_confidence_fullres(self._h, f0, f1, b0, ctypes.byref(params), _ptr(frames0),
+                                                _ptr(frames1), frame_stride, _ptr(conf), _ptr(terms), width_org,
+                                                height_org, memkind))
+        return conf, terms
 
     def disparity_fullres(self, f0, f1, b0, width_org, height_org, lr_check=0, alpha=0.0, beta=1.0, speckle_size=0,
                           speckle_diff=1.0, fill=0, camera=None, outputs=("disp", "status"), memkind=MEM_HOST,
@@ -1111,12 +1168,14 @@ class Context:
         return poses.reshape(-1, 12)
 
     def fuse_push(self, disp, poses, camera, *, width_org, height_org, max_depth=float("inf"), frames=None,
-                  disp_stride=None, frame_stride=None, memkind=MEM_HOST):
+                  disp_stride=None, frame_stride=None, memkind=MEM_HOST, weights=None, weight_stride=None):
         """Integrates n frames into the volume (ofdis_fuse_push; preprocess.fuse_integrate restates it): disp (n, H, W)
         positive disparities (NaN unknown), poses (n, 3, 4) camera-to-world float64 on the host, camera a mapping
         with STEREO_CAMERA_FIELDS and, when the volume keeps colour, frames (n, H, W[, noc]) uint8.  Host arrays'
         frames must be C-contiguous and equally spaced; with memkind=MEM_DEVICE disp and frames are device addresses
-        the caller owns and the strides count floats and bytes between frames (default one frame)."""
+        the caller owns and the strides count floats and bytes between frames (default one frame).  weights (n, H, W)
+        float32 (e.g. confidence_fullres's conf), or a device address with weight_stride floats between frames,
+        calls ofdis_fuse_push_weighted instead."""
         poses = self._fuse_poses(poses)
         n = poses.shape[0]
         pix = width_org * height_org
@@ -1130,11 +1189,31 @@ class Context:
             if frames is not None:
                 frame_stride = self._frames_u8("fuse_push: frames", frames, n, width_org, height_org)
                 frames = frames.ctypes.data
+            if weights is not None:
+                weight_stride = self._weights_f32("fuse_push: weights", weights, n, width_org, height_org)
         else:
             disp_stride = pix if disp_stride is None else disp_stride
             frame_stride = pix * self.prm.noc if frame_stride is None else frame_stride
-        self._ck(lib().ofdis_fuse_push(self._h, n, _ptr(disp), disp_stride, _ptr(poses), self._fuse_cam(camera),
-                                       max_depth, _ptr(frames), frame_stride or 0, width_org, height_org, memkind))
+            weight_stride = pix if weight_stride is None else weight_stride
+        if weights is None:
+            self._ck(lib().ofdis_fuse_push(self._h, n, _ptr(disp), disp_stride, _ptr(poses), self._fuse_cam(camera),
+                                           max_depth, _ptr(frames), frame_stride or 0, width_org, height_org, memkind))
+        else:
+            self._ck(lib().ofdis_fuse_push_weighted(self._h, n, _ptr(disp), disp_stride, _ptr(poses),
+                                                    self._fuse_cam(camera), max_depth, _ptr(frames), frame_stride or 0,
+                                                    _ptr(weights), weight_stride, width_org, height_org, memkind))
+
+    @staticmethod
+    def _weights_f32(name, weights, n, width_org, height_org):
+        """Checks a host float32 array of n (height_org, width_org) maps whose maps are C-contiguous and returns its
+        stride in floats."""
+        ok = isinstance(weights, np.ndarray) and weights.dtype == np.float32 and \
+            weights.shape == (n, height_org, width_org) and (n == 0 or weights[0].flags["C_CONTIGUOUS"]) and \
+            weights.strides[0] % 4 == 0 and (n < 2 or weights.strides[0] >= 4 * height_org * width_org)
+        if not ok:
+            raise ValueError("%s must be a float32 array of shape %s whose maps are C-contiguous"
+                             % (name, (n, height_org, width_org)))
+        return weights.strides[0] // 4 if n > 1 else width_org * height_org
 
     def fuse_extract(self, min_weight=1.0, capacity=None, memkind=MEM_HOST, out=None):
         """The volume's zero crossings (ofdis_fuse_extract; preprocess.fuse_extract restates it).  Host: returns
@@ -1218,15 +1297,16 @@ class Context:
             n_faces.value
 
     def fuse_track(self, disp, motions, prev, camera, params, *, width_org, height_org, frames=None, disp_stride=None,
-                   frame_stride=None, n=None, memkind=MEM_HOST):
+                   frame_stride=None, n=None, memkind=MEM_HOST, weights=None, weight_stride=None):
         """Aligns n frames to the volume, each before the next, and with params["integrate"] pushes each at its final
         pose (ofdis_fuse_track; preprocess.fuse_track restates it).  disp (n, H, W) float32 positive disparities (NaN
         unknown), motions (n, 3, 4) float64 camera k-1 to camera k or None (the identity), prev (3, 4) the
         camera-to-world pose before frame 0, params a mapping with preprocess.FUSE_TRACK_PARAM_FIELDS or a
         FuseTrackParams, frames (n, H, W[, noc]) uint8 when integrating into a volume with colour.  With
         memkind=MEM_DEVICE disp and frames are device addresses the caller owns, n is required and the strides count
-        floats and bytes between frames (default one frame).  Returns (poses (n, 3, 4) float64, stats (n,)
-        FUSE_TRACK_STATS_DTYPE)."""
+        floats and bytes between frames (default one frame).  weights (n, H, W) float32, or a device address with
+        weight_stride floats between frames, calls ofdis_fuse_track_weighted instead.  Returns (poses (n, 3, 4)
+        float64, stats (n,) FUSE_TRACK_STATS_DTYPE)."""
         if not isinstance(params, FuseTrackParams):
             params = FuseTrackParams(*[params[k] for k in FUSE_TRACK_PARAM_FIELDS])
         pix = width_org * height_org
@@ -1241,11 +1321,14 @@ class Context:
             if frames is not None:
                 frame_stride = self._frames_u8("fuse_track: frames", frames, n, width_org, height_org)
                 frames = frames.ctypes.data
+            if weights is not None:
+                weight_stride = self._weights_f32("fuse_track: weights", weights, n, width_org, height_org)
         else:
             if n is None:
                 raise ValueError("fuse_track: device input needs n, the number of frames at the address")
             disp_stride = pix if disp_stride is None else disp_stride
             frame_stride = pix * self.prm.noc if frame_stride is None else frame_stride
+            weight_stride = pix if weight_stride is None else weight_stride
         if motions is not None:
             motions = np.ascontiguousarray(motions, np.float64)
             if motions.size != 12 * n:
@@ -1256,9 +1339,15 @@ class Context:
         poses = np.zeros((max(n, 1), 3, 4))
         stats = np.zeros(max(n, 1), FUSE_TRACK_STATS_DTYPE)
         st = (FuseTrackStats * max(n, 1))()
-        self._ck(lib().ofdis_fuse_track(self._h, n, _ptr(disp), disp_stride, _ptr(motions), _ptr(prev),
-                                        self._fuse_cam(camera), ctypes.byref(params), _ptr(frames), frame_stride or 0,
-                                        _ptr(poses), st, width_org, height_org, memkind))
+        if weights is None:
+            self._ck(lib().ofdis_fuse_track(self._h, n, _ptr(disp), disp_stride, _ptr(motions), _ptr(prev),
+                                            self._fuse_cam(camera), ctypes.byref(params), _ptr(frames),
+                                            frame_stride or 0, _ptr(poses), st, width_org, height_org, memkind))
+        else:
+            self._ck(lib().ofdis_fuse_track_weighted(self._h, n, _ptr(disp), disp_stride, _ptr(motions), _ptr(prev),
+                                                     self._fuse_cam(camera), ctypes.byref(params), _ptr(frames),
+                                                     frame_stride or 0, _ptr(weights), weight_stride, _ptr(poses), st,
+                                                     width_org, height_org, memkind))
         for k in range(n):
             stats[k] = (st[k].status, st[k].n_corr, st[k].rounds, st[k].cost0, st[k].cost)
         return poses[:n], stats[:n]

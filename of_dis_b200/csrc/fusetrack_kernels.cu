@@ -7,8 +7,10 @@
 //                      update and the stop and guard rules, and writes the pose the next launch reads.  The sums'
 //                      order is fixed by the cells, so the arrival order cannot change a bit.  A launch for a frame
 //                      that has stopped returns at once.
-// The push of an integrating call is the existing fuse_integrate_kernel with n = 1, reading its float32
-// world-to-camera pose from FuseTrack::g.  float32 and float64 without contraction, IEEE division and square root.
+// The push of an integrating call is the existing fuse_integrate_kernel with n = 1 (weighted for a weighted call),
+// reading its float32 world-to-camera pose from FuseTrack::g.  float32 and float64 without contraction, IEEE division and square root.
+#include <cfloat>
+
 #include <cuda_runtime.h>
 
 #include "ofdis_internal.cuh"
@@ -155,7 +157,12 @@ __device__ void ft_finish(const FuseTrack& t, int k, int r, const double (&M)[12
   }
 }
 
-__global__ void __launch_bounds__(FT_THREADS) fuse_track_kernel(FuseGeom g, FuseVolume v, FuseTrack t, int k, int r) {
+// WEIGHTED: ofdis_fuse_track_weighted -- a cell is valid only where its weight c = wk[py * w + px] is finite and > 0,
+// and its Huber
+// weight becomes wt * c.  The false instance is ofdis_fuse_track (wk unused, after the parameters it reads).
+template <bool WEIGHTED>
+__global__ void __launch_bounds__(FT_THREADS) fuse_track_kernel(FuseGeom g, FuseVolume v, FuseTrack t, int k, int r,
+                                                                 const float* wk) {
   __shared__ double terms[FT_WARPS][FTRACK_NE][FT_PAD];
   __shared__ double Ms[12];
   __shared__ float gs[12];
@@ -174,14 +181,23 @@ __global__ void __launch_bounds__(FT_THREADS) fuse_track_kernel(FuseGeom g, Fuse
   const int chunk = blockIdx.x * FT_WARPS + warp, c = chunk * 32 + lane;
   double (*tw)[FT_PAD] = terms[warp];
   float res = 0.0f, G[3], Pw[3];
-  const bool valid = c < t.cells && ft_cell(g, v, t, t.disp + (size_t)k * t.disp_stride, gs, c, res, G, Pw);
+  bool valid = c < t.cells && ft_cell(g, v, t, t.disp + (size_t)k * t.disp_stride, gs, c, res, G, Pw);
+  float cw = 1.0f;
+  if constexpr (WEIGHTED) {
+    if (valid) {
+      const int px = min((c % t.ncx) * t.s + t.s / 2, t.w - 1), py = min((c / t.ncx) * t.s + t.s / 2, t.h - 1);
+      cw = __ldg(wk + (size_t)py * t.w + px);
+      valid = cw > 0.0f && cw <= FLT_MAX;
+    }
+  }
   if (valid) {
     const double a[3] = {(double)G[0], (double)G[1], (double)G[2]};
     const double w0 = 2.0 * (double)Pw[0], w1 = 2.0 * (double)Pw[1], w2 = 2.0 * (double)Pw[2];
     const double J[6] = {(a[1] * -w2) + (a[2] * w1), (a[0] * w2) + (a[2] * -w0), (a[0] * -w1) + (a[1] * w0),
                          a[0], a[1], a[2]};
     const float ar = fabsf(res);
-    const double wt = (double)(ar <= t.huber ? 1.0f : t.huber / ar), rd = (double)res;
+    const float wf = ar <= t.huber ? 1.0f : t.huber / ar;
+    const double wt = (double)(WEIGHTED ? wf * cw : wf), rd = (double)res;
     int e = 0;
 #pragma unroll
     for (int i = 0; i < 6; ++i) {
@@ -236,9 +252,11 @@ __global__ void __launch_bounds__(FT_THREADS) fuse_track_kernel(FuseGeom g, Fuse
 
 }  // namespace
 
-int launch_fuse_track_eval(const FuseGeom& g, const FuseVolume& v, const FuseTrack& t, int k, int r, cudaStream_t st) {
+int launch_fuse_track_eval(const FuseGeom& g, const FuseVolume& v, const FuseTrack& t, int k, int r, cudaStream_t st,
+                           const float* wk) {
   const int blocks = (t.nchunks + FT_WARPS - 1) / FT_WARPS;
-  fuse_track_kernel<<<blocks, FT_THREADS, 0, st>>>(g, v, t, k, r);
+  if (wk) fuse_track_kernel<true><<<blocks, FT_THREADS, 0, st>>>(g, v, t, k, r, wk);
+  else fuse_track_kernel<false><<<blocks, FT_THREADS, 0, st>>>(g, v, t, k, r, wk);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

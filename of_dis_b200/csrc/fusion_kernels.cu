@@ -14,6 +14,8 @@
 //   fuse_cube_count_kernel triangles per scan block of FUSE_BLOCK cubes (cube = the voxel of its corner 0), scanned by
 //                          fuse_scan_kernel into a second offset array;
 //   fuse_face_kernel       the block's triangles again, written at their global index while it is below the capacity.
+#include <cfloat>
+
 #include <cuda_runtime.h>
 
 #include "ofdis_internal.cuh"
@@ -290,6 +292,9 @@ __constant__ unsigned char FUSE_MC[256][16] = {
     {0, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255, 255},
 };
 
+// WEIGHTED: ofdis_fuse_push_weighted -- frame f's observation at pixel o counts with c = p.weight[f * weight_stride
+// + o] in place of 1, and only when c is finite and > 0.  The false instance is ofdis_fuse_push.
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(FUSE_THREADS) fuse_integrate_kernel(FuseGeom g, FuseVolume v, FusePush p) {
   const long long a = (long long)blockIdx.x * FUSE_THREADS + threadIdx.x;
   if (a >= g.count) return;
@@ -315,6 +320,11 @@ __global__ void __launch_bounds__(FUSE_THREADS) fuse_integrate_kernel(FuseGeom g
     if (!(uu >= 0.0f && uu < (float)p.w && vv >= 0.0f && vv < (float)p.h)) continue;
     const int px = (int)floorf(uu), py = (int)floorf(vv);
     const size_t o = (size_t)py * p.w + px;
+    float cw = 1.0f;
+    if constexpr (WEIGHTED) {
+      cw = __ldg(p.weight + f * p.weight_stride + o);
+      if (!(cw > 0.0f && cw <= FLT_MAX)) continue;
+    }
     const float d = __ldg(p.disp + f * p.disp_stride + o);
     const float s = d + cam.doffs;
     if (!known_d(d) || !(s > 0.0f)) continue;
@@ -323,14 +333,14 @@ __global__ void __launch_bounds__(FUSE_THREADS) fuse_integrate_kernel(FuseGeom g
     const float sdf = z - Zc;
     if (sdf < -g.mu) continue;
     const float fv = fminf(1.0f, sdf / g.mu);
-    const float W1 = Wt + 1.0f;
-    T = (T * Wt + fv) / W1;
+    const float W1 = Wt + (WEIGHTED ? cw : 1.0f);
+    T = (T * Wt + (WEIGHTED ? fv * cw : fv)) / W1;
     if (v.C) {
       const unsigned char* I = p.frames + f * p.frame_stride + o * p.noc;
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) {
         const float obs = (float)__ldg(I + (p.noc == 3 ? ch : 0));
-        c[ch] = (unsigned char)floorf(((float)c[ch] * Wt + obs) / W1 + 0.5f);
+        c[ch] = (unsigned char)floorf(((float)c[ch] * Wt + (WEIGHTED ? obs * cw : obs)) / W1 + 0.5f);
       }
     }
     Wt = fminf(W1, g.max_weight);
@@ -618,7 +628,8 @@ __global__ void __launch_bounds__(32 * FUSE_RENDER_ROWS) fuse_render_kernel(Fuse
 
 int launch_fuse_push(const FuseGeom& g, const FuseVolume& v, const FusePush& p, cudaStream_t st) {
   const long long blocks = (g.count + FUSE_THREADS - 1) / FUSE_THREADS;
-  fuse_integrate_kernel<<<(unsigned)blocks, FUSE_THREADS, 0, st>>>(g, v, p);
+  if (p.weight) fuse_integrate_kernel<true><<<(unsigned)blocks, FUSE_THREADS, 0, st>>>(g, v, p);
+  else fuse_integrate_kernel<false><<<(unsigned)blocks, FUSE_THREADS, 0, st>>>(g, v, p);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

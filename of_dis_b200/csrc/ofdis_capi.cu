@@ -1032,6 +1032,53 @@ int ofdis_consistency_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, unsigned c
   return OFDIS_OK;
 }
 
+int ofdis_confidence_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_conf_params* p,
+                             const unsigned char* frames0, const unsigned char* frames1, size_t frame_stride,
+                             float* conf, float* terms, int width_org, int height_org, int memkind) {
+  if (!ctx) return OFDIS_ERR_ARG;
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  const int side = p ? 2 * p->radius + 1 : 0;
+  if (f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || (b0 >= 0 && b0 > ctx->max_frames - (f1 - f0)) || !p ||
+      p->radius < 1 || p->radius > OFDIS_CONF_MAX_RADIUS || !(p->s_fb > 0.f && p->s_fb <= FLT_MAX) ||
+      !(p->s_tex > 0.f && p->s_tex <= FLT_MAX) || p->min_count < 1 || p->min_count > side * side || !frames0 ||
+      !frames1 || (!conf && !terms) ||
+      (dev && (reinterpret_cast<uintptr_t>(conf) % sizeof(float) || reinterpret_cast<uintptr_t>(terms) % sizeof(float))))
+    return fail(ctx, OFDIS_ERR_ARG, "confidence_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  const size_t pix = (size_t)width_org * height_org, hwc = pix * ctx->prm.noc;
+  if (frame_stride < hwc) return fail(ctx, OFDIS_ERR_ARG, "confidence_fullres: frame_stride below one frame");
+  NvtxRange nvtx("confidence", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0, D = ctx->dirs;
+  ConfArgs a{frames0, frames1, frame_stride, conf, terms, width_org, height_org, cx, cy, p->radius, p->min_count,
+             p->s_fb, p->s_tex};
+  if (!dev) {
+    // both frames of every pair into the staging buffer (2 x max_frames images), conf then terms through the
+    // full-resolution scratch, sized for max_frames and at least what ofdis_get_flow_fullres asks for
+    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    rc = ensure_full(ctx, pix * std::max(ctx->nop, 4) * (size_t)ctx->max_frames);
+    if (rc) return rc;
+    unsigned char* st = static_cast<unsigned char*>(ctx->d_stage);
+    CK(cudaMemcpy2DAsync(st, hwc, frames0, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(st + hwc * n, hwc, frames1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    a.i0 = st, a.i1 = st + hwc * n, a.stride = hwc;
+    a.conf = conf ? ctx->d_full : nullptr;
+    a.terms = terms ? ctx->d_full + pix * n : nullptr;
+  }
+  if (launch_confidence(stepped(ctx->lev[0], D), f0 * D, b0 >= 0 ? b0 * D : -1, n, ctx->prm.noc, a, ctx->stream) < 0)
+    return fail(ctx, OFDIS_ERR_CUDA, "confidence_kernel launch", cudaGetLastError());
+  ctx->launches += 1;
+  if (!dev) {
+    if (conf) CK(cudaMemcpyAsync(conf, a.conf, sizeof(float) * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (terms) CK(cudaMemcpyAsync(terms, a.terms, sizeof(float) * 3 * pix * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  return OFDIS_OK;
+}
+
 // The workspace of ofdis_interpolate_fullres for max_frames pairs of the context's size (InterpWork), allocated on
 // the first call: per pixel and pair the keys (8 bytes), u_t (4 nop), the fill stamps (4), two hole lists (4 + 4) and
 // the two consistency masks (1 + 1); then one word per pair and width + height round counts.
@@ -1532,17 +1579,21 @@ int ofdis_fuse_begin(ofdis_ctx* ctx, const ofdis_fuse_params* p) {
   return OFDIS_OK;
 }
 
-int ofdis_fuse_push(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* poses,
-                    const ofdis_stereo_camera* cam, float max_depth, const unsigned char* frames, size_t frame_stride,
-                    int width_org, int height_org, int memkind) {
+// ofdis_fuse_push (weighted false) and ofdis_fuse_push_weighted
+static int fuse_push_impl(ofdis_ctx* ctx, bool weighted, int n, const float* disp, size_t disp_stride,
+                          const double* poses, const ofdis_stereo_camera* cam, float max_depth,
+                          const unsigned char* frames, size_t frame_stride, const float* weight, size_t weight_stride,
+                          int width_org, int height_org, int memkind) {
   if (!ctx) return OFDIS_ERR_ARG;
-  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_push: no live volume (ofdis_fuse_begin)");
+  const char* name = weighted ? "fuse_push_weighted" : "fuse_push";
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, (std::string(name) + ": no live volume (ofdis_fuse_begin)").c_str());
   const bool dev = memkind == OFDIS_MEM_DEVICE, color = ctx->fuse_vol.C != nullptr;
   const size_t pix = (size_t)std::max(width_org, 0) * std::max(height_org, 0), hwc = pix * ctx->prm.noc;
   if (n < 1 || n > ctx->max_frames + 1 || !disp || !poses || (color && !frames) || !fuse_cam_ok(cam) ||
       !(max_depth > 0.0f) || disp_stride < pix || (color && frame_stride < hwc) ||
-      (dev && reinterpret_cast<uintptr_t>(disp) % sizeof(float)))
-    return fail(ctx, OFDIS_ERR_ARG, "fuse_push: bad argument");
+      (dev && reinterpret_cast<uintptr_t>(disp) % sizeof(float)) ||
+      (weighted && (!weight || weight_stride < pix || (dev && reinterpret_cast<uintptr_t>(weight) % sizeof(float)))))
+    return fail(ctx, OFDIS_ERR_ARG, (std::string(name) + ": bad argument").c_str());
   int cx, cy;
   int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
   if (rc) return rc;
@@ -1554,12 +1605,15 @@ int ofdis_fuse_push(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride
   fp.n = n, fp.w = width_org, fp.h = height_org, fp.noc = ctx->prm.noc, fp.max_depth = max_depth;
   fp.cam = DispCamera{cam->fx * cam->baseline, cam->fx, cam->fy, cam->cx, cam->cy, cam->doffs};
   fp.g = ctx->fuse_ws.g;
+  fp.weight = weighted ? weight : nullptr, fp.weight_stride = weight_stride;
   rc = fuse_poses(ctx, n, poses, true);
   if (rc) return rc;
   if (!dev) {
-    // the staging buffer: the disparity maps, then the frames, packed; sized for max_frames + 1 of each
+    // the staging buffer: the disparity maps, then the frames, then the weights, packed; sized for max_frames + 1 of
+    // each
     const size_t b_d = align16(sizeof(float) * pix * (size_t)(ctx->max_frames + 1));
-    rc = ensure_stage(ctx, b_d + (color ? hwc * (size_t)(ctx->max_frames + 1) : 0));
+    const size_t b_f = color ? align16(hwc * (size_t)(ctx->max_frames + 1)) : 0;
+    rc = ensure_stage(ctx, b_d + b_f + (weighted ? b_d : 0));
     if (rc) return rc;
     char* st = static_cast<char*>(ctx->d_stage);
     CK(cudaMemcpy2DAsync(st, sizeof(float) * pix, disp, sizeof(float) * disp_stride, sizeof(float) * pix, n,
@@ -1569,11 +1623,31 @@ int ofdis_fuse_push(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride
       CK(cudaMemcpy2DAsync(st + b_d, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
       fp.frames = reinterpret_cast<const unsigned char*>(st + b_d), fp.frame_stride = hwc;
     }
+    if (weighted) {
+      CK(cudaMemcpy2DAsync(st + b_d + b_f, sizeof(float) * pix, weight, sizeof(float) * weight_stride,
+                           sizeof(float) * pix, n, cudaMemcpyHostToDevice, ctx->stream));
+      fp.weight = reinterpret_cast<const float*>(st + b_d + b_f), fp.weight_stride = pix;
+    }
   }
   const int k = launch_fuse_push(ctx->fuse_geom, ctx->fuse_vol, fp, ctx->stream);
   if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_integrate_kernel launch", cudaGetLastError());
   ctx->launches += k;
   return OFDIS_OK;
+}
+
+int ofdis_fuse_push(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* poses,
+                    const ofdis_stereo_camera* cam, float max_depth, const unsigned char* frames, size_t frame_stride,
+                    int width_org, int height_org, int memkind) {
+  return fuse_push_impl(ctx, false, n, disp, disp_stride, poses, cam, max_depth, frames, frame_stride, nullptr, 0,
+                        width_org, height_org, memkind);
+}
+
+int ofdis_fuse_push_weighted(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* poses,
+                             const ofdis_stereo_camera* cam, float max_depth, const unsigned char* frames,
+                             size_t frame_stride, const float* weight, size_t weight_stride, int width_org,
+                             int height_org, int memkind) {
+  return fuse_push_impl(ctx, true, n, disp, disp_stride, poses, cam, max_depth, frames, frame_stride, weight,
+                        weight_stride, width_org, height_org, memkind);
 }
 
 int ofdis_fuse_extract(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, long capacity, long* count,
@@ -1766,17 +1840,22 @@ int ofdis_fuse_set_volume(ofdis_ctx* ctx, const float* T, const float* W, const 
 
 static bool finite_f64(double v) { return std::fabs(v) <= DBL_MAX; }
 
-int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* motions,
-                     const double* prev, const ofdis_stereo_camera* cam, const ofdis_fuse_track_params* p,
-                     const unsigned char* frames, size_t frame_stride, double* poses, ofdis_fuse_track_stats* stats,
-                     int width_org, int height_org, int memkind) {
+// ofdis_fuse_track (weighted false) and ofdis_fuse_track_weighted
+static int fuse_track_impl(ofdis_ctx* ctx, bool weighted, int n, const float* disp, size_t disp_stride,
+                           const double* motions, const double* prev, const ofdis_stereo_camera* cam,
+                           const ofdis_fuse_track_params* p, const unsigned char* frames, size_t frame_stride,
+                           const float* weight, size_t weight_stride, double* poses, ofdis_fuse_track_stats* stats,
+                           int width_org, int height_org, int memkind) {
   static_assert(sizeof(ofdis_fuse_track_stats) == 32, "ofdis_fuse_track_stats: 32 bytes, as FUSE_TRACK_STATS_DTYPE");
   if (!ctx) return OFDIS_ERR_ARG;
-  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, "fuse_track: no live volume (ofdis_fuse_begin)");
+  const char* name = weighted ? "fuse_track_weighted" : "fuse_track";
+  if (!ctx->fuse_on) return fail(ctx, OFDIS_ERR_ARG, (std::string(name) + ": no live volume (ofdis_fuse_begin)").c_str());
   const bool dev = memkind == OFDIS_MEM_DEVICE, color = ctx->fuse_vol.C != nullptr;
   const size_t pix = (size_t)std::max(width_org, 0) * std::max(height_org, 0), hwc = pix * ctx->prm.noc;
   bool ok = n >= 1 && n <= ctx->max_frames + 1 && disp && prev && poses && stats && fuse_cam_ok(cam) && p &&
             disp_stride >= pix && !(dev && reinterpret_cast<uintptr_t>(disp) % sizeof(float));
+  ok = ok && (!weighted || (weight && weight_stride >= pix &&
+                            !(dev && reinterpret_cast<uintptr_t>(weight) % sizeof(float))));
   ok = ok && p->step >= 1 && p->rounds >= 0 && p->rounds <= 32 && !std::isnan(p->min_weight) &&
        p->max_depth > 0.0f && finite_gt0(p->huber) && finite_f64(p->damping) && p->damping >= 0.0 &&
        p->min_corr >= 6 && finite_f64(p->max_shift) && p->max_shift > 0.0 && p->min_cos >= -1.0 && p->min_cos <= 1.0 &&
@@ -1785,7 +1864,7 @@ int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_strid
   ok = ok && (!use_frames || (frames && frame_stride >= hwc));
   for (int i = 0; ok && i < 12; ++i) ok = finite_f64(prev[i]);
   for (size_t i = 0; ok && motions && i < (size_t)12 * n; ++i) ok = finite_f64(motions[i]);
-  if (!ok) return fail(ctx, OFDIS_ERR_ARG, "fuse_track: bad argument");
+  if (!ok) return fail(ctx, OFDIS_ERR_ARG, (std::string(name) + ": bad argument").c_str());
   int cx, cy;
   int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
   if (rc) return rc;
@@ -1826,10 +1905,13 @@ int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_strid
   t.disp = disp, t.disp_stride = disp_stride;
   const unsigned char* fr = use_frames ? frames : nullptr;
   size_t fstride = frame_stride;
+  const float* wt = weighted ? weight : nullptr;
+  size_t wstride = weight_stride;
   if (!dev) {
-    // the staging buffer: the disparity maps, then the frames, packed; sized for max_frames + 1 of each, as the push
-    const size_t b_d = align16(sizeof(float) * pix * F);
-    rc = ensure_stage(ctx, b_d + (color ? hwc * F : 0));
+    // the staging buffer: the disparity maps, then the frames, then the weights, packed; sized for max_frames + 1 of
+    // each, as the push
+    const size_t b_d = align16(sizeof(float) * pix * F), b_f = color ? align16(hwc * F) : 0;
+    rc = ensure_stage(ctx, b_d + b_f + (weighted ? b_d : 0));
     if (rc) return rc;
     char* st = static_cast<char*>(ctx->d_stage);
     CK(cudaMemcpy2DAsync(st, sizeof(float) * pix, disp, sizeof(float) * disp_stride, sizeof(float) * pix, n,
@@ -1838,6 +1920,11 @@ int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_strid
     if (use_frames) {
       CK(cudaMemcpy2DAsync(st + b_d, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
       fr = reinterpret_cast<const unsigned char*>(st + b_d), fstride = hwc;
+    }
+    if (weighted) {
+      CK(cudaMemcpy2DAsync(st + b_d + b_f, sizeof(float) * pix, weight, sizeof(float) * weight_stride,
+                           sizeof(float) * pix, n, cudaMemcpyHostToDevice, ctx->stream));
+      wt = reinterpret_cast<const float*>(st + b_d + b_f), wstride = pix;
     }
   }
   FuseTrackState init{};
@@ -1853,13 +1940,15 @@ int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_strid
   fp.cam = t.cam;
   for (int k = 0; k < n; ++k) {
     for (int r = 0; r <= p->rounds; ++r) {
-      const int kk = launch_fuse_track_eval(ctx->fuse_geom, ctx->fuse_vol, t, k, r, ctx->stream);
+      const int kk = launch_fuse_track_eval(ctx->fuse_geom, ctx->fuse_vol, t, k, r, ctx->stream,
+                                            wt ? wt + (size_t)k * wstride : nullptr);
       if (kk < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_track_kernel launch", cudaGetLastError());
       ctx->launches += kk;
     }
     if (!p->integrate) continue;
     fp.disp = t.disp + (size_t)k * t.disp_stride, fp.disp_stride = t.disp_stride;
     fp.frames = fr ? fr + (size_t)k * fstride : nullptr, fp.frame_stride = fstride;
+    fp.weight = wt ? wt + (size_t)k * wstride : nullptr, fp.weight_stride = wstride;
     const int kk = launch_fuse_push(ctx->fuse_geom, ctx->fuse_vol, fp, ctx->stream);
     if (kk < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_integrate_kernel launch", cudaGetLastError());
     ctx->launches += kk;
@@ -1872,6 +1961,23 @@ int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_strid
   std::memcpy(poses, P.data(), sizeof(double) * P.size());
   std::memcpy(stats, S.data(), sizeof(ofdis_fuse_track_stats) * n);
   return OFDIS_OK;
+}
+
+int ofdis_fuse_track(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* motions,
+                     const double* prev, const ofdis_stereo_camera* cam, const ofdis_fuse_track_params* p,
+                     const unsigned char* frames, size_t frame_stride, double* poses, ofdis_fuse_track_stats* stats,
+                     int width_org, int height_org, int memkind) {
+  return fuse_track_impl(ctx, false, n, disp, disp_stride, motions, prev, cam, p, frames, frame_stride, nullptr, 0,
+                         poses, stats, width_org, height_org, memkind);
+}
+
+int ofdis_fuse_track_weighted(ofdis_ctx* ctx, int n, const float* disp, size_t disp_stride, const double* motions,
+                              const double* prev, const ofdis_stereo_camera* cam, const ofdis_fuse_track_params* p,
+                              const unsigned char* frames, size_t frame_stride, const float* weight,
+                              size_t weight_stride, double* poses, ofdis_fuse_track_stats* stats, int width_org,
+                              int height_org, int memkind) {
+  return fuse_track_impl(ctx, true, n, disp, disp_stride, motions, prev, cam, p, frames, frame_stride, weight,
+                         weight_stride, poses, stats, width_org, height_org, memkind);
 }
 
 // The tracker's workspace for geometry t: the state, two track lists, the flags, the occupancy, the scan blocks'

@@ -588,6 +588,13 @@ int main(int argc, char** argv) {
 // with the scale M, so that the frames of a clip compare.  3 bytes per pixel come back for it.  The other output files
 // keep their bytes.
 //
+// --confidence R (1 <= R <= 7): every pair also gets <stem>_conf.pfm, the forward slot's per-pixel confidence
+// (ofdis_confidence_fullres with radius R, s_fb 1, s_tex 100 and min_count (2R+1)^2 / 2, integer division) as float32
+// in [0, 1], stored as is (read_pfm returns it negated, as it returns every PFM of this front-end).  The forward-backward
+// term is used when the backward slots already run (--bidirectional, --lr-check, --interpolate or --tracks); no flag
+// adds them.  With verbosity > 0 every batch prints `CONF pairs N mean M`, M the float64 mean over the batch's pixels
+// (%.9g).  Not with --warm-start; every other output keeps its bytes.
+//
 // --interpolate T (0 < T < 1): every pair also gets <stem>_interp.png, the frame at time T between image1 and image2
 // synthesised on the device from the pair's forward and backward flows (ofdis_interpolate_fullres, with the
 // consistency thresholds of --bidirectional): 8-bit gray from the *_INT binaries, 8-bit RGB from the *_RGB binaries
@@ -1180,6 +1187,7 @@ struct Options {
   const char* odo_dir = nullptr;                      // --odometry DIR
   const char* odo_gtlist = nullptr;                   // --gt-poses LIST
   const char* fuse = nullptr;                         // --fuse voxel,trunc,x0,y0,z0,nx,ny,nz
+  const char* conf_arg = nullptr;                     // --confidence R
   int nnum = 0;                                       // the operating point or the 20 parameters after the flags
   char** nums = nullptr;
 
@@ -1199,6 +1207,7 @@ struct Options {
   vector<double> stab_wts;
   ofdis_disp_filter dfilt{};
   ofdis_stereo_camera dcam{};
+  ofdis_conf_params cp{};
 };
 
 // The flags, read from argv[2] on until the first word that is none of them.  An argument-taking flag without its
@@ -1236,6 +1245,7 @@ static int parse_flags(int argc, char** argv, Options& o) {
       {"--mesh", 0, nullptr, &o.mesh, nullptr},
       {"--gt-poses", 1, &o.odo_gtlist, nullptr, "one list of KITTI poses files"},
       {"--gt", 1, &o.gtlist, nullptr, "one ground-truth list file"},
+      {"--confidence", 1, &o.conf_arg, nullptr, "one window radius"},
   };
   int i = 2;
   while (i < argc) {
@@ -1360,6 +1370,15 @@ static int read_interpolate(Options& o) {
   return 0;
 }
 
+static int read_confidence(Options& o) {
+  char* end = nullptr;
+  const long r = strtol(o.conf_arg, &end, 10);
+  if (end == o.conf_arg || *end || r < 1 || r > 7) return refuse(2, "--confidence takes a radius 1..7, got %s", o.conf_arg);
+  const int side = 2 * (int)r + 1;
+  o.cp = ofdis_conf_params{(int)r, 1.0f, 100.0f, side * side / 2};
+  return 0;
+}
+
 static int read_color_max(Options& o) {
   char* end = nullptr;
   o.color_max = strtof(o.color_max_arg, &end);
@@ -1423,6 +1442,7 @@ static int check_options(Options& o) {
       {o.interp_arg != nullptr, "--interpolate", kAny, nullptr, false, true, nullptr, read_interpolate},
       {o.color_max_arg != nullptr, "--color-max", kAny, nullptr, false, o.color, "--color-max needs --color",
        read_color_max},
+      {o.conf_arg != nullptr, "--confidence", kAny, nullptr, true, true, nullptr, read_confidence},
   };
   for (const Rule& r : rules) {
     if (!r.given) continue;
@@ -1631,6 +1651,7 @@ struct Batch {
   vector<float> gm_res;
   vector<float> sf_d0, sf_d1, sf_w, sf_m;  // --scene-flow: the disparities of image1 and image2, outputs
   vector<double> odo_pose;                 // --odometry: the relative poses
+  vector<float> conf;                      // --confidence: the forward slots' confidence maps
 };
 
 // The run's state across batches: the context and what clips and the end-of-run summary carry over
@@ -1826,6 +1847,13 @@ static int run_interpolate(State& s, Batch& b) {
   return ofdis_interpolate_fullres(s.ctx.get(), 0, b.n, b.n, b.frames.data(), b.frames.data() + b.hwc, b.fs,
                                    s.o.interp_t, s.nop == 2 ? 0.01f : 0.0f, s.nop == 2 ? 0.5f : 1.0f, b.interp.data(),
                                    nullptr, b.w, b.h, OFDIS_MEM_HOST);
+}
+
+// --confidence: the forward slots' maps, with the forward-backward term when the backward slots run
+static int run_confidence(State& s, Batch& b) {
+  b.conf.resize((size_t)b.n * b.w * b.h);
+  return ofdis_confidence_fullres(s.ctx.get(), 0, b.n, s.o.two_way ? b.n : -1, &s.o.cp, b.frames.data(),
+                                  b.frames.data() + b.hwc, b.fs, b.conf.data(), nullptr, b.w, b.h, OFDIS_MEM_HOST);
 }
 
 static int run_global_motion(State& s, Batch& b) {
@@ -2225,6 +2253,7 @@ static int run_stages(State& s, Batch& b) {
   const Options& o = s.o;
   int rc = run_flows(s, b);
   if (rc == OFDIS_OK && o.interp_arg) rc = run_interpolate(s, b);
+  if (rc == OFDIS_OK && o.conf_arg) rc = run_confidence(s, b);
   if (rc == OFDIS_OK && o.gm_model) rc = run_global_motion(s, b);
   if (rc == OFDIS_OK && o.disp_on) rc = run_disparity(s, b);
   if (rc == OFDIS_OK && o.tracks) rc = run_tracks(s, b);
@@ -2341,6 +2370,13 @@ static void write_outputs(State& s, const Batch& b) {
              with_suffix(s.jobs[b.j0 + k].out, "_interp", ".png").c_str());
   if (o.gm_model) write_global_motion(s, b);
   if (o.disp_on) write_disparities(s, b);
+  if (o.conf_arg) {
+    double sum = 0.0;
+    for (int k = 0; k < b.n; ++k)
+      save_pfm1(b.conf.data() + (size_t)k * w * h, w, h, with_suffix(s.jobs[b.j0 + k].out, "_conf", ".pfm"));
+    for (const float c : b.conf) sum += c;
+    if (s.verbosity > 0) printf("CONF pairs %d mean %.9g\n", b.n, sum / (double)b.conf.size());
+  }
   if (!o.kitti) write_flows(s, b);
 }
 

@@ -824,6 +824,71 @@ def track_seed_eigen(frame: np.ndarray, spacing: int):
     return cx, cy, lam
 
 
+# ---- per-pixel confidence (ofdis_confidence_fullres) -----------------------------------------------------------
+CONF_PARAM_FIELDS = ("radius", "s_fb", "s_tex", "min_count")
+_QNAN32 = np.uint32(0x7FC00000).view(np.float32)
+
+
+def confidence(frame0: np.ndarray, frame1: np.ndarray, F: np.ndarray, B: np.ndarray | None, params):
+    """Restates ofdis_confidence_fullres for one pair: frame0, frame1 (H, W[, 3]) uint8, F and its partner B (H, W, nop)
+    or (H, W) float32 full-resolution flows (B None: no forward-backward term), params a mapping with
+    CONF_PARAM_FIELDS.  Returns (conf (H, W), terms (H, W, 3): z, e, lambda), float32, in the header's order."""
+    r, min_count = int(params["radius"]), int(params["min_count"])
+    s_fb, s_tex = f32(params["s_fb"]), f32(params["s_tex"])
+    g0, g1 = _brightness(np.asarray(frame0, np.uint8)), _brightness(np.asarray(frame1, np.uint8))
+    H, W = g0.shape
+    Fa = np.asarray(F, f32).reshape(H, W, -1)
+    xs_, ys_ = np.arange(W), np.arange(H)
+    Ix = (g0[:, np.minimum(xs_ + 1, W - 1)] - g0[:, np.maximum(xs_ - 1, 0)]) * f32(0.5)
+    Iy = (g0[np.minimum(ys_ + 1, H - 1), :] - g0[np.maximum(ys_ - 1, 0), :]) * f32(0.5)
+    with np.errstate(invalid="ignore", over="ignore"):
+        xs = np.arange(W, dtype=f32)[None, :] + Fa[..., 0]
+        ys = np.arange(H, dtype=f32)[:, None] + (Fa[..., 1] if Fa.shape[2] == 2 else f32(0))
+        inside = (xs >= 0) & (xs <= f32(W - 1)) & (ys >= 0) & (ys <= f32(H - 1))
+        Iw = _bilinear_frame(g1[..., None], np.where(inside, xs, f32(0)), np.where(inside, ys, f32(0)))[..., 0]
+    Iw = np.where(inside, Iw, _QNAN32).astype(f32)
+    win = [(np.clip(ys_ + dy, 0, H - 1)[:, None], np.clip(xs_ + dx, 0, W - 1)[None, :])
+           for dy in range(-r, r + 1) for dx in range(-r, r + 1)]
+    zero = np.zeros((H, W), f32)
+    n = np.zeros((H, W), np.int64)
+    s0, s1, a, b, c = zero.copy(), zero.copy(), zero.copy(), zero.copy(), zero.copy()
+    for q in win:
+        v = inside[q]
+        n += v
+        s0 = s0 + np.where(v, g0[q], f32(0))  # adding +0.0 to these sums leaves them as they are
+        s1 = s1 + np.where(v, Iw[q], f32(0))
+        ix, iy = Ix[q], Iy[q]
+        a = a + ix * ix
+        b = b + ix * iy
+        c = c + iy * iy
+    d = a - c
+    lam = (a + c) * f32(0.5) - np.sqrt(d * d * f32(0.25) + b * b)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        nf = n.astype(f32)
+        m0, m1 = s0 / nf, s1 / nf
+        c00, c11, c01 = zero.copy(), zero.copy(), zero.copy()
+        for q in win:
+            v = inside[q]
+            p0, p1 = g0[q] - m0, Iw[q] - m1
+            c00 = c00 + np.where(v, p0 * p0, f32(0))
+            c11 = c11 + np.where(v, p1 * p1, f32(0))
+            c01 = c01 + np.where(v, p0 * p1, f32(0))
+        den = c00 * c11
+        z = np.where((n >= min_count) & (den > 0), c01 / np.sqrt(den), _QNAN32).astype(f32)
+    if B is None:
+        e = np.full((H, W), _QNAN32, f32)
+        ce = np.ones((H, W), f32)
+    else:
+        e = consistency_check(Fa, np.asarray(B, f32).reshape(H, W, -1), 0.0, 0.0)[1]
+        with np.errstate(invalid="ignore", over="ignore"):
+            ce = np.where(e >= 0, s_fb / (s_fb + e), f32(0)).astype(f32)
+    with np.errstate(invalid="ignore"):
+        cz = np.where(z > 0, z, f32(0)).astype(f32)
+        cl = np.where(lam > 0, lam / (lam + s_tex), f32(0)).astype(f32)
+    conf = ((cz * ce) * cl).astype(f32)
+    return conf, np.stack([z, e, lam.astype(f32)], -1)
+
+
 def _track_seed(frame, tracks, next_id, stats, p):
     s = int(p["spacing"])
     h, w = frame.shape[:2]
@@ -1768,9 +1833,11 @@ def _fuse_axes(params):
             for e, k in enumerate(("nx", "ny", "nz"))]
 
 
-def fuse_integrate(vol: dict, params, disp, poses, camera, max_depth=np.inf, frames=None) -> dict:
+def fuse_integrate(vol: dict, params, disp, poses, camera, max_depth=np.inf, frames=None, weights=None) -> dict:
     """Restates ofdis_fuse_push on vol (fuse_new_volume's dict), in place: disp (n, H, W) float32 positive disparities
-    (NaN unknown), poses (n, 3, 4) camera-to-world float64, frames (n, H, W[, 3]) uint8 when the volume keeps colour."""
+    (NaN unknown), poses (n, 3, 4) camera-to-world float64, frames (n, H, W[, 3]) uint8 when the volume keeps colour.
+    With weights (n, H, W) float32 it restates ofdis_fuse_push_weighted: an observation counts with its pixel's weight
+    c in place of 1, and only where 0 < c <= FLT_MAX."""
     disp = np.asarray(disp, f32).reshape((-1,) + np.shape(disp)[-2:])
     n, H, W = disp.shape
     poses = np.asarray(poses, np.float64).reshape(n, 12)
@@ -1802,12 +1869,21 @@ def fuse_integrate(vol: dict, params, disp, poses, camera, max_depth=np.inf, fra
             sdf = z - Zc
             ok &= ~(sdf < -mu)
             f = np.minimum(one, sdf / mu)
-        W1 = Wt + one
-        Tn = (T * Wt + f) / W1
+            if weights is None:
+                c, fc = one, f
+            else:
+                c = np.asarray(weights[k], f32).reshape(H, W)[py, px]
+                ok &= (c > 0) & (c <= np.finfo(f32).max)
+                fc = f * c
+        with np.errstate(all="ignore"):  # where a weight skips, W1 may be 0 or NaN
+            W1 = Wt + c
+            Tn = (T * Wt + fc) / W1
         if C is not None:
             fr = np.asarray(frames[k], np.uint8).reshape(H, W, -1)
             obs = fr[py, px] if fr.shape[-1] == 3 else np.repeat(fr[py, px], 3, -1)
-            cn = np.floor((C.astype(f32) * Wt[..., None] + obs.astype(f32)) / W1[..., None] + half)
+            with np.errstate(all="ignore"):
+                obs = obs.astype(f32) if weights is None else obs.astype(f32) * c[..., None]
+                cn = np.floor((C.astype(f32) * Wt[..., None] + obs) / W1[..., None] + half)
             C[ok] = cn[ok].astype(np.uint8)
         T[ok] = Tn[ok]
         Wt[ok] = np.fmin(W1, maxw)[ok]  # fminf: a NaN W becomes max_weight
@@ -2160,14 +2236,16 @@ def fuse_track_cells(vol: dict, params, D: np.ndarray, cam: dict, step: int, min
     return ok, r.astype(f32), np.stack([G0, G1, G2], -1).astype(f32), np.stack(Pw, -1).astype(f32)
 
 
-def fuse_track_terms(r, G, Pw, huber) -> np.ndarray:
-    """The 28 float64 terms of cells (m, 28): N (21, upper triangle row-major), b (6) and the cost, step 2's order."""
+def fuse_track_terms(r, G, Pw, huber, c=None) -> np.ndarray:
+    """The 28 float64 terms of cells (m, 28): N (21, upper triangle row-major), b (6) and the cost, step 2's order.
+    c (m,) float32: the cells' weights of ofdis_fuse_track_weighted, which multiply the Huber weight in float32."""
     a = [G[:, e].astype(np.float64) for e in range(3)]
     w0, w1, w2 = (2.0 * Pw[:, e].astype(np.float64) for e in range(3))
     J = [(a[1] * -w2) + (a[2] * w1), (a[0] * w2) + (a[2] * -w0), (a[0] * -w1) + (a[1] * w0), a[0], a[1], a[2]]
     ar = np.abs(r)
     with np.errstate(all="ignore"):
-        wt = np.where(ar <= f32(huber), f32(1), f32(huber) / ar).astype(np.float64)
+        wt = np.where(ar <= f32(huber), f32(1), f32(huber) / ar).astype(f32)
+        wt = (wt if c is None else wt * np.asarray(c, f32)).astype(np.float64)
     rd = r.astype(np.float64)
     terms = [(wt * J[i]) * J[j] for i in range(6) for j in range(i, 6)]
     terms += [-((wt * J[i]) * rd) for i in range(6)]
@@ -2175,11 +2253,21 @@ def fuse_track_terms(r, G, Pw, huber) -> np.ndarray:
     return np.stack(terms, -1)
 
 
-def fuse_track_eval(vol: dict, params, D, cam: dict, p: dict, M):
-    """One evaluation of ofdis_fuse_track: (N (6, 6) mirrored, b (6,), cost, n_corr) at the pose M."""
+def fuse_track_eval(vol: dict, params, D, cam: dict, p: dict, M, weight=None):
+    """One evaluation of ofdis_fuse_track: (N (6, 6) mirrored, b (6,), cost, n_corr) at the pose M; with weight (H, W)
+    float32, of ofdis_fuse_track_weighted."""
     ok, r, G, Pw = fuse_track_cells(vol, params, D, cam, p["step"], p["min_weight"], p["max_depth"], M)
+    c = None
+    if weight is not None:
+        H, W = D.shape
+        s = int(p["step"])
+        ncx, ncy = (W - 1) // s + 1, (H - 1) // s + 1
+        cell = np.arange(ncx * ncy)
+        c = np.asarray(weight, f32).reshape(H, W)[np.minimum((cell // ncx) * s + s // 2, H - 1),
+                                                  np.minimum((cell % ncx) * s + s // 2, W - 1)]
+        ok = ok & (c > 0) & (c <= np.finfo(f32).max)
     with np.errstate(all="ignore"):
-        T = np.where(ok[:, None], fuse_track_terms(r, G, Pw, p["huber"]), 0.0)
+        T = np.where(ok[:, None], fuse_track_terms(r, G, Pw, p["huber"], c), 0.0)
     v = _chunk_tree(T)
     A = np.zeros((6, 6))
     e = 0
@@ -2203,10 +2291,11 @@ def fuse_track_params(params) -> dict:
     return {k: params[k] for k in FUSE_TRACK_PARAM_FIELDS}
 
 
-def fuse_track(vol: dict, fuse_params, track_params, disp, motions, prev, camera, frames=None):
+def fuse_track(vol: dict, fuse_params, track_params, disp, motions, prev, camera, frames=None, weights=None):
     """Restates ofdis_fuse_track: disp (n, H, W) float32, motions (n, 3, 4) float64 or None (the identity), prev (3, 4)
     camera-to-world, frames (n, H, W[, 3]) uint8 when integrating into a volume with colour.  With integrate, vol is
-    updated in place by fuse_integrate.  Returns (poses (n, 3, 4) float64, stats (n,) FUSE_TRACK_STATS_DTYPE)."""
+    updated in place by fuse_integrate.  With weights (n, H, W) float32 it restates ofdis_fuse_track_weighted.
+    Returns (poses (n, 3, 4) float64, stats (n,) FUSE_TRACK_STATS_DTYPE)."""
     p = fuse_track_params(track_params)
     cam = _ego_cam(camera)
     disp = np.asarray(disp, f32).reshape((-1,) + np.shape(disp)[-2:])
@@ -2219,7 +2308,8 @@ def fuse_track(vol: dict, fuse_params, track_params, disp, motions, prev, camera
         pred = fuse_track_predict(P, None if mot is None else mot[k])
         M, applied, status = pred, 0, 0
         for r in range(int(p["rounds"]) + 1):
-            A, b, cost, cnt = fuse_track_eval(vol, fuse_params, disp[k], cam, p, M)
+            A, b, cost, cnt = fuse_track_eval(vol, fuse_params, disp[k], cam, p, M,
+                                              None if weights is None else weights[k])
             if r == 0:
                 cost0 = cost
             if cnt < int(p["min_corr"]):
@@ -2240,7 +2330,8 @@ def fuse_track(vol: dict, fuse_params, track_params, disp, motions, prev, camera
         stats[k] = (status, cnt, applied, cost0, cost)
         if p["integrate"]:
             fuse_integrate(vol, fuse_params, disp[k:k + 1], F.reshape(1, 3, 4), camera, p["max_depth"],
-                           None if vol["C"] is None else np.asarray(frames)[k:k + 1])
+                           None if vol["C"] is None else np.asarray(frames)[k:k + 1],
+                           None if weights is None else np.asarray(weights)[k:k + 1])
         P = F
     return poses.reshape(n, 3, 4), stats
 

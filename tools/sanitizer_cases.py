@@ -10,8 +10,9 @@ the bulk-copied score tiles with and without refills, refits, per-pixel outputs)
 stages on 32-byte correspondences, non-finite disparities, score tile refills), a Fisher encoding (projection,
 posteriors, float64 statistics, the take) and a TSDF fusion (integration, crossing count, scan and write, ray casting)
 and its marching cubes (set_volume, the write with vertex bases, cube count, scan, faces) and a camera tracking
-against it (the evaluation kernel's chunk sums, arrival counter and tree, with and without the push) checked against
-their restatements.  Results are checked against the
+against it (the evaluation kernel's chunk sums, arrival counter and tree, with and without the push), the same
+tracking and push weighted by per-pixel weights with special values, and a per-pixel confidence (the halo-staged tile
+and its window sums, planted level flows) checked against their restatements.  Results are checked against the
 oracle so that a clean log means a correct run."""
 import os
 import sys
@@ -303,6 +304,72 @@ for integrate in (0, 1):
         all(np.array_equal(*(np.where(np.isnan(a), np.float32(np.nan), a).view(np.uint8) if a.dtype == np.float32
                              else a for a in (gv[k], ev[k]))) for k in ("T", "W", "C"))
 print("%-22s %s" % ("fuse_track", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# confidence-weighted push and tracking on the same volume: weights with 0, -0, NaN, +-inf, negative values, 3e9 and
+# 1e-30, the tracking with integration; poses, stats and volume checked bitwise
+wts = rng.uniform(0.05, 2.0, tmaps.shape).astype(np.float32)
+for v, share in ((0.0, 0.03), (-0.0, 0.03), (np.nan, 0.03), (np.inf, 0.02), (-np.inf, 0.02), (-1.0, 0.03),
+                 (3e9, 0.02), (1e-30, 0.02)):
+    wts[rng.random(wts.shape) < share] = v
+trk = dict(step=1, rounds=4, min_weight=1.0, max_depth=float("inf"), huber=0.2, damping=0.1, min_corr=6,
+           max_shift=0.5, min_cos=0.99, eps=0.0, integrate=1)
+ctx = api.Context(prm, w3, h3, prm.p_samp_s, 2)
+ctx.fuse_begin(tp_)
+ctx.fuse_set_volume(tv["T"], tv["W"], tv["C"])
+gpo, gst = ctx.fuse_track(tmaps, tmot, tprev, cam, trk, width_org=w3, height_org=h3, frames=rgb, weights=wts)
+ctx.fuse_push(tmaps, gpo, cam, width_org=w3, height_org=h3, frames=rgb, weights=wts)
+gv = ctx.fuse_volume()
+ctx.close()
+ev = {k: v.copy() for k, v in tv.items()}
+epo, est = preprocess.fuse_track(ev, tp_, trk, tmaps, tmot, tprev, cam, rgb, weights=wts)
+preprocess.fuse_integrate(ev, tp_, tmaps, epo, cam, frames=rgb, weights=wts)
+ok = np.array_equal(gpo.view(np.uint64), epo.view(np.uint64)) and \
+    all(np.array_equal(gst[k], est[k]) for k in est.dtype.names) and (est["rounds"] > 0).any() and \
+    all(np.array_equal(*(np.where(np.isnan(a), np.float32(np.nan), a).view(np.uint8) if a.dtype == np.float32
+                         else a for a in (gv[k], ev[k]))) for k in ("T", "W", "C"))
+print("%-22s %s" % ("fuse_weighted", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# per-pixel confidence: a two-way RGB flow clip of partial tiles, one forward and one backward level flow planted
+# with NaN, +-inf, -0 and 3e9, r = 1 and 7, with and without partners, host and device outputs
+cprm = params.from_cli_numbers("3 1 8 8 0.05 0.95 0 8 0.4 0 1 0 1 10 10 5 1 3 1.6 0".split(), noc=3, nop=2)
+ch_, cw_, cn = 45, 77, 2
+cframes = synth.synthetic_sequence(cn + 1, ch_, cw_, 3, seed=9, amp=3.0)
+scf = 1 << cprm.sc_f
+ctx = api.Context(cprm, (cw_ + scf - 1) // scf * scf, (ch_ + scf - 1) // scf * scf, cprm.p_samp_s, 2 * cn)
+ctx.upload_sequence_bidir_u8(0, cn, cframes, cw_, ch_)
+ctx.run(2 * cn)
+for slot in (0, cn + 1):
+    lv = ctx.get_flow(slot, cprm.sc_l)
+    for v, share in ((np.nan, 0.05), (np.inf, 0.03), (-np.inf, 0.03), (-0.0, 0.05), (3e9, 0.03)):
+        lv[rng.random(lv.shape) < share] = np.float32(v)
+    ctx.set_flow(slot, cprm.sc_l, lv)
+F = np.empty((2 * cn, ch_, cw_, 2), np.float32)
+ctx.get_flow_fullres(0, 2 * cn, F, cw_, ch_)
+ctx.sync()
+d_frames = torch.from_numpy(cframes).cuda()
+d_conf = torch.zeros((cn, ch_, cw_), device="cuda")
+d_terms = torch.zeros((cn, ch_, cw_, 3), device="cuda")
+torch.cuda.synchronize()
+canon = lambda a: np.where(np.isnan(a), np.float32(np.nan), a).view(np.uint32)  # NaN of arithmetic: any payload
+ok = True
+for r in (1, 7):
+    cp = dict(radius=r, s_fb=1.0, s_tex=100.0, min_count=(2 * r + 1) ** 2 // 2)
+    for b0 in (cn, -1):
+        hc, ht = ctx.confidence_fullres(0, cn, b0, cframes[:-1], cframes[1:], cp, cw_, ch_, with_terms=True)
+        ctx.confidence_fullres(0, cn, b0, d_frames.data_ptr(), d_frames.data_ptr() + ch_ * cw_ * 3, cp, cw_, ch_,
+                               with_terms=True, memkind=api.MEM_DEVICE, conf=d_conf.data_ptr(),
+                               terms=d_terms.data_ptr(), frame_stride=ch_ * cw_ * 3)
+        ctx.sync()
+        for k in range(cn):
+            ec, et = preprocess.confidence(cframes[k], cframes[k + 1], F[k], None if b0 < 0 else F[cn + k], cp)
+            ok = ok and np.array_equal(hc[k].view(np.uint32), ec.view(np.uint32)) and \
+                np.array_equal(canon(ht[k]), canon(et)) and \
+                np.array_equal(d_conf[k].cpu().numpy().view(np.uint32), ec.view(np.uint32)) and \
+                np.array_equal(canon(d_terms[k].cpu().numpy()), canon(et))
+ctx.close()
+print("%-22s %s" % ("confidence", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
