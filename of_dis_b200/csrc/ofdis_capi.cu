@@ -21,6 +21,35 @@
 
 using namespace ofdis;
 
+// A lazily allocated device buffer that only grows (the workspaces of the stages outside ofdis_run)
+struct DevBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+  // at least n bytes: nothing when the buffer holds them, else the stream synchronised, the old buffer freed and a new
+  // one allocated; on failure p is null, bytes 0, and the error OFDIS_ERR_NOMEM with `what`
+  int reserve(ofdis_ctx* ctx, size_t n, const char* what);
+};
+
+// Hands out consecutive typed arrays of a workspace, each on a 16-byte boundary.  Without a base it only counts, so
+// one layout function both sizes a workspace (size()) and places its arrays; offsets stay integers until placed.
+struct Carve {
+  char* base = nullptr;
+  size_t off = 0;
+  template <class T>
+  T* take(size_t count) {
+    const size_t at = (off + 15) & ~(size_t)15;
+    off = at + sizeof(T) * count;
+    return base ? reinterpret_cast<T*>(base + at) : nullptr;
+  }
+  // the same room, but null unless `want`: an output a call does not ask for keeps its place in the layout
+  template <class T>
+  T* take(size_t count, bool want) {
+    T* p = take<T>(count);
+    return want ? p : nullptr;
+  }
+  size_t size() const { return (off + 15) & ~(size_t)15; }
+};
+
 struct ofdis_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -58,27 +87,20 @@ struct ofdis_ctx {
   // swapped marks (ofdis_set_swapped_slots), one byte per internal frame, in the same allocation right in front of
   // d_img (LevelGeom::swap_off); this is the pointer the allocation is freed by
   unsigned char* d_swapped = nullptr;
-  // lazily allocated staging of the pyramid / output stages (ofdis_upload_frames_u8,
-  // ofdis_upload_finest_level, ofdis_get_flow_fullres)
-  void* d_stage = nullptr;
-  size_t stage_bytes = 0;
-  float* d_full = nullptr;
-  size_t full_floats = 0;
-  // lazily allocated workspace of ofdis_flow_error_fullres: the row partials [max_frames][16][height], then the
-  // device stats [max_frames][16]; never touched by ofdis_run
-  ErrRowPartial* d_eval = nullptr;
-  // lazily allocated workspace of ofdis_flow_color_fullres: the automatic scales' maxima [max_frames] as float bit
-  // patterns; never touched by ofdis_run
-  unsigned int* d_color = nullptr;
-  // lazily allocated workspace of ofdis_interpolate_fullres (InterpWork for max_frames pairs of width x height
-  // pixels); never touched by ofdis_run
-  void* d_interp = nullptr;
+  // The workspaces below (DevBuf) are lazily allocated and never touched by ofdis_run.
+  // staging of host inputs (ofdis_upload_frames_u8, ofdis_upload_finest_level, ...) and the scratch of host outputs
+  // (ofdis_get_flow_fullres, ...)
+  DevBuf d_stage, d_full;
+  // ofdis_flow_error_fullres: the row partials [max_frames][16][height], then the device stats [max_frames][16]
+  DevBuf d_eval;
+  // ofdis_flow_color_fullres: the automatic scales' maxima [max_frames] as float bit patterns
+  DevBuf d_color;
+  // ofdis_interpolate_fullres (InterpWork for max_frames pairs of width x height pixels)
+  DevBuf d_interp;
   InterpWork interp{};
   // the tracker of ofdis_track_begin / ofdis_track_advance: its workspace (TrackWork, then the host-output records of
-  // max_frames pairs), the geometry of the last begin and the list that holds the live tracks; never touched by
-  // ofdis_run
-  void* d_track = nullptr;
-  size_t track_bytes = 0;
+  // max_frames pairs), the geometry of the last begin and the list that holds the live tracks
+  DevBuf d_track;
   TrackWork track{};
   ofdis_track_point* track_out = nullptr;
   TrackGeom tgeom{};
@@ -86,65 +108,51 @@ struct ofdis_ctx {
   bool track_on = false;
   // the descriptor stage of ofdis_traj_begin / ofdis_traj_advance on top of the tracker: its workspace (TrajWork, then
   // the host-output records and descriptors of max_frames pairs), the geometry of the last begin and the frames seen
-  // since it; ended by ofdis_track_begin and ofdis_track_advance; never touched by ofdis_run
-  void* d_traj = nullptr;
-  size_t traj_bytes = 0;
+  // since it; ended by ofdis_track_begin and ofdis_track_advance
+  DevBuf d_traj;
   TrajWork traj{};
   TrajGeom trgeom{};
   ofdis_traj_record* traj_rec = nullptr;
   float* traj_desc = nullptr;
   int traj_frame = 0;
   bool traj_on = false;
-  // lazily allocated workspace of ofdis_disparity_fullres (DispWork for max_frames pairs of width x height pixels);
-  // never touched by ofdis_run
-  void* d_disp = nullptr;
-  // lazily allocated counters of ofdis_scene_flow_fullres ([max_frames][16] ofdis_sf_stats); never touched by ofdis_run
-  ofdis_sf_stats* d_sf = nullptr;
-  // lazily allocated workspace of ofdis_global_motion_fullres (MotionWork for max_frames pairs of motion_cells cells
-  // and motion_hyps hypotheses); grows, never shrinks; never touched by ofdis_run
-  void* d_motion = nullptr;
+  // ofdis_disparity_fullres (DispWork for max_frames pairs of width x height pixels)
+  DevBuf d_disp;
+  // ofdis_scene_flow_fullres's counters ([max_frames][16] ofdis_sf_stats)
+  DevBuf d_sf;
+  // ofdis_global_motion_fullres (MotionWork for max_frames pairs of motion_cells cells and motion_hyps hypotheses)
+  DevBuf d_motion;
   size_t motion_cells = 0, motion_hyps = 0;
   MotionWork motion{};
-  // lazily allocated workspace of ofdis_egomotion_fullres (EgoWork for max_frames pairs of ego_cells cells and
-  // ego_hyps hypotheses); grows, never shrinks; never touched by ofdis_run
-  void* d_ego = nullptr;
+  // ofdis_egomotion_fullres (EgoWork for max_frames pairs of ego_cells cells and ego_hyps hypotheses)
+  DevBuf d_ego;
   size_t ego_cells = 0, ego_hyps = 0;
   EgoWork ego{};
   // the stabiliser of ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish: its workspace (StabWork: the frame ring,
-  // the model ring, the per-frame records), the geometry and weights of the last begin, L and the next frame to emit;
-  // grows, never shrinks; never touched by ofdis_run
-  void* d_stab = nullptr;
-  size_t stab_bytes = 0;
+  // the model ring, the per-frame records), the geometry and weights of the last begin, L and the next frame to emit
+  DevBuf d_stab;
   StabWork stab{};
   StabGeom sgeom{};
   long long stab_last = 0, stab_next = 0;
   bool stab_on = false;
   // the Fisher encoder of ofdis_fisher_begin / ofdis_fisher_push / ofdis_fisher_take: its workspace (FisherWork), the
-  // geometry of the last begin and the descriptors pushed since it or the last take; grows, never shrinks; never
-  // touched by ofdis_run
-  void* d_fisher = nullptr;
-  size_t fisher_bytes = 0;
+  // geometry of the last begin and the descriptors pushed since it or the last take
+  DevBuf d_fisher;
   FisherWork fisher{};
   FisherGeom fgeom{};
   long long fisher_pushed = 0;
   bool fisher_on = false;
   // the volume of ofdis_fuse_begin / ofdis_fuse_push / ofdis_fuse_extract / ofdis_fuse_render: T, W, the colour bytes,
-  // then FuseWork's poses and scan blocks; the geometry of the last begin; grows, never shrinks; never touched by
-  // ofdis_run
-  void* d_fuse = nullptr;
-  size_t fuse_bytes = 0;
+  // then FuseWork's poses and scan blocks; the geometry of the last begin
+  DevBuf d_fuse;
   FuseGeom fuse_geom{};
   FuseVolume fuse_vol{};
   FuseWork fuse_ws{};
   bool fuse_on = false;
-  // lazily allocated workspace of ofdis_fuse_mesh (FuseMeshWork: the per-voxel first vertex indices, the second scan
-  // blocks and their total); grows, never shrinks; never touched by ofdis_run
-  void* d_mesh = nullptr;
-  size_t mesh_bytes = 0;
-  // lazily allocated workspace of ofdis_fuse_track (the pose chain's state, motions, poses and stats, the push pose,
-  // then the chunk sums); grows, never shrinks; never touched by ofdis_run
-  void* d_ftrack = nullptr;
-  size_t ftrack_bytes = 0;
+  // ofdis_fuse_mesh (FuseMeshWork: the per-voxel first vertex indices, the second scan blocks and their total)
+  DevBuf d_mesh;
+  // ofdis_fuse_track (the pose chain's state, motions, poses and stats, the push pose, then the chunk sums)
+  DevBuf d_ftrack;
   std::vector<float*> d_flow;   // index level - sc_l, plus one extra entry for level sc_f+1 (initflow)
   std::vector<size_t> flow_floats;
   VarRefPlanes planes{};
@@ -338,6 +346,59 @@ bool alloc_refinement(ofdis_ctx* ctx, size_t recf4, int chain_nb) {
 
 }  // namespace
 
+int DevBuf::reserve(ofdis_ctx* ctx, size_t n, const char* what) {
+  if (bytes >= n) return OFDIS_OK;
+  CK(cudaStreamSynchronize(ctx->stream));
+  cudaFree(p);
+  p = nullptr;
+  bytes = 0;
+  if (cudaMalloc(&p, n) != cudaSuccess) {
+    p = nullptr;
+    return fail(ctx, OFDIS_ERR_NOMEM, what);
+  }
+  bytes = n;
+  return OFDIS_OK;
+}
+
+// The bytes of the workspace `layout` lays out
+template <class F>
+static size_t measure(F&& layout) {
+  Carve c;
+  layout(c);
+  return c.size();
+}
+
+// Reserves buf for `layout` and at least `floor` bytes, then has `layout` place its arrays in it
+template <class F>
+static int carve(ofdis_ctx* ctx, DevBuf& buf, const char* what, F&& layout, size_t floor = 0) {
+  const int rc = buf.reserve(ctx, std::max(measure(layout), floor), what);
+  if (rc) return rc;
+  Carve c{static_cast<char*>(buf.p)};
+  layout(c);
+  return OFDIS_OK;
+}
+
+// The scratch of host outputs for frames of pix pixels: at least the pix * nop * max_frames floats
+// ofdis_get_flow_fullres asks for, so that host-memory calls that alternate with it never reallocate
+template <class F>
+static int carve_full(ofdis_ctx* ctx, size_t pix, F&& layout) {
+  return carve(ctx, ctx->d_full, "full-resolution flow buffer", layout,
+               sizeof(float) * pix * ctx->nop * (size_t)ctx->max_frames);
+}
+
+// The staging of host inputs
+template <class F>
+static int carve_stage(ofdis_ctx* ctx, F&& layout) {
+  return carve(ctx, ctx->d_stage, "staging buffer", layout);
+}
+
+// The staging of host 8-bit frames of hwc bytes: at least two frames per pair of max_frames, as the pair upload
+// needs, so that the uploads, the tracker, confidence and interpolation never reallocate when they alternate
+template <class F>
+static int carve_stage_u8(ofdis_ctx* ctx, size_t hwc, F&& layout) {
+  return carve(ctx, ctx->d_stage, "staging buffer", layout, hwc * 2 * (size_t)ctx->max_frames);
+}
+
 extern "C" {
 
 const char* ofdis_version(void) { return "ofdis_b200 0.1 (sm_90a)"; }
@@ -506,22 +567,10 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
   for (auto& kv : ctx->graphs) cudaGraphExecDestroy(kv.second);
   cudaFree(ctx->d_swapped);  // d_img lies in the same allocation
-  cudaFree(ctx->d_stage);
-  cudaFree(ctx->d_full);
-  cudaFree(ctx->d_eval);
-  cudaFree(ctx->d_color);
-  cudaFree(ctx->d_interp);
-  cudaFree(ctx->d_track);
-  cudaFree(ctx->d_disp);
-  cudaFree(ctx->d_sf);
-  cudaFree(ctx->d_motion);
-  cudaFree(ctx->d_ego);
-  cudaFree(ctx->d_traj);
-  cudaFree(ctx->d_stab);
-  cudaFree(ctx->d_fisher);
-  cudaFree(ctx->d_fuse);
-  cudaFree(ctx->d_mesh);
-  cudaFree(ctx->d_ftrack);
+  for (DevBuf* b : {&ctx->d_stage, &ctx->d_full, &ctx->d_eval, &ctx->d_color, &ctx->d_interp, &ctx->d_track,
+                    &ctx->d_disp, &ctx->d_sf, &ctx->d_motion, &ctx->d_ego, &ctx->d_traj, &ctx->d_stab, &ctx->d_fisher,
+                    &ctx->d_fuse, &ctx->d_mesh, &ctx->d_ftrack})
+    cudaFree(b->p);
   for (float* p : ctx->d_flow) cudaFree(p);
   for (LevelGeom& L : ctx->lev) {
     cudaFree(L.pat_p);
@@ -680,17 +729,6 @@ static int finish_pyramid(ofdis_ctx* ctx, int f0, int f1, PyramidSource src = PA
   return finish_gradients(ctx, f0, f1);
 }
 
-static int ensure_stage(ofdis_ctx* ctx, size_t bytes) {
-  if (ctx->stage_bytes >= bytes) return OFDIS_OK;
-  CK(cudaStreamSynchronize(ctx->stream));
-  cudaFree(ctx->d_stage);
-  ctx->d_stage = nullptr;
-  ctx->stage_bytes = 0;
-  if (cudaMalloc(&ctx->d_stage, bytes) != cudaSuccess) return fail(ctx, OFDIS_ERR_NOMEM, "staging buffer");
-  ctx->stage_bytes = bytes;
-  return OFDIS_OK;
-}
-
 static int org_padding(ofdis_ctx* ctx, int width_org, int height_org, int* padl, int* padt) {
   // run_dense.cpp:299-311: pad up to the next multiple of 2^lv_f -- or of 2^(lv_f+1), as for a run with an init flow
   // (run_dense.cpp:301) -- floor(pad/2) on the left/top
@@ -719,11 +757,12 @@ int ofdis_upload_frames_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char* 
   src.image_bytes = (size_t)width_org * height_org * ctx->prm.noc;
   src.frames = frames;
   if (memkind != OFDIS_MEM_DEVICE) {
-    const size_t bytes = src.image_bytes * 2 * (size_t)(f1 - f0);
-    rc = ensure_stage(ctx, src.image_bytes * 2 * (size_t)ctx->max_frames);
+    unsigned char* st = nullptr;
+    rc = carve_stage_u8(ctx, src.image_bytes,
+                        [&](Carve& c) { st = c.take<unsigned char>(src.image_bytes * 2 * (size_t)ctx->max_frames); });
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_stage, frames, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    src.frames = static_cast<const unsigned char*>(ctx->d_stage);
+    CK(cudaMemcpyAsync(st, frames, src.image_bytes * 2 * (size_t)(f1 - f0), cudaMemcpyHostToDevice, ctx->stream));
+    src.frames = st;
   }
   if (launch_pyr_from_u8(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, f0 * ctx->dirs + (f1 - f0), src, ctx->stream) < 0)
     return fail(ctx, OFDIS_ERR_CUDA, "pyr_from_u8_kernel launch", cudaGetLastError());
@@ -746,12 +785,12 @@ int ofdis_upload_sequence_u8(ofdis_ctx* ctx, int f0, int f1, const unsigned char
   src.image_bytes = (size_t)width_org * height_org * ctx->prm.noc;
   src.frames = frames;
   if (memkind != OFDIS_MEM_DEVICE) {
-    // the staging size of ofdis_upload_frames_u8 (2 x max_frames images; n + 1 <= max_frames + 1 frames fit), so
-    // that alternating the two uploads never reallocates
-    rc = ensure_stage(ctx, src.image_bytes * 2 * (size_t)ctx->max_frames);
+    unsigned char* st = nullptr;
+    rc = carve_stage_u8(ctx, src.image_bytes,
+                        [&](Carve& c) { st = c.take<unsigned char>(src.image_bytes * (size_t)(ctx->max_frames + 1)); });
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_stage, frames, src.image_bytes * (size_t)(n + 1), cudaMemcpyHostToDevice, ctx->stream));
-    src.frames = static_cast<const unsigned char*>(ctx->d_stage);
+    CK(cudaMemcpyAsync(st, frames, src.image_bytes * (size_t)(n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    src.frames = st;
   }
   if (launch_pyr_from_u8_seq(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, n, src, ctx->stream) < 0)
     return fail(ctx, OFDIS_ERR_CUDA, "pyr_from_u8_kernel launch", cudaGetLastError());
@@ -775,11 +814,12 @@ int ofdis_upload_sequence_bidir_u8(ofdis_ctx* ctx, int f0, int n, const unsigned
   src.image_bytes = (size_t)width_org * height_org * ctx->prm.noc;
   src.frames = frames;
   if (memkind != OFDIS_MEM_DEVICE) {
-    // the staging size of ofdis_upload_frames_u8; n + 1 <= max_frames / 2 + 1 frames fit
-    rc = ensure_stage(ctx, src.image_bytes * 2 * (size_t)ctx->max_frames);
+    unsigned char* st = nullptr;
+    const size_t cap = src.image_bytes * (size_t)(ctx->max_frames / 2 + 1);
+    rc = carve_stage_u8(ctx, src.image_bytes, [&](Carve& c) { st = c.take<unsigned char>(cap); });
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_stage, frames, src.image_bytes * (size_t)(n + 1), cudaMemcpyHostToDevice, ctx->stream));
-    src.frames = static_cast<const unsigned char*>(ctx->d_stage);
+    CK(cudaMemcpyAsync(st, frames, src.image_bytes * (size_t)(n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    src.frames = st;
   }
   const int D = ctx->dirs;
   if (launch_pyr_from_u8_bidir(stepped(ctx->lev[0], D), f0 * D, n, src, ctx->stream) < 0)
@@ -814,28 +854,16 @@ int ofdis_upload_finest_level(ofdis_ctx* ctx, int f0, int f1, const float* packe
   const size_t per = ofdis_finest_level_frame_floats(ctx);
   const float* src = packed;
   if (memkind != OFDIS_MEM_DEVICE) {
-    int rc = ensure_stage(ctx, sizeof(float) * per * (size_t)ctx->max_frames);
+    float* st = nullptr;
+    int rc = carve_stage(ctx, [&](Carve& c) { st = c.take<float>(per * (size_t)ctx->max_frames); });
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_stage, packed, sizeof(float) * per * (size_t)(f1 - f0), cudaMemcpyHostToDevice, ctx->stream));
-    src = static_cast<const float*>(ctx->d_stage);
+    CK(cudaMemcpyAsync(st, packed, sizeof(float) * per * (size_t)(f1 - f0), cudaMemcpyHostToDevice, ctx->stream));
+    src = st;
   }
   if (launch_pyr_from_level(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, f0 * ctx->dirs + (f1 - f0), src, ctx->stream) < 0)
     return fail(ctx, OFDIS_ERR_CUDA, "pyr_from_level_kernel launch", cudaGetLastError());
   ctx->launches += 1;
   return finish_pyramid(ctx, f0, f1);
-}
-
-// full-resolution flow scratch of at least `floats` floats (ofdis_get_flow_fullres, ofdis_set_initflow_from_result)
-static int ensure_full(ofdis_ctx* ctx, size_t floats) {
-  if (ctx->full_floats >= floats) return OFDIS_OK;
-  CK(cudaStreamSynchronize(ctx->stream));
-  cudaFree(ctx->d_full);
-  ctx->d_full = nullptr;
-  ctx->full_floats = 0;
-  if (cudaMalloc((void**)&ctx->d_full, sizeof(float) * floats) != cudaSuccess)
-    return fail(ctx, OFDIS_ERR_NOMEM, "full-resolution flow buffer");
-  ctx->full_floats = floats;
-  return OFDIS_OK;
 }
 
 // Level sc_f+1 of pairs [f0, f0 + n) from full-resolution device flows (run_dense.cpp:355-378).  The context must
@@ -872,10 +900,11 @@ int ofdis_set_initflow_fullres(ofdis_ctx* ctx, int f0, int f1, const float* flow
   const size_t per = (size_t)width_org * height_org * ctx->nop;
   const float* src = flow;
   if (memkind != OFDIS_MEM_DEVICE) {
-    rc = ensure_stage(ctx, sizeof(float) * per * (size_t)ctx->max_frames);
+    float* st = nullptr;
+    rc = carve_stage(ctx, [&](Carve& c) { st = c.take<float>(per * (size_t)ctx->max_frames); });
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_stage, flow, sizeof(float) * per * (size_t)(f1 - f0), cudaMemcpyHostToDevice, ctx->stream));
-    src = static_cast<const float*>(ctx->d_stage);
+    CK(cudaMemcpyAsync(st, flow, sizeof(float) * per * (size_t)(f1 - f0), cudaMemcpyHostToDevice, ctx->stream));
+    src = st;
   }
   return prepare_initflow(ctx, f0, f1 - f0, src, width_org, height_org);
 }
@@ -892,16 +921,18 @@ int ofdis_set_initflow_from_result(ofdis_ctx* ctx, int f0, int f1, int src_f0, i
   CK(cudaSetDevice(ctx->device));
   // exactly ofdis_get_flow_fullres(DEVICE) into the full-resolution scratch, then ofdis_set_initflow_fullres(DEVICE);
   // the source (level sc_l) and the destination (level sc_f+1) are different buffers, so the slots may overlap
-  rc = ensure_full(ctx, (size_t)width_org * height_org * ctx->nop * (size_t)ctx->max_frames);
+  const size_t pix = (size_t)width_org * height_org;
+  float* flow = nullptr;
+  rc = carve_full(ctx, pix, [&](Carve& c) { flow = c.take<float>(pix * ctx->nop * (size_t)ctx->max_frames); });
   if (rc) return rc;
   {
     NvtxRange nvtx("upsample", -1);
     if (launch_flow_upsample(stepped(ctx->lev[0], ctx->dirs), src_f0 * ctx->dirs, src_f0 * ctx->dirs + (f1 - f0),
-                             ctx->d_full, width_org, height_org, cx, cy, ctx->stream) < 0)
+                             flow, width_org, height_org, cx, cy, ctx->stream) < 0)
       return fail(ctx, OFDIS_ERR_CUDA, "flow_upsample_kernel launch", cudaGetLastError());
     ctx->launches += 1;
   }
-  return prepare_initflow(ctx, f0, f1 - f0, ctx->d_full, width_org, height_org);
+  return prepare_initflow(ctx, f0, f1 - f0, flow, width_org, height_org);
 }
 
 int ofdis_get_flow_fullres(ofdis_ctx* ctx, int f0, int f1, float* out, int width_org, int height_org, int memkind) {
@@ -912,12 +943,11 @@ int ofdis_get_flow_fullres(ofdis_ctx* ctx, int f0, int f1, float* out, int width
   if (rc) return rc;
   NvtxRange nvtx("upsample", -1);
   CK(cudaSetDevice(ctx->device));
-  const size_t per = (size_t)width_org * height_org * ctx->nop;
+  const size_t pix = (size_t)width_org * height_org, per = pix * ctx->nop;
   float* dst = out;
   if (memkind != OFDIS_MEM_DEVICE) {
-    rc = ensure_full(ctx, per * (size_t)ctx->max_frames);
+    rc = carve_full(ctx, pix, [&](Carve& c) { dst = c.take<float>(per * (size_t)ctx->max_frames); });
     if (rc) return rc;
-    dst = ctx->d_full;
   }
   if (launch_flow_upsample(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, f0 * ctx->dirs + (f1 - f0), dst, width_org, height_org,
                            cx, cy, ctx->stream) < 0)
@@ -945,10 +975,8 @@ int ofdis_get_flow_fullres_encoded(ofdis_ctx* ctx, int f0, int f1, int encoding,
   const size_t per = encoding == OFDIS_ENC_F16 ? pix * ctx->nop : pix * (ctx->nop == 2 ? 3 : 1);
   unsigned short* dst = static_cast<unsigned short*>(out);
   if (memkind != OFDIS_MEM_DEVICE) {
-    // the size ofdis_get_flow_fullres asks for; every encoding fits in it
-    rc = ensure_full(ctx, pix * ctx->nop * (size_t)ctx->max_frames);
+    rc = carve_full(ctx, pix, [&](Carve& c) { dst = c.take<unsigned short>(per * (size_t)ctx->max_frames); });
     if (rc) return rc;
-    dst = reinterpret_cast<unsigned short*>(ctx->d_full);
   }
   if (launch_flow_encode(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, f1 - f0, encoding, dst, width_org, height_org,
                          cx, cy, ctx->stream) < 0)
@@ -972,21 +1000,20 @@ int ofdis_flow_color_fullres(ofdis_ctx* ctx, int f0, int f1, unsigned char* rgb,
   CK(cudaSetDevice(ctx->device));
   const int n = f1 - f0;
   const size_t pix = (size_t)width_org * height_org;
-  if (!ctx->d_color && cudaMalloc((void**)&ctx->d_color, sizeof(unsigned int) * ctx->max_frames) != cudaSuccess) {
-    ctx->d_color = nullptr;
-    return fail(ctx, OFDIS_ERR_NOMEM, "flow_color_fullres workspace");
-  }
+  unsigned int* dmax = nullptr;
+  rc = carve(ctx, ctx->d_color, "flow_color_fullres workspace",
+             [&](Carve& c) { dmax = c.take<unsigned int>(ctx->max_frames); });
+  if (rc) return rc;
   unsigned char* drgb = rgb;
   float* dscale = scale;
   if (memkind != OFDIS_MEM_DEVICE) {
-    // the full-resolution scratch: the images, then the scales at the next float; the size ofdis_get_flow_fullres
-    // asks for holds both unless a frame has fewer than 8 pixels
-    rc = ensure_full(ctx, std::max(pix * ctx->nop, (3 * pix + 7) / 4 + 1) * (size_t)ctx->max_frames);
+    rc = carve_full(ctx, pix, [&](Carve& c) {
+      drgb = c.take<unsigned char>(3 * pix * ctx->max_frames);
+      dscale = c.take<float>(ctx->max_frames, scale);
+    });
     if (rc) return rc;
-    drgb = reinterpret_cast<unsigned char*>(ctx->d_full);
-    dscale = scale ? ctx->d_full + (3 * pix * n + 3) / 4 : nullptr;
   }
-  const int k = launch_flow_color(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, n, ctx->d_color, max_value, drgb,
+  const int k = launch_flow_color(stepped(ctx->lev[0], ctx->dirs), f0 * ctx->dirs, n, dmax, max_value, drgb,
                                   dscale, width_org, height_org, cx, cy, ctx->stream);
   if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "flow_color_kernel launch", cudaGetLastError());
   ctx->launches += k;
@@ -1013,12 +1040,11 @@ int ofdis_consistency_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, unsigned c
   unsigned char* dmask = mask;
   float* derr = err;
   if (memkind != OFDIS_MEM_DEVICE) {
-    // the full-resolution scratch: err (if asked for) then the mask; sized for max_frames, and at least what
-    // ofdis_get_flow_fullres asks for, so that alternating the two never reallocates
-    rc = ensure_full(ctx, std::max(pix * ctx->nop, (pix * 5 + 3) / 4) * (size_t)ctx->max_frames);
+    rc = carve_full(ctx, pix, [&](Carve& c) {
+      derr = c.take<float>(pix * ctx->max_frames, err);
+      dmask = c.take<unsigned char>(pix * ctx->max_frames);
+    });
     if (rc) return rc;
-    derr = err ? ctx->d_full : nullptr;
-    dmask = reinterpret_cast<unsigned char*>(ctx->d_full + (err ? pix * n : 0));
   }
   const int D = ctx->dirs;
   if (launch_consistency(stepped(ctx->lev[0], D), f0 * D, b0 * D, n, dmask, derr, width_org, height_org, cx, cy, alpha,
@@ -1055,18 +1081,20 @@ int ofdis_confidence_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis
   ConfArgs a{frames0, frames1, frame_stride, conf, terms, width_org, height_org, cx, cy, p->radius, p->min_count,
              p->s_fb, p->s_tex};
   if (!dev) {
-    // both frames of every pair into the staging buffer (2 x max_frames images), conf then terms through the
-    // full-resolution scratch, sized for max_frames and at least what ofdis_get_flow_fullres asks for
-    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    unsigned char *i0 = nullptr, *i1 = nullptr;
+    rc = carve_stage_u8(ctx, hwc, [&](Carve& c) {
+      i0 = c.take<unsigned char>(hwc * ctx->max_frames);
+      i1 = c.take<unsigned char>(hwc * ctx->max_frames);
+    });
     if (rc) return rc;
-    rc = ensure_full(ctx, pix * std::max(ctx->nop, 4) * (size_t)ctx->max_frames);
+    rc = carve_full(ctx, pix, [&](Carve& c) {
+      a.conf = c.take<float>(pix * ctx->max_frames, conf);
+      a.terms = c.take<float>(3 * pix * ctx->max_frames, terms);
+    });
     if (rc) return rc;
-    unsigned char* st = static_cast<unsigned char*>(ctx->d_stage);
-    CK(cudaMemcpy2DAsync(st, hwc, frames0, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpy2DAsync(st + hwc * n, hwc, frames1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-    a.i0 = st, a.i1 = st + hwc * n, a.stride = hwc;
-    a.conf = conf ? ctx->d_full : nullptr;
-    a.terms = terms ? ctx->d_full + pix * n : nullptr;
+    CK(cudaMemcpy2DAsync(i0, hwc, frames0, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(i1, hwc, frames1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    a.i0 = i0, a.i1 = i1, a.stride = hwc;
   }
   if (launch_confidence(stepped(ctx->lev[0], D), f0 * D, b0 >= 0 ? b0 * D : -1, n, ctx->prm.noc, a, ctx->stream) < 0)
     return fail(ctx, OFDIS_ERR_CUDA, "confidence_kernel launch", cudaGetLastError());
@@ -1083,33 +1111,20 @@ int ofdis_confidence_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis
 // the first call: per pixel and pair the keys (8 bytes), u_t (4 nop), the fill stamps (4), two hole lists (4 + 4) and
 // the two consistency masks (1 + 1); then one word per pair and width + height round counts.
 static int ensure_interp(ofdis_ctx* ctx) {
-  if (ctx->d_interp) return OFDIS_OK;
   const size_t P = (size_t)ctx->max_frames * ctx->width * ctx->height;
   if (P > UINT_MAX) return fail(ctx, OFDIS_ERR_UNSUPPORTED, "interpolate_fullres: more than 2^32 pixels per call");
-  const size_t bytes = P * (22 + 4 * (size_t)ctx->nop) + sizeof(int) * ctx->max_frames +
-                       sizeof(unsigned int) * (ctx->width + ctx->height);
-  void* p = nullptr;
-  if (cudaMalloc(&p, bytes) != cudaSuccess) return fail(ctx, OFDIS_ERR_NOMEM, "interpolate_fullres workspace");
-  char* b = static_cast<char*>(p);
   InterpWork& ws = ctx->interp;
-  ws.keys = reinterpret_cast<unsigned long long*>(b);
-  b += 8 * P;
-  ws.ut = reinterpret_cast<float*>(b);
-  b += 4 * ctx->nop * P;
-  ws.stamp = reinterpret_cast<int*>(b);
-  b += 4 * P;
-  ws.list[0] = reinterpret_cast<unsigned int*>(b);
-  b += 4 * P;
-  ws.list[1] = reinterpret_cast<unsigned int*>(b);
-  b += 4 * P;
-  ws.any = reinterpret_cast<int*>(b);
-  b += sizeof(int) * ctx->max_frames;
-  ws.count = reinterpret_cast<unsigned int*>(b);
-  b += sizeof(unsigned int) * (ctx->width + ctx->height);
-  ws.m0 = reinterpret_cast<unsigned char*>(b);
-  ws.m1 = ws.m0 + P;
-  ctx->d_interp = p;
-  return OFDIS_OK;
+  return carve(ctx, ctx->d_interp, "interpolate_fullres workspace", [&](Carve& c) {
+    ws.keys = c.take<unsigned long long>(P);
+    ws.ut = c.take<float>(ctx->nop * P);
+    ws.stamp = c.take<int>(P);
+    ws.list[0] = c.take<unsigned int>(P);
+    ws.list[1] = c.take<unsigned int>(P);
+    ws.any = c.take<int>(ctx->max_frames);
+    ws.count = c.take<unsigned int>(ctx->width + ctx->height);
+    ws.m0 = c.take<unsigned char>(P);
+    ws.m1 = c.take<unsigned char>(P);
+  });
 }
 
 int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned char* i0, const unsigned char* i1,
@@ -1134,17 +1149,17 @@ int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsi
   InterpSrc s{i0, i1, frame_stride, width_org, height_org, cx, cy, t};
   unsigned char* dout = out;
   if (memkind != OFDIS_MEM_DEVICE) {
-    // both frames of every pair into the staging buffer (2 x max_frames images), output through the full-resolution
-    // scratch at the size ofdis_get_flow_fullres asks for (an 8-bit frame is never larger than the float flow)
-    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    unsigned char *s0 = nullptr, *s1 = nullptr;
+    rc = carve_stage_u8(ctx, hwc, [&](Carve& c) {
+      s0 = c.take<unsigned char>(hwc * ctx->max_frames);
+      s1 = c.take<unsigned char>(hwc * ctx->max_frames);
+    });
     if (rc) return rc;
-    rc = ensure_full(ctx, pix * nop * (size_t)ctx->max_frames);
+    rc = carve_full(ctx, pix, [&](Carve& c) { dout = c.take<unsigned char>(hwc * ctx->max_frames); });
     if (rc) return rc;
-    unsigned char* st = static_cast<unsigned char*>(ctx->d_stage);
-    CK(cudaMemcpy2DAsync(st, hwc, i0, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpy2DAsync(st + hwc * n, hwc, i1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-    s = InterpSrc{st, st + hwc * n, hwc, width_org, height_org, cx, cy, t};
-    dout = reinterpret_cast<unsigned char*>(ctx->d_full);
+    CK(cudaMemcpy2DAsync(s0, hwc, i0, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(s1, hwc, i1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    s = InterpSrc{s0, s1, hwc, width_org, height_org, cx, cy, t};
   }
   const LevelGeom g = stepped(ctx->lev[0], D);
   CK(cudaMemsetAsync(ws.keys, 0xff, sizeof(unsigned long long) * pix * n, ctx->stream));
@@ -1191,19 +1206,15 @@ int ofdis_interpolate_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const unsi
 // pairs densely at the front of each array.
 static int ensure_disp(ofdis_ctx* ctx, DispWork* ws) {
   const size_t P = (size_t)ctx->max_frames * ctx->width * ctx->height, R = (size_t)ctx->max_frames * ctx->height;
-  if (!ctx->d_disp && cudaMalloc(&ctx->d_disp, P * 13 + R * 12) != cudaSuccess) {
-    ctx->d_disp = nullptr;
-    return fail(ctx, OFDIS_ERR_NOMEM, "disparity_fullres workspace");
-  }
-  char* b = static_cast<char*>(ctx->d_disp);
-  ws->val = reinterpret_cast<float*>(b);
-  ws->parent = reinterpret_cast<int*>(b + 4 * P);
-  ws->size = reinterpret_cast<int*>(b + 8 * P);
-  ws->rowfull = reinterpret_cast<int*>(b + 12 * P);
-  ws->up = ws->rowfull + R;
-  ws->down = ws->up + R;
-  ws->status = reinterpret_cast<unsigned char*>(b + 12 * P + 12 * R);
-  return OFDIS_OK;
+  return carve(ctx, ctx->d_disp, "disparity_fullres workspace", [&](Carve& c) {
+    ws->val = c.take<float>(P);
+    ws->parent = c.take<int>(P);
+    ws->size = c.take<int>(P);
+    ws->rowfull = c.take<int>(R);
+    ws->up = c.take<int>(R);
+    ws->down = c.take<int>(R);
+    ws->status = c.take<unsigned char>(P);
+  });
 }
 
 static bool finite_ge0(float v) { return v >= 0.f && v <= FLT_MAX; }
@@ -1240,15 +1251,14 @@ int ofdis_disparity_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
   const size_t np = pix * n;
   DispOutputs out{disp, status, depth, xyz};
   if (!dev) {
-    // the full-resolution scratch: disp, depth and xyz floats (those asked for), then the status bytes; sized for
-    // max_frames, and at least what ofdis_get_flow_fullres asks for
-    rc = ensure_full(ctx, std::max(pix * ctx->nop, pix * 5 + (pix + 3) / 4) * (size_t)ctx->max_frames);
+    const size_t cap = pix * ctx->max_frames;
+    rc = carve_full(ctx, pix, [&](Carve& c) {
+      out.disp = c.take<float>(cap, disp);
+      out.depth = c.take<float>(cap, depth);
+      out.xyz = c.take<float>(3 * cap, xyz);
+      out.status = c.take<unsigned char>(cap, status);
+    });
     if (rc) return rc;
-    float* q = ctx->d_full;
-    if (disp) out.disp = q, q += np;
-    if (depth) out.depth = q, q += np;
-    if (xyz) out.xyz = q, q += 3 * np;
-    out.status = status ? reinterpret_cast<unsigned char*>(q) : nullptr;
   }
   const DispFilter f{filt->lr_check, filt->alpha, filt->beta, filt->speckle_size, filt->speckle_diff, filt->fill};
   DispCamera c{};
@@ -1267,49 +1277,28 @@ int ofdis_disparity_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
   return OFDIS_OK;
 }
 
-static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
-
 // The workspace of ofdis_global_motion_fullres for max_frames pairs of at least `cells` cells and `hyps` hypotheses:
 // per cell the correspondence (16 bytes), its flag (1) and the refit's chunk sums (44 doubles per 32 cells, 11); per
-// hypothesis its float64 parameters (64) and MotionHyp (48); per pair MotionOut, the key and the count.  Grows, never
-// shrinks.
+// hypothesis its float64 parameters (64) and MotionHyp (48); per pair MotionOut, the key and the count.  The cell and
+// hypothesis capacities grow independently, never shrink.
 static int ensure_motion(ofdis_ctx* ctx, size_t cells, size_t hyps) {
-  cells = (cells + 31) / 32 * 32;
-  const size_t n = (size_t)ctx->max_frames;
-  if (ctx->d_motion && cells <= ctx->motion_cells && hyps <= ctx->motion_hyps) return OFDIS_OK;
-  cells = std::max(cells, ctx->motion_cells);
+  cells = std::max((cells + 31) / 32 * 32, ctx->motion_cells);
   hyps = std::max(hyps, ctx->motion_hyps);
-  const size_t b_corr = n * cells * sizeof(float4), b_chunk = n * (cells / 32) * MOTION_NE * sizeof(double);
-  const size_t b_hp = n * hyps * 8 * sizeof(double), b_hg = n * hyps * sizeof(MotionHyp);
-  const size_t b_out = align16(n * sizeof(MotionOut)), b_key = align16(n * 8), b_m = align16(n * 4);
-  CK(cudaStreamSynchronize(ctx->stream));
-  cudaFree(ctx->d_motion);
-  ctx->d_motion = nullptr;
-  ctx->motion_cells = ctx->motion_hyps = 0;
-  if (cudaMalloc(&ctx->d_motion, b_corr + b_chunk + b_hp + b_hg + b_out + b_key + b_m + n * cells) != cudaSuccess) {
-    ctx->d_motion = nullptr;
-    return fail(ctx, OFDIS_ERR_NOMEM, "global_motion_fullres workspace");
-  }
-  char* b = static_cast<char*>(ctx->d_motion);
+  const size_t n = (size_t)ctx->max_frames;
   MotionWork& ws = ctx->motion;
-  ws.corr = reinterpret_cast<float4*>(b);
-  b += b_corr;
-  ws.chunk = reinterpret_cast<double*>(b);
-  b += b_chunk;
-  ws.hp = reinterpret_cast<double*>(b);
-  b += b_hp;
-  ws.hg = reinterpret_cast<MotionHyp*>(b);
-  b += b_hg;
-  ws.out = reinterpret_cast<MotionOut*>(b);
-  b += b_out;
-  ws.key = reinterpret_cast<unsigned long long*>(b);
-  b += b_key;
-  ws.m = reinterpret_cast<int*>(b);
-  b += b_m;
-  ws.flag = reinterpret_cast<unsigned char*>(b);
-  ctx->motion_cells = cells;
-  ctx->motion_hyps = hyps;
-  return OFDIS_OK;
+  const int rc = carve(ctx, ctx->d_motion, "global_motion_fullres workspace", [&](Carve& c) {
+    ws.corr = c.take<float4>(n * cells);
+    ws.chunk = c.take<double>(n * (cells / 32) * MOTION_NE);
+    ws.hp = c.take<double>(n * hyps * 8);
+    ws.hg = c.take<MotionHyp>(n * hyps);
+    ws.out = c.take<MotionOut>(n);
+    ws.key = c.take<unsigned long long>(n);
+    ws.m = c.take<int>(n);
+    ws.flag = c.take<unsigned char>(n * cells);
+  });
+  ctx->motion_cells = rc ? 0 : cells;
+  ctx->motion_hyps = rc ? 0 : hyps;
+  return rc;
 }
 
 int ofdis_global_motion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_motion_params* p,
@@ -1351,20 +1340,19 @@ int ofdis_global_motion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const of
   mg.cell_cap = ctx->motion_cells, mg.chunk_cap = ctx->motion_cells / 32, mg.hyp_cap = ctx->motion_hyps;
   MotionOutputs o{mask, residual, registered, i1, frame_stride};
   if (!dev && (mask || residual || registered)) {
-    // the full-resolution scratch: residual floats, then the mask and registered bytes (those asked for); sized for
-    // max_frames, and at least what ofdis_get_flow_fullres asks for.  I1 goes through the staging buffer.
-    rc = ensure_full(ctx, std::max(pix * ctx->nop, 2 * pix + (pix * (1 + noc) + 3) / 4) * (size_t)ctx->max_frames);
+    const size_t cap = pix * ctx->max_frames;
+    rc = carve_full(ctx, pix, [&](Carve& c) {
+      o.residual = c.take<float>(2 * cap, residual);
+      o.mask = c.take<unsigned char>(cap, mask);
+      o.registered = c.take<unsigned char>(noc * cap, registered);
+    });
     if (rc) return rc;
-    float* q = ctx->d_full;
-    if (residual) o.residual = q, q += 2 * pix * n;
-    unsigned char* qb = reinterpret_cast<unsigned char*>(q);
-    if (mask) o.mask = qb, qb += pix * n;
     if (registered) {
-      o.registered = qb;
-      rc = ensure_stage(ctx, hwc * (size_t)ctx->max_frames);
+      unsigned char* st = nullptr;
+      rc = carve_stage(ctx, [&](Carve& c) { st = c.take<unsigned char>(hwc * ctx->max_frames); });
       if (rc) return rc;
-      CK(cudaMemcpy2DAsync(ctx->d_stage, hwc, i1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-      o.i1 = static_cast<const unsigned char*>(ctx->d_stage);
+      CK(cudaMemcpy2DAsync(st, hwc, i1, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+      o.i1 = st;
       o.stride = hwc;
     }
   }
@@ -1389,44 +1377,26 @@ int ofdis_global_motion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const of
 
 // The workspace of ofdis_egomotion_fullres for max_frames pairs of at least `cells` cells and `hyps` hypotheses: per
 // cell the correspondence (32 bytes), its flag (1) and the refit's chunk sums (27 doubles per 32 cells); per hypothesis
-// its float64 [R | t] (96) and EgoHyp (64); per pair EgoOut, the key and the count.  Grows, never shrinks.
+// its float64 [R | t] (96) and EgoHyp (64); per pair EgoOut, the key and the count.  The cell and hypothesis
+// capacities grow independently, never shrink.
 static int ensure_ego(ofdis_ctx* ctx, size_t cells, size_t hyps) {
-  cells = (cells + 31) / 32 * 32;
-  const size_t n = (size_t)ctx->max_frames;
-  if (ctx->d_ego && cells <= ctx->ego_cells && hyps <= ctx->ego_hyps) return OFDIS_OK;
-  cells = std::max(cells, ctx->ego_cells);
+  cells = std::max((cells + 31) / 32 * 32, ctx->ego_cells);
   hyps = std::max(hyps, ctx->ego_hyps);
-  const size_t b_corr = n * cells * sizeof(EgoCorr), b_chunk = n * (cells / 32) * EGO_NE * sizeof(double);
-  const size_t b_hp = n * hyps * 12 * sizeof(double), b_hg = n * hyps * sizeof(EgoHyp);
-  const size_t b_out = align16(n * sizeof(EgoOut)), b_key = align16(n * 8), b_m = align16(n * 4);
-  CK(cudaStreamSynchronize(ctx->stream));
-  cudaFree(ctx->d_ego);
-  ctx->d_ego = nullptr;
-  ctx->ego_cells = ctx->ego_hyps = 0;
-  if (cudaMalloc(&ctx->d_ego, b_corr + b_chunk + b_hp + b_hg + b_out + b_key + b_m + n * cells) != cudaSuccess) {
-    ctx->d_ego = nullptr;
-    return fail(ctx, OFDIS_ERR_NOMEM, "egomotion_fullres workspace");
-  }
-  char* b = static_cast<char*>(ctx->d_ego);
+  const size_t n = (size_t)ctx->max_frames;
   EgoWork& ws = ctx->ego;
-  ws.corr = reinterpret_cast<EgoCorr*>(b);
-  b += b_corr;
-  ws.chunk = reinterpret_cast<double*>(b);
-  b += b_chunk;
-  ws.hp = reinterpret_cast<double*>(b);
-  b += b_hp;
-  ws.hg = reinterpret_cast<EgoHyp*>(b);
-  b += b_hg;
-  ws.out = reinterpret_cast<EgoOut*>(b);
-  b += b_out;
-  ws.key = reinterpret_cast<unsigned long long*>(b);
-  b += b_key;
-  ws.m = reinterpret_cast<int*>(b);
-  b += b_m;
-  ws.flag = reinterpret_cast<unsigned char*>(b);
-  ctx->ego_cells = cells;
-  ctx->ego_hyps = hyps;
-  return OFDIS_OK;
+  const int rc = carve(ctx, ctx->d_ego, "egomotion_fullres workspace", [&](Carve& c) {
+    ws.corr = c.take<EgoCorr>(n * cells);
+    ws.chunk = c.take<double>(n * (cells / 32) * EGO_NE);
+    ws.hp = c.take<double>(n * hyps * 12);
+    ws.hg = c.take<EgoHyp>(n * hyps);
+    ws.out = c.take<EgoOut>(n);
+    ws.key = c.take<unsigned long long>(n);
+    ws.m = c.take<int>(n);
+    ws.flag = c.take<unsigned char>(n * cells);
+  });
+  ctx->ego_cells = rc ? 0 : cells;
+  ctx->ego_hyps = rc ? 0 : hyps;
+  return rc;
 }
 
 int ofdis_egomotion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_egomotion_params* p,
@@ -1469,23 +1439,25 @@ int ofdis_egomotion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
   eg.disp0 = disp0, eg.disp1 = disp1, eg.stride = disp_stride;
   EgoOutputs o{mask, residual, object_motion};
   if (!dev) {
-    // the staging buffer: disp0 and disp1 packed to one map per pair; sized for max_frames
-    rc = ensure_stage(ctx, sizeof(float) * 2 * pix * (size_t)ctx->max_frames);
+    // disp0 and disp1 packed to one map per pair
+    const size_t cap = pix * ctx->max_frames;
+    float *d0 = nullptr, *d1 = nullptr;
+    rc = carve_stage(ctx, [&](Carve& c) {
+      d0 = c.take<float>(cap);
+      d1 = c.take<float>(cap);
+    });
     if (rc) return rc;
-    float* st = static_cast<float*>(ctx->d_stage);
     const size_t row = sizeof(float) * pix, pitch = sizeof(float) * disp_stride;
-    CK(cudaMemcpy2DAsync(st, row, disp0, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpy2DAsync(st + np, row, disp1, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
-    eg.disp0 = st, eg.disp1 = st + np, eg.stride = pix;
+    CK(cudaMemcpy2DAsync(d0, row, disp0, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(d1, row, disp1, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
+    eg.disp0 = d0, eg.disp1 = d1, eg.stride = pix;
     if (mask || residual || object_motion) {
-      // the full-resolution scratch: residual and object_motion floats (those asked for), then the mask bytes; sized
-      // for max_frames, and at least what ofdis_get_flow_fullres asks for
-      rc = ensure_full(ctx, std::max(pix * ctx->nop, 5 * pix + (pix + 3) / 4) * (size_t)ctx->max_frames);
+      rc = carve_full(ctx, pix, [&](Carve& c) {
+        o.residual = c.take<float>(2 * cap, residual);
+        o.object_motion = c.take<float>(3 * cap, object_motion);
+        o.mask = c.take<unsigned char>(cap, mask);
+      });
       if (rc) return rc;
-      float* q = ctx->d_full;
-      if (residual) o.residual = q, q += 2 * np;
-      if (object_motion) o.object_motion = q, q += 3 * np;
-      if (mask) o.mask = reinterpret_cast<unsigned char*>(q);
     }
   }
   const int k = launch_egomotion(stepped(ctx->lev[0], D), f0 * D, (p->fb_check ? b0 : f0) * D, n, eg, ctx->ego, o,
@@ -1544,29 +1516,18 @@ int ofdis_fuse_begin(ofdis_ctx* ctx, const ofdis_fuse_params* p) {
   NvtxRange nvtx("fuse", -1);
   CK(cudaSetDevice(ctx->device));
   const size_t N = (size_t)p->nx * p->ny * p->nz, nb = (N + FUSE_BLOCK - 1) / FUSE_BLOCK;
-  const size_t b_t = align16(4 * N), b_c = p->color ? align16(3 * N) : 0;
-  const size_t b_g = align16(sizeof(float) * 12 * (size_t)(ctx->max_frames + 1)), b_s = 8 * (nb + 1);
-  const size_t bytes = 2 * b_t + b_c + b_g + b_s;
-  if (bytes > ctx->fuse_bytes) {
-    ctx->fuse_on = false;
-    CK(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_fuse);
-    ctx->d_fuse = nullptr;
-    ctx->fuse_bytes = 0;
-    if (cudaMalloc(&ctx->d_fuse, bytes) != cudaSuccess) {
-      ctx->d_fuse = nullptr;
-      return fail(ctx, OFDIS_ERR_NOMEM, "fuse volume");
-    }
-    ctx->fuse_bytes = bytes;
-  }
-  char* b = static_cast<char*>(ctx->d_fuse);
   FuseVolume& v = ctx->fuse_vol;
-  v.T = reinterpret_cast<float*>(b);
-  v.W = reinterpret_cast<float*>(b + b_t);
-  v.C = p->color ? reinterpret_cast<unsigned char*>(b + 2 * b_t) : nullptr;
-  ctx->fuse_ws.g = reinterpret_cast<float*>(b + 2 * b_t + b_c);
-  ctx->fuse_ws.bsum = reinterpret_cast<unsigned long long*>(b + 2 * b_t + b_c + b_g);
-  ctx->fuse_ws.total = ctx->fuse_ws.bsum + nb;
+  auto layout = [&](Carve& c) {
+    v.T = c.take<float>(N);
+    v.W = c.take<float>(N);
+    v.C = p->color ? c.take<unsigned char>(3 * N) : nullptr;
+    ctx->fuse_ws.g = c.take<float>(12 * (size_t)(ctx->max_frames + 1));
+    ctx->fuse_ws.bsum = c.take<unsigned long long>(nb);
+    ctx->fuse_ws.total = c.take<unsigned long long>(1);
+  };
+  if (measure(layout) > ctx->d_fuse.bytes) ctx->fuse_on = false;  // the live volume goes with the old buffer
+  const int rc = carve(ctx, ctx->d_fuse, "fuse volume", layout);
+  if (rc) return rc;
   FuseGeom& g = ctx->fuse_geom;
   g.count = (long long)N;
   g.nx = p->nx, g.ny = p->ny, g.nz = p->nz;
@@ -1576,6 +1537,36 @@ int ofdis_fuse_begin(ofdis_ctx* ctx, const ofdis_fuse_params* p) {
   CK(cudaMemsetAsync(v.W, 0, 4 * N, ctx->stream));
   if (v.C) CK(cudaMemsetAsync(v.C, 0, 3 * N, ctx->stream));
   ctx->fuse_on = true;
+  return OFDIS_OK;
+}
+
+// Host inputs of n frames of the fusion calls through the staging buffer: the disparity maps, the frames and the
+// weights (those not null) are copied there and replaced by their copies.  The layout holds max_frames + 1 of each,
+// with the frames' room whenever the volume has colour and the weights' whenever the call is weighted.
+static int fuse_stage(ofdis_ctx* ctx, int n, size_t pix, size_t hwc, bool color, const float** disp,
+                      size_t* disp_stride, const unsigned char** frames, size_t* frame_stride, const float** weight,
+                      size_t* weight_stride) {
+  const size_t F = (size_t)ctx->max_frames + 1;
+  float *d = nullptr, *w = nullptr;
+  unsigned char* f = nullptr;
+  const int rc = carve_stage(ctx, [&](Carve& c) {
+    d = c.take<float>(pix * F);
+    if (color) f = c.take<unsigned char>(hwc * F);
+    if (*weight) w = c.take<float>(pix * F);
+  });
+  if (rc) return rc;
+  CK(cudaMemcpy2DAsync(d, sizeof(float) * pix, *disp, sizeof(float) * *disp_stride, sizeof(float) * pix, n,
+                       cudaMemcpyHostToDevice, ctx->stream));
+  *disp = d, *disp_stride = pix;
+  if (*frames) {
+    CK(cudaMemcpy2DAsync(f, hwc, *frames, *frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+    *frames = f, *frame_stride = hwc;
+  }
+  if (*weight) {
+    CK(cudaMemcpy2DAsync(w, sizeof(float) * pix, *weight, sizeof(float) * *weight_stride, sizeof(float) * pix, n,
+                         cudaMemcpyHostToDevice, ctx->stream));
+    *weight = w, *weight_stride = pix;
+  }
   return OFDIS_OK;
 }
 
@@ -1609,25 +1600,9 @@ static int fuse_push_impl(ofdis_ctx* ctx, bool weighted, int n, const float* dis
   rc = fuse_poses(ctx, n, poses, true);
   if (rc) return rc;
   if (!dev) {
-    // the staging buffer: the disparity maps, then the frames, then the weights, packed; sized for max_frames + 1 of
-    // each
-    const size_t b_d = align16(sizeof(float) * pix * (size_t)(ctx->max_frames + 1));
-    const size_t b_f = color ? align16(hwc * (size_t)(ctx->max_frames + 1)) : 0;
-    rc = ensure_stage(ctx, b_d + b_f + (weighted ? b_d : 0));
+    rc = fuse_stage(ctx, n, pix, hwc, color, &fp.disp, &fp.disp_stride, &fp.frames, &fp.frame_stride, &fp.weight,
+                    &fp.weight_stride);
     if (rc) return rc;
-    char* st = static_cast<char*>(ctx->d_stage);
-    CK(cudaMemcpy2DAsync(st, sizeof(float) * pix, disp, sizeof(float) * disp_stride, sizeof(float) * pix, n,
-                         cudaMemcpyHostToDevice, ctx->stream));
-    fp.disp = reinterpret_cast<const float*>(st), fp.disp_stride = pix;
-    if (color) {
-      CK(cudaMemcpy2DAsync(st + b_d, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-      fp.frames = reinterpret_cast<const unsigned char*>(st + b_d), fp.frame_stride = hwc;
-    }
-    if (weighted) {
-      CK(cudaMemcpy2DAsync(st + b_d + b_f, sizeof(float) * pix, weight, sizeof(float) * weight_stride,
-                           sizeof(float) * pix, n, cudaMemcpyHostToDevice, ctx->stream));
-      fp.weight = reinterpret_cast<const float*>(st + b_d + b_f), fp.weight_stride = pix;
-    }
   }
   const int k = launch_fuse_push(ctx->fuse_geom, ctx->fuse_vol, fp, ctx->stream);
   if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_integrate_kernel launch", cudaGetLastError());
@@ -1672,11 +1647,9 @@ int ofdis_fuse_extract(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, 
     CK(cudaMemcpyAsync(&total, ctx->fuse_ws.total, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     cap = (long long)std::min<unsigned long long>(total, (unsigned long long)capacity);
-    if (cap > 0) {
-      const int rc = ensure_full(ctx, (size_t)cap * sizeof(ofdis_fuse_point) / sizeof(float));
-      if (rc) return rc;
-    }
-    out = reinterpret_cast<ofdis_fuse_point*>(ctx->d_full);
+    const int rc = carve(ctx, ctx->d_full, "full-resolution flow buffer",
+                         [&](Carve& c) { out = c.take<ofdis_fuse_point>((size_t)cap); });
+    if (rc) return rc;
   }
   k = launch_fuse_write(ctx->fuse_geom, ctx->fuse_vol, min_weight, ctx->fuse_ws, out, cap, ctx->stream);
   if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_write_kernel launch", cudaGetLastError());
@@ -1708,11 +1681,9 @@ int ofdis_fuse_render(ofdis_ctx* ctx, int n, const double* poses, const ofdis_st
   FuseRender fr{};
   fr.depth = depth;
   if (!dev) {
-    // the full-resolution scratch, sized for max_frames + 1 maps and at least what ofdis_get_flow_fullres asks for
     const size_t pix = (size_t)width_org * height_org;
-    rc = ensure_full(ctx, std::max(pix * ctx->nop * (size_t)ctx->max_frames, pix * (size_t)(ctx->max_frames + 1)));
+    rc = carve_full(ctx, pix, [&](Carve& c) { fr.depth = c.take<float>(pix * (ctx->max_frames + 1)); });
     if (rc) return rc;
-    fr.depth = ctx->d_full;
   }
   rc = fuse_poses(ctx, n, poses, false);
   if (rc) return rc;
@@ -1759,23 +1730,14 @@ int ofdis_fuse_mesh(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, lon
   NvtxRange nvtx("fuse", -1);
   CK(cudaSetDevice(ctx->device));
   const FuseGeom& g = ctx->fuse_geom;
-  const size_t N = (size_t)g.count, nb = (N + FUSE_BLOCK - 1) / FUSE_BLOCK, b_v = align16(4 * N);
-  const size_t bytes = b_v + 8 * (nb + 1);
-  if (bytes > ctx->mesh_bytes) {
-    CK(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_mesh);
-    ctx->d_mesh = nullptr;
-    ctx->mesh_bytes = 0;
-    if (cudaMalloc(&ctx->d_mesh, bytes) != cudaSuccess) {
-      ctx->d_mesh = nullptr;
-      return fail(ctx, OFDIS_ERR_NOMEM, "fuse_mesh workspace");
-    }
-    ctx->mesh_bytes = bytes;
-  }
+  const size_t N = (size_t)g.count, nb = (N + FUSE_BLOCK - 1) / FUSE_BLOCK;
   FuseMeshWork mw;
-  mw.vbase = static_cast<unsigned int*>(ctx->d_mesh);
-  mw.bsum = reinterpret_cast<unsigned long long*>(static_cast<char*>(ctx->d_mesh) + b_v);
-  mw.total = mw.bsum + nb;
+  const int rc = carve(ctx, ctx->d_mesh, "fuse_mesh workspace", [&](Carve& c) {
+    mw.vbase = c.take<unsigned int>(N);
+    mw.bsum = c.take<unsigned long long>(nb);
+    mw.total = c.take<unsigned long long>(1);
+  });
+  if (rc) return rc;
   int k = launch_fuse_count(g, ctx->fuse_vol, min_weight, ctx->fuse_ws, ctx->stream);
   if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_count_kernel launch", cudaGetLastError());
   ctx->launches += k;
@@ -1793,13 +1755,11 @@ int ofdis_fuse_mesh(ofdis_ctx* ctx, float min_weight, ofdis_fuse_point* pts, lon
     CK(cudaStreamSynchronize(ctx->stream));
     pcap = (long long)std::min<unsigned long long>(total[0], (unsigned long long)pt_capacity);
     fcap = (long long)std::min<unsigned long long>(total[1], (unsigned long long)face_capacity);
-    const size_t b_p = align16(sizeof(ofdis_fuse_point) * (size_t)pcap);
-    if (pcap > 0 || fcap > 0) {
-      const int rc = ensure_full(ctx, (b_p + 12 * (size_t)fcap + 3) / sizeof(float));
-      if (rc) return rc;
-    }
-    out = reinterpret_cast<ofdis_fuse_point*>(ctx->d_full);
-    fout = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(ctx->d_full) + b_p);
+    const int rc = carve(ctx, ctx->d_full, "full-resolution flow buffer", [&](Carve& c) {
+      out = c.take<ofdis_fuse_point>((size_t)pcap);
+      fout = c.take<unsigned int>(3 * (size_t)fcap);
+    });
+    if (rc) return rc;
   }
   k = launch_fuse_write(g, ctx->fuse_vol, min_weight, ctx->fuse_ws, out, pcap, ctx->stream, mw.vbase);
   if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "fuse_write_kernel launch", cudaGetLastError());
@@ -1879,53 +1839,26 @@ static int fuse_track_impl(ofdis_ctx* ctx, bool weighted, int n, const float* di
   t.min_weight = p->min_weight, t.max_depth = p->max_depth, t.huber = p->huber;
   t.damping = p->damping, t.max_shift = p->max_shift, t.min_cos = p->min_cos, t.eps = p->eps;
   t.cam = DispCamera{cam->fx * cam->baseline, cam->fx, cam->fy, cam->cx, cam->cy, cam->doffs};
-  // the workspace: the state, the motions, poses and stats of max_frames + 1 frames, the push pose, the chunk sums
+  // the workspace: the state, the motions, poses and stats of max_frames + 1 frames, the push pose, the chunk sums;
+  // host inputs through the staging buffer as the push's
   const size_t F = (size_t)ctx->max_frames + 1;
-  const size_t b_s = align16(sizeof(FuseTrackState)), b_m = align16(sizeof(double) * 12 * F);
-  const size_t b_st = align16(sizeof(ofdis_fuse_track_stats) * F), b_g = align16(sizeof(float) * 12);
-  const size_t bytes = b_s + 2 * b_m + b_st + b_g + sizeof(double) * FTRACK_NE * (size_t)t.nchunks;
-  if (bytes > ctx->ftrack_bytes) {
-    CK(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_ftrack);
-    ctx->d_ftrack = nullptr;
-    ctx->ftrack_bytes = 0;
-    if (cudaMalloc(&ctx->d_ftrack, bytes) != cudaSuccess) {
-      ctx->d_ftrack = nullptr;
-      return fail(ctx, OFDIS_ERR_NOMEM, "fuse_track workspace");
-    }
-    ctx->ftrack_bytes = bytes;
-  }
-  char* b = static_cast<char*>(ctx->d_ftrack);
-  t.state = reinterpret_cast<FuseTrackState*>(b);
-  t.motion = reinterpret_cast<const double*>(b + b_s);
-  t.pose = reinterpret_cast<double*>(b + b_s + b_m);
-  t.stats = reinterpret_cast<ofdis_fuse_track_stats*>(b + b_s + 2 * b_m);
-  t.g = reinterpret_cast<float*>(b + b_s + 2 * b_m + b_st);
-  t.chunk = reinterpret_cast<double*>(b + b_s + 2 * b_m + b_st + b_g);
+  rc = carve(ctx, ctx->d_ftrack, "fuse_track workspace", [&](Carve& c) {
+    t.state = c.take<FuseTrackState>(1);
+    t.motion = c.take<double>(12 * F);
+    t.pose = c.take<double>(12 * F);
+    t.stats = c.take<ofdis_fuse_track_stats>(F);
+    t.g = c.take<float>(12);
+    t.chunk = c.take<double>(FTRACK_NE * (size_t)t.nchunks);
+  });
+  if (rc) return rc;
   t.disp = disp, t.disp_stride = disp_stride;
   const unsigned char* fr = use_frames ? frames : nullptr;
   size_t fstride = frame_stride;
   const float* wt = weighted ? weight : nullptr;
   size_t wstride = weight_stride;
   if (!dev) {
-    // the staging buffer: the disparity maps, then the frames, then the weights, packed; sized for max_frames + 1 of
-    // each, as the push
-    const size_t b_d = align16(sizeof(float) * pix * F), b_f = color ? align16(hwc * F) : 0;
-    rc = ensure_stage(ctx, b_d + b_f + (weighted ? b_d : 0));
+    rc = fuse_stage(ctx, n, pix, hwc, color, &t.disp, &t.disp_stride, &fr, &fstride, &wt, &wstride);
     if (rc) return rc;
-    char* st = static_cast<char*>(ctx->d_stage);
-    CK(cudaMemcpy2DAsync(st, sizeof(float) * pix, disp, sizeof(float) * disp_stride, sizeof(float) * pix, n,
-                         cudaMemcpyHostToDevice, ctx->stream));
-    t.disp = reinterpret_cast<const float*>(st), t.disp_stride = pix;
-    if (use_frames) {
-      CK(cudaMemcpy2DAsync(st + b_d, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-      fr = reinterpret_cast<const unsigned char*>(st + b_d), fstride = hwc;
-    }
-    if (weighted) {
-      CK(cudaMemcpy2DAsync(st + b_d + b_f, sizeof(float) * pix, weight, sizeof(float) * weight_stride,
-                           sizeof(float) * pix, n, cudaMemcpyHostToDevice, ctx->stream));
-      wt = reinterpret_cast<const float*>(st + b_d + b_f), wstride = pix;
-    }
   }
   FuseTrackState init{};
   std::memcpy(init.prev, prev, sizeof(init.prev));
@@ -1983,40 +1916,27 @@ int ofdis_fuse_track_weighted(ofdis_ctx* ctx, int n, const float* disp, size_t d
 // The tracker's workspace for geometry t: the state, two track lists, the flags, the occupancy, the scan blocks'
 // sums, the counts of max_frames pairs, then the host-output records of max_frames pairs.  Grows, never shrinks.
 static int ensure_track(ofdis_ctx* ctx, const TrackGeom& t) {
-  const size_t list = align16(sizeof(ofdis_track_point) * t.capacity);
   const size_t nflags = (size_t)t.cap_pad + t.cells_pad;
-  const size_t part[7] = {align16(sizeof(TrackState)), list, list, nflags, align16(t.cells),
-                          align16(sizeof(unsigned int) * (nflags / TRACK_BLOCK)), align16(sizeof(int) * ctx->max_frames)};
-  size_t bytes = sizeof(ofdis_track_point) * t.capacity * (size_t)ctx->max_frames;
-  for (size_t p : part) bytes += p;
-  if (bytes > ctx->track_bytes) {
-    CK(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_track);
-    ctx->d_track = nullptr;
-    ctx->track_bytes = 0;
-    if (cudaMalloc(&ctx->d_track, bytes) != cudaSuccess) {
-      ctx->d_track = nullptr;
-      return fail(ctx, OFDIS_ERR_NOMEM, "track workspace");
-    }
-    ctx->track_bytes = bytes;
-  }
-  char* b = static_cast<char*>(ctx->d_track);
   TrackWork& ws = ctx->track;
-  ws.state = reinterpret_cast<TrackState*>(b);
-  b += part[0];
-  ws.list[0] = reinterpret_cast<ofdis_track_point*>(b);
-  b += part[1];
-  ws.list[1] = reinterpret_cast<ofdis_track_point*>(b);
-  b += part[2];
-  ws.flags = reinterpret_cast<unsigned char*>(b);
-  b += part[3];
-  ws.occ = reinterpret_cast<unsigned char*>(b);
-  b += part[4];
-  ws.bsum = reinterpret_cast<unsigned int*>(b);
-  b += part[5];
-  ws.counts = reinterpret_cast<int*>(b);
-  b += part[6];
-  ctx->track_out = reinterpret_cast<ofdis_track_point*>(b);
+  return carve(ctx, ctx->d_track, "track workspace", [&](Carve& c) {
+    ws.state = c.take<TrackState>(1);
+    ws.list[0] = c.take<ofdis_track_point>(t.capacity);
+    ws.list[1] = c.take<ofdis_track_point>(t.capacity);
+    ws.flags = c.take<unsigned char>(nflags);
+    ws.occ = c.take<unsigned char>(t.cells);
+    ws.bsum = c.take<unsigned int>(nflags / TRACK_BLOCK);
+    ws.counts = c.take<int>(ctx->max_frames);
+    ctx->track_out = c.take<ofdis_track_point>((size_t)t.capacity * ctx->max_frames);
+  });
+}
+
+// n host frames of hwc bytes, *stride apart, packed into the staging buffer; *frames and *stride then name the copy
+static int stage_frames_u8(ofdis_ctx* ctx, int n, size_t hwc, const unsigned char** frames, size_t* stride) {
+  unsigned char* st = nullptr;
+  const int rc = carve_stage_u8(ctx, hwc, [&](Carve& c) { st = c.take<unsigned char>(hwc * ctx->max_frames); });
+  if (rc) return rc;
+  CK(cudaMemcpy2DAsync(st, hwc, *frames, *stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
+  *frames = st, *stride = hwc;
   return OFDIS_OK;
 }
 
@@ -2059,10 +1979,11 @@ int ofdis_track_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const un
   const size_t hwc = (size_t)width_org * height_org * ctx->prm.noc;
   const unsigned char* I = frame;
   if (memkind != OFDIS_MEM_DEVICE) {
-    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    unsigned char* st = nullptr;
+    rc = carve_stage_u8(ctx, hwc, [&](Carve& c) { st = c.take<unsigned char>(hwc); });
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_stage, frame, hwc, cudaMemcpyHostToDevice, ctx->stream));
-    I = static_cast<const unsigned char*>(ctx->d_stage);
+    CK(cudaMemcpyAsync(st, frame, hwc, cudaMemcpyHostToDevice, ctx->stream));
+    I = st;
   }
   // no track yet: every keep flag and every cell's occupancy is 0
   CK(cudaMemsetAsync(ws.state, 0, sizeof(TrackState), ctx->stream));
@@ -2106,11 +2027,8 @@ int ofdis_track_advance(ofdis_ctx* ctx, int f0, int f1, int b0, const unsigned c
   const unsigned char* src = frames;
   size_t stride = frame_stride;
   if (memkind != OFDIS_MEM_DEVICE) {
-    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    rc = stage_frames_u8(ctx, n, hwc, &src, &stride);
     if (rc) return rc;
-    CK(cudaMemcpy2DAsync(ctx->d_stage, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-    src = static_cast<const unsigned char*>(ctx->d_stage);
-    stride = hwc;
   }
   ofdis_track_point* out = memkind == OFDIS_MEM_DEVICE ? points : ctx->track_out;
   const LevelGeom g = stepped(ctx->lev[0], D);
@@ -2184,49 +2102,28 @@ static size_t traj_bound(const TrajGeom& tg, int capacity, int n) {
 // their metadata, the per-slot scan arrays, the per-pixel fields, the models of max_frames pairs, the kept frame,
 // then the host-output records and descriptors of max_frames pairs.  Grows, never shrinks.
 static int ensure_traj(ofdis_ctx* ctx, const TrackGeom& t, const TrajGeom& tg) {
-  const size_t cp = (size_t)t.cap_pad, px = (size_t)tg.w * tg.h, nb = cp / TRACK_BLOCK;
+  const size_t cp = (size_t)t.cap_pad, px = (size_t)tg.w * tg.h;
   const size_t bound = traj_bound(tg, t.capacity, ctx->max_frames);
-  const size_t part[14] = {align16(sizeof(TrajState)), sizeof(float) * tg.ss * cp, sizeof(float) * tg.ss * cp,
-                           sizeof(int2) * cp, sizeof(int2) * cp, align16(sizeof(uchar4) * px),
-                           sizeof(float4) * 2 * px, align16(sizeof(float2) * px),
-                           align16(sizeof(float) * 9 * ctx->max_frames),
-                           align16(sizeof(int) * cp), align16(sizeof(int) * cp), align16(sizeof(TrajSeg) * cp),
-                           align16(sizeof(unsigned int) * nb), align16(sizeof(int) * ctx->max_frames)};
-  const size_t frame = align16(px * ctx->prm.noc), rec = align16(sizeof(ofdis_traj_record) * bound);
-  size_t bytes = frame + rec + sizeof(float) * tg.dim * bound;
-  for (size_t p : part) bytes += p;
-  if (bytes > ctx->traj_bytes) {
-    CK(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_traj);
-    ctx->d_traj = nullptr;
-    ctx->traj_bytes = 0;
-    if (cudaMalloc(&ctx->d_traj, bytes) != cudaSuccess) {
-      ctx->d_traj = nullptr;
-      return fail(ctx, OFDIS_ERR_NOMEM, "traj workspace");
-    }
-    ctx->traj_bytes = bytes;
-  }
-  char* b = static_cast<char*>(ctx->d_traj);
   TrajWork& tw = ctx->traj;
-  auto take = [&b](size_t n) { char* r = b; b += n; return r; };
-  tw.state = reinterpret_cast<TrajState*>(take(part[0]));
-  tw.st[0] = reinterpret_cast<float*>(take(part[1]));
-  tw.st[1] = reinterpret_cast<float*>(take(part[2]));
-  tw.meta[0] = reinterpret_cast<int2*>(take(part[3]));
-  tw.meta[1] = reinterpret_cast<int2*>(take(part[4]));
-  tw.bins = reinterpret_cast<uchar4*>(take(part[5]));
-  tw.mag = reinterpret_cast<float4*>(take(part[6]));
-  tw.res = reinterpret_cast<float2*>(take(part[7]));
-  tw.models = reinterpret_cast<float*>(take(part[8]));
-  tw.dst = reinterpret_cast<int*>(take(part[9]));
-  tw.eoff = reinterpret_cast<int*>(take(part[10]));
-  tw.seg = reinterpret_cast<TrajSeg*>(take(part[11]));
-  tw.ebsum = reinterpret_cast<unsigned int*>(take(part[12]));
-  tw.ndesc = reinterpret_cast<int*>(take(part[13]));
-  tw.frame = reinterpret_cast<unsigned char*>(take(frame));
-  ctx->traj_rec = reinterpret_cast<ofdis_traj_record*>(take(rec));
-  ctx->traj_desc = reinterpret_cast<float*>(b);
-  return OFDIS_OK;
+  return carve(ctx, ctx->d_traj, "traj workspace", [&](Carve& c) {
+    tw.state = c.take<TrajState>(1);
+    tw.st[0] = c.take<float>(tg.ss * cp);
+    tw.st[1] = c.take<float>(tg.ss * cp);
+    tw.meta[0] = c.take<int2>(cp);
+    tw.meta[1] = c.take<int2>(cp);
+    tw.bins = c.take<uchar4>(px);
+    tw.mag = c.take<float4>(2 * px);
+    tw.res = c.take<float2>(px);
+    tw.models = c.take<float>(9 * ctx->max_frames);
+    tw.dst = c.take<int>(cp);
+    tw.eoff = c.take<int>(cp);
+    tw.seg = c.take<TrajSeg>(cp);
+    tw.ebsum = c.take<unsigned int>(cp / TRACK_BLOCK);
+    tw.ndesc = c.take<int>(ctx->max_frames);
+    tw.frame = c.take<unsigned char>(px * ctx->prm.noc);
+    ctx->traj_rec = c.take<ofdis_traj_record>(bound);
+    ctx->traj_desc = c.take<float>(tg.dim * bound);
+  });
 }
 
 int ofdis_traj_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const ofdis_traj_params* traj,
@@ -2272,7 +2169,7 @@ int ofdis_traj_begin(ofdis_ctx* ctx, const ofdis_track_params* params, const ofd
   // frame 0's tracks start their first segment at frame 0; track_begin staged a host frame in d_stage
   CK(cudaMemsetAsync(tw.state, 0, sizeof(TrajState), ctx->stream));
   CK(cudaMemsetAsync(tw.meta[ctx->track_cur], 0, sizeof(int2) * t.cap_pad, ctx->stream));
-  CK(cudaMemcpyAsync(tw.frame, memkind == OFDIS_MEM_DEVICE ? frame : static_cast<const unsigned char*>(ctx->d_stage),
+  CK(cudaMemcpyAsync(tw.frame, memkind == OFDIS_MEM_DEVICE ? frame : static_cast<const unsigned char*>(ctx->d_stage.p),
                      hwc, cudaMemcpyDeviceToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->traj_frame = 0;
@@ -2321,11 +2218,8 @@ static int traj_advance_impl(ofdis_ctx* ctx, int f0, int f1, int b0, const unsig
   const unsigned char* src = frames;
   size_t stride = frame_stride;
   if (memkind != OFDIS_MEM_DEVICE) {
-    rc = ensure_stage(ctx, hwc * 2 * (size_t)ctx->max_frames);
+    rc = stage_frames_u8(ctx, n, hwc, &src, &stride);
     if (rc) return rc;
-    CK(cudaMemcpy2DAsync(ctx->d_stage, hwc, frames, frame_stride, hwc, n, cudaMemcpyHostToDevice, ctx->stream));
-    src = static_cast<const unsigned char*>(ctx->d_stage);
-    stride = hwc;
   }
   ofdis_track_point* out = memkind == OFDIS_MEM_DEVICE ? points : ctx->track_out;
   ofdis_traj_record* rout = memkind == OFDIS_MEM_DEVICE && !to_fisher ? records : ctx->traj_rec;
@@ -2415,23 +2309,12 @@ int ofdis_traj_stats_get(const ofdis_ctx* ctx, ofdis_traj_stats* out) {
 // ring (2r + max_frames models) and max(r, max_frames) records.  Grows, never shrinks.
 static int ensure_stab(ofdis_ctx* ctx, size_t hwc, int r) {
   const int ring = r + ctx->max_frames, mring = 2 * r + ctx->max_frames, nrec = std::max(r, ctx->max_frames);
-  const size_t b_frames = align16(hwc * ring), b_models = align16(sizeof(double) * 9 * mring);
-  const size_t bytes = b_frames + b_models + sizeof(StabRec) * nrec;
-  if (bytes > ctx->stab_bytes) {
-    CK(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_stab);
-    ctx->d_stab = nullptr;
-    ctx->stab_bytes = 0;
-    if (cudaMalloc(&ctx->d_stab, bytes) != cudaSuccess) {
-      ctx->d_stab = nullptr;
-      return fail(ctx, OFDIS_ERR_NOMEM, "stab workspace");
-    }
-    ctx->stab_bytes = bytes;
-  }
-  char* b = static_cast<char*>(ctx->d_stab);
-  ctx->stab.frames = reinterpret_cast<unsigned char*>(b);
-  ctx->stab.models = reinterpret_cast<double*>(b + b_frames);
-  ctx->stab.rec = reinterpret_cast<StabRec*>(b + b_frames + b_models);
+  const int rc = carve(ctx, ctx->d_stab, "stab workspace", [&](Carve& c) {
+    ctx->stab.frames = c.take<unsigned char>(hwc * ring);
+    ctx->stab.models = c.take<double>(9 * (size_t)mring);
+    ctx->stab.rec = c.take<StabRec>(nrec);
+  });
+  if (rc) return rc;
   ctx->sgeom.ring = ring;
   ctx->sgeom.mring = mring;
   return OFDIS_OK;
@@ -2483,11 +2366,10 @@ static int stab_emit(ofdis_ctx* ctx, int count, int cut, unsigned char* out, ofd
   if (count > 0) {
     unsigned char* dout = out;
     if (memkind != OFDIS_MEM_DEVICE) {
-      // the full-resolution scratch, at least what ofdis_get_flow_fullres asks for
+      // at the scratch's start, which sg.vec finds aligned
       const size_t frames = (size_t)std::max(sg.radius, ctx->max_frames);
-      int rc = ensure_full(ctx, std::max(pix * ctx->nop * (size_t)ctx->max_frames, (hwc * frames + 3) / 4));
+      const int rc = carve_full(ctx, pix, [&](Carve& c) { dout = c.take<unsigned char>(hwc * frames); });
       if (rc) return rc;
-      dout = reinterpret_cast<unsigned char*>(ctx->d_full);
     }
     sg.vec = sg.w % 4 == 0 && reinterpret_cast<uintptr_t>(dout) % 4 == 0;
     const int k = launch_stab(sg, ctx->stab, dout, ctx->stream);
@@ -2561,34 +2443,17 @@ int ofdis_stab_finish(ofdis_ctx* ctx, unsigned char* out, ofdis_stab_frame* info
 // staging, y, the posteriors and the skip flags, then the host-output vector.  Grows, never shrinks.
 static int ensure_fisher(ofdis_ctx* ctx, const FisherGeom& g, size_t body, size_t nstats) {
   const size_t C = FISHER_CHUNK;
-  const size_t b_cb = align16(sizeof(float) * body), b_st = align16(sizeof(double) * nstats);
-  const size_t b_cnt = align16(sizeof(unsigned long long) * 2 * FISHER_MAX_BLOCKS);
-  const size_t b_x = align16(sizeof(float) * C * g.desc_dim), b_y = align16(sizeof(float) * C * g.ydim);
-  const size_t b_g = align16(sizeof(float) * C * g.nblocks * g.K), b_sk = align16(C * g.nblocks);
-  const size_t b_fv = align16(sizeof(float) * 2 * g.K * g.ydim);
-  const size_t bytes = b_cb + b_st + b_cnt + b_x + b_y + b_g + b_sk + b_fv;
-  if (bytes > ctx->fisher_bytes) {
-    CK(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_fisher);
-    ctx->d_fisher = nullptr;
-    ctx->fisher_bytes = 0;
-    if (cudaMalloc(&ctx->d_fisher, bytes) != cudaSuccess) {
-      ctx->d_fisher = nullptr;
-      return fail(ctx, OFDIS_ERR_NOMEM, "fisher workspace");
-    }
-    ctx->fisher_bytes = bytes;
-  }
-  char* p = static_cast<char*>(ctx->d_fisher);
   FisherWork& w = ctx->fisher;
-  w.cb = reinterpret_cast<float*>(p);
-  w.stats = reinterpret_cast<double*>(p += b_cb);
-  w.count = reinterpret_cast<unsigned long long*>(p += b_st);
-  w.x = reinterpret_cast<float*>(p += b_cnt);
-  w.y = reinterpret_cast<float*>(p += b_x);
-  w.gamma = reinterpret_cast<float*>(p += b_y);
-  w.skip = reinterpret_cast<unsigned char*>(p += b_g);
-  w.fv = reinterpret_cast<float*>(p += b_sk);
-  return OFDIS_OK;
+  return carve(ctx, ctx->d_fisher, "fisher workspace", [&](Carve& c) {
+    w.cb = c.take<float>(body);
+    w.stats = c.take<double>(nstats);
+    w.count = c.take<unsigned long long>(2 * FISHER_MAX_BLOCKS);
+    w.x = c.take<float>(C * g.desc_dim);
+    w.y = c.take<float>(C * g.ydim);
+    w.gamma = c.take<float>(C * g.nblocks * g.K);
+    w.skip = c.take<unsigned char>(C * g.nblocks);
+    w.fv = c.take<float>(2 * (size_t)g.K * g.ydim);
+  });
 }
 
 static size_t fisher_nstats(const FisherGeom& g) {
@@ -2746,37 +2611,36 @@ int ofdis_flow_error_fullres(ofdis_ctx* ctx, int f0, int f1, const float* gt, co
   CK(cudaSetDevice(ctx->device));
   const int n = f1 - f0;
   const size_t pix = (size_t)width_org * height_org, nop = (size_t)ctx->nop;
-  // the workspace: row partials for max_frames x 16 classes x the level-0 rows, then the device stats
-  const size_t part_count = (size_t)ctx->max_frames * kEvalMaxClasses * ctx->height;
-  if (!ctx->d_eval &&
-      cudaMalloc((void**)&ctx->d_eval, sizeof(ErrRowPartial) * part_count +
-                                           sizeof(ofdis_error_stats) * ctx->max_frames * kEvalMaxClasses) != cudaSuccess) {
-    ctx->d_eval = nullptr;
-    return fail(ctx, OFDIS_ERR_NOMEM, "flow_error_fullres workspace");
-  }
-  ofdis_error_stats* dstats = reinterpret_cast<ofdis_error_stats*>(ctx->d_eval + part_count);
+  ErrRowPartial* part = nullptr;
+  ofdis_error_stats* dstats = nullptr;
+  rc = carve(ctx, ctx->d_eval, "flow_error_fullres workspace", [&](Carve& c) {
+    part = c.take<ErrRowPartial>((size_t)ctx->max_frames * kEvalMaxClasses * ctx->height);
+    dstats = c.take<ofdis_error_stats>((size_t)ctx->max_frames * kEvalMaxClasses);
+  });
+  if (rc) return rc;
   const float* dgt = gt;
   const unsigned char* dcls = classes;
   float* derr = err;
   if (memkind != OFDIS_MEM_DEVICE) {
-    // the full-resolution scratch: gt, err (if asked for), then the classes (if given); sized for max_frames
-    rc = ensure_full(ctx, (pix * (nop + 1) + (pix + 3) / 4) * (size_t)ctx->max_frames);
+    // gt and the classes go in, err comes out through the same scratch
+    const size_t cap = pix * ctx->max_frames;
+    float* sgt = nullptr;
+    unsigned char* scls = nullptr;
+    rc = carve_full(ctx, pix, [&](Carve& c) {
+      sgt = c.take<float>(nop * cap);
+      derr = c.take<float>(cap, err);
+      scls = c.take<unsigned char>(cap);
+    });
     if (rc) return rc;
-    float* s = ctx->d_full;
-    CK(cudaMemcpyAsync(s, gt, sizeof(float) * pix * nop * n, cudaMemcpyHostToDevice, ctx->stream));
-    dgt = s;
-    s += pix * nop * n;
-    if (err) {
-      derr = s;
-      s += pix * n;
-    }
+    CK(cudaMemcpyAsync(sgt, gt, sizeof(float) * pix * nop * n, cudaMemcpyHostToDevice, ctx->stream));
+    dgt = sgt;
     if (classes) {
-      CK(cudaMemcpyAsync(s, classes, pix * n, cudaMemcpyHostToDevice, ctx->stream));
-      dcls = reinterpret_cast<const unsigned char*>(s);
+      CK(cudaMemcpyAsync(scls, classes, pix * n, cudaMemcpyHostToDevice, ctx->stream));
+      dcls = scls;
     }
   }
   const int D = ctx->dirs;
-  if (launch_flow_error(stepped(ctx->lev[0], D), f0 * D, n, dgt, dcls, nclasses, derr, ctx->d_eval, dstats, width_org,
+  if (launch_flow_error(stepped(ctx->lev[0], D), f0 * D, n, dgt, dcls, nclasses, derr, part, dstats, width_org,
                         height_org, cx, cy, ctx->stream) < 0)
     return fail(ctx, OFDIS_ERR_CUDA, "flow_error_kernel launch", cudaGetLastError());
   ctx->launches += 2;
@@ -2813,10 +2677,11 @@ int ofdis_scene_flow_fullres(ofdis_ctx* ctx, int f0, int f1, const float* disp0,
   CK(cudaSetDevice(ctx->device));
   const int n = f1 - f0, D = ctx->dirs;
   const size_t np = pix * n;
-  if (stats && !ctx->d_sf &&
-      cudaMalloc((void**)&ctx->d_sf, sizeof(ofdis_sf_stats) * ctx->max_frames * kEvalMaxClasses) != cudaSuccess) {
-    ctx->d_sf = nullptr;
-    return fail(ctx, OFDIS_ERR_NOMEM, "scene_flow_fullres counters");
+  ofdis_sf_stats* dstats = nullptr;
+  if (stats) {
+    rc = carve(ctx, ctx->d_sf, "scene_flow_fullres counters",
+               [&](Carve& c) { dstats = c.take<ofdis_sf_stats>((size_t)ctx->max_frames * kEvalMaxClasses); });
+    if (rc) return rc;
   }
   SfArgs a{};
   a.disp0 = disp0;
@@ -2832,44 +2697,49 @@ int ofdis_scene_flow_fullres(ofdis_ctx* ctx, int f0, int f1, const float* disp0,
     a.gt_d1 = gt->disp1;
     a.gt_flow = gt->flow;
     a.classes = classes;
-    a.stats = ctx->d_sf;
+    a.stats = dstats;
   }
   a.nclasses = nclasses;
   if (!dev) {
-    // the staging buffer: disp0 and disp1 packed to one map per pair, then gt's disp0, disp1 and flow and the classes
-    // (those given); sized for max_frames
-    rc = ensure_stage(ctx, (sizeof(float) * 6 + 1) * pix * (size_t)ctx->max_frames);
+    // disp0 and disp1 packed to one map per pair, then gt's disp0, disp1 and flow and the classes (those given)
+    const size_t cap = pix * ctx->max_frames;
+    float *d0 = nullptr, *d1 = nullptr, *g0 = nullptr, *g1 = nullptr, *gf = nullptr;
+    unsigned char* cls = nullptr;
+    rc = carve_stage(ctx, [&](Carve& c) {
+      d0 = c.take<float>(cap);
+      d1 = c.take<float>(cap);
+      g0 = c.take<float>(cap);
+      g1 = c.take<float>(cap);
+      gf = c.take<float>(2 * cap);
+      cls = c.take<unsigned char>(cap);
+    });
     if (rc) return rc;
-    float* s = static_cast<float*>(ctx->d_stage);
     const size_t row = sizeof(float) * pix, pitch = sizeof(float) * disp_stride;
-    CK(cudaMemcpy2DAsync(s, row, disp0, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpy2DAsync(s + np, row, disp1, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
-    a.disp0 = s;
-    a.disp1 = s + np;
+    CK(cudaMemcpy2DAsync(d0, row, disp0, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(d1, row, disp1, pitch, row, n, cudaMemcpyHostToDevice, ctx->stream));
+    a.disp0 = d0;
+    a.disp1 = d1;
     a.stride = pix;
-    s += 2 * np;
     if (gt) {
-      CK(cudaMemcpyAsync(s, gt->disp0, sizeof(float) * np, cudaMemcpyHostToDevice, ctx->stream));
-      CK(cudaMemcpyAsync(s + np, gt->disp1, sizeof(float) * np, cudaMemcpyHostToDevice, ctx->stream));
-      CK(cudaMemcpyAsync(s + 2 * np, gt->flow, sizeof(float) * 2 * np, cudaMemcpyHostToDevice, ctx->stream));
-      a.gt_d0 = s;
-      a.gt_d1 = s + np;
-      a.gt_flow = s + 2 * np;
+      CK(cudaMemcpyAsync(g0, gt->disp0, sizeof(float) * np, cudaMemcpyHostToDevice, ctx->stream));
+      CK(cudaMemcpyAsync(g1, gt->disp1, sizeof(float) * np, cudaMemcpyHostToDevice, ctx->stream));
+      CK(cudaMemcpyAsync(gf, gt->flow, sizeof(float) * 2 * np, cudaMemcpyHostToDevice, ctx->stream));
+      a.gt_d0 = g0;
+      a.gt_d1 = g1;
+      a.gt_flow = gf;
       if (classes) {
-        CK(cudaMemcpyAsync(s + 4 * np, classes, np, cudaMemcpyHostToDevice, ctx->stream));
-        a.classes = reinterpret_cast<const unsigned char*>(s + 4 * np);
+        CK(cudaMemcpyAsync(cls, classes, np, cudaMemcpyHostToDevice, ctx->stream));
+        a.classes = cls;
       }
     }
-    // the full-resolution scratch: disp1_warped and motion floats (those asked for), then the status bytes; sized for
-    // max_frames, and at least what ofdis_get_flow_fullres asks for
-    rc = ensure_full(ctx, std::max(pix * ctx->nop, pix * 4 + (pix + 3) / 4) * (size_t)ctx->max_frames);
+    rc = carve_full(ctx, pix, [&](Carve& c) {
+      a.disp1w = c.take<float>(cap, disp1_warped);
+      a.motion = c.take<float>(3 * cap, motion);
+      a.status = c.take<unsigned char>(cap, status);
+    });
     if (rc) return rc;
-    float* q = ctx->d_full;
-    if (disp1_warped) a.disp1w = q, q += np;
-    if (motion) a.motion = q, q += 3 * np;
-    a.status = status ? reinterpret_cast<unsigned char*>(q) : nullptr;
   }
-  if (stats) CK(cudaMemsetAsync(ctx->d_sf, 0, sizeof(ofdis_sf_stats) * n * nclasses, ctx->stream));
+  if (stats) CK(cudaMemsetAsync(dstats, 0, sizeof(ofdis_sf_stats) * n * nclasses, ctx->stream));
   if (launch_scene_flow(stepped(ctx->lev[0], D), f0 * D, n, a, width_org, height_org, cx, cy, ctx->stream) < 0)
     return fail(ctx, OFDIS_ERR_CUDA, "sceneflow_kernel launch", cudaGetLastError());
   ctx->launches += 1;
@@ -2879,7 +2749,7 @@ int ofdis_scene_flow_fullres(ofdis_ctx* ctx, int f0, int f1, const float* disp0,
     if (status) CK(cudaMemcpyAsync(status, a.status, np, cudaMemcpyDeviceToHost, ctx->stream));
   }
   if (stats)
-    CK(cudaMemcpyAsync(stats, ctx->d_sf, sizeof(ofdis_sf_stats) * n * nclasses, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(stats, dstats, sizeof(ofdis_sf_stats) * n * nclasses, cudaMemcpyDeviceToHost, ctx->stream));
   if (!dev || stats) CK(cudaStreamSynchronize(ctx->stream));
   return OFDIS_OK;
 }
