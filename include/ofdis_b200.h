@@ -671,6 +671,103 @@ int ofdis_egomotion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
                             unsigned char* mask, float* residual, float* object_motion,
                             int width_org, int height_org, int memkind);
 
+/* Monocular relative pose from dense flows (extension, flow contexts only): a RANSAC eight-point fit of one essential
+ * matrix per pair with one calibrated camera, its decomposition, Gauss-Newton refits of the 5-DoF motion on the
+ * epipolar inliers, a parallax guard, and per pixel an epipolar mask, the Sampson distance and the depth up to scale.
+ * preprocess.relpose restates it bit for bit.  float32 where marked, float64 in the solver, everything without
+ * contraction and with IEEE division and square root; no transcendental function.  W = width_org, H = height_org,
+ * s = step, qNaN = the quiet NaN 0x7fc00000, K = [fx, 0, cx; 0, fy, cy; 0, 0, 1].  For every pair k < f1-f0, slot
+ * a = f0+k:
+ *   1. Correspondences.  The cells, their order and validity rule of ofdis_global_motion_fullres (fb_check included);
+ *      the m valid cells give pixel correspondences c = (px, py, xs, ys) float32 and normalized ones x = ((float)px -
+ *      cx) / fx, y = ((float)py - cy) / fy, x' = (xs - cx) / fx, y' = (ys - cy) / fy (float32).  m < 8: status 1.
+ *   2. Hypotheses h = 0 .. hypotheses-1.  Draws d = 0..7 by ofdis_global_motion_fullres's SplitMix64 rule give the
+ *      rows [x'x, x'y, x', y'x, y'y, y', x, y, 1] (float64 products of the float32 values) of an 8 x 9 system A e = 0.
+ *      Its null vector by full pivoting: for j = 0..7 the pivot is the first entry, rows i >= j outer and columns
+ *      c >= j inner, of the largest |a_ic| (NaN is never largest); a pivot that is not > 0 fails; rows j and i are
+ *      swapped (columns >= j), then columns j and c in every row together with the column permutation; for each
+ *      i > j: f = a_ij / a_jj, a_ic = a_ic - f * a_jc for c > j.  Then y_8 = 1 and for i = 7..0: y_i = -a_i8,
+ *      y_i = y_i - a_ic * y_c for c = i+1..7, y_i = y_i / a_ii; e is y un-permuted, divided entry by entry by
+ *      L = sqrt(((e0*e0 + e1*e1) + ...) + e8*e8) summed in order from +0.0.  A failed pivot or a non-finite entry of
+ *      e makes the hypothesis unsolvable (repeated or degenerate draws).  E = e row-major.
+ *   3. Scoring.  F = K^-T E K^-1 in float64 with ifx = 1.0/fx, ify = 1.0/fy, ux = -(cx*ifx), uy = -(cy*ify):
+ *      G_i0 = E_i0*ifx, G_i1 = E_i1*ify, G_i2 = ((E_i0*ux) + (E_i1*uy)) + E_i2; F_0j = ifx*G_0j, F_1j = ify*G_1j,
+ *      F_2j = ((ux*G_0j) + (uy*G_1j)) + G_2j, rounded to float32 g.  With a = g (px, py, 1) (a_r = (g_r0*px + g_r1*py)
+ *      + g_r2), b0 = (g0*xs + g3*ys) + g6, b1 = (g1*xs + g4*ys) + g7, e = (xs*a0 + ys*a1) + a2 and den = (a0*a0 +
+ *      a1*a1) + (b0*b0 + b1*b1), a correspondence is an inlier iff e*e <= (threshold*threshold) * den (float32): the
+ *      Sampson distance in pixels <= threshold, without a division.  The raw E is scored.  The best solvable
+ *      hypothesis has the most inliers, the lowest h on a tie.  No solvable hypothesis: status 2.
+ *   4. Refits.  The best E: S = E^T E (S_ij = ((E_0i*E_0j) + (E_1i*E_1j)) + (E_2i*E_2j)), V = I, then 8 sweeps of
+ *      the pairs (0,1), (0,2), (1,2) of the cyclic Jacobi method: where S_pq != 0, th = (S_qq - S_pp) / (2.0*S_pq),
+ *      t = 1.0 / (|th| + sqrt(th*th + 1.0)) negated when th < 0, c = 1.0 / sqrt(t*t + 1.0), s = t*c; the columns p, q
+ *      of S, then its rows p, q, then the columns p, q of V become (c*a - s*b, s*a + c*b) of the old (a, b).  v1, v2
+ *      are the columns of V of the largest diagonal entry of S and the larger of the other two (first on ties);
+ *      unit(a) = a / sqrt((a0*a0 + a1*a1) + a2*a2), x the cross product (a1*b2 - a2*b1, a2*b0 - a0*b2, a0*b1 - a1*b0):
+ *      v1 = unit(v1), v3 = unit(v1 x v2), v2 = v3 x v1, u1 = unit(E v1), u3 = unit(u1 x E v2), u2 = u3 x u1 (E v with
+ *      rows ((E_i0*v0) + (E_i1*v1)) + (E_i2*v2)).  R1_ij = ((u2_i*v1_j) - (u1_i*v2_j)) + (u3_i*v3_j), R2_ij =
+ *      ((u1_i*v2_j) - (u2_i*v1_j)) + (u3_i*v3_j); the candidates q = 0..3 are (R1, u3), (R1, -u3), (R2, u3),
+ *      (R2, -u3).  Over the inliers of the best hypothesis (step 3), with r0 = (x, y, 1), r1 = (x', y', 1) in float64
+ *      and Y = R r0 (Y_i = ((R_i0*x) + (R_i1*y)) + R_i2), c1 = r1 x Y, c2 = r1 x t, lambda = -(c1.c2) / (c1.c1)
+ *      (a.b = (a0*b0 + a1*b1) + a2*b2): the candidate with the most inliers of lambda > 0 and lambda*Y_2 + t_2 > 0
+ *      (in front of both cameras), the lowest q on a tie, is the model.  Then rounds r = 0, 1, ...: E = [t]x R
+ *      (E_0j = (-(t2*R_1j)) + (t1*R_2j), E_1j = (t2*R_0j) - (t0*R_2j), E_2j = (-(t1*R_0j)) + (t0*R_1j)), g its F as in
+ *      step 3, the tangent basis b1 = unit(t x e_a) with e_a the unit axis of the first smallest |t_a|, b2 = t x b1.
+ *      The inliers of g (step 3's test), each with Y = R r0, a = E r0 and b = E^T r1 (rows as above, b_j = ((E_0j*x')
+ *      + (E_1j*y')) + E_2j), the residual res = ((x'*a0) + (y'*a1)) + a2, the Sampson weight w = 1.0 / sqrt(((s0*s0 +
+ *      s1*s1) + s2*s2) + s3*s3) with s = (a0*ifx, a1*ify, b0*ifx, b1*ify), rr = w*res and the Jacobian row of
+ *      (omega, delta) J = (w*(2.0*g_0), w*(2.0*g_1), w*(2.0*g_2), w*(b1.n), w*(b2.n)) with g = Y x (r1 x t), n = Y x r1,
+ *      give N_pq = J_p*J_q (p <= q), the right side -(J_p*rr), the derotated flow length sqrt(dx*dx + dy*dy),
+ *      dx = fx*(x' - Y_0/Y_2), dy = fy*(y' - Y_1/Y_2), and the same length with Y = Rw r0 of the twisted pair
+ *      Rw_ij = sum over k = 0..2 from +0.0 of ((2.0*(t_i*t_k)) - (i == k ? 1.0 : 0.0)) * R_kj (the rotation by 180
+ *      degrees about t composed with R, which explains the same E), summed as ofdis_global_motion_fullres's refits sum (chunks of
+ *      32 from +0.0, then the pairwise tree).  When r = refine or fewer than 8 inliers: stop.  Else N is mirrored
+ *      and solved by ofdis_global_motion_fullres's elimination; a failure stops and keeps the model; else R <- C R
+ *      with ofdis_egomotion_fullres's Cayley rotation C of omega (R_ij = ((C_i0*R_0j) + (C_i1*R_1j)) + (C_i2*R_2j)),
+ *      t_i <- (t_i + delta_0*b1_i) + delta_1*b2_i, t <- unit(t), next round.
+ *   5. Parallax guard.  With Lr and Lw the last round's two length sums, parallax = (Lw < Lr ? Lw : Lr) /
+ *      (double)its inlier count: the mean derotated flow in pixels under R or its twisted pair, whichever is
+ *      smaller.  Without translation E is degenerate and the cheirality vote may pick the twisted candidate; one of
+ *      the two rotations then explains the flow alone.  Unless parallax >= min_parallax (a NaN fails): status 3, the
+ *      translation is unobservable (identical frames, or a pure rotation of a static scene; an object that moves on
+ *      its own among the inliers adds its own parallax to the mean).
+ *   6. pose = [n][12] float64 row-major [R | t], |t| = 1, camera-t coordinates to camera-t+1 coordinates (the
+ *      convention of ofdis_egomotion_fullres).  Status != 0: twelve float64 qNaN 0x7ff8000000000000.
+ *   7. Per pixel (X, Y), F = (u, v) and validity by step 1's rule at the pixel, c = ((float)X, (float)Y, X + u, Y + v):
+ *      mask 2 where the pixel is not valid or the status is not 0, else 0 where step 3's test passes with the final
+ *      model's g, else 1 (moves on its own, or a bad flow).  sampson = sqrtf((e*e) / den) of that test where mask
+ *      != 2, else qNaN.  depth: with the pose rounded to float32 (R, t), x, y, x', y' of step 1 and float32 Y = R r0
+ *      (Y_i = (R_i0*x + R_i1*y) + R_i2), c1 = (y'*Y2 - Y1, Y0 - x'*Y2, x'*Y1 - y'*Y0), c2 = (y'*t2 - t1,
+ *      t0 - x'*t2, x'*t1 - y'*t0), lambda = -((c1_0*c2_0 + c1_1*c2_1) + c1_2*c2_2) / ((c1_0*c1_0 + c1_1*c1_1) +
+ *      c1_2*c1_2): lambda where mask != 2, lambda > 0 and lambda*Y2 + t2 > 0, else qNaN -- the depth at t in units of
+ *      |t|.  Every NaN written is qNaN.
+ * stats per pair: status (0 fitted, 1 fewer than 8 correspondences, 2 no solvable hypothesis, 3 too little parallax),
+ * n_corr = m, best_hypothesis (-1 for status 1 and 2), ransac_inliers (its count), refits (rounds that replaced the
+ * model), n_inliers (the final model's count).  pose and stats are host memory; mask [n][H][W] bytes, sampson and depth
+ * [n][H][W] float32 are optional (NULL skips them) and in memkind; host outputs go through the full-resolution scratch.
+ * OFDIS_ERR_ARG: a stereo context, slots outside the context (b0 only with fb_check), a NULL p or one out of range
+ * (fx, fy finite and > 0, cx, cy finite, step >= 1, fb_check 0|1, alpha and beta finite and >= 0, hypotheses
+ * 1..65536, threshold finite and > 0, refine 0..16, min_parallax finite and >= 0), NULL pose or stats, a device
+ * sampson or depth not 4-byte aligned, or more than 2^24 cells per pair; frame sizes as ofdis_get_flow_fullres checks
+ * them.  The workspace -- per cell and pair 22.5 bytes (the correspondence, its flag, the refit's 22 chunk sums per
+ * 32 cells), per hypothesis and pair 120 (its float64 E and the float32 F record) and 176 per pair -- is allocated on
+ * the first call, grows, never shrinks and is freed by ofdis_destroy.  Enqueued on the context's stream as 5 kernels,
+ * plus one when a per-pixel output is asked for, whatever the number of pairs; the call synchronises the stream once,
+ * at the end, for pose and stats.  Not part of ofdis_run's graph; the flows are not changed. */
+typedef struct ofdis_relpose_params {
+  float fx, fy, cx, cy;      /* pinhole intrinsics of both frames; finite, fx, fy > 0 */
+  int step;                  /* correspondence grid step s >= 1, as ofdis_global_motion_fullres */
+  int fb_check;              /* 0 | 1: only correspondences whose consistency mask against slot b0+k is 0 */
+  float alpha, beta;         /* the rule of ofdis_consistency_fullres; finite, >= 0 */
+  int hypotheses;            /* 1 .. 65536 */
+  float threshold;           /* inlier Sampson distance in pixels; finite, > 0 */
+  int refine;                /* 0 .. 16 Gauss-Newton rounds on the inliers */
+  float min_parallax;        /* pixels, finite, >= 0: below it status 3 */
+  unsigned long long seed;
+} ofdis_relpose_params;
+int ofdis_relpose_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_relpose_params* p, double* pose,
+                          ofdis_motion_stats* stats, unsigned char* mask, float* sampson, float* depth,
+                          int width_org, int height_org, int memkind);
+
 /* Volumetric fusion (extension): a truncated signed distance function (TSDF; Curless and Levoy, SIGGRAPH 1996;
  * KinectFusion, Newcombe et al., ISMAR 2011) integrated from a clip's disparity maps and camera poses, its zero
  * crossings as surface points and its depth rendered by ray casting.  The context owns one volume: T, W and, with

@@ -15,7 +15,7 @@ import numpy as np
 
 from .params import CParams, DisParams
 from .preprocess import (CONF_PARAM_FIELDS, DISP_FILTER_FIELDS, EGO_PARAM_FIELDS, FUSE_PARAM_FIELDS, FUSE_POINT_DTYPE,
-                         FUSE_TRACK_PARAM_FIELDS, FUSE_TRACK_STATS_DTYPE, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, SF_STATS_DTYPE,
+                         FUSE_TRACK_PARAM_FIELDS, FUSE_TRACK_STATS_DTYPE, FISHER_MAX_BLOCKS, FISHER_STATS_DTYPE, MOTION_PARAM_FIELDS, MOTION_STATS_DTYPE, RELPOSE_PARAM_FIELDS, SF_STATS_DTYPE,
                          STAB_FRAME_DTYPE, STAB_PARAM_FIELDS, STEREO_CAMERA_FIELDS, TRACK_PARAM_FIELDS,
                          TRACK_POINT_DTYPE, TRACK_STATS_FIELDS, TRAJ_PARAM_FIELDS, TRAJ_RECORD_DTYPE, TRAJ_STATS_FIELDS,
                          fisher_fit, fisher_pack, fisher_sizes, gaussian_weights, motion_params,
@@ -47,7 +47,7 @@ EXPORTS = [
     "ofdis_fisher_begin", "ofdis_fisher_push", "ofdis_fisher_take", "ofdis_traj_advance_fisher",
     "ofdis_egomotion_fullres", "ofdis_fuse_begin", "ofdis_fuse_push", "ofdis_fuse_extract", "ofdis_fuse_render",
     "ofdis_fuse_get_volume", "ofdis_fuse_set_volume", "ofdis_fuse_mesh", "ofdis_fuse_track",
-    "ofdis_confidence_fullres", "ofdis_fuse_push_weighted", "ofdis_fuse_track_weighted",
+    "ofdis_confidence_fullres", "ofdis_fuse_push_weighted", "ofdis_fuse_track_weighted", "ofdis_relpose_fullres",
 ]
 
 # outputs of disparity_fullres, in the C-ABI's argument order
@@ -58,6 +58,9 @@ SF_OUTPUTS = ("disp1", "status", "motion")
 
 # per-pixel outputs of egomotion_fullres, in the C-ABI's argument order
 EGO_OUTPUTS = ("mask", "residual", "object_motion")
+
+# per-pixel outputs of relpose_fullres, in the C-ABI's argument order
+RELPOSE_OUTPUTS = ("mask", "sampson", "depth")
 
 # encodings of get_flow_fullres_encoded (OFDIS_ENC_F16, OFDIS_ENC_KITTI)
 ENCODINGS = {"f16": 1, "kitti": 2}
@@ -128,6 +131,17 @@ class EgoParams(ctypes.Structure):
 
 
 assert tuple(k for k, _ in EgoParams._fields_) == EGO_PARAM_FIELDS
+
+
+class RelposeParams(ctypes.Structure):
+    """ofdis_relpose_params (include/ofdis_b200.h)."""
+    _fields_ = [(k, ctypes.c_float) for k in ("fx", "fy", "cx", "cy")] + \
+        [("step", ctypes.c_int), ("fb_check", ctypes.c_int), ("alpha", ctypes.c_float), ("beta", ctypes.c_float),
+         ("hypotheses", ctypes.c_int), ("threshold", ctypes.c_float), ("refine", ctypes.c_int),
+         ("min_parallax", ctypes.c_float), ("seed", ctypes.c_ulonglong)]
+
+
+assert tuple(k for k, _ in RelposeParams._fields_) == RELPOSE_PARAM_FIELDS
 
 
 class FuseParams(ctypes.Structure):
@@ -282,6 +296,8 @@ def lib():
         L.ofdis_egomotion_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
             [ctypes.POINTER(EgoParams)] + [ctypes.c_void_p] * 2 + [ctypes.c_size_t, ctypes.POINTER(StereoCamera)] + \
             [ctypes.c_void_p] * 5 + [ctypes.c_int] * 3
+        L.ofdis_relpose_fullres.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + \
+            [ctypes.POINTER(RelposeParams)] + [ctypes.c_void_p] * 5 + [ctypes.c_int] * 3
         L.ofdis_track_stats_get.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackStats)]
         L.ofdis_traj_begin.argtypes = [ctypes.c_void_p, ctypes.POINTER(TrackParams), ctypes.POINTER(TrajParams)] + \
             [ctypes.c_void_p] * 3 + [ctypes.c_int] * 3
@@ -753,6 +769,42 @@ class Context:
         self._ck(lib().ofdis_egomotion_fullres(self._h, f0, f1, -1 if b0 is None else b0, ctypes.byref(params),
                                                _ptr(disp0), _ptr(disp1), disp_stride, cam, _ptr(pose), _ptr(stats),
                                                *ptrs, width_org, height_org, memkind))
+        return pose, stats, {k: out.get(k) for k in outputs}
+
+    def relpose_fullres(self, f0, f1, params, *, width_org, height_org, b0=None, outputs=(), out=None,
+                        memkind=MEM_HOST):
+        """The monocular relative pose of the last run's flow slots [f0, f1) (ofdis_relpose_fullres; preprocess.relpose
+        restates it): one essential-matrix fit per pair with one calibrated camera, camera t to camera t+1 with a unit
+        translation.  params: a mapping with preprocess.RELPOSE_PARAM_FIELDS or a RelposeParams; b0: the partner slots
+        of fb_check.  outputs: any of RELPOSE_OUTPUTS ("mask" uint8, "sampson" and "depth" float32, each (n, H, W)).
+        Returns (pose (n, 3, 4) float64, stats (n,) of MOTION_STATS_DTYPE, outs), pose and stats always on the host;
+        the call synchronises the stream.  Host: the outputs new or given in `out` as numpy arrays of exactly their
+        dtype and shape.  With memkind=MEM_DEVICE every output is a device address the caller owns."""
+        unknown = set(outputs) - set(RELPOSE_OUTPUTS)
+        if unknown:
+            raise ValueError("relpose_fullres: unknown outputs %s" % sorted(unknown))
+        if not isinstance(params, RelposeParams):
+            params = RelposeParams(*[params[k] for k in RELPOSE_PARAM_FIELDS])
+        n = max(f1 - f0, 0)
+        shape = (n, height_org, width_org)
+        out = dict(out or {})
+        if memkind == MEM_HOST:
+            for name in outputs:
+                dt = np.uint8 if name == "mask" else np.float32
+                arr = out.setdefault(name, np.empty(shape, dt))
+                if not (isinstance(arr, np.ndarray) and arr.dtype == dt and arr.shape == shape
+                        and arr.flags["C_CONTIGUOUS"] and arr.flags["WRITEABLE"]):
+                    raise ValueError("relpose_fullres: %s must be a writeable C-contiguous %s array of shape %s"
+                                     % (name, np.dtype(dt).name, shape))
+        else:
+            missing = [name for name in outputs if out.get(name) is None]
+            if missing:
+                raise ValueError("relpose_fullres: no device address for the requested outputs %s" % missing)
+        pose = np.empty((n, 3, 4), np.float64)
+        stats = np.zeros(n, MOTION_STATS_DTYPE)
+        ptrs = [_ptr(out.get(k)) if k in outputs else None for k in RELPOSE_OUTPUTS]
+        self._ck(lib().ofdis_relpose_fullres(self._h, f0, f1, -1 if b0 is None else b0, ctypes.byref(params),
+                                             _ptr(pose), _ptr(stats), *ptrs, width_org, height_org, memkind))
         return pose, stats, {k: out.get(k) for k in outputs}
 
     def flow_error_fullres(self, f0, f1, gt, width_org, height_org, classes=None, nclasses=None, with_err=False,

@@ -19,7 +19,7 @@ LIB = os.path.join(LIBDIR, "libofdis_b200.so")
 SOURCES = ["ofdis_capi.cu", "patch_kernels.cu", "pyramid_kernels.cu", "varref_kernels.cu", "interp_kernels.cu",
            "track_kernels.cu", "disparity_kernels.cu", "motion_kernels.cu", "stab_kernels.cu",
            "traj_kernels.cu", "sceneflow_kernels.cu", "fisher_kernels.cu", "egomotion_kernels.cu",
-           "fusion_kernels.cu", "fusetrack_kernels.cu", "confidence_kernels.cu"]
+           "fusion_kernels.cu", "fusetrack_kernels.cu", "confidence_kernels.cu", "relpose_kernels.cu"]
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",

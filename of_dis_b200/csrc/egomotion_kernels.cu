@@ -177,9 +177,7 @@ __global__ void __launch_bounds__(kHypThreads) ego_hyp_kernel(EgoGeom eg, EgoWor
     double P[3][3], Q[3][3];
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
-      const unsigned long long z =
-          splitmix64(eg.seed + (unsigned long long)(8 * h + d + 1) * 0x9E3779B97F4A7C15ull);
-      const unsigned idx = (unsigned)(((z >> 32) * (unsigned long long)m) >> 32);
+      const unsigned idx = motion_draw(eg.seed, h, d, m);
       const EgoCorr c = corr[idx];
       float X1, Y1, Z1;
       ego_q(eg.cam, c.a.w, c.b.x, c.b.z, X1, Y1, Z1);
@@ -385,15 +383,7 @@ __global__ void __launch_bounds__(kRefitThreads) ego_refit_kernel(EgoGeom eg, Eg
     atomicAdd(&count, local);
     __syncthreads();
     if (!acc || count < 3) break;  // uniform: every thread reads the same shared values
-    // the pairwise tree over the chunk sums, padded with +0.0 to P leaves, in place: v_j += v_(j + stride)
-    for (int stride = 1; stride < P; stride <<= 1) {
-      for (int j = threadIdx.x * 2 * stride; j < nc; j += kRefitThreads * 2 * stride) {
-        const int o = j + stride;
-        for (int e = 0; e < EGO_NE; ++e)
-          chunk[(size_t)j * EGO_NE + e] = chunk[(size_t)j * EGO_NE + e] + (o < nc ? chunk[(size_t)o * EGO_NE + e] : 0.0);
-      }
-      __syncthreads();
-    }
+    refit_tree<EGO_NE>(chunk, nc, P, kRefitThreads);
     if (threadIdx.x == 0) {
       double A[6][6], b[6], x[6];
       int e = 0;

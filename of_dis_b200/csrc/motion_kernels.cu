@@ -4,30 +4,24 @@
 //   motion_corr_kernel     one thread per (cell, pair): the validity flag and the normalized correspondence;
 //   motion_compact_kernel  one CTA per pair: a block scan over the cells in tiles, compacting in place in cell order;
 //   motion_hyp_kernel      one thread per (hypothesis, pair): the draws and the float64 elimination;
-//   motion_score_kernel    the hot path: the pair's correspondences stream through shared memory in 64 KB tiles
-//                          (cp.async.bulk + mbarrier, two buffers); each warp tests 4 hypotheses per shared read and
-//                          takes one 64-bit atomicMax per hypothesis;
+//   motion_score_kernel    the hot path (motion_score.cuh, shared with relative pose): the pair's correspondences
+//                          stream through shared memory in 64 KB tiles; each warp tests 4 hypotheses per shared read
+//                          and takes one 64-bit atomicMax per hypothesis;
 //   motion_refit_kernel    one CTA per pair: every refit round (inlier test, chunk sums, tree, solve) and the model;
 //   motion_apply_kernel    one thread per pixel: residual, mask and registered bytes (only when asked for).
 // The flows are read through upsample_at / consistency_at; no full-resolution copy is stored.  float32 and float64
 // without contraction (-fmad=false), IEEE division.
 #include <cuda_runtime.h>
 
-#include "bulk_tile.cuh"
-#include "ofdis_internal.cuh"
+#include "motion_score.cuh"
 
 namespace ofdis {
 
 namespace {
 
-using namespace tiles;
-
 constexpr int kCorrThreads = 256;
 constexpr int kCompactThreads = 1024;
 constexpr int kHypThreads = 128;
-constexpr int kScoreWarps = 16, kScoreHpw = 4, kScoreHpb = kScoreWarps * kScoreHpw;  // hypotheses per warp / CTA
-constexpr int kTile = 4096;                                                          // float4 per 64 KB tile
-constexpr size_t kScoreSmem = 2 * kTile * sizeof(float4) + 16;                       // two tiles, two mbarriers
 constexpr int kRefitThreads = 256;
 constexpr int kChunk = 32;
 
@@ -139,9 +133,7 @@ __global__ void __launch_bounds__(kHypThreads) motion_hyp_kernel(MotionGeom mg, 
     double A[K][K], b[K];
 #pragma unroll
     for (int d = 0; d < N; ++d) {
-      const unsigned long long z =
-          splitmix64(mg.seed + (unsigned long long)(8 * h + d + 1) * 0x9E3779B97F4A7C15ull);
-      const unsigned idx = (unsigned)(((z >> 32) * (unsigned long long)m) >> 32);
+      const unsigned idx = motion_draw(mg.seed, h, d, m);
       motion_rows<MODEL>(corr[idx], A[2 * d], A[2 * d + 1], b[2 * d], b[2 * d + 1]);
     }
     ok = motion_solve<K>(A, b, x);
@@ -173,73 +165,11 @@ __device__ __forceinline__ int motion_inlier(const float* g, float4 c, float t) 
   return (ex * ex + ey * ey <= t * t) ? 1 : 0;
 }
 
+// the scoring kernel's inlier tests of the similarity and affine map (PERSP false) and the homography (true)
 template <bool PERSP>
-__global__ void __launch_bounds__(kScoreWarps * 32, 1) motion_score_kernel(MotionGeom mg, MotionWork ws) {
-  extern __shared__ __align__(16) float4 tiles[];  // [2][kTile], then two mbarriers
-  const int k = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int m = ws.m[k];
-  if (m < mg.n_min) return;  // no solvable hypothesis (uniform over the CTA)
-  const int h0 = blockIdx.x * kScoreHpb + warp * kScoreHpw;
-  float g[kScoreHpw][9];
-  bool ok[kScoreHpw];
-#pragma unroll
-  for (int i = 0; i < kScoreHpw; ++i) {
-    const int h = h0 + i;
-    ok[i] = false;
-    for (int e = 0; e < 9; ++e) g[i][e] = 0.f;
-    if (h < mg.nh) {
-      const MotionHyp& r = ws.hg[(size_t)k * mg.hyp_cap + h];
-      ok[i] = r.ok != 0;
-#pragma unroll
-      for (int e = 0; e < 9; ++e) g[i][e] = r.g[e];
-    }
-  }
-  const unsigned buf0 = smem_u32(tiles), mbar0 = buf0 + 2u * kTile * sizeof(float4);
-  const float4* src = ws.corr + (size_t)k * mg.cell_cap;
-  const int ntiles = (m + kTile - 1) / kTile;
-  auto issue = [&](int t) {
-    const int cnt = min(kTile, m - t * kTile);
-    bulk_tile(buf0 + (unsigned)(t & 1) * kTile * sizeof(float4), src + (size_t)t * kTile, (unsigned)cnt * 16u,
-              mbar0 + 8u * (t & 1));
-  };
-  if (threadIdx.x == 0) {
-    mbar_init(mbar0, 1);
-    mbar_init(mbar0 + 8, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    issue(0);
-    if (ntiles > 1) issue(1);
-  }
-  int cnt[kScoreHpw];
-#pragma unroll
-  for (int i = 0; i < kScoreHpw; ++i) cnt[i] = 0;
-  const float t = mg.t;
-  for (int tt = 0; tt < ntiles; ++tt) {
-    const int b = tt & 1;
-    mbar_wait(mbar0 + 8u * b, (unsigned)(tt >> 1) & 1u);
-    const float4* tile = tiles + b * kTile;
-    const int n_in = min(kTile, m - tt * kTile);
-#pragma unroll 4
-    for (int e = lane; e < n_in; e += 32) {
-      const float4 c = tile[e];
-#pragma unroll
-      for (int i = 0; i < kScoreHpw; ++i) cnt[i] += motion_inlier<PERSP>(g[i], c, t);
-    }
-    __syncthreads();  // every warp is done with buffer b
-    if (threadIdx.x == 0 && tt + 2 < ntiles) {
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      issue(tt + 2);
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < kScoreHpw; ++i) {
-    const unsigned total = __reduce_add_sync(0xffffffffu, (unsigned)cnt[i]);
-    if (lane == 0 && ok[i])
-      atomicMax(ws.key + k, ((unsigned long long)total << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)(h0 + i)));
-  }
-}
+struct MotionTest {
+  static __device__ __forceinline__ int inlier(const float* g, float4 c, float t) { return motion_inlier<PERSP>(g, c, t); }
+};
 
 // ---- 5. refits and the model -------------------------------------------------------------------------------------------
 template <int MODEL>
@@ -412,25 +342,27 @@ template <int MODEL>
 int launch_model(const MotionGeom& mg, const MotionWork& ws, int n, cudaStream_t st) {
   motion_hyp_kernel<MODEL><<<dim3((mg.nh + kHypThreads - 1) / kHypThreads, n), kHypThreads, 0, st>>>(mg, ws);
   if (cudaGetLastError() != cudaSuccess) return -1;
-  auto score = MODEL == OFDIS_MOTION_HOMOGRAPHY ? motion_score_kernel<true> : motion_score_kernel<false>;
-  if (smem_optin((const void*)score, kScoreSmem, false) != cudaSuccess) return -1;
-  score<<<dim3((mg.nh + kScoreHpb - 1) / kScoreHpb, n), kScoreWarps * 32, kScoreSmem, st>>>(mg, ws);
-  if (cudaGetLastError() != cudaSuccess) return -1;
+  if (launch_motion_score<MotionTest<MODEL == OFDIS_MOTION_HOMOGRAPHY>>(mg, ws, n, st) < 0) return -1;
   motion_refit_kernel<MODEL><<<n, kRefitThreads, 0, st>>>(mg, ws);
   return cudaGetLastError() == cudaSuccess ? 3 : -1;
 }
 
 }  // namespace
 
-int launch_global_motion(const LevelGeom& g, int fa, int fb, int n, const MotionGeom& mg, const MotionWork& ws,
-                         const MotionOutputs& o, cudaStream_t st) {
-  if (g.nop != 2 || (mg.noc != 1 && mg.noc != 3)) return -1;
+int launch_motion_corr(const LevelGeom& g, int fa, int fb, int n, const MotionGeom& mg, const MotionWork& ws,
+                       cudaStream_t st) {
   const dim3 cgrid((mg.cells + kCorrThreads - 1) / kCorrThreads, n);
   if (mg.fb_check) motion_corr_kernel<true><<<cgrid, kCorrThreads, 0, st>>>(g, fa, fb, mg, ws);
   else motion_corr_kernel<false><<<cgrid, kCorrThreads, 0, st>>>(g, fa, fb, mg, ws);
   if (cudaGetLastError() != cudaSuccess) return -1;
   motion_compact_kernel<<<n, kCompactThreads, 0, st>>>(mg, ws);
-  if (cudaGetLastError() != cudaSuccess) return -1;
+  return cudaGetLastError() == cudaSuccess ? 2 : -1;
+}
+
+int launch_global_motion(const LevelGeom& g, int fa, int fb, int n, const MotionGeom& mg, const MotionWork& ws,
+                         const MotionOutputs& o, cudaStream_t st) {
+  if (g.nop != 2 || (mg.noc != 1 && mg.noc != 3)) return -1;
+  if (launch_motion_corr(g, fa, fb, n, mg, ws, st) < 0) return -1;
   const int l = mg.model == OFDIS_MOTION_SIMILARITY ? launch_model<OFDIS_MOTION_SIMILARITY>(mg, ws, n, st)
                 : mg.model == OFDIS_MOTION_AFFINE   ? launch_model<OFDIS_MOTION_AFFINE>(mg, ws, n, st)
                                                     : launch_model<OFDIS_MOTION_HOMOGRAPHY>(mg, ws, n, st);

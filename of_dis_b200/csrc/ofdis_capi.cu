@@ -128,6 +128,12 @@ struct ofdis_ctx {
   DevBuf d_ego;
   size_t ego_cells = 0, ego_hyps = 0;
   EgoWork ego{};
+  // ofdis_relpose_fullres (global motion's MotionWork layout with float64 E per hypothesis and RELPOSE_NE chunk sums,
+  // then the RelposeOut records, for max_frames pairs of relpose_cells cells and relpose_hyps hypotheses)
+  DevBuf d_relpose;
+  size_t relpose_cells = 0, relpose_hyps = 0;
+  MotionWork relpose{};
+  RelposeOut* relpose_out = nullptr;
   // the stabiliser of ofdis_stab_begin / ofdis_stab_push / ofdis_stab_finish: its workspace (StabWork: the frame ring,
   // the model ring, the per-frame records), the geometry and weights of the last begin, L and the next frame to emit
   DevBuf d_stab;
@@ -568,7 +574,7 @@ int ofdis_destroy(ofdis_ctx* ctx) {
   for (auto& kv : ctx->graphs) cudaGraphExecDestroy(kv.second);
   cudaFree(ctx->d_swapped);  // d_img lies in the same allocation
   for (DevBuf* b : {&ctx->d_stage, &ctx->d_full, &ctx->d_eval, &ctx->d_color, &ctx->d_interp, &ctx->d_track,
-                    &ctx->d_disp, &ctx->d_sf, &ctx->d_motion, &ctx->d_ego, &ctx->d_traj, &ctx->d_stab, &ctx->d_fisher,
+                    &ctx->d_disp, &ctx->d_sf, &ctx->d_motion, &ctx->d_ego, &ctx->d_relpose, &ctx->d_traj, &ctx->d_stab, &ctx->d_fisher,
                     &ctx->d_fuse, &ctx->d_mesh, &ctx->d_ftrack})
     cudaFree(b->p);
   for (float* p : ctx->d_flow) cudaFree(p);
@@ -1472,6 +1478,95 @@ int ofdis_egomotion_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_
   }
   std::vector<EgoOut> res(n);
   CK(cudaMemcpyAsync(res.data(), ctx->ego.out, sizeof(EgoOut) * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (int q = 0; q < n; ++q) {
+    std::memcpy(pose + 12 * (size_t)q, res[q].pose, sizeof(res[q].pose));
+    stats[q] = res[q].st;
+  }
+  return OFDIS_OK;
+}
+
+// The workspace of ofdis_relpose_fullres for max_frames pairs of at least `cells` cells and `hyps` hypotheses: per cell
+// the correspondence (16 bytes), its flag (1) and the refit's chunk sums (21 doubles per 32 cells); per hypothesis its
+// float64 E (72) and MotionHyp (48); per pair RelposeOut, the key and the count.  The cell and hypothesis capacities
+// grow independently, never shrink.
+static int ensure_relpose(ofdis_ctx* ctx, size_t cells, size_t hyps) {
+  cells = std::max((cells + 31) / 32 * 32, ctx->relpose_cells);
+  hyps = std::max(hyps, ctx->relpose_hyps);
+  const size_t n = (size_t)ctx->max_frames;
+  MotionWork& ws = ctx->relpose;
+  const int rc = carve(ctx, ctx->d_relpose, "relpose_fullres workspace", [&](Carve& c) {
+    ws.corr = c.take<float4>(n * cells);
+    ws.chunk = c.take<double>(n * (cells / 32) * RELPOSE_NE);
+    ws.hp = c.take<double>(n * hyps * 9);
+    ws.hg = c.take<MotionHyp>(n * hyps);
+    ctx->relpose_out = c.take<RelposeOut>(n);
+    ws.key = c.take<unsigned long long>(n);
+    ws.m = c.take<int>(n);
+    ws.flag = c.take<unsigned char>(n * cells);
+  });
+  ctx->relpose_cells = rc ? 0 : cells;
+  ctx->relpose_hyps = rc ? 0 : hyps;
+  return rc;
+}
+
+int ofdis_relpose_fullres(ofdis_ctx* ctx, int f0, int f1, int b0, const ofdis_relpose_params* p, double* pose,
+                          ofdis_motion_stats* stats, unsigned char* mask, float* sampson, float* depth, int width_org,
+                          int height_org, int memkind) {
+  static_assert(sizeof(RelposeOut) == 160, "relpose record");
+  if (!ctx) return OFDIS_ERR_ARG;
+  const bool dev = memkind == OFDIS_MEM_DEVICE;
+  auto misaligned = [dev](const float* q) { return dev && reinterpret_cast<uintptr_t>(q) % sizeof(float); };
+  if (ctx->nop != 2 || f0 < 0 || f1 > ctx->max_frames || f0 >= f1 || !p ||
+      (p->fb_check && (b0 < 0 || b0 > ctx->max_frames - (f1 - f0))) || p->step < 1 ||
+      (p->fb_check != 0 && p->fb_check != 1) || !finite_ge0(p->alpha) || !finite_ge0(p->beta) ||
+      !finite_gt0(p->fx) || !finite_gt0(p->fy) || !finite_f32(p->cx) || !finite_f32(p->cy) ||
+      p->hypotheses < 1 || p->hypotheses > 65536 || !finite_gt0(p->threshold) || p->refine < 0 || p->refine > 16 ||
+      !finite_ge0(p->min_parallax) || !pose || !stats || misaligned(sampson) || misaligned(depth))
+    return fail(ctx, OFDIS_ERR_ARG, "relpose_fullres: bad argument");
+  int cx, cy;
+  int rc = org_padding(ctx, width_org, height_org, &cx, &cy);
+  if (rc) return rc;
+  const size_t pix = (size_t)width_org * height_org;
+  const int s = p->step, ncx = (width_org - 1) / s + 1, ncy = (height_org - 1) / s + 1;
+  if ((long long)ncx * ncy > (1ll << 24)) return fail(ctx, OFDIS_ERR_ARG, "relpose_fullres: more than 2^24 cells");
+  NvtxRange nvtx("relpose", -1);
+  CK(cudaSetDevice(ctx->device));
+  const int n = f1 - f0, D = ctx->dirs;
+  const size_t np = pix * n;
+  rc = ensure_relpose(ctx, (size_t)ncx * ncy, (size_t)p->hypotheses);
+  if (rc) return rc;
+  RelposeGeom rg{};
+  MotionGeom& mg = rg.mg;
+  mg.w = width_org, mg.h = height_org, mg.s = s, mg.ncx = ncx, mg.cells = ncx * ncy, mg.model = 0;
+  mg.n_min = 8, mg.nh = p->hypotheses, mg.fb_check = p->fb_check, mg.refine = p->refine;
+  mg.crop_x = cx, mg.crop_y = cy, mg.noc = ctx->prm.noc, mg.alpha = p->alpha, mg.beta = p->beta;
+  mg.cx = 0.f, mg.cy = 0.f, mg.sigma = 1.f;  // global motion's correspondences in pixel coordinates
+  mg.t = p->threshold, mg.thr = p->threshold;
+  mg.seed = p->seed;
+  mg.cell_cap = ctx->relpose_cells, mg.chunk_cap = ctx->relpose_cells / 32, mg.hyp_cap = ctx->relpose_hyps;
+  rg.fx = p->fx, rg.fy = p->fy, rg.cx = p->cx, rg.cy = p->cy, rg.min_parallax = p->min_parallax;
+  RelposeOutputs o{mask, sampson, depth};
+  if (!dev && (mask || sampson || depth)) {
+    const size_t cap = pix * ctx->max_frames;
+    rc = carve_full(ctx, pix, [&](Carve& c) {
+      o.sampson = c.take<float>(cap, sampson);
+      o.depth = c.take<float>(cap, depth);
+      o.mask = c.take<unsigned char>(cap, mask);
+    });
+    if (rc) return rc;
+  }
+  const int k = launch_relpose(stepped(ctx->lev[0], D), f0 * D, (p->fb_check ? b0 : f0) * D, n, rg, ctx->relpose,
+                               ctx->relpose_out, o, ctx->stream);
+  if (k < 0) return fail(ctx, OFDIS_ERR_CUDA, "relpose kernel launch", cudaGetLastError());
+  ctx->launches += k;
+  if (!dev) {
+    if (sampson) CK(cudaMemcpyAsync(sampson, o.sampson, sizeof(float) * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (depth) CK(cudaMemcpyAsync(depth, o.depth, sizeof(float) * np, cudaMemcpyDeviceToHost, ctx->stream));
+    if (mask) CK(cudaMemcpyAsync(mask, o.mask, np, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  std::vector<RelposeOut> res(n);
+  CK(cudaMemcpyAsync(res.data(), ctx->relpose_out, sizeof(RelposeOut) * n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   for (int q = 0; q < n; ++q) {
     std::memcpy(pose + 12 * (size_t)q, res[q].pose, sizeof(res[q].pose));

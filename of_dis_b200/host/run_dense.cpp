@@ -698,6 +698,20 @@ int main(int argc, char** argv) {
 // --odometry, a list that does not match the clips or a file with too few lines, and a DIR that cannot be written.
 // Every other output keeps its bytes.
 //
+// --mono-odometry DIR with --intrinsics fx,fy,cx,cy (flow binaries only): the monocular relative pose of every pair
+// (ofdis_relpose_fullres) with step 8, 1024 hypotheses, a 1 px Sampson threshold, 5 Gauss-Newton rounds, a 0.5 px
+// parallax guard and seed 0; with --bidirectional only correspondences whose forward consistency mask is 0.
+// DIR/monodometry.txt gets one line per pair, `clip frame status` and the 12 numbers of [R | t] with |t| = 1 (camera
+// t to camera t+1, row-major, %.17g, NaN unless status 0); DIR/poses_<clip %04d>.txt the clip's camera-to-world poses
+// as --odometry writes them, chained with unit steps, or with --gt-poses with the ground truth's step lengths.  Every
+// pair gets <stem>_epimask.pgm (0 epipolar inlier, 255 outlier, 128 unknown) and <stem>_depthrel.pfm (1-channel PFM,
+// the depth at image1 in units of the step, NaN where unknown).  With --gt-poses and verbosity > 0 every pair prints
+// `MONOEVAL clip frame r_err t_dir_err` (degrees) and the end `MONOEVAL (<P> pairs) r_err <mean> t_dir_err <mean>`
+// over the pairs of status 0.  Refused before any device work: the stereo binaries, --warm-start, --mono-odometry
+// without --intrinsics or the reverse, intrinsics that are not four finite numbers with fx, fy > 0, and a DIR that
+// cannot be written.  --gt-poses is valid with --odometry or --mono-odometry; with both, the two share its poses
+// files and --mono-odometry's poses files are DIR/poses_<clip>.txt of its own DIR.
+//
 // --fuse voxel,trunc,x0,y0,z0,nx,ny,nz (needs --odometry, whose poses place the disparities): one TSDF volume per clip
 // of --odometry (ofdis_fuse_begin / ofdis_fuse_push / ofdis_fuse_extract), nx x ny x nz voxels of `voxel` metres from
 // (x0, y0, z0) in the clip's first camera, truncation `trunc` metres, max_weight 64, max_depth +inf, with colour.  The
@@ -1186,11 +1200,14 @@ struct Options {
   const char* sf_gtlist = nullptr;                    // --gt-scene-flow GTLIST
   const char* odo_dir = nullptr;                      // --odometry DIR
   const char* odo_gtlist = nullptr;                   // --gt-poses LIST
+  const char* mono_dir = nullptr;                     // --mono-odometry DIR
+  const char* intrinsics = nullptr;                   // --intrinsics fx,fy,cx,cy
   const char* fuse = nullptr;                         // --fuse voxel,trunc,x0,y0,z0,nx,ny,nz
   const char* conf_arg = nullptr;                     // --confidence R
   int nnum = 0;                                       // the operating point or the 20 parameters after the flags
   char** nums = nullptr;
 
+  ofdis_relpose_params rpp{};  // --intrinsics: the parameters of --mono-odometry
   int maxb = 64;
   float color_max = 0.0f;   // 0: every pair's own maximum
   float interp_t = 0.0f;
@@ -1244,6 +1261,8 @@ static int parse_flags(int argc, char** argv, Options& o) {
       {"--fuse", 1, &o.fuse, nullptr, "voxel,trunc,x0,y0,z0,nx,ny,nz"},
       {"--mesh", 0, nullptr, &o.mesh, nullptr},
       {"--gt-poses", 1, &o.odo_gtlist, nullptr, "one list of KITTI poses files"},
+      {"--mono-odometry", 1, &o.mono_dir, nullptr, "one output directory"},
+      {"--intrinsics", 1, &o.intrinsics, nullptr, "fx,fy,cx,cy"},
       {"--gt", 1, &o.gtlist, nullptr, "one ground-truth list file"},
       {"--confidence", 1, &o.conf_arg, nullptr, "one window radius"},
   };
@@ -1362,6 +1381,31 @@ static int read_camera(Options& o) {
   return 0;
 }
 
+static int read_intrinsics(Options& o) {
+  float v[4];
+  const char* q = o.intrinsics;
+  bool ok = true;
+  for (int i = 0; i < 4 && ok; ++i) {
+    char* end = nullptr;
+    v[i] = strtof(q, &end);
+    ok = end != q && (i < 3 ? *end == ',' : *end == 0) && v[i] >= -FLT_MAX && v[i] <= FLT_MAX;
+    q = end + (i < 3 ? 1 : 0);
+  }
+  if (!ok || !(v[0] > 0.0f) || !(v[1] > 0.0f))
+    return refuse(2, "--intrinsics takes four finite numbers fx,fy,cx,cy with fx and fy > 0, got %s", o.intrinsics);
+  memset(&o.rpp, 0, sizeof(o.rpp));
+  o.rpp.fx = v[0], o.rpp.fy = v[1], o.rpp.cx = v[2], o.rpp.cy = v[3];
+  o.rpp.step = 8;
+  o.rpp.alpha = 0.01f;
+  o.rpp.beta = 0.5f;
+  o.rpp.hypotheses = 1024;
+  o.rpp.threshold = 1.0f;
+  o.rpp.refine = 5;
+  o.rpp.min_parallax = 0.5f;
+  o.rpp.seed = 0;
+  return 0;
+}
+
 static int read_interpolate(Options& o) {
   char* end = nullptr;
   o.interp_t = strtof(o.interp_arg, &end);
@@ -1420,7 +1464,12 @@ static int check_options(Options& o) {
       {o.odo_dir != nullptr, "--odometry", kFlow, "--odometry fits the rig's motion from flows", true,
        o.sf_list && o.camera, "--odometry needs the disparities of --scene-flow and the stereo camera of --camera",
        nullptr},
-      {o.odo_gtlist != nullptr, "--gt-poses", kAny, nullptr, false, o.odo_dir != nullptr,
+      {o.mono_dir != nullptr, "--mono-odometry", kFlow, "--mono-odometry fits the camera's motion from flows", true,
+       o.intrinsics != nullptr, "--mono-odometry needs the camera intrinsics of --intrinsics", nullptr},
+      {o.intrinsics != nullptr, "--intrinsics", kFlow, "--intrinsics calibrates the camera of --mono-odometry", true,
+       o.mono_dir != nullptr, "--intrinsics calibrates the camera of --mono-odometry; give --mono-odometry too",
+       read_intrinsics},
+      {o.odo_gtlist != nullptr, "--gt-poses", kAny, nullptr, false, o.odo_dir != nullptr || o.mono_dir != nullptr,
        "--gt-poses evaluates the poses of --odometry; give --odometry too", nullptr},
       {o.fuse != nullptr, "--fuse", kFlow, "--fuse places disparities with the poses of --odometry", true,
        o.odo_dir != nullptr, "--fuse places disparities with the poses of --odometry; give --odometry too", read_fuse},
@@ -1570,7 +1619,7 @@ struct ListOutputs {
     FILE* f = nullptr;
     string path;
   };
-  File odo, desc, fisher, tracks, stab, gm;
+  File odo, desc, fisher, tracks, stab, gm, mono;
 
   bool open(File& x, const string& path) {
     x.path = path;
@@ -1580,7 +1629,7 @@ struct ListOutputs {
   // The end of a run: stab.txt, tracks, descriptors, fisher, global motion and odometry.txt are closed in this order,
   // and the first that cannot be written is refused
   int close() {
-    for (File* x : {&stab, &tracks, &desc, &fisher, &gm, &odo}) {
+    for (File* x : {&stab, &tracks, &desc, &fisher, &gm, &odo, &mono}) {
       if (!x->f) continue;
       const bool ok = fclose(x->f) == 0;
       x->f = nullptr;
@@ -1589,7 +1638,7 @@ struct ListOutputs {
     return 0;
   }
   ~ListOutputs() {  // a refused run
-    for (File* x : {&stab, &tracks, &desc, &fisher, &gm, &odo})
+    for (File* x : {&stab, &tracks, &desc, &fisher, &gm, &odo, &mono})
       if (x->f) fclose(x->f);
   }
 };
@@ -1600,6 +1649,8 @@ struct ListOutputs {
 static int open_outputs(const Options& o, const vector<Job>& jobs, ListOutputs& out) {
   if (o.odo_dir && !out.open(out.odo, string(o.odo_dir) + "/odometry.txt"))
     return refuse(2, "--odometry: cannot write %s", out.odo.path.c_str());
+  if (o.mono_dir && !out.open(out.mono, string(o.mono_dir) + "/monodometry.txt"))
+    return refuse(2, "--mono-odometry: cannot write %s", out.mono.path.c_str());
   for (size_t k = 0; k < jobs.size() && o.traj_stage; ++k) {  // an N x N patch in every frame
     int iw = 0, ih = 0;
     if (!image_size(jobs[k].a.c_str(), iw, ih)) return refuse_pair(jobs[k]);
@@ -1662,6 +1713,7 @@ struct State {
     memset(eval_total.data(), 0, sizeof(ofdis_error_stats) * eval_total.size());
     memset(sf_total.data(), 0, sizeof(ofdis_sf_stats) * sf_total.size());
     if (o.odo_dir) odo_rel.resize(clips.count);
+    if (o.mono_dir) mono_rel.resize(clips.count);
   }
   const Options& o;
   const vector<Job>& jobs;
@@ -1687,6 +1739,13 @@ struct State {
   long long fpushed = 0, fskipped[OFDIS_FISHER_MAX_BLOCKS] = {0};
   int sclip = -1;  // --stabilize: the clip being stabilised (-1 none)
   vector<vector<double>> odo_rel;  // --odometry: per clip, 12 numbers per pair
+  vector<vector<double>> mono_rel;  // --mono-odometry: per clip, 12 numbers per pair (|t| = 1)
+  double mono_rerr = 0.0, mono_terr = 0.0;
+  size_t mono_eval = 0;
+  vector<ofdis_motion_stats> mono_stats;
+  vector<double> mono_pose;
+  vector<uint8_t> mono_mask;
+  vector<float> mono_depth;
   double odo_terr = 0.0, odo_rerr = 0.0;
   size_t odo_eval = 0;
   double fuse_T[12];    // --fuse: the chained pose of the clip's next image1
@@ -2182,6 +2241,61 @@ static int run_odometry(State& s, Batch& b) {
   return rc;
 }
 
+// The ground truth's relative motion of frames G0 -> G1 (camera-to-world): Q = inv(G1) G0, camera t to camera t+1
+static void gt_relative(const double* G0, const double* G1, double* Q) {
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) Q[4 * i + j] = G1[i] * G0[j] + G1[4 + i] * G0[4 + j] + G1[8 + i] * G0[8 + j];
+    Q[4 * i + 3] = G1[i] * (G0[3] - G1[3]) + G1[4 + i] * (G0[7] - G1[7]) + G1[8 + i] * (G0[11] - G1[11]);
+  }
+}
+
+// --mono-odometry: the camera's motion of every pair to monodometry.txt, <stem>_epimask.pgm and <stem>_depthrel.pfm;
+// --gt-poses its rotation and translation-direction errors
+static int run_mono(State& s, Batch& b) {
+  const int n = b.n, w = b.w, h = b.h;
+  const size_t pix = (size_t)w * h;
+  FILE* f = s.out.mono.f;
+  ofdis_relpose_params p = s.o.rpp;
+  p.fb_check = s.o.bidir ? 1 : 0;
+  s.mono_pose.resize((size_t)12 * n);
+  s.mono_stats.resize(n);
+  s.mono_mask.resize(n * pix);
+  s.mono_depth.resize(n * pix);
+  const int rc = ofdis_relpose_fullres(s.ctx.get(), 0, n, n, &p, s.mono_pose.data(), s.mono_stats.data(),
+                                       s.mono_mask.data(), nullptr, s.mono_depth.data(), w, h, OFDIS_MEM_HOST);
+  for (int k = 0; k < n && rc == OFDIS_OK; ++k) {
+    const int c = s.clips.clip[b.j0 + k], fr = s.clips.frame[b.j0 + k];
+    const ofdis_motion_stats& st = s.mono_stats[k];
+    const double* P = s.mono_pose.data() + (size_t)12 * k;
+    const string& out = s.jobs[b.j0 + k].out;
+    fprintf(f, "%d %d %d", c, fr, st.status);
+    for (int i = 0; i < 12; ++i) fprintf(f, " %.17g", P[i]);
+    fprintf(f, "\n");
+    s.mono_rel[c].insert(s.mono_rel[c].end(), P, P + 12);
+    save_mask_pgm(s.mono_mask.data() + k * pix, w, h, with_suffix(out, "_epimask", ".pgm").c_str());
+    save_pfm1(&s.mono_depth[k * pix], w, h, with_suffix(out, "_depthrel", ".pfm"));  // as _depth.pfm
+    if (!s.o.odo_gtlist || st.status != 0) continue;
+    const vector<double>& gt = s.in.odo_gt[c];
+    double Q[12];
+    gt_relative(&gt[(size_t)12 * fr], &gt[(size_t)12 * (fr + 1)], Q);
+    double tr = 0.0, dt = 0.0, nq = 0.0, np_ = 0.0;
+    for (int i = 0; i < 3; ++i) {
+      for (int j = 0; j < 3; ++j) tr += Q[4 * i + j] * P[4 * i + j];
+      dt += Q[4 * i + 3] * P[4 * i + 3];
+      nq += Q[4 * i + 3] * Q[4 * i + 3];
+      np_ += P[4 * i + 3] * P[4 * i + 3];
+    }
+    const double kDeg = 180.0 / 3.14159265358979323846;
+    const double re = acos(std::min(1.0, std::max(-1.0, 0.5 * (tr - 1.0)))) * kDeg;
+    const double te = acos(std::min(1.0, std::max(-1.0, dt / sqrt(nq * np_)))) * kDeg;
+    s.mono_rerr += re;
+    s.mono_terr += te;
+    ++s.mono_eval;
+    if (s.verbosity > 0) printf("MONOEVAL %d %d %.9g %.9g\n", c, fr, re, te);
+  }
+  return rc;
+}
+
 // --fuse: the end of a clip's volume, pushed with its last image2: the surface to DIR/fused_<clip>.ply, with --mesh
 // the triangle mesh to DIR/fused_<clip>_mesh.ply
 static int end_fuse_clip(State& s, const Batch& b, const ClipRun& r) {
@@ -2262,6 +2376,7 @@ static int run_stages(State& s, Batch& b) {
   if (rc == OFDIS_OK && o.gtlist) rc = run_eval(s, b);
   if (rc == OFDIS_OK && o.sf_list) rc = run_scene_flow(s, b);
   if (rc == OFDIS_OK && o.odo_dir) rc = run_odometry(s, b);
+  if (rc == OFDIS_OK && o.mono_dir) rc = run_mono(s, b);
   if (rc == OFDIS_OK && o.fuse) rc = run_fuse(s, b);
   return rc;
 }
@@ -2381,19 +2496,34 @@ static void write_outputs(State& s, const Batch& b) {
 }
 
 // --odometry: every clip's camera-to-world poses to DIR/poses_<clip>.txt
+// --mono-odometry: the same into its own DIR, each unit step scaled by the ground truth's step length with --gt-poses
 static int write_poses(const State& s) {
-  for (size_t c = 0; c < s.odo_rel.size(); ++c) {
-    char name[32];
-    snprintf(name, sizeof(name), "/poses_%04zu.txt", c);
-    const string path = string(s.o.odo_dir) + name;
-    FILE* f = fopen(path.c_str(), "w");
-    double T[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
-    for (size_t k = 0; f && k <= s.odo_rel[c].size() / 12; ++k) {
-      if (k > 0) chain_pose(T, &s.odo_rel[c][12 * (k - 1)]);
-      for (int i = 0; i < 12; ++i) fprintf(f, i ? " %.17g" : "%.17g", T[i]);
-      fprintf(f, "\n");
+  for (int mono = 0; mono < 2; ++mono) {
+    const vector<vector<double>>& rel = mono ? s.mono_rel : s.odo_rel;
+    for (size_t c = 0; c < rel.size(); ++c) {
+      char name[32];
+      snprintf(name, sizeof(name), "/poses_%04zu.txt", c);
+      const string path = string(mono ? s.o.mono_dir : s.o.odo_dir) + name;
+      FILE* f = fopen(path.c_str(), "w");
+      double T[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+      for (size_t k = 0; f && k <= rel[c].size() / 12; ++k) {
+        if (k > 0) {
+          double P[12];
+          memcpy(P, &rel[c][12 * (k - 1)], sizeof(P));
+          if (mono && s.o.odo_gtlist) {
+            const double* G0 = &s.in.odo_gt[c][12 * (k - 1)];
+            const double* G1 = G0 + 12;
+            const double dx = G1[3] - G0[3], dy = G1[7] - G0[7], dz = G1[11] - G0[11];
+            const double len = sqrt(dx * dx + dy * dy + dz * dz);
+            for (int i = 0; i < 3; ++i) P[4 * i + 3] *= len;
+          }
+          chain_pose(T, P);
+        }
+        for (int i = 0; i < 12; ++i) fprintf(f, i ? " %.17g" : "%.17g", T[i]);
+        fprintf(f, "\n");
+      }
+      if (!f || fclose(f) != 0) return refuse(1, "cannot write %s", path.c_str());
     }
-    if (!f || fclose(f) != 0) return refuse(1, "cannot write %s", path.c_str());
   }
   return 0;
 }
@@ -2422,9 +2552,12 @@ static void print_summary(const State& s, timeval& tv) {
     print_eval("", s.done, s.eval_total[0]);
     for (int c = 0; c < s.nclasses && o.bidir; ++c) print_eval(kClassNames[c], s.done, s.eval_total[1 + c]);
   }
-  if (o.odo_gtlist)
+  if (o.odo_dir && o.odo_gtlist)
     printf("ODOEVAL (%zu pairs) t_err %.9g r_err %.9g\n", s.odo_eval, s.odo_eval ? s.odo_terr / s.odo_eval : 0.0,
            s.odo_eval ? s.odo_rerr / s.odo_eval : 0.0);
+  if (o.mono_dir && o.odo_gtlist)
+    printf("MONOEVAL (%zu pairs) r_err %.9g t_dir_err %.9g\n", s.mono_eval,
+           s.mono_eval ? s.mono_rerr / s.mono_eval : 0.0, s.mono_eval ? s.mono_terr / s.mono_eval : 0.0);
   if (o.sf_gtlist) {
     print_sfeval("", s.done, s.sf_total[0]);
     for (int c = 0; c < s.nclasses && o.bidir; ++c) print_sfeval(kClassNames[c], s.done, s.sf_total[1 + c]);

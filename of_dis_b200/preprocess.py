@@ -1748,6 +1748,363 @@ def egomotion(F: np.ndarray, B: np.ndarray | None, disp0: np.ndarray, disp1: np.
             np.stack([o[4] for o in out]))
 
 
+# ---- monocular relative pose (ofdis_relpose_fullres) -----------------------------------------------------------------
+# ofdis_relpose_params, field for field; the stats are MOTION_STATS_DTYPE (status 3: too little parallax)
+RELPOSE_PARAM_FIELDS = ("fx", "fy", "cx", "cy", "step", "fb_check", "alpha", "beta", "hypotheses", "threshold",
+                        "refine", "min_parallax", "seed")
+RELPOSE_JACOBI_SWEEPS = 8
+
+
+def relpose_null(A: np.ndarray):
+    """The full-pivot null vector of ofdis_relpose_fullres's step 2 on a batch of systems A (s, 8, 9) float64: returns
+    (e (s, 9) unit vectors, ok (s,))."""
+    A = np.array(A, np.float64)
+    s = A.shape[0]
+    ar = np.arange(s)
+    perm = np.tile(np.arange(9), (s, 1))
+    ok = np.ones(s, bool)
+    with np.errstate(all="ignore"):
+        for j in range(8):
+            best = np.full(s, -1.0)
+            pr = np.full(s, j)
+            pc = np.full(s, j)
+            for i in range(j, 8):
+                for c in range(j, 9):
+                    a = np.abs(A[:, i, c])
+                    upd = a > best
+                    best = np.where(upd, a, best)
+                    pr = np.where(upd, i, pr)
+                    pc = np.where(upd, c, pc)
+            ok &= best > 0
+            rj, rp = A[ar, j].copy(), A[ar, pr].copy()
+            A[ar, pr], A[ar, j] = rj, rp
+            cj, cp = A[ar, :, j].copy(), A[ar, :, pc].copy()
+            A[ar, :, pc], A[ar, :, j] = cj, cp
+            qj, qp = perm[ar, j].copy(), perm[ar, pc].copy()
+            perm[ar, pc], perm[ar, j] = qj, qp
+            for i in range(j + 1, 8):
+                f = A[:, i, j] / A[:, j, j]
+                A[:, i, j + 1:] = A[:, i, j + 1:] - f[:, None] * A[:, j, j + 1:]
+        y = np.zeros((s, 9))
+        y[:, 8] = 1.0
+        for i in range(7, -1, -1):
+            v = -A[:, i, 8]
+            for c in range(i + 1, 8):
+                v = v - A[:, i, c] * y[:, c]
+            y[:, i] = v / A[:, i, i]
+        e = np.zeros((s, 9))
+        e[ar[:, None], perm] = y
+        n2 = np.zeros(s)
+        for d in range(9):
+            n2 = n2 + e[:, d] * e[:, d]
+        e = e / np.sqrt(n2)[:, None]
+    return e, ok & np.isfinite(e).all(axis=1)
+
+
+def relpose_fmat(E: np.ndarray, fx, fy, cx, cy) -> np.ndarray:
+    """F = K^-T E K^-1 of E (..., 9) float64 in the header's expression order, rounded to float32."""
+    ifx, ify = 1.0 / float(np.float32(fx)), 1.0 / float(np.float32(fy))
+    ux, uy = -(float(np.float32(cx)) * ifx), -(float(np.float32(cy)) * ify)
+    E = np.asarray(E, np.float64)
+    G = [None] * 9
+    for i in range(3):
+        G[3 * i] = E[..., 3 * i] * ifx
+        G[3 * i + 1] = E[..., 3 * i + 1] * ify
+        G[3 * i + 2] = ((E[..., 3 * i] * ux) + (E[..., 3 * i + 1] * uy)) + E[..., 3 * i + 2]
+    F = [None] * 9
+    for j in range(3):
+        F[j] = ifx * G[j]
+        F[3 + j] = ify * G[3 + j]
+        F[6 + j] = ((ux * G[j]) + (uy * G[3 + j])) + G[6 + j]
+    return np.stack(F, -1).astype(np.float32)
+
+
+def relpose_sampson(g: np.ndarray, c: np.ndarray, threshold):
+    """Step 3's test, float32: g (..., 9) against pixel correspondences c (m, 4) (px, py, xs, ys).  Returns (inlier,
+    e, den), each (..., m)."""
+    f32 = np.float32
+    g = np.asarray(g, f32)[..., None, :]
+    x, y, xs, ys = c[:, 0], c[:, 1], c[:, 2], c[:, 3]
+    with np.errstate(all="ignore"):
+        a0 = (g[..., 0] * x + g[..., 1] * y) + g[..., 2]
+        a1 = (g[..., 3] * x + g[..., 4] * y) + g[..., 5]
+        a2 = (g[..., 6] * x + g[..., 7] * y) + g[..., 8]
+        b0 = (g[..., 0] * xs + g[..., 3] * ys) + g[..., 6]
+        b1 = (g[..., 1] * xs + g[..., 4] * ys) + g[..., 7]
+        e = (xs * a0 + ys * a1) + a2
+        den = (a0 * a0 + a1 * a1) + (b0 * b0 + b1 * b1)
+        t = f32(threshold)
+        return e * e <= (t * t) * den, e, den
+
+
+def _relpose_norm(c: np.ndarray, p: dict):
+    f32 = np.float32
+    fx, fy, cx, cy = (f32(p[k]) for k in ("fx", "fy", "cx", "cy"))
+    return (c[..., 0] - cx) / fx, (c[..., 1] - cy) / fy, (c[..., 2] - cx) / fx, (c[..., 3] - cy) / fy
+
+
+def _unit3(a):
+    """a / |a| in float64 scalars: a zero or non-finite a gives NaN or inf as on the device."""
+    a = [np.float64(v) for v in a]
+    with np.errstate(all="ignore"):
+        L = np.sqrt((a[0] * a[0] + a[1] * a[1]) + a[2] * a[2])
+        return [a[0] / L, a[1] / L, a[2] / L]
+
+
+def relpose_decompose(E) -> tuple:
+    """The four (R (9,), t (3,)) candidates of E (9,) float64 by step 4's Jacobi decomposition, in the header's
+    order (R1, u3), (R1, -u3), (R2, u3), (R2, -u3)."""
+    E = [float(v) for v in E]
+    S = [[((E[i] * E[j]) + (E[3 + i] * E[3 + j])) + (E[6 + i] * E[6 + j]) for j in range(3)] for i in range(3)]
+    V = [[1.0 if i == j else 0.0 for j in range(3)] for i in range(3)]
+    with np.errstate(all="ignore"):
+        for _ in range(RELPOSE_JACOBI_SWEEPS):
+            for p, q in ((0, 1), (0, 2), (1, 2)):
+                apq = S[p][q]
+                if apq == 0.0:
+                    continue
+                th = (S[q][q] - S[p][p]) / (2.0 * apq)
+                t = 1.0 / (abs(th) + _sqrt(th * th + 1.0))
+                if th < 0.0:
+                    t = -t
+                c = 1.0 / _sqrt(t * t + 1.0)
+                s = t * c
+                for M, rows in ((S, False), (S, True), (V, False)):
+                    for r in range(3):
+                        if rows:
+                            a, b = M[p][r], M[q][r]
+                            M[p][r], M[q][r] = c * a - s * b, s * a + c * b
+                        else:
+                            a, b = M[r][p], M[r][q]
+                            M[r][p], M[r][q] = c * a - s * b, s * a + c * b
+    d0, d1, d2 = S[0][0], S[1][1], S[2][2]
+    i1 = (2 if d2 > d1 else 1) if d1 > d0 else (2 if d2 > d0 else 0)
+    i2 = (2 if d2 > d1 else 1) if i1 == 0 else (2 if d2 > d0 else 0) if i1 == 1 else (1 if d1 > d0 else 0)
+    v1 = _unit3([V[i][i1] for i in range(3)])
+    v2 = [V[i][i2] for i in range(3)]
+    v3 = _unit3(_vcross(v1, v2))
+    v2 = _vcross(v3, v1)
+    u1 = _unit3([((E[3 * i] * v1[0]) + (E[3 * i + 1] * v1[1])) + (E[3 * i + 2] * v1[2]) for i in range(3)])
+    w = [((E[3 * i] * v2[0]) + (E[3 * i + 1] * v2[1])) + (E[3 * i + 2] * v2[2]) for i in range(3)]
+    u3 = _unit3(_vcross(u1, w))
+    u2 = _vcross(u3, u1)
+    R1 = np.array([((u2[i] * v1[j]) - (u1[i] * v2[j])) + (u3[i] * v3[j]) for i in range(3) for j in range(3)])
+    R2 = np.array([((u1[i] * v2[j]) - (u2[i] * v1[j])) + (u3[i] * v3[j]) for i in range(3) for j in range(3)])
+    t = np.array(u3)
+    return [(R1, t), (R1, -t), (R2, t), (R2, -t)]
+
+
+def _sqrt(v: float) -> float:
+    return math.sqrt(v) if v >= 0 else float("nan")
+
+
+def _relpose_rot(R, x, y):
+    return [((R[3 * i] * x) + (R[3 * i + 1] * y)) + R[3 * i + 2] for i in range(3)]
+
+
+def _vcross(a, b):
+    return [a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0]]
+
+
+def _vdot(a, b):
+    return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2]
+
+
+def relpose_front(R, t, x, y, xp, yp) -> np.ndarray:
+    """Step 4's cheirality test in float64 of (R (9,), t (3,)) on normalized correspondences (arrays)."""
+    Y = _relpose_rot(R, x, y)
+    r1 = [xp, yp, np.ones_like(xp)]
+    tt = [np.full_like(x, t[i]) for i in range(3)]
+    with np.errstate(all="ignore"):
+        c1, c2 = _vcross(r1, Y), _vcross(r1, tt)
+        lam = -_vdot(c1, c2) / _vdot(c1, c1)
+        return (lam > 0) & (lam * Y[2] + t[2] > 0)
+
+
+def relpose_refit_terms(R, t, b1, b2, E, x, y, xp, yp, fx, fy) -> np.ndarray:
+    """Step 4's accumulators (m, 22) of normalized correspondences (float64 arrays) at the model (R, t)."""
+    ifx, ify = 1.0 / fx, 1.0 / fy
+    one = np.ones_like(x)
+    with np.errstate(all="ignore"):
+        Y = _relpose_rot(R, x, y)
+        a = [((E[3 * q] * x) + (E[3 * q + 1] * y)) + E[3 * q + 2] for q in range(3)]
+        b = [((E[q] * xp) + (E[3 + q] * yp)) + E[6 + q] for q in range(3)]
+        res = ((xp * a[0]) + (yp * a[1])) + a[2]
+        s0, s1, s2, s3 = a[0] * ifx, a[1] * ify, b[0] * ifx, b[1] * ify
+        wt = 1.0 / np.sqrt(((s0 * s0 + s1 * s1) + s2 * s2) + s3 * s3)
+        rr = wt * res
+        z = [xp, yp, one]
+        zt = _vcross(z, [t[0] * one, t[1] * one, t[2] * one])
+        gw = _vcross(Y, zt)
+        yz = _vcross(Y, z)
+        J = [wt * (2.0 * gw[q]) for q in range(3)]
+        J += [wt * _vdot([b1[0] * one, b1[1] * one, b1[2] * one], yz), wt * _vdot([b2[0] * one, b2[1] * one,
+                                                                                     b2[2] * one], yz)]
+        terms = [J[p] * J[q] for p in range(5) for q in range(p, 5)] + [-(J[p] * rr) for p in range(5)]
+        dx, dy = fx * (xp - Y[0] / Y[2]), fy * (yp - Y[1] / Y[2])
+        terms.append(np.sqrt(dx * dx + dy * dy))
+        Rw = [sum_(((2.0 * (t[i] * t[k])) - (1.0 if i == k else 0.0)) * R[3 * k + j] for k in range(3))
+              for i in range(3) for j in range(3)]
+        Yw = _relpose_rot(Rw, x, y)
+        wx, wy = fx * (xp - Yw[0] / Yw[2]), fy * (yp - Yw[1] / Yw[2])
+        terms.append(np.sqrt(wx * wx + wy * wy))
+    return np.stack(terms, -1)
+
+
+def sum_(terms) -> float:
+    """Left-to-right float64 sum from +0.0."""
+    v = 0.0
+    for x in terms:
+        v = v + x
+    return v
+
+
+def _relpose_pair(F, B, p):
+    f32 = np.float32
+    h, w = F.shape[:2]
+    s = int(p["step"])
+    u, v = F[..., 0], F[..., 1]
+    X = np.arange(w, dtype=f32)[None, :]
+    Y = np.arange(h, dtype=f32)[:, None]
+    with np.errstate(invalid="ignore", over="ignore"):
+        xs, ys = X + u, Y + v
+        lim = f32(MOTION_UNKNOWN_THRESH)
+        valid = (np.abs(u) <= lim) & (np.abs(v) <= lim) & (xs >= 0) & (xs <= f32(w - 1)) & (ys >= 0) & \
+            (ys <= f32(h - 1))
+    if p["fb_check"]:
+        valid &= consistency_check(F, B, p["alpha"], p["beta"])[0] == 0
+    ncx, ncy = (w - 1) // s + 1, (h - 1) // s + 1
+    cell = np.arange(ncx * ncy)
+    cxs = np.minimum((cell % ncx) * s + s // 2, w - 1)
+    cys = np.minimum((cell // ncx) * s + s // 2, h - 1)
+    sel = valid[cys, cxs]
+    cxs, cys = cxs[sel], cys[sel]
+    corr = np.stack([cxs.astype(f32), cys.astype(f32), xs[cys, cxs], ys[cys, cxs]], -1).astype(f32)
+    m = corr.shape[0]
+    thr = p["threshold"]
+    fx, fy = float(f32(p["fx"])), float(f32(p["fy"]))
+    st = np.zeros((), MOTION_STATS_DTYPE)
+    st["n_corr"], st["best_hypothesis"] = m, -1
+    status = 1 if m < 8 else 0
+    nx, ny, nxp, nyp = (a.astype(np.float64) for a in _relpose_norm(corr, p))
+    if not status:
+        idx = motion_draws(int(p["seed"]), int(p["hypotheses"]), 8, m)
+        x, y, xp, yp = nx[idx], ny[idx], nxp[idx], nyp[idx]
+        A = np.stack([xp * x, xp * y, xp, yp * x, yp * y, yp, x, y, np.ones_like(x)], -1)
+        Es, ok = relpose_null(A)
+        g = relpose_fmat(Es, p["fx"], p["fy"], p["cx"], p["cy"])
+        counts = np.zeros(idx.shape[0], np.int64)
+        for h0 in range(0, idx.shape[0], 256):
+            counts[h0:h0 + 256] = relpose_sampson(g[h0:h0 + 256], corr, thr)[0].sum(axis=1)
+        if not ok.any():
+            status = 2
+    pose = np.full(12, _QNAN64)
+    if not status:
+        keys = np.where(ok, (counts << 32) | (0xFFFFFFFF - np.arange(idx.shape[0])), -1)
+        best = int(np.argmax(keys))
+        st["best_hypothesis"], st["ransac_inliers"] = best, counts[best]
+        inl = relpose_sampson(g[best], corr, thr)[0]
+        cands = relpose_decompose(Es[best])
+        votes = [int(relpose_front(Rc, tc, nx[inl], ny[inl], nxp[inl], nyp[inl]).sum()) for Rc, tc in cands]
+        R, t = cands[int(np.argmax(votes))]
+        R, t = [float(v) for v in R], [float(v) for v in t]
+        refits = 0
+        for r in range(int(p["refine"]) + 1):
+            E = [(-(t[2] * R[3 + j])) + (t[1] * R[6 + j]) for j in range(3)] + \
+                [(t[2] * R[j]) - (t[0] * R[6 + j]) for j in range(3)] + \
+                [(-(t[1] * R[j])) + (t[0] * R[3 + j]) for j in range(3)]
+            gm = relpose_fmat(np.array(E), p["fx"], p["fy"], p["cx"], p["cy"])
+            a = min(range(3), key=lambda i: (abs(t[i]), i))
+            ea = [1.0 if i == a else 0.0 for i in range(3)]
+            b1 = _unit3(_vcross(t, ea))
+            b2 = _vcross(t, b1)
+            inl = relpose_sampson(gm, corr, thr)[0]
+            cnt = int(inl.sum())
+            T = relpose_refit_terms(R, t, b1, b2, E, nx, ny, nxp, nyp, fx, fy)
+            v = _chunk_tree(np.where(inl[:, None], T, 0.0))
+            if r == int(p["refine"]) or cnt < 8:
+                break
+            An = np.zeros((5, 5))
+            e = 0
+            for a_ in range(5):
+                for b_ in range(a_, 5):
+                    An[a_, b_] = An[b_, a_] = v[e]
+                    e += 1
+            xs_, okn = motion_solve(An[None], v[None, 15:20])
+            if not okn[0]:
+                break
+            d = xs_[0]
+            Rm = ego_update(np.array([R[0], R[1], R[2], 0.0, R[3], R[4], R[5], 0.0, R[6], R[7], R[8], 0.0]),
+                            np.array([d[0], d[1], d[2], 0.0, 0.0, 0.0]))
+            R = [float(Rm[4 * i + j]) for i in range(3) for j in range(3)]
+            t = _unit3([(t[i] + d[3] * b1[i]) + d[4] * b2[i] for i in range(3)])
+            refits += 1
+        st["refits"], st["n_inliers"] = refits, cnt
+        with np.errstate(all="ignore"):
+            parallax = (v[21] if v[21] < v[20] else v[20]) / np.float64(cnt)
+        status = 0 if parallax >= float(f32(p["min_parallax"])) else 3
+        if not status:
+            P = np.array([R[0], R[1], R[2], t[0], R[3], R[4], R[5], t[1], R[6], R[7], R[8], t[2]])
+            pose = np.where(np.isnan(P), _QNAN64, P)
+    st["status"] = status
+    mask = np.full((h, w), 2, np.uint8)
+    samp = np.full((h, w), _QNAN, f32)
+    depth = np.full((h, w), _QNAN, f32)
+    if status:
+        return pose, st, mask, samp, depth
+    cpx = np.stack([np.broadcast_to(X, (h, w)), np.broadcast_to(Y, (h, w)), xs, ys], -1).reshape(-1, 4).astype(f32)
+    inl, e, den = (a.reshape(h, w) for a in relpose_sampson(gm, cpx, thr))
+    mask = np.where(valid, np.where(inl, 0, 1), 2).astype(np.uint8)
+    with np.errstate(all="ignore"):
+        sq = np.sqrt((e * e) / den).astype(f32)
+        g32 = pose.astype(f32)
+        Rf, tf = g32[[0, 1, 2, 4, 5, 6, 8, 9, 10]], g32[[3, 7, 11]]
+        x, y, xp, yp = (a.reshape(h, w) for a in _relpose_norm(cpx, p))
+        q = [(Rf[3 * i] * x + Rf[3 * i + 1] * y) + Rf[3 * i + 2] for i in range(3)]
+        c1 = [yp * q[2] - q[1], q[0] - xp * q[2], xp * q[1] - yp * q[0]]
+        c2 = [yp * tf[2] - tf[1], tf[0] - xp * tf[2], xp * tf[1] - yp * tf[0]]
+        lam = -((c1[0] * c2[0] + c1[1] * c2[1]) + c1[2] * c2[2]) / ((c1[0] * c1[0] + c1[1] * c1[1]) + c1[2] * c1[2])
+        front = (lam > 0) & (lam * q[2] + tf[2] > 0)
+    samp = np.where(valid, np.where(np.isnan(sq), _QNAN, sq), _QNAN).astype(f32)
+    depth = np.where(valid & front, lam, _QNAN).astype(f32)
+    return pose, st, mask, samp, depth
+
+
+def relpose_params(params) -> dict:
+    return {k: params[k] for k in RELPOSE_PARAM_FIELDS}
+
+
+def relpose(F: np.ndarray, B: np.ndarray | None, params):
+    """ofdis_relpose_fullres bit for bit.  F: the forward flows (n, h, w, 2) exactly as ofdis_get_flow_fullres returns
+    them, B the partner flows of fb_check (else None); params a mapping with RELPOSE_PARAM_FIELDS.  Returns (pose
+    (n, 3, 4) float64, stats (n,) MOTION_STATS_DTYPE, mask (n, h, w) uint8, sampson and depth (n, h, w) float32)."""
+    p = relpose_params(params)
+    F = np.asarray(F, np.float32)
+    n, h, w = F.shape[:3]
+    out = [_relpose_pair(F[k], None if B is None else np.asarray(B[k], np.float32), p) for k in range(n)]
+    pose = np.stack([o[0] for o in out]).reshape(n, 3, 4) if n else np.zeros((0, 3, 4))
+    stats = np.array([o[1] for o in out], MOTION_STATS_DTYPE).reshape(n)
+    return (pose, stats, np.stack([o[2] for o in out]), np.stack([o[3] for o in out]),
+            np.stack([o[4] for o in out]))
+
+
+def relpose_errors(rel, gt_rel):
+    """The standard monocular metrics of relative poses rel against ground truth gt_rel (n, 3, 4) (camera t to camera
+    t+1): the rotation error acos((trace(R_gt^T R) - 1) / 2) in degrees and the angle between the translation
+    directions in degrees.  Returns (r_err (n,), t_dir_err (n,)); NaN where a pose is NaN or a translation is zero."""
+    rel = np.asarray(rel, np.float64).reshape(-1, 3, 4)
+    gt = np.asarray(gt_rel, np.float64).reshape(-1, 3, 4)
+    r_err, t_err = [], []
+    for P, G in zip(rel, gt):
+        c = 0.5 * (np.trace(G[:, :3].T @ P[:, :3]) - 1.0)
+        r_err.append(float(np.degrees(np.arccos(np.clip(c, -1.0, 1.0)))) if np.isfinite(c) else np.nan)
+        a, b = P[:, 3], G[:, 3]
+        with np.errstate(all="ignore"):
+            ct = float(a @ b / (np.linalg.norm(a) * np.linalg.norm(b)))
+        t_err.append(float(np.degrees(np.arccos(np.clip(ct, -1.0, 1.0)))) if np.isfinite(ct) else np.nan)
+    return np.array(r_err), np.array(t_err)
+
+
 # ---- poses (float64 host helpers, no bit contract) -------------------------------------------------------------------
 def _pose44(P) -> np.ndarray:
     T = np.eye(4)
@@ -1755,14 +2112,19 @@ def _pose44(P) -> np.ndarray:
     return T
 
 
-def chain_poses(rel) -> np.ndarray:
+def chain_poses(rel, scales=None) -> np.ndarray:
     """Camera-to-world poses (n+1, 3, 4) of a clip in KITTI's odometry convention from its relative poses rel (n, 3, 4)
-    (camera t to camera t+1, as ofdis_egomotion_fullres returns them): T_0 = I, T_(k+1) = T_k inv([R | t]_k)."""
+    (camera t to camera t+1, as ofdis_egomotion_fullres returns them): T_0 = I, T_(k+1) = T_k inv([R | t]_k).
+    scales: optional (n,) factors of the translations, e.g. ground-truth step lengths for the unit translations of
+    ofdis_relpose_fullres."""
     rel = np.asarray(rel, np.float64).reshape(-1, 3, 4)
     T = np.eye(4)
     out = [T[:3].copy()]
-    for P in rel:
-        T = T @ np.linalg.inv(_pose44(P))
+    for k, P in enumerate(rel):
+        Q = _pose44(P)
+        if scales is not None:
+            Q[:3, 3] *= float(scales[k])
+        T = T @ np.linalg.inv(Q)
         out.append(T[:3].copy())
     return np.stack(out)
 

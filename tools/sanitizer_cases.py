@@ -11,8 +11,9 @@ stages on 32-byte correspondences, non-finite disparities, score tile refills), 
 posteriors, float64 statistics, the take) and a TSDF fusion (integration, crossing count, scan and write, ray casting)
 and its marching cubes (set_volume, the write with vertex bases, cube count, scan, faces) and a camera tracking
 against it (the evaluation kernel's chunk sums, arrival counter and tree, with and without the push), the same
-tracking and push weighted by per-pixel weights with special values, and a per-pixel confidence (the halo-staged tile
-and its window sums, planted level flows) checked against their restatements.  Results are checked against the
+tracking and push weighted by per-pixel weights with special values, a per-pixel confidence (the halo-staged tile
+and its window sums, planted level flows) and a monocular relative pose (full-pivot hypotheses, Sampson score tiles,
+the refit CTA, per-pixel outputs, planted level flows) checked against their restatements.  Results are checked against the
 oracle so that a clean log means a correct run."""
 import os
 import sys
@@ -370,6 +371,38 @@ for r in (1, 7):
                 np.array_equal(canon(d_terms[k].cpu().numpy()), canon(et))
 ctx.close()
 print("%-22s %s" % ("confidence", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
+if not ok:
+    sys.exit(1)
+# monocular relative pose: a rigid clip's exact flow with NaN, +-inf and 3e9 planted as level flows, an all-invalid
+# pair, step 1 (more than two 4096-entry score tiles), every per-pixel output in device memory
+h3, w3 = 96, 160
+rcam = dict(fx=180.0, fy=176.5, cx=79.75, cy=48.5, baseline=0.54, doffs=0.0)
+rmo = np.concatenate([synth.axis_angle((0.0, 0.01, 0.0)), np.array([[0.03], [0.0], [-0.5]])], 1)
+rclip = synth.rigid_stereo_clip(1, h3, w3, 1, 4, rcam, [rmo])
+a = rclip["flow"][0].astype(np.float32).copy()
+a[::3, ::5] = np.nan
+a[1::7, ::2, 0] = np.inf
+a[2::5, 1::3, 1] = -np.inf
+a[3::4, 3::4, 0] = 3e9
+rflows = np.stack([a, np.full((h3, w3, 2), np.nan, np.float32)])
+rprm = params.from_cli_numbers("3 0 8 8 0.05 0.95 0 8 0.4 0 1 0 0 10 10 5 1 3 1.6 0".split(), noc=1, nop=2)
+ctx = api.Context(rprm, w3, h3, rprm.p_samp_s, 2)
+for k in range(2):
+    ctx.set_flow(k, 0, rflows[k])
+rp = dict(fx=180.0, fy=176.5, cx=79.75, cy=48.5, step=1, fb_check=0, alpha=0.01, beta=0.5, hypotheses=96,
+          threshold=1.0, refine=3, min_parallax=0.25, seed=7)
+dev = {"mask": torch.empty((2, h3, w3), dtype=torch.uint8, device="cuda"),
+       "sampson": torch.empty((2, h3, w3), device="cuda"), "depth": torch.empty((2, h3, w3), device="cuda")}
+torch.cuda.synchronize()
+pose, stats, _ = ctx.relpose_fullres(0, 2, rp, width_org=w3, height_org=h3, outputs=tuple(dev),
+                                     out={k: v.data_ptr() for k, v in dev.items()}, memkind=api.MEM_DEVICE)
+ctx.close()
+exp = preprocess.relpose(rflows, None, rp)
+ok = stats["n_corr"][0] > 2 * 4096 and stats["status"].tolist()[1] == 1 and all(
+    np.array_equal(np.asarray(g).view(np.uint8), np.asarray(e).view(np.uint8))
+    for g, e in zip((pose, stats, dev["mask"].cpu().numpy(), dev["sampson"].cpu().numpy(), dev["depth"].cpu().numpy()),
+                    exp))
+print("%-22s %s" % ("relpose", "bitwise equal to the restatement" if ok else "MISMATCH"), flush=True)
 if not ok:
     sys.exit(1)
 print("all cases ok")
